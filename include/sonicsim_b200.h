@@ -49,11 +49,24 @@ typedef enum {
 
 /* per-source options (ss_source.flags) */
 typedef enum {
-    SS_RIR_NORMALIZE = 1      /* `rir` is the raw simulator output, clipped and stacked: divide every tap by the global
+    SS_RIR_NORMALIZE = 1,     /* `rir` is the raw simulator output, clipped and stacked: divide every tap by the global
                                * abs-max of the source's whole (P, C, L) tensor before convolving, i.e. the
                                * `ir_output /= ir_output.abs().max()` of generate_rir_combination
                                * (SonicSim_audio.py:391-398), fused into the spectra kernel's row loads (one reduction
                                * kernel + an IEEE division per tap; same bits as normalising first) */
+    SS_DIRECT_TARGET = 2      /* also render the direct-path stem into `out_direct` (speech-enhancement /
+                               * dereverberation target), in the same launches as the reverberant stem `out`.
+                               * Each row h[p, c, :] (after normalisation when SS_RIR_NORMALIZE is set) is cut after
+                               *   peak[p, c] = first index of max_k |h[p, c, k]|   (np.argmax's tie rule; 0 for an
+                               *                                                     all-zero row)
+                               *   cut[p, c]  = min(L, peak[p, c] + direct_taps)
+                               * i.e. h_d[p, c, k] = h[p, c, k] for k < cut[p, c], 0 otherwise, and rendered with the
+                               * source's own trajectory, blocking and weights: `out_direct` has the bits of rendering h_d
+                               * as a separate source of the same mode, `out` the bits of the source without this flag.
+                               * The peak is the strongest tap, which in a simulated RIR may be a reflection rather
+                               * than the earliest arrival.  direct_taps = 40 is 2.5 ms at 16 kHz; a longer one (e.g.
+                               * 50 ms) gives an early-reflections target.  With ss_render_host_ex loudness
+                               * normalisation the direct stem is scaled by the reverberant stem's gain. */
 } ss_source_flags;
 
 /* One (utterance, source) unit of work = one call of convolve_moving_receiver /
@@ -71,7 +84,9 @@ typedef struct {
     int32_t flags;            /* ss_source_flags, 0 = none */
     const int32_t* bounds_host; /* ss_render_dev only, optional: HOST copy of `bounds` (P ints).  With it the block
                                  * table is built on the host and one small kernel launch per chunk is saved.     */
-} ss_source;
+    float* out_direct;        /* SS_DIRECT_TARGET: (C, N) direct-path stem, same pointer kind as `out`, != out    */
+    int32_t direct_taps;      /* SS_DIRECT_TARGET: taps kept from each row's peak on, >= 1                        */
+} ss_source;                  /* fields appended since version 100: a zeroed (memset) struct leaves them off      */
 
 /* library / build identification */
 int ss_version(void);

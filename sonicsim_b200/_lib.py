@@ -19,7 +19,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
 
 SS_OK, SS_ERR_INVALID, SS_ERR_INDEX, SS_ERR_CUDA, SS_ERR_NOMEM, SS_ERR_UNSUPPORTED = 0, -1, -2, -3, -4, -5
 SS_STATIC, SS_MOVING_BOUNDS, SS_MOVING_INDEXED = 0, 1, 2
-SS_RIR_NORMALIZE = 1
+SS_RIR_NORMALIZE, SS_DIRECT_TARGET = 1, 2
 
 
 class SsLoudItem(ctypes.Structure):
@@ -59,7 +59,8 @@ class SsSource(ctypes.Structure):
     _fields_ = [("x", ctypes.c_void_p), ("rir", ctypes.c_void_p), ("out", ctypes.c_void_p),
                 ("bounds", ctypes.c_void_p), ("idx", ctypes.c_void_p), ("w", ctypes.c_void_p),
                 ("N", ctypes.c_int32), ("P", ctypes.c_int32), ("C", ctypes.c_int32), ("L", ctypes.c_int32),
-                ("mode", ctypes.c_int32), ("flags", ctypes.c_int32), ("bounds_host", ctypes.c_void_p)]
+                ("mode", ctypes.c_int32), ("flags", ctypes.c_int32), ("bounds_host", ctypes.c_void_p),
+                ("out_direct", ctypes.c_void_p), ("direct_taps", ctypes.c_int32)]
 
 
 def _stale():

@@ -55,6 +55,12 @@ extern thread_local int g_last_cuda;
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// data[i] *= (float)result[1] over the N * C floats of each item, with k_loud_scale's arithmetic: a stem that takes the
+// linear gain another stem's loudness measurement left in `result` (ss_render_host_ex: the direct-path stem takes its
+// reverberant stem's gain, so that target and mixture stay consistent).  Device pointers, asynchronous on `stream`.
+struct ScaleItem { float* data; const double* result; int32_t N, C; };
+int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t stream);
+
 // Take the next slot of the descriptor ring (pinned host block + its device twin), grown to `bytes`.
 // Blocks the host until the slot's previous host->device copy has completed.  The caller fills `*h`,
 // copies it to `*d` on its stream and records c->desc_ev[*slot] right after the copy.

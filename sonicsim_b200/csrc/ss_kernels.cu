@@ -18,6 +18,8 @@
 //               per-sample lerp and the (C, N) store.  <LONG>: RIR partitions >= 1 (staged one after the other).
 //   k_render_fast : the same for all-aligned chunks (one item = one transform), see its own header below
 //   k_rir_absmax  : optional, SS_RIR_NORMALIZE: global abs-max of a source's RIR tensor for k_prepare's row loads
+//   k_rir_direct  : optional, SS_DIRECT_TARGET: per-row direct-path length (argmax |h| + direct_taps); k_prepare then
+//                   transforms the truncated rows as a second RIR set and fills a second group of items per block
 // Consecutive chunks rotate through three streams / scratch buffers so that they overlap; a bound batch (ss_plan_*)
 // captures all of it into one CUDA graph.
 // fp32 throughout (the reference is float32 end to end, SURVEY 8), no cuFFT.
@@ -135,9 +137,30 @@ k_rir_absmax(const Source* __restrict__ srcs) {
     }
 }
 
+// ----------------------------------------------------------------------------- k_rir_direct
+// SS_DIRECT_TARGET: one warp per (p, c) RIR row of every direct-target source of the chunk (`per_src` CTAs of 8 rows
+// per source): first-occurrence argmax of |h| over the row - on the normalised taps when the source has
+// SS_RIR_NORMALIZE, so after k_rir_absmax - and the row's direct-path length cut[p, c] = min(L, peak + direct_taps),
+// which k_prepare's direct rows use as their length.
+__global__ void __launch_bounds__(256)
+k_rir_direct(const Source* __restrict__ srcs, int per_src) {
+    const Source& S = srcs[blockIdx.x / per_src];
+    const int row = (blockIdx.x % per_src) * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (!S.cut || row >= S.P * S.C) return;
+    const float div = S.norm_part ? rir_absmax(S) : 0.f;
+    PeakAt m = peak_scan(S.rir + (size_t)row * S.L, S.L, div, lane, 32);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        PeakAt q; q.v = __shfl_xor_sync(0xffffffffu, m.v, o); q.i = __shfl_xor_sync(0xffffffffu, m.i, o);
+        m = peak_first(m, q);
+    }
+    if (lane == 0) S.cut[row] = direct_cut(m.i, S.L, S.direct_taps);
+}
+
 // ----------------------------------------------------------------------------- k_prepare
 // CTA kinds, flattened per source through `prefix`:
-//   [0, nh)            two RIR-partition rows  -> two half spectra (one complex FFT)
+//   [0, nh)            two RIR-partition rows  -> two half spectra (one complex FFT); a direct-target source's
+//                      direct rows (length cut[p, c]) follow its reverberant ones
 //   [nh, nh + nx)      two dry windows         -> two half spectra
 //   [nh + nx, ...)     8 blocks each (one warp per block): position range of the block and its
 //                      k_render work items (RItem)
@@ -197,7 +220,7 @@ k_prepare(const Source* __restrict__ srcs_g, const int* __restrict__ prefix_g, i
         fill_items(S, items, blk, bk, lane, 32);
         return;
     }
-    if (local < nh) { ra = make_row_h(S, 2 * local); rb = make_row_h(S, 2 * local + 1); }
+    if (local < nh) rows_of_pair_h(S, local, ra, rb);
     else { local -= nh; ra = make_row_x(S, 2 * local); rb = make_row_x(S, 2 * local + 1); }
     if (!ra.dst && !rb.dst) return;              // both block slots unused (aligned blocking over-allocates)
 
@@ -517,7 +540,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 100; }
+extern "C" int ss_version(void) { return 101; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -702,12 +725,19 @@ static int validate_item(const ss_source& it) {
     // 32-bit sample / table indices inside the kernels: leave one FFT of headroom below 2^31
     if (it.N > 0x7fffffff - 2 * kF) return SS_ERR_UNSUPPORTED;
     if ((int64_t)it.P * it.C * ((it.L + kB - 1) / kB) > (int64_t)1 << 28) return SS_ERR_UNSUPPORTED;
-    if (it.flags & ~SS_RIR_NORMALIZE) return SS_ERR_INVALID;
+    if (it.flags & ~(SS_RIR_NORMALIZE | SS_DIRECT_TARGET)) return SS_ERR_INVALID;
+    if ((it.flags & SS_DIRECT_TARGET) && (!it.out_direct || it.direct_taps < 1 || it.out_direct == it.out))
+        return SS_ERR_INVALID;
     if (it.mode == SS_STATIC) { if (it.P != 1) return SS_ERR_INVALID; }
     else if (it.mode == SS_MOVING_BOUNDS) { if (it.P < 2 || !it.bounds) return SS_ERR_INVALID; }
     else if (it.mode == SS_MOVING_INDEXED) { if (it.P < 2 || !it.idx || !it.w) return SS_ERR_INVALID; }
     else return SS_ERR_INVALID;
     return SS_OK;
+}
+// SS_DIRECT_TARGET: a second RIR set (spectra, items per block) and the P*C cut table
+static int direct_sets(const ss_source& it) { return (it.flags & SS_DIRECT_TARGET) ? 2 : 1; }
+static size_t cut_bytes(const ss_source& it) {
+    return (it.flags & SS_DIRECT_TARGET) ? align_up(sizeof(int) * (size_t)it.P * it.C, 256) : 0;
 }
 // shapes derived from one ss_source
 struct Shape { int K, nb, aligned, nblk_max, per, max_items; };
@@ -736,15 +766,16 @@ static Shape shape_of(const ss_source& it) {
     s.K = (it.L + kB - 1) / kB; s.nb = (it.N + kB - 1) / kB;
     s.aligned = choose_aligned(it, s.K, s.nb) ? 1 : 0;
     s.nblk_max = s.aligned ? s.nb + it.P - 1 : s.nb;
-    s.per = it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C;
+    s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
     s.max_items = s.nblk_max * s.per;
     return s;
 }
 static size_t spectra_bytes(const ss_source& it) {
     const Shape sh = shape_of(it);
-    return ((size_t)it.P * it.C * sh.K + sh.nblk_max) * kSpec * sizeof(float2) + (size_t)sh.max_items * sizeof(RItem) +
+    return ((size_t)it.P * it.C * sh.K * direct_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
+           (size_t)sh.max_items * sizeof(RItem) +
            align_up(sizeof(Block) * (size_t)sh.nblk_max, 256) + align_up(sizeof(double) * (size_t)it.P, 256) + 256 +
-           ((it.flags & SS_RIR_NORMALIZE) ? 512 : 0);
+           ((it.flags & SS_RIR_NORMALIZE) ? 512 : 0) + cut_bytes(it);
 }
 
 // Host-side twin of k_blocks for one source whose trajectory bounds are visible on the host.
@@ -796,6 +827,7 @@ extern "C" int ss_debug_plan(const ss_source* item, int32_t* blocks_out, int32_t
 // Everything the launches need besides the descriptor block in device memory.
 struct ChunkLaunch {
     int n = 0, ps = 0, grid_r = 0, n_known = -1;
+    int grid_direct = 0;                  // k_rir_direct CTAs per source (8 rows each), 0: no direct target in the chunk
     bool host_tables = true, any_long = false, all_aligned = true, any_norm = false;
     const Source* ds = nullptr; const int* dps = nullptr; RItem* d_items = nullptr; int* d_total = nullptr;
     PrepParams pp;
@@ -835,6 +867,7 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
     int ps = 0, pr = 0, total_items = 0;
     size_t tab_off = off_tot + 16;
     bool any_long = false, all_aligned = true, any_norm = false;
+    int grid_direct = 0;
     for (int i = 0; i < n; ++i) {
         const ss_source& it = items[first + i];
         const Shape sh = shape_of(it);
@@ -846,9 +879,14 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
         s.w = it.mode == SS_MOVING_INDEXED ? it.w : nullptr;
         s.N = it.N; s.P = it.P; s.C = it.C; s.L = it.L;
         s.K = sh.K; s.nb = sh.nb; s.mode = it.mode; s.aligned = sh.aligned; s.nblk_max = sh.nblk_max;
-        s.hspec = (float2*)scratch; scratch += (size_t)s.P * s.C * s.K * kSpec * sizeof(float2);
+        s.hspec = (float2*)scratch; scratch += (size_t)s.P * s.C * s.K * direct_sets(it) * kSpec * sizeof(float2);
         s.xspec = (float2*)scratch; scratch += (size_t)s.nblk_max * kSpec * sizeof(float2);
         if (it.flags & SS_RIR_NORMALIZE) { s.norm_part = (const float*)scratch; scratch += 512; any_norm = true; }
+        if (it.flags & SS_DIRECT_TARGET) {
+            s.cut = (int*)scratch; scratch += cut_bytes(it);
+            s.out_direct = it.out_direct; s.direct_taps = it.direct_taps;
+            grid_direct = std::max(grid_direct, (s.P * s.C + 7) / 8);
+        }
         if (host_tables) {
             // tables live in the descriptor block itself: filled here, copied with it
             Block* hb_blocks = (Block*)(hbase + tab_off);
@@ -879,6 +917,7 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
     if (host_tables) { *(int*)(hbase + off_tot) = total_items; pr = total_items; }
     L->n = n; L->ps = ps; L->host_tables = host_tables; L->any_long = any_long; L->all_aligned = all_aligned;
     L->any_norm = any_norm;
+    L->grid_direct = grid_direct;
     L->n_known = host_tables ? total_items : -1;
     L->grid_r = pr < sm_count * SS_RENDER_MINB ? pr : sm_count * SS_RENDER_MINB;
     L->ds = (const Source*)dbase;
@@ -899,6 +938,11 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, s
     }
     if (L.any_norm) {
         k_rir_absmax<<<L.n * kNormParts, 256, 0, stream>>>(L.ds);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
+    if (L.grid_direct > 0) {
+        k_rir_direct<<<L.n * L.grid_direct, 256, 0, stream>>>(L.ds, L.grid_direct);
         CK(cudaGetLastError());
         c->launches += 1;
     }
@@ -1127,7 +1171,8 @@ static int plan_build(ss_plan* p, const ss_source* items, int n_items) {
     for (size_t k = 0; k < n_chunks; ++k) {
         chunk_describe(items, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
                        p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k]);
-        p->launches_per_run += (p->chunks[k].host_tables ? 2 : 3) + (p->chunks[k].any_norm ? 1 : 0);
+        p->launches_per_run += (p->chunks[k].host_tables ? 2 : 3) + (p->chunks[k].any_norm ? 1 : 0) +
+                               (p->chunks[k].grid_direct > 0 ? 1 : 0);
     }
     CK(cudaMemcpy(p->d_desc, host.data(), off[n_chunks], cudaMemcpyHostToDevice));
     return SS_OK;
@@ -1255,6 +1300,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     make_chunks(c, items, n_items, cuts, c->chunk_bytes_host);
     std::vector<ss_source> dev(n_items);
     std::vector<ss_loud_item> loud;
+    std::vector<ScaleItem> direct_gain;                  // direct-path stems scaled by their reverberant stem's gain
     std::vector<double*> res_dev(n_items, nullptr);
     // loudness: (a) the gating tables of all sources that share them (same host arrays = same clip length, the normal
     // case) are uploaded once per call from a pinned staging copy; (b) the two result doubles of every stem come back
@@ -1318,7 +1364,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
             in_b += align_up(sizeof(float) * (size_t)it.N, 256) + align_up(sizeof(float) * (size_t)it.P * it.C * it.L, 256);
             if (it.mode == SS_MOVING_BOUNDS) in_b += align_up(sizeof(int32_t) * (size_t)it.P, 256);
             if (it.mode == SS_MOVING_INDEXED) in_b += 2 * align_up(4 * (size_t)it.N, 256);
-            out_b += align_up(sizeof(float) * (size_t)it.C * it.N, 256);
+            out_b += align_up(sizeof(float) * (size_t)it.C * it.N, 256) * direct_sets(it);
             if (post && post[i].brk)
                 out_b += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * it.C * post[i].n_e, 256) + 256;
         }
@@ -1327,6 +1373,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         if ((rc = ensure(&sl.d_out, &sl.out_cap, out_b)) != SS_OK) break;
         char* pi = sl.d_in; char* po = sl.d_out;
         loud.clear();
+        direct_gain.clear();
         for (int i = first; i < last; ++i) {
             const ss_source& it = items[i];
             ss_source d = it;
@@ -1345,6 +1392,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
                 CK(cudaMemcpyAsync(pi, it.w, nb, cudaMemcpyHostToDevice, c->s_in)); d.w = (const float*)pi; pi += align_up(nb, 256);
             }
             d.out = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * it.N, 256);
+            if (it.flags & SS_DIRECT_TARGET) { d.out_direct = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * it.N, 256); }
             dev[i] = d;
             if (post && post[i].brk) {
                 const ss_post_lufs& pl = post[i];
@@ -1358,6 +1406,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
                 li.stride_n = 1; li.stride_c = it.N; li.N = it.N; li.C = it.C; li.n_e = pl.n_e; li.n_blocks = pl.n_blocks;
                 li.rate = pl.rate; li.block_size = pl.block_size; li.target_lufs = pl.target_lufs;
                 loud.push_back(li);
+                if (it.flags & SS_DIRECT_TARGET) direct_gain.push_back(ScaleItem{d.out_direct, li.result, it.N, it.C});
             }
         }
         CK(cudaEventRecord(sl.ev_in, c->s_in));
@@ -1370,6 +1419,8 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
             CK(cudaStreamWaitEvent(s_l, sl.ev_rend, 0));
             rc = ss_loudness_dev(c, loud.data(), (int)loud.size(), (void*)s_l);
             if (rc != SS_OK) break;
+            rc = loud_scale_dev(c, direct_gain.data(), (int)direct_gain.size(), s_l);
+            if (rc != SS_OK) break;
             CK(cudaEventRecord(sl.ev_done, s_l));
         } else {
             CK(cudaEventRecord(sl.ev_done, c->s_cmp));
@@ -1378,6 +1429,9 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         for (int i = first; i < last; ++i) {
             CK(cudaMemcpyAsync(items[i].out, dev[i].out, sizeof(float) * (size_t)items[i].C * items[i].N,
                                cudaMemcpyDeviceToHost, c->s_out));
+            if (items[i].flags & SS_DIRECT_TARGET)
+                CK(cudaMemcpyAsync(items[i].out_direct, dev[i].out_direct, sizeof(float) * (size_t)items[i].C * items[i].N,
+                                   cudaMemcpyDeviceToHost, c->s_out));
             if (res_dev[i])
                 CK(cudaMemcpyAsync(h_res + 2 * i, res_dev[i], 2 * sizeof(double), cudaMemcpyDeviceToHost, c->s_out));
         }

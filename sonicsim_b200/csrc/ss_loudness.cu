@@ -267,6 +267,27 @@ extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items
     return SS_OK;
 }
 
+// Internal (ss_internal.h): k_loud_scale alone, for stems that take the gain measured on another stem.
+int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t stream) {
+    if (n_items == 0) return SS_OK;
+    const size_t bytes = sizeof(LoudItem) * n_items;
+    int slot; char *hblk, *dblk;
+    { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
+    LoudItem* h = (LoudItem*)hblk;
+    for (int i = 0; i < n_items; ++i) {
+        memset(&h[i], 0, sizeof(LoudItem));
+        h[i].data = items[i].data; h[i].out = items[i].data;
+        h[i].result = const_cast<double*>(items[i].result);
+        h[i].N = items[i].N; h[i].C = items[i].C;
+    }
+    CK(cudaMemcpyAsync(dblk, hblk, bytes, cudaMemcpyHostToDevice, stream));
+    CK(cudaEventRecord(c->desc_ev[slot], stream));
+    k_loud_scale<<<dim3(c->sm_count * 2, n_items), 256, 0, stream>>>((const LoudItem*)dblk);
+    CK(cudaGetLastError());
+    c->launches += 1;
+    return SS_OK;
+}
+
 // Single stem, host arrays (the drop-in lufs_norm): data / out hold N*C floats in the caller's layout.
 extern "C" int ss_lufs_norm_host(ss_ctx* c, const float* data, float* out, int32_t N, int32_t C,
                                  int64_t stride_n, int64_t stride_c, double rate, double block_size,

@@ -30,19 +30,22 @@ struct Source {
     const int* bounds;     // compact trajectory: S+1 cumulative segment bounds (mode 1), else null
     const int* idx;        // per-sample interp_index  (mode 2), else null
     const float* w;        // per-sample interp_weight (mode 2), else null
-    float2* hspec;         // scratch: P*C*K half spectra of the RIR partitions, pre-scaled by 1/F
+    float2* hspec;         // scratch: P*C*K half spectra of the RIR partitions, pre-scaled by 1/F; a direct-target
+                           // source has a second P*C*K block right behind it for the direct rows (same layout)
     float2* xspec;         // scratch: nblk_max half spectra of the dry windows
     Block* blocks;         // scratch: nblk_max blocks (k_blocks)
     double* rstep;         // scratch: 1 / (samples in segment s), s < P - 1 (mode 1)
     int* counts;           // scratch: [0] = blocks in use, [1] = index of this source's first render item
     const float* norm_part;// scratch: kNormParts partial abs-maxima of the RIR tensor (k_rir_absmax), or null: taps used as given
+    int* cut;              // scratch: P*C direct-path row lengths (k_rir_direct), or null: no direct target
+    float* out_direct;     // (C, N) direct-path stem (with `cut`)
     int N, P, C, L;
     int K;                 // RIR partitions = ceil(L / kB)
     int nb;                // ceil(N / kB)
     int mode;              // 0 static, 1 moving (bounds), 2 moving (idx, w)
     int aligned;           // 1: blocks aligned to the trajectory segments (mode 1 and K == 1)
     int nblk_max;          // table size: nb (grid) or nb + P - 1 (aligned)
-    int pad_[1];
+    int direct_taps;       // taps kept from each row's peak on (with `cut`)
 };
 constexpr int kNormParts = 128;    // CTAs (partial maxima) per normalised source in k_rir_absmax
 
@@ -88,16 +91,23 @@ struct XDesc {
 };
 static_assert(sizeof(XDesc) == 112, "XDesc layout");
 
-SS_HD int spectra_pairs_h(const Source& s) { return (s.P * s.C * s.K + 1) >> 1; }
+// RIR rows are transformed two per complex FFT, and the bits of a half spectrum depend on its partner row: the direct
+// rows are paired among themselves exactly as a separate source's rows would be, never with a reverberant row.
+SS_HD int rows_h(const Source& s) { return s.P * s.C * s.K; }                 // per set (reverberant, direct)
+SS_HD int pairs_per_set_h(const Source& s) { return (rows_h(s) + 1) >> 1; }
+SS_HD int spectra_pairs_h(const Source& s) { return pairs_per_set_h(s) * (s.cut ? 2 : 1); }
 SS_HD int spectra_pairs_x(const Source& s) { return (s.nblk_max + 1) >> 1; }
 SS_HD int range_ctas(const Source& s) { return (s.nblk_max + 7) >> 3; }       // k_prepare: one warp per block
-SS_HD int items_per_block(const Source& s) { return s.mode == MODE_STATIC ? (s.C + 1) >> 1 : s.C; }
+SS_HD int items_per_set(const Source& s) { return s.mode == MODE_STATIC ? (s.C + 1) >> 1 : s.C; }
+SS_HD int items_per_block(const Source& s) { return items_per_set(s) * (s.cut ? 2 : 1); }
 SS_HD int max_render_items(const Source& s) { return s.nblk_max * items_per_block(s); }
 
 // blocks of one segment under aligned blocking
 SS_HD int seg_blocks(int n_s) { return (n_s + kB - 1) / kB; }
 
-// fill the work items of block `blk` once its position range is known (lanes split the channels)
+// fill the work items of block `blk` once its position range is known (lanes split the channels).  A direct-target
+// source's block has the reverberant items first, then as many direct items (direct spectra, `out_direct`): all of
+// them carry the block's X, so k_render_fast stages it once for both stems.
 SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, int lane, int nlanes) {
     RItem it;
     it.X = s.xspec + (size_t)blk * kSpec;
@@ -108,26 +118,27 @@ SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, i
     it.kparts = reach < s.K ? reach : s.K;
     it.b0 = 0; it.step = 0.0; it.pad_[0] = 0; it.pad_[1] = 0;
     if (s.aligned) { it.b0 = s.bounds[bk.p_lo]; it.step = s.rstep[bk.p_lo]; }
-    const int per = items_per_block(s);
-    RItem* dst = items + s.counts[1] + (size_t)blk * per;
-    if (s.mode == MODE_STATIC) {
-        for (int cp = lane; cp < per; cp += nlanes) {
-            it.H0 = s.hspec + (size_t)(2 * cp) * s.K * kSpec;
-            it.row = s.out + (size_t)(2 * cp) * s.N;
-            it.row1 = (2 * cp + 1 < s.C) ? it.row + s.N : nullptr;
+    const int per = items_per_set(s);
+    RItem* dst = items + s.counts[1] + (size_t)blk * items_per_block(s);
+    for (int i = lane; i < items_per_block(s); i += nlanes) {
+        const bool direct = i >= per;
+        const int c = direct ? i - per : i;
+        const float2* const spec = s.hspec + (direct ? (size_t)rows_h(s) * kSpec : 0);
+        float* const out = direct ? s.out_direct : s.out;
+        if (s.mode == MODE_STATIC) {                 // item c: channels 2c, 2c + 1
+            it.H0 = spec + (size_t)(2 * c) * s.K * kSpec;
+            it.row = out + (size_t)(2 * c) * s.N;
+            it.row1 = (2 * c + 1 < s.C) ? it.row + s.N : nullptr;
             it.pstride = s.K * kSpec;
             it.p_lo = 0; it.p_hi = 0;
-            dst[cp] = it;
-        }
-    } else {
-        for (int c = lane; c < per; c += nlanes) {
-            it.H0 = s.hspec + (size_t)c * s.K * kSpec;
-            it.row = s.out + (size_t)c * s.N;
+        } else {
+            it.H0 = spec + (size_t)c * s.K * kSpec;
+            it.row = out + (size_t)c * s.N;
             it.row1 = nullptr;
             it.pstride = s.C * s.K * kSpec;
             it.p_lo = bk.p_lo; it.p_hi = bk.p_hi;
-            dst[c] = it;
         }
+        dst[i] = it;
     }
 }
 
@@ -195,12 +206,22 @@ SS_HD float rir_absmax(const Source& s) {
     for (int i = 0; i < kNormParts; ++i) { const float v = s.norm_part[i]; m = v > m ? v : m; }
     return m;
 }
-SS_HD Row make_row_h(const Source& s, int row) {
-    if (row >= s.P * s.C * s.K) return no_row();
+// RIR row `row` (= (p * C + c) * K + partition) of set 0 (reverberant) or 1 (direct: the same taps, zero from
+// cut[p, c] on - make_row zero-fills beyond `len`)
+SS_HD Row make_row_h(const Source& s, int row, int set = 0) {
+    if (row >= rows_h(s)) return no_row();
     int part = row % s.K, pc = row / s.K;
-    Row r = make_row(s.rir + (size_t)pc * s.L, s.hspec + (size_t)row * kSpec, part * kB, s.L, kB, 1.0f / (float)kF);
+    const int len = set ? s.cut[pc] : s.L;
+    Row r = make_row(s.rir + (size_t)pc * s.L, s.hspec + ((size_t)set * rows_h(s) + row) * kSpec, part * kB, len, kB,
+                     1.0f / (float)kF);
     if (s.norm_part) r.div = rir_absmax(s);
     return r;
+}
+// the two rows of k_prepare's RIR CTA `local` (< spectra_pairs_h): pairs of the reverberant set, then of the direct set
+SS_HD void rows_of_pair_h(const Source& s, int local, Row& ra, Row& rb) {
+    const int set = local >= pairs_per_set_h(s) ? 1 : 0, j = local - set * pairs_per_set_h(s);
+    ra = make_row_h(s, 2 * j, set);
+    rb = make_row_h(s, 2 * j + 1, set);
 }
 SS_HD Row make_row_x(const Source& s, int blk) {
     if (blk >= s.nblk_max) return no_row();
@@ -219,6 +240,22 @@ SS_HD float div_rn(float a, float b) {
     return a / b;
 #endif
 }
+
+// Direct-path cut of one RIR row (k_rir_direct; lane `lane` of `nlanes` scans taps lane, lane + nlanes, ...):
+// first index of the maximum of |h| (|h / div| when div != 0, the bits k_prepare's row loads produce).  Partial
+// results combine with peak_first, which prefers the smaller index on equal values, so the result is that of a
+// sequential scan whatever the lane order.
+struct PeakAt { float v; int i; };
+SS_HD PeakAt peak_first(PeakAt a, PeakAt b) { return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a; }
+SS_HD PeakAt peak_scan(const float* h, int L, float div, int lane, int nlanes) {
+    PeakAt m; m.v = -1.f; m.i = 0;                   // below every |h|: an all-zero row peaks at 0
+    for (int k = lane; k < L; k += nlanes) {
+        const float a = fabsf(div != 0.f ? div_rn(h[k], div) : h[k]);
+        if (a > m.v) { m.v = a; m.i = k; }
+    }
+    return m;
+}
+SS_HD int direct_cut(int peak, int L, int taps) { return peak < L - taps ? peak + taps : L; }   // min(L, peak + taps)
 
 struct Regs32 { float2 a[16]; float2 b[16]; };
 

@@ -27,6 +27,8 @@ class MovingSource(T.NamedTuple):
     bounds_host: T.Any = None
     normalize_rirs: bool = False      # rirs = raw simulator output (formats.stack_rirs): divide by their global
                                       # abs-max on the device like generate_rir_combination (SonicSim_audio.py:398)
+    direct_taps: int = 0              # > 0: also render the direct-path stem (every RIR row cut `direct_taps` taps
+                                      # after its peak, see SS_DIRECT_TARGET) into the source's direct_outs entry
 
 
 class StaticSource(T.NamedTuple):
@@ -34,6 +36,25 @@ class StaticSource(T.NamedTuple):
     dry: T.Any
     rir: T.Any
     normalize_rirs: bool = False
+    direct_taps: int = 0              # as MovingSource.direct_taps
+
+
+def _flags(s, i, direct_out) -> int:
+    """ss_source.flags of source i; checks that a direct-path stem has an output and an output has a stem."""
+    taps = int(s.direct_taps)
+    if taps < 0:
+        raise ValueError("direct_taps of source %d must be >= 0, got %d" % (i, taps))
+    if taps > 0 and direct_out is None:
+        raise ValueError("source %d has direct_taps = %d but no direct output (direct_outs[%d])" % (i, taps, i))
+    if taps == 0 and direct_out is not None:
+        raise ValueError("direct_outs[%d] is given but source %d has no direct_taps" % (i, i))
+    return (_lib.SS_RIR_NORMALIZE if s.normalize_rirs else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
+
+
+def _check_direct_outs(direct_outs, n):
+    if direct_outs is not None and len(direct_outs) != n:
+        raise ValueError("%d sources but %d entries in direct_outs" % (n, len(direct_outs)))
+    return direct_outs if direct_outs is not None else [None] * n
 
 
 class Renderer:
@@ -47,12 +68,14 @@ class Renderer:
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
                   outs: T.Optional[T.Sequence[np.ndarray]] = None,
-                  lufs_targets: T.Optional[T.Sequence[T.Optional[float]]] = None, sr: float = 16000) -> "HostPlan":
+                  lufs_targets: T.Optional[T.Sequence[T.Optional[float]]] = None, sr: float = 16000,
+                  direct_outs: T.Optional[T.Sequence[T.Optional[np.ndarray]]] = None) -> "HostPlan":
         """Validate a batch once and bind it to its host buffers; `plan.run()` then renders it with a single
         C-ABI call (a generation loop refills the same pinned buffers and calls run() again).
         See render_host for the arguments."""
         from .SonicSim_audio import gating_plan
         n = len(sources)
+        direct_outs = _check_direct_outs(direct_outs, n)
         items = (SsSource * n)()
         post = (SsPostLufs * n)() if lufs_targets is not None else None
         results_l = np.full((n, 2), np.nan, dtype=np.float64)
@@ -75,10 +98,17 @@ class Renderer:
             out = outs[i] if outs is not None else np.empty((C, N), dtype=np.float32)
             if out.shape != (C, N) or out.dtype != np.float32 or not out.flags.c_contiguous:
                 raise ValueError("out[%d] must be C-contiguous float32 of shape (C, N)" % i)
+            dout = direct_outs[i]
+            flags = _flags(s, i, dout)
+            if dout is not None and (not isinstance(dout, np.ndarray) or dout.shape != (C, N) or
+                                     dout.dtype != np.float32 or not dout.flags.c_contiguous):
+                raise ValueError("direct_outs[%d] must be C-contiguous float32 of shape (C, N)" % i)
             items[i] = SsSource(x=x.ctypes.data, rir=h.ctypes.data, out=out.ctypes.data,
                                 bounds=bounds.ctypes.data if bounds is not None else None,
-                                N=N, P=P, C=C, L=L, mode=mode, flags=_lib.SS_RIR_NORMALIZE if s.normalize_rirs else 0)
-            keep.append((x, h, bounds, out))
+                                N=N, P=P, C=C, L=L, mode=mode, flags=flags,
+                                out_direct=dout.ctypes.data if dout is not None else None,
+                                direct_taps=int(s.direct_taps))
+            keep.append((x, h, bounds, out, dout))
             results.append(out)
             if post is not None and lufs_targets[i] is not None:
                 if C > 8:
@@ -94,42 +124,48 @@ class Renderer:
     def render_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
                     outs: T.Optional[T.Sequence[np.ndarray]] = None,
                     lufs_targets: T.Optional[T.Sequence[T.Optional[float]]] = None, sr: float = 16000,
-                    loudness_out: T.Optional[list] = None) -> T.List[np.ndarray]:
+                    loudness_out: T.Optional[list] = None,
+                    direct_outs: T.Optional[T.Sequence[T.Optional[np.ndarray]]] = None) -> T.List[np.ndarray]:
         """Render every source; returns a list of (C, N) float32 arrays (pinned `outs` may be passed).
         `lufs_targets[i]` (or None) additionally normalises stem i to that integrated loudness on
         the device before the copy out - SonicSim_audio.lufs_norm fused behind the render
-        (SonicSet.py:97-101).  `loudness_out`, if a list, receives (measured LUFS, linear gain) per source."""
-        plan = self.plan_host(sources, outs, lufs_targets, sr)
+        (SonicSet.py:97-101).  `loudness_out`, if a list, receives (measured LUFS, linear gain) per source.
+        `direct_outs[i]`: a (C, N) float32 array that receives the direct-path stem of a source with direct_taps > 0
+        (None for the other sources); with a loudness target it is scaled by the reverberant stem's gain."""
+        plan = self.plan_host(sources, outs, lufs_targets, sr, direct_outs)
         res = plan.run()
         if loudness_out is not None and lufs_targets is not None:
             loudness_out[:] = plan.loudness()
         return res
 
     # ------------------------------------------------------------------ device tensors
-    def render_device(self, sources, outs, stream: T.Optional[int] = None):
+    def render_device(self, sources, outs, stream: T.Optional[int] = None, direct_outs=None):
         """`sources`: MovingSource / StaticSource whose fields are CUDA float32 / int32 tensors;
-        `outs`: preallocated CUDA (C, N) tensors.  Asynchronous on `stream` (torch current stream)."""
-        items, n, keep = self._device_items(sources, outs)
+        `outs`: preallocated CUDA (C, N) tensors; `direct_outs`: the same for the direct-path stems of sources with
+        direct_taps > 0, None for the others.  Asynchronous on `stream` (torch current stream)."""
+        items, n, keep = self._device_items(sources, outs, direct_outs)
         if stream is None:
             import torch
             stream = torch.cuda.current_stream().cuda_stream
         _lib.check(self.lib.ss_render_dev(self.ctx, items, n, ctypes.c_void_p(stream)))
 
-    def plan_device(self, sources, outs) -> "DevicePlan":
+    def plan_device(self, sources, outs, direct_outs=None) -> "DevicePlan":
         """Bind a batch of device-resident sources to its output tensors once; `plan.run()` then renders it with a
         single C-ABI call - one CUDA graph launch (ss_plan_run; a generation loop overwrites the same tensors and
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
-        (N,), RIRs (P, C, L) / (C, L), outs[i] (C, N) for that source's own C and N; int32 bounds (P,)."""
-        return DevicePlan(self, *self._device_items(sources, outs))
+        (N,), RIRs (P, C, L) / (C, L), outs[i] (C, N) for that source's own C and N; int32 bounds (P,); direct_outs[i]
+        as outs[i] for a source with direct_taps > 0, else None."""
+        return DevicePlan(self, *self._device_items(sources, outs, direct_outs))
 
-    def _device_items(self, sources, outs):
+    def _device_items(self, sources, outs, direct_outs=None):
         """Validated ss_source array of a device-resident batch: (items, n, objects to keep alive)."""
         import torch
         n = len(sources)
         if len(outs) != n:
             raise ValueError("plan_device: %d sources but %d output tensors" % (n, len(outs)))
+        direct_outs = _check_direct_outs(direct_outs, n)
         items = (SsSource * n)()
-        keep = [sources, outs]
+        keep = [sources, outs, direct_outs]
 
         def chk(t, name, i, dtype, shape=None):
             if not isinstance(t, torch.Tensor) or not t.is_cuda:
@@ -155,8 +191,7 @@ class Renderer:
                 C, L = s.rir.shape
                 chk(outs[i], "out", i, torch.float32, (C, N))
                 items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rir.data_ptr(), out=outs[i].data_ptr(),
-                                    N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC,
-                                    flags=_lib.SS_RIR_NORMALIZE if s.normalize_rirs else 0)
+                                    N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC)
             else:
                 chk(s.rirs, "rirs", i, torch.float32)
                 if s.rirs.dim() != 3:
@@ -172,8 +207,12 @@ class Renderer:
                     keep.append(bh)
                 items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rirs.data_ptr(), out=outs[i].data_ptr(),
                                     bounds=s.bounds.data_ptr(), N=N, P=P, C=C, L=L,
-                                    mode=_lib.SS_MOVING_BOUNDS, bounds_host=bh.ctypes.data if bh is not None else None,
-                                    flags=_lib.SS_RIR_NORMALIZE if s.normalize_rirs else 0)
+                                    mode=_lib.SS_MOVING_BOUNDS, bounds_host=bh.ctypes.data if bh is not None else None)
+            items[i].flags = _flags(s, i, direct_outs[i])
+            if direct_outs[i] is not None:
+                chk(direct_outs[i], "direct_out", i, torch.float32, (C, N))
+                items[i].out_direct = direct_outs[i].data_ptr()
+                items[i].direct_taps = int(s.direct_taps)
         return items, n, keep
 
     def check_device_errors(self):
