@@ -148,6 +148,9 @@ int ss_convolve_moving_receiver(ss_ctx* ctx, const float* source_audio, const fl
  * truncated with int()), and passed as `brk` = the sorted distinct bounds (n_e + 1 values) plus,
  * per gating block j, the range [blk_lo[j], blk_hi[j]) of elementary intervals it covers. */
 #define SS_LOUD_SCRATCH_DOUBLES 20
+/* Layout: a measure-only item (out == NULL) may use any strides.  With `out`, the strides must describe a
+ * dense block of N*C floats - (stride_n, stride_c) = (C, 1) for (N, C) or (1, N) for (C, N) - because
+ * out[q] = gain * data[q] for q < N*C; other strides return SS_ERR_INVALID. */
 typedef struct {
     const float* data;        /* element (n, c) at data[n * stride_n + c * stride_c]                   */
     float* out;               /* N*C contiguous floats = gain * data (may alias data); NULL = measure  */
@@ -163,11 +166,13 @@ typedef struct {
     double target_lufs;       /* `norm` of lufs_norm                                                   */
 } ss_loud_item;
 
-/* Device pointers, asynchronous on `stream`; all items share one sample rate. */
+/* Device pointers, asynchronous on `stream`; all items share one sample rate; C <= 8 (channel gains
+ * 1, 1, 1, 1.41, 1.41, then 1 for channels 5-7), else SS_ERR_UNSUPPORTED. */
 int ss_loudness_dev(ss_ctx* ctx, const ss_loud_item* items, int n_items, void* stream);
 
-/* One stem in host memory (any layout through the strides); returns when `out` (if given), the
- * measured loudness and the linear gain are available. */
+/* One stem in host memory, N*C floats in a dense (N, C) or (C, N) layout given by the strides (other
+ * strides return SS_ERR_INVALID, even when measuring only: the block is copied as it is); returns when
+ * `out` (if given, same layout), the measured loudness and the linear gain are available. */
 int ss_lufs_norm_host(ss_ctx* ctx, const float* data, float* out, int32_t N, int32_t C,
                       int64_t stride_n, int64_t stride_c, double rate, double block_size,
                       double target_lufs, const int32_t* brk, int32_t n_e, const int32_t* blk_lo,
@@ -183,7 +188,9 @@ typedef struct {
     double* result;           /* host, 2 doubles: measured LUFS, linear gain (may be NULL)             */
 } ss_post_lufs;
 
-/* ss_render_host + optional loudness normalisation of each stem while it is still in HBM. */
+/* ss_render_host + optional loudness normalisation of each stem while it is still in HBM.  Every source
+ * with a target must have C <= 8 and the rate of the first source that has one; otherwise the call returns
+ * SS_ERR_INVALID before anything is copied. */
 int ss_render_host_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss_post_lufs* post);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py

@@ -125,6 +125,9 @@ def fft_conv(sig, kernel):
 # --------------------------------------------------------------------------- a5
 # pyloudnorm 0.1.1 restatement ("parity unpinned", see module docstring).
 _BS1770_G = [1.0, 1.0, 1.0, 1.41, 1.41]        # pyloudnorm/meter.py channel gains
+# The library's extension to 6-8 channels (mic arrays; include/sonicsim_b200.h ss_loudness_dev): weight 1 beyond
+# pyloudnorm's five.  Off by default, where more than five channels raise as in pyloudnorm.
+_BS1770_G8 = _BS1770_G + [1.0, 1.0, 1.0]
 
 
 def bs1770_k_weighting(rate):
@@ -167,13 +170,15 @@ def bs1770_block_bounds(num_samples, rate, block_size):
     return lo, hi
 
 
-def bs1770_integrated_loudness(data, rate, block_size=0.400):
-    """pyloudnorm 0.1.1 Meter(rate, block_size=...).integrated_loudness(data), data (N,C) or (N,)."""
+def _bs1770_gating(data, rate, block_size, up_to_8_channels):
+    """The steps of integrated_loudness: (block loudness l_j, relative gate gamma_r, integrated loudness)."""
     data = np.asarray(data)
     if not np.issubdtype(data.dtype, np.floating):
         raise ValueError("Data must be floating point.")
-    if data.ndim == 2 and data.shape[1] > 5:
-        raise ValueError("Audio must have five channels or less.")
+    max_ch = 8 if up_to_8_channels else 5
+    if data.ndim == 2 and data.shape[1] > max_ch:
+        raise ValueError("Audio must have five channels or less." if max_ch == 5 else
+                         "Audio must have eight channels or less.")
     if data.shape[0] < block_size * rate:
         raise ValueError("Audio must have length greater than the block size.")
     x = data.copy()
@@ -190,7 +195,7 @@ def bs1770_integrated_loudness(data, rate, block_size=0.400):
     for i in range(n_ch):
         for j in range(nb):
             z[i, j] = (1.0 / (T_g * rate)) * np.sum(np.square(x[lo[j]:hi[j], i]))
-    G = _BS1770_G
+    G = _BS1770_G8 if up_to_8_channels else _BS1770_G
     with np.errstate(divide="ignore", invalid="ignore"):
         l = [-0.691 + 10.0 * np.log10(np.sum([G[i] * z[i, j] for i in range(n_ch)])) for j in range(nb)]
         J_g = [j for j, l_j in enumerate(l) if l_j >= -70.0]
@@ -199,15 +204,28 @@ def bs1770_integrated_loudness(data, rate, block_size=0.400):
         J_g = [j for j, l_j in enumerate(l) if (l_j > gamma_r and l_j > -70.0)]
         z_avg = np.nan_to_num(np.array([np.mean([z[i, j] for j in J_g]) for i in range(n_ch)]))
         lufs = -0.691 + 10.0 * np.log10(np.sum([G[i] * z_avg[i] for i in range(n_ch)]))
-    return float(lufs)
+    return np.array(l, dtype=np.float64), float(gamma_r), float(lufs)
 
 
-def lufs_norm(data, sr, norm=-6):
+def bs1770_integrated_loudness(data, rate, block_size=0.400, up_to_8_channels=False):
+    """pyloudnorm 0.1.1 Meter(rate, block_size=...).integrated_loudness(data), data (N,C) or (N,).
+    `up_to_8_channels`: accept 6-8 channels with weight 1 for channels 5-7 (the library's extension)."""
+    return _bs1770_gating(data, rate, block_size, up_to_8_channels)[2]
+
+
+def bs1770_block_loudness(data, rate, block_size=0.400, up_to_8_channels=False):
+    """(loudness of every gating block, relative gate) of integrated_loudness, for tests that must keep their
+    signals away from the two gates."""
+    l, gamma_r, _ = _bs1770_gating(data, rate, block_size, up_to_8_channels)
+    return l, gamma_r
+
+
+def lufs_norm(data, sr, norm=-6, up_to_8_channels=False):
     """SonicSim_audio.py:68-81.  Output kept in the input dtype (float32), which is what the
     reference's pinned numpy 1.23.5 produces for `np.float64 scalar * float32 array`."""
     data = np.asarray(data)
     block_size = 0.4 if len(data) / sr >= 0.4 else len(data) / sr                   # :69
-    loudness = bs1770_integrated_loudness(data, sr, block_size)                     # :71-72
+    loudness = bs1770_integrated_loudness(data, sr, block_size, up_to_8_channels)   # :71-72
     if math.isinf(loudness):                                                        # :73
         loudness = -40
     gain_lin = np.power(10.0, (norm - loudness) / 20.0)                             # pyln.normalize.loudness

@@ -1286,12 +1286,16 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     if (!c || (!items && n_items > 0) || n_items < 0) return SS_ERR_INVALID;
     if (n_items == 0) return SS_OK;
     CK(cudaSetDevice(c->device));
+    // every stem with a target shares one sample rate (ss_loudness_dev runs one set of filter coefficients per call);
+    // checked against the first source that has a target, so that the answer does not depend on the chunking
+    const ss_post_lufs* first_post = nullptr;
     for (int i = 0; i < n_items; ++i) {
         int st = validate_item(items[i]); if (st) return st;
         st = check_traj_host(items[i]); if (st) return st;
         if (post && post[i].brk) {
             if (!post[i].blk_lo || !post[i].blk_hi || post[i].n_e <= 0 || post[i].rate <= 0 || items[i].C > 8) return SS_ERR_INVALID;
-            if (post[i].rate != post[0].rate && post[0].brk) return SS_ERR_INVALID;
+            if (!first_post) first_post = &post[i];
+            if (post[i].rate != first_post->rate) return SS_ERR_INVALID;
         }
     }
     // an earlier asynchronous ss_render_dev may still be using scratch buffer 0 on its internal streams

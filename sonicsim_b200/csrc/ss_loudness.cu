@@ -201,10 +201,17 @@ k_loud_scale(const LoudItem* __restrict__ items) {
     }
 }
 
+// (stride_n, stride_c) describe a dense (N, C) or (C, N) block of N*C floats: k_loud_scale writes `out` as the N*C
+// floats that follow it, so that is the only layout in which out[q] = gain * data[q] scales element (n, c) in place.
+static bool dense_layout(int64_t N, int64_t C, int64_t sn, int64_t sc) {
+    return (sc == 1 && (sn == C || N == 1)) || (sn == 1 && (sc == N || C == 1));
+}
+
 static int validate_loud(const ss_loud_item& it) {
     if (!it.data || !it.brk || !it.blk_lo || !it.blk_hi || !it.scratch || !it.result) return SS_ERR_INVALID;
     if (it.N <= 0 || it.C <= 0 || it.n_e <= 0 || it.n_blocks < 0 || it.rate <= 0) return SS_ERR_INVALID;
     if (it.C > 8) return SS_ERR_UNSUPPORTED;
+    if (it.out && !dense_layout(it.N, it.C, it.stride_n, it.stride_c)) return SS_ERR_INVALID;   // measuring: any strides
     return SS_OK;
 }
 
@@ -288,12 +295,14 @@ int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t 
     return SS_OK;
 }
 
-// Single stem, host arrays (the drop-in lufs_norm): data / out hold N*C floats in the caller's layout.
+// Single stem, host arrays (the drop-in lufs_norm): data / out hold N*C floats in the caller's layout, which is copied
+// to the device as one block, so the strides must describe a dense layout even when only measuring.
 extern "C" int ss_lufs_norm_host(ss_ctx* c, const float* data, float* out, int32_t N, int32_t C,
                                  int64_t stride_n, int64_t stride_c, double rate, double block_size,
                                  double target_lufs, const int32_t* brk, int32_t n_e, const int32_t* blk_lo,
                                  const int32_t* blk_hi, int32_t n_blocks, double* loudness, double* gain) {
     if (!c || !data || !brk || !blk_lo || !blk_hi || N <= 0 || C <= 0 || n_e <= 0) return SS_ERR_INVALID;
+    if (!dense_layout(N, C, stride_n, stride_c)) return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     const size_t nel = (size_t)N * C;
     const size_t o_data = 0;

@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+from chunk_budget import chunk_budget  # noqa: F401  (fixture)
 from conftest import TOL
 from oracle import sonicsim_oracle as so
 
@@ -170,56 +171,52 @@ def test_long_rir_partitioned_cfg4_shape_reduced(sm):
     assert so.rel_rms(sm.convolve_fixed_receiver(x[None], h[0]), so.convolve_fixed_receiver(x[None], h[0])) < TOL
 
 
-def test_large_mixed_batch_multi_chunk_two_streams():
+def test_large_mixed_batch_multi_chunk_two_streams(chunk_budget):
     """Many heterogeneous sources in one device-path call (several chunks, alternating streams, both
     blocking modes, long RIRs, static sources) == the same sources rendered one by one."""
     from sonicsim_b200 import render
     rng = np.random.default_rng(99)
-    R = render.default_renderer()
-    R.set_chunk_bytes(8 << 20)                       # force many chunks
-    try:
-        srcs_np = []
-        for i in range(23):
-            N = int(rng.integers(3000, 90000))
-            C = int(rng.integers(1, 7))
-            kind = i % 4
-            if kind == 0:
-                srcs_np.append(("static", so.synth_dry(rng, N), so.synth_rirs(rng, 1, C, int(rng.integers(8, 3000)))[0]))
-            else:
-                P = int(rng.integers(2, 12))
-                L = int(rng.integers(8, 3000)) if kind != 3 else int(rng.integers(4097, 9000))
-                pos = so.synth_path(rng, P)
-                np.random.seed(i)
-                srcs_np.append(("moving", so.synth_dry(rng, N), so.synth_rirs(rng, P, C, L), render.trajectory_bounds(pos, N)))
-        dev, outs = [], []
-        for s in srcs_np:
-            if s[0] == "static":
-                dev.append(render.StaticSource(torch.from_numpy(s[1]).cuda(), torch.from_numpy(s[2]).cuda()))
-                outs.append(torch.empty((s[2].shape[0], s[1].shape[0]), device="cuda"))
-            else:
-                bh = s[3] if len(dev) % 2 == 0 else None          # mix host-built and device-built block tables
-                dev.append(render.MovingSource(torch.from_numpy(s[1]).cuda(), torch.from_numpy(s[2]).cuda(),
-                                               torch.from_numpy(s[3]).cuda(), bh))
-                outs.append(torch.empty((s[2].shape[1], s[1].shape[0]), device="cuda"))
-        R.render_device(dev, outs)
-        torch.cuda.synchronize()
-        for s, o, dsrc in zip(srcs_np, outs, dev):
-            if s[0] == "static":
-                one = R.render_host([render.StaticSource(s[1], s[2])])[0]
-                ref = so.convolve_fixed_receiver(s[1][None], s[2])
-            else:
-                one = R.render_host([render.MovingSource(s[1], s[2], s[3])])[0]
-                idx = np.repeat(np.arange(len(s[3]) - 1), np.diff(s[3]))
-                w = np.concatenate([np.linspace(0, 1, n, endpoint=False) for n in np.diff(s[3])]).astype(np.float32)
-                ref = so.convolve_moving_receiver(s[1], s[2], idx, w)
-            same_plan = s[0] == "static" or dsrc.bounds_host is not None      # without host bounds the blocking plan is a heuristic
-            if same_plan:
-                assert np.array_equal(o.cpu().numpy(), one)
-            else:
-                assert so.rel_rms(o.cpu().numpy(), one) < 2e-6
-            assert so.rel_rms(one, ref) < TOL
-    finally:
-        R.set_chunk_bytes(96 << 20)
+    R = chunk_budget(8 << 20)                       # force many chunks
+    srcs_np = []
+    for i in range(23):
+        N = int(rng.integers(3000, 90000))
+        C = int(rng.integers(1, 7))
+        kind = i % 4
+        if kind == 0:
+            srcs_np.append(("static", so.synth_dry(rng, N), so.synth_rirs(rng, 1, C, int(rng.integers(8, 3000)))[0]))
+        else:
+            P = int(rng.integers(2, 12))
+            L = int(rng.integers(8, 3000)) if kind != 3 else int(rng.integers(4097, 9000))
+            pos = so.synth_path(rng, P)
+            np.random.seed(i)
+            srcs_np.append(("moving", so.synth_dry(rng, N), so.synth_rirs(rng, P, C, L), render.trajectory_bounds(pos, N)))
+    dev, outs = [], []
+    for s in srcs_np:
+        if s[0] == "static":
+            dev.append(render.StaticSource(torch.from_numpy(s[1]).cuda(), torch.from_numpy(s[2]).cuda()))
+            outs.append(torch.empty((s[2].shape[0], s[1].shape[0]), device="cuda"))
+        else:
+            bh = s[3] if len(dev) % 2 == 0 else None          # mix host-built and device-built block tables
+            dev.append(render.MovingSource(torch.from_numpy(s[1]).cuda(), torch.from_numpy(s[2]).cuda(),
+                                           torch.from_numpy(s[3]).cuda(), bh))
+            outs.append(torch.empty((s[2].shape[1], s[1].shape[0]), device="cuda"))
+    R.render_device(dev, outs)
+    torch.cuda.synchronize()
+    for s, o, dsrc in zip(srcs_np, outs, dev):
+        if s[0] == "static":
+            one = R.render_host([render.StaticSource(s[1], s[2])])[0]
+            ref = so.convolve_fixed_receiver(s[1][None], s[2])
+        else:
+            one = R.render_host([render.MovingSource(s[1], s[2], s[3])])[0]
+            idx = np.repeat(np.arange(len(s[3]) - 1), np.diff(s[3]))
+            w = np.concatenate([np.linspace(0, 1, n, endpoint=False) for n in np.diff(s[3])]).astype(np.float32)
+            ref = so.convolve_moving_receiver(s[1], s[2], idx, w)
+        same_plan = s[0] == "static" or dsrc.bounds_host is not None      # without host bounds the blocking plan is a heuristic
+        if same_plan:
+            assert np.array_equal(o.cpu().numpy(), one)
+        else:
+            assert so.rel_rms(o.cpu().numpy(), one) < 2e-6
+        assert so.rel_rms(one, ref) < TOL
 
 
 def test_many_small_sources_in_one_chunk():
@@ -283,62 +280,58 @@ def test_host_plan_rerun_with_refilled_buffers():
         xs[:] = so.synth_dry(rng, N)
 
 
-def test_device_plan_is_one_graph_launch_and_matches_direct_launches():
+def test_device_plan_is_one_graph_launch_and_matches_direct_launches(chunk_budget):
     """Renderer.plan_device -> ss_plan_*: descriptors + scratch resident, launches captured into a CUDA graph (several
     chunks forked over the internal streams).  Must equal ss_render_dev bit for bit, pick up refilled buffers, and
     reject tensors that would make the kernels write out of bounds (ADVICE r1)."""
     from sonicsim_b200 import render
     rng = np.random.default_rng(321)
-    R = render.default_renderer()
-    R.set_chunk_bytes(8 << 20)                       # several chunks -> fork / join inside the graph
-    try:
-        dev, outs, host = [], [], []
-        for i in range(9):
-            N, C, P = int(rng.integers(20000, 60000)), int(rng.integers(1, 5)), int(rng.integers(2, 9))
-            L = int(rng.integers(100, 4096)) if i % 3 else int(rng.integers(4097, 7000))
-            x, h = so.synth_dry(rng, N), so.synth_rirs(rng, P, C, L)
-            np.random.seed(40 + i)
-            b = render.trajectory_bounds(so.synth_path(rng, P), N)
-            host.append((x, h, b))
-            dev.append(render.MovingSource(torch.from_numpy(x).cuda(), torch.from_numpy(h).cuda(), torch.from_numpy(b).cuda(),
-                                           b if i % 2 == 0 else None))
-            outs.append(torch.empty((C, N), device="cuda"))
-        xs, hs_ = so.synth_dry(rng, 30000), so.synth_rirs(rng, 1, 3, 700)[0]
-        dev.append(render.StaticSource(torch.from_numpy(xs).cuda(), torch.from_numpy(hs_).cuda()))
-        outs.append(torch.empty((3, 30000), device="cuda"))
-        direct = [torch.empty_like(o) for o in outs]
-        R.render_device(dev, direct)
-        plan = R.plan_device(dev, outs)
-        n0 = R.launch_count()
-        plan.run()
-        torch.cuda.synchronize()
-        assert plan.is_graph()
-        assert R.launch_count() > n0                  # the graph's kernels are counted
-        for o, d in zip(outs, direct):
-            assert torch.equal(o, d)
-        # refill one dry signal in place: the next run must see it
-        x0 = so.synth_dry(rng, host[0][0].shape[0])
-        dev[0].dry.copy_(torch.from_numpy(x0))
-        for o in outs:
-            o.zero_()
-        plan.run()
-        torch.cuda.synchronize()
-        one = R.render_host([render.MovingSource(x0, host[0][1], host[0][2])])[0]
-        assert np.array_equal(outs[0].cpu().numpy(), one)
-        for o, d in zip(outs[1:], direct[1:]):
-            assert torch.equal(o, d)
-        plan.close()
-        # validation of device tensors
-        with pytest.raises(ValueError):
-            R.plan_device([dev[0]], [torch.empty((outs[0].shape[0], outs[0].shape[1] - 1), device="cuda")])
-        with pytest.raises(ValueError):
-            R.plan_device([dev[0]], [outs[0].double()])
-        with pytest.raises(ValueError):
-            R.plan_device([render.MovingSource(dev[0].dry, dev[0].rirs.transpose(1, 2), dev[0].bounds)], [outs[0]])
-        with pytest.raises(ValueError):
-            R.plan_device([render.MovingSource(dev[0].dry.cpu(), dev[0].rirs, dev[0].bounds)], [outs[0]])
-    finally:
-        R.set_chunk_bytes(96 << 20)
+    R = chunk_budget(8 << 20)                       # several chunks -> fork / join inside the graph
+    dev, outs, host = [], [], []
+    for i in range(9):
+        N, C, P = int(rng.integers(20000, 60000)), int(rng.integers(1, 5)), int(rng.integers(2, 9))
+        L = int(rng.integers(100, 4096)) if i % 3 else int(rng.integers(4097, 7000))
+        x, h = so.synth_dry(rng, N), so.synth_rirs(rng, P, C, L)
+        np.random.seed(40 + i)
+        b = render.trajectory_bounds(so.synth_path(rng, P), N)
+        host.append((x, h, b))
+        dev.append(render.MovingSource(torch.from_numpy(x).cuda(), torch.from_numpy(h).cuda(), torch.from_numpy(b).cuda(),
+                                       b if i % 2 == 0 else None))
+        outs.append(torch.empty((C, N), device="cuda"))
+    xs, hs_ = so.synth_dry(rng, 30000), so.synth_rirs(rng, 1, 3, 700)[0]
+    dev.append(render.StaticSource(torch.from_numpy(xs).cuda(), torch.from_numpy(hs_).cuda()))
+    outs.append(torch.empty((3, 30000), device="cuda"))
+    direct = [torch.empty_like(o) for o in outs]
+    R.render_device(dev, direct)
+    plan = R.plan_device(dev, outs)
+    n0 = R.launch_count()
+    plan.run()
+    torch.cuda.synchronize()
+    assert plan.is_graph()
+    assert R.launch_count() > n0                  # the graph's kernels are counted
+    for o, d in zip(outs, direct):
+        assert torch.equal(o, d)
+    # refill one dry signal in place: the next run must see it
+    x0 = so.synth_dry(rng, host[0][0].shape[0])
+    dev[0].dry.copy_(torch.from_numpy(x0))
+    for o in outs:
+        o.zero_()
+    plan.run()
+    torch.cuda.synchronize()
+    one = R.render_host([render.MovingSource(x0, host[0][1], host[0][2])])[0]
+    assert np.array_equal(outs[0].cpu().numpy(), one)
+    for o, d in zip(outs[1:], direct[1:]):
+        assert torch.equal(o, d)
+    plan.close()
+    # validation of device tensors
+    with pytest.raises(ValueError):
+        R.plan_device([dev[0]], [torch.empty((outs[0].shape[0], outs[0].shape[1] - 1), device="cuda")])
+    with pytest.raises(ValueError):
+        R.plan_device([dev[0]], [outs[0].double()])
+    with pytest.raises(ValueError):
+        R.plan_device([render.MovingSource(dev[0].dry, dev[0].rirs.transpose(1, 2), dev[0].bounds)], [outs[0]])
+    with pytest.raises(ValueError):
+        R.plan_device([render.MovingSource(dev[0].dry.cpu(), dev[0].rirs, dev[0].bounds)], [outs[0]])
 
 
 def test_device_path_reports_trajectories_it_cannot_refuse():
@@ -380,39 +373,35 @@ def test_device_path_reports_trajectories_it_cannot_refuse():
         R.check_device_errors()
 
 
-def test_fast_kernel_gives_the_same_bits_run_after_run():
+def test_fast_kernel_gives_the_same_bits_run_after_run(chunk_budget):
     """k_render_fast hands its buffers over through mbarriers, a cp.async item ring and a last-warp-out election.  A
     lost hand-over would show as a changed sample: 40 runs of a multi-chunk batch (several items per CTA, X kept and
     replaced) must all equal the first one bit for bit, and the first must match the oracle."""
     from sonicsim_b200 import render
     rng = np.random.default_rng(2024)
-    R = render.default_renderer()
-    R.set_chunk_bytes(24 << 20)
-    try:
-        dev, outs, host = [], [], []
-        for i in range(10):
-            N, P, C, L = 200000 + 4096 * i, 14, 6, 4096
-            x, h = so.synth_dry(rng, N), so.synth_rirs(rng, P, C, L)
-            np.random.seed(300 + i)
-            b = render.trajectory_bounds(so.synth_path(rng, P), N)
-            host.append((x, h, b))
-            dev.append(render.MovingSource(torch.from_numpy(x).cuda(), torch.from_numpy(h).cuda(), torch.from_numpy(b).cuda(), b))
-            outs.append(torch.empty((C, N), device="cuda"))
-        plan = R.plan_device(dev, outs)
+    R = chunk_budget(24 << 20)
+    dev, outs, host = [], [], []
+    for i in range(10):
+        N, P, C, L = 200000 + 4096 * i, 14, 6, 4096
+        x, h = so.synth_dry(rng, N), so.synth_rirs(rng, P, C, L)
+        np.random.seed(300 + i)
+        b = render.trajectory_bounds(so.synth_path(rng, P), N)
+        host.append((x, h, b))
+        dev.append(render.MovingSource(torch.from_numpy(x).cuda(), torch.from_numpy(h).cuda(), torch.from_numpy(b).cuda(), b))
+        outs.append(torch.empty((C, N), device="cuda"))
+    plan = R.plan_device(dev, outs)
+    plan.run()
+    torch.cuda.synchronize()
+    first = [o.clone() for o in outs]
+    for _ in range(40):
+        for o in outs:
+            o.fill_(float("nan"))
         plan.run()
         torch.cuda.synchronize()
-        first = [o.clone() for o in outs]
-        for _ in range(40):
-            for o in outs:
-                o.fill_(float("nan"))
-            plan.run()
-            torch.cuda.synchronize()
-            for o, f in zip(outs, first):
-                assert torch.equal(o, f)
-        x, h, b = host[3]
-        idx = np.repeat(np.arange(len(b) - 1), np.diff(b))
-        w = np.concatenate([np.linspace(0, 1, n, endpoint=False) for n in np.diff(b)]).astype(np.float32)
-        assert so.rel_rms(first[3].cpu().numpy(), so.convolve_moving_receiver(x, h, idx, w)) < TOL
-        plan.close()
-    finally:
-        R.set_chunk_bytes(96 << 20)
+        for o, f in zip(outs, first):
+            assert torch.equal(o, f)
+    x, h, b = host[3]
+    idx = np.repeat(np.arange(len(b) - 1), np.diff(b))
+    w = np.concatenate([np.linspace(0, 1, n, endpoint=False) for n in np.diff(b)]).astype(np.float32)
+    assert so.rel_rms(first[3].cpu().numpy(), so.convolve_moving_receiver(x, h, idx, w)) < TOL
+    plan.close()

@@ -181,3 +181,11 @@ def test_chunking_respects_the_budget_and_balances():
     k = lib.ss_debug_chunks(b.ctypes.data, 32, 96 << 20, cuts.ctypes.data, 33)
     d = np.diff(cuts[:k])
     assert k == 6 and d.min() >= 6 and d.max() <= 7
+
+
+def test_chunk_budget_fixture_restores_the_library_default():
+    """The chunk_budget fixture (tests/chunk_budget.py) puts back the device-path budget a fresh context starts with."""
+    from chunk_budget import DEFAULT_CHUNK_BYTES
+    src = open(os.path.join(ROOT, "sonicsim_b200", "csrc", "ss_internal.h")).read()
+    m = re.search(r"int64_t chunk_bytes = (\d+)ll << (\d+);", src)
+    assert m and (int(m.group(1)) << int(m.group(2))) == DEFAULT_CHUNK_BYTES

@@ -61,6 +61,130 @@ def test_gating_plan_matches_pyloudnorm_expressions():
         assert np.all(np.diff(brk) > 0)
 
 
+def subsonic(seed, N, C, sr=16000):
+    """Noise over a strong 20 Hz tone: the 38 Hz high-pass carries a large state from one interval into the next."""
+    rng = np.random.default_rng(seed)
+    t = np.arange(N) / sr
+    return (0.6 * np.sin(2 * np.pi * 20 * t)[:, None] + 0.05 * rng.standard_normal((N, C))).astype(np.float32)
+
+
+RATES = [8000, 16000, 22050, 44100, 48000]
+EXACT_DB = 1e-6           # kernels vs the float64 restatement: they differ only by float64 rounding of the filter state
+
+
+def block_size_of(N, sr):
+    return 0.4 if N / sr >= 0.4 else N / sr                                   # SonicSim_audio.py:69
+
+
+def assert_clear_of_gates(x, sr, block, margin=1e-3):
+    """No gating block of `x` is within `margin` dB of the absolute (-70) or the relative gate, so rounding cannot
+    move a block across a gate and the comparison with the reference cannot turn on a near-tie."""
+    l, gamma_r = so.bs1770_block_loudness(x, sr, block, up_to_8_channels=True)
+    fin = l[np.isfinite(l)]
+    assert np.all(np.abs(fin + 70.0) > margin), np.min(np.abs(fin + 70.0))
+    if np.isfinite(gamma_r):
+        assert np.all(np.abs(fin - gamma_r) > margin), np.min(np.abs(fin - gamma_r))
+    return l, gamma_r
+
+
+def n_samples_for(n_e, sr):
+    """A clip length whose gating plan has exactly `n_e` elementary intervals (shortest such N from 0.05 s on)."""
+    from sonicsim_b200.SonicSim_audio import gating_plan
+    N = int(0.05 * sr)
+    while True:
+        brk = gating_plan(N, float(sr), float(block_size_of(N, sr)), 1)[0]
+        if len(brk) - 1 == n_e:
+            return N
+        assert len(brk) - 1 < n_e, "no clip length at %g Hz has %d intervals" % (sr, n_e)
+        N += max(1, int(0.01 * sr)) if len(brk) - 1 < n_e - 1 else 1
+
+
+def _emu_vs_reference(emu, x, sr):
+    N = x.shape[0]
+    block = block_size_of(N, sr)
+    assert_clear_of_gates(x, sr, block)
+    ref = so.bs1770_integrated_loudness(x, sr, block, up_to_8_channels=True)
+    got, gain = emu.lufs(x, sr, block, target=-23.0)
+    assert abs(got - ref) <= EXACT_DB, (got, ref)
+    used = -40.0 if np.isinf(got) else got
+    assert abs(gain / 10 ** ((-23.0 - used) / 20) - 1) < 1e-12
+    return got
+
+
+def test_oracle_extension_to_eight_channels():
+    """Channels 5-7 weigh 1 (the documented extension); by default more than five channels still raise like pyloudnorm,
+    and five or fewer give the same value either way."""
+    x = stems(3, 16000, 8)
+    with pytest.raises(ValueError):
+        so.bs1770_integrated_loudness(x[:, :6], 16000)
+    with pytest.raises(ValueError):
+        so.bs1770_integrated_loudness(np.zeros((16000, 9), np.float32), 16000, up_to_8_channels=True)
+    assert so.bs1770_integrated_loudness(x[:, :5], 16000) == so.bs1770_integrated_loudness(x[:, :5], 16000, up_to_8_channels=True)
+    # channel 7 alone weighs like channel 0 alone, channel 3 like 1.41 x channel 0
+    def one(c):
+        y = np.zeros_like(x)
+        y[:, c] = x[:, 0]
+        return y
+    l0 = so.bs1770_integrated_loudness(one(0), 16000, up_to_8_channels=True)
+    assert abs(so.bs1770_integrated_loudness(one(7), 16000, up_to_8_channels=True) - l0) < 1e-12
+    assert abs(so.bs1770_integrated_loudness(one(3), 16000, up_to_8_channels=True) - (l0 + 10 * np.log10(1.41))) < 1e-9
+    y, _ = so.lufs_norm(x, 16000, -20.0, up_to_8_channels=True)
+    assert abs(so.bs1770_integrated_loudness(y, 16000, up_to_8_channels=True) - (-20.0)) < 1e-4
+
+
+@pytest.mark.parametrize("C", range(1, 9))
+def test_emulated_kernels_every_channel_count(emu, C):
+    _emu_vs_reference(emu, stems(40 + C, 27001, C), 16000)
+
+
+@pytest.mark.parametrize("sr", RATES)
+def test_emulated_kernels_every_rate(emu, sr):
+    for C in (1, 6):
+        _emu_vs_reference(emu, stems(sr + C, int(2.37 * sr), C, sr), sr)
+
+
+@pytest.mark.parametrize("n_e", [1, 31, 32, 33, 600])
+def test_emulated_kernels_interval_counts(emu, n_e):
+    """n_e = elementary intervals of a channel: one (a clip shorter than a gating block), around the 32 lanes of the
+    device scan, and many per lane."""
+    sr = 16000
+    N = n_samples_for(n_e, sr)
+    _emu_vs_reference(emu, stems(n_e, N, 2, sr), sr)
+
+
+@pytest.mark.parametrize("sr", [16000, 44100])
+def test_emulated_kernels_last_block_clipped_at_n(emu, sr):
+    """1.06 s: round() adds a gating block whose end lies past the clip; pyloudnorm's x[l:u] clips it at N."""
+    N = int(1.06 * sr)
+    lo, hi = so.bs1770_block_bounds(N, sr, 0.4)
+    assert hi[-1] > N and lo[-1] < N
+    _emu_vs_reference(emu, stems(7, N, 3, sr), sr)
+
+
+PARTITION_CASES = [(16000, 100001, 2, stems), (48000, int(1.06 * 48000), 7, stems), (22050, 5000, 1, stems),
+                   (8000, int(0.41 * 8000), 2, subsonic), (48000, int(1.3 * 48000), 3, subsonic)]
+REFINES = (1, 2, 5, 32)
+
+
+def test_emulated_kernels_do_not_depend_on_the_partition(emu, monkeypatch):
+    """gating_plan(refine=k) cuts each interval into k: more, shorter per-thread recurrences, the same loudness.  The
+    emulation takes its gating tables from SonicSim_audio.gating_plan, which is bound here to each refinement."""
+    from sonicsim_b200 import SonicSim_audio as sa
+    plan = sa.gating_plan
+    for sr, N, C, signal in PARTITION_CASES:
+        x = signal(N + C, N, C, sr)
+        got, n_e = [], []
+        for k in REFINES:
+            def refined(num_samples, rate, block_size, k=k):
+                brk, lo, hi = plan(num_samples, rate, block_size, k)
+                n_e.append(len(brk) - 1)
+                return brk, lo, hi
+            monkeypatch.setattr(sa, "gating_plan", refined)
+            got.append(_emu_vs_reference(emu, x, sr))
+        assert n_e[-1] >= 32 * n_e[0] // 2 and n_e == sorted(n_e), n_e
+        assert max(got) - min(got) < 1e-8, got
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("N,C", [(480000, 2), (960000, 1), (100001, 5), (5000, 2)])
 def test_gpu_lufs_norm_matches_oracle(N, C):
