@@ -86,7 +86,35 @@ typedef struct {
                                  * table is built on the host and one small kernel launch per chunk is saved.     */
     float* out_direct;        /* SS_DIRECT_TARGET: (C, N) direct-path stem, same pointer kind as `out`, != out    */
     int32_t direct_taps;      /* SS_DIRECT_TARGET: taps kept from each row's peak on, >= 1                        */
+    int32_t win_start, win_len; /* time window, see below; win_len == 0: the whole stem                          */
 } ss_source;                  /* fields appended since version 100: a zeroed (memset) struct leaves them off      */
+
+/* Time window (win_len > 0, version 102): the source renders only output samples [win_start, win_start + win_len)
+ * with 0 <= win_start and win_start + win_len <= N.  `out` (and `out_direct`) is then a dense (C, win_len) buffer,
+ * row stride win_len, and every value stored has the bits of the same sample of the full render of the same source by
+ * the same kernel variant: the blocking is chosen over the whole trajectory and length N exactly as for the full stem
+ * (ss_debug_plan), and only the blocks that meet the window are rendered.  The kernel variant depends on the source's
+ * kind - one transform per block (aligned blocking, or static with L <= 4096), L > 4096, or any other - and never on
+ * its window.  ss_render_dev and plans run each kind on its own variant, so there a window always has the bits of the
+ * full stem.  ss_render_host renders each of its chunks with one variant: a chunk that mixes kinds takes the most
+ * general one present, whose roundings may differ from those of the one-transform kernel.  A host-path window therefore
+ * has the full stem's bits when both are rendered in batches whose sources are all of its kind.  Whole stems on the
+ * host path depend on their batch in the same way.  A loudness target of ss_render_host_ex cannot be combined with a
+ * window (the reference normalises the whole stem; a window does not know that stem's gain): SS_ERR_INVALID.
+ *
+ * Read set of a windowed source - everything outside it may hold anything (NaN, garbage; on the host path it is not
+ * even copied):
+ *   - dry x: the windows [start - 4096, start + 4096) of the blocks that meet the window, of the RIR partitions'
+ *     K - 1 = ceil(L / 4096) - 1 grid blocks in front of the first of them, and of the partner block each of these
+ *     is paired with in the forward transform (blocks 2i and 2i + 1 of the full plan share one FFT);
+ *   - bounds: all P entries;  idx / w (SS_MOVING_INDEXED): the samples of the blocks that meet the window;
+ *   - RIR positions: every position a block that meets the window interpolates between, widened to the rows paired
+ *     with them in the forward transform (rows 2r and 2r + 1 of the P * C * K row list share one FFT: when C * K is
+ *     odd, the last row of the position in front may be read);  all P positions under SS_RIR_NORMALIZE (the global
+ *     abs-max) and whenever the trajectory is not visible on the host (SS_MOVING_INDEXED, or a device `bounds` without
+ *     `bounds_host`).
+ * On the device path, ss_device_errors reports only what the kernels read: the idx entries of the read set, and the
+ * bounds table of a grid-blocked source. */
 
 /* library / build identification */
 int ss_version(void);
@@ -257,7 +285,8 @@ int ss_get_profile(ss_ctx* ctx, double* ms_spectra, double* ms_render, int64_t* 
 /* Test hook, pure host code (no CUDA call): the blocking plan of one source whose trajectory bounds are on the host
  * (`bounds_host`): blocks_out receives (start, len, p_lo, p_hi) per block, *aligned_out whether the blocks follow
  * the trajectory's waypoints (one transform each) or the 4096-sample grid.  Returns the number of blocks, or a
- * negative ss_status (SS_ERR_NOMEM: max_blocks too small). */
+ * negative ss_status (SS_ERR_NOMEM: max_blocks too small).  A windowed item gets exactly the entries of its full
+ * plan whose [start, start + len) meets the window, unchanged. */
 int ss_debug_plan(const ss_source* item, int32_t* blocks_out, int32_t max_blocks, int32_t* aligned_out);
 
 /* Test hook, pure host code: how a batch whose items need bytes[i] of scratch is cut into launch groups under `budget`

@@ -60,7 +60,8 @@ class SsSource(ctypes.Structure):
                 ("bounds", ctypes.c_void_p), ("idx", ctypes.c_void_p), ("w", ctypes.c_void_p),
                 ("N", ctypes.c_int32), ("P", ctypes.c_int32), ("C", ctypes.c_int32), ("L", ctypes.c_int32),
                 ("mode", ctypes.c_int32), ("flags", ctypes.c_int32), ("bounds_host", ctypes.c_void_p),
-                ("out_direct", ctypes.c_void_p), ("direct_taps", ctypes.c_int32)]
+                ("out_direct", ctypes.c_void_p), ("direct_taps", ctypes.c_int32),
+                ("win_start", ctypes.c_int32), ("win_len", ctypes.c_int32)]
 
 
 def _stale():

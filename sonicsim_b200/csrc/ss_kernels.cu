@@ -48,6 +48,72 @@ __device__ float2 g_twB[kTabB];      // [r][k] exp(-2 pi i k r / 256)
 __device__ float2 g_twC[kTabC];      // [r][k] exp(-2 pi i k r / 4096)
 
 // ----------------------------------------------------------------------------- k_blocks
+// Windowed source (one warp): the blocks [g0, g1) of the full plan (window_span) and the kept range.  Aligned blocking
+// walks the segments twice - once to find the full-table indices of the blocks holding the window's first and last
+// samples, once to write the blocks in [g0, g1) - so the table never holds the full plan.
+__device__ void blocks_window(const Source& S, int lane) {
+    const int ws = S.counts[4], we = ws + S.counts[5];
+    int k0, k1, nfull;
+    if (S.aligned) {
+        int carry = 0, f0 = -1, f1 = -1;
+        for (int base = 0; base < S.P - 1; base += 32) {
+            const int sg = base + lane;
+            const int b0 = sg < S.P - 1 ? S.bounds[sg] : 0;
+            const int n_s = sg < S.P - 1 ? S.bounds[sg + 1] - b0 : 0;
+            const int cnt = n_s > 0 ? seg_blocks(n_s) : 0;
+            int incl = cnt;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+            const int first = carry + incl - cnt;
+            if (cnt > 0 && ws >= b0 && ws < b0 + n_s) f0 = first + (ws - b0) / kB;
+            if (cnt > 0 && we - 1 >= b0 && we - 1 < b0 + n_s) f1 = first + (we - 1 - b0) / kB;
+            carry += __shfl_sync(0xffffffffu, incl, 31);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            f0 = max(f0, __shfl_xor_sync(0xffffffffu, f0, o));
+            f1 = max(f1, __shfl_xor_sync(0xffffffffu, f1, o));
+        }
+        nfull = carry;
+        k0 = f0 < 0 ? 0 : f0;                     // (-1: a bounds table outside the contract; keep the writes in range)
+        k1 = f1 < k0 ? k0 + 1 : f1 + 1;
+    } else {
+        nfull = S.nb; k0 = ws / kB; k1 = (we + kB - 1) / kB;
+    }
+    const WinSpan w = window_span(k0, k1, nfull, S.K);
+    const int g1 = w.g1 - w.g0 > S.nblk_max ? w.g0 + S.nblk_max : w.g1;
+    if (S.aligned) {
+        int carry = 0;
+        for (int base = 0; base < S.P - 1; base += 32) {
+            const int sg = base + lane;
+            const int b0 = sg < S.P - 1 ? S.bounds[sg] : 0;
+            const int n_s = sg < S.P - 1 ? S.bounds[sg + 1] - b0 : 0;
+            const int cnt = n_s > 0 ? seg_blocks(n_s) : 0;
+            int incl = cnt;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+            const int first = carry + incl - cnt;
+            for (int q = 0; q < cnt; ++q) {
+                if (first + q < w.g0 || first + q >= g1) continue;
+                Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
+                S.blocks[first + q - w.g0] = bk;
+            }
+            carry += __shfl_sync(0xffffffffu, incl, 31);
+        }
+    } else {
+        for (int bi = w.g0 + lane; bi < g1; bi += 32) {
+            Block bk; bk.start = bi * kB; bk.len = S.N - bi * kB < kB ? S.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
+            S.blocks[bi - w.g0] = bk;
+        }
+    }
+    for (int bi = g1 - w.g0 + lane; bi < S.nblk_max; bi += 32) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; S.blocks[bi] = z; }
+    if (lane == 0) {
+        S.counts[0] = g1 - w.g0;
+        S.counts[2] = w.k0 - w.g0;
+        S.counts[3] = (w.k1 < g1 ? w.k1 : g1) - w.k0;
+    }
+}
+
 // One small CTA per chunk: block table of every source (one warp per source), 1 / n_s table, then the
 // exclusive scan that packs the render work items of all sources into one dense table.
 __global__ void __launch_bounds__(256)
@@ -56,6 +122,12 @@ k_blocks(const Source* __restrict__ srcs, int n_src, int* __restrict__ total_ite
     for (int si = warp; si < n_src; si += nwarps) {
         const Source& S = srcs[si];
         int nblk;
+        if (S.h_rows) {
+            blocks_window(S, lane);
+            if (S.mode == MODE_MOVING_BOUNDS)
+                for (int sg = lane; sg < S.P - 1; sg += 32) S.rstep[sg] = 1.0 / (double)(S.bounds[sg + 1] - S.bounds[sg]);
+            continue;
+        }
         if (S.aligned) {
             int carry = 0;
             for (int base = 0; base < S.P - 1; base += 32) {
@@ -91,7 +163,7 @@ k_blocks(const Source* __restrict__ srcs, int n_src, int* __restrict__ total_ite
         int carry = 0;
         for (int base = 0; base < n_src; base += 32) {
             const int si = base + lane;
-            const int cnt = si < n_src ? srcs[si].counts[0] * items_per_block(srcs[si]) : 0;
+            const int cnt = si < n_src ? win_blocks(srcs[si]) * items_per_block(srcs[si]) : 0;
             int incl = cnt;
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
@@ -147,6 +219,8 @@ k_rir_direct(const Source* __restrict__ srcs, int per_src) {
     const Source& S = srcs[blockIdx.x / per_src];
     const int row = (blockIdx.x % per_src) * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (!S.cut || row >= S.P * S.C) return;
+    // windowed source: only the (p, c) rows its transformed RIR rows come from (the others may not even be in memory)
+    if (S.h_rows && (row < S.h_row0 / S.K || row > (S.h_row0 + S.h_rows - 1) / S.K)) return;
     const float div = S.norm_part ? rir_absmax(S) : 0.f;
     PeakAt m = peak_scan(S.rir + (size_t)row * S.L, S.L, div, lane, 32);
 #pragma unroll
@@ -196,12 +270,14 @@ k_prepare(const Source* __restrict__ srcs_g, const int* __restrict__ prefix_g, i
         const int blk = (local - nh - nx) * 8 + (t >> 5), lane = t & 31;
         if (blk >= S.counts[0]) return;
         Block bk = S.blocks[blk];
+        if (S.mode == MODE_MOVING_BOUNDS && !S.aligned && blk == 0 && lane == 0) {
+            // one warp per source checks the device-side bounds table
+            bool bad = S.bounds[0] != 0 || S.bounds[S.P - 1] != S.N;
+            for (int q = 0; q + 1 < S.P && !bad; ++q) bad = S.bounds[q + 1] < S.bounds[q];
+            if (bad) atomicOr(&g_dev_err, 2u);
+        }
+        if ((unsigned)(blk - win_first(S)) >= (unsigned)win_blocks(S)) return;     // windowed: block outside the window
         if (S.mode == MODE_MOVING_BOUNDS && !S.aligned) {
-            if (blk == 0 && lane == 0) {                   // one warp per source checks the device-side bounds table
-                bool bad = S.bounds[0] != 0 || S.bounds[S.P - 1] != S.N;
-                for (int q = 0; q + 1 < S.P && !bad; ++q) bad = S.bounds[q + 1] < S.bounds[q];
-                if (bad) atomicOr(&g_dev_err, 2u);
-            }
             bk.p_lo = seg_of(S.bounds, S.P - 1, bk.start);
             bk.p_hi = seg_of(S.bounds, S.P - 1, bk.start + bk.len - 1) + 1;
         } else if (S.mode == MODE_MOVING_INDEXED) {
@@ -540,7 +616,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 101; }
+extern "C" int ss_version(void) { return 102; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -732,7 +808,17 @@ static int validate_item(const ss_source& it) {
     else if (it.mode == SS_MOVING_BOUNDS) { if (it.P < 2 || !it.bounds) return SS_ERR_INVALID; }
     else if (it.mode == SS_MOVING_INDEXED) { if (it.P < 2 || !it.idx || !it.w) return SS_ERR_INVALID; }
     else return SS_ERR_INVALID;
+    if (it.win_len < 0 || it.win_start < 0 || (it.win_len == 0 && it.win_start != 0) ||
+        (int64_t)it.win_start + it.win_len > (int64_t)it.N)
+        return SS_ERR_INVALID;
     return SS_OK;
+}
+// A trajectory bounds table as the header requires it: ascending from 0 to N.  Checked before anything plans blocks from
+// it - a table outside the contract would make the host-side block planner write past the table it sized.
+static bool bounds_ok(const int32_t* b, int P, int N) {
+    if (b[0] != 0 || b[P - 1] != N) return false;
+    for (int q = 0; q + 1 < P; ++q) if (b[q + 1] < b[q]) return false;
+    return true;
 }
 // SS_DIRECT_TARGET: a second RIR set (spectra, items per block) and the P*C cut table
 static int direct_sets(const ss_source& it) { return (it.flags & SS_DIRECT_TARGET) ? 2 : 1; }
@@ -740,7 +826,17 @@ static size_t cut_bytes(const ss_source& it) {
     return (it.flags & SS_DIRECT_TARGET) ? align_up(sizeof(int) * (size_t)it.P * it.C, 256) : 0;
 }
 // shapes derived from one ss_source
-struct Shape { int K, nb, aligned, nblk_max, per, max_items; };
+struct Shape {
+    int K, nb, aligned, nblk_max, per, max_items;
+    // time window (win_len > 0); zero otherwise
+    int win;
+    int tab_host;             // the window's blocks are known here (all but aligned blocking over device-side bounds)
+    int g0, g1, k0, k1;       // tab_host: full-table blocks in the table / meeting the window (window_span)
+    int row0, rows;           // RIR rows transformed per set (window_rows)
+    int pa, pb;               // RIR positions read: [pa, pb]
+    int xa, xb;               // dry samples read: [xa, xb)
+    int ia, ib;               // idx / w entries read: [ia, ib)
+};
 // Aligned blocking costs one transform per block, sum_s ceil(n_s / 4096); grid blocking costs
 // ceil(positions touched / 2) per 4096-block.  With the bounds on the host both counts are exact and the
 // cheaper plan wins (trajectories with many short segments are better off on the grid); without them the
@@ -761,41 +857,96 @@ static bool choose_aligned(const ss_source& it, int K, int nb) {
     }
     return aligned <= grid;
 }
+// The full plan's blocks in use (aligned: from the host-side bounds `hb`), ascending; returns their number.  Writes at
+// most `cap` blocks (nb + P - 1 for a bounds table ascending from 0 to N; a table outside that contract stops there).
+static int full_blocks(const ss_source& it, int aligned, int nb, const int32_t* hb, Block* blocks, int cap) {
+    int nblk = 0;
+    if (aligned) {
+        for (int sg = 0; sg < it.P - 1; ++sg) {
+            const int b0 = hb[sg], n_s = hb[sg + 1] - b0;
+            for (int q = 0; q < seg_blocks(n_s) && nblk < cap; ++q) {
+                Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
+                blocks[nblk++] = bk;
+            }
+        }
+    } else {
+        nblk = nb;
+        for (int bi = 0; bi < nblk; ++bi) {
+            Block bk; bk.start = bi * kB; bk.len = it.N - bi * kB < kB ? it.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
+            blocks[bi] = bk;
+        }
+    }
+    return nblk;
+}
+// Window of a windowed source: which blocks, RIR rows, dry samples and trajectory entries it uses (its read set, see
+// include/sonicsim_b200.h).  The blocking itself is the full source's (choose_aligned over the whole trajectory).
+static void window_shape(const ss_source& it, Shape& s) {
+    const int ws = it.win_start, we = it.win_start + it.win_len;
+    const int32_t* hb = it.mode == SS_MOVING_BOUNDS ? it.bounds_host : nullptr;
+    s.win = 1;
+    s.tab_host = !s.aligned || hb != nullptr;
+    int pa = 0, pb = it.P - 1;                           // all positions unless the trajectory is visible here
+    if (s.tab_host) {
+        std::vector<Block> full((size_t)s.nblk_max);
+        const int n = full_blocks(it, s.aligned, s.nb, hb, full.data(), s.nblk_max);
+        const WinSpan w = window_blocks(full.data(), n, ws, we, s.K);
+        if (w.k0 < w.k1) {
+            s.g0 = w.g0; s.g1 = w.g1; s.k0 = w.k0; s.k1 = w.k1;
+            s.nblk_max = w.g1 - w.g0;
+            s.xa = std::max(0, full[w.g0].start - kB); s.xb = std::min(it.N, full[w.g1 - 1].start + kB);
+            s.ia = full[w.k0].start; s.ib = full[w.k1 - 1].start + full[w.k1 - 1].len;
+            if (s.aligned) { pa = full[w.k0].p_lo; pb = full[w.k1 - 1].p_hi; }
+            else if (hb) { pa = seg_of(hb, it.P - 1, s.ia); pb = seg_of(hb, it.P - 1, s.ib - 1) + 1; }
+        } else {
+            // no block meets the window: only a bounds_host outside the contract (ascending from 0 to N) gets here,
+            // which the render paths refuse before they plan; size it as if the blocks were found on the device
+            s.tab_host = 0;
+        }
+    }
+    if (!s.tab_host) {
+        // k_blocks finds the blocks on the device: a window meets at most ceil(o / 4096) + 1 blocks of each segment it
+        // overlaps by o samples, plus one block in front (even start) and the last one's partner
+        const int64_t bound = (int64_t)(it.win_len + kB - 1) / kB + 2 * (int64_t)(it.P - 1) + 2;
+        if (bound < s.nblk_max) s.nblk_max = (int)bound;
+        s.xa = 0; s.xb = it.N; s.ia = 0; s.ib = it.N;
+    }
+    if (it.mode == SS_STATIC) { pa = 0; pb = 0; }
+    window_rows(it.P, it.C, s.K, pa, pb, s.row0, s.rows);
+    if (it.flags & SS_RIR_NORMALIZE) { s.pa = 0; s.pb = it.P - 1; }         // the global abs-max reads every tap
+    else { s.pa = s.row0 / (it.C * s.K); s.pb = (s.row0 + s.rows - 1) / (it.C * s.K); }
+}
 static Shape shape_of(const ss_source& it) {
     Shape s;
+    memset(&s, 0, sizeof(s));
     s.K = (it.L + kB - 1) / kB; s.nb = (it.N + kB - 1) / kB;
     s.aligned = choose_aligned(it, s.K, s.nb) ? 1 : 0;
     s.nblk_max = s.aligned ? s.nb + it.P - 1 : s.nb;
     s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
+    if (it.win_len > 0) window_shape(it, s);
     s.max_items = s.nblk_max * s.per;
     return s;
 }
+// RIR rows transformed per set
+static size_t rir_rows(const ss_source& it, const Shape& sh) { return sh.win ? (size_t)sh.rows : (size_t)it.P * it.C * sh.K; }
 static size_t spectra_bytes(const ss_source& it) {
     const Shape sh = shape_of(it);
-    return ((size_t)it.P * it.C * sh.K * direct_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
+    return (rir_rows(it, sh) * direct_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
            (size_t)sh.max_items * sizeof(RItem) +
            align_up(sizeof(Block) * (size_t)sh.nblk_max, 256) + align_up(sizeof(double) * (size_t)it.P, 256) + 256 +
            ((it.flags & SS_RIR_NORMALIZE) ? 512 : 0) + cut_bytes(it);
 }
 
 // Host-side twin of k_blocks for one source whose trajectory bounds are visible on the host.
-// Returns the number of blocks in use.
+// Returns the number of blocks in use (windowed source: the full table's blocks [g0, g1)).
 static int build_blocks_host(const ss_source& it, const Shape& sh, const int32_t* hb, Block* blocks, double* rstep) {
     int nblk = 0;
-    if (sh.aligned) {
-        for (int sg = 0; sg < it.P - 1; ++sg) {
-            const int b0 = hb[sg], n_s = hb[sg + 1] - b0;
-            for (int q = 0; q < seg_blocks(n_s); ++q) {
-                Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
-                blocks[nblk++] = bk;
-            }
-        }
+    if (sh.win) {
+        std::vector<Block> full((size_t)(sh.aligned ? sh.nb + it.P - 1 : sh.nb));
+        full_blocks(it, sh.aligned, sh.nb, hb, full.data(), (int)full.size());
+        nblk = sh.g1 - sh.g0;
+        for (int bi = 0; bi < nblk; ++bi) blocks[bi] = full[sh.g0 + bi];
     } else {
-        nblk = sh.nb;
-        for (int bi = 0; bi < nblk; ++bi) {
-            Block bk; bk.start = bi * kB; bk.len = it.N - bi * kB < kB ? it.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
-            blocks[bi] = bk;
-        }
+        nblk = full_blocks(it, sh.aligned, sh.nb, hb, blocks, sh.nblk_max);
     }
     for (int bi = nblk; bi < sh.nblk_max; ++bi) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; blocks[bi] = z; }
     if (it.mode == SS_MOVING_BOUNDS && hb)
@@ -805,19 +956,28 @@ static int build_blocks_host(const ss_source& it, const Shape& sh, const int32_t
 
 // Test hook (pure host, no CUDA call): the blocking plan the library would use for `item` - the choice between
 // waypoint-aligned and 4096-grid blocking and the block table of the host-built path.  blocks_out receives
-// (start, len, p_lo, p_hi) per block in use; returns their number or a negative ss_status.
+// (start, len, p_lo, p_hi) per block in use; returns their number or a negative ss_status.  Windowed item: the
+// entries of the full table that meet the window.
 extern "C" int ss_debug_plan(const ss_source* item, int32_t* blocks_out, int32_t max_blocks, int32_t* aligned_out) {
     if (!item || !blocks_out || max_blocks < 0) return SS_ERR_INVALID;
     if (item->N <= 0 || item->C <= 0 || item->L <= 0 || item->P <= 0) return SS_ERR_INVALID;
     if (item->mode == SS_MOVING_BOUNDS && (!item->bounds_host || item->P < 2)) return SS_ERR_INVALID;
+    if (item->mode == SS_MOVING_BOUNDS && !bounds_ok(item->bounds_host, item->P, item->N)) return SS_ERR_INVALID;
+    if (item->win_len < 0 || item->win_start < 0 || (item->win_len == 0 && item->win_start != 0) ||
+        (int64_t)item->win_start + item->win_len > (int64_t)item->N)
+        return SS_ERR_INVALID;
     const Shape sh = shape_of(*item);
-    if (sh.nblk_max > max_blocks) return SS_ERR_NOMEM;
+    const int first = sh.win ? sh.k0 - sh.g0 : 0;
+    const int nout = sh.win ? sh.k1 - sh.k0 : -1;
+    if ((sh.win ? nout : sh.nblk_max) > max_blocks) return SS_ERR_NOMEM;
     std::vector<Block> blocks((size_t)sh.nblk_max);
     std::vector<double> rstep((size_t)item->P);
-    const int nblk = build_blocks_host(*item, sh, item->bounds_host, blocks.data(), rstep.data());
+    const int n_tab = build_blocks_host(*item, sh, item->bounds_host, blocks.data(), rstep.data());
+    const int nblk = sh.win ? nout : n_tab;
     for (int i = 0; i < nblk; ++i) {
-        blocks_out[4 * i] = blocks[i].start; blocks_out[4 * i + 1] = blocks[i].len;
-        blocks_out[4 * i + 2] = blocks[i].p_lo; blocks_out[4 * i + 3] = blocks[i].p_hi;
+        const Block& b = blocks[first + i];
+        blocks_out[4 * i] = b.start; blocks_out[4 * i + 1] = b.len;
+        blocks_out[4 * i + 2] = b.p_lo; blocks_out[4 * i + 3] = b.p_hi;
     }
     if (aligned_out) *aligned_out = sh.aligned;
     return nblk;
@@ -843,15 +1003,23 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
         if (items[i].mode == SS_MOVING_BOUNDS && !items[i].bounds_host) return false;
     return true;
 }
-// descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts
+// counts of a source (Source::counts): [0, 1] and, windowed, [2, 5] - which the host fills even when k_blocks builds the
+// block table, so that they always travel in the descriptor block
+static size_t counts_bytes(const Shape& sh) { return sh.win ? 32 : 16; }
+// descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
+// counts (windowed source, device-built tables)
 static size_t chunk_desc_bytes(const ss_source* items, int first, int last) {
     const int n = last - first;
     size_t bytes = align_up(sizeof(Source) * n, 16) + align_up(sizeof(int) * (n + 1), 16) + 16;
-    if (chunk_host_tables(items, first, last))
-        for (int i = first; i < last; ++i) {
-            const Shape sh = shape_of(items[i]);
-            bytes += align_up(sizeof(Block) * (size_t)sh.nblk_max, 16) + align_up(sizeof(double) * (size_t)items[i].P, 16) + 16;
-        }
+    const bool host_tables = chunk_host_tables(items, first, last);
+    for (int i = first; i < last; ++i) {
+        const Shape sh = shape_of(items[i]);
+        if (host_tables)
+            bytes += align_up(sizeof(Block) * (size_t)sh.nblk_max, 16) + align_up(sizeof(double) * (size_t)items[i].P, 16) +
+                     counts_bytes(sh);
+        else if (sh.win)
+            bytes += counts_bytes(sh);
+    }
     return bytes;
 }
 // Fill the descriptor block of items[first, last) at `hbase` (host memory) for its device address `dbase`, carve the
@@ -879,7 +1047,8 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
         s.w = it.mode == SS_MOVING_INDEXED ? it.w : nullptr;
         s.N = it.N; s.P = it.P; s.C = it.C; s.L = it.L;
         s.K = sh.K; s.nb = sh.nb; s.mode = it.mode; s.aligned = sh.aligned; s.nblk_max = sh.nblk_max;
-        s.hspec = (float2*)scratch; scratch += (size_t)s.P * s.C * s.K * direct_sets(it) * kSpec * sizeof(float2);
+        s.hspec = (float2*)scratch; scratch += rir_rows(it, sh) * direct_sets(it) * kSpec * sizeof(float2);
+        if (sh.win) { s.h_row0 = sh.row0; s.h_rows = sh.rows; }
         s.xspec = (float2*)scratch; scratch += (size_t)s.nblk_max * kSpec * sizeof(float2);
         if (it.flags & SS_RIR_NORMALIZE) { s.norm_part = (const float*)scratch; scratch += 512; any_norm = true; }
         if (it.flags & SS_DIRECT_TARGET) {
@@ -894,14 +1063,26 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
             double* hb_rstep = (double*)(hbase + tab_off);
             s.rstep = (double*)(dbase + tab_off); tab_off += align_up(sizeof(double) * (size_t)s.P, 16);
             int* hb_counts = (int*)(hbase + tab_off);
-            s.counts = (int*)(dbase + tab_off); tab_off += 16;
+            s.counts = (int*)(dbase + tab_off); tab_off += counts_bytes(sh);
             const int nblk = build_blocks_host(it, sh, it.bounds_host, hb_blocks, hb_rstep);
             hb_counts[0] = nblk; hb_counts[1] = total_items; hb_counts[2] = 0; hb_counts[3] = 0;
-            total_items += nblk * sh.per;
+            if (sh.win) {
+                hb_counts[2] = sh.k0 - sh.g0; hb_counts[3] = sh.k1 - sh.k0;
+                hb_counts[4] = it.win_start; hb_counts[5] = it.win_len; hb_counts[6] = 0; hb_counts[7] = 0;
+            }
+            total_items += (sh.win ? sh.k1 - sh.k0 : nblk) * sh.per;
         } else {
             s.blocks = (Block*)scratch; scratch += align_up(sizeof(Block) * (size_t)s.nblk_max, 256);
             s.rstep = (double*)scratch; scratch += align_up(sizeof(double) * (size_t)s.P, 256);
-            s.counts = (int*)scratch; scratch += 256;
+            if (sh.win) {                               // k_blocks reads the window from the counts and fills [0, 3]
+                int* hb_counts = (int*)(hbase + tab_off);
+                s.counts = (int*)(dbase + tab_off); tab_off += counts_bytes(sh);
+                memset(hb_counts, 0, counts_bytes(sh));
+                hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
+            } else {
+                s.counts = (int*)scratch;
+            }
+            scratch += 256;
         }
         hs[i] = s;
         hps[i] = ps;
@@ -1063,11 +1244,9 @@ extern "C" int ss_debug_chunks(const int64_t* bytes, int32_t n, int64_t budget, 
 static int validate_dev_items(const ss_source* items, int n_items) {
     for (int i = 0; i < n_items; ++i) {
         int st = validate_item(items[i]); if (st) return st;
-        if (items[i].mode == SS_MOVING_BOUNDS && items[i].bounds_host) {
-            const int32_t* b = items[i].bounds_host;
-            if (b[0] != 0 || b[items[i].P - 1] != items[i].N) return SS_ERR_INVALID;
-            for (int q = 0; q + 1 < items[i].P; ++q) if (b[q + 1] < b[q]) return SS_ERR_INVALID;
-        }
+        if (items[i].mode == SS_MOVING_BOUNDS && items[i].bounds_host &&
+            !bounds_ok(items[i].bounds_host, items[i].P, items[i].N))
+            return SS_ERR_INVALID;
     }
     return SS_OK;
 }
@@ -1256,14 +1435,23 @@ extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
 extern "C" int ss_plan_is_graph(const ss_plan* p) { return p ? (p->exec ? 1 : 0) : SS_ERR_INVALID; }
 
 // ----------------------------------------------------------------------------- host path
-static int check_traj_host(const ss_source& it) {
-    if (it.mode == SS_MOVING_BOUNDS) {
-        const int32_t* b = it.bounds;
-        if (b[0] != 0 || b[it.P - 1] != it.N) return SS_ERR_INVALID;
-        for (int i = 0; i + 1 < it.P; ++i) if (b[i + 1] < b[i]) return SS_ERR_INVALID;
-    } else if (it.mode == SS_MOVING_INDEXED) {
-        for (int n = 0; n < it.N; ++n) { int v = it.idx[n]; if (v < 0 || v + 1 >= it.P) return SS_ERR_INDEX; }
+// What the host path copies in and out for one source: dry samples [xa, xb), RIR positions [pa, pb], idx / w entries
+// [ia, ib), and C * wl output floats per stem - the whole source, or a windowed source's read set (window_shape)
+struct ReadSet { int xa, xb, pa, pb, ia, ib, wl; };
+static ReadSet read_set(const ss_source& it) {
+    ReadSet r = {0, it.N, 0, it.P - 1, 0, it.N, it.N};
+    if (it.win_len > 0) {
+        ss_source h = it;
+        if (h.mode == SS_MOVING_BOUNDS) h.bounds_host = h.bounds;          // host pointers: the trajectory is visible
+        const Shape sh = shape_of(h);
+        r.xa = sh.xa; r.xb = sh.xb; r.pa = sh.pa; r.pb = sh.pb; r.ia = sh.ia; r.ib = sh.ib; r.wl = it.win_len;
     }
+    return r;
+}
+// idx (SS_MOVING_INDEXED): the entries the render reads (the bounds table is checked whole, before read_set plans from it)
+static int check_idx_host(const ss_source& it, const ReadSet& rs) {
+    if (it.mode == SS_MOVING_INDEXED)
+        for (int n = rs.ia; n < rs.ib; ++n) { int v = it.idx[n]; if (v < 0 || v + 1 >= it.P) return SS_ERR_INDEX; }
     return SS_OK;
 }
 
@@ -1289,9 +1477,14 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     // every stem with a target shares one sample rate (ss_loudness_dev runs one set of filter coefficients per call);
     // checked against the first source that has a target, so that the answer does not depend on the chunking
     const ss_post_lufs* first_post = nullptr;
+    std::vector<ReadSet> rset(n_items);
     for (int i = 0; i < n_items; ++i) {
         int st = validate_item(items[i]); if (st) return st;
-        st = check_traj_host(items[i]); if (st) return st;
+        // a window cannot be loudness-normalised: the reference measures the whole stem
+        if (post && post[i].brk && items[i].win_len > 0) return SS_ERR_INVALID;
+        if (items[i].mode == SS_MOVING_BOUNDS && !bounds_ok(items[i].bounds, items[i].P, items[i].N)) return SS_ERR_INVALID;
+        rset[i] = read_set(items[i]);
+        st = check_idx_host(items[i], rset[i]); if (st) return st;
         if (post && post[i].brk) {
             if (!post[i].blk_lo || !post[i].blk_hi || post[i].n_e <= 0 || post[i].rate <= 0 || items[i].C > 8) return SS_ERR_INVALID;
             if (!first_post) first_post = &post[i];
@@ -1365,10 +1558,12 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         size_t in_b = 0, out_b = 0;
         for (int i = first; i < last; ++i) {
             const ss_source& it = items[i];
-            in_b += align_up(sizeof(float) * (size_t)it.N, 256) + align_up(sizeof(float) * (size_t)it.P * it.C * it.L, 256);
+            const ReadSet& rs = rset[i];
+            in_b += align_up(sizeof(float) * (size_t)(rs.xb - rs.xa), 256) +
+                    align_up(sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L, 256);
             if (it.mode == SS_MOVING_BOUNDS) in_b += align_up(sizeof(int32_t) * (size_t)it.P, 256);
-            if (it.mode == SS_MOVING_INDEXED) in_b += 2 * align_up(4 * (size_t)it.N, 256);
-            out_b += align_up(sizeof(float) * (size_t)it.C * it.N, 256) * direct_sets(it);
+            if (it.mode == SS_MOVING_INDEXED) in_b += 2 * align_up(4 * (size_t)(rs.ib - rs.ia), 256);
+            out_b += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256) * direct_sets(it);
             if (post && post[i].brk)
                 out_b += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * it.C * post[i].n_e, 256) + 256;
         }
@@ -1380,23 +1575,26 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         direct_gain.clear();
         for (int i = first; i < last; ++i) {
             const ss_source& it = items[i];
+            const ReadSet& rs = rset[i];
             ss_source d = it;
             size_t nb;
-            nb = sizeof(float) * (size_t)it.N;
-            CK(cudaMemcpyAsync(pi, it.x, nb, cudaMemcpyHostToDevice, c->s_in)); d.x = (const float*)pi; pi += align_up(nb, 256);
-            nb = sizeof(float) * (size_t)it.P * it.C * it.L;
-            CK(cudaMemcpyAsync(pi, it.rir, nb, cudaMemcpyHostToDevice, c->s_in)); d.rir = (const float*)pi; pi += align_up(nb, 256);
+            // only the read set is copied; the device pointers are offset so that the kernels index the full arrays
+            nb = sizeof(float) * (size_t)(rs.xb - rs.xa);
+            CK(cudaMemcpyAsync(pi, it.x + rs.xa, nb, cudaMemcpyHostToDevice, c->s_in)); d.x = (const float*)pi - rs.xa; pi += align_up(nb, 256);
+            const size_t pos0 = (size_t)rs.pa * it.C * it.L;
+            nb = sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L;
+            CK(cudaMemcpyAsync(pi, it.rir + pos0, nb, cudaMemcpyHostToDevice, c->s_in)); d.rir = (const float*)pi - pos0; pi += align_up(nb, 256);
             if (it.mode == SS_MOVING_BOUNDS) {
                 nb = sizeof(int32_t) * (size_t)it.P;
                 CK(cudaMemcpyAsync(pi, it.bounds, nb, cudaMemcpyHostToDevice, c->s_in)); d.bounds = (const int32_t*)pi; pi += align_up(nb, 256);
                 d.bounds_host = it.bounds;
             } else if (it.mode == SS_MOVING_INDEXED) {
-                nb = 4 * (size_t)it.N;
-                CK(cudaMemcpyAsync(pi, it.idx, nb, cudaMemcpyHostToDevice, c->s_in)); d.idx = (const int32_t*)pi; pi += align_up(nb, 256);
-                CK(cudaMemcpyAsync(pi, it.w, nb, cudaMemcpyHostToDevice, c->s_in)); d.w = (const float*)pi; pi += align_up(nb, 256);
+                nb = 4 * (size_t)(rs.ib - rs.ia);
+                CK(cudaMemcpyAsync(pi, it.idx + rs.ia, nb, cudaMemcpyHostToDevice, c->s_in)); d.idx = (const int32_t*)pi - rs.ia; pi += align_up(nb, 256);
+                CK(cudaMemcpyAsync(pi, it.w + rs.ia, nb, cudaMemcpyHostToDevice, c->s_in)); d.w = (const float*)pi - rs.ia; pi += align_up(nb, 256);
             }
-            d.out = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * it.N, 256);
-            if (it.flags & SS_DIRECT_TARGET) { d.out_direct = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * it.N, 256); }
+            d.out = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256);
+            if (it.flags & SS_DIRECT_TARGET) { d.out_direct = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256); }
             dev[i] = d;
             if (post && post[i].brk) {
                 const ss_post_lufs& pl = post[i];
@@ -1431,11 +1629,10 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         }
         CK(cudaStreamWaitEvent(c->s_out, sl.ev_done, 0));
         for (int i = first; i < last; ++i) {
-            CK(cudaMemcpyAsync(items[i].out, dev[i].out, sizeof(float) * (size_t)items[i].C * items[i].N,
-                               cudaMemcpyDeviceToHost, c->s_out));
+            const size_t ob = sizeof(float) * (size_t)items[i].C * rset[i].wl;
+            CK(cudaMemcpyAsync(items[i].out, dev[i].out, ob, cudaMemcpyDeviceToHost, c->s_out));
             if (items[i].flags & SS_DIRECT_TARGET)
-                CK(cudaMemcpyAsync(items[i].out_direct, dev[i].out_direct, sizeof(float) * (size_t)items[i].C * items[i].N,
-                                   cudaMemcpyDeviceToHost, c->s_out));
+                CK(cudaMemcpyAsync(items[i].out_direct, dev[i].out_direct, ob, cudaMemcpyDeviceToHost, c->s_out));
             if (res_dev[i])
                 CK(cudaMemcpyAsync(h_res + 2 * i, res_dev[i], 2 * sizeof(double), cudaMemcpyDeviceToHost, c->s_out));
         }

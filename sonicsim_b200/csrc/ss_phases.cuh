@@ -23,6 +23,11 @@ struct RItem;
 
 // One (utterance, source) unit.  Reference shapes: dry (N,), RIRs (P, C, L), output (C, N)
 // (SonicSim_moving.py:63-96); static source has P = 1 (SonicSim_moving.py:47-61).
+// Biased pointers: the kernels index x, rir, idx and w as the full arrays (sample n at x[n], position p at
+// rir + p * C * L), but for a windowed source the host path copies only its read set, so these four may point in
+// front of their allocation (device buffer - first index copied), and RItem::row / row1 point win_start samples in
+// front of the (C, win_len) output.  Only indices inside the read set / the window are ever dereferenced; code that
+// reads any other element of these arrays must first be added to the read set (include/sonicsim_b200.h).
 struct Source {
     const float* x;        // dry waveform, N samples
     const float* rir;      // (P, C, L) row-major
@@ -35,7 +40,9 @@ struct Source {
     float2* xspec;         // scratch: nblk_max half spectra of the dry windows
     Block* blocks;         // scratch: nblk_max blocks (k_blocks)
     double* rstep;         // scratch: 1 / (samples in segment s), s < P - 1 (mode 1)
-    int* counts;           // scratch: [0] = blocks in use, [1] = index of this source's first render item
+    int* counts;           // scratch: [0] = blocks in use, [1] = index of this source's first render item; windowed
+                           // source (h_rows != 0): [2] = first block that meets the window, [3] = blocks that do,
+                           // [4] = win_start, [5] = win_len
     const float* norm_part;// scratch: kNormParts partial abs-maxima of the RIR tensor (k_rir_absmax), or null: taps used as given
     int* cut;              // scratch: P*C direct-path row lengths (k_rir_direct), or null: no direct target
     float* out_direct;     // (C, N) direct-path stem (with `cut`)
@@ -46,6 +53,11 @@ struct Source {
     int aligned;           // 1: blocks aligned to the trajectory segments (mode 1 and K == 1)
     int nblk_max;          // table size: nb (grid) or nb + P - 1 (aligned)
     int direct_taps;       // taps kept from each row's peak on (with `cut`)
+    // Time window (0, 0: the whole stem).  A windowed source transforms only the RIR rows [h_row0, h_row0 + h_rows) of
+    // each set (h_row0 even: rows pair as in the full row list), stored from hspec on, and only a contiguous range of
+    // the full plan's blocks (k_blocks / the host: first block even, see window_span); out / out_direct are
+    // (C, win_len).  h_rows != 0 marks a windowed source.
+    int h_row0, h_rows;
 };
 constexpr int kNormParts = 128;    // CTAs (partial maxima) per normalised source in k_rir_absmax
 
@@ -67,7 +79,9 @@ struct RItem {
     int kparts;            // RIR partitions that reach back into the signal: min(K, n0 / 4096 + 1)
     int b0;                // aligned blocking: first sample of the block's segment, bounds[p_lo] ...
     double step;           // ... and 1 / (samples in that segment), so that k_render_fast's output stage loads no table
-    int pad_[2];
+    int n_lo;              // samples [n_lo, n_end) are stored (n_lo > n0: a window starts inside the block); the
+                           // epilogues tie register r to sample n0 + t + 256 r, so n0 stays the block start
+    int pad_;
 };
 static_assert(sizeof(RItem) == 112, "RItem is copied as 7 x 16 B");
 
@@ -87,14 +101,15 @@ struct XDesc {
     int valid;
     int mode;
     int kparts;
-    int pad_;
+    int n_lo;              // as RItem::n_lo
 };
 static_assert(sizeof(XDesc) == 112, "XDesc layout");
 
 // RIR rows are transformed two per complex FFT, and the bits of a half spectrum depend on its partner row: the direct
 // rows are paired among themselves exactly as a separate source's rows would be, never with a reverberant row.
 SS_HD int rows_h(const Source& s) { return s.P * s.C * s.K; }                 // per set (reverberant, direct)
-SS_HD int pairs_per_set_h(const Source& s) { return (rows_h(s) + 1) >> 1; }
+SS_HD int rows_stored_h(const Source& s) { return s.h_rows ? s.h_rows : rows_h(s); }     // transformed rows per set
+SS_HD int pairs_per_set_h(const Source& s) { return (rows_stored_h(s) + 1) >> 1; }
 SS_HD int spectra_pairs_h(const Source& s) { return pairs_per_set_h(s) * (s.cut ? 2 : 1); }
 SS_HD int spectra_pairs_x(const Source& s) { return (s.nblk_max + 1) >> 1; }
 SS_HD int range_ctas(const Source& s) { return (s.nblk_max + 7) >> 3; }       // k_prepare: one warp per block
@@ -105,35 +120,79 @@ SS_HD int max_render_items(const Source& s) { return s.nblk_max * items_per_bloc
 // blocks of one segment under aligned blocking
 SS_HD int seg_blocks(int n_s) { return (n_s + kB - 1) / kB; }
 
+// ---- time windows.  A windowed source keeps the full plan's blocking (aligned or grid, chosen over the whole
+// trajectory) and renders the blocks [k0, k1) of the full table that meet the window.  Its table holds the full
+// table's blocks [g0, g1): the K - 1 blocks in front of k0 too (their dry windows feed RIR partitions 1 .. K - 1), g0
+// even and g1 past the last kept block's partner, because two dry windows share one forward FFT - blocks 2i and 2i + 1
+// of the full table - and the bits of each half spectrum depend on its partner.
+struct WinSpan { int g0, g1, k0, k1; };
+SS_HD WinSpan window_span(int k0, int k1, int nblk, int K) {
+    WinSpan r; r.k0 = k0; r.k1 = k1;
+    const int a = k0 - (K - 1);
+    r.g0 = (a > 0 ? a : 0) & ~1;
+    r.g1 = (k1 + 1) & ~1;
+    if (r.g1 > nblk) r.g1 = nblk;
+    return r;
+}
+// the same from the full table itself (ascending starts, no empty block): the blocks meeting output samples [ws, we)
+SS_HD WinSpan window_blocks(const Block* b, int nblk, int ws, int we, int K) {
+    int lo = 0, hi = nblk;                               // first block that ends after ws
+    while (lo < hi) { const int m = (lo + hi) >> 1; if (b[m].start + b[m].len <= ws) lo = m + 1; else hi = m; }
+    const int k0 = lo;
+    hi = nblk;                                           // first block that starts at or after we
+    while (lo < hi) { const int m = (lo + hi) >> 1; if (b[m].start < we) lo = m + 1; else hi = m; }
+    return window_span(k0, lo, nblk, K);
+}
+// first RIR row and row count of a windowed source whose kept blocks interpolate between positions [pa, pb]: whole
+// positions, started on an even row and ended past the last row's partner (rows 2r, 2r + 1 share one forward FFT)
+SS_HD void window_rows(int P, int C, int K, int pa, int pb, int& row0, int& rows) {
+    const int ck = C * K;
+    const int r0 = (pa * ck) & ~1;
+    int r1 = ((pb + 1) * ck + 1) & ~1;
+    if (r1 > P * ck) r1 = P * ck;
+    row0 = r0; rows = r1 - r0;
+}
+// blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
+SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
+SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }
+
 // fill the work items of block `blk` once its position range is known (lanes split the channels).  A direct-target
 // source's block has the reverberant items first, then as many direct items (direct spectra, `out_direct`): all of
-// them carry the block's X, so k_render_fast stages it once for both stems.
+// them carry the block's X, so k_render_fast stages it once for both stems.  Windowed source: only blocks that meet
+// the window have items; output rows have stride win_len and sample n of the stem lands at row[n - win_start].
 SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, int lane, int nlanes) {
     RItem it;
     it.X = s.xspec + (size_t)blk * kSpec;
     it.bounds = s.bounds; it.rstep = s.rstep; it.idx = s.idx; it.w = s.w;
     it.n0 = bk.start; it.n_end = bk.start + bk.len;
+    it.n_lo = bk.start;
+    const int ws = s.h_rows ? s.counts[4] : 0, wl = s.h_rows ? s.counts[5] : s.N;
+    if (s.h_rows) {
+        if (it.n_lo < ws) it.n_lo = ws;
+        if (it.n_end > ws + wl) it.n_end = ws + wl;
+    }
     it.mode = s.mode;
     const int reach = bk.start / kB + 1;
     it.kparts = reach < s.K ? reach : s.K;
-    it.b0 = 0; it.step = 0.0; it.pad_[0] = 0; it.pad_[1] = 0;
+    it.b0 = 0; it.step = 0.0; it.pad_ = 0;
     if (s.aligned) { it.b0 = s.bounds[bk.p_lo]; it.step = s.rstep[bk.p_lo]; }
     const int per = items_per_set(s);
-    RItem* dst = items + s.counts[1] + (size_t)blk * items_per_block(s);
+    RItem* dst = items + s.counts[1] + (size_t)(blk - win_first(s)) * items_per_block(s);
     for (int i = lane; i < items_per_block(s); i += nlanes) {
         const bool direct = i >= per;
         const int c = direct ? i - per : i;
-        const float2* const spec = s.hspec + (direct ? (size_t)rows_h(s) * kSpec : 0);
-        float* const out = direct ? s.out_direct : s.out;
+        // row r of the set at spec + (r - h_row0) * kSpec
+        const float2* const spec = s.hspec + (direct ? (size_t)rows_stored_h(s) * kSpec : 0) - (ptrdiff_t)s.h_row0 * kSpec;
+        float* const out = (direct ? s.out_direct : s.out) - ws;
         if (s.mode == MODE_STATIC) {                 // item c: channels 2c, 2c + 1
             it.H0 = spec + (size_t)(2 * c) * s.K * kSpec;
-            it.row = out + (size_t)(2 * c) * s.N;
-            it.row1 = (2 * c + 1 < s.C) ? it.row + s.N : nullptr;
+            it.row = out + (size_t)(2 * c) * wl;
+            it.row1 = (2 * c + 1 < s.C) ? it.row + wl : nullptr;
             it.pstride = s.K * kSpec;
             it.p_lo = 0; it.p_hi = 0;
         } else {
             it.H0 = spec + (size_t)c * s.K * kSpec;
-            it.row = out + (size_t)c * s.N;
+            it.row = out + (size_t)c * wl;
             it.row1 = nullptr;
             it.pstride = s.C * s.K * kSpec;
             it.p_lo = bk.p_lo; it.p_hi = bk.p_hi;
@@ -160,7 +219,7 @@ SS_HD XDesc make_xdesc(const RItem& it, int p) {
     d.Hq = has_q ? d.Hp + it.pstride : nullptr;
     d.row = it.row; d.row1 = it.row1;
     d.bounds = it.bounds; d.rstep = it.rstep; d.idx = it.idx; d.w = it.w;
-    d.n0 = it.n0; d.n_end = it.n_end; d.p = p; d.p_lo = it.p_lo; d.p_hi = it.p_hi; d.pad_ = 0;
+    d.n0 = it.n0; d.n_end = it.n_end; d.p = p; d.p_lo = it.p_lo; d.p_hi = it.p_hi; d.n_lo = it.n_lo;
     d.first = (p == it.p_lo);
     d.valid = 1;
     d.mode = it.mode;
@@ -212,16 +271,16 @@ SS_HD Row make_row_h(const Source& s, int row, int set = 0) {
     if (row >= rows_h(s)) return no_row();
     int part = row % s.K, pc = row / s.K;
     const int len = set ? s.cut[pc] : s.L;
-    Row r = make_row(s.rir + (size_t)pc * s.L, s.hspec + ((size_t)set * rows_h(s) + row) * kSpec, part * kB, len, kB,
-                     1.0f / (float)kF);
+    Row r = make_row(s.rir + (size_t)pc * s.L, s.hspec + ((size_t)set * rows_stored_h(s) + (row - s.h_row0)) * kSpec,
+                     part * kB, len, kB, 1.0f / (float)kF);
     if (s.norm_part) r.div = rir_absmax(s);
     return r;
 }
 // the two rows of k_prepare's RIR CTA `local` (< spectra_pairs_h): pairs of the reverberant set, then of the direct set
 SS_HD void rows_of_pair_h(const Source& s, int local, Row& ra, Row& rb) {
     const int set = local >= pairs_per_set_h(s) ? 1 : 0, j = local - set * pairs_per_set_h(s);
-    ra = make_row_h(s, 2 * j, set);
-    rb = make_row_h(s, 2 * j + 1, set);
+    ra = make_row_h(s, s.h_row0 + 2 * j, set);
+    rb = make_row_h(s, s.h_row0 + 2 * j + 1, set);
 }
 SS_HD Row make_row_x(const Source& s, int blk) {
     if (blk >= s.nblk_max) return no_row();
@@ -545,6 +604,9 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
     // `d` lives in shared memory: copy what the loop needs into registers once - after every global
     // store the compiler would otherwise have to reload each field (generic pointers may alias)
     const int nbase = d.n0 + t, n_end = d.n_end, mode = d.mode, p = d.p;
+    // samples stored: [n_lo, n_end), one unsigned compare (n_lo == n0 unless a window starts inside the block)
+    const int n_lo = d.n_lo;
+    const unsigned span = (unsigned)(n_end - n_lo);
     float* const row = d.row;
     const bool first = d.first != 0;
     if (nbase >= n_end) return;
@@ -553,7 +615,7 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
 #pragma unroll
         for (int r = 0; r < 16; ++r) {
             const int n = nbase + 256 * r;
-            if (n < n_end) {
+            if ((unsigned)(n - n_lo) < span) {
                 const float2 z = R.a[out16(r)];
                 row[n] = z.x;
                 if (row1) row1[n] = z.y;
@@ -574,7 +636,7 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
             const int n = nbase + 256 * r;
             const float2 z = R.a[out16(r)];
             const float v = lerp_terms(one_minus(w[r]), z.x, w[r], z.y);
-            if (n < n_end) row[n] = v;
+            if ((unsigned)(n - n_lo) < span) row[n] = v;
         }
     } else if (mode == MODE_MOVING_BOUNDS) {
         const int* const bounds = d.bounds;
@@ -587,7 +649,7 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
 #pragma unroll
         for (int r = 0; r < 16; ++r) {
             const int n = nbase + 256 * r;
-            if (n < n_end) {
+            if ((unsigned)(n - n_lo) < span) {
                 if (n >= b1) {
                     do { ++sg; b1 = bounds[sg + 1]; } while (n >= b1);
                     b0 = bounds[sg]; step = rstep[sg];
@@ -606,7 +668,7 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
 #pragma unroll
         for (int r = 0; r < 16; ++r) {
             const int n = nbase + 256 * r;
-            if (n < n_end) {
+            if ((unsigned)(n - n_lo) < span) {
                 float fa, fb;
                 hat_pair(idx[n], wv[n], p, fa, fb);
                 const float2 z = R.a[out16(r)];
@@ -621,6 +683,8 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
 // single-segment branch above, with the segment's first sample and 1 / length taken from the work item itself.
 SS_HD void render_epilogue_item(int t, const RItem& it, const Regs32& R) {
     const int nbase = it.n0 + t, n_end = it.n_end;
+    const int n_lo = it.n_lo;                                // stored: [n_lo, n_end), as in render_epilogue
+    const unsigned span = (unsigned)(n_end - n_lo);
     float* const row = it.row;
     if (nbase >= n_end) return;
     if (it.mode == MODE_STATIC) {                            // Re -> channel c, Im -> channel c + 1 (item-uniform branch)
@@ -628,7 +692,7 @@ SS_HD void render_epilogue_item(int t, const RItem& it, const Regs32& R) {
 #pragma unroll
         for (int r = 0; r < 16; ++r) {
             const int n = nbase + 256 * r;
-            if (n < n_end) {
+            if ((unsigned)(n - n_lo) < span) {
                 const float2 z = R.a[out16(r)];
                 row[n] = z.x;
                 if (row1) row1[n] = z.y;
@@ -645,7 +709,7 @@ SS_HD void render_epilogue_item(int t, const RItem& it, const Regs32& R) {
     for (int r = 0; r < 16; ++r) {
         const int n = nbase + 256 * r;
         const float v = lerp_pair(w[r], R.a[out16(r)]);
-        if (n < n_end) row[n] = v;
+        if ((unsigned)(n - n_lo) < span) row[n] = v;
     }
 }
 

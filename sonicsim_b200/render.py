@@ -29,6 +29,8 @@ class MovingSource(T.NamedTuple):
                                       # abs-max on the device like generate_rir_combination (SonicSim_audio.py:398)
     direct_taps: int = 0              # > 0: also render the direct-path stem (every RIR row cut `direct_taps` taps
                                       # after its peak, see SS_DIRECT_TARGET) into the source's direct_outs entry
+    window: T.Optional[T.Tuple[int, int]] = None   # (start, length): render only output samples [start, start + length)
+                                      # into a (C, length) output, bit-identical to those samples of the full render
 
 
 class StaticSource(T.NamedTuple):
@@ -37,6 +39,18 @@ class StaticSource(T.NamedTuple):
     rir: T.Any
     normalize_rirs: bool = False
     direct_taps: int = 0              # as MovingSource.direct_taps
+    window: T.Optional[T.Tuple[int, int]] = None   # as MovingSource.window
+
+
+def _window(s, i, N):
+    """(win_start, win_len, samples per output row) of source i; a window must lie inside [0, N] and not be empty."""
+    if s.window is None:
+        return 0, 0, N
+    a, n = (int(v) for v in s.window)
+    if a < 0 or n < 1 or a + n > N:
+        raise ValueError("window of source %d must be (start, length) with 0 <= start, length >= 1 and "
+                         "start + length <= N = %d, got (%d, %d)" % (i, N, a, n))
+    return a, n, n
 
 
 def _flags(s, i, direct_out) -> int:
@@ -95,22 +109,27 @@ class Renderer:
                 if bounds.shape != (P,):
                     raise ValueError("bounds must have P entries (cumulative segment bounds with leading 0)")
             N = x.shape[0]
-            out = outs[i] if outs is not None else np.empty((C, N), dtype=np.float32)
-            if out.shape != (C, N) or out.dtype != np.float32 or not out.flags.c_contiguous:
-                raise ValueError("out[%d] must be C-contiguous float32 of shape (C, N)" % i)
+            ws, wl, n_out = _window(s, i, N)
+            shape = "(C, N)" if s.window is None else "(C, length) of its window"
+            out = outs[i] if outs is not None else np.empty((C, n_out), dtype=np.float32)
+            if out.shape != (C, n_out) or out.dtype != np.float32 or not out.flags.c_contiguous:
+                raise ValueError("out[%d] must be C-contiguous float32 of shape %s" % (i, shape))
             dout = direct_outs[i]
             flags = _flags(s, i, dout)
-            if dout is not None and (not isinstance(dout, np.ndarray) or dout.shape != (C, N) or
+            if dout is not None and (not isinstance(dout, np.ndarray) or dout.shape != (C, n_out) or
                                      dout.dtype != np.float32 or not dout.flags.c_contiguous):
-                raise ValueError("direct_outs[%d] must be C-contiguous float32 of shape (C, N)" % i)
+                raise ValueError("direct_outs[%d] must be C-contiguous float32 of shape %s" % (i, shape))
             items[i] = SsSource(x=x.ctypes.data, rir=h.ctypes.data, out=out.ctypes.data,
                                 bounds=bounds.ctypes.data if bounds is not None else None,
                                 N=N, P=P, C=C, L=L, mode=mode, flags=flags,
                                 out_direct=dout.ctypes.data if dout is not None else None,
-                                direct_taps=int(s.direct_taps))
+                                direct_taps=int(s.direct_taps), win_start=ws, win_len=wl)
             keep.append((x, h, bounds, out, dout))
             results.append(out)
             if post is not None and lufs_targets[i] is not None:
+                if s.window is not None:
+                    raise ValueError("source %d has a window and a loudness target: the loudness of a stem is "
+                                     "measured over the whole stem" % i)
                 if C > 8:
                     raise ValueError("loudness normalisation supports at most 8 channels")
                 block = 0.4 if N / sr >= 0.4 else N / sr                      # SonicSim_audio.py:69
@@ -131,7 +150,10 @@ class Renderer:
         the device before the copy out - SonicSim_audio.lufs_norm fused behind the render
         (SonicSet.py:97-101).  `loudness_out`, if a list, receives (measured LUFS, linear gain) per source.
         `direct_outs[i]`: a (C, N) float32 array that receives the direct-path stem of a source with direct_taps > 0
-        (None for the other sources); with a loudness target it is scaled by the reverberant stem's gain."""
+        (None for the other sources); with a loudness target it is scaled by the reverberant stem's gain.
+        A source with a `window` (start, length) renders (C, length) arrays instead - the samples
+        [start, start + length) of its full render, bit for bit - and reads and copies only what those need; it
+        cannot have a loudness target."""
         plan = self.plan_host(sources, outs, lufs_targets, sr, direct_outs)
         res = plan.run()
         if loudness_out is not None and lufs_targets is not None:
@@ -141,8 +163,9 @@ class Renderer:
     # ------------------------------------------------------------------ device tensors
     def render_device(self, sources, outs, stream: T.Optional[int] = None, direct_outs=None):
         """`sources`: MovingSource / StaticSource whose fields are CUDA float32 / int32 tensors;
-        `outs`: preallocated CUDA (C, N) tensors; `direct_outs`: the same for the direct-path stems of sources with
-        direct_taps > 0, None for the others.  Asynchronous on `stream` (torch current stream)."""
+        `outs`: preallocated CUDA (C, N) tensors - (C, length) for a source with a `window`; `direct_outs`: the same
+        for the direct-path stems of sources with direct_taps > 0, None for the others.  Asynchronous on `stream`
+        (torch current stream).  Crops that move from call to call are rendered here (a plan binds its windows)."""
         items, n, keep = self._device_items(sources, outs, direct_outs)
         if stream is None:
             import torch
@@ -153,8 +176,9 @@ class Renderer:
         """Bind a batch of device-resident sources to its output tensors once; `plan.run()` then renders it with a
         single C-ABI call - one CUDA graph launch (ss_plan_run; a generation loop overwrites the same tensors and
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
-        (N,), RIRs (P, C, L) / (C, L), outs[i] (C, N) for that source's own C and N; int32 bounds (P,); direct_outs[i]
-        as outs[i] for a source with direct_taps > 0, else None."""
+        (N,), RIRs (P, C, L) / (C, L), outs[i] (C, N) for that source's own C and N ((C, length) with a `window`);
+        int32 bounds (P,); direct_outs[i] as outs[i] for a source with direct_taps > 0, else None.  The plan binds
+        each source's window: crops that move between runs go through render_device."""
         return DevicePlan(self, *self._device_items(sources, outs, direct_outs))
 
     def _device_items(self, sources, outs, direct_outs=None):
@@ -184,12 +208,13 @@ class Renderer:
         for i, s in enumerate(sources):
             chk(s.dry, "dry", i, torch.float32)
             N = s.dry.numel()
+            ws, wl, n_out = _window(s, i, N)
             if isinstance(s, StaticSource):
                 chk(s.rir, "rir", i, torch.float32)
                 if s.rir.dim() != 2:
                     raise ValueError("plan_device: rir of static source %d must be (C, L)" % i)
                 C, L = s.rir.shape
-                chk(outs[i], "out", i, torch.float32, (C, N))
+                chk(outs[i], "out", i, torch.float32, (C, n_out))
                 items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rir.data_ptr(), out=outs[i].data_ptr(),
                                     N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC)
             else:
@@ -197,7 +222,7 @@ class Renderer:
                 if s.rirs.dim() != 3:
                     raise ValueError("plan_device: rirs of moving source %d must be (P, C, L)" % i)
                 P, C, L = s.rirs.shape
-                chk(outs[i], "out", i, torch.float32, (C, N))
+                chk(outs[i], "out", i, torch.float32, (C, n_out))
                 chk(s.bounds, "bounds", i, torch.int32, (P,))
                 bh = None
                 if s.bounds_host is not None:
@@ -209,8 +234,9 @@ class Renderer:
                                     bounds=s.bounds.data_ptr(), N=N, P=P, C=C, L=L,
                                     mode=_lib.SS_MOVING_BOUNDS, bounds_host=bh.ctypes.data if bh is not None else None)
             items[i].flags = _flags(s, i, direct_outs[i])
+            items[i].win_start, items[i].win_len = ws, wl
             if direct_outs[i] is not None:
-                chk(direct_outs[i], "direct_out", i, torch.float32, (C, N))
+                chk(direct_outs[i], "direct_out", i, torch.float32, (C, n_out))
                 items[i].out_direct = direct_outs[i].data_ptr()
                 items[i].direct_taps = int(s.direct_taps)
         return items, n, keep
