@@ -30,6 +30,7 @@ extern "C" {
 #endif
 
 typedef struct ss_ctx ss_ctx;
+typedef struct ss_bank ss_bank;
 
 typedef enum {
     SS_OK = 0,
@@ -74,7 +75,8 @@ typedef enum {
  * host pointers for ss_render_host. */
 typedef struct {
     const float* x;           /* (N,)       dry source, SonicSim_moving.py:64                        */
-    const float* rir;         /* (P, C, L)  per-position RIRs, SonicSim_moving.py:65; (C, L) if static */
+    const float* rir;         /* (P, C, L)  per-position RIRs, SonicSim_moving.py:65; (C, L) if static;
+                               *            NULL with `rir_bank`                                        */
     float* out;               /* (C, N)     rendered stem, SonicSim_moving.py:96 / :60               */
     const int32_t* bounds;    /* SS_MOVING_BOUNDS: np.cumsum(samples_per_interval) with leading 0    */
     const int32_t* idx;       /* SS_MOVING_INDEXED: interp_index (SonicSim_moving.py:42)             */
@@ -87,6 +89,7 @@ typedef struct {
     float* out_direct;        /* SS_DIRECT_TARGET: (C, N) direct-path stem, same pointer kind as `out`, != out    */
     int32_t direct_taps;      /* SS_DIRECT_TARGET: taps kept from each row's peak on, >= 1                        */
     int32_t win_start, win_len; /* time window, see below; win_len == 0: the whole stem                          */
+    const ss_bank* rir_bank;  /* RIR spectrum bank (version 103) instead of `rir`, which is then NULL; see below   */
 } ss_source;                  /* fields appended since version 100: a zeroed (memset) struct leaves them off      */
 
 /* Time window (win_len > 0, version 102): the source renders only output samples [win_start, win_start + win_len)
@@ -113,8 +116,42 @@ typedef struct {
  *     odd, the last row of the position in front may be read);  all P positions under SS_RIR_NORMALIZE (the global
  *     abs-max) and whenever the trajectory is not visible on the host (SS_MOVING_INDEXED, or a device `bounds` without
  *     `bounds_host`).
+ * A source with a `rir_bank` reads no RIR positions at all, windowed or not.
  * On the device path, ss_device_errors reports only what the kernels read: the idx entries of the read set, and the
  * bounds table of a grid-blocked source. */
+
+/* ---- RIR spectrum banks (version 103).  The half spectra of a source's RIR partitions depend on nothing but its taps,
+ * SS_RIR_NORMALIZE and direct_taps - not on the dry signal, the trajectory, the window or the batch.  A bank holds them
+ * in device memory, transformed once by the same kernels and in the same layout as every render transforms them into
+ * its scratch: (P, C, K = ceil(L / 4096), 4096) complex64 pre-scaled by 1/8192, with a direct set a second block of
+ * that shape right behind it and the P * C cut table.  A source that names a bank renders bit-identically to the same
+ * source given the raw RIRs (same flags, through the same kernel variant), without transforming, copying or reading
+ * any RIR: re-rendering a fixed RIR set (a trajectory of an RIR dump, a training scene) with new dry signals.
+ *
+ * rir: (P, C, L) float32, or (C, L) with P = 1 for a static source.  flags: SS_RIR_NORMALIZE (the bank holds the
+ * normalised taps' spectra) and / or SS_DIRECT_TARGET (also the direct-path set, direct_taps >= 1; see that flag).
+ * _dev: device pointer, asynchronous on `stream`: the caller keeps `rir` unchanged until the stream gets there.  The bank
+ * records an event behind its construction, and every call that uses it - ss_render_dev (on its `stream`),
+ * ss_render_host / _ex (on the context's own streams) and every ss_plan_run - makes its work wait on that event, so a
+ * render never reads a bank that is still being built, whatever stream built it.  _host: host pointer, returns when the
+ * bank is complete.  The bank holds 8 * 4096 * P * C * K bytes per set (ss_bank_bytes: everything it holds on the device).
+ *
+ * A source that uses a bank (every violation is SS_ERR_INVALID, before any work):
+ *   - sets `rir_bank` and leaves `rir` NULL;
+ *   - has the bank's P, C and L; a static source takes a bank with P == 1, a moving source one with P >= 2;
+ *   - does not set SS_RIR_NORMALIZE (normalisation is a property of the bank);
+ *   - sets SS_DIRECT_TARGET only with a bank that holds a direct set, and then with the bank's direct_taps (a bank with
+ *     a direct set also serves sources that render only the reverberant stem);
+ *   - is rendered with the context that created the bank (and so on its device).
+ * Windows, ss_render_host_ex loudness targets and plans work with banked sources as with raw RIRs.  Lifetime: a bank
+ * must outlive every call and every plan that uses it (see the plan rules below); ss_bank_destroy waits for the device
+ * before it frees the bank, like ss_plan_destroy.  Bank bytes are not part of the chunk budget (ss_set_chunk_bytes). */
+int ss_bank_create_dev(ss_ctx* ctx, const float* rir, int32_t P, int32_t C, int32_t L, int32_t flags,
+                       int32_t direct_taps, void* stream, ss_bank** out);
+int ss_bank_create_host(ss_ctx* ctx, const float* rir, int32_t P, int32_t C, int32_t L, int32_t flags,
+                        int32_t direct_taps, ss_bank** out);
+int64_t ss_bank_bytes(const ss_bank* bank);   /* device bytes held */
+void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their context */
 
 /* library / build identification */
 int ss_version(void);
@@ -152,7 +189,9 @@ int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
  * internal streams and join back).  Results are identical to ss_render_dev on the same items.  The pointers in
  * `items` and the values behind bounds_host must stay valid and unchanged while the plan lives; the contents of the
  * x / rir / out buffers may change between runs.  Device-side `bounds` / `idx` are read at run time and must satisfy the
- * same preconditions as for ss_render_dev.  Not thread-safe; destroy plans before their context. */
+ * same preconditions as for ss_render_dev.  A plan may hold banked sources: every ss_bank they name must outlive the
+ * plan (destroy the plan first; a bank's spectra are read at every run).  Not thread-safe; destroy plans before their
+ * context. */
 typedef struct ss_plan ss_plan;
 int ss_plan_create(ss_ctx* ctx, const ss_source* items, int n_items, ss_plan** out);
 int ss_plan_run(ss_plan* plan, void* stream);

@@ -20,6 +20,8 @@
 //   k_rir_absmax  : optional, SS_RIR_NORMALIZE: global abs-max of a source's RIR tensor for k_prepare's row loads
 //   k_rir_direct  : optional, SS_DIRECT_TARGET: per-row direct-path length (argmax |h| + direct_taps); k_prepare then
 //                   transforms the truncated rows as a second RIR set and fills a second group of items per block
+// A source with an RIR spectrum bank (ss_bank) has its RIR spectra (and cuts) already: it adds no k_rir_absmax /
+// k_rir_direct work and no RIR CTAs to k_prepare.  A bank is built by these same launches over a source without blocks.
 // Consecutive chunks rotate through three streams / scratch buffers so that they overlap; a bound batch (ss_plan_*)
 // captures all of it into one CUDA graph.
 // fp32 throughout (the reference is float32 end to end, SURVEY 8), no cuFFT.
@@ -218,7 +220,7 @@ __global__ void __launch_bounds__(256)
 k_rir_direct(const Source* __restrict__ srcs, int per_src) {
     const Source& S = srcs[blockIdx.x / per_src];
     const int row = (blockIdx.x % per_src) * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (!S.cut || row >= S.P * S.C) return;
+    if (!S.cut || !S.rir || row >= S.P * S.C) return;          // banked source (no rir): its cut table is the bank's
     // windowed source: only the (p, c) rows its transformed RIR rows come from (the others may not even be in memory)
     if (S.h_rows && (row < S.h_row0 / S.K || row > (S.h_row0 + S.h_rows - 1) / S.K)) return;
     const float div = S.norm_part ? rir_absmax(S) : 0.f;
@@ -616,7 +618,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 102; }
+extern "C" int ss_version(void) { return 103; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -795,8 +797,43 @@ extern "C" int ss_host_alloc(void** p, int64_t bytes) {
 }
 extern "C" void ss_host_free(void* p) { if (p) cudaFreeHost(p); }
 
+// RIR spectrum bank: one device allocation = [reverberant set | direct set] (P*C*K rows of kSpec float2 each, the layout
+// k_prepare writes into chunk scratch) | cut table (direct set) | descriptor of the blockless source that built it |
+// its norm_part slots (SS_RIR_NORMALIZE).
+struct ss_bank {
+    ss_ctx* c = nullptr;                  // the context that made it; sources of other contexts are refused
+    char* d_mem = nullptr;
+    size_t bytes = 0;
+    float2* spec = nullptr;
+    int* cut = nullptr;                   // P*C direct-path row lengths, or null: no direct set
+    int P = 0, C = 0, L = 0, K = 0, flags = 0, direct_taps = 0;
+    cudaEvent_t ready = nullptr;          // recorded behind the launches that build it; every use waits on it
+};
+// Order `stream` after the construction of every bank the items use (a bank built from device memory is built
+// asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
+static int wait_banks(const ss_source* items, int n, cudaStream_t stream) {
+    const ss_bank* last = nullptr;
+    for (int i = 0; i < n; ++i) {
+        const ss_bank* b = items[i].rir_bank;
+        if (!b || b == last) continue;                  // (one wait per run of sources sharing a bank)
+        CK(cudaStreamWaitEvent(stream, b->ready, 0));
+        last = b;
+    }
+    return SS_OK;
+}
+
+// A banked source against its bank (include/sonicsim_b200.h): same shape, normalisation left to the bank, a direct
+// target only with the bank's direct set and taps.  (A static source has P == 1 and a moving one P >= 2, checked by
+// validate_item, so the shape check also gives the bank's P the source's mode.)
+static int validate_bank_use(const ss_source& it) {
+    const ss_bank* b = it.rir_bank;
+    if (it.P != b->P || it.C != b->C || it.L != b->L) return SS_ERR_INVALID;
+    if (it.flags & SS_RIR_NORMALIZE) return SS_ERR_INVALID;
+    if ((it.flags & SS_DIRECT_TARGET) && (!b->cut || it.direct_taps != b->direct_taps)) return SS_ERR_INVALID;
+    return SS_OK;
+}
 static int validate_item(const ss_source& it) {
-    if (!it.x || !it.rir || !it.out) return SS_ERR_INVALID;
+    if (!it.x || !it.out || (it.rir != nullptr) == (it.rir_bank != nullptr)) return SS_ERR_INVALID;   // rir xor bank
     if (it.N <= 0 || it.C <= 0 || it.L <= 0 || it.P <= 0) return SS_ERR_INVALID;
     // 32-bit sample / table indices inside the kernels: leave one FFT of headroom below 2^31
     if (it.N > 0x7fffffff - 2 * kF) return SS_ERR_UNSUPPORTED;
@@ -811,7 +848,13 @@ static int validate_item(const ss_source& it) {
     if (it.win_len < 0 || it.win_start < 0 || (it.win_len == 0 && it.win_start != 0) ||
         (int64_t)it.win_start + it.win_len > (int64_t)it.N)
         return SS_ERR_INVALID;
-    return SS_OK;
+    return it.rir_bank ? validate_bank_use(it) : SS_OK;
+}
+// every bank of a batch belongs to the context that renders it
+static int validate_item_ctx(const ss_ctx* c, const ss_source& it) {
+    const int st = validate_item(it);
+    if (st) return st;
+    return (it.rir_bank && it.rir_bank->c != c) ? SS_ERR_INVALID : SS_OK;
 }
 // A trajectory bounds table as the header requires it: ascending from 0 to N.  Checked before anything plans blocks from
 // it - a table outside the contract would make the host-side block planner write past the table it sized.
@@ -822,8 +865,10 @@ static bool bounds_ok(const int32_t* b, int P, int N) {
 }
 // SS_DIRECT_TARGET: a second RIR set (spectra, items per block) and the P*C cut table
 static int direct_sets(const ss_source& it) { return (it.flags & SS_DIRECT_TARGET) ? 2 : 1; }
+// RIR sets and cut table in the chunk's scratch: none for a banked source, whose spectra and cuts live in its bank
+static int scratch_sets(const ss_source& it) { return it.rir_bank ? 0 : direct_sets(it); }
 static size_t cut_bytes(const ss_source& it) {
-    return (it.flags & SS_DIRECT_TARGET) ? align_up(sizeof(int) * (size_t)it.P * it.C, 256) : 0;
+    return ((it.flags & SS_DIRECT_TARGET) && !it.rir_bank) ? align_up(sizeof(int) * (size_t)it.P * it.C, 256) : 0;
 }
 // shapes derived from one ss_source
 struct Shape {
@@ -930,7 +975,7 @@ static Shape shape_of(const ss_source& it) {
 static size_t rir_rows(const ss_source& it, const Shape& sh) { return sh.win ? (size_t)sh.rows : (size_t)it.P * it.C * sh.K; }
 static size_t spectra_bytes(const ss_source& it) {
     const Shape sh = shape_of(it);
-    return (rir_rows(it, sh) * direct_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
+    return (rir_rows(it, sh) * scratch_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
            (size_t)sh.max_items * sizeof(RItem) +
            align_up(sizeof(Block) * (size_t)sh.nblk_max, 256) + align_up(sizeof(double) * (size_t)it.P, 256) + 256 +
            ((it.flags & SS_RIR_NORMALIZE) ? 512 : 0) + cut_bytes(it);
@@ -1047,14 +1092,21 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
         s.w = it.mode == SS_MOVING_INDEXED ? it.w : nullptr;
         s.N = it.N; s.P = it.P; s.C = it.C; s.L = it.L;
         s.K = sh.K; s.nb = sh.nb; s.mode = it.mode; s.aligned = sh.aligned; s.nblk_max = sh.nblk_max;
-        s.hspec = (float2*)scratch; scratch += rir_rows(it, sh) * direct_sets(it) * kSpec * sizeof(float2);
-        if (sh.win) { s.h_row0 = sh.row0; s.h_rows = sh.rows; }
+        if (it.rir_bank) {
+            // spectra (and cuts) from the bank: no RIR rows, no cut table, no k_rir_absmax / k_rir_direct work
+            set_banked(s, it.rir_bank->spec, (it.flags & SS_DIRECT_TARGET) ? it.rir_bank->cut : nullptr, sh.win != 0);
+        } else {
+            s.hspec = (float2*)scratch; scratch += rir_rows(it, sh) * direct_sets(it) * kSpec * sizeof(float2);
+            if (sh.win) { s.h_row0 = sh.row0; s.h_rows = sh.rows; }
+        }
         s.xspec = (float2*)scratch; scratch += (size_t)s.nblk_max * kSpec * sizeof(float2);
         if (it.flags & SS_RIR_NORMALIZE) { s.norm_part = (const float*)scratch; scratch += 512; any_norm = true; }
         if (it.flags & SS_DIRECT_TARGET) {
-            s.cut = (int*)scratch; scratch += cut_bytes(it);
+            if (!it.rir_bank) {
+                s.cut = (int*)scratch; scratch += cut_bytes(it);
+                grid_direct = std::max(grid_direct, (s.P * s.C + 7) / 8);
+            }
             s.out_direct = it.out_direct; s.direct_taps = it.direct_taps;
-            grid_direct = std::max(grid_direct, (s.P * s.C + 7) / 8);
         }
         if (host_tables) {
             // tables live in the descriptor block itself: filled here, copied with it
@@ -1140,8 +1192,101 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, s
         CK(cudaGetLastError());
     }
     if (pf) CK(cudaEventRecord(pf->e2, stream));
-    c->launches += 2;
+    c->launches += (L.ps > 0 ? 1 : 0) + (L.grid_r > 0 ? 1 : 0);      // (both, for every chunk of a render)
     return SS_OK;
+}
+
+// ----------------------------------------------------------------------------- RIR spectrum banks
+// A bank is built by the render pipeline itself: one chunk whose only source has the bank's RIRs and no blocks
+// (nblk_max = 0), so that k_rir_absmax (SS_RIR_NORMALIZE), k_rir_direct (SS_DIRECT_TARGET) and k_prepare's RIR CTAs run
+// exactly as for a whole source of a render - rows paired (2r, 2r + 1) per set - and write into the bank instead of
+// chunk scratch.  Its spectra therefore have the bits a render would transform itself.
+static int bank_args(const ss_ctx* c, const float* rir, int P, int C, int L, int flags, int direct_taps, ss_bank** out) {
+    if (!c || !rir || !out || P < 1 || C < 1 || L < 1) return SS_ERR_INVALID;
+    if (flags & ~(SS_RIR_NORMALIZE | SS_DIRECT_TARGET)) return SS_ERR_INVALID;
+    if ((flags & SS_DIRECT_TARGET) && direct_taps < 1) return SS_ERR_INVALID;
+    if ((int64_t)P * C * ((L + kB - 1) / kB) > (int64_t)1 << 28) return SS_ERR_UNSUPPORTED;    // as validate_item
+    return SS_OK;
+}
+static int ensure(char** p, size_t* cap, size_t need);      // (host path, below)
+static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stream) {
+    const bool direct = (b->flags & SS_DIRECT_TARGET) != 0, norm = (b->flags & SS_RIR_NORMALIZE) != 0;
+    const size_t spec_b = (direct ? 2 : 1) * (size_t)b->P * b->C * b->K * kSpec * sizeof(float2);
+    const size_t cut_b = direct ? align_up(sizeof(int) * (size_t)b->P * b->C, 256) : 0;
+    const size_t src_b = align_up(sizeof(Source), 256);
+    b->bytes = spec_b + cut_b + src_b + (norm ? 512 : 0);
+    CK(cudaMalloc((void**)&b->d_mem, b->bytes));
+    char* p = b->d_mem;
+    b->spec = (float2*)p; p += spec_b;
+    if (direct) { b->cut = (int*)p; p += cut_b; }
+    Source* d_src = (Source*)p; p += src_b;
+    Source s;
+    memset(&s, 0, sizeof(s));
+    s.rir = rir; s.N = 1; s.P = b->P; s.C = b->C; s.L = b->L; s.K = b->K; s.nb = 1;
+    s.mode = b->P == 1 ? MODE_STATIC : MODE_MOVING_BOUNDS;
+    s.nblk_max = 0;                                      // no blocks: no dry windows, no range CTAs, no items
+    s.hspec = b->spec;
+    if (norm) s.norm_part = (const float*)p;
+    if (direct) { s.cut = b->cut; s.direct_taps = b->direct_taps; }
+    static thread_local ChunkLaunch L;                  // kernel parameters, as in launch_chunk
+    L = ChunkLaunch();
+    L.n = 1; L.ps = spectra_pairs_h(s); L.grid_r = 0; L.n_known = 0;
+    L.any_norm = norm; L.grid_direct = direct ? (s.P * s.C + 7) / 8 : 0;
+    L.ds = d_src;
+    L.pp.n_inline = 1; L.pp.prefix[0] = 0; L.pp.prefix[1] = L.ps; L.pp.srcs[0] = s;
+    CK(cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming));
+    CK(cudaMemcpyAsync(d_src, &s, sizeof(s), cudaMemcpyHostToDevice, stream));  // k_rir_absmax / k_rir_direct read it
+    { int st = chunk_enqueue(c, L, stream, nullptr); if (st) return st; }
+    CK(cudaEventRecord(b->ready, stream));
+    return SS_OK;
+}
+
+// Waits for the whole device: a render that used the bank may run on any stream of the caller (cudaFree would wait for
+// the device anyway).
+extern "C" void ss_bank_destroy(ss_bank* b) {
+    if (!b) return;
+    cudaSetDevice(b->c->device);
+    cudaDeviceSynchronize();
+    if (b->d_mem) cudaFree(b->d_mem);
+    if (b->ready) cudaEventDestroy(b->ready);
+    delete b;
+}
+extern "C" int64_t ss_bank_bytes(const ss_bank* b) { return b ? (int64_t)b->bytes : 0; }
+
+extern "C" int ss_bank_create_dev(ss_ctx* c, const float* rir, int32_t P, int32_t C, int32_t L, int32_t flags,
+                                  int32_t direct_taps, void* stream, ss_bank** out) {
+    { int st = bank_args(c, rir, P, C, L, flags, direct_taps, out); if (st) return st; }
+    *out = nullptr;
+    CK(cudaSetDevice(c->device));
+    ss_bank* b = new (std::nothrow) ss_bank();
+    if (!b) return SS_ERR_NOMEM;
+    b->c = c; b->P = P; b->C = C; b->L = L; b->K = (L + kB - 1) / kB; b->flags = flags;
+    b->direct_taps = (flags & SS_DIRECT_TARGET) ? direct_taps : 0;
+    const int st = bank_build(c, b, rir, (cudaStream_t)stream);
+    if (st != SS_OK) { ss_bank_destroy(b); return st; }
+    *out = b;
+    return SS_OK;
+}
+
+extern "C" int ss_bank_create_host(ss_ctx* c, const float* rir, int32_t P, int32_t C, int32_t L, int32_t flags,
+                                   int32_t direct_taps, ss_bank** out) {
+    { int st = bank_args(c, rir, P, C, L, flags, direct_taps, out); if (st) return st; }
+    *out = nullptr;
+    CK(cudaSetDevice(c->device));
+    // the RIRs pass through the host path's first input slot, idle between calls (ss_render_host_ex returns after its
+    // streams): no allocation per bank once the slot is large enough
+    const size_t nb = sizeof(float) * (size_t)P * C * L;
+    ss_ctx::Slot& sl = c->slot[0];
+    { int st = ensure(&sl.d_in, &sl.in_cap, nb); if (st) return st; }
+    const float* d_rir = (const float*)sl.d_in;
+    int st = SS_OK;
+    cudaError_t e = cudaMemcpyAsync(sl.d_in, rir, nb, cudaMemcpyHostToDevice, c->s_in);
+    if (e != cudaSuccess) { g_last_cuda = (int)e; st = SS_ERR_CUDA; }
+    if (st == SS_OK) st = ss_bank_create_dev(c, d_rir, P, C, L, flags, direct_taps, (void*)c->s_in, out);
+    e = cudaStreamSynchronize(c->s_in);                 // the bank is complete; the slot is free again
+    if (st == SS_OK && e != cudaSuccess) { g_last_cuda = (int)e; st = SS_ERR_CUDA; }
+    if (st != SS_OK && *out) { ss_bank_destroy(*out); *out = nullptr; }
+    return st;
 }
 
 // Describe items[first, last) (device pointers) in the next slot of the descriptor ring, copy the block and enqueue
@@ -1241,9 +1386,9 @@ extern "C" int ss_debug_chunks(const int64_t* bytes, int32_t n, int64_t budget, 
     return (int)cuts.size();
 }
 
-static int validate_dev_items(const ss_source* items, int n_items) {
+static int validate_dev_items(const ss_ctx* c, const ss_source* items, int n_items) {
     for (int i = 0; i < n_items; ++i) {
-        int st = validate_item(items[i]); if (st) return st;
+        int st = validate_item_ctx(c, items[i]); if (st) return st;
         if (items[i].mode == SS_MOVING_BOUNDS && items[i].bounds_host &&
             !bounds_ok(items[i].bounds_host, items[i].P, items[i].N))
             return SS_ERR_INVALID;
@@ -1255,7 +1400,8 @@ extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, voi
     if (!c || (!items && n_items > 0) || n_items < 0) return SS_ERR_INVALID;
     if (n_items == 0) return SS_OK;
     CK(cudaSetDevice(c->device));
-    { int st = validate_dev_items(items, n_items); if (st) return st; }
+    { int st = validate_dev_items(c, items, n_items); if (st) return st; }
+    { int st = wait_banks(items, n_items, (cudaStream_t)stream); if (st) return st; }   // before the fork: every chunk
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
     arrange_chunks(c, items, n_items, arranged, cuts);
@@ -1308,6 +1454,7 @@ struct ss_plan {
     // which the context's events are)
     cudaEvent_t ev_fork = nullptr, ev_join[ss_ctx::kAux] = {};
     cudaStream_t s_cap = nullptr;      // capture origin: the caller's stream may be the legacy default stream, which cannot capture
+    std::vector<ss_bank*> banks;       // banks of the plan's sources: every run waits for their construction
 };
 
 extern "C" void ss_plan_destroy(ss_plan* p) {
@@ -1361,10 +1508,14 @@ extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
-    { int st = validate_dev_items(items, n_items); if (st) return st; }
+    { int st = validate_dev_items(c, items, n_items); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
+    for (int i = 0; i < n_items; ++i) {
+        ss_bank* b = const_cast<ss_bank*>(items[i].rir_bank);
+        if (b && std::find(p->banks.begin(), p->banks.end(), b) == p->banks.end()) p->banks.push_back(b);
+    }
     const int st = plan_build(p, items, n_items);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     *out = p;
@@ -1395,6 +1546,7 @@ extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
     ss_ctx* c = p->c;
     cudaStream_t stream = (cudaStream_t)stream_;
     CK(cudaSetDevice(c->device));
+    for (ss_bank* b : p->banks) CK(cudaStreamWaitEvent(stream, b->ready, 0));    // (outside any capture)
     if (c->profiling) {
         // per-kernel timing: chunks one after the other on the caller's stream, events around every launch
         c->prof_chunk = 0;
@@ -1479,7 +1631,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     const ss_post_lufs* first_post = nullptr;
     std::vector<ReadSet> rset(n_items);
     for (int i = 0; i < n_items; ++i) {
-        int st = validate_item(items[i]); if (st) return st;
+        int st = validate_item_ctx(c, items[i]); if (st) return st;
         // a window cannot be loudness-normalised: the reference measures the whole stem
         if (post && post[i].brk && items[i].win_len > 0) return SS_ERR_INVALID;
         if (items[i].mode == SS_MOVING_BOUNDS && !bounds_ok(items[i].bounds, items[i].P, items[i].N)) return SS_ERR_INVALID;
@@ -1493,6 +1645,8 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     }
     // an earlier asynchronous ss_render_dev may still be using scratch buffer 0 on its internal streams
     for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_cmp, c->ev_join[i], 0));
+    // banks built asynchronously on the caller's stream: every render of this call (on s_cmp) comes after them
+    { int st = wait_banks(items, n_items, c->s_cmp); if (st) return st; }
     std::vector<int> cuts;
     make_chunks(c, items, n_items, cuts, c->chunk_bytes_host);
     std::vector<ss_source> dev(n_items);
@@ -1559,8 +1713,8 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         for (int i = first; i < last; ++i) {
             const ss_source& it = items[i];
             const ReadSet& rs = rset[i];
-            in_b += align_up(sizeof(float) * (size_t)(rs.xb - rs.xa), 256) +
-                    align_up(sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L, 256);
+            in_b += align_up(sizeof(float) * (size_t)(rs.xb - rs.xa), 256);
+            if (!it.rir_bank) in_b += align_up(sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L, 256);
             if (it.mode == SS_MOVING_BOUNDS) in_b += align_up(sizeof(int32_t) * (size_t)it.P, 256);
             if (it.mode == SS_MOVING_INDEXED) in_b += 2 * align_up(4 * (size_t)(rs.ib - rs.ia), 256);
             out_b += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256) * direct_sets(it);
@@ -1581,9 +1735,11 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
             // only the read set is copied; the device pointers are offset so that the kernels index the full arrays
             nb = sizeof(float) * (size_t)(rs.xb - rs.xa);
             CK(cudaMemcpyAsync(pi, it.x + rs.xa, nb, cudaMemcpyHostToDevice, c->s_in)); d.x = (const float*)pi - rs.xa; pi += align_up(nb, 256);
-            const size_t pos0 = (size_t)rs.pa * it.C * it.L;
-            nb = sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L;
-            CK(cudaMemcpyAsync(pi, it.rir + pos0, nb, cudaMemcpyHostToDevice, c->s_in)); d.rir = (const float*)pi - pos0; pi += align_up(nb, 256);
+            if (!it.rir_bank) {                              // a banked source's spectra are on the device already
+                const size_t pos0 = (size_t)rs.pa * it.C * it.L;
+                nb = sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L;
+                CK(cudaMemcpyAsync(pi, it.rir + pos0, nb, cudaMemcpyHostToDevice, c->s_in)); d.rir = (const float*)pi - pos0; pi += align_up(nb, 256);
+            }
             if (it.mode == SS_MOVING_BOUNDS) {
                 nb = sizeof(int32_t) * (size_t)it.P;
                 CK(cudaMemcpyAsync(pi, it.bounds, nb, cudaMemcpyHostToDevice, c->s_in)); d.bounds = (const int32_t*)pi; pi += align_up(nb, 256);

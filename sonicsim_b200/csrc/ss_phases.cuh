@@ -59,6 +59,15 @@ struct Source {
     // (C, win_len).  h_rows != 0 marks a windowed source.
     int h_row0, h_rows;
 };
+// A banked source (ss_bank, include/sonicsim_b200.h) has rir == null: hspec (and cut, with a direct target) point into
+// the bank, which holds all P*C*K rows of each set from row 0 - what a whole source transforms into its scratch - so
+// k_prepare transforms none of its rows (spectra_pairs_h == 0), k_rir_direct skips it and it has no norm_part.  Windowed
+// or not, the set stride and row origin are the bank's: h_row0 = 0, and h_rows = P*C*K when windowed (still nonzero,
+// it marks the window).  Needs P, C and K set.
+SS_HD void set_banked(Source& s, float2* spec, int* cut, bool windowed) {
+    s.rir = nullptr; s.hspec = spec; s.cut = cut; s.norm_part = nullptr;
+    s.h_row0 = 0; s.h_rows = windowed ? s.P * s.C * s.K : 0;
+}
 constexpr int kNormParts = 128;    // CTAs (partial maxima) per normalised source in k_rir_absmax
 
 // One unit of k_render work: one block of channel c (static: channels c, c+1), written by k_prepare
@@ -110,7 +119,7 @@ static_assert(sizeof(XDesc) == 112, "XDesc layout");
 SS_HD int rows_h(const Source& s) { return s.P * s.C * s.K; }                 // per set (reverberant, direct)
 SS_HD int rows_stored_h(const Source& s) { return s.h_rows ? s.h_rows : rows_h(s); }     // transformed rows per set
 SS_HD int pairs_per_set_h(const Source& s) { return (rows_stored_h(s) + 1) >> 1; }
-SS_HD int spectra_pairs_h(const Source& s) { return pairs_per_set_h(s) * (s.cut ? 2 : 1); }
+SS_HD int spectra_pairs_h(const Source& s) { return s.rir ? pairs_per_set_h(s) * (s.cut ? 2 : 1) : 0; }   // banked: 0
 SS_HD int spectra_pairs_x(const Source& s) { return (s.nblk_max + 1) >> 1; }
 SS_HD int range_ctas(const Source& s) { return (s.nblk_max + 7) >> 3; }       // k_prepare: one warp per block
 SS_HD int items_per_set(const Source& s) { return s.mode == MODE_STATIC ? (s.C + 1) >> 1 : s.C; }

@@ -7,6 +7,7 @@ has no such symbols.  They render many (utterance, source) units with one C-ABI 
 """
 import ctypes
 import typing as T
+import weakref
 
 import numpy as np
 
@@ -20,7 +21,8 @@ class MovingSource(T.NamedTuple):
     `bounds_host` (device path only, optional): NumPy copy of `bounds`; lets the library build the block
     table on the host (exact choice of the blocking plan, one small kernel less).  It must hold the same values as
     the device tensor whenever the batch runs - a plan that is re-run after `bounds` was overwritten on the device
-    needs a new plan (or no `bounds_host`)."""
+    needs a new plan (or no `bounds_host`).
+    `rirs` may be a RirBank (Renderer.rir_bank) of the same (P, C, L) instead of the raw RIRs, on every path."""
     dry: T.Any
     rirs: T.Any
     bounds: T.Any
@@ -34,7 +36,7 @@ class MovingSource(T.NamedTuple):
 
 
 class StaticSource(T.NamedTuple):
-    """One static source: dry (N,), RIR (C, L)."""
+    """One static source: dry (N,), RIR (C, L), or a RirBank of shape (C, L) / (1, C, L)."""
     dry: T.Any
     rir: T.Any
     normalize_rirs: bool = False
@@ -65,6 +67,92 @@ def _flags(s, i, direct_out) -> int:
     return (_lib.SS_RIR_NORMALIZE if s.normalize_rirs else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
 
 
+class RirBank:
+    """The half spectra of one RIR set, transformed once and held in device memory (Renderer.rir_bank; ss_bank of the C
+    ABI).  Pass it as `MovingSource.rirs` / `StaticSource.rir`: the source renders bit-identically to the same source
+    given the raw RIRs, which are never read again.  It belongs to the context of the renderer that made it.  Every
+    render that uses it is ordered after its construction by the library, on every path, whatever stream built it.
+    Plans hold the bank: it is freed only once it is closed (or collected) and no live plan uses it any more."""
+
+    def __init__(self, renderer, handle, shape, normalize, direct_taps):
+        self.renderer, self._h = renderer, handle
+        self.shape = tuple(int(v) for v in shape)          # as given: (P, C, L) or (C, L)
+        self.normalize, self.direct_taps = bool(normalize), int(direct_taps)
+        self.nbytes = int(renderer.lib.ss_bank_bytes(handle))
+        self._closing, self._plans = False, 0
+
+    @property
+    def pcl(self) -> T.Tuple[int, int, int]:
+        return self.shape if len(self.shape) == 3 else (1,) + self.shape
+
+    @property
+    def closed(self) -> bool:
+        """True once close() was called: new sources may not use the bank (plans made before keep working)."""
+        return self._closing or not self._h
+
+    def close(self):
+        """Refuse the bank to new sources and free its device memory - at once, or, while plans that use it are alive,
+        when the last of them is closed or collected (their runs keep reading it until then)."""
+        self._closing = True
+        if self._plans == 0:
+            self._free()
+
+    def _free(self):
+        if self._h:
+            self.renderer.lib.ss_bank_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def _hold(self):
+        self._plans += 1
+
+    def _release(self):
+        self._plans -= 1
+        if self._closing and self._plans == 0:
+            self._free()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _bank_of(renderer, s, i, P, C, L):
+    """Checks a banked source against its bank before any C call; returns the ss_bank handle."""
+    b = s.rir if isinstance(s, StaticSource) else s.rirs
+    if b.closed:
+        raise ValueError("source %d: its RirBank is closed" % i)
+    if b.renderer.ctx.value != renderer.ctx.value:
+        raise ValueError("source %d: its RirBank belongs to another renderer's context" % i)
+    if b.pcl != (P, C, L):
+        raise ValueError("source %d: its RirBank holds (P, C, L) = %s, the source has %s" % (i, b.pcl, (P, C, L)))
+    if s.normalize_rirs:
+        raise ValueError("source %d: normalisation is a property of its RirBank (normalize=%s); leave normalize_rirs "
+                         "False" % (i, b.normalize))
+    if int(s.direct_taps) not in (0, b.direct_taps):
+        raise ValueError("source %d: direct_taps = %d, its RirBank holds %s" % (
+            i, int(s.direct_taps), "direct_taps = %d" % b.direct_taps if b.direct_taps else "no direct set"))
+    return b._h.value
+
+
+def _release_banks(banks):
+    for b in banks:
+        b._release()
+
+
+def _hold_banks(plan, sources):
+    """The RirBanks of a plan's sources are held until the plan is closed or collected: a bank closed meanwhile is
+    freed only then.  Returns the finalizer that releases them (calling it releases them at once, once)."""
+    banks = []
+    for s in sources:
+        b = s.rir if isinstance(s, StaticSource) else s.rirs
+        if isinstance(b, RirBank) and all(b is not o for o in banks):
+            banks.append(b)
+    for b in banks:
+        b._hold()
+    return weakref.finalize(plan, _release_banks, banks)
+
+
 def _check_direct_outs(direct_outs, n):
     if direct_outs is not None and len(direct_outs) != n:
         raise ValueError("%d sources but %d entries in direct_outs" % (n, len(direct_outs)))
@@ -78,6 +166,40 @@ class Renderer:
         self.lib = _lib.load()
         self.device = _lib.default_device() if device is None else int(device)
         self.ctx = _lib.context(self.device)
+
+    # ------------------------------------------------------------------ RIR spectrum banks
+    def rir_bank(self, rirs, normalize: bool = False, direct_taps: int = 0) -> RirBank:
+        """Transform an RIR set (P, C, L) - or (C, L) for a static source - once into a RirBank on this renderer's
+        device: a NumPy array is copied in and the call returns when the bank is complete; a CUDA float32 tensor of this
+        device is transformed asynchronously on the current stream (keep it unchanged until that stream gets there).
+        Either way the bank can be used at once, on every path: every render that uses it - render_host / plan_host on
+        the library's own streams, render_device / plan_device on any stream - waits for its construction first.
+        `normalize` / `direct_taps` are the normalize_rirs / direct_taps every source of the bank renders with (a bank
+        with a direct set also serves sources with direct_taps = 0)."""
+        taps = int(direct_taps)
+        if taps < 0:
+            raise ValueError("direct_taps must be >= 0, got %d" % taps)
+        flags = (_lib.SS_RIR_NORMALIZE if normalize else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
+        h = ctypes.c_void_p()
+        if type(rirs).__module__.split(".")[0] == "torch":
+            import torch
+            if not rirs.is_cuda or rirs.device.index != self.device:
+                raise ValueError("rir_bank: a tensor must be on cuda:%d" % self.device)
+            if rirs.dtype != torch.float32 or not rirs.is_contiguous() or rirs.dim() not in (2, 3):
+                raise ValueError("rir_bank: rirs must be a contiguous float32 (P, C, L) or (C, L) tensor")
+            shape = tuple(rirs.shape)
+            P, C, L = shape if len(shape) == 3 else (1,) + shape
+            stream = torch.cuda.current_stream(rirs.device).cuda_stream
+            _lib.check(self.lib.ss_bank_create_dev(self.ctx, rirs.data_ptr(), P, C, L, flags, taps,
+                                                   ctypes.c_void_p(stream), ctypes.byref(h)))
+        else:
+            a = _as_f32(rirs)
+            if a.ndim not in (2, 3):
+                raise ValueError("rir_bank: rirs must be (P, C, L) or (C, L), got shape %s" % (a.shape,))
+            shape = a.shape
+            P, C, L = shape if len(shape) == 3 else (1,) + shape
+            _lib.check(self.lib.ss_bank_create_host(self.ctx, a.ctypes.data, P, C, L, flags, taps, ctypes.byref(h)))
+        return RirBank(self, h, shape, normalize, taps)
 
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
@@ -97,13 +219,22 @@ class Renderer:
         results = []
         for i, s in enumerate(sources):
             x = _as_f32(s.dry).reshape(-1)
+            rb = s.rir if isinstance(s, StaticSource) else s.rirs
+            rb = rb if isinstance(rb, RirBank) else None
+            h = None
             if isinstance(s, StaticSource):
-                h = _as_f32(s.rir)
-                C, L = h.shape
+                if rb is None:
+                    h = _as_f32(s.rir)
+                    C, L = h.shape
+                else:
+                    C, L = rb.pcl[1:]
                 P, mode, bounds = 1, _lib.SS_STATIC, None
             else:
-                h = _as_f32(s.rirs)
-                P, C, L = h.shape
+                if rb is None:
+                    h = _as_f32(s.rirs)
+                    P, C, L = h.shape
+                else:
+                    P, C, L = rb.pcl
                 bounds = np.ascontiguousarray(s.bounds, dtype=np.int32)
                 mode = _lib.SS_MOVING_BOUNDS
                 if bounds.shape != (P,):
@@ -119,12 +250,13 @@ class Renderer:
             if dout is not None and (not isinstance(dout, np.ndarray) or dout.shape != (C, n_out) or
                                      dout.dtype != np.float32 or not dout.flags.c_contiguous):
                 raise ValueError("direct_outs[%d] must be C-contiguous float32 of shape %s" % (i, shape))
-            items[i] = SsSource(x=x.ctypes.data, rir=h.ctypes.data, out=out.ctypes.data,
+            items[i] = SsSource(x=x.ctypes.data, rir=h.ctypes.data if h is not None else None, out=out.ctypes.data,
                                 bounds=bounds.ctypes.data if bounds is not None else None,
                                 N=N, P=P, C=C, L=L, mode=mode, flags=flags,
                                 out_direct=dout.ctypes.data if dout is not None else None,
-                                direct_taps=int(s.direct_taps), win_start=ws, win_len=wl)
-            keep.append((x, h, bounds, out, dout))
+                                direct_taps=int(s.direct_taps), win_start=ws, win_len=wl,
+                                rir_bank=_bank_of(self, s, i, P, C, L) if rb is not None else None)
+            keep.append((x, h, bounds, out, dout, rb))
             results.append(out)
             if post is not None and lufs_targets[i] is not None:
                 if s.window is not None:
@@ -138,7 +270,7 @@ class Renderer:
                                      n_e=len(brk) - 1, n_blocks=len(blo), rate=float(sr), block_size=float(block),
                                      target_lufs=float(lufs_targets[i]), result=results_l[i].ctypes.data)
                 keep.append((brk, blo, bhi))
-        return HostPlan(self, items, post, n, results, results_l, keep)
+        return HostPlan(self, items, post, n, results, results_l, keep, sources)
 
     def render_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
                     outs: T.Optional[T.Sequence[np.ndarray]] = None,
@@ -209,19 +341,28 @@ class Renderer:
             chk(s.dry, "dry", i, torch.float32)
             N = s.dry.numel()
             ws, wl, n_out = _window(s, i, N)
+            rb = s.rir if isinstance(s, StaticSource) else s.rirs
+            rb = rb if isinstance(rb, RirBank) else None
             if isinstance(s, StaticSource):
-                chk(s.rir, "rir", i, torch.float32)
-                if s.rir.dim() != 2:
-                    raise ValueError("plan_device: rir of static source %d must be (C, L)" % i)
-                C, L = s.rir.shape
+                if rb is None:
+                    chk(s.rir, "rir", i, torch.float32)
+                    if s.rir.dim() != 2:
+                        raise ValueError("plan_device: rir of static source %d must be (C, L)" % i)
+                    C, L = s.rir.shape
+                else:
+                    C, L = rb.pcl[1:]
                 chk(outs[i], "out", i, torch.float32, (C, n_out))
-                items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rir.data_ptr(), out=outs[i].data_ptr(),
-                                    N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC)
+                items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rir.data_ptr() if rb is None else None,
+                                    out=outs[i].data_ptr(), N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC)
+                P = 1
             else:
-                chk(s.rirs, "rirs", i, torch.float32)
-                if s.rirs.dim() != 3:
-                    raise ValueError("plan_device: rirs of moving source %d must be (P, C, L)" % i)
-                P, C, L = s.rirs.shape
+                if rb is None:
+                    chk(s.rirs, "rirs", i, torch.float32)
+                    if s.rirs.dim() != 3:
+                        raise ValueError("plan_device: rirs of moving source %d must be (P, C, L)" % i)
+                    P, C, L = s.rirs.shape
+                else:
+                    P, C, L = rb.pcl
                 chk(outs[i], "out", i, torch.float32, (C, n_out))
                 chk(s.bounds, "bounds", i, torch.int32, (P,))
                 bh = None
@@ -230,9 +371,11 @@ class Renderer:
                     if bh.shape != (P,):
                         raise ValueError("plan_device: bounds_host of source %d must have P entries" % i)
                     keep.append(bh)
-                items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rirs.data_ptr(), out=outs[i].data_ptr(),
-                                    bounds=s.bounds.data_ptr(), N=N, P=P, C=C, L=L,
+                items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rirs.data_ptr() if rb is None else None,
+                                    out=outs[i].data_ptr(), bounds=s.bounds.data_ptr(), N=N, P=P, C=C, L=L,
                                     mode=_lib.SS_MOVING_BOUNDS, bounds_host=bh.ctypes.data if bh is not None else None)
+            if rb is not None:
+                items[i].rir_bank = _bank_of(self, s, i, P, C, L)
             items[i].flags = _flags(s, i, direct_outs[i])
             items[i].win_start, items[i].win_len = ws, wl
             if direct_outs[i] is not None:
@@ -280,6 +423,7 @@ class DevicePlan:
         self._plan = ctypes.c_void_p()
         if n > 0:
             _lib.check(renderer.lib.ss_plan_create(renderer.ctx, items, n, ctypes.byref(self._plan)))
+        self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
         """Asynchronous on `stream` (default: torch's current stream)."""
@@ -297,6 +441,8 @@ class DevicePlan:
         if self._plan:
             self.renderer.lib.ss_plan_destroy(self._plan)
             self._plan = ctypes.c_void_p()
+        if getattr(self, "_banks", None) is not None:
+            self._banks()                      # the plan no longer reads its banks: a closed one may be freed now
 
     def __del__(self):
         try:
@@ -308,9 +454,10 @@ class DevicePlan:
 class HostPlan:
     """A validated batch bound to its host input / output buffers (Renderer.plan_host)."""
 
-    def __init__(self, renderer, items, post, n, results, results_l, keep):
+    def __init__(self, renderer, items, post, n, results, results_l, keep, sources=()):
         self.renderer, self.items, self.post, self.n = renderer, items, post, n
         self.results, self.results_l, self._keep = results, results_l, keep
+        self._banks = _hold_banks(self, sources)
 
     def run(self) -> T.List[np.ndarray]:
         """H2D -> render [-> loudness] -> D2H of the whole batch; returns the (C, N) output arrays."""
