@@ -277,6 +277,15 @@ typedef struct {
                                  n[e] = (s[e-D] + s[e+D]) + s[e]  (enhancement/.../movingdatamodule.py:34-48,240) */
 } ss_mix_item;
 
+/* Limits, each checked before any copy or launch, with the outputs left untouched:
+ *   - 1 <= S <= 8 and 1 <= M <= 8 (more: SS_ERR_UNSUPPORTED); sirs may be NULL only when S == 1, and
+ *     E <= UINT64_MAX / 32, so that every range's byte size is representable (SS_ERR_INVALID);
+ *   - ss_mix_dev takes at most 65535 items per call (more: SS_ERR_UNSUPPORTED);
+ *   - within an item, every range the call writes - mix (E floats), scratch and a separate speakers_out (S * E
+ *     floats) - overlaps no other range of the item (speakers, noises, sirs, mix, scratch, speakers_out); the one
+ *     exception is speakers_out == speakers exactly, which scales the speakers in place (SS_ERR_INVALID);
+ *   - across items (not checked): no item writes into a range another item of the same call reads or writes, and
+ *     every item has its own scratch. */
 int64_t ss_mix_scratch_doubles(void);
 int ss_mix_dev(ss_ctx* ctx, const ss_mix_item* items, int n_items, void* stream);      /* device pointers, async */
 int ss_mix_host(ss_ctx* ctx, const float* speakers, const float* noises, const float* sirs, float snr,
@@ -285,7 +294,8 @@ int ss_mix_host_ex(ss_ctx* ctx, const float* speakers, const float* noises, cons
                    float* mix, float* speakers_out, int32_t S, int32_t M, int64_t E, int32_t noise_delay);
 
 /* overlap_audio (enhancement/look2hear/datas/movingdatamodule.py:34-48): y[r][n] = (x[r][n-D] + x[r][n+D]) + x[r][n],
- * zeros outside [0, T); x != y. */
+ * zeros outside [0, T).  [x, x + rows * T) and [y, y + rows * T) must not overlap (SS_ERR_INVALID: a thread would
+ * read x[n +- D] that another thread is writing); rows <= 65535 (more: SS_ERR_UNSUPPORTED). */
 int ss_overlap_dev(ss_ctx* ctx, const float* x, float* y, int32_t rows, int64_t T, int64_t delay, void* stream);
 int ss_overlap_host(ss_ctx* ctx, const float* x, float* y, int32_t rows, int64_t T, int64_t delay);
 
@@ -304,7 +314,10 @@ typedef struct {
     int32_t orig, new_rate;   /* sample rates divided by their gcd (Resample.orig_freq / gcd, new_freq / gcd)    */
     int32_t width, taps;      /* Resample.width; taps = 2 * width + orig                                         */
 } ss_dry_clip;
-/* zero-fills out[0, total) and adds every clip; device pointers, asynchronous on `stream` */
+/* zero-fills out[0, total) and adds every clip; device pointers, asynchronous on `stream`.  Before any copy or launch,
+ * leaving `out` untouched: the destination ranges [dst_start, dst_start + count) of the clips must not overlap
+ * (SS_ERR_INVALID: clips are added from different CTAs without atomics; touching ranges and count = 0 are fine), and
+ * n_clips <= 65535 (more: SS_ERR_UNSUPPORTED). */
 int ss_dry_assemble_dev(ss_ctx* ctx, const ss_dry_clip* clips, int n_clips, float* out, int64_t total, void* stream);
 
 /* Counters since ss_create / ss_reset_stats: kernels launched and device time is NOT measured

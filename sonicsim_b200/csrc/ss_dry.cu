@@ -12,6 +12,9 @@
 // clips agree to rounding (~1e-7 relative), un-resampled ones bit for bit.
 #include <string.h>
 
+#include <algorithm>
+#include <utility>
+
 #include "ss_internal.h"
 
 namespace {
@@ -54,8 +57,9 @@ __global__ void __launch_bounds__(256) k_dry_assemble(const DryClip* __restrict_
 
 extern "C" int ss_dry_assemble_dev(ss_ctx* c, const ss_dry_clip* clips, int n_clips, float* out, int64_t total, void* stream_) {
     if (!c || !out || total <= 0 || n_clips < 0 || (n_clips > 0 && !clips)) return SS_ERR_INVALID;
+    if (n_clips > 65535) return SS_ERR_UNSUPPORTED;             // one gridDim.y row per clip
     cudaStream_t stream = (cudaStream_t)stream_;
-    CK(cudaSetDevice(c->device));
+    std::vector<std::pair<int64_t, int64_t>> ranges;            // destination [start, end) of every non-empty clip
     for (int i = 0; i < n_clips; ++i) {
         const ss_dry_clip& k = clips[i];
         if (!k.src || k.channels < 1 || k.channels > 2 || k.src_len <= 0 || k.count < 0) return SS_ERR_INVALID;
@@ -65,7 +69,13 @@ extern "C" int ss_dry_assemble_dev(ss_ctx* c, const ss_dry_clip* clips, int n_cl
             const int64_t res_len = ((int64_t)k.new_rate * k.src_len + k.orig - 1) / k.orig;      // ceil(new * len / orig)
             if (k.src_start + k.count > res_len) return SS_ERR_INVALID;
         } else if (k.src_start + k.count > k.src_len) return SS_ERR_INVALID;
+        if (k.count > 0) ranges.emplace_back(k.dst_start, k.dst_start + k.count);
     }
+    // clips add onto the stream from different CTAs without atomics, so no two may write the same sample
+    std::sort(ranges.begin(), ranges.end());
+    for (size_t i = 1; i < ranges.size(); ++i)
+        if (ranges[i].first < ranges[i - 1].second) return SS_ERR_INVALID;
+    CK(cudaSetDevice(c->device));
     CK(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)total, stream));
     if (n_clips == 0) return SS_OK;
     const size_t bytes = sizeof(DryClip) * (size_t)n_clips;

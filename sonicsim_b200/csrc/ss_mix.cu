@@ -12,6 +12,7 @@ namespace {
 
 constexpr int kMixBlocks = 64;        // partial sums per mixture
 constexpr int kMaxStems = 8;
+constexpr uint64_t kMaxE = UINT64_MAX / 4 / kMaxStems;   // so that the byte size of any (S, E) or (M, E) block fits
 
 struct MixItem {
     const float* spk;      // (S, E)
@@ -200,20 +201,46 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
     }
 }
 
+// true when the byte ranges [a, a + na) and [b, b + nb) share a byte
+bool ranges_meet(const void* a, size_t na, const void* b, size_t nb) {
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return na > 0 && nb > 0 && x < y + nb && y < x + na;
+}
+
+// The kernels read an item's inputs while other CTAs write its outputs, so every range an item writes (mix, scratch,
+// a separate speakers_out) must meet no other range of the item; speakers_out may instead be exactly `speakers`.
+bool mix_item_disjoint(const ss_mix_item& a) {
+    const bool alias = a.speakers_out == a.speakers;
+    struct R { const void* p; size_t n; bool written; } r[6] = {
+        {a.speakers, 4 * (size_t)a.S * a.E, alias},
+        {a.noises, 4 * (size_t)a.M * a.E, false},
+        {a.sirs, 4 * (size_t)(a.S - 1), false},
+        {a.mix, 4 * (size_t)a.E, true},
+        {a.scratch, 8 * (size_t)(kMixBlocks * (kMaxStems + 2) + kMaxStems + 1), true},
+        {alias ? nullptr : a.speakers_out, a.speakers_out && !alias ? 4 * (size_t)a.S * a.E : 0, true}};
+    for (int i = 0; i < 6; ++i)
+        for (int j = i + 1; j < 6; ++j)
+            if ((r[i].written || r[j].written) && ranges_meet(r[i].p, r[i].n, r[j].p, r[j].n)) return false;
+    return true;
+}
+
 }  // namespace
 
 extern "C" int ss_mix_dev(ss_ctx* c, const ss_mix_item* items, int n_items, void* stream_) {
     if (!c || (!items && n_items > 0) || n_items < 0) return SS_ERR_INVALID;
     if (n_items == 0) return SS_OK;
-    CK(cudaSetDevice(c->device));
-    cudaStream_t stream = (cudaStream_t)stream_;
+    if (n_items > 65535) return SS_ERR_UNSUPPORTED;             // one gridDim.y row per item
     for (int i = 0; i < n_items; ++i) {
         const ss_mix_item& a = items[i];
         if (!a.speakers || !a.noises || !a.mix || !a.scratch || a.E <= 0 || a.S < 1 || a.M < 1) return SS_ERR_INVALID;
         if (a.S > kMaxStems || a.M > kMaxStems) return SS_ERR_UNSUPPORTED;
+        if ((uint64_t)a.E > kMaxE) return SS_ERR_INVALID;
         if (a.S > 1 && !a.sirs) return SS_ERR_INVALID;
         if (a.noise_delay < 0) return SS_ERR_INVALID;
+        if (!mix_item_disjoint(a)) return SS_ERR_INVALID;
     }
+    CK(cudaSetDevice(c->device));
+    cudaStream_t stream = (cudaStream_t)stream_;
     const size_t bytes = align_up(sizeof(MixItem) * n_items, 16);
     int slot; char *hblk, *dblk;
     { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
@@ -243,6 +270,8 @@ extern "C" int64_t ss_mix_scratch_doubles(void) { return (int64_t)kMixBlocks * (
 extern "C" int ss_mix_host_ex(ss_ctx* c, const float* speakers, const float* noises, const float* sirs, float snr,
                               float* mix, float* speakers_out, int32_t S, int32_t M, int64_t E, int32_t noise_delay) {
     if (!c || !speakers || !noises || !mix || S < 1 || M < 1 || E <= 0 || noise_delay < 0) return SS_ERR_INVALID;
+    if (S > kMaxStems || M > kMaxStems) return SS_ERR_UNSUPPORTED;       // ss_mix_dev's limits, before any upload
+    if ((uint64_t)E > kMaxE || (S > 1 && !sirs)) return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     const size_t o_spk = 0, o_noise = align_up(4 * (size_t)S * E, 256), o_mix = o_noise + align_up(4 * (size_t)M * E, 256);
     const size_t o_sir = o_mix + align_up(4 * (size_t)E, 256), o_scr = o_sir + 256;
@@ -295,6 +324,10 @@ extern "C" int ss_overlap_dev(ss_ctx* c, const float* x, float* y, int32_t rows,
     if (!c || !x || !y || x == y || rows < 0 || T < 0 || delay < 0) return SS_ERR_INVALID;
     if (rows == 0 || T == 0) return SS_OK;
     if (rows > 65535) return SS_ERR_UNSUPPORTED;
+    // k_overlap reads x[n +- D] that other threads may be writing when y overlaps x
+    if ((uint64_t)T > UINT64_MAX / 4 / (uint64_t)rows) return SS_ERR_INVALID;
+    const size_t bytes = 4 * (size_t)rows * (size_t)T;
+    if (ranges_meet(x, bytes, y, bytes)) return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     long long nb = (T + 255) / 256;
     if (nb > 8ll * c->sm_count) nb = 8ll * c->sm_count;   // 8 waves of CTAs, grid-stride beyond that

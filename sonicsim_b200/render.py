@@ -528,7 +528,9 @@ def render_mixtures(utterances: T.Sequence[dict], device: T.Optional[int] = None
                  "noises":   [(dry (N,), rir (C, L)), ...],
                  "sirs": (S-1,) dB, "snr": dB}
     Returns per utterance {"mix": (C, N) float32, "speakers": (S, C, N) float32 (after their gains)}.
-    Every stem of an utterance must have the same (C, N)."""
+    Every stem of an utterance must have the same (C, N).  Each speaker's trajectory goes through trajectory_bounds,
+    which draws from the global NumPy RNG like the reference, so identical calls give identical bits only from the
+    same NumPy RNG state."""
     import torch
     from ._lib import SsMixItem
     R = default_renderer() if device is None else Renderer(device)
