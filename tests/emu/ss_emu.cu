@@ -176,51 +176,59 @@ static void cta_render(const RItem* items, int n_items, int cta, int grid, const
 
 // One persistent k_render_fast CTA: the kernel's control flow with the split barriers collapsed (every phase runs for all
 // threads before the next starts) and the bulk copies / item prefetches done at the points where the kernel issues them.
+// As in the kernel: the CTA renders a contiguous range of items (per / rem), the filter spectra Hp, Hq land in the FFT
+// buffer and the dry spectrum X in its own buffer behind it, X is copied only when the next item belongs to another
+// block, and the inter-pass twiddles come from tw_get.
 static void cta_render_fast(const RItem* items, int n_items, int cta, int grid, const Tables& T) {
     std::vector<float2> smem(kPadF + kSpec);
     std::vector<Regs32> R(kThreads);
     float2* const fftbuf = smem.data();
-    float2* const sX = fftbuf;
-    float2* const sHp = fftbuf + kSpec;
-    float2* const sHq = fftbuf + kPadF;
-    const int n_k = (n_items - cta + grid - 1) / grid;
+    float2* const sHp = fftbuf;
+    float2* const sHq = fftbuf + kSpec;
+    float2* const sX = fftbuf + kPadF;
+    const int per = n_items / grid, rem = n_items % grid;
+    const int n_k = per + (cta < rem ? 1 : 0);
     if (n_k <= 0) return;
-    const RItem* my_items = items + cta;
+    const RItem* my_items = items + (size_t)cta * per + (cta < rem ? cta : rem);
     RItem s_item[3];
     s_item[0] = my_items[0];
-    if (n_k > 1) s_item[1] = my_items[grid];
+    if (n_k > 1) s_item[1] = my_items[1];
     {
-        memcpy(sX, s_item[0].X, sizeof(float2) * kSpec);
         memcpy(sHp, item_hp(s_item[0]), sizeof(float2) * kSpec);
         memcpy(sHq, item_hq(s_item[0]), sizeof(float2) * kSpec);
+        memcpy(sX, s_item[0].X, sizeof(float2) * kSpec);
     }
     XDesc unused; memset(&unused, 0, sizeof(unused)); unused.kparts = 1;
     std::vector<float2> w(kThreads * 16);
     for (int k = 0; k < n_k; ++k) {
         for (int t = 0; t < kThreads; ++t) form_z<false, true>(t, sX, sHp, sHq, unused, R[t]);
         for (int t = 0; t < kThreads; ++t) { fft16<true>(R[t].a); fft16<true>(R[t].b); }
+        // B1 (kItemLane): the next item's X only if it belongs to another block; item k + 2 into the ring
         if (k + 1 < n_k) {
             const RItem& nx = s_item[(k + 1) % 3];
-            memcpy(sHq, item_hq(nx), sizeof(float2) * kSpec);
+            if (nx.X != s_item[k % 3].X) memcpy(sX, nx.X, sizeof(float2) * kSpec);
         }
-        if (k + 2 < n_k) s_item[(k + 2) % 3] = my_items[(size_t)(k + 2) * grid];
+        if (k + 2 < n_k) s_item[(k + 2) % 3] = my_items[k + 2];
         for (int t = 0; t < kThreads; ++t) { passA_store(fftbuf, passA_jA(t), R[t].a); passA_store(fftbuf, passA_jB(t), R[t].b); }
         for (int t = 0; t < kThreads; ++t) load2(t, fftbuf, R[t]);
         for (int t = 0; t < kThreads; ++t) {
             float2 (&wt)[16] = *reinterpret_cast<float2 (*)[16]>(&w[16 * t]);
-            tw_load<true, 16>(T.twB + (t & 15), wt);
+            tw_get<true, 16>(T.twB + (t & 15), wt);
             fft16_w<true>(R[t].a, wt); fft16_w<true>(R[t].b, wt);
         }
         for (int t = 0; t < kThreads; ++t) { passB_store(fftbuf, t, R[t].a); passB_store(fftbuf, t + 256, R[t].b); }
-        for (int t = 0; t < kThreads; ++t) load2(t, fftbuf, R[t]);
-        if (k + 1 < n_k) {
+        for (int t = 0; t < kThreads; ++t) {
+            load2(t, fftbuf, R[t]);
+            float2 (&wt)[16] = *reinterpret_cast<float2 (*)[16]>(&w[16 * t]);
+            tw_get<true, 256>(T.twC + t, wt);
+        }
+        if (k + 1 < n_k) {                          // last warp out of the FFT buffer: Hp, Hq of transform k + 1 into it
             const RItem& nx = s_item[(k + 1) % 3];
-            memcpy(sX, nx.X, sizeof(float2) * kSpec);
             memcpy(sHp, item_hp(nx), sizeof(float2) * kSpec);
+            memcpy(sHq, item_hq(nx), sizeof(float2) * kSpec);
         }
         for (int t = 0; t < kThreads; ++t) {
             float2 (&wt)[16] = *reinterpret_cast<float2 (*)[16]>(&w[16 * t]);
-            tw_load<true, 256>(T.twC + t, wt);
             fft16_w<true>(R[t].a, wt); fft16_w<true>(R[t].b, wt);
             render_phase3_close(t, R[t], T);
             render_epilogue_item(t, s_item[k % 3], R[t]);
