@@ -50,115 +50,81 @@ __device__ float2 g_twB[kTabB];      // [r][k] exp(-2 pi i k r / 256)
 __device__ float2 g_twC[kTabC];      // [r][k] exp(-2 pi i k r / 4096)
 
 // ----------------------------------------------------------------------------- k_blocks
-// Windowed source (one warp): the blocks [g0, g1) of the full plan (window_span) and the kept range.  Aligned blocking
-// walks the segments twice - once to find the full-table indices of the blocks holding the window's first and last
-// samples, once to write the blocks in [g0, g1) - so the table never holds the full plan.
-__device__ void blocks_window(const Source& S, int lane) {
+// One warp walks the aligned segments of S, 32 at a time: body(sg, b0, n_s, first) for every segment [b0, b0 + n_s)
+// that has blocks, `first` = full-plan index of its first block (inclusive shuffle sum of seg_blocks).  Returns the
+// full plan's block count.
+template <class Body>
+__device__ int seg_scan(const Source& S, int lane, Body body) {
+    int carry = 0;
+    for (int base = 0; base < S.P - 1; base += 32) {
+        const int sg = base + lane;
+        const int b0 = sg < S.P - 1 ? S.bounds[sg] : 0;
+        const int n_s = sg < S.P - 1 ? S.bounds[sg + 1] - b0 : 0;
+        const int cnt = n_s > 0 ? seg_blocks(n_s) : 0;
+        int incl = cnt;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+        if (cnt > 0) body(sg, b0, n_s, carry + incl - cnt);
+        carry += __shfl_sync(0xffffffffu, incl, 31);
+    }
+    return carry;
+}
+
+// Windowed source: the full-plan blocks holding the window's first and last samples, then window_span.  The table never
+// holds the full plan.
+__device__ WinSpan window_blocks_dev(const Source& S, int lane) {
     const int ws = S.counts[4], we = ws + S.counts[5];
-    int k0, k1, nfull;
+    if (!S.aligned) return window_span(ws / kB, (we + kB - 1) / kB, S.nb, S.K);
+    int f0 = -1, f1 = -1;
+    const int nfull = seg_scan(S, lane, [&](int sg, int b0, int n_s, int first) {
+        if (ws >= b0 && ws < b0 + n_s) f0 = first + (ws - b0) / kB;
+        if (we - 1 >= b0 && we - 1 < b0 + n_s) f1 = first + (we - 1 - b0) / kB;
+    });
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        f0 = max(f0, __shfl_xor_sync(0xffffffffu, f0, o));
+        f1 = max(f1, __shfl_xor_sync(0xffffffffu, f1, o));
+    }
+    const int k0 = f0 < 0 ? 0 : f0;               // (-1: a bounds table outside the contract; keep the writes in range)
+    return window_span(k0, f1 < k0 ? k0 + 1 : f1 + 1, nfull, S.K);
+}
+
+// The full plan's blocks [g0, g1) into the table (one warp), the rest of the table cleared, 1 / n_s table, counts[0].
+__device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
+    int nfull = S.nb;
     if (S.aligned) {
-        int carry = 0, f0 = -1, f1 = -1;
-        for (int base = 0; base < S.P - 1; base += 32) {
-            const int sg = base + lane;
-            const int b0 = sg < S.P - 1 ? S.bounds[sg] : 0;
-            const int n_s = sg < S.P - 1 ? S.bounds[sg + 1] - b0 : 0;
-            const int cnt = n_s > 0 ? seg_blocks(n_s) : 0;
-            int incl = cnt;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-            const int first = carry + incl - cnt;
-            if (cnt > 0 && ws >= b0 && ws < b0 + n_s) f0 = first + (ws - b0) / kB;
-            if (cnt > 0 && we - 1 >= b0 && we - 1 < b0 + n_s) f1 = first + (we - 1 - b0) / kB;
-            carry += __shfl_sync(0xffffffffu, incl, 31);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            f0 = max(f0, __shfl_xor_sync(0xffffffffu, f0, o));
-            f1 = max(f1, __shfl_xor_sync(0xffffffffu, f1, o));
-        }
-        nfull = carry;
-        k0 = f0 < 0 ? 0 : f0;                     // (-1: a bounds table outside the contract; keep the writes in range)
-        k1 = f1 < k0 ? k0 + 1 : f1 + 1;
+        nfull = seg_scan(S, lane, [&](int sg, int b0, int n_s, int first) {
+            for (int q = 0; q < seg_blocks(n_s); ++q)
+                if (first + q >= g0 && first + q < g1) S.blocks[first + q - g0] = seg_block(b0, n_s, q, sg);
+        });
     } else {
-        nfull = S.nb; k0 = ws / kB; k1 = (we + kB - 1) / kB;
+        for (int bi = g0 + lane; bi < g1 && bi < S.nb; bi += 32) S.blocks[bi - g0] = grid_block(S.N, bi);
     }
-    const WinSpan w = window_span(k0, k1, nfull, S.K);
-    const int g1 = w.g1 - w.g0 > S.nblk_max ? w.g0 + S.nblk_max : w.g1;
-    if (S.aligned) {
-        int carry = 0;
-        for (int base = 0; base < S.P - 1; base += 32) {
-            const int sg = base + lane;
-            const int b0 = sg < S.P - 1 ? S.bounds[sg] : 0;
-            const int n_s = sg < S.P - 1 ? S.bounds[sg + 1] - b0 : 0;
-            const int cnt = n_s > 0 ? seg_blocks(n_s) : 0;
-            int incl = cnt;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-            const int first = carry + incl - cnt;
-            for (int q = 0; q < cnt; ++q) {
-                if (first + q < w.g0 || first + q >= g1) continue;
-                Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
-                S.blocks[first + q - w.g0] = bk;
-            }
-            carry += __shfl_sync(0xffffffffu, incl, 31);
-        }
-    } else {
-        for (int bi = w.g0 + lane; bi < g1; bi += 32) {
-            Block bk; bk.start = bi * kB; bk.len = S.N - bi * kB < kB ? S.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
-            S.blocks[bi - w.g0] = bk;
-        }
-    }
-    for (int bi = g1 - w.g0 + lane; bi < S.nblk_max; bi += 32) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; S.blocks[bi] = z; }
-    if (lane == 0) {
-        S.counts[0] = g1 - w.g0;
-        S.counts[2] = w.k0 - w.g0;
-        S.counts[3] = (w.k1 < g1 ? w.k1 : g1) - w.k0;
-    }
+    const int nblk = (g1 < nfull ? g1 : nfull) - g0;
+    clear_blocks(S.blocks, nblk, S.nblk_max, lane, 32);
+    if (S.mode == MODE_MOVING_BOUNDS) fill_rstep(S.bounds, S.P, S.rstep, lane, 32);
+    if (lane == 0) S.counts[0] = nblk;
 }
 
 // One small CTA per chunk: block table of every source (one warp per source), 1 / n_s table, then the
-// exclusive scan that packs the render work items of all sources into one dense table.
+// exclusive scan that packs the render work items of all sources into one dense table.  A whole source's table is the
+// full plan; a windowed one's holds the full plan's blocks [g0, g1) (window_span, cut to the table size).
 __global__ void __launch_bounds__(256)
 k_blocks(const Source* __restrict__ srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     for (int si = warp; si < n_src; si += nwarps) {
         const Source& S = srcs[si];
-        int nblk;
+        int g0 = 0, g1 = S.nblk_max;
         if (S.h_rows) {
-            blocks_window(S, lane);
-            if (S.mode == MODE_MOVING_BOUNDS)
-                for (int sg = lane; sg < S.P - 1; sg += 32) S.rstep[sg] = 1.0 / (double)(S.bounds[sg + 1] - S.bounds[sg]);
-            continue;
-        }
-        if (S.aligned) {
-            int carry = 0;
-            for (int base = 0; base < S.P - 1; base += 32) {
-                const int sg = base + lane;
-                const int b0 = sg < S.P - 1 ? S.bounds[sg] : 0;
-                const int n_s = sg < S.P - 1 ? S.bounds[sg + 1] - b0 : 0;
-                const int cnt = seg_blocks(n_s);
-                int incl = cnt;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-                const int first = carry + incl - cnt;
-                for (int q = 0; q < cnt; ++q) {
-                    Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
-                    S.blocks[first + q] = bk;
-                }
-                carry += __shfl_sync(0xffffffffu, incl, 31);
-            }
-            nblk = carry;
-        } else {
-            nblk = S.nb;
-            for (int bi = lane; bi < nblk; bi += 32) {
-                Block bk; bk.start = bi * kB; bk.len = S.N - bi * kB < kB ? S.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
-                S.blocks[bi] = bk;
+            const WinSpan w = window_blocks_dev(S, lane);
+            g0 = w.g0;
+            g1 = w.g1 - w.g0 > S.nblk_max ? w.g0 + S.nblk_max : w.g1;
+            if (lane == 0) {
+                S.counts[2] = w.k0 - w.g0;
+                S.counts[3] = (w.k1 < g1 ? w.k1 : g1) - w.k0;
             }
         }
-        for (int bi = nblk + lane; bi < S.nblk_max; bi += 32) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; S.blocks[bi] = z; }
-        if (S.mode == MODE_MOVING_BOUNDS)
-            for (int sg = lane; sg < S.P - 1; sg += 32) S.rstep[sg] = 1.0 / (double)(S.bounds[sg + 1] - S.bounds[sg]);
-        if (lane == 0) S.counts[0] = nblk;
+        write_blocks(S, lane, g0, g1);
     }
     __syncthreads();
     if (warp == 0) {
@@ -271,7 +237,7 @@ k_prepare(const Source* __restrict__ srcs_g, const int* __restrict__ prefix_g, i
     if (local >= nh + nx) {
         const int blk = (local - nh - nx) * 8 + (t >> 5), lane = t & 31;
         if (blk >= S.counts[0]) return;
-        Block bk = S.blocks[blk];
+        const Block bk = S.blocks[blk];
         if (S.mode == MODE_MOVING_BOUNDS && !S.aligned && blk == 0 && lane == 0) {
             // one warp per source checks the device-side bounds table
             bool bad = S.bounds[0] != 0 || S.bounds[S.P - 1] != S.N;
@@ -279,23 +245,18 @@ k_prepare(const Source* __restrict__ srcs_g, const int* __restrict__ prefix_g, i
             if (bad) atomicOr(&g_dev_err, 2u);
         }
         if ((unsigned)(blk - win_first(S)) >= (unsigned)win_blocks(S)) return;     // windowed: block outside the window
-        if (S.mode == MODE_MOVING_BOUNDS && !S.aligned) {
-            bk.p_lo = seg_of(S.bounds, S.P - 1, bk.start);
-            bk.p_hi = seg_of(S.bounds, S.P - 1, bk.start + bk.len - 1) + 1;
-        } else if (S.mode == MODE_MOVING_INDEXED) {
-            int pmin = 0x7fffffff, pmax = -1;
-            for (int n = bk.start + lane; n < bk.start + bk.len; n += 32) { int v = S.idx[n]; pmin = v < pmin ? v : pmin; pmax = v > pmax ? v : pmax; }
+        int pmin = 0, pmax = 0;
+        if (S.mode == MODE_MOVING_INDEXED) {
+            block_pos_scan(S, bk, lane, 32, pmin, pmax);
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
                 int a = __shfl_xor_sync(0xffffffffu, pmin, o), bm = __shfl_xor_sync(0xffffffffu, pmax, o);
                 pmin = a < pmin ? a : pmin; pmax = bm > pmax ? bm : pmax;
             }
-            // the reference raises IndexError for idx + 1 >= P (checked on the host path); clamp here, leave a mark
+            // the reference raises IndexError for idx + 1 >= P (checked on the host path); block_positions clamps, leave a mark
             if (lane == 0 && (pmin < 0 || pmax + 1 > S.P - 1)) atomicOr(&g_dev_err, 1u);
-            bk.p_lo = pmin < 0 ? 0 : pmin;
-            bk.p_hi = pmax + 1 > S.P - 1 ? S.P - 1 : pmax + 1;
         }
-        fill_items(S, items, blk, bk, lane, 32);
+        fill_items(S, items, blk, block_positions(S, bk, pmin, pmax), lane, 32);
         return;
     }
     if (local < nh) rows_of_pair_h(S, local, ra, rb);
@@ -902,27 +863,6 @@ static bool choose_aligned(const ss_source& it, int K, int nb) {
     }
     return aligned <= grid;
 }
-// The full plan's blocks in use (aligned: from the host-side bounds `hb`), ascending; returns their number.  Writes at
-// most `cap` blocks (nb + P - 1 for a bounds table ascending from 0 to N; a table outside that contract stops there).
-static int full_blocks(const ss_source& it, int aligned, int nb, const int32_t* hb, Block* blocks, int cap) {
-    int nblk = 0;
-    if (aligned) {
-        for (int sg = 0; sg < it.P - 1; ++sg) {
-            const int b0 = hb[sg], n_s = hb[sg + 1] - b0;
-            for (int q = 0; q < seg_blocks(n_s) && nblk < cap; ++q) {
-                Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
-                blocks[nblk++] = bk;
-            }
-        }
-    } else {
-        nblk = nb;
-        for (int bi = 0; bi < nblk; ++bi) {
-            Block bk; bk.start = bi * kB; bk.len = it.N - bi * kB < kB ? it.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
-            blocks[bi] = bk;
-        }
-    }
-    return nblk;
-}
 // Window of a windowed source: which blocks, RIR rows, dry samples and trajectory entries it uses (its read set, see
 // include/sonicsim_b200.h).  The blocking itself is the full source's (choose_aligned over the whole trajectory).
 static void window_shape(const ss_source& it, Shape& s) {
@@ -932,8 +872,9 @@ static void window_shape(const ss_source& it, Shape& s) {
     s.tab_host = !s.aligned || hb != nullptr;
     int pa = 0, pb = it.P - 1;                           // all positions unless the trajectory is visible here
     if (s.tab_host) {
+        // (a bounds table outside the contract - ascending from 0 to N - may plan more blocks than the table holds)
         std::vector<Block> full((size_t)s.nblk_max);
-        const int n = full_blocks(it, s.aligned, s.nb, hb, full.data(), s.nblk_max);
+        const int n = std::min(plan_blocks(s.aligned, hb, it.P, it.N, s.nb, 0, s.nblk_max, full.data()), s.nblk_max);
         const WinSpan w = window_blocks(full.data(), n, ws, we, s.K);
         if (w.k0 < w.k1) {
             s.g0 = w.g0; s.g1 = w.g1; s.k0 = w.k0; s.k1 = w.k1;
@@ -965,7 +906,7 @@ static Shape shape_of(const ss_source& it) {
     memset(&s, 0, sizeof(s));
     s.K = (it.L + kB - 1) / kB; s.nb = (it.N + kB - 1) / kB;
     s.aligned = choose_aligned(it, s.K, s.nb) ? 1 : 0;
-    s.nblk_max = s.aligned ? s.nb + it.P - 1 : s.nb;
+    s.nblk_max = table_cap(s.aligned, s.nb, it.P);
     s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
     if (it.win_len > 0) window_shape(it, s);
     s.max_items = s.nblk_max * s.per;
@@ -984,18 +925,10 @@ static size_t spectra_bytes(const ss_source& it) {
 // Host-side twin of k_blocks for one source whose trajectory bounds are visible on the host.
 // Returns the number of blocks in use (windowed source: the full table's blocks [g0, g1)).
 static int build_blocks_host(const ss_source& it, const Shape& sh, const int32_t* hb, Block* blocks, double* rstep) {
-    int nblk = 0;
-    if (sh.win) {
-        std::vector<Block> full((size_t)(sh.aligned ? sh.nb + it.P - 1 : sh.nb));
-        full_blocks(it, sh.aligned, sh.nb, hb, full.data(), (int)full.size());
-        nblk = sh.g1 - sh.g0;
-        for (int bi = 0; bi < nblk; ++bi) blocks[bi] = full[sh.g0 + bi];
-    } else {
-        nblk = full_blocks(it, sh.aligned, sh.nb, hb, blocks, sh.nblk_max);
-    }
-    for (int bi = nblk; bi < sh.nblk_max; ++bi) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; blocks[bi] = z; }
-    if (it.mode == SS_MOVING_BOUNDS && hb)
-        for (int sg = 0; sg < it.P - 1; ++sg) rstep[sg] = 1.0 / (double)(hb[sg + 1] - hb[sg]);
+    const int g0 = sh.win ? sh.g0 : 0, g1 = sh.win ? sh.g1 : sh.nblk_max;
+    const int nblk = std::min(plan_blocks(sh.aligned, hb, it.P, it.N, sh.nb, g0, g1, blocks), g1) - g0;
+    clear_blocks(blocks, nblk, sh.nblk_max, 0, 1);
+    if (it.mode == SS_MOVING_BOUNDS && hb) fill_rstep(hb, it.P, rstep, 0, 1);
     return nblk;
 }
 

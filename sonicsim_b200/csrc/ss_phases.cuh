@@ -126,8 +126,44 @@ SS_HD int items_per_set(const Source& s) { return s.mode == MODE_STATIC ? (s.C +
 SS_HD int items_per_block(const Source& s) { return items_per_set(s) * (s.cut ? 2 : 1); }
 SS_HD int max_render_items(const Source& s) { return s.nblk_max * items_per_block(s); }
 
+// ---- the block table: one planner for the host, k_blocks and the CPU emulation.
 // blocks of one segment under aligned blocking
 SS_HD int seg_blocks(int n_s) { return (n_s + kB - 1) / kB; }
+// block q of segment sg = [b0, b0 + n_s) under aligned blocking
+SS_HD Block seg_block(int b0, int n_s, int q, int sg) {
+    Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
+    return bk;
+}
+// block bi of an N-sample source under grid blocking (its positions are found by k_prepare's range warps)
+SS_HD Block grid_block(int N, int bi) {
+    Block bk; bk.start = bi * kB; bk.len = N - bi * kB < kB ? N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
+    return bk;
+}
+// table size of a whole source: nb (grid), nb + P - 1 (aligned: at most one partial block per waypoint)
+SS_HD int table_cap(int aligned, int nb, int P) { return aligned ? nb + P - 1 : nb; }
+// unused slots [n, cap) of a table (lane `lane` of `nlanes`)
+SS_HD void clear_blocks(Block* b, int n, int cap, int lane, int nlanes) {
+    for (int bi = n + lane; bi < cap; bi += nlanes) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; b[bi] = z; }
+}
+// 1 / (samples in segment sg) for every segment of a bounds trajectory (lane `lane` of `nlanes`)
+SS_HD void fill_rstep(const int* bounds, int P, double* rstep, int lane, int nlanes) {
+    for (int sg = lane; sg < P - 1; sg += nlanes) rstep[sg] = 1.0 / (double)(bounds[sg + 1] - bounds[sg]);
+}
+// The full plan's blocks with index in [g0, g1), written to out[0 ..]; returns the full plan's block count (whole
+// source: g0 = 0, g1 = table_cap).  Aligned blocking reads the bounds, grid blocking does not.
+SS_HD int plan_blocks(int aligned, const int* bounds, int P, int N, int nb, int g0, int g1, Block* out) {
+    if (!aligned) {
+        for (int bi = g0; bi < g1 && bi < nb; ++bi) out[bi - g0] = grid_block(N, bi);
+        return nb;
+    }
+    int n = 0;
+    for (int sg = 0; sg < P - 1; ++sg) {
+        const int b0 = bounds[sg], n_s = bounds[sg + 1] - b0;
+        for (int q = 0; q < seg_blocks(n_s); ++q, ++n)
+            if (n >= g0 && n < g1) out[n - g0] = seg_block(b0, n_s, q, sg);
+    }
+    return n;
+}
 
 // ---- time windows.  A windowed source keeps the full plan's blocking (aligned or grid, chosen over the whole
 // trajectory) and renders the blocks [k0, k1) of the full table that meet the window.  Its table holds the full
@@ -164,6 +200,25 @@ SS_HD void window_rows(int P, int C, int K, int pa, int pb, int& row0, int& rows
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
 SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }
+
+// Position range of a block (k_prepare's range warps).  Indexed source: block_pos_scan gives lane `lane` of `nlanes` the
+// min / max of idx over its share of the block's samples; block_positions takes the combined [pmin, pmax].
+SS_HD void block_pos_scan(const Source& S, const Block& bk, int lane, int nlanes, int& pmin, int& pmax) {
+    pmin = 0x7fffffff; pmax = -1;
+    for (int n = bk.start + lane; n < bk.start + bk.len; n += nlanes) { int v = S.idx[n]; pmin = v < pmin ? v : pmin; pmax = v > pmax ? v : pmax; }
+}
+// the positions block bk interpolates between: from the bounds (grid blocking), [pmin, pmax + 1] clamped to
+// [0, P - 1] (indexed), as planned otherwise (aligned blocking, static source)
+SS_HD Block block_positions(const Source& S, Block bk, int pmin, int pmax) {
+    if (S.mode == MODE_MOVING_BOUNDS && !S.aligned) {
+        bk.p_lo = seg_of(S.bounds, S.P - 1, bk.start);
+        bk.p_hi = seg_of(S.bounds, S.P - 1, bk.start + bk.len - 1) + 1;
+    } else if (S.mode == MODE_MOVING_INDEXED) {
+        bk.p_lo = pmin < 0 ? 0 : pmin;
+        bk.p_hi = pmax + 1 > S.P - 1 ? S.P - 1 : pmax + 1;
+    }
+    return bk;
+}
 
 // fill the work items of block `blk` once its position range is known (lanes split the channels).  A direct-target
 // source's block has the reverberant items first, then as many direct items (direct spectra, `out_direct`): all of

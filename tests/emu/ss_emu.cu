@@ -38,12 +38,29 @@ struct HostTables {
 };
 static const Tables& tables() { static HostTables h; return h.T; }
 
+// k_rir_absmax (all partial maxima in slot 0) and k_rir_direct, one emulated lane per row; as in the kernels, a banked
+// source (no rir) has its cuts already
+static void emu_rir_prep(const Source& S, float* norm_part) {
+    if (S.norm_part) {
+        float m = 0.f;
+        for (size_t i = 0; i < (size_t)S.P * S.C * S.L; ++i) m = fabsf(S.rir[i]) > m ? fabsf(S.rir[i]) : m;
+        for (int i = 0; i < kNormParts; ++i) norm_part[i] = i == 0 ? m : 0.f;
+    }
+    if (S.cut && S.rir) {
+        const float div = S.norm_part ? rir_absmax(S) : 0.f;
+        for (int row = 0; row < S.P * S.C; ++row)
+            S.cut[row] = direct_cut(peak_scan(S.rir + (size_t)row * S.L, S.L, div, 0, 1).i, S.L, S.direct_taps);
+    }
+}
+
+// one k_prepare spectra CTA, rows chosen as the kernel chooses them (reverberant pairs, then direct pairs, then dry
+// windows)
 static void cta_spectra(const Source& S, int local, const Tables& T) {
     std::vector<float2> smem(kPadF);
     std::vector<Regs32> R(kThreads);
     Row ra, rb;
     const int nh = spectra_pairs_h(S);
-    if (local < nh) { ra = make_row_h(S, 2 * local); rb = make_row_h(S, 2 * local + 1); }
+    if (local < nh) rows_of_pair_h(S, local, ra, rb);
     else { local -= nh; ra = make_row_x(S, 2 * local); rb = make_row_x(S, 2 * local + 1); }
     if (!ra.dst && !rb.dst) return;
     float2* s = smem.data();
@@ -55,45 +72,15 @@ static void cta_spectra(const Source& S, int local, const Tables& T) {
     for (int t = 0; t < kThreads; ++t) spectra_phase4(t, s, ra, rb);
 }
 
-// k_blocks: block table, 1 / n_s table, dense item numbering (one source here)
-static void emu_blocks(const Source& S) {
-    int nblk = 0;
-    if (S.aligned) {
-        for (int sg = 0; sg < S.P - 1; ++sg) {
-            const int b0 = S.bounds[sg], n_s = S.bounds[sg + 1] - b0;
-            for (int q = 0; q < seg_blocks(n_s); ++q) {
-                Block bk; bk.start = b0 + kB * q; bk.len = n_s - kB * q < kB ? n_s - kB * q : kB; bk.p_lo = sg; bk.p_hi = sg + 1;
-                S.blocks[nblk++] = bk;
-            }
-        }
-    } else {
-        nblk = S.nb;
-        for (int bi = 0; bi < nblk; ++bi) {
-            Block bk; bk.start = bi * kB; bk.len = S.N - bi * kB < kB ? S.N - bi * kB : kB; bk.p_lo = 0; bk.p_hi = 0;
-            S.blocks[bi] = bk;
-        }
-    }
-    for (int bi = nblk; bi < S.nblk_max; ++bi) { Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0; S.blocks[bi] = z; }
-    if (S.mode == MODE_MOVING_BOUNDS)
-        for (int sg = 0; sg < S.P - 1; ++sg) S.rstep[sg] = 1.0 / (double)(S.bounds[sg + 1] - S.bounds[sg]);
-    S.counts[0] = nblk;
-    S.counts[1] = 0;
-}
-
-// k_prepare's range CTAs: position range of every block in use + its work items
+// k_prepare's range warps: position range and work items of every block in use; a windowed source's blocks outside the
+// window get no items
 static void prepare_ranges(const Source& S, RItem* items) {
     for (int blk = 0; blk < S.counts[0]; ++blk) {
-        Block bk = S.blocks[blk];
-        if (S.mode == MODE_MOVING_BOUNDS && !S.aligned) {
-            bk.p_lo = seg_of(S.bounds, S.P - 1, bk.start);
-            bk.p_hi = seg_of(S.bounds, S.P - 1, bk.start + bk.len - 1) + 1;
-        } else if (S.mode == MODE_MOVING_INDEXED) {
-            int pmin = 0x7fffffff, pmax = -1;
-            for (int n = bk.start; n < bk.start + bk.len; ++n) { int v = S.idx[n]; pmin = v < pmin ? v : pmin; pmax = v > pmax ? v : pmax; }
-            bk.p_lo = pmin < 0 ? 0 : pmin;
-            bk.p_hi = pmax + 1 > S.P - 1 ? S.P - 1 : pmax + 1;
-        }
-        for (int lane = 0; lane < 32; ++lane) fill_items(S, items, blk, bk, lane, 32);
+        if ((unsigned)(blk - win_first(S)) >= (unsigned)win_blocks(S)) continue;
+        const Block bk = S.blocks[blk];
+        int pmin = 0, pmax = 0;
+        if (S.mode == MODE_MOVING_INDEXED) block_pos_scan(S, bk, 0, 1, pmin, pmax);
+        fill_items(S, items, blk, block_positions(S, bk, pmin, pmax), 0, 1);
     }
 }
 
@@ -236,34 +223,86 @@ static void cta_render_fast(const RItem* items, int n_items, int cta, int grid, 
     }
 }
 
-extern "C" {
-
-// Emulate k_spectra + k_render for one source.  mode: 0 static, 1 bounds, 2 (idx, w).
-int emu_render(const float* x, const float* rir, float* out, const int32_t* bounds, const int32_t* idx,
-               const float* w, int N, int P, int C, int L, int mode) {
+// The launches of one emulated source, as the library runs them: k_rir_absmax / k_rir_direct, the block table (k_blocks;
+// windowed, win_len > 0: the full plan's blocks [g0, g1) that window_blocks finds), k_prepare's spectra CTAs and range
+// warps, and the render CTAs.  aligned: the blocking plan.  rir == null: a banked source, spectra (and cuts) from
+// bank / bank_cut.  direct_taps > 0: a direct-path stem into out_direct.  restrict_rows (windowed, with rir): transform
+// only the RIR rows of the positions the window's blocks touch, else all of them.  win_stats (may be null) receives
+// [table blocks, kept blocks, first RIR row, RIR rows per set], bank_stats (may be null) [RIR pair CTAs of k_prepare,
+// dry-window pair CTAs, render items].
+static void emu_source(const float* x, const float* rir, const float2* bank, const int* bank_cut, float* out,
+                       const int32_t* bounds, const int32_t* idx, const float* w, int N, int P, int C, int L, int mode,
+                       int aligned, int win_start, int win_len, float* out_direct, int direct_taps, int normalize,
+                       int restrict_rows, int* win_stats, int* bank_stats) {
     const Tables& T = tables();
     Source S;
     memset(&S, 0, sizeof(S));
     S.x = x; S.rir = rir; S.out = out; S.bounds = bounds; S.idx = idx; S.w = w;
     S.N = N; S.P = P; S.C = C; S.L = L; S.K = (L + kB - 1) / kB; S.nb = (N + kB - 1) / kB; S.mode = mode;
-    S.aligned = (mode == MODE_MOVING_BOUNDS && S.K == 1) ? 1 : 0;
-    S.nblk_max = S.aligned ? S.nb + P - 1 : S.nb;
-    std::vector<float2> hs((size_t)P * C * S.K * kSpec), xs((size_t)S.nblk_max * kSpec);
-    std::vector<RItem> items(max_render_items(S));
+    S.aligned = aligned;
+    const bool windowed = win_len > 0;
+    S.nblk_max = table_cap(aligned, S.nb, P);
+    WinSpan ws = {0, S.nblk_max, 0, 0};
+    if (windowed) {
+        std::vector<Block> full(S.nblk_max);
+        const int nfull = plan_blocks(aligned, bounds, P, N, S.nb, 0, S.nblk_max, full.data());
+        ws = window_blocks(full.data(), nfull, win_start, win_start + win_len, S.K);
+        S.nblk_max = ws.g1 - ws.g0;
+    }
     std::vector<Block> blocks(S.nblk_max);
+    const int nfull = plan_blocks(aligned, bounds, P, N, S.nb, ws.g0, ws.g1, blocks.data());
+    const int nblk = (nfull < ws.g1 ? nfull : ws.g1) - ws.g0;
+    clear_blocks(blocks.data(), nblk, S.nblk_max, 0, 1);
     std::vector<double> rstep(P);
-    int counts[2] = {0, 0};
-    S.hspec = hs.data(); S.xspec = xs.data(); S.blocks = blocks.data(); S.rstep = rstep.data(); S.counts = counts;
-    emu_blocks(S);
+    if (mode == MODE_MOVING_BOUNDS) fill_rstep(bounds, P, rstep.data(), 0, 1);
+    int counts[8] = {nblk, 0, ws.k0 - ws.g0, ws.k1 - ws.k0, win_start, win_len, 0, 0};
+    S.blocks = blocks.data(); S.rstep = rstep.data(); S.counts = counts;
+    std::vector<float2> hs, xs((size_t)S.nblk_max * kSpec);
+    std::vector<float> norm_part(kNormParts);
+    std::vector<int> cut((size_t)P * C);
+    if (rir) {
+        if (normalize) S.norm_part = norm_part.data();
+        if (direct_taps > 0) S.cut = cut.data();
+        if (windowed) {                           // RIR positions the kept blocks interpolate between
+            int pa = 0, pb = P - 1;
+            if (mode == MODE_STATIC) pb = 0;
+            else if (restrict_rows && mode == MODE_MOVING_BOUNDS) {
+                pa = block_positions(S, blocks[counts[2]], 0, 0).p_lo;
+                pb = block_positions(S, blocks[counts[2] + counts[3] - 1], 0, 0).p_hi;
+            }
+            window_rows(P, C, S.K, pa, pb, S.h_row0, S.h_rows);
+        }
+        hs.resize((size_t)(S.cut ? 2 : 1) * rows_stored_h(S) * kSpec);
+        S.hspec = hs.data();
+    } else {
+        set_banked(S, const_cast<float2*>(bank), direct_taps > 0 ? const_cast<int*>(bank_cut) : nullptr, windowed);
+    }
+    if (direct_taps > 0) { S.out_direct = out_direct; S.direct_taps = direct_taps; }
+    S.xspec = xs.data();
+    std::vector<RItem> items(max_render_items(S));
+    emu_rir_prep(S, norm_part.data());
     const int ns = spectra_pairs_h(S) + spectra_pairs_x(S);
     for (int i = 0; i < ns; ++i) cta_spectra(S, i, T);
     prepare_ranges(S, items.data());
-    const int nr = counts[0] * items_per_block(S);
+    const int nr = win_blocks(S) * items_per_block(S);
     const int grid = nr < 3 ? nr : 3;              // a few persistent CTAs, each looping over many items
     for (int cta = 0; cta < grid; ++cta) {
         if (S.aligned || (mode == MODE_STATIC && S.K == 1)) cta_render_fast(items.data(), nr, cta, grid, T);
         else cta_render(items.data(), nr, cta, grid, T, false, S.K > 1);
     }
+    if (win_stats) { win_stats[0] = S.nblk_max; win_stats[1] = ws.k1 - ws.k0; win_stats[2] = S.h_row0; win_stats[3] = S.h_rows; }
+    if (bank_stats) { bank_stats[0] = spectra_pairs_h(S); bank_stats[1] = spectra_pairs_x(S); bank_stats[2] = nr; }
+}
+
+extern "C" {
+
+// Emulate k_spectra + k_render for one source.  mode: 0 static, 1 bounds, 2 (idx, w).  Aligned blocking for every
+// bounds trajectory with one RIR partition.
+int emu_render(const float* x, const float* rir, float* out, const int32_t* bounds, const int32_t* idx,
+               const float* w, int N, int P, int C, int L, int mode) {
+    const int aligned = mode == MODE_MOVING_BOUNDS && (L + kB - 1) / kB == 1;
+    emu_source(x, rir, nullptr, nullptr, out, bounds, idx, w, N, P, C, L, mode, aligned, 0, 0, nullptr, 0, 0, 0,
+               nullptr, nullptr);
     return 0;
 }
 

@@ -24,7 +24,7 @@ int emu_bank_create(const float* rir, int P, int C, int L, int normalize, int di
     if (direct_taps > 0) { S.cut = cut; S.direct_taps = direct_taps; }
     emu_rir_prep(S, norm_part.data());
     const int ns = spectra_pairs_h(S) + spectra_pairs_x(S) + range_ctas(S);
-    for (int i = 0; i < ns; ++i) cta_spectra_sets(S, i, T);
+    for (int i = 0; i < ns; ++i) cta_spectra(S, i, T);
     return ns;
 }
 
@@ -34,42 +34,8 @@ int emu_bank_create(const float* rir, int P, int C, int L, int normalize, int di
 int emu_render_banked(const float* x, const float2* spec, const int* cut, float* out, const int32_t* bounds,
                       const int32_t* idx, const float* w, int N, int P, int C, int L, int mode, int aligned,
                       int win_start, int win_len, float* out_direct, int direct_taps, int* stats) {
-    const Tables& T = tables();
-    Source S;
-    memset(&S, 0, sizeof(S));
-    S.x = x; S.out = out; S.bounds = bounds; S.idx = idx; S.w = w;
-    S.N = N; S.P = P; S.C = C; S.L = L; S.K = (L + kB - 1) / kB; S.nb = (N + kB - 1) / kB; S.mode = mode;
-    S.aligned = aligned;
-    const bool windowed = win_len > 0;
-    std::vector<Block> full(S.aligned ? S.nb + P - 1 : S.nb);
-    const int nfull = emu_full_blocks(S, full.data());
-    WinSpan ws = {0, nfull, 0, nfull};
-    if (windowed) ws = window_blocks(full.data(), nfull, win_start, win_start + win_len, S.K);
-    S.nblk_max = windowed ? ws.g1 - ws.g0 : (int)full.size();
-    set_banked(S, const_cast<float2*>(spec), direct_taps > 0 ? const_cast<int*>(cut) : nullptr, windowed);
-    if (direct_taps > 0) { S.out_direct = out_direct; S.direct_taps = direct_taps; }
-    std::vector<float2> xs((size_t)S.nblk_max * kSpec);
-    std::vector<Block> blocks(S.nblk_max);
-    for (int i = 0; i < S.nblk_max; ++i) {
-        Block z; z.start = 0; z.len = 0; z.p_lo = 0; z.p_hi = 0;
-        blocks[i] = windowed ? full[ws.g0 + i] : (i < nfull ? full[i] : z);
-    }
-    std::vector<double> rstep(P);
-    if (mode == MODE_MOVING_BOUNDS)
-        for (int sg = 0; sg < P - 1; ++sg) rstep[sg] = 1.0 / (double)(bounds[sg + 1] - bounds[sg]);
-    int counts[8] = {windowed ? S.nblk_max : nfull, 0, ws.k0 - ws.g0, ws.k1 - ws.k0, win_start, win_len, 0, 0};
-    S.xspec = xs.data(); S.blocks = blocks.data(); S.rstep = rstep.data(); S.counts = counts;
-    std::vector<RItem> items((size_t)S.nblk_max * items_per_block(S));
-    const int ns = spectra_pairs_h(S) + spectra_pairs_x(S);
-    for (int i = 0; i < ns; ++i) cta_spectra_sets(S, i, T);
-    prepare_ranges_window(S, items.data());
-    const int nr = win_blocks(S) * items_per_block(S);
-    const int grid = nr < 3 ? nr : 3;
-    for (int cta = 0; cta < grid; ++cta) {
-        if (S.aligned || (mode == MODE_STATIC && S.K == 1)) cta_render_fast(items.data(), nr, cta, grid, T);
-        else cta_render(items.data(), nr, cta, grid, T, false, S.K > 1);
-    }
-    if (stats) { stats[0] = spectra_pairs_h(S); stats[1] = spectra_pairs_x(S); stats[2] = nr; }
+    emu_source(x, nullptr, spec, cut, out, bounds, idx, w, N, P, C, L, mode, aligned, win_start, win_len, out_direct,
+               direct_taps, 0, 0, nullptr, stats);
     return 0;
 }
 
