@@ -90,6 +90,8 @@ typedef struct {
     int32_t direct_taps;      /* SS_DIRECT_TARGET: taps kept from each row's peak on, >= 1                        */
     int32_t win_start, win_len; /* time window, see below; win_len == 0: the whole stem                          */
     const ss_bank* rir_bank;  /* RIR spectrum bank (version 103) instead of `rir`, which is then NULL; see below   */
+    const int32_t* win_start_dev; /* moving window (version 104): DEVICE pointer to the start, read at every run in
+                                   * place of win_start; see below                                                  */
 } ss_source;                  /* fields appended since version 100: a zeroed (memset) struct leaves them off      */
 
 /* Time window (win_len > 0, version 102): the source renders only output samples [win_start, win_start + win_len)
@@ -118,7 +120,20 @@ typedef struct {
  *     `bounds_host`).
  * A source with a `rir_bank` reads no RIR positions at all, windowed or not.
  * On the device path, ss_device_errors reports only what the kernels read: the idx entries of the read set, and the
- * bounds table of a grid-blocked source. */
+ * bounds table of a grid-blocked source.
+ *
+ * Moving window (version 104): `win_start_dev` points to one int32 in device memory (4-byte aligned) that holds the
+ * start, so that a crop can move between runs of a plan (or be drawn on the device) without any host work.  Only with
+ * win_len > 0 and win_start == 0; anything else, or an unaligned pointer, is SS_ERR_INVALID before any work.
+ * ss_render_dev and ss_plan_create take such sources; ss_render_host / _ex refuse them (SS_ERR_INVALID): the host path
+ * copies a read set that depends on the start.  The value is read when the run's first kernel reaches it: write it on
+ * the run's stream, or in an order that is guaranteed to come before that stream.  A start outside [0, N - win_len] is
+ * clamped into that range, the window is rendered there, and ss_device_errors reports bit 2.  win_len fixes the output
+ * shape and stays bound.  Bits, blocking and kernel variant are those of a fixed window at the same start.  A chunk that
+ * holds a moving window builds its block tables on the device (k_blocks, as without bounds_host), sized once for the
+ * largest table any start needs.  Read set: all of x; all of bounds / idx / w; all P RIR positions (the RIR rows of
+ * every position are transformed at every run), none with a `rir_bank` - a bank is the way to crop a fixed RIR set
+ * step after step without transforming it again. */
 
 /* ---- RIR spectrum banks (version 103).  The half spectra of a source's RIR partitions depend on nothing but its taps,
  * SS_RIR_NORMALIZE and direct_taps - not on the dry signal, the trajectory, the window or the batch.  A bank holds them
@@ -154,7 +169,7 @@ int64_t ss_bank_bytes(const ss_bank* bank);   /* device bytes held */
 void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their context */
 
 /* library / build identification */
-int ss_version(void);
+int ss_version(void);        /* 104: ss_source.win_start_dev (moving windows), ss_device_errors bit 2 */
 const char* ss_strerror(int status);
 int ss_last_cuda_error(void);
 
@@ -178,7 +193,8 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
 /* The device path cannot return SS_ERR_INDEX: kernels that meet a trajectory outside the contract above render the
  * offending samples as silence (clamped positions) and set a bit that this call returns and clears after waiting for
  * the device: bit 0 = an interp_index outside [0, P - 2], bit 1 = a device-side bounds table that is not ascending from
- * 0 to N (checked for grid-blocked sources).  The Python device API raises IndexError / ValueError from it on request
+ * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
+ * (rendered clamped into that range).  The Python device API raises IndexError / ValueError from it on request
  * (Renderer.check_device_errors). */
 int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
 
@@ -190,8 +206,11 @@ int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
  * `items` and the values behind bounds_host must stay valid and unchanged while the plan lives; the contents of the
  * x / rir / out buffers may change between runs.  Device-side `bounds` / `idx` are read at run time and must satisfy the
  * same preconditions as for ss_render_dev.  A plan may hold banked sources: every ss_bank they name must outlive the
- * plan (destroy the plan first; a bank's spectra are read at every run).  Not thread-safe; destroy plans before their
- * context. */
+ * plan (destroy the plan first; a bank's spectra are read at every run).  A plan binds each source's window length;
+ * the start is bound too unless the source names a `win_start_dev`, whose int32 is read at every run and may change
+ * between runs (written in stream order before the run).  A chunk that holds such a source runs k_blocks too: 3 kernel
+ * launches per chunk, plus one each for k_rir_absmax (SS_RIR_NORMALIZE) and k_rir_direct (SS_DIRECT_TARGET with raw
+ * RIRs) when present.  Not thread-safe; destroy plans before their context. */
 typedef struct ss_plan ss_plan;
 int ss_plan_create(ss_ctx* ctx, const ss_source* items, int n_items, ss_plan** out);
 int ss_plan_run(ss_plan* plan, void* stream);

@@ -61,7 +61,8 @@ class SsSource(ctypes.Structure):
                 ("N", ctypes.c_int32), ("P", ctypes.c_int32), ("C", ctypes.c_int32), ("L", ctypes.c_int32),
                 ("mode", ctypes.c_int32), ("flags", ctypes.c_int32), ("bounds_host", ctypes.c_void_p),
                 ("out_direct", ctypes.c_void_p), ("direct_taps", ctypes.c_int32),
-                ("win_start", ctypes.c_int32), ("win_len", ctypes.c_int32), ("rir_bank", ctypes.c_void_p)]
+                ("win_start", ctypes.c_int32), ("win_len", ctypes.c_int32), ("rir_bank", ctypes.c_void_p),
+                ("win_start_dev", ctypes.c_void_p)]
 
 
 def _stale():

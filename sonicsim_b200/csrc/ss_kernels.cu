@@ -41,7 +41,8 @@ using namespace ss;
 
 // Device-path trajectory check: the kernels cannot raise, so a source whose device-side trajectory breaks the contract
 // of ss_render_dev (idx outside [0, P - 2]; bounds not ascending from 0 to N) sets a bit here; ss_device_errors reads
-// and clears it.  bit 0: index out of range, bit 1: bounds not monotone / not ending at N.
+// and clears it.  bit 0: index out of range, bit 1: bounds not monotone / not ending at N, bit 2: a moving window's
+// start outside [0, N - win_len] (clamped).
 __device__ unsigned g_dev_err;
 
 // twiddle tables, filled from the host in double precision (ss_create)
@@ -108,7 +109,9 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 
 // One small CTA per chunk: block table of every source (one warp per source), 1 / n_s table, then the
 // exclusive scan that packs the render work items of all sources into one dense table.  A whole source's table is the
-// full plan; a windowed one's holds the full plan's blocks [g0, g1) (window_span, cut to the table size).
+// full plan; a windowed one's holds the full plan's blocks [g0, g1) (window_span, cut to the table size).  A moving
+// window first reads its start from device memory, clamps it (bit 2 of g_dev_err) and stores it as counts[4], where
+// the window search here and k_prepare's range warps take it; its table is sized for every start (window_table_cap).
 __global__ void __launch_bounds__(256)
 k_blocks(const Source* __restrict__ srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -116,6 +119,13 @@ k_blocks(const Source* __restrict__ srcs, int n_src, int* __restrict__ total_ite
         const Source& S = srcs[si];
         int g0 = 0, g1 = S.nblk_max;
         if (S.h_rows) {
+            const int* const ws_dev = win_start_ptr(S);
+            if (ws_dev && lane == 0) {
+                bool bad;
+                S.counts[4] = clamp_win_start(*ws_dev, S.N, S.counts[5], bad);
+                if (bad) atomicOr(&g_dev_err, 4u);
+            }
+            __syncwarp();
             const WinSpan w = window_blocks_dev(S, lane);
             g0 = w.g0;
             g1 = w.g1 - w.g0 > S.nblk_max ? w.g0 + S.nblk_max : w.g1;
@@ -579,7 +589,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 103; }
+extern "C" int ss_version(void) { return 104; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -809,6 +819,9 @@ static int validate_item(const ss_source& it) {
     if (it.win_len < 0 || it.win_start < 0 || (it.win_len == 0 && it.win_start != 0) ||
         (int64_t)it.win_start + it.win_len > (int64_t)it.N)
         return SS_ERR_INVALID;
+    // a moving window: a length, no host start, an int32 the kernels can load
+    if (it.win_start_dev && (it.win_len == 0 || it.win_start != 0 || ((uintptr_t)it.win_start_dev & 3)))
+        return SS_ERR_INVALID;
     return it.rir_bank ? validate_bank_use(it) : SS_OK;
 }
 // every bank of a batch belongs to the context that renders it
@@ -869,6 +882,21 @@ static void window_shape(const ss_source& it, Shape& s) {
     const int ws = it.win_start, we = it.win_start + it.win_len;
     const int32_t* hb = it.mode == SS_MOVING_BOUNDS ? it.bounds_host : nullptr;
     s.win = 1;
+    if (it.win_start_dev) {
+        // moving window: k_blocks finds the blocks of each run's start on the device, in a table sized for every start;
+        // the read set is the whole source (every RIR row, all of x, idx, w)
+        std::vector<Block> full;
+        int n = 0;
+        if (!s.aligned || hb) {
+            full.resize((size_t)s.nblk_max);
+            n = std::min(plan_blocks(s.aligned, hb, it.P, it.N, s.nb, 0, s.nblk_max, full.data()), s.nblk_max);
+        }
+        s.nblk_max = window_table_cap(full.empty() ? nullptr : full.data(), n, it.N, it.win_len, s.K, it.P, s.nblk_max);
+        s.xa = 0; s.xb = it.N; s.ia = 0; s.ib = it.N;
+        window_rows(it.P, it.C, s.K, 0, it.mode == SS_STATIC ? 0 : it.P - 1, s.row0, s.rows);
+        s.pa = 0; s.pb = it.P - 1;
+        return;
+    }
     s.tab_host = !s.aligned || hb != nullptr;
     int pa = 0, pb = it.P - 1;                           // all positions unless the trajectory is visible here
     if (s.tab_host) {
@@ -890,10 +918,8 @@ static void window_shape(const ss_source& it, Shape& s) {
         }
     }
     if (!s.tab_host) {
-        // k_blocks finds the blocks on the device: a window meets at most ceil(o / 4096) + 1 blocks of each segment it
-        // overlaps by o samples, plus one block in front (even start) and the last one's partner
-        const int64_t bound = (int64_t)(it.win_len + kB - 1) / kB + 2 * (int64_t)(it.P - 1) + 2;
-        if (bound < s.nblk_max) s.nblk_max = (int)bound;
+        // k_blocks finds the blocks on the device, in a table that holds them wherever the window lies
+        s.nblk_max = window_table_cap(nullptr, 0, it.N, it.win_len, s.K, it.P, s.nblk_max);
         s.xa = 0; s.xb = it.N; s.ia = 0; s.ib = it.N;
     }
     if (it.mode == SS_STATIC) { pa = 0; pb = 0; }
@@ -942,7 +968,7 @@ extern "C" int ss_debug_plan(const ss_source* item, int32_t* blocks_out, int32_t
     if (item->mode == SS_MOVING_BOUNDS && (!item->bounds_host || item->P < 2)) return SS_ERR_INVALID;
     if (item->mode == SS_MOVING_BOUNDS && !bounds_ok(item->bounds_host, item->P, item->N)) return SS_ERR_INVALID;
     if (item->win_len < 0 || item->win_start < 0 || (item->win_len == 0 && item->win_start != 0) ||
-        (int64_t)item->win_start + item->win_len > (int64_t)item->N)
+        (int64_t)item->win_start + item->win_len > (int64_t)item->N || item->win_start_dev)
         return SS_ERR_INVALID;
     const Shape sh = shape_of(*item);
     const int first = sh.win ? sh.k0 - sh.g0 : 0;
@@ -975,10 +1001,10 @@ static size_t chunk_scratch_bytes(const ss_source* items, int first, int last) {
     for (int i = first; i < last; ++i) need += spectra_bytes(items[i]);
     return need;
 }
-// Block tables on the host when every trajectory is host-visible (always true on the host path)
+// Block tables on the host when every trajectory is host-visible and every window fixed (always true on the host path)
 static bool chunk_host_tables(const ss_source* items, int first, int last) {
     for (int i = first; i < last; ++i)
-        if (items[i].mode == SS_MOVING_BOUNDS && !items[i].bounds_host) return false;
+        if ((items[i].mode == SS_MOVING_BOUNDS && !items[i].bounds_host) || items[i].win_start_dev) return false;
     return true;
 }
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 5] - which the host fills even when k_blocks builds the
@@ -1064,6 +1090,7 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
                 s.counts = (int*)(dbase + tab_off); tab_off += counts_bytes(sh);
                 memset(hb_counts, 0, counts_bytes(sh));
                 hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
+                memcpy(hb_counts + 6, &it.win_start_dev, sizeof(it.win_start_dev));      // win_start_ptr
             } else {
                 s.counts = (int*)scratch;
             }
@@ -1567,6 +1594,8 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         int st = validate_item_ctx(c, items[i]); if (st) return st;
         // a window cannot be loudness-normalised: the reference measures the whole stem
         if (post && post[i].brk && items[i].win_len > 0) return SS_ERR_INVALID;
+        // a moving window's read set depends on a start that only the device knows
+        if (items[i].win_start_dev) return SS_ERR_INVALID;
         if (items[i].mode == SS_MOVING_BOUNDS && !bounds_ok(items[i].bounds, items[i].P, items[i].N)) return SS_ERR_INVALID;
         rset[i] = read_set(items[i]);
         st = check_idx_host(items[i], rset[i]); if (st) return st;

@@ -42,7 +42,8 @@ struct Source {
     double* rstep;         // scratch: 1 / (samples in segment s), s < P - 1 (mode 1)
     int* counts;           // scratch: [0] = blocks in use, [1] = index of this source's first render item; windowed
                            // source (h_rows != 0): [2] = first block that meets the window, [3] = blocks that do,
-                           // [4] = win_start, [5] = win_len
+                           // [4] = win_start, [5] = win_len, [6..7] = device pointer of a moving window's start or
+                           // null (win_start_ptr)
     const float* norm_part;// scratch: kNormParts partial abs-maxima of the RIR tensor (k_rir_absmax), or null: taps used as given
     int* cut;              // scratch: P*C direct-path row lengths (k_rir_direct), or null: no direct target
     float* out_direct;     // (C, N) direct-path stem (with `cut`)
@@ -197,6 +198,37 @@ SS_HD void window_rows(int P, int C, int K, int pa, int pb, int& row0, int& rows
     if (r1 > P * ck) r1 = P * ck;
     row0 = r0; rows = r1 - r0;
 }
+// Table size that holds the window's blocks [g0, g1) whatever its start in [0, N - win_len] (a moving window: the start
+// is read on the device at every run, the table is sized once).  full / nfull: the full plan's blocks when the host
+// knows them (grid blocking, or aligned blocking with bounds_host) - they tile [0, N), and for a fixed first block k0
+// g1 - g0 grows with the start, so one sliding pass over the largest start of each k0 gives the exact maximum.  Under
+// grid blocking that is at most ceil(win_len / 4096) + K + 2 (one straddling block, K - 1 partition blocks and the
+// even rounding in front, the partner behind).  full == null (aligned blocking over device-side bounds): a window
+// meets at most ceil(o / 4096) + 1 blocks of each segment it overlaps by o samples, plus one block in front (even
+// start) and the last one's partner.  Never more than `cap`, the whole source's table.
+SS_HD int window_table_cap(const Block* full, int nfull, int N, int win_len, int K, int P, int cap) {
+    if (!full) {
+        const int64_t bound = (int64_t)(win_len + kB - 1) / kB + 2 * (int64_t)(P - 1) + 2;
+        return bound < cap ? (int)bound : cap;
+    }
+    int best = 0, k1 = 0;
+    for (int k0 = 0; k0 < nfull && full[k0].start <= N - win_len; ++k0) {
+        const int end = full[k0].start + full[k0].len - 1;
+        const int we = (end < N - win_len ? end : N - win_len) + win_len;   // largest start whose first block is k0
+        while (k1 < nfull && full[k1].start < we) ++k1;
+        const WinSpan w = window_span(k0, k1, nfull, K);
+        best = w.g1 - w.g0 > best ? w.g1 - w.g0 : best;
+    }
+    return best < cap ? best : cap;
+}
+// A moving window's start as read from device memory, clamped into [0, N - win_len]; bad = it was outside
+SS_HD int clamp_win_start(int v, int N, int win_len, bool& bad) {
+    const int hi = N - win_len;
+    bad = v < 0 || v > hi;
+    return v < 0 ? 0 : (v > hi ? hi : v);
+}
+// a windowed source's moving start (counts[6..7], 8-byte aligned), or null: the start is counts[4]
+SS_HD const int* win_start_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 6); }
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
 SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }

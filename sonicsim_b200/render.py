@@ -31,8 +31,11 @@ class MovingSource(T.NamedTuple):
                                       # abs-max on the device like generate_rir_combination (SonicSim_audio.py:398)
     direct_taps: int = 0              # > 0: also render the direct-path stem (every RIR row cut `direct_taps` taps
                                       # after its peak, see SS_DIRECT_TARGET) into the source's direct_outs entry
-    window: T.Optional[T.Tuple[int, int]] = None   # (start, length): render only output samples [start, start + length)
-                                      # into a (C, length) output, bit-identical to those samples of the full render
+    window: T.Optional[T.Tuple[T.Any, int]] = None  # (start, length): render only output samples [start, start + length)
+                                      # into a (C, length) output, bit-identical to those samples of the full render.
+                                      # Device path: `start` may be a one-element CUDA int32 tensor (0-d, e.g.
+                                      # starts[k]) read on the device at every run - a plan's crop can move between
+                                      # runs without host work; out-of-range starts are clamped (check_device_errors)
 
 
 class StaticSource(T.NamedTuple):
@@ -41,18 +44,42 @@ class StaticSource(T.NamedTuple):
     rir: T.Any
     normalize_rirs: bool = False
     direct_taps: int = 0              # as MovingSource.direct_taps
-    window: T.Optional[T.Tuple[int, int]] = None   # as MovingSource.window
+    window: T.Optional[T.Tuple[T.Any, int]] = None  # as MovingSource.window
+
+
+def _is_tensor(v) -> bool:
+    return type(v).__module__.split(".")[0] == "torch"
 
 
 def _window(s, i, N):
     """(win_start, win_len, samples per output row) of source i; a window must lie inside [0, N] and not be empty."""
     if s.window is None:
         return 0, 0, N
+    if _is_tensor(s.window[0]):
+        raise ValueError("window of source %d: a tensor start is read on the device at every run; only render_device "
+                         "and plan_device take one" % i)
     a, n = (int(v) for v in s.window)
     if a < 0 or n < 1 or a + n > N:
         raise ValueError("window of source %d must be (start, length) with 0 <= start, length >= 1 and "
                          "start + length <= N = %d, got (%d, %d)" % (i, N, a, n))
     return a, n, n
+
+
+def _window_dev(s, i, N, device):
+    """_window for the device path, plus the start tensor of a moving window (else None): a one-element CUDA int32
+    tensor on cuda:`device`, whose value the kernels read at every run (win_start_dev)."""
+    if s.window is None or not _is_tensor(s.window[0]):
+        return _window(s, i, N) + (None,)
+    import torch
+    t, n = s.window[0], int(s.window[1])
+    if t.dtype != torch.int32 or t.numel() != 1:
+        raise ValueError("window of source %d: a start tensor must hold one int32, got %s with %d elements"
+                         % (i, t.dtype, t.numel()))
+    if not t.is_cuda or t.device.index != device:
+        raise ValueError("window of source %d: a start tensor must be on cuda:%d, got %s" % (i, device, t.device))
+    if n < 1 or n > N:
+        raise ValueError("window of source %d must have 1 <= length <= N = %d, got %d" % (i, N, n))
+    return 0, n, n, t
 
 
 def _flags(s, i, direct_out) -> int:
@@ -297,7 +324,8 @@ class Renderer:
         """`sources`: MovingSource / StaticSource whose fields are CUDA float32 / int32 tensors;
         `outs`: preallocated CUDA (C, N) tensors - (C, length) for a source with a `window`; `direct_outs`: the same
         for the direct-path stems of sources with direct_taps > 0, None for the others.  Asynchronous on `stream`
-        (torch current stream).  Crops that move from call to call are rendered here (a plan binds its windows)."""
+        (torch current stream).  A window's start may be a CUDA int32 tensor (see MovingSource.window); a crop that
+        moves every step is cheaper through a plan_device whose start tensors are rewritten between runs."""
         items, n, keep = self._device_items(sources, outs, direct_outs)
         if stream is None:
             import torch
@@ -310,7 +338,11 @@ class Renderer:
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
         (N,), RIRs (P, C, L) / (C, L), outs[i] (C, N) for that source's own C and N ((C, length) with a `window`);
         int32 bounds (P,); direct_outs[i] as outs[i] for a source with direct_taps > 0, else None.  The plan binds
-        each source's window: crops that move between runs go through render_device."""
+        each window's length, and its start when that is an int.  A start given as a one-element CUDA int32 tensor
+        (e.g. starts[k] of a (B,) tensor; stems of one scene may share one element) is read on the device at every
+        run: write new starts on the run's stream (starts.copy_(...)) and call run() again - crops that move every
+        step, with no host work beyond the graph launch.  Such a plan transforms every RIR row of a raw-RIR source at
+        every run; pass a RirBank to transform them once."""
         return DevicePlan(self, *self._device_items(sources, outs, direct_outs))
 
     def _device_items(self, sources, outs, direct_outs=None):
@@ -340,7 +372,7 @@ class Renderer:
         for i, s in enumerate(sources):
             chk(s.dry, "dry", i, torch.float32)
             N = s.dry.numel()
-            ws, wl, n_out = _window(s, i, N)
+            ws, wl, n_out, start = _window_dev(s, i, N, self.device)
             rb = s.rir if isinstance(s, StaticSource) else s.rirs
             rb = rb if isinstance(rb, RirBank) else None
             if isinstance(s, StaticSource):
@@ -378,6 +410,8 @@ class Renderer:
                 items[i].rir_bank = _bank_of(self, s, i, P, C, L)
             items[i].flags = _flags(s, i, direct_outs[i])
             items[i].win_start, items[i].win_len = ws, wl
+            if start is not None:
+                items[i].win_start_dev = start.data_ptr()         # kept alive with `sources`
             if direct_outs[i] is not None:
                 chk(direct_outs[i], "direct_out", i, torch.float32, (C, n_out))
                 items[i].out_direct = direct_outs[i].data_ptr()
@@ -387,13 +421,17 @@ class Renderer:
     def check_device_errors(self):
         """Waits for the device and raises what the reference would have raised for a trajectory the device path met
         but could not refuse up front: IndexError for an interp_index outside [0, P - 2] (NumPy's fancy index at
-        SonicSim_moving.py:89-90), ValueError for a device-side bounds table that is not ascending from 0 to N."""
+        SonicSim_moving.py:89-90), ValueError for a device-side bounds table that is not ascending from 0 to N or for a
+        window start tensor that held a value outside [0, N - length] (the window was rendered clamped into range)."""
         bits = ctypes.c_uint32()
         _lib.check(self.lib.ss_device_errors(self.ctx, ctypes.byref(bits)))
         if bits.value & 1:
             raise IndexError("an interp_index on the device was out of bounds for the number of RIR positions")
         if bits.value & 2:
             raise ValueError("a device-side trajectory bounds table is not ascending from 0 to N")
+        if bits.value & 4:
+            raise ValueError("a window start on the device was outside [0, N - length]; the window was clamped into "
+                             "that range")
 
     def launch_count(self) -> int:
         return int(self.lib.ss_launch_count(self.ctx))
