@@ -169,7 +169,7 @@ int64_t ss_bank_bytes(const ss_bank* bank);   /* device bytes held */
 void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their context */
 
 /* library / build identification */
-int ss_version(void);        /* 104: ss_source.win_start_dev (moving windows), ss_device_errors bit 2 */
+int ss_version(void);        /* 105: mixtures in plans (ss_plan_create_mix) */
 const char* ss_strerror(int status);
 int ss_last_cuda_error(void);
 
@@ -216,6 +216,53 @@ int ss_plan_create(ss_ctx* ctx, const ss_source* items, int n_items, ss_plan** o
 int ss_plan_run(ss_plan* plan, void* stream);
 int ss_plan_is_graph(const ss_plan* plan);     /* 1 once the plan runs as an instantiated CUDA graph */
 void ss_plan_destroy(ss_plan* plan);
+
+/* ---- mixtures in plans (version 105): the training step of the separation dataloader
+ * (separation/look2hear/datas/movingdatamodule.py:56-126) behind a plan's crops.  At every run, after the renders of
+ * every chunk have joined, the plan assembles each mixture from its own sources' outputs with the arithmetic of
+ * ss_mix_dev (compute_mch_rms_dB, SIR gains of the interferers and SNR gain of the summed noise clamped at +40 dB,
+ * sums), reading the mixture's SIRs and SNR from device memory at that run.  The run stays one CUDA graph launch; a plan
+ * with mixtures runs 4 more kernel launches per run, whatever the number of mixtures.
+ *
+ * T is a stem's output length (win_len, or N for a whole stem), E = C * T, or T with SS_MIX_MONO.
+ *   - Indices name entries of the `items` passed to ss_plan_create_mix, in the caller's order.  A mixture reads the
+ *     reverberant `out` of each named item (a direct-path stem is rendered as usual and is not a mixture input).  A stem
+ *     may appear in several mixtures (one noise stem shared by several scenes) but only once within one mixture.
+ *   - SS_MIX_MONO: every stem, speakers and noises alike, is first folded to its channel mean (the dataloader's
+ *     is_mono, :62-63, :76-77): at every element t, the float32 sum of its C rows in channel order 0..C-1, every add
+ *     rounded on its own, then an IEEE division by C.  The same bits on every path.  torch's CPU x.mean(dim=0) does not
+ *     keep one summation order for every C and length, so against it the fold agrees to a few float32 ulps, not bit
+ *     for bit.
+ *   - Outputs: mix (E), speakers_out (S, E) = each speaker after its gain (speaker 0's gain is 1), rms_db (S) =
+ *     compute_mch_rms_dB (:29-32) of every speaker stem before its gain, after the fold with SS_MIX_MONO, rounded to
+ *     float32 (-200 for a silent stem, from the 1e-20 floor).  rms_db lets a caller apply the dataloader's silence rule
+ *     (:84-101, redraw when a speaker's crop is below -40 dB) by masking or redrawing; the plan itself does not loop.
+ *   - sirs, snr (and every win_start_dev of the plan's sources) are read on the device at every run: write them on the
+ *     run's stream before the run, or in an order that is guaranteed to come before it.
+ * Refused at creation, before anything is allocated and with no plan created:
+ *   - S or M outside 1..8, more than 65535 mixtures: SS_ERR_UNSUPPORTED;
+ *   - an index outside [0, n_items), an index repeated within one mixture (among speakers and noises), stems of one
+ *     mixture that differ in C or T, a NULL snr or mix, a NULL sirs with S > 1, unknown flag bits, noise_delay < 0:
+ *     SS_ERR_INVALID;
+ *   - a written range (mix: E floats, speakers_out: S * E floats, rms_db: S floats) that meets another range:
+ *     another written range of any mixture (its own included), any mixture's sirs (S - 1 floats) or snr (1 float), or
+ *     any range an item reads or writes (x, rir, out, out_direct, bounds, idx, w, win_start_dev, whole): SS_ERR_INVALID.
+ * n_mixes == 0 makes ss_plan_create_mix exactly ss_plan_create. */
+#define SS_MIX_MONO 1u                /* channel mean of every stem before mixing (movingdatamodule.py:62-63, 76-77) */
+typedef struct {
+    int32_t speakers[8];              /* indices into `items`; speaker 0 is the reference                             */
+    int32_t noises[8];
+    int32_t S, M;                     /* 1..8 each                                                                    */
+    const float* sirs;                /* device, S - 1 floats in dB, read at every run; NULL only when S == 1          */
+    const float* snr;                 /* device, 1 float in dB, read at every run                                      */
+    float* mix;                       /* device, E floats: (C, T), or (T,) with SS_MIX_MONO                            */
+    float* speakers_out;              /* device, S * E floats (speakers after their gains), or NULL                    */
+    float* rms_db;                    /* device, S floats, or NULL                                                     */
+    uint32_t flags;                   /* SS_MIX_MONO or 0                                                             */
+    int32_t noise_delay;              /* 0, or overlap_audio's shift of the summed noise in elements, as in ss_mix_item */
+} ss_plan_mix;
+int ss_plan_create_mix(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                       ss_plan** out);
 
 /* Same, host pointers: H2D -> render -> D2H, pipelined over chunks on internal streams.  Returns
  * when every `out` is complete.  This is what the drop-in Python functions call. */

@@ -20,6 +20,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-
 SS_OK, SS_ERR_INVALID, SS_ERR_INDEX, SS_ERR_CUDA, SS_ERR_NOMEM, SS_ERR_UNSUPPORTED = 0, -1, -2, -3, -4, -5
 SS_STATIC, SS_MOVING_BOUNDS, SS_MOVING_INDEXED = 0, 1, 2
 SS_RIR_NORMALIZE, SS_DIRECT_TARGET = 1, 2
+SS_MIX_MONO = 1
 
 
 class SsLoudItem(ctypes.Structure):
@@ -36,6 +37,14 @@ class SsMixItem(ctypes.Structure):
     _fields_ = [("speakers", ctypes.c_void_p), ("noises", ctypes.c_void_p), ("sirs", ctypes.c_void_p),
                 ("mix", ctypes.c_void_p), ("speakers_out", ctypes.c_void_p), ("scratch", ctypes.c_void_p),
                 ("E", ctypes.c_int64), ("S", ctypes.c_int32), ("M", ctypes.c_int32), ("snr", ctypes.c_float),
+                ("noise_delay", ctypes.c_int32)]
+
+
+class SsPlanMix(ctypes.Structure):
+    """`ss_plan_mix` of include/sonicsim_b200.h."""
+    _fields_ = [("speakers", ctypes.c_int32 * 8), ("noises", ctypes.c_int32 * 8), ("S", ctypes.c_int32),
+                ("M", ctypes.c_int32), ("sirs", ctypes.c_void_p), ("snr", ctypes.c_void_p), ("mix", ctypes.c_void_p),
+                ("speakers_out", ctypes.c_void_p), ("rms_db", ctypes.c_void_p), ("flags", ctypes.c_uint32),
                 ("noise_delay", ctypes.c_int32)]
 
 
@@ -122,6 +131,8 @@ def load():
         lib.ss_render_dev.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, vp]
         lib.ss_device_errors.argtypes = [vp, ctypes.POINTER(ctypes.c_uint32)]
         lib.ss_plan_create.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(vp)]
+        lib.ss_plan_create_mix.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPlanMix),
+                                            ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_plan_run.argtypes = [vp, vp]
         lib.ss_plan_is_graph.argtypes = [vp]
         lib.ss_plan_destroy.argtypes = [vp]
@@ -164,7 +175,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

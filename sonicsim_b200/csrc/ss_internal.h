@@ -61,6 +61,28 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 struct ScaleItem { float* data; const double* result; int32_t N, C; };
 int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t stream);
 
+// One mixture of the dataloader's arithmetic (ss_mix.cu), as ss_mix_dev and plans with mixtures describe it on the
+// device.  A stem is Cf rows of E floats at row stride T (Cf = 1: the stem's E floats as they are; Cf = C under
+// SS_MIX_MONO: its (C, T) channels, folded to their mean at every element).
+constexpr int kMixBlocks = 64;        // partial sums per mixture
+constexpr int kMixStems = 8;          // at most 8 speakers and 8 noise stems per mixture
+struct MixItem {
+    const float* spk[kMixStems];     // speaker stems; speaker 0 is the reference
+    const float* noise[kMixStems];   // noise stems
+    const float* sirs;                // (S - 1) dB
+    const float* snr;                 // dB, read by k_mix_write at every launch
+    float* mix;                       // (E)
+    float* spk_out;                   // (S, E) scaled speakers (may alias the speakers), or null
+    float* rms_out;                   // (S) compute_mch_rms_dB of every speaker stem, or null
+    double* scratch;                  // ss_mix_scratch_doubles(): kMixBlocks * (S + 2) partial sums, then the gains
+    long long E, T;
+    int S, M, Cf;
+    int delay;                        // overlap_audio shift of the summed noise in elements (0 = none)
+    float snr_val;                    // ss_mix_dev: the item's SNR, which `snr` points at in the uploaded descriptor
+};
+// The four mixture kernels over the n descriptors at `d` (device memory), asynchronous on `stream`.
+int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream);
+
 // Take the next slot of the descriptor ring (pinned host block + its device twin), grown to `bytes`.
 // Blocks the host until the slot's previous host->device copy has completed.  The caller fills `*h`,
 // copies it to `*d` on its stream and records c->desc_ev[*slot] right after the copy.

@@ -589,7 +589,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 104; }
+extern "C" int ss_version(void) { return 105; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -1415,6 +1415,8 @@ struct ss_plan {
     cudaEvent_t ev_fork = nullptr, ev_join[ss_ctx::kAux] = {};
     cudaStream_t s_cap = nullptr;      // capture origin: the caller's stream may be the legacy default stream, which cannot capture
     std::vector<ss_bank*> banks;       // banks of the plan's sources: every run waits for their construction
+    const MixItem* d_mix = nullptr;    // the mixtures' descriptors, in d_desc behind the chunk descriptors
+    int n_mix = 0;
 };
 
 extern "C" void ss_plan_destroy(ss_plan* p) {
@@ -1430,8 +1432,23 @@ extern "C" void ss_plan_destroy(ss_plan* p) {
     delete p;
 }
 
-static int plan_build(ss_plan* p, const ss_source* items, int n_items) {
+// The descriptor of mixture m of a plan: rows of the callers' `items` outputs (before arrange_chunks regroups them)
+static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double* scratch) {
+    MixItem d; memset(&d, 0, sizeof(d));
+    const ss_source& a = items[m.speakers[0]];
+    const int64_t T = a.win_len > 0 ? a.win_len : a.N;
+    const bool mono = (m.flags & SS_MIX_MONO) != 0;
+    for (int s = 0; s < m.S; ++s) d.spk[s] = items[m.speakers[s]].out;
+    for (int q = 0; q < m.M; ++q) d.noise[q] = items[m.noises[q]].out;
+    d.sirs = m.sirs; d.snr = m.snr; d.mix = m.mix; d.spk_out = m.speakers_out; d.rms_out = m.rms_db; d.scratch = scratch;
+    d.E = mono ? T : (int64_t)a.C * T; d.T = T; d.Cf = mono ? a.C : 1;
+    d.S = m.S; d.M = m.M; d.delay = m.noise_delay;
+    return d;
+}
+
+static int plan_build(ss_plan* p, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes) {
     ss_ctx* c = p->c;
+    const ss_source* caller_items = items;
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
     arrange_chunks(c, items, n_items, arranged, cuts);
@@ -1448,10 +1465,14 @@ static int plan_build(ss_plan* p, const ss_source* items, int n_items) {
     CK(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
     for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaEventCreateWithFlags(&p->ev_join[i], cudaEventDisableTiming));
     CK(cudaStreamCreateWithFlags(&p->s_cap, cudaStreamNonBlocking));
-    CK(cudaMalloc((void**)&p->d_desc, off[n_chunks] + 256));
+    // behind the chunk descriptors: the mixtures' descriptors, then one mixture scratch block each
+    const size_t mix_off = off[n_chunks], scr_off = mix_off + align_up(sizeof(MixItem) * n_mixes, 256);
+    const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
+    const size_t desc_bytes = scr_off + scr_bytes * n_mixes;
+    CK(cudaMalloc((void**)&p->d_desc, desc_bytes + 256));
     for (int i = 0; i < ss_ctx::kAux; ++i)
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
-    std::vector<char> host(off[n_chunks] + 256);
+    std::vector<char> host(desc_bytes + 256);
     p->chunks.resize(n_chunks);
     p->launches_per_run = 0;
     for (size_t k = 0; k < n_chunks; ++k) {
@@ -1460,15 +1481,87 @@ static int plan_build(ss_plan* p, const ss_source* items, int n_items) {
         p->launches_per_run += (p->chunks[k].host_tables ? 2 : 3) + (p->chunks[k].any_norm ? 1 : 0) +
                                (p->chunks[k].grid_direct > 0 ? 1 : 0);
     }
-    CK(cudaMemcpy(p->d_desc, host.data(), off[n_chunks], cudaMemcpyHostToDevice));
+    for (int k = 0; k < n_mixes; ++k)
+        ((MixItem*)(host.data() + mix_off))[k] =
+            mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
+    if (n_mixes > 0) {
+        p->d_mix = (const MixItem*)(p->d_desc + mix_off);
+        p->n_mix = n_mixes;
+        p->launches_per_run += 4;
+    }
+    CK(cudaMemcpy(p->d_desc, host.data(), scr_off, cudaMemcpyHostToDevice));
     return SS_OK;
 }
 
-extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
+// Byte ranges of a plan's mixtures: every range a mixture writes (mix, speakers_out, rms_db) meets no other range of
+// the plan - no other written range, no mixture's sirs / snr, nothing an item reads or writes.  One sort and one sweep.
+struct ByteRange { uintptr_t lo, hi; bool written; };
+static void add_range(std::vector<ByteRange>& r, const void* p, uint64_t bytes, bool written) {
+    if (p && bytes > 0) r.push_back({(uintptr_t)p, (uintptr_t)p + (uintptr_t)bytes, written});
+}
+static bool written_ranges_disjoint(std::vector<ByteRange>& r) {
+    std::sort(r.begin(), r.end(), [](const ByteRange& a, const ByteRange& b) { return a.lo < b.lo; });
+    uintptr_t end_any = 0, end_written = 0;                 // furthest end of the ranges that start before this one
+    for (const ByteRange& x : r) {
+        if (x.lo < (x.written ? end_any : end_written)) return false;
+        end_any = x.hi > end_any ? x.hi : end_any;
+        if (x.written) end_written = x.hi > end_written ? x.hi : end_written;
+    }
+    return true;
+}
+
+static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes) {
+    if (n_mixes > 65535) return SS_ERR_UNSUPPORTED;         // one gridDim.y row per mixture
+    std::vector<ByteRange> r;
+    for (int k = 0; k < n_mixes; ++k) {
+        const ss_plan_mix& m = mixes[k];
+        if (m.S < 1 || m.M < 1 || m.S > kMixStems || m.M > kMixStems) return SS_ERR_UNSUPPORTED;
+        if (!m.snr || (m.S > 1 && !m.sirs) || !m.mix || (m.flags & ~SS_MIX_MONO) || m.noise_delay < 0)
+            return SS_ERR_INVALID;
+        int stems[2 * kMixStems];
+        for (int s = 0; s < m.S; ++s) stems[s] = m.speakers[s];
+        for (int q = 0; q < m.M; ++q) stems[m.S + q] = m.noises[q];
+        for (int j = 0; j < m.S + m.M; ++j) {
+            if (stems[j] < 0 || stems[j] >= n_items) return SS_ERR_INVALID;
+            for (int i = 0; i < j; ++i) if (stems[i] == stems[j]) return SS_ERR_INVALID;
+        }
+        const ss_source& a = items[stems[0]];
+        const int64_t T = a.win_len > 0 ? a.win_len : a.N;
+        for (int j = 1; j < m.S + m.M; ++j) {
+            const ss_source& b = items[stems[j]];
+            if (b.C != a.C || (b.win_len > 0 ? b.win_len : b.N) != T) return SS_ERR_INVALID;
+        }
+        const uint64_t E = (m.flags & SS_MIX_MONO) ? (uint64_t)T : (uint64_t)a.C * T;
+        add_range(r, m.mix, 4 * E, true);
+        add_range(r, m.speakers_out, 4 * E * m.S, true);
+        add_range(r, m.rms_db, 4 * (uint64_t)m.S, true);
+        add_range(r, m.sirs, 4 * (uint64_t)(m.S - 1), false);
+        add_range(r, m.snr, 4, false);
+    }
+    for (int i = 0; i < n_items; ++i) {
+        const ss_source& it = items[i];
+        const uint64_t n_out = 4 * (uint64_t)it.C * (it.win_len > 0 ? it.win_len : it.N);
+        add_range(r, it.x, 4 * (uint64_t)it.N, false);
+        add_range(r, it.rir, 4 * (uint64_t)it.P * it.C * it.L, false);
+        add_range(r, it.out, n_out, false);
+        if (it.flags & SS_DIRECT_TARGET) add_range(r, it.out_direct, n_out, false);
+        if (it.mode == SS_MOVING_BOUNDS) add_range(r, it.bounds, 4 * (uint64_t)it.P, false);
+        if (it.mode == SS_MOVING_INDEXED) {
+            add_range(r, it.idx, 4 * (uint64_t)it.N, false);
+            add_range(r, it.w, 4 * (uint64_t)it.N, false);
+        }
+        add_range(r, it.win_start_dev, 4, false);
+    }
+    return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
+}
+
+static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                       ss_plan** out) {
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     { int st = validate_dev_items(c, items, n_items); if (st) return st; }
+    { int st = validate_mixes(items, n_items, mixes, n_mixes); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
@@ -1476,29 +1569,41 @@ extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss
         ss_bank* b = const_cast<ss_bank*>(items[i].rir_bank);
         if (b && std::find(p->banks.begin(), p->banks.end(), b) == p->banks.end()) p->banks.push_back(b);
     }
-    const int st = plan_build(p, items, n_items);
+    const int st = plan_build(p, items, n_items, mixes, n_mixes);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     *out = p;
     return SS_OK;
 }
 
-// the launches of every chunk, forked over the context's internal streams and joined back into `stream`
+extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
+    return plan_create(c, items, n_items, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                  int n_mixes, ss_plan** out) {
+    if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
+    return plan_create(c, items, n_items, mixes, n_mixes, out);
+}
+
+// the launches of every chunk, forked over the context's internal streams and joined back into `stream`, then the
+// mixtures (which read every chunk's outputs) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
     const size_t n_chunks = p->chunks.size();
     if (n_chunks < 2 || c->single_stream) {
         for (size_t k = 0; k < n_chunks; ++k) { int st = chunk_enqueue(c, p->chunks[k], stream, nullptr); if (st) return st; }
-        return SS_OK;
+    } else {
+        CK(cudaEventRecord(p->ev_fork, stream));
+        for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_aux[i], p->ev_fork, 0));
+        int rc = SS_OK;
+        for (size_t k = 0; k < n_chunks && rc == SS_OK; ++k) rc = chunk_enqueue(c, p->chunks[k], c->s_aux[k % ss_ctx::kAux], nullptr);
+        for (int i = 0; i < ss_ctx::kAux; ++i) {
+            CK(cudaEventRecord(p->ev_join[i], c->s_aux[i]));
+            CK(cudaStreamWaitEvent(stream, p->ev_join[i], 0));
+        }
+        if (rc) return rc;
     }
-    CK(cudaEventRecord(p->ev_fork, stream));
-    for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_aux[i], p->ev_fork, 0));
-    int rc = SS_OK;
-    for (size_t k = 0; k < n_chunks && rc == SS_OK; ++k) rc = chunk_enqueue(c, p->chunks[k], c->s_aux[k % ss_ctx::kAux], nullptr);
-    for (int i = 0; i < ss_ctx::kAux; ++i) {
-        CK(cudaEventRecord(p->ev_join[i], c->s_aux[i]));
-        CK(cudaStreamWaitEvent(stream, p->ev_join[i], 0));
-    }
-    return rc;
+    return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream) : SS_OK;
 }
 
 extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
@@ -1520,7 +1625,7 @@ extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
             c->prof.push_back(pf);
             if (st) return st;
         }
-        return SS_OK;
+        return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream) : SS_OK;
     }
     if (!p->exec && !p->graph_failed && !c->no_graph) {
         const int64_t launches_before = c->launches;

@@ -4,28 +4,15 @@
 // noise, sum.  Three streaming passes over stems that are already in HBM + one tiny gain kernel;
 // per-block partial sums are combined in a fixed order, so results are run-to-run deterministic.
 #include <math.h>
+#include <stddef.h>
 #include <string.h>
 
 #include "ss_internal.h"
 
 namespace {
 
-constexpr int kMixBlocks = 64;        // partial sums per mixture
-constexpr int kMaxStems = 8;
+constexpr int kMaxStems = kMixStems;
 constexpr uint64_t kMaxE = UINT64_MAX / 4 / kMaxStems;   // so that the byte size of any (S, E) or (M, E) block fits
-
-struct MixItem {
-    const float* spk;      // (S, E)
-    const float* noise;    // (M, E)
-    const float* sirs;     // (S - 1)
-    float* mix;            // (E)
-    float* spk_out;        // (S, E) scaled speakers (may alias spk)
-    double* scratch;       // kMixBlocks * (S + 2) partial sums, then S + 1 gains at the end
-    long long E;
-    int S, M;
-    float snr;
-    int delay;             // overlap_audio shift of the summed noise in elements (0 = none)
-};
 
 __device__ __forceinline__ double block_sum(double v, double* sh) {
 #pragma unroll
@@ -39,12 +26,31 @@ __device__ __forceinline__ double block_sum(double v, double* sh) {
     return r;          // valid in thread 0
 }
 
+// element e of a stem: its own value (Cf = 1), or the mean of its Cf channel rows at e - a float32 sum in channel order
+// 0..Cf-1, every add rounded on its own, then an IEEE division by Cf.  fold4 gives the same bits four elements at a time.
+__device__ __forceinline__ float fold(const MixItem& it, const float* p, long long e) {
+    float v = p[e];
+    if (it.Cf == 1) return v;
+    for (int c = 1; c < it.Cf; ++c) v = __fadd_rn(v, p[(long long)c * it.T + e]);
+    return __fdiv_rn(v, (float)it.Cf);
+}
+__device__ __forceinline__ float4 fold4(const MixItem& it, const float* p, long long q) {
+    float4 v = ((const float4*)p)[q];
+    if (it.Cf == 1) return v;
+    for (int c = 1; c < it.Cf; ++c) {
+        const float4 a = ((const float4*)(p + (long long)c * it.T))[q];
+        v.x = __fadd_rn(v.x, a.x); v.y = __fadd_rn(v.y, a.y); v.z = __fadd_rn(v.z, a.z); v.w = __fadd_rn(v.w, a.w);
+    }
+    const float C = (float)it.Cf;
+    v.x = __fdiv_rn(v.x, C); v.y = __fdiv_rn(v.y, C); v.z = __fdiv_rn(v.z, C); v.w = __fdiv_rn(v.w, C);
+    return v;
+}
 
 // summed noise stems at element e; with delay D > 0 the enhancement dataloader's overlap_audio
 // (enhancement/look2hear/datas/movingdatamodule.py:34-48) on top: (s[e-D] + s[e+D]) + s[e], zeros outside [0, E)
 __device__ __forceinline__ float noise_sum(const MixItem& it, long long e) {
     float n = 0.f;
-    for (int m = 0; m < it.M; ++m) n += it.noise[(long long)m * it.E + e];
+    for (int m = 0; m < it.M; ++m) n += fold(it, it.noise[m], e);
     return n;
 }
 __device__ __forceinline__ float noise_at(const MixItem& it, long long e) {
@@ -55,16 +61,19 @@ __device__ __forceinline__ float noise_at(const MixItem& it, long long e) {
     return __fadd_rn(__fadd_rn(f, b), n);
 }
 
-// 16-byte path of the three streaming passes: element count a multiple of 4, every row 16-byte aligned, no overlap_audio
-// shift (whose +-D neighbours need not be aligned)
+// 16-byte path of the three streaming passes: element count (and channel stride) a multiple of 4, every row 16-byte
+// aligned, no overlap_audio shift (whose +-D neighbours need not be aligned)
 __device__ __forceinline__ bool mix_vec_ok(const MixItem& it) {
-    return it.delay <= 0 && (it.E & 3) == 0 &&
-           ((((uintptr_t)it.spk) | ((uintptr_t)it.noise) | ((uintptr_t)it.mix) | ((uintptr_t)it.spk_out)) & 15) == 0;
+    if (it.delay > 0 || (it.E & 3) != 0 || (it.Cf > 1 && (it.T & 3) != 0)) return false;
+    uintptr_t a = (uintptr_t)it.mix | (uintptr_t)it.spk_out;
+    for (int s = 0; s < it.S; ++s) a |= (uintptr_t)it.spk[s];
+    for (int m = 0; m < it.M; ++m) a |= (uintptr_t)it.noise[m];
+    return (a & 15) == 0;
 }
 __device__ __forceinline__ float4 noise_sum4(const MixItem& it, long long q) {
     float4 n = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int m = 0; m < it.M; ++m) {
-        const float4 v = ((const float4*)(it.noise + (long long)m * it.E))[q];
+        const float4 v = fold4(it, it.noise[m], q);
         n.x += v.x; n.y += v.y; n.z += v.z; n.w += v.w;
     }
     return n;
@@ -81,7 +90,7 @@ __global__ void __launch_bounds__(256) k_mix_energy(const MixItem* __restrict__ 
         for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < (it.E >> 2); q += (long long)gridDim.x * blockDim.x) {
 #pragma unroll
             for (int s = 0; s < kMaxStems; ++s) if (s < it.S) {
-                const float4 v = ((const float4*)(it.spk + (long long)s * it.E))[q];
+                const float4 v = fold4(it, it.spk[s], q);
                 acc[s] += (double)(v.x * v.x) + (double)(v.y * v.y) + (double)(v.z * v.z) + (double)(v.w * v.w);
             }
             const float4 n = noise_sum4(it, q);
@@ -90,7 +99,7 @@ __global__ void __launch_bounds__(256) k_mix_energy(const MixItem* __restrict__ 
     } else
     for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < it.E; e += (long long)gridDim.x * blockDim.x) {
 #pragma unroll
-        for (int s = 0; s < kMaxStems; ++s) if (s < it.S) { float v = it.spk[(long long)s * it.E + e]; acc[s] += (double)(v * v); }
+        for (int s = 0; s < kMaxStems; ++s) if (s < it.S) { float v = fold(it, it.spk[s], e); acc[s] += (double)(v * v); }
         const float n = noise_at(it, e);
         acc[kMaxStems] += (double)(n * n);
     }
@@ -109,7 +118,7 @@ __device__ double rms_db(double sum_sq, long long count) {
     return 10.0 * log10(ms);
 }
 
-// gains of the interferers: gain_i = min(E(spk0) - E(spk_i) - sir_i, 40) dB   (:108-113)
+// gains of the interferers: gain_i = min(E(spk0) - E(spk_i) - sir_i, 40) dB   (:108-113); the speakers' E to rms_out
 __global__ void k_mix_gain(const MixItem* __restrict__ items, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -126,6 +135,13 @@ __global__ void k_mix_gain(const MixItem* __restrict__ items, int n) {
         if (gain > 40.0) gain = 40.0;
         g[s] = pow(10.0, gain / 20.0);
     }
+    // rms_db's value again with a product of its own (__dmul_rn), so that the gains above keep their contraction
+    if (it.rms_out)
+        for (int s = 0; s < it.S; ++s) {
+            double ms = tot[s] / (double)it.E;
+            if (ms < 1e-20) ms = 1e-20;
+            it.rms_out[s] = (float)__dmul_rn(10.0, log10(ms));
+        }
     g[kMaxStems] = rms_db(tot[kMaxStems], it.E);      // noise energy (dB), consumed by k_mix_write
 }
 
@@ -143,7 +159,7 @@ __global__ void __launch_bounds__(256) k_mix_speech_energy(const MixItem* __rest
             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int s = 0; s < kMaxStems; ++s) if (s < it.S) {
-                const float4 a = ((const float4*)(it.spk + (long long)s * it.E))[q];
+                const float4 a = fold4(it, it.spk[s], q);
                 v.x += a.x * gf[s]; v.y += a.y * gf[s]; v.z += a.z * gf[s]; v.w += a.w * gf[s];
             }
             acc += (double)(v.x * v.x) + (double)(v.y * v.y) + (double)(v.z * v.z) + (double)(v.w * v.w);
@@ -152,7 +168,7 @@ __global__ void __launch_bounds__(256) k_mix_speech_energy(const MixItem* __rest
     for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < it.E; e += (long long)gridDim.x * blockDim.x) {
         float v = 0.f;
 #pragma unroll
-        for (int s = 0; s < kMaxStems; ++s) if (s < it.S) v += it.spk[(long long)s * it.E + e] * gf[s];
+        for (int s = 0; s < kMaxStems; ++s) if (s < it.S) v += fold(it, it.spk[s], e) * gf[s];
         acc += (double)(v * v);
     }
     double r = block_sum(acc, sh);
@@ -165,7 +181,7 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
     const double* g = it.scratch + (long long)kMixBlocks * (kMaxStems + 2);
     double tot = 0;
     for (int b = 0; b < kMixBlocks; ++b) tot += it.scratch[(long long)b * (kMaxStems + 2) + kMaxStems + 1];
-    double gain = rms_db(tot, it.E) - g[kMaxStems] - (double)it.snr;
+    double gain = rms_db(tot, it.E) - g[kMaxStems] - (double)*it.snr;
     if (gain > 40.0) gain = 40.0;
     const float gn = (float)pow(10.0, gain / 20.0);
     float gf[kMaxStems];
@@ -176,7 +192,7 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
             float4 sp = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int s = 0; s < kMaxStems; ++s) if (s < it.S) {
-                float4 v = ((const float4*)(it.spk + (long long)s * it.E))[q];
+                float4 v = fold4(it, it.spk[s], q);
                 v.x = __fmul_rn(v.x, gf[s]); v.y = __fmul_rn(v.y, gf[s]); v.z = __fmul_rn(v.z, gf[s]); v.w = __fmul_rn(v.w, gf[s]);
                 if (it.spk_out) ((float4*)(it.spk_out + (long long)s * it.E))[q] = v;
                 sp.x += v.x; sp.y += v.y; sp.z += v.z; sp.w += v.w;
@@ -193,7 +209,7 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
         float sp = 0.f;
 #pragma unroll
         for (int s = 0; s < kMaxStems; ++s) if (s < it.S) {
-            float v = __fmul_rn(it.spk[(long long)s * it.E + e], gf[s]);        // products and sums rounded separately, as torch does
+            float v = __fmul_rn(fold(it, it.spk[s], e), gf[s]);               // products and sums rounded separately, as torch does
             if (it.spk_out) it.spk_out[(long long)s * it.E + e] = v;
             sp += v;
         }
@@ -248,16 +264,23 @@ extern "C" int ss_mix_dev(ss_ctx* c, const ss_mix_item* items, int n_items, void
     for (int i = 0; i < n_items; ++i) {
         const ss_mix_item& a = items[i];
         MixItem m; memset(&m, 0, sizeof(m));
-        m.spk = a.speakers; m.noise = a.noises; m.sirs = a.sirs; m.mix = a.mix; m.spk_out = a.speakers_out;
-        m.scratch = a.scratch; m.E = a.E; m.S = a.S; m.M = a.M; m.snr = a.snr; m.delay = a.noise_delay;
+        for (int s = 0; s < a.S; ++s) m.spk[s] = a.speakers + (long long)s * a.E;
+        for (int q = 0; q < a.M; ++q) m.noise[q] = a.noises + (long long)q * a.E;
+        m.sirs = a.sirs; m.mix = a.mix; m.spk_out = a.speakers_out; m.scratch = a.scratch;
+        m.E = a.E; m.T = a.E; m.S = a.S; m.M = a.M; m.Cf = 1; m.delay = a.noise_delay;
+        m.snr_val = a.snr;
+        m.snr = (const float*)(c->d_desc[slot] + sizeof(MixItem) * i + offsetof(MixItem, snr_val));
         h[i] = m;
     }
     CK(cudaMemcpyAsync(c->d_desc[slot], c->h_desc[slot], bytes, cudaMemcpyHostToDevice, stream));
     CK(cudaEventRecord(c->desc_ev[slot], stream));
-    const MixItem* d = (const MixItem*)c->d_desc[slot];
-    dim3 grid(kMixBlocks, n_items);
+    return mix_enqueue(c, (const MixItem*)c->d_desc[slot], n_items, stream);
+}
+
+int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream) {
+    dim3 grid(kMixBlocks, n);
     k_mix_energy<<<grid, 256, 0, stream>>>(d);
-    k_mix_gain<<<(n_items + 63) / 64, 64, 0, stream>>>(d, n_items);
+    k_mix_gain<<<(n + 63) / 64, 64, 0, stream>>>(d, n);
     k_mix_speech_energy<<<grid, 256, 0, stream>>>(d);
     k_mix_write<<<grid, 256, 0, stream>>>(d);
     CK(cudaGetLastError());

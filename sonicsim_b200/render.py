@@ -47,6 +47,29 @@ class StaticSource(T.NamedTuple):
     window: T.Optional[T.Tuple[T.Any, int]] = None  # as MovingSource.window
 
 
+class Mixture(T.NamedTuple):
+    """One training mixture of a device plan (Renderer.plan_device): the separation dataloader's (mix_wav, speaker_wav)
+    (movingdatamodule.py:56-126) assembled on the device from the plan's own stems at every run.  `speakers` / `noises`:
+    indices into the plan's `sources` (speaker 0 is the reference; 1 to 8 of each, each stem at most once per mixture,
+    a stem may serve several mixtures), every stem of one (C, T).  `sirs`: CUDA float32 tensor of S - 1 elements (dB,
+    e.g. sirs[b] of a (B, S - 1) tensor), None when S == 1; `snr`: one-element CUDA float32 tensor (dB, e.g. snr[b]);
+    both are read on the device at every run.  Outputs, CUDA float32 and contiguous (slices of batch tensors such as
+    mix[b] are the intended use): `mix` (C, T), or (T,) with `mono`; `speakers_out` (S, C, T) or (S, T): the speakers
+    after their gains; `rms_db` (S,): compute_mch_rms_dB of every speaker stem before its gain (-200 for silence), for
+    the dataloader's silence rule (redraw when a speaker is below -40 dB).  `mono`: fold every stem to its channel
+    mean first (float32 sum in channel order, then a division by C).  `noise_delay`: overlap_audio's shift of the summed
+    noise, in elements (see ss_mix_item)."""
+    speakers: T.Sequence[int]
+    noises: T.Sequence[int]
+    sirs: T.Any
+    snr: T.Any
+    mix: T.Any
+    speakers_out: T.Any = None
+    rms_db: T.Any = None
+    mono: bool = False
+    noise_delay: int = 0
+
+
 def _is_tensor(v) -> bool:
     return type(v).__module__.split(".")[0] == "torch"
 
@@ -332,7 +355,7 @@ class Renderer:
             stream = torch.cuda.current_stream().cuda_stream
         _lib.check(self.lib.ss_render_dev(self.ctx, items, n, ctypes.c_void_p(stream)))
 
-    def plan_device(self, sources, outs, direct_outs=None) -> "DevicePlan":
+    def plan_device(self, sources, outs, direct_outs=None, mixtures=None) -> "DevicePlan":
         """Bind a batch of device-resident sources to its output tensors once; `plan.run()` then renders it with a
         single C-ABI call - one CUDA graph launch (ss_plan_run; a generation loop overwrites the same tensors and
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
@@ -342,8 +365,81 @@ class Renderer:
         (e.g. starts[k] of a (B,) tensor; stems of one scene may share one element) is read on the device at every
         run: write new starts on the run's stream (starts.copy_(...)) and call run() again - crops that move every
         step, with no host work beyond the graph launch.  Such a plan transforms every RIR row of a raw-RIR source at
-        every run; pass a RirBank to transform them once."""
-        return DevicePlan(self, *self._device_items(sources, outs, direct_outs))
+        every run; pass a RirBank to transform them once.
+
+        `mixtures`: Mixture entries over the plan's stems, assembled at every run after the renders, inside the same
+        graph launch (4 more kernel launches per run).  A training step of the separation dataloader is then
+
+            starts.copy_(torch.randint(...)); sirs.uniform_(-6, 6); snr.uniform_(10, 20)   # movingdatamodule.py:106, :119
+            plan.run()                                          # crops, gains and mixtures of every scene
+
+        and the model takes (mix, speakers_out) from there; rms_db (Mixture) carries each speaker's level for the
+        dataloader's silence rule."""
+        items, n, keep = self._device_items(sources, outs, direct_outs)
+        mixes = self._device_mixes(mixtures, outs, keep) if mixtures else None
+        return DevicePlan(self, items, n, keep, mixes)
+
+    def _device_mixes(self, mixtures, outs, keep):
+        """Validated ss_plan_mix array of a plan's mixtures; their tensors are appended to `keep`."""
+        import torch
+        n = len(outs)
+        arr = (_lib.SsPlanMix * len(mixtures))()
+        for k, m in enumerate(mixtures):
+            spk, noi = [int(v) for v in m.speakers], [int(v) for v in m.noises]
+            S, M = len(spk), len(noi)
+            if not 1 <= S <= 8 or not 1 <= M <= 8:
+                raise ValueError("plan_device: mixture %d must have 1 to 8 speakers and 1 to 8 noises, got %d and %d"
+                                 % (k, S, M))
+            for v in spk + noi:
+                if not 0 <= v < n:
+                    raise ValueError("plan_device: mixture %d names source %d of %d" % (k, v, n))
+            if len(set(spk + noi)) != S + M:
+                raise ValueError("plan_device: mixture %d names a source more than once" % k)
+            C, Tn = outs[spk[0]].shape
+            for v in spk + noi:
+                if tuple(outs[v].shape) != (C, Tn):
+                    raise ValueError("plan_device: the stems of mixture %d must share one (C, T); source %d has %s, "
+                                     "source %d has %s" % (k, spk[0], (C, Tn), v, tuple(outs[v].shape)))
+            mono = bool(m.mono)
+            row = (Tn,) if mono else (C, Tn)
+
+            def chk(t, name, shape, numel=None):
+                if not isinstance(t, torch.Tensor) or not t.is_cuda:
+                    raise ValueError("plan_device: %s of mixture %d must be a CUDA tensor" % (name, k))
+                if t.device.index != self.device:
+                    raise ValueError("plan_device: %s of mixture %d is on cuda:%s, the renderer on cuda:%d"
+                                     % (name, k, t.device.index, self.device))
+                if t.dtype != torch.float32:
+                    raise ValueError("plan_device: %s of mixture %d must be torch.float32, got %s" % (name, k, t.dtype))
+                if not t.is_contiguous():
+                    raise ValueError("plan_device: %s of mixture %d must be contiguous" % (name, k))
+                if numel is not None and t.numel() != numel:
+                    raise ValueError("plan_device: %s of mixture %d must hold %d elements, got %d"
+                                     % (name, k, numel, t.numel()))
+                if shape is not None and tuple(t.shape) != tuple(shape):
+                    raise ValueError("plan_device: %s of mixture %d must have shape %s, got %s"
+                                     % (name, k, tuple(shape), tuple(t.shape)))
+                return t.data_ptr()
+
+            if S == 1 and m.sirs is not None:
+                raise ValueError("plan_device: mixture %d has one speaker: its sirs must be None" % k)
+            sirs = chk(m.sirs, "sirs", None, S - 1) if S > 1 else None
+            snr = chk(m.snr, "snr", None, 1)
+            mix = chk(m.mix, "mix", row)
+            sp_out = chk(m.speakers_out, "speakers_out", (S,) + row) if m.speakers_out is not None else None
+            rms = chk(m.rms_db, "rms_db", (S,)) if m.rms_db is not None else None
+            delay = int(m.noise_delay)
+            if delay < 0:
+                raise ValueError("plan_device: noise_delay of mixture %d must be >= 0, got %d" % (k, delay))
+            e = arr[k]
+            for i, v in enumerate(spk):
+                e.speakers[i] = v
+            for i, v in enumerate(noi):
+                e.noises[i] = v
+            e.S, e.M, e.sirs, e.snr, e.mix, e.speakers_out, e.rms_db = S, M, sirs, snr, mix, sp_out, rms
+            e.flags, e.noise_delay = _lib.SS_MIX_MONO if mono else 0, delay
+        keep.append(list(mixtures))
+        return arr
 
     def _device_items(self, sources, outs, direct_outs=None):
         """Validated ss_source array of a device-resident batch: (items, n, objects to keep alive)."""
@@ -454,12 +550,16 @@ class Renderer:
 
 class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
-    descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph."""
+    descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
+    mixtures, the plan also assembles them at every run (ss_plan_create_mix)."""
 
-    def __init__(self, renderer, items, n, keep):
-        self.renderer, self.items, self.n, self._keep = renderer, items, n, keep
+    def __init__(self, renderer, items, n, keep, mixes=None):
+        self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self._plan = ctypes.c_void_p()
-        if n > 0:
+        if n > 0 and mixes:
+            _lib.check(renderer.lib.ss_plan_create_mix(renderer.ctx, items, n, mixes, len(mixes),
+                                                       ctypes.byref(self._plan)))
+        elif n > 0:
             _lib.check(renderer.lib.ss_plan_create(renderer.ctx, items, n, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
