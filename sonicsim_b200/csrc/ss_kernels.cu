@@ -940,8 +940,7 @@ static Shape shape_of(const ss_source& it) {
 }
 // RIR rows transformed per set
 static size_t rir_rows(const ss_source& it, const Shape& sh) { return sh.win ? (size_t)sh.rows : (size_t)it.P * it.C * sh.K; }
-static size_t spectra_bytes(const ss_source& it) {
-    const Shape sh = shape_of(it);
+static size_t spectra_bytes(const ss_source& it, const Shape& sh) {
     return (rir_rows(it, sh) * scratch_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
            (size_t)sh.max_items * sizeof(RItem) +
            align_up(sizeof(Block) * (size_t)sh.nblk_max, 256) + align_up(sizeof(double) * (size_t)it.P, 256) + 256 +
@@ -996,9 +995,10 @@ struct ChunkLaunch {
     const Source* ds = nullptr; const int* dps = nullptr; RItem* d_items = nullptr; int* d_total = nullptr;
     PrepParams pp;
 };
-static size_t chunk_scratch_bytes(const ss_source* items, int first, int last) {
+// A chunk is items[first, last) with their shapes at shapes[first, last), worked out once per call (shape_of).
+static size_t chunk_scratch_bytes(const ss_source* items, const Shape* shapes, int first, int last) {
     size_t need = 256;
-    for (int i = first; i < last; ++i) need += spectra_bytes(items[i]);
+    for (int i = first; i < last; ++i) need += spectra_bytes(items[i], shapes[i]);
     return need;
 }
 // Block tables on the host when every trajectory is host-visible and every window fixed (always true on the host path)
@@ -1012,12 +1012,12 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
 static size_t counts_bytes(const Shape& sh) { return sh.win ? 32 : 16; }
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
 // counts (windowed source, device-built tables)
-static size_t chunk_desc_bytes(const ss_source* items, int first, int last) {
+static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int first, int last) {
     const int n = last - first;
     size_t bytes = align_up(sizeof(Source) * n, 16) + align_up(sizeof(int) * (n + 1), 16) + 16;
     const bool host_tables = chunk_host_tables(items, first, last);
     for (int i = first; i < last; ++i) {
-        const Shape sh = shape_of(items[i]);
+        const Shape& sh = shapes[i];
         if (host_tables)
             bytes += align_up(sizeof(Block) * (size_t)sh.nblk_max, 16) + align_up(sizeof(double) * (size_t)items[i].P, 16) +
                      counts_bytes(sh);
@@ -1028,8 +1028,8 @@ static size_t chunk_desc_bytes(const ss_source* items, int first, int last) {
 }
 // Fill the descriptor block of items[first, last) at `hbase` (host memory) for its device address `dbase`, carve the
 // chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.
-static void chunk_describe(const ss_source* items, int first, int last, char* hbase, char* dbase, char* scratch,
-                           int sm_count, ChunkLaunch* L) {
+static void chunk_describe(const ss_source* items, const Shape* shapes, int first, int last, char* hbase, char* dbase,
+                           char* scratch, int sm_count, ChunkLaunch* L) {
     const int n = last - first;
     const bool host_tables = chunk_host_tables(items, first, last);
     const size_t off_ps = align_up(sizeof(Source) * n, 16);
@@ -1042,7 +1042,7 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
     int grid_direct = 0;
     for (int i = 0; i < n; ++i) {
         const ss_source& it = items[first + i];
-        const Shape sh = shape_of(it);
+        const Shape& sh = shapes[first + i];
         Source s;
         memset(&s, 0, sizeof(s));
         s.x = it.x; s.rir = it.rir; s.out = it.out;
@@ -1101,7 +1101,7 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
         ps += spectra_pairs_h(s) + spectra_pairs_x(s) + range_ctas(s);
         pr += sh.max_items;
         any_long = any_long || s.K > 1;
-        all_aligned = all_aligned && (s.aligned || (s.mode == MODE_STATIC && s.K == 1));      // one transform per item: k_render_fast
+        all_aligned = all_aligned && one_transform_per_item(s.aligned, s.mode, s.K);
     }
     hps[n] = ps;
     // work-item table of the whole chunk (dense) + its length
@@ -1122,8 +1122,15 @@ static void chunk_describe(const ss_source* items, int first, int last, char* hb
     }
 }
 // The kernel launches of one described chunk (its descriptor block is, or will be by stream order, in device memory).
-static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, ss_ctx::Prof* pf) {
-    if (pf) CK(cudaEventRecord(pf->e0, stream));
+// `timed`: events around its prepare and render launches, for ss_get_profile.
+static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, bool timed) {
+    ss_ctx::Prof pf = {};
+    if (timed) {
+        CK(cudaEventCreate(&pf.e0)); CK(cudaEventCreate(&pf.e1)); CK(cudaEventCreate(&pf.e2));
+        pf.chunk = c->prof_chunk++;
+        c->prof.push_back(pf);
+        CK(cudaEventRecord(pf.e0, stream));
+    }
     if (!L.host_tables) {
         k_blocks<<<1, 256, 0, stream>>>(L.ds, L.n, L.d_total);
         CK(cudaGetLastError());
@@ -1144,14 +1151,14 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, s
         else k_prepare<false><<<L.ps, kThreads, kPadF * (int)sizeof(float2), stream>>>(L.ds, L.dps, L.n, L.d_items, L.pp);
         CK(cudaGetLastError());
     }
-    if (pf) CK(cudaEventRecord(pf->e1, stream));
+    if (timed) CK(cudaEventRecord(pf.e1, stream));
     if (L.grid_r > 0) {
         if (L.any_long) k_render<true, false><<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
         else if (L.all_aligned && !c->no_fast) k_render_fast<<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
         else k_render<false, false><<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
         CK(cudaGetLastError());
     }
-    if (pf) CK(cudaEventRecord(pf->e2, stream));
+    if (timed) CK(cudaEventRecord(pf.e2, stream));
     c->launches += (L.ps > 0 ? 1 : 0) + (L.grid_r > 0 ? 1 : 0);      // (both, for every chunk of a render)
     return SS_OK;
 }
@@ -1196,7 +1203,7 @@ static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stre
     L.pp.n_inline = 1; L.pp.prefix[0] = 0; L.pp.prefix[1] = L.ps; L.pp.srcs[0] = s;
     CK(cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming));
     CK(cudaMemcpyAsync(d_src, &s, sizeof(s), cudaMemcpyHostToDevice, stream));  // k_rir_absmax / k_rir_direct read it
-    { int st = chunk_enqueue(c, L, stream, nullptr); if (st) return st; }
+    { int st = chunk_enqueue(c, L, stream, false); if (st) return st; }
     CK(cudaEventRecord(b->ready, stream));
     return SS_OK;
 }
@@ -1250,9 +1257,10 @@ extern "C" int ss_bank_create_host(ss_ctx* c, const float* rir, int32_t P, int32
 }
 
 // Describe items[first, last) (device pointers) in the next slot of the descriptor ring, copy the block and enqueue
-// the launches on `stream`.
-static int launch_chunk(ss_ctx* c, const ss_source* items, int first, int last, cudaStream_t stream, int buf = 0) {
-    const size_t need = chunk_scratch_bytes(items, first, last);
+// the launches on `stream`, with scratch buffer `buf`.
+static int launch_chunk(ss_ctx* c, const ss_source* items, const Shape* shapes, int first, int last,
+                        cudaStream_t stream, int buf) {
+    const size_t need = chunk_scratch_bytes(items, shapes, first, last);
     if (need > c->scratch_cap[buf]) {
         CK(cudaDeviceSynchronize());
         if (c->d_scratch[buf]) CK(cudaFree(c->d_scratch[buf]));
@@ -1261,21 +1269,14 @@ static int launch_chunk(ss_ctx* c, const ss_source* items, int first, int last, 
         CK(cudaMalloc(&c->d_scratch[buf], cap));
         c->scratch_cap[buf] = cap;
     }
-    const size_t bytes = chunk_desc_bytes(items, first, last);
+    const size_t bytes = chunk_desc_bytes(items, shapes, first, last);
     int slot; char *hblk, *dblk;
     { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
     static thread_local ChunkLaunch L;                  // holds 3.2 KB of kernel parameters: not on the stack
-    chunk_describe(items, first, last, hblk, dblk, c->d_scratch[buf], c->sm_count, &L);
+    chunk_describe(items, shapes, first, last, hblk, dblk, c->d_scratch[buf], c->sm_count, &L);
     CK(cudaMemcpyAsync(dblk, hblk, bytes, cudaMemcpyHostToDevice, stream));
     CK(cudaEventRecord(c->desc_ev[slot], stream));
-    ss_ctx::Prof pf;
-    if (c->profiling) {
-        CK(cudaEventCreate(&pf.e0)); CK(cudaEventCreate(&pf.e1)); CK(cudaEventCreate(&pf.e2));
-        pf.chunk = c->prof_chunk++;
-    }
-    const int st = chunk_enqueue(c, L, stream, c->profiling ? &pf : nullptr);
-    if (c->profiling) c->prof.push_back(pf);
-    return st;
+    return chunk_enqueue(c, L, stream, c->profiling);
 }
 
 // split [0, n) into chunks whose spectra fit the L2-sized budget
@@ -1305,31 +1306,33 @@ static void make_chunks_bytes(const std::vector<size_t>& sb, int64_t budget, std
     }
     cuts.push_back(n);
 }
-static void make_chunks(const ss_ctx* c, const ss_source* items, int n, std::vector<int>& cuts, int64_t budget = 0) {
-    if (budget <= 0) budget = c->chunk_bytes;
+static void make_chunks(const ss_source* items, const Shape* shapes, int n, int64_t budget, std::vector<int>& cuts) {
     std::vector<size_t> sb(n);
-    for (int i = 0; i < n; ++i) sb[i] = spectra_bytes(items[i]);
+    for (int i = 0; i < n; ++i) sb[i] = spectra_bytes(items[i], shapes[i]);
     make_chunks_bytes(sb, budget, cuts);
 }
 // Device path: sources are independent, so a batch is regrouped by the kernel variant its chunk would run - one
 // transform per item (aligned moving sources and static ones: k_render_fast), long RIRs (k_render<LONG>), everything
 // else (k_render<0, 0>) - and each group
 // is chunked on its own: one static source no longer sends the moving sources of its chunk through the generic kernel
-// (a SonicSet scene is 3 moving + 2 static sources).  `arranged` receives the regrouped items, `cuts` the chunk bounds.
-static void arrange_chunks(const ss_ctx* c, const ss_source* items, int n, std::vector<ss_source>& arranged, std::vector<int>& cuts) {
+// (a SonicSet scene is 3 moving + 2 static sources).  `arranged` / `arranged_shapes` receive the regrouped items and
+// their shapes, `cuts` the chunk bounds.
+static void arrange_chunks(const ss_ctx* c, const ss_source* items, const Shape* shapes, int n,
+                           std::vector<ss_source>& arranged, std::vector<Shape>& arranged_shapes, std::vector<int>& cuts) {
     arranged.clear(); arranged.reserve(n);
+    arranged_shapes.clear(); arranged_shapes.reserve(n);
     cuts.clear(); cuts.push_back(0);
     for (int cls = 0; cls < 3; ++cls) {
         const int lo = (int)arranged.size();
         for (int i = 0; i < n; ++i) {
-            const Shape sh = shape_of(items[i]);
-            const int k = sh.K > 1 ? 1 : ((sh.aligned || items[i].mode == SS_STATIC) ? 0 : 2);
-            if (k == cls) arranged.push_back(items[i]);
+            const Shape& sh = shapes[i];
+            const int k = sh.K > 1 ? 1 : (one_transform_per_item(sh.aligned, items[i].mode, sh.K) ? 0 : 2);
+            if (k == cls) { arranged.push_back(items[i]); arranged_shapes.push_back(sh); }
         }
         const int cnt = (int)arranged.size() - lo;
         if (cnt == 0) continue;
         std::vector<int> local;
-        make_chunks(c, arranged.data() + lo, cnt, local);
+        make_chunks(arranged.data() + lo, arranged_shapes.data() + lo, cnt, c->chunk_bytes, local);
         for (size_t q = 1; q < local.size(); ++q) cuts.push_back(lo + local[q]);
     }
 }
@@ -1346,54 +1349,70 @@ extern "C" int ss_debug_chunks(const int64_t* bytes, int32_t n, int64_t budget, 
     return (int)cuts.size();
 }
 
-static int validate_dev_items(const ss_ctx* c, const ss_source* items, int n_items) {
+// Validate a device-path batch and work out the shape of every source, once per call.
+static int shape_dev_items(const ss_ctx* c, const ss_source* items, int n_items, std::vector<Shape>& shapes) {
+    shapes.resize(n_items);
     for (int i = 0; i < n_items; ++i) {
         int st = validate_item_ctx(c, items[i]); if (st) return st;
         if (items[i].mode == SS_MOVING_BOUNDS && items[i].bounds_host &&
             !bounds_ok(items[i].bounds_host, items[i].P, items[i].N))
             return SS_ERR_INVALID;
+        shapes[i] = shape_of(items[i]);
     }
     return SS_OK;
 }
 
-extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, void* stream) {
+// Profiling: let the host enqueue a call's launches while the GPU idles, so that no timed interval contains a wait for
+// the host; chunk positions restart for the grouping in ss_get_profile.
+static int profile_start(ss_ctx* c, cudaStream_t stream) {
+    c->prof_chunk = 0;
+    k_delay<<<1, 1, 0, stream>>>(300000u);
+    CK(cudaGetLastError());
+    return SS_OK;
+}
+// Chunks run one after another on the caller's stream when there is only one, under SS_SINGLE_STREAM, and while
+// profiling (serialised kernels give clean per-kernel times).
+static bool chunks_serial(const ss_ctx* c, size_t n_chunks) { return n_chunks < 2 || c->single_stream || c->profiling; }
+// Enqueue chunks [0, n_chunks) behind `stream` through run(k, stream, scratch buffer): serially on `stream` with buffer
+// 0, or chunk k on internal stream and buffer k % kAux, forked from `stream` at ev_fork and joined back into it.  When
+// it returns, ev_join[i] marks the last use of buffer i (serially: ev_join[0]).
+template <class Run>
+static int run_chunks(ss_ctx* c, size_t n_chunks, cudaStream_t stream, cudaEvent_t ev_fork, const cudaEvent_t* ev_join,
+                      Run run) {
+    if (chunks_serial(c, n_chunks)) {
+        for (size_t k = 0; k < n_chunks; ++k) { int st = run(k, stream, 0); if (st) return st; }
+        CK(cudaEventRecord(ev_join[0], stream));
+        return SS_OK;
+    }
+    CK(cudaEventRecord(ev_fork, stream));
+    for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_aux[i], ev_fork, 0));
+    int rc = SS_OK;
+    for (size_t k = 0; k < n_chunks && rc == SS_OK; ++k) rc = run(k, c->s_aux[k % ss_ctx::kAux], (int)(k % ss_ctx::kAux));
+    for (int i = 0; i < ss_ctx::kAux; ++i) {
+        CK(cudaEventRecord(ev_join[i], c->s_aux[i]));
+        CK(cudaStreamWaitEvent(stream, ev_join[i], 0));
+    }
+    return rc;
+}
+
+extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, void* stream_) {
     if (!c || (!items && n_items > 0) || n_items < 0) return SS_ERR_INVALID;
     if (n_items == 0) return SS_OK;
     CK(cudaSetDevice(c->device));
-    { int st = validate_dev_items(c, items, n_items); if (st) return st; }
-    { int st = wait_banks(items, n_items, (cudaStream_t)stream); if (st) return st; }   // before the fork: every chunk
+    const cudaStream_t stream = (cudaStream_t)stream_;
+    std::vector<Shape> shapes;
+    { int st = shape_dev_items(c, items, n_items, shapes); if (st) return st; }
+    { int st = wait_banks(items, n_items, stream); if (st) return st; }   // before the fork: every chunk
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
-    arrange_chunks(c, items, n_items, arranged, cuts);
-    items = arranged.data();
+    std::vector<Shape> arranged_shapes;
+    arrange_chunks(c, items, shapes.data(), n_items, arranged, arranged_shapes, cuts);
     const size_t n_chunks = cuts.size() - 1;
-    if (c->profiling) {
-        // let the host enqueue this call's launches while the GPU idles, so no timed interval contains a wait for
-        // the host; chunk positions restart for the grouping in ss_get_profile
-        c->prof_chunk = 0;
-        k_delay<<<1, 1, 0, (cudaStream_t)stream>>>(300000u);
-        CK(cudaGetLastError());
-    }
-    if (n_chunks < 2 || c->single_stream || c->profiling) {      // profiling: kernels serialised -> clean per-kernel times
-        for (size_t k = 0; k < n_chunks; ++k) {
-            int st = launch_chunk(c, items, cuts[k], cuts[k + 1], (cudaStream_t)stream, 0);
-            if (st) return st;
-        }
-        CK(cudaEventRecord(c->ev_join[0], (cudaStream_t)stream));      // scratch buffer 0 busy until here
-        return SS_OK;
-    }
-    // fork: chunks alternate between two internal streams / scratch buffers; join back into `stream`
-    CK(cudaEventRecord(c->ev_fork, (cudaStream_t)stream));
-    for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_aux[i], c->ev_fork, 0));
-    c->ring_pos = 0;                                    // slot k % kRing <-> stream k % kAux
-    int rc = SS_OK;
-    for (size_t k = 0; k < n_chunks && rc == SS_OK; ++k)
-        rc = launch_chunk(c, items, cuts[k], cuts[k + 1], c->s_aux[k % ss_ctx::kAux], (int)(k % ss_ctx::kAux));
-    for (int i = 0; i < ss_ctx::kAux; ++i) {
-        CK(cudaEventRecord(c->ev_join[i], c->s_aux[i]));
-        CK(cudaStreamWaitEvent((cudaStream_t)stream, c->ev_join[i], 0));
-    }
-    return rc;
+    if (c->profiling) { int st = profile_start(c, stream); if (st) return st; }
+    if (!chunks_serial(c, n_chunks)) c->ring_pos = 0;  // forked: descriptor ring slot k % kRing <-> stream k % kAux
+    return run_chunks(c, n_chunks, stream, c->ev_fork, c->ev_join, [&](size_t k, cudaStream_t s, int buf) {
+        return launch_chunk(c, arranged.data(), arranged_shapes.data(), cuts[k], cuts[k + 1], s, buf);
+    });
 }
 
 // ----------------------------------------------------------------------------- plans (device path)
@@ -1446,19 +1465,20 @@ static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double
     return d;
 }
 
-static int plan_build(ss_plan* p, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes) {
+static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
+                      const ss_plan_mix* mixes, int n_mixes) {
     ss_ctx* c = p->c;
-    const ss_source* caller_items = items;
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
-    arrange_chunks(c, items, n_items, arranged, cuts);
-    items = arranged.data();
+    std::vector<Shape> arranged_shapes;
+    arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts);
+    const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     const size_t n_chunks = cuts.size() - 1;
     std::vector<size_t> off(n_chunks + 1, 0);
     size_t scratch_need[ss_ctx::kAux] = {};
     for (size_t k = 0; k < n_chunks; ++k) {
-        off[k + 1] = off[k] + align_up(chunk_desc_bytes(items, cuts[k], cuts[k + 1]), 256);
-        const size_t sb = chunk_scratch_bytes(items, cuts[k], cuts[k + 1]);
+        off[k + 1] = off[k] + align_up(chunk_desc_bytes(items, shapes, cuts[k], cuts[k + 1]), 256);
+        const size_t sb = chunk_scratch_bytes(items, shapes, cuts[k], cuts[k + 1]);
         size_t& m = scratch_need[n_chunks < 2 ? 0 : k % ss_ctx::kAux];
         m = sb > m ? sb : m;
     }
@@ -1474,20 +1494,15 @@ static int plan_build(ss_plan* p, const ss_source* items, int n_items, const ss_
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
     std::vector<char> host(desc_bytes + 256);
     p->chunks.resize(n_chunks);
-    p->launches_per_run = 0;
-    for (size_t k = 0; k < n_chunks; ++k) {
-        chunk_describe(items, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
+    for (size_t k = 0; k < n_chunks; ++k)
+        chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
                        p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k]);
-        p->launches_per_run += (p->chunks[k].host_tables ? 2 : 3) + (p->chunks[k].any_norm ? 1 : 0) +
-                               (p->chunks[k].grid_direct > 0 ? 1 : 0);
-    }
     for (int k = 0; k < n_mixes; ++k)
         ((MixItem*)(host.data() + mix_off))[k] =
             mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
     if (n_mixes > 0) {
         p->d_mix = (const MixItem*)(p->d_desc + mix_off);
         p->n_mix = n_mixes;
-        p->launches_per_run += 4;
     }
     CK(cudaMemcpy(p->d_desc, host.data(), scr_off, cudaMemcpyHostToDevice));
     return SS_OK;
@@ -1560,7 +1575,8 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
-    { int st = validate_dev_items(c, items, n_items); if (st) return st; }
+    std::vector<Shape> shapes;
+    { int st = shape_dev_items(c, items, n_items, shapes); if (st) return st; }
     { int st = validate_mixes(items, n_items, mixes, n_mixes); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
@@ -1569,7 +1585,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_bank* b = const_cast<ss_bank*>(items[i].rir_bank);
         if (b && std::find(p->banks.begin(), p->banks.end(), b) == p->banks.end()) p->banks.push_back(b);
     }
-    const int st = plan_build(p, items, n_items, mixes, n_mixes);
+    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     *out = p;
     return SS_OK;
@@ -1585,24 +1601,13 @@ extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items
     return plan_create(c, items, n_items, mixes, n_mixes, out);
 }
 
-// the launches of every chunk, forked over the context's internal streams and joined back into `stream`, then the
-// mixtures (which read every chunk's outputs) on `stream`
+// the launches of every chunk (run_chunks), then the mixtures (which read every chunk's outputs) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
-    const size_t n_chunks = p->chunks.size();
-    if (n_chunks < 2 || c->single_stream) {
-        for (size_t k = 0; k < n_chunks; ++k) { int st = chunk_enqueue(c, p->chunks[k], stream, nullptr); if (st) return st; }
-    } else {
-        CK(cudaEventRecord(p->ev_fork, stream));
-        for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_aux[i], p->ev_fork, 0));
-        int rc = SS_OK;
-        for (size_t k = 0; k < n_chunks && rc == SS_OK; ++k) rc = chunk_enqueue(c, p->chunks[k], c->s_aux[k % ss_ctx::kAux], nullptr);
-        for (int i = 0; i < ss_ctx::kAux; ++i) {
-            CK(cudaEventRecord(p->ev_join[i], c->s_aux[i]));
-            CK(cudaStreamWaitEvent(stream, p->ev_join[i], 0));
-        }
-        if (rc) return rc;
-    }
+    const int rc = run_chunks(c, p->chunks.size(), stream, p->ev_fork, p->ev_join, [&](size_t k, cudaStream_t s, int) {
+        return chunk_enqueue(c, p->chunks[k], s, c->profiling);
+    });
+    if (rc) return rc;
     return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream) : SS_OK;
 }
 
@@ -1612,20 +1617,9 @@ extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     CK(cudaSetDevice(c->device));
     for (ss_bank* b : p->banks) CK(cudaStreamWaitEvent(stream, b->ready, 0));    // (outside any capture)
-    if (c->profiling) {
-        // per-kernel timing: chunks one after the other on the caller's stream, events around every launch
-        c->prof_chunk = 0;
-        k_delay<<<1, 1, 0, stream>>>(300000u);
-        CK(cudaGetLastError());
-        for (auto& L : p->chunks) {
-            ss_ctx::Prof pf;
-            CK(cudaEventCreate(&pf.e0)); CK(cudaEventCreate(&pf.e1)); CK(cudaEventCreate(&pf.e2));
-            pf.chunk = c->prof_chunk++;
-            int st = chunk_enqueue(c, L, stream, &pf);
-            c->prof.push_back(pf);
-            if (st) return st;
-        }
-        return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream) : SS_OK;
+    if (c->profiling) {                                 // per-kernel timing: no graph, chunks one after the other
+        { int st = profile_start(c, stream); if (st) return st; }
+        return plan_enqueue(p, stream);
     }
     if (!p->exec && !p->graph_failed && !c->no_graph) {
         const int64_t launches_before = c->launches;
@@ -1638,7 +1632,8 @@ extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
         }
         if (ok) ok = cudaGraphInstantiate(&p->exec, g, 0) == cudaSuccess;
         if (g) cudaGraphDestroy(g);
-        c->launches = launches_before;                      // nothing ran while capturing
+        p->launches_per_run = (int)(c->launches - launches_before);      // what the graph launches at every run ...
+        c->launches = launches_before;                                    // ... none of which ran while capturing
         if (!ok) { p->exec = nullptr; p->graph_failed = true; (void)cudaGetLastError(); }
     }
     if (p->exec) {
@@ -1655,14 +1650,9 @@ extern "C" int ss_plan_is_graph(const ss_plan* p) { return p ? (p->exec ? 1 : 0)
 // What the host path copies in and out for one source: dry samples [xa, xb), RIR positions [pa, pb], idx / w entries
 // [ia, ib), and C * wl output floats per stem - the whole source, or a windowed source's read set (window_shape)
 struct ReadSet { int xa, xb, pa, pb, ia, ib, wl; };
-static ReadSet read_set(const ss_source& it) {
+static ReadSet read_set(const ss_source& it, const Shape& sh) {
     ReadSet r = {0, it.N, 0, it.P - 1, 0, it.N, it.N};
-    if (it.win_len > 0) {
-        ss_source h = it;
-        if (h.mode == SS_MOVING_BOUNDS) h.bounds_host = h.bounds;          // host pointers: the trajectory is visible
-        const Shape sh = shape_of(h);
-        r.xa = sh.xa; r.xb = sh.xb; r.pa = sh.pa; r.pb = sh.pb; r.ia = sh.ia; r.ib = sh.ib; r.wl = it.win_len;
-    }
+    if (sh.win) { r.xa = sh.xa; r.xb = sh.xb; r.pa = sh.pa; r.pb = sh.pb; r.ia = sh.ia; r.ib = sh.ib; r.wl = it.win_len; }
     return r;
 }
 // idx (SS_MOVING_INDEXED): the entries the render reads (the bounds table is checked whole, before read_set plans from it)
@@ -1694,6 +1684,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     // every stem with a target shares one sample rate (ss_loudness_dev runs one set of filter coefficients per call);
     // checked against the first source that has a target, so that the answer does not depend on the chunking
     const ss_post_lufs* first_post = nullptr;
+    std::vector<Shape> shapes(n_items);
     std::vector<ReadSet> rset(n_items);
     for (int i = 0; i < n_items; ++i) {
         int st = validate_item_ctx(c, items[i]); if (st) return st;
@@ -1702,7 +1693,11 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         // a moving window's read set depends on a start that only the device knows
         if (items[i].win_start_dev) return SS_ERR_INVALID;
         if (items[i].mode == SS_MOVING_BOUNDS && !bounds_ok(items[i].bounds, items[i].P, items[i].N)) return SS_ERR_INVALID;
-        rset[i] = read_set(items[i]);
+        // planned as it is rendered: with the trajectory in host memory (bounds_host = bounds, as below)
+        ss_source h = items[i];
+        if (h.mode == SS_MOVING_BOUNDS) h.bounds_host = h.bounds;
+        shapes[i] = shape_of(h);
+        rset[i] = read_set(items[i], shapes[i]);
         st = check_idx_host(items[i], rset[i]); if (st) return st;
         if (post && post[i].brk) {
             if (!post[i].blk_lo || !post[i].blk_hi || post[i].n_e <= 0 || post[i].rate <= 0 || items[i].C > 8) return SS_ERR_INVALID;
@@ -1715,7 +1710,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     // banks built asynchronously on the caller's stream: every render of this call (on s_cmp) comes after them
     { int st = wait_banks(items, n_items, c->s_cmp); if (st) return st; }
     std::vector<int> cuts;
-    make_chunks(c, items, n_items, cuts, c->chunk_bytes_host);
+    make_chunks(items, shapes.data(), n_items, c->chunk_bytes_host, cuts);
     std::vector<ss_source> dev(n_items);
     std::vector<ss_loud_item> loud;
     std::vector<ScaleItem> direct_gain;                  // direct-path stems scaled by their reverberant stem's gain
@@ -1836,7 +1831,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         }
         CK(cudaEventRecord(sl.ev_in, c->s_in));
         CK(cudaStreamWaitEvent(c->s_cmp, sl.ev_in, 0));
-        rc = launch_chunk(c, dev.data(), first, last, c->s_cmp);
+        rc = launch_chunk(c, dev.data(), shapes.data(), first, last, c->s_cmp, 0);
         if (rc != SS_OK) break;
         if (!loud.empty()) {
             cudaStream_t s_l = c->s_aux[k % ss_ctx::kAux];

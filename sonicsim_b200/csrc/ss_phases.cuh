@@ -126,6 +126,9 @@ SS_HD int range_ctas(const Source& s) { return (s.nblk_max + 7) >> 3; }       //
 SS_HD int items_per_set(const Source& s) { return s.mode == MODE_STATIC ? (s.C + 1) >> 1 : s.C; }
 SS_HD int items_per_block(const Source& s) { return items_per_set(s) * (s.cut ? 2 : 1); }
 SS_HD int max_render_items(const Source& s) { return s.nblk_max * items_per_block(s); }
+// Every render item of the source needs one inverse transform (k_render_fast): aligned blocking, or a static source
+// with one RIR partition.  Everything else goes through k_render, with LONG when K > 1.
+SS_HD bool one_transform_per_item(int aligned, int mode, int K) { return aligned || (mode == MODE_STATIC && K == 1); }
 
 // ---- the block table: one planner for the host, k_blocks and the CPU emulation.
 // blocks of one segment under aligned blocking

@@ -287,7 +287,7 @@ static void emu_source(const float* x, const float* rir, const float2* bank, con
     const int nr = win_blocks(S) * items_per_block(S);
     const int grid = nr < 3 ? nr : 3;              // a few persistent CTAs, each looping over many items
     for (int cta = 0; cta < grid; ++cta) {
-        if (S.aligned || (mode == MODE_STATIC && S.K == 1)) cta_render_fast(items.data(), nr, cta, grid, T);
+        if (one_transform_per_item(S.aligned, mode, S.K)) cta_render_fast(items.data(), nr, cta, grid, T);
         else cta_render(items.data(), nr, cta, grid, T, false, S.K > 1);
     }
     if (win_stats) { win_stats[0] = S.nblk_max; win_stats[1] = ws.k1 - ws.k0; win_stats[2] = S.h_row0; win_stats[3] = S.h_rows; }
