@@ -300,7 +300,8 @@ typedef struct {
 } ss_loud_item;
 
 /* Device pointers, asynchronous on `stream`; all items share one sample rate; C <= 8 (channel gains
- * 1, 1, 1, 1.41, 1.41, then 1 for channels 5-7), else SS_ERR_UNSUPPORTED. */
+ * 1, 1, 1, 1.41, 1.41, then 1 for channels 5-7), else SS_ERR_UNSUPPORTED; at most 65535 items per call
+ * (more: SS_ERR_UNSUPPORTED, before any copy or launch). */
 int ss_loudness_dev(ss_ctx* ctx, const ss_loud_item* items, int n_items, void* stream);
 
 /* One stem in host memory, N*C floats in a dense (N, C) or (C, N) layout given by the strides (other

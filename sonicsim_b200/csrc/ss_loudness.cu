@@ -231,6 +231,7 @@ static LoudItem to_item(const ss_loud_item& a) {
 extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items, void* stream_) {
     if (!c || (!items && n_items > 0) || n_items < 0) return SS_ERR_INVALID;
     if (n_items == 0) return SS_OK;
+    if (n_items > 65535) return SS_ERR_UNSUPPORTED;             // one gridDim.y row per item (k_kw_scan, k_loud_scale)
     CK(cudaSetDevice(c->device));
     cudaStream_t stream = (cudaStream_t)stream_;
     for (int i = 0; i < n_items; ++i) {

@@ -151,6 +151,45 @@ def test_loudness_dev_does_not_depend_on_the_partition(case):
         check_stem(s, ref)
 
 
+def _copies(s, n):
+    """n measure-only items over the data of Stem `s`, each with its own scratch and a NaN-filled result."""
+    from sonicsim_b200 import _lib
+    per = s.scratch.numel()
+    scratch = torch.empty(n * per, dtype=torch.float64, device="cuda")
+    res = torch.full((n, 2), NAN, dtype=torch.float64, device="cuda")
+    arr = (_lib.SsLoudItem * n)()
+    for i in range(n):
+        it = _lib.SsLoudItem.from_buffer_copy(s.item)
+        it.out, it.scratch, it.result = None, scratch.data_ptr() + 8 * per * i, res[i].data_ptr()
+        arr[i] = it
+    return arr, scratch, res
+
+
+def test_loudness_dev_item_limit():
+    """One gridDim.y row per item in k_kw_scan and k_loud_scale: 65536 items are refused (SS_ERR_UNSUPPORTED) before
+    anything is written; 65535 measure-only items over one tiny stem are accepted and each gives the single item's
+    result, which matches the float64 reference."""
+    from sonicsim_b200 import _lib, render
+    R = render.default_renderer()
+    sr, N = 16000, 1600
+    x = stems(5, N, 1, sr)
+    assert_clear_of_gates(x, sr, block_size_of(N, sr))
+    one = Stem(x, sr, -23.0, "cn", "none")
+    assert loudness_dev([one]) == 0
+    check_stem(one)
+    want = one.res.cpu().numpy()
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    arr, scratch, res = _copies(one, 65536)
+    assert R.lib.ss_loudness_dev(R.ctx, arr, 65536, stream) == _lib.SS_ERR_UNSUPPORTED
+    torch.cuda.synchronize()
+    assert torch.isnan(res).all()
+    assert R.lib.ss_loudness_dev(R.ctx, arr, 65535, stream) == 0
+    torch.cuda.synchronize()
+    got = res.cpu().numpy()
+    assert np.array_equal(got[:65535], np.broadcast_to(want, (65535, 2)))
+    assert np.isnan(got[65535]).all()
+
+
 def test_loudness_dev_mixed_rates_in_one_call_are_rejected():
     a = Stem(stems(1, 8000, 2, 16000), 16000, -20.0)
     b = Stem(stems(2, 24000, 2, 48000), 48000, -20.0)
