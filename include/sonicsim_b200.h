@@ -31,6 +31,7 @@ extern "C" {
 
 typedef struct ss_ctx ss_ctx;
 typedef struct ss_bank ss_bank;
+typedef struct ss_pool ss_pool;
 
 typedef enum {
     SS_OK = 0,
@@ -92,6 +93,8 @@ typedef struct {
     const ss_bank* rir_bank;  /* RIR spectrum bank (version 103) instead of `rir`, which is then NULL; see below   */
     const int32_t* win_start_dev; /* moving window (version 104): DEVICE pointer to the start, read at every run in
                                    * place of win_start; see below                                                  */
+    const ss_pool* pool;      /* pooled slot (version 106): the source rendered is the candidate of `pool` ...      */
+    const int32_t* pick_dev;  /* ... named by the int32 at this DEVICE pointer, read at every run; see below         */
 } ss_source;                  /* fields appended since version 100: a zeroed (memset) struct leaves them off      */
 
 /* Time window (win_len > 0, version 102): the source renders only output samples [win_start, win_start + win_len)
@@ -168,8 +171,50 @@ int ss_bank_create_host(ss_ctx* ctx, const float* rir, int32_t P, int32_t C, int
 int64_t ss_bank_bytes(const ss_bank* bank);   /* device bytes held */
 void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their context */
 
+/* ---- source pools (version 106): the dataloader's random choices of separation/look2hear/datas/movingdatamodule.py
+ * :57-59 (`random.choice(self.data_dirs)`, `random.sample(range(1, 4), num_spks)`) and :68-77 (the scene's noise) made
+ * on the device.  A pool is a set of banked candidate sources, validated and uploaded once.  A pooled slot of a plan
+ * (ss_source.pool + pick_dev) renders, at every run, the candidate named by the int32 at pick_dev: its dry signal,
+ * trajectory, N, P and bank.  The slot's outputs, window length, flags and mixture membership stay bound.  Bits, blocking
+ * and kernel variant are those of the picked candidate rendered as a windowed source at the same (clamped) start under
+ * the pool's blocking (below); when every candidate would choose that blocking on its own, a pooled output equals
+ * ss_render_dev of the picked candidate with the same window, bit for bit.
+ *
+ * Candidates (every violation is SS_ERR_INVALID, before anything is allocated):
+ *   - 1 <= n <= 2^24;
+ *   - banked: rir == NULL, rir_bank set, a bank of this context, with the candidate's P, C and L; `x` set;
+ *   - one `mode` for all, SS_MOVING_BOUNDS or SS_STATIC (SS_MOVING_INDEXED is refused), one C, one L;
+ *   - a moving candidate has `bounds` and `bounds_host` (ascending from 0 to N), so that the pool's blocking and table
+ *     sizes are exact; idx and w are NULL;
+ *   - out, out_direct, flags, direct_taps, win_start, win_len, win_start_dev, pool and pick_dev are zero.
+ * Banks with and without a direct set may be mixed in one pool; the direct rule is enforced per slot.
+ * Blocking: aligned if every candidate would choose aligned blocking on its own (ss_debug_plan), otherwise the
+ * 4096-sample grid for all of them, so the kernel variant of a pooled slot is fixed when the pool is created.
+ * The pool copies what it needs (including the bounds_host values); the candidates' device buffers (x, bounds) and banks
+ * must outlive the pool.  ss_pool_create returns when the pool's table is in device memory; the pool records one event
+ * behind the construction of all its banks, which every plan run that uses the pool waits on.
+ *
+ * A pooled slot (every violation is SS_ERR_INVALID, before anything is allocated):
+ *   - x, rir, rir_bank, bounds, bounds_host, idx and w are NULL, N and P are 0; pool of this context; pick_dev a 4-byte
+ *     aligned device pointer;
+ *   - mode, C and L are the pool's;
+ *   - win_len > 0 with a fixed win_start (win_start + win_len <= every candidate's N) or a win_start_dev (win_start == 0
+ *     and win_len <= every candidate's N); the window start is clamped against the picked candidate's N (bit 2);
+ *   - SS_DIRECT_TARGET only if every candidate's bank holds a direct set with the slot's direct_taps; no
+ *     SS_RIR_NORMALIZE (normalisation is a property of the banks).
+ * ss_plan_create and ss_plan_create_mix take pooled slots; ss_render_dev, ss_render_host and ss_render_host_ex refuse
+ * them (SS_ERR_INVALID).  The pick is read when the run's first kernel reaches it (as win_start_dev); a pick outside
+ * [0, n) is clamped into that range and ss_device_errors reports bit 3.  Read set of a pooled slot: the picked
+ * candidate's whole x and bounds (and its bank); for the mixture range checks of ss_plan_create_mix, every candidate's x
+ * and bounds and the pick.  A chunk that holds a pooled slot builds its block tables on the device, sized once, when the
+ * plan is created, for the largest any candidate needs: 3 kernel launches per chunk, as with a moving window.
+ * Lifetime: a pool must outlive every plan that uses it; ss_pool_destroy waits for the device before it frees it. */
+int ss_pool_create(ss_ctx* ctx, const ss_source* candidates, int n, ss_pool** out);
+int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact candidate entries */
+void ss_pool_destroy(ss_pool* pool);          /* destroy pools after the plans that use them, before their context */
+
 /* library / build identification */
-int ss_version(void);        /* 105: mixtures in plans (ss_plan_create_mix) */
+int ss_version(void);        /* 106: source pools (ss_pool_create, pooled slots in plans) */
 const char* ss_strerror(int status);
 int ss_last_cuda_error(void);
 
@@ -194,7 +239,7 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * offending samples as silence (clamped positions) and set a bit that this call returns and clears after waiting for
  * the device: bit 0 = an interp_index outside [0, P - 2], bit 1 = a device-side bounds table that is not ascending from
  * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
- * (rendered clamped into that range).  The Python device API raises IndexError / ValueError from it on request
+ * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped).  The Python device API raises IndexError / ValueError from it on request
  * (Renderer.check_device_errors). */
 int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
 

@@ -71,7 +71,7 @@ class SsSource(ctypes.Structure):
                 ("mode", ctypes.c_int32), ("flags", ctypes.c_int32), ("bounds_host", ctypes.c_void_p),
                 ("out_direct", ctypes.c_void_p), ("direct_taps", ctypes.c_int32),
                 ("win_start", ctypes.c_int32), ("win_len", ctypes.c_int32), ("rir_bank", ctypes.c_void_p),
-                ("win_start_dev", ctypes.c_void_p)]
+                ("win_start_dev", ctypes.c_void_p), ("pool", ctypes.c_void_p), ("pick_dev", ctypes.c_void_p)]
 
 
 def _stale():
@@ -143,6 +143,11 @@ def load():
         lib.ss_bank_bytes.restype = i64
         lib.ss_bank_destroy.argtypes = [vp]
         lib.ss_bank_destroy.restype = None
+        lib.ss_pool_create.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(vp)]
+        lib.ss_pool_bytes.argtypes = [vp]
+        lib.ss_pool_bytes.restype = i64
+        lib.ss_pool_destroy.argtypes = [vp]
+        lib.ss_pool_destroy.restype = None
         lib.ss_render_host.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int]
         lib.ss_render_host_ex.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPostLufs)]
         lib.ss_convolve_fixed_receiver.argtypes = [vp, vp, vp, vp, i32, i32, i32]
@@ -175,7 +180,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_destroy", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

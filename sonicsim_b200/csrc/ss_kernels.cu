@@ -42,7 +42,7 @@ using namespace ss;
 // Device-path trajectory check: the kernels cannot raise, so a source whose device-side trajectory breaks the contract
 // of ss_render_dev (idx outside [0, P - 2]; bounds not ascending from 0 to N) sets a bit here; ss_device_errors reads
 // and clears it.  bit 0: index out of range, bit 1: bounds not monotone / not ending at N, bit 2: a moving window's
-// start outside [0, N - win_len] (clamped).
+// start outside [0, N - win_len] (clamped), bit 3: a pooled slot's pick outside [0, n) (clamped).
 __device__ unsigned g_dev_err;
 
 // twiddle tables, filled from the host in double precision (ss_create)
@@ -112,13 +112,22 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 // full plan; a windowed one's holds the full plan's blocks [g0, g1) (window_span, cut to the table size).  A moving
 // window first reads its start from device memory, clamps it (bit 2 of g_dev_err) and stores it as counts[4], where
 // the window search here and k_prepare's range warps take it; its table is sized for every start (window_table_cap).
+// A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate into its Source in the
+// descriptor block, which is why k_prepare then reads the Source table from global memory (k_prepare<false>).
 __global__ void __launch_bounds__(256)
-k_blocks(const Source* __restrict__ srcs, int n_src, int* __restrict__ total_items) {
+k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     for (int si = warp; si < n_src; si += nwarps) {
-        const Source& S = srcs[si];
+        Source& S = srcs[si];
         int g0 = 0, g1 = S.nblk_max;
         if (S.h_rows) {
+            const PoolEntry* const pool = pool_table(S);
+            if (pool && lane == 0) {
+                bool bad;
+                pick_candidate(S, pool[clamp_pick(*pick_ptr(S), pool_size(S), bad)]);
+                if (bad) atomicOr(&g_dev_err, 8u);
+            }
+            __syncwarp();
             const int* const ws_dev = win_start_ptr(S);
             if (ws_dev && lane == 0) {
                 bool bad;
@@ -589,7 +598,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 105; }
+extern "C" int ss_version(void) { return 106; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -780,6 +789,20 @@ struct ss_bank {
     int P = 0, C = 0, L = 0, K = 0, flags = 0, direct_taps = 0;
     cudaEvent_t ready = nullptr;          // recorded behind the launches that build it; every use waits on it
 };
+// Source pool: the candidates' compact entries in one device allocation, and on the host what validation, sizing and the
+// mixture range checks need.
+struct ss_pool {
+    ss_ctx* c = nullptr;
+    PoolEntry* table = nullptr;           // device, n entries
+    int n = 0, mode = 0, C = 0, L = 0, K = 0, aligned = 0;
+    int n_min = 0, p_max = 0;             // shortest candidate (window rule), most positions (rstep table)
+    int direct_taps = 0;                  // > 0: every candidate's bank holds a direct set with these taps
+    std::vector<PoolEntry> host;          // the table's entries
+    std::vector<int32_t> bounds_host;     // every moving candidate's bounds, back to back
+    std::vector<int64_t> bounds_off;      // candidate i's bounds at bounds_host[bounds_off[i]]
+    std::vector<std::pair<int, int>> caps;  // (win_len, table size) already worked out (pool_table_cap)
+    cudaEvent_t ready = nullptr;          // behind the construction of every candidate's bank
+};
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
 static int wait_banks(const ss_source* items, int n, cudaStream_t stream) {
@@ -804,6 +827,7 @@ static int validate_bank_use(const ss_source& it) {
     return SS_OK;
 }
 static int validate_item(const ss_source& it) {
+    if (it.pool || it.pick_dev) return SS_ERR_INVALID;              // pooled slots: plans only (validate_pooled)
     if (!it.x || !it.out || (it.rir != nullptr) == (it.rir_bank != nullptr)) return SS_ERR_INVALID;   // rir xor bank
     if (it.N <= 0 || it.C <= 0 || it.L <= 0 || it.P <= 0) return SS_ERR_INVALID;
     // 32-bit sample / table indices inside the kernels: leave one FFT of headroom below 2^31
@@ -837,16 +861,36 @@ static bool bounds_ok(const int32_t* b, int P, int N) {
     for (int q = 0; q + 1 < P; ++q) if (b[q + 1] < b[q]) return false;
     return true;
 }
+// A pooled slot against its pool (include/sonicsim_b200.h): no source fields of its own, the pool's mode / C / L, a
+// window every candidate holds, a direct target only when every candidate's bank has the slot's direct set.
+static int validate_pooled(const ss_ctx* c, const ss_source& it) {
+    const ss_pool* pl = it.pool;
+    if (pl->c != c || !it.pick_dev || ((uintptr_t)it.pick_dev & 3) || !it.out) return SS_ERR_INVALID;
+    if (it.x || it.rir || it.rir_bank || it.bounds || it.bounds_host || it.idx || it.w || it.N || it.P)
+        return SS_ERR_INVALID;
+    if (it.mode != pl->mode || it.C != pl->C || it.L != pl->L) return SS_ERR_INVALID;
+    if (it.win_len <= 0 || it.win_start < 0 || (int64_t)it.win_start + it.win_len > (int64_t)pl->n_min)
+        return SS_ERR_INVALID;
+    if (it.win_start_dev && (it.win_start != 0 || ((uintptr_t)it.win_start_dev & 3))) return SS_ERR_INVALID;
+    if (it.flags & ~SS_DIRECT_TARGET) return SS_ERR_INVALID;
+    if ((it.flags & SS_DIRECT_TARGET) && (!it.out_direct || it.out_direct == it.out || it.direct_taps < 1 ||
+                                          it.direct_taps != pl->direct_taps))
+        return SS_ERR_INVALID;
+    return SS_OK;
+}
 // SS_DIRECT_TARGET: a second RIR set (spectra, items per block) and the P*C cut table
 static int direct_sets(const ss_source& it) { return (it.flags & SS_DIRECT_TARGET) ? 2 : 1; }
+// spectra and cuts in a bank (a pooled slot's: in its candidates' banks), not in the chunk's scratch
+static bool banked(const ss_source& it) { return it.rir_bank || it.pool; }
 // RIR sets and cut table in the chunk's scratch: none for a banked source, whose spectra and cuts live in its bank
-static int scratch_sets(const ss_source& it) { return it.rir_bank ? 0 : direct_sets(it); }
+static int scratch_sets(const ss_source& it) { return banked(it) ? 0 : direct_sets(it); }
 static size_t cut_bytes(const ss_source& it) {
-    return ((it.flags & SS_DIRECT_TARGET) && !it.rir_bank) ? align_up(sizeof(int) * (size_t)it.P * it.C, 256) : 0;
+    return ((it.flags & SS_DIRECT_TARGET) && !banked(it)) ? align_up(sizeof(int) * (size_t)it.P * it.C, 256) : 0;
 }
 // shapes derived from one ss_source
 struct Shape {
     int K, nb, aligned, nblk_max, per, max_items;
+    int p_max;                // rstep entries: P, or the largest candidate's P for a pooled slot
     // time window (win_len > 0); zero otherwise
     int win;
     int tab_host;             // the window's blocks are known here (all but aligned blocking over device-side bounds)
@@ -934,7 +978,36 @@ static Shape shape_of(const ss_source& it) {
     s.aligned = choose_aligned(it, s.K, s.nb) ? 1 : 0;
     s.nblk_max = table_cap(s.aligned, s.nb, it.P);
     s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
+    s.p_max = it.P;
     if (it.win_len > 0) window_shape(it, s);
+    s.max_items = s.nblk_max * s.per;
+    return s;
+}
+// A pooled slot: a moving window (tables built by k_blocks, the whole candidate read) under the pool's blocking, sized
+// once for the largest table, position count and item count any candidate needs.  The table sizes are worked out once
+// per pool and window length.
+static Shape shape_pooled(const ss_source& it) {
+    ss_pool* pl = const_cast<ss_pool*>(it.pool);
+    Shape s;
+    memset(&s, 0, sizeof(s));
+    s.K = pl->K; s.aligned = pl->aligned; s.win = 1; s.p_max = pl->p_max;
+    s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
+    s.nblk_max = -1;
+    for (const auto& q : pl->caps) if (q.first == it.win_len) s.nblk_max = q.second;
+    if (s.nblk_max < 0) {
+        std::vector<const int*> bounds;
+        std::vector<int> N(pl->n), P(pl->n);
+        int cap_max = 0;
+        for (int i = 0; i < pl->n; ++i) {
+            N[i] = pl->host[i].N; P[i] = pl->host[i].P;
+            cap_max = std::max(cap_max, table_cap(pl->aligned, (N[i] + kB - 1) / kB, P[i]));
+            if (pl->mode == SS_MOVING_BOUNDS) bounds.push_back(pl->bounds_host.data() + pl->bounds_off[i]);
+        }
+        std::vector<Block> full((size_t)cap_max);
+        s.nblk_max = pool_table_cap(pl->aligned, bounds.empty() ? nullptr : bounds.data(), N.data(), P.data(), pl->n,
+                                    it.win_len, pl->K, full.data());
+        pl->caps.push_back({it.win_len, s.nblk_max});
+    }
     s.max_items = s.nblk_max * s.per;
     return s;
 }
@@ -943,7 +1016,7 @@ static size_t rir_rows(const ss_source& it, const Shape& sh) { return sh.win ? (
 static size_t spectra_bytes(const ss_source& it, const Shape& sh) {
     return (rir_rows(it, sh) * scratch_sets(it) + sh.nblk_max) * kSpec * sizeof(float2) +
            (size_t)sh.max_items * sizeof(RItem) +
-           align_up(sizeof(Block) * (size_t)sh.nblk_max, 256) + align_up(sizeof(double) * (size_t)it.P, 256) + 256 +
+           align_up(sizeof(Block) * (size_t)sh.nblk_max, 256) + align_up(sizeof(double) * (size_t)sh.p_max, 256) + 256 +
            ((it.flags & SS_RIR_NORMALIZE) ? 512 : 0) + cut_bytes(it);
 }
 
@@ -967,7 +1040,8 @@ extern "C" int ss_debug_plan(const ss_source* item, int32_t* blocks_out, int32_t
     if (item->mode == SS_MOVING_BOUNDS && (!item->bounds_host || item->P < 2)) return SS_ERR_INVALID;
     if (item->mode == SS_MOVING_BOUNDS && !bounds_ok(item->bounds_host, item->P, item->N)) return SS_ERR_INVALID;
     if (item->win_len < 0 || item->win_start < 0 || (item->win_len == 0 && item->win_start != 0) ||
-        (int64_t)item->win_start + item->win_len > (int64_t)item->N || item->win_start_dev)
+        (int64_t)item->win_start + item->win_len > (int64_t)item->N || item->win_start_dev || item->pool ||
+        item->pick_dev)
         return SS_ERR_INVALID;
     const Shape sh = shape_of(*item);
     const int first = sh.win ? sh.k0 - sh.g0 : 0;
@@ -1001,15 +1075,17 @@ static size_t chunk_scratch_bytes(const ss_source* items, const Shape* shapes, i
     for (int i = first; i < last; ++i) need += spectra_bytes(items[i], shapes[i]);
     return need;
 }
-// Block tables on the host when every trajectory is host-visible and every window fixed (always true on the host path)
+// Block tables on the host when every trajectory is host-visible, every window fixed and no candidate picked on the
+// device (always true on the host path)
 static bool chunk_host_tables(const ss_source* items, int first, int last) {
     for (int i = first; i < last; ++i)
-        if ((items[i].mode == SS_MOVING_BOUNDS && !items[i].bounds_host) || items[i].win_start_dev) return false;
+        if ((items[i].mode == SS_MOVING_BOUNDS && !items[i].bounds_host) || items[i].win_start_dev || items[i].pool)
+            return false;
     return true;
 }
-// counts of a source (Source::counts): [0, 1] and, windowed, [2, 5] - which the host fills even when k_blocks builds the
+// counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
 // block table, so that they always travel in the descriptor block
-static size_t counts_bytes(const Shape& sh) { return sh.win ? 32 : 16; }
+static size_t counts_bytes(const Shape& sh) { return sh.win ? 64 : 16; }
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
 // counts (windowed source, device-built tables)
 static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int first, int last) {
@@ -1019,7 +1095,7 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
     for (int i = first; i < last; ++i) {
         const Shape& sh = shapes[i];
         if (host_tables)
-            bytes += align_up(sizeof(Block) * (size_t)sh.nblk_max, 16) + align_up(sizeof(double) * (size_t)items[i].P, 16) +
+            bytes += align_up(sizeof(Block) * (size_t)sh.nblk_max, 16) + align_up(sizeof(double) * (size_t)sh.p_max, 16) +
                      counts_bytes(sh);
         else if (sh.win)
             bytes += counts_bytes(sh);
@@ -1038,7 +1114,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
     int* hps = (int*)(hbase + off_ps);
     int ps = 0, pr = 0, total_items = 0;
     size_t tab_off = off_tot + 16;
-    bool any_long = false, all_aligned = true, any_norm = false;
+    bool any_long = false, all_aligned = true, any_norm = false, any_pooled = false;
     int grid_direct = 0;
     for (int i = 0; i < n; ++i) {
         const ss_source& it = items[first + i];
@@ -1051,7 +1127,12 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
         s.w = it.mode == SS_MOVING_INDEXED ? it.w : nullptr;
         s.N = it.N; s.P = it.P; s.C = it.C; s.L = it.L;
         s.K = sh.K; s.nb = sh.nb; s.mode = it.mode; s.aligned = sh.aligned; s.nblk_max = sh.nblk_max;
-        if (it.rir_bank) {
+        if (it.flags & SS_DIRECT_TARGET) { s.out_direct = it.out_direct; s.direct_taps = it.direct_taps; }
+        if (it.pool) {
+            // candidate 0 until k_blocks writes the pick of each run over it
+            pick_candidate(s, it.pool->host[0]);
+            any_pooled = true;
+        } else if (it.rir_bank) {
             // spectra (and cuts) from the bank: no RIR rows, no cut table, no k_rir_absmax / k_rir_direct work
             set_banked(s, it.rir_bank->spec, (it.flags & SS_DIRECT_TARGET) ? it.rir_bank->cut : nullptr, sh.win != 0);
         } else {
@@ -1060,37 +1141,40 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
         }
         s.xspec = (float2*)scratch; scratch += (size_t)s.nblk_max * kSpec * sizeof(float2);
         if (it.flags & SS_RIR_NORMALIZE) { s.norm_part = (const float*)scratch; scratch += 512; any_norm = true; }
-        if (it.flags & SS_DIRECT_TARGET) {
-            if (!it.rir_bank) {
-                s.cut = (int*)scratch; scratch += cut_bytes(it);
-                grid_direct = std::max(grid_direct, (s.P * s.C + 7) / 8);
-            }
-            s.out_direct = it.out_direct; s.direct_taps = it.direct_taps;
+        if ((it.flags & SS_DIRECT_TARGET) && !banked(it)) {
+            s.cut = (int*)scratch; scratch += cut_bytes(it);
+            grid_direct = std::max(grid_direct, (s.P * s.C + 7) / 8);
         }
         if (host_tables) {
             // tables live in the descriptor block itself: filled here, copied with it
             Block* hb_blocks = (Block*)(hbase + tab_off);
             s.blocks = (Block*)(dbase + tab_off); tab_off += align_up(sizeof(Block) * (size_t)s.nblk_max, 16);
             double* hb_rstep = (double*)(hbase + tab_off);
-            s.rstep = (double*)(dbase + tab_off); tab_off += align_up(sizeof(double) * (size_t)s.P, 16);
+            s.rstep = (double*)(dbase + tab_off); tab_off += align_up(sizeof(double) * (size_t)sh.p_max, 16);
             int* hb_counts = (int*)(hbase + tab_off);
             s.counts = (int*)(dbase + tab_off); tab_off += counts_bytes(sh);
+            memset(hb_counts, 0, counts_bytes(sh));
             const int nblk = build_blocks_host(it, sh, it.bounds_host, hb_blocks, hb_rstep);
-            hb_counts[0] = nblk; hb_counts[1] = total_items; hb_counts[2] = 0; hb_counts[3] = 0;
+            hb_counts[0] = nblk; hb_counts[1] = total_items;
             if (sh.win) {
                 hb_counts[2] = sh.k0 - sh.g0; hb_counts[3] = sh.k1 - sh.k0;
-                hb_counts[4] = it.win_start; hb_counts[5] = it.win_len; hb_counts[6] = 0; hb_counts[7] = 0;
+                hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
             }
             total_items += (sh.win ? sh.k1 - sh.k0 : nblk) * sh.per;
         } else {
             s.blocks = (Block*)scratch; scratch += align_up(sizeof(Block) * (size_t)s.nblk_max, 256);
-            s.rstep = (double*)scratch; scratch += align_up(sizeof(double) * (size_t)s.P, 256);
+            s.rstep = (double*)scratch; scratch += align_up(sizeof(double) * (size_t)sh.p_max, 256);
             if (sh.win) {                               // k_blocks reads the window from the counts and fills [0, 3]
                 int* hb_counts = (int*)(hbase + tab_off);
                 s.counts = (int*)(dbase + tab_off); tab_off += counts_bytes(sh);
                 memset(hb_counts, 0, counts_bytes(sh));
                 hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
                 memcpy(hb_counts + 6, &it.win_start_dev, sizeof(it.win_start_dev));      // win_start_ptr
+                if (it.pool) {                                                           // pool_table, pool_size, pick_ptr
+                    memcpy(hb_counts + 8, &it.pool->table, sizeof(it.pool->table));
+                    hb_counts[10] = it.pool->n;
+                    memcpy(hb_counts + 12, &it.pick_dev, sizeof(it.pick_dev));
+                }
             } else {
                 s.counts = (int*)scratch;
             }
@@ -1115,7 +1199,8 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
     L->grid_r = pr < sm_count * SS_RENDER_MINB ? pr : sm_count * SS_RENDER_MINB;
     L->ds = (const Source*)dbase;
     L->dps = (const int*)(dbase + off_ps);
-    L->pp.n_inline = n <= kPrepInline ? n : 0;
+    // a pooled slot's Source is written by k_blocks at every run: k_prepare reads the table from global memory
+    L->pp.n_inline = n <= kPrepInline && !any_pooled ? n : 0;
     if (L->pp.n_inline) {
         memcpy(L->pp.prefix, hps, sizeof(int) * (size_t)(n + 1));
         memcpy(L->pp.srcs, hs, sizeof(Source) * (size_t)n);
@@ -1132,7 +1217,7 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, b
         CK(cudaEventRecord(pf.e0, stream));
     }
     if (!L.host_tables) {
-        k_blocks<<<1, 256, 0, stream>>>(L.ds, L.n, L.d_total);
+        k_blocks<<<1, 256, 0, stream>>>(const_cast<Source*>(L.ds), L.n, L.d_total);
         CK(cudaGetLastError());
         c->launches += 1;
     }
@@ -1256,6 +1341,95 @@ extern "C" int ss_bank_create_host(ss_ctx* c, const float* rir, int32_t P, int32
     return st;
 }
 
+// ----------------------------------------------------------------------------- source pools
+// A candidate of a pool (include/sonicsim_b200.h): a banked source of this context, moving over host-visible bounds or
+// static, with none of a slot's fields.
+static int validate_candidate(const ss_ctx* c, const ss_source& it) {
+    if (!it.x || it.rir || !it.rir_bank || it.rir_bank->c != c || it.idx || it.w) return SS_ERR_INVALID;
+    if (it.out || it.out_direct || it.flags || it.direct_taps || it.win_start || it.win_len || it.win_start_dev ||
+        it.pool || it.pick_dev)
+        return SS_ERR_INVALID;
+    if (it.N <= 0 || it.C <= 0 || it.L <= 0 || it.P <= 0) return SS_ERR_INVALID;
+    if (it.N > 0x7fffffff - 2 * kF) return SS_ERR_INVALID;                 // as validate_item
+    if (it.mode == SS_STATIC) { if (it.P != 1 || it.bounds || it.bounds_host) return SS_ERR_INVALID; }
+    else if (it.mode == SS_MOVING_BOUNDS) {
+        if (it.P < 2 || !it.bounds || !it.bounds_host || !bounds_ok(it.bounds_host, it.P, it.N)) return SS_ERR_INVALID;
+    } else return SS_ERR_INVALID;
+    return validate_bank_use(it);
+}
+
+extern "C" void ss_pool_destroy(ss_pool* pl) {
+    if (!pl) return;
+    cudaSetDevice(pl->c->device);
+    cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
+    if (pl->table) cudaFree(pl->table);
+    if (pl->ready) cudaEventDestroy(pl->ready);
+    delete pl;
+}
+extern "C" int64_t ss_pool_bytes(const ss_pool* pl) { return pl ? (int64_t)sizeof(PoolEntry) * pl->n : 0; }
+
+static int pool_build(ss_pool* pl, const ss_source* cand) {
+    ss_ctx* c = pl->c;
+    const ss_source& a = cand[0];
+    pl->mode = a.mode; pl->C = a.C; pl->L = a.L; pl->K = (a.L + kB - 1) / kB; pl->aligned = 1;
+    pl->n_min = a.N; pl->direct_taps = a.rir_bank->cut ? a.rir_bank->direct_taps : 0;
+    pl->host.resize(pl->n);
+    if (pl->mode == SS_MOVING_BOUNDS) pl->bounds_off.resize(pl->n);
+    std::vector<ss_bank*> banks;
+    for (int i = 0; i < pl->n; ++i) {
+        const ss_source& it = cand[i];
+        const ss_bank* b = it.rir_bank;
+        PoolEntry e;
+        e.x = it.x; e.bounds = it.mode == SS_MOVING_BOUNDS ? it.bounds : nullptr; e.spec = b->spec; e.cut = b->cut;
+        e.N = it.N; e.P = it.P;
+        pl->host[i] = e;
+        pl->n_min = std::min(pl->n_min, it.N); pl->p_max = std::max(pl->p_max, it.P);
+        if (pl->direct_taps != (b->cut ? b->direct_taps : 0)) pl->direct_taps = 0;
+        // the pool's blocking: aligned only if every candidate would choose it
+        if (!choose_aligned(it, pl->K, (it.N + kB - 1) / kB)) pl->aligned = 0;
+        if (pl->mode == SS_MOVING_BOUNDS) {
+            pl->bounds_off[i] = (int64_t)pl->bounds_host.size();
+            pl->bounds_host.insert(pl->bounds_host.end(), it.bounds_host, it.bounds_host + it.P);
+        }
+        if (std::find(banks.begin(), banks.end(), b) == banks.end()) banks.push_back(const_cast<ss_bank*>(b));
+    }
+    CK(cudaMalloc((void**)&pl->table, sizeof(PoolEntry) * (size_t)pl->n));
+    CK(cudaMemcpy(pl->table, pl->host.data(), sizeof(PoolEntry) * (size_t)pl->n, cudaMemcpyHostToDevice));
+    // one event behind every bank's construction: a plan run waits once per pool, not once per candidate bank
+    CK(cudaEventCreateWithFlags(&pl->ready, cudaEventDisableTiming));
+    cudaStream_t s = nullptr;
+    CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    int st = SS_OK;
+    for (ss_bank* b : banks) {
+        const cudaError_t e = cudaStreamWaitEvent(s, b->ready, 0);
+        if (e != cudaSuccess) { g_last_cuda = (int)e; st = SS_ERR_CUDA; break; }
+    }
+    if (st == SS_OK) {
+        const cudaError_t e = cudaEventRecord(pl->ready, s);
+        if (e != cudaSuccess) { g_last_cuda = (int)e; st = SS_ERR_CUDA; }
+    }
+    cudaStreamDestroy(s);                               // (the recorded work completes on its own)
+    return st;
+}
+
+extern "C" int ss_pool_create(ss_ctx* c, const ss_source* cand, int n, ss_pool** out) {
+    if (!c || !cand || !out || n < 1 || n > (1 << 24)) return SS_ERR_INVALID;
+    *out = nullptr;
+    for (int i = 0; i < n; ++i) {
+        const int st = validate_candidate(c, cand[i]);
+        if (st) return st;
+        if (cand[i].mode != cand[0].mode || cand[i].C != cand[0].C || cand[i].L != cand[0].L) return SS_ERR_INVALID;
+    }
+    CK(cudaSetDevice(c->device));
+    ss_pool* pl = new (std::nothrow) ss_pool();
+    if (!pl) return SS_ERR_NOMEM;
+    pl->c = c; pl->n = n;
+    const int st = pool_build(pl, cand);
+    if (st != SS_OK) { ss_pool_destroy(pl); return st; }
+    *out = pl;
+    return SS_OK;
+}
+
 // Describe items[first, last) (device pointers) in the next slot of the descriptor ring, copy the block and enqueue
 // the launches on `stream`, with scratch buffer `buf`.
 static int launch_chunk(ss_ctx* c, const ss_source* items, const Shape* shapes, int first, int last,
@@ -1349,10 +1523,16 @@ extern "C" int ss_debug_chunks(const int64_t* bytes, int32_t n, int64_t budget, 
     return (int)cuts.size();
 }
 
-// Validate a device-path batch and work out the shape of every source, once per call.
-static int shape_dev_items(const ss_ctx* c, const ss_source* items, int n_items, std::vector<Shape>& shapes) {
+// Validate a device-path batch and work out the shape of every source, once per call.  Pooled slots only in plans.
+static int shape_dev_items(const ss_ctx* c, const ss_source* items, int n_items, std::vector<Shape>& shapes,
+                           bool pools_ok) {
     shapes.resize(n_items);
     for (int i = 0; i < n_items; ++i) {
+        if (pools_ok && items[i].pool) {
+            const int st = validate_pooled(c, items[i]); if (st) return st;
+            shapes[i] = shape_pooled(items[i]);
+            continue;
+        }
         int st = validate_item_ctx(c, items[i]); if (st) return st;
         if (items[i].mode == SS_MOVING_BOUNDS && items[i].bounds_host &&
             !bounds_ok(items[i].bounds_host, items[i].P, items[i].N))
@@ -1401,7 +1581,7 @@ extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, voi
     CK(cudaSetDevice(c->device));
     const cudaStream_t stream = (cudaStream_t)stream_;
     std::vector<Shape> shapes;
-    { int st = shape_dev_items(c, items, n_items, shapes); if (st) return st; }
+    { int st = shape_dev_items(c, items, n_items, shapes, false); if (st) return st; }
     { int st = wait_banks(items, n_items, stream); if (st) return st; }   // before the fork: every chunk
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
@@ -1434,7 +1614,8 @@ struct ss_plan {
     cudaEvent_t ev_fork = nullptr, ev_join[ss_ctx::kAux] = {};
     cudaStream_t s_cap = nullptr;      // capture origin: the caller's stream may be the legacy default stream, which cannot capture
     std::vector<ss_bank*> banks;       // banks of the plan's sources: every run waits for their construction
-    const MixItem* d_mix = nullptr;    // the mixtures' descriptors, in d_desc behind the chunk descriptors
+    std::vector<ss_pool*> pools;       // pools of its pooled slots: every run waits for each pool's `ready` event
+    const MixItem* d_mix = nullptr;   // the mixtures' descriptors, in d_desc behind the chunk descriptors
     int n_mix = 0;
 };
 
@@ -1566,7 +1747,17 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
             add_range(r, it.w, 4 * (uint64_t)it.N, false);
         }
         add_range(r, it.win_start_dev, 4, false);
+        add_range(r, it.pick_dev, 4, false);
     }
+    // a pooled slot may read any candidate: every candidate's x and bounds, once per pool
+    std::vector<const ss_pool*> pools;
+    for (int i = 0; i < n_items; ++i)
+        if (items[i].pool && std::find(pools.begin(), pools.end(), items[i].pool) == pools.end()) pools.push_back(items[i].pool);
+    for (const ss_pool* pl : pools)
+        for (const PoolEntry& e : pl->host) {
+            add_range(r, e.x, 4 * (uint64_t)e.N, false);
+            add_range(r, e.bounds, 4 * (uint64_t)e.P, false);
+        }
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
 
@@ -1576,7 +1767,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
-    { int st = shape_dev_items(c, items, n_items, shapes); if (st) return st; }
+    { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
     { int st = validate_mixes(items, n_items, mixes, n_mixes); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
@@ -1584,6 +1775,8 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     for (int i = 0; i < n_items; ++i) {
         ss_bank* b = const_cast<ss_bank*>(items[i].rir_bank);
         if (b && std::find(p->banks.begin(), p->banks.end(), b) == p->banks.end()) p->banks.push_back(b);
+        ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
+        if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
     const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
@@ -1617,6 +1810,7 @@ extern "C" int ss_plan_run(ss_plan* p, void* stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     CK(cudaSetDevice(c->device));
     for (ss_bank* b : p->banks) CK(cudaStreamWaitEvent(stream, b->ready, 0));    // (outside any capture)
+    for (ss_pool* pl : p->pools) CK(cudaStreamWaitEvent(stream, pl->ready, 0));
     if (c->profiling) {                                 // per-kernel timing: no graph, chunks one after the other
         { int st = profile_start(c, stream); if (st) return st; }
         return plan_enqueue(p, stream);

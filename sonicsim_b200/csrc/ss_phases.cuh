@@ -43,7 +43,8 @@ struct Source {
     int* counts;           // scratch: [0] = blocks in use, [1] = index of this source's first render item; windowed
                            // source (h_rows != 0): [2] = first block that meets the window, [3] = blocks that do,
                            // [4] = win_start, [5] = win_len, [6..7] = device pointer of a moving window's start or
-                           // null (win_start_ptr)
+                           // null (win_start_ptr); tables built on the device: [8..13] the pool of a pooled slot
+                           // (pool_table, pool_size, pick_ptr)
     const float* norm_part;// scratch: kNormParts partial abs-maxima of the RIR tensor (k_rir_absmax), or null: taps used as given
     int* cut;              // scratch: P*C direct-path row lengths (k_rir_direct), or null: no direct target
     float* out_direct;     // (C, N) direct-path stem (with `cut`)
@@ -232,6 +233,48 @@ SS_HD int clamp_win_start(int v, int N, int win_len, bool& bad) {
 }
 // a windowed source's moving start (counts[6..7], 8-byte aligned), or null: the start is counts[4]
 SS_HD const int* win_start_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 6); }
+
+// ---- source pools (ss_pool, include/sonicsim_b200.h).  A pooled slot is a windowed source whose candidate is picked on
+// the device at every run: the head of k_blocks reads the pick, clamps it and writes the candidate's fields into the
+// slot's Source (pick_candidate) before anything reads them.  One compact entry per candidate in the pool's table:
+struct PoolEntry {
+    const float* x;        // dry signal, N samples
+    const int* bounds;     // trajectory bounds (moving pool), else null
+    float2* spec;          // the bank's spectra (reverberant set, then the direct set)
+    int* cut;              // the bank's direct-path cut table, or null: no direct set
+    int N, P;
+};
+static_assert(sizeof(PoolEntry) == 40, "PoolEntry layout");
+// A pooled slot's counts (counts_bytes = 64 for every windowed source whose tables k_blocks builds): [8..9] the pool's
+// device table or null (not pooled), [10] its candidate count, [12..13] the device pointer of the pick
+SS_HD const PoolEntry* pool_table(const Source& s) { return *reinterpret_cast<const PoolEntry* const*>(s.counts + 8); }
+SS_HD int pool_size(const Source& s) { return s.counts[10]; }
+SS_HD const int* pick_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 12); }
+// A pick as read from device memory, clamped into [0, n); bad = it was outside
+SS_HD int clamp_pick(int v, int n, bool& bad) {
+    bad = v < 0 || v >= n;
+    return v < 0 ? 0 : (v >= n ? n - 1 : v);
+}
+// The picked candidate into the slot's Source, as set_banked sets a windowed banked source (K, C, mode, aligned and the
+// slot's own buffers stay): the direct set only for a slot that renders a direct stem
+SS_HD void pick_candidate(Source& s, const PoolEntry& e) {
+    s.x = e.x; s.bounds = e.bounds; s.N = e.N; s.P = e.P; s.nb = (e.N + kB - 1) / kB;
+    set_banked(s, e.spec, s.out_direct ? e.cut : nullptr, true);
+}
+// Table size of a pooled slot with windows of win_len: the largest window_table_cap over the candidates' full plans under
+// the pool's blocking (bounds[i]: candidate i's host bounds, null for a static pool), so that the table holds the blocks
+// of every candidate at every start.  `full` holds table_cap(aligned, nb, P) blocks of the largest candidate.
+SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, const int* P, int n, int win_len, int K,
+                         Block* full) {
+    int best = 0;
+    for (int i = 0; i < n; ++i) {
+        const int nb = (N[i] + kB - 1) / kB, cap = table_cap(aligned, nb, P[i]);
+        const int nfull = plan_blocks(aligned, bounds ? bounds[i] : nullptr, P[i], N[i], nb, 0, cap, full);
+        const int c = window_table_cap(full, nfull < cap ? nfull : cap, N[i], win_len, K, P[i], cap);
+        best = c > best ? c : best;
+    }
+    return best;
+}
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
 SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }

@@ -70,6 +70,20 @@ class Mixture(T.NamedTuple):
     noise_delay: int = 0
 
 
+class Pooled(T.NamedTuple):
+    """A pooled slot of a device plan (Renderer.plan_device): at every run it renders the candidate of `pool`
+    (Renderer.source_pool) named by `pick`, a one-element CUDA int32 tensor read on the device at that run (e.g.
+    picks[b, k] of a (B, S) tensor) - the dataloader's random choice of scene, speakers and noise without host work.
+    `window` = (start, length) as MovingSource.window: the start an int or a one-element CUDA int32 tensor; the length
+    at most every candidate's N.  The output is (C, length).  `direct_taps` > 0 also renders the direct-path stem, which
+    needs every candidate's bank to hold a direct set with these taps.  A pick outside [0, n) is clamped into range and a
+    start beyond the picked candidate's N - length is clamped too (check_device_errors).  Only plan_device takes it."""
+    pool: T.Any
+    pick: T.Any
+    window: T.Tuple[T.Any, int]
+    direct_taps: int = 0
+
+
 def _is_tensor(v) -> bool:
     return type(v).__module__.split(".")[0] == "torch"
 
@@ -114,43 +128,25 @@ def _flags(s, i, direct_out) -> int:
         raise ValueError("source %d has direct_taps = %d but no direct output (direct_outs[%d])" % (i, taps, i))
     if taps == 0 and direct_out is not None:
         raise ValueError("direct_outs[%d] is given but source %d has no direct_taps" % (i, i))
-    return (_lib.SS_RIR_NORMALIZE if s.normalize_rirs else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
+    norm = getattr(s, "normalize_rirs", False)              # (a pooled slot has none: normalisation is the banks')
+    return (_lib.SS_RIR_NORMALIZE if norm else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
 
 
-class RirBank:
-    """The half spectra of one RIR set, transformed once and held in device memory (Renderer.rir_bank; ss_bank of the C
-    ABI).  Pass it as `MovingSource.rirs` / `StaticSource.rir`: the source renders bit-identically to the same source
-    given the raw RIRs, which are never read again.  It belongs to the context of the renderer that made it.  Every
-    render that uses it is ordered after its construction by the library, on every path, whatever stream built it.
-    Plans hold the bank: it is freed only once it is closed (or collected) and no live plan uses it any more."""
-
-    def __init__(self, renderer, handle, shape, normalize, direct_taps):
-        self.renderer, self._h = renderer, handle
-        self.shape = tuple(int(v) for v in shape)          # as given: (P, C, L) or (C, L)
-        self.normalize, self.direct_taps = bool(normalize), int(direct_taps)
-        self.nbytes = int(renderer.lib.ss_bank_bytes(handle))
-        self._closing, self._plans = False, 0
-
-    @property
-    def pcl(self) -> T.Tuple[int, int, int]:
-        return self.shape if len(self.shape) == 3 else (1,) + self.shape
+class _Held:
+    """Device memory that plans (and pools) hold: close() refuses it to new users and frees it once no holder is left."""
+    _closing, _plans = False, 0
 
     @property
     def closed(self) -> bool:
-        """True once close() was called: new sources may not use the bank (plans made before keep working)."""
+        """True once close() was called: new sources may not use it (plans made before keep working)."""
         return self._closing or not self._h
 
     def close(self):
-        """Refuse the bank to new sources and free its device memory - at once, or, while plans that use it are alive,
-        when the last of them is closed or collected (their runs keep reading it until then)."""
+        """Refuse it to new sources and free its device memory - at once, or, while plans that use it are alive, when
+        the last of them is closed or collected (their runs keep reading it until then)."""
         self._closing = True
         if self._plans == 0:
             self._free()
-
-    def _free(self):
-        if self._h:
-            self.renderer.lib.ss_bank_destroy(self._h)
-            self._h = ctypes.c_void_p()
 
     def _hold(self):
         self._plans += 1
@@ -165,6 +161,51 @@ class RirBank:
             self.close()
         except Exception:
             pass
+
+
+class RirBank(_Held):
+    """The half spectra of one RIR set, transformed once and held in device memory (Renderer.rir_bank; ss_bank of the C
+    ABI).  Pass it as `MovingSource.rirs` / `StaticSource.rir`: the source renders bit-identically to the same source
+    given the raw RIRs, which are never read again.  It belongs to the context of the renderer that made it.  Every
+    render that uses it is ordered after its construction by the library, on every path, whatever stream built it.
+    Plans and source pools hold the bank: it is freed only once it is closed (or collected) and nothing alive uses it."""
+
+    def __init__(self, renderer, handle, shape, normalize, direct_taps):
+        self.renderer, self._h = renderer, handle
+        self.shape = tuple(int(v) for v in shape)          # as given: (P, C, L) or (C, L)
+        self.normalize, self.direct_taps = bool(normalize), int(direct_taps)
+        self.nbytes = int(renderer.lib.ss_bank_bytes(handle))
+
+    @property
+    def pcl(self) -> T.Tuple[int, int, int]:
+        return self.shape if len(self.shape) == 3 else (1,) + self.shape
+
+    def _free(self):
+        if self._h:
+            self.renderer.lib.ss_bank_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+
+class SourcePool(_Held):
+    """A set of banked candidate sources validated and uploaded once (Renderer.source_pool; ss_pool of the C ABI), which
+    pooled slots (render.Pooled) of device plans pick from at every run.  `n` candidates of one `mode`, `C` and `L`;
+    `n_min` is the shortest candidate's N (the longest window a slot may take); `direct_taps` > 0 when every candidate's
+    bank holds a direct set with these taps.  The pool holds its candidates' banks and keeps their tensors alive; plans
+    hold the pool, which is freed once it is closed (or collected) and no live plan uses it any more."""
+
+    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps):
+        self.renderer, self._h = renderer, handle
+        self.candidates = list(candidates)
+        self.n, self.mode, self.C, self.L = len(self.candidates), mode, C, L
+        self.n_min, self.direct_taps = n_min, direct_taps
+        self.nbytes = int(renderer.lib.ss_pool_bytes(handle))
+        self._banks = _hold_banks(self, self.candidates)
+
+    def _free(self):
+        if self._h:
+            self.renderer.lib.ss_pool_destroy(self._h)
+            self._h = ctypes.c_void_p()
+            self._banks()                      # the pool no longer reads its banks
 
 
 def _bank_of(renderer, s, i, P, C, L):
@@ -185,18 +226,30 @@ def _bank_of(renderer, s, i, P, C, L):
     return b._h.value
 
 
+def _kind(k):
+    return ("static" if k[0] == _lib.SS_STATIC else "moving", k[1], k[2])
+
+
+def _refuse_pooled(sources, where):
+    for i, s in enumerate(sources):
+        if isinstance(s, Pooled):
+            raise ValueError("%s: source %d is a pooled slot (render.Pooled), which only device plans (plan_device) "
+                             "render" % (where, i))
+
+
 def _release_banks(banks):
     for b in banks:
         b._release()
 
 
 def _hold_banks(plan, sources):
-    """The RirBanks of a plan's sources are held until the plan is closed or collected: a bank closed meanwhile is
-    freed only then.  Returns the finalizer that releases them (calling it releases them at once, once)."""
+    """The RirBanks and SourcePools of a plan's sources (of a pool's candidates) are held until the plan (the pool) is
+    closed or collected: one closed meanwhile is freed only then.  Returns the finalizer that releases them (calling it
+    releases them at once, once)."""
     banks = []
     for s in sources:
-        b = s.rir if isinstance(s, StaticSource) else s.rirs
-        if isinstance(b, RirBank) and all(b is not o for o in banks):
+        b = s.pool if isinstance(s, Pooled) else (s.rir if isinstance(s, StaticSource) else s.rirs)
+        if isinstance(b, (RirBank, SourcePool)) and all(b is not o for o in banks):
             banks.append(b)
     for b in banks:
         b._hold()
@@ -251,6 +304,70 @@ class Renderer:
             _lib.check(self.lib.ss_bank_create_host(self.ctx, a.ctypes.data, P, C, L, flags, taps, ctypes.byref(h)))
         return RirBank(self, h, shape, normalize, taps)
 
+    # ------------------------------------------------------------------ source pools
+    def source_pool(self, candidates: T.Sequence[T.Union[MovingSource, StaticSource]]) -> SourcePool:
+        """Validate and upload a set of candidate sources once, for pooled slots (render.Pooled) of device plans to pick
+        from at every run.  Every candidate is a MovingSource or StaticSource whose RIRs are a RirBank of this renderer
+        (`dry`, `bounds`: contiguous CUDA tensors of its device; a moving candidate needs `bounds_host`), with no window,
+        normalize_rirs or direct_taps (those belong to the slot and the bank); all share one kind (moving or static), C
+        and L.  The candidates' tensors and banks are kept alive by the pool."""
+        import torch
+        n = len(candidates)
+        if not 1 <= n <= 1 << 24:
+            raise ValueError("source_pool: a pool holds 1 to 2^24 candidates, got %d" % n)
+        items = (SsSource * n)()
+        keep = []
+        first = None
+        for i, s in enumerate(candidates):
+            if not isinstance(s, (MovingSource, StaticSource)):
+                raise ValueError("source_pool: candidate %d must be a MovingSource or StaticSource, got %s"
+                                 % (i, type(s).__name__))
+            static = isinstance(s, StaticSource)
+            rb = s.rir if static else s.rirs
+            if not isinstance(rb, RirBank):
+                raise ValueError("source_pool: candidate %d must take its RIRs from a RirBank" % i)
+            if rb.closed:
+                raise ValueError("source_pool: the RirBank of candidate %d is closed" % i)
+            if rb.renderer.ctx.value != self.ctx.value:
+                raise ValueError("source_pool: the RirBank of candidate %d belongs to another renderer's context" % i)
+            if s.window is not None or s.normalize_rirs or int(s.direct_taps):
+                raise ValueError("source_pool: candidate %d has a window, normalize_rirs or direct_taps; those belong to "
+                                 "the pooled slot (render.Pooled) and the bank" % i)
+            P, C, L = rb.pcl
+            kind = (_lib.SS_STATIC if static else _lib.SS_MOVING_BOUNDS, C, L)
+            if first is None:
+                first = kind
+            elif kind != first:
+                raise ValueError("source_pool: candidate %d is (%s, C=%d, L=%d), candidate 0 (%s, C=%d, L=%d): every "
+                                 "candidate has one kind, C and L" % ((i,) + _kind(kind) + _kind(first)))
+
+            def chk(t, name, dtype, shape):
+                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                    raise ValueError("source_pool: %s of candidate %d must be a CUDA tensor on cuda:%d"
+                                     % (name, i, self.device))
+                if t.dtype != dtype or not t.is_contiguous() or (shape is not None and tuple(t.shape) != shape):
+                    raise ValueError("source_pool: %s of candidate %d must be a contiguous %s tensor%s"
+                                     % (name, i, dtype, "" if shape is None else " of shape %s" % (shape,)))
+
+            chk(s.dry, "dry", torch.float32, None)
+            N = s.dry.numel()
+            items[i] = SsSource(x=s.dry.data_ptr(), N=N, P=P, C=C, L=L, mode=kind[0], rir_bank=rb._h.value)
+            if not static:
+                chk(s.bounds, "bounds", torch.int32, (P,))
+                if s.bounds_host is None:
+                    raise ValueError("source_pool: moving candidate %d needs bounds_host" % i)
+                bh = np.ascontiguousarray(s.bounds_host, dtype=np.int32)
+                if bh.shape != (P,):
+                    raise ValueError("source_pool: bounds_host of candidate %d must have P = %d entries" % (i, P))
+                keep.append(bh)
+                items[i].bounds, items[i].bounds_host = s.bounds.data_ptr(), bh.ctypes.data
+        h = ctypes.c_void_p()
+        _lib.check(self.lib.ss_pool_create(self.ctx, items, n, ctypes.byref(h)))
+        banks = [s.rir if isinstance(s, StaticSource) else s.rirs for s in candidates]
+        taps = {b.direct_taps for b in banks}
+        return SourcePool(self, h, candidates, first[0], first[1], first[2], min(s.dry.numel() for s in candidates),
+                          taps.pop() if len(taps) == 1 else 0)
+
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
                   outs: T.Optional[T.Sequence[np.ndarray]] = None,
@@ -260,6 +377,7 @@ class Renderer:
         C-ABI call (a generation loop refills the same pinned buffers and calls run() again).
         See render_host for the arguments."""
         from .SonicSim_audio import gating_plan
+        _refuse_pooled(sources, "plan_host")
         n = len(sources)
         direct_outs = _check_direct_outs(direct_outs, n)
         items = (SsSource * n)()
@@ -349,6 +467,7 @@ class Renderer:
         for the direct-path stems of sources with direct_taps > 0, None for the others.  Asynchronous on `stream`
         (torch current stream).  A window's start may be a CUDA int32 tensor (see MovingSource.window); a crop that
         moves every step is cheaper through a plan_device whose start tensors are rewritten between runs."""
+        _refuse_pooled(sources, "render_device")
         items, n, keep = self._device_items(sources, outs, direct_outs)
         if stream is None:
             import torch
@@ -466,11 +585,36 @@ class Renderer:
                                  % (name, i, tuple(shape), tuple(t.shape)))
 
         for i, s in enumerate(sources):
-            chk(s.dry, "dry", i, torch.float32)
-            N = s.dry.numel()
-            ws, wl, n_out, start = _window_dev(s, i, N, self.device)
-            rb = s.rir if isinstance(s, StaticSource) else s.rirs
-            rb = rb if isinstance(rb, RirBank) else None
+            if isinstance(s, Pooled):
+                pl = s.pool
+                if not isinstance(pl, SourcePool):
+                    raise ValueError("plan_device: the pool of source %d must be a SourcePool" % i)
+                if pl.closed:
+                    raise ValueError("plan_device: the SourcePool of source %d is closed" % i)
+                if pl.renderer.ctx.value != self.ctx.value:
+                    raise ValueError("plan_device: the SourcePool of source %d belongs to another renderer's context" % i)
+                chk(s.pick, "pick", i, torch.int32)
+                if s.pick.numel() != 1:
+                    raise ValueError("plan_device: pick of source %d must hold one int32, got %d elements"
+                                     % (i, s.pick.numel()))
+                if s.window is None:
+                    raise ValueError("plan_device: pooled source %d needs a window (start, length)" % i)
+                ws, wl, n_out, start = _window_dev(s, i, pl.n_min, self.device)
+                taps = int(s.direct_taps)
+                if taps > 0 and taps != pl.direct_taps:
+                    raise ValueError("plan_device: pooled source %d has direct_taps = %d, but not every candidate's bank "
+                                     "holds a direct set with these taps" % (i, taps))
+                C, L = pl.C, pl.L
+                chk(outs[i], "out", i, torch.float32, (C, n_out))
+                items[i] = SsSource(out=outs[i].data_ptr(), C=C, L=L, mode=pl.mode, pool=pl._h.value,
+                                    pick_dev=s.pick.data_ptr())
+                rb = None
+            else:
+                chk(s.dry, "dry", i, torch.float32)
+                N = s.dry.numel()
+                ws, wl, n_out, start = _window_dev(s, i, N, self.device)
+                rb = s.rir if isinstance(s, StaticSource) else s.rirs
+                rb = rb if isinstance(rb, RirBank) else None
             if isinstance(s, StaticSource):
                 if rb is None:
                     chk(s.rir, "rir", i, torch.float32)
@@ -483,7 +627,7 @@ class Renderer:
                 items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rir.data_ptr() if rb is None else None,
                                     out=outs[i].data_ptr(), N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC)
                 P = 1
-            else:
+            elif not isinstance(s, Pooled):
                 if rb is None:
                     chk(s.rirs, "rirs", i, torch.float32)
                     if s.rirs.dim() != 3:
@@ -523,6 +667,9 @@ class Renderer:
         _lib.check(self.lib.ss_device_errors(self.ctx, ctypes.byref(bits)))
         if bits.value & 1:
             raise IndexError("an interp_index on the device was out of bounds for the number of RIR positions")
+        if bits.value & 8:
+            raise IndexError("a pick on the device was out of range for the candidates of its SourcePool; it was clamped "
+                             "into [0, n)")
         if bits.value & 2:
             raise ValueError("a device-side trajectory bounds table is not ascending from 0 to N")
         if bits.value & 4:
