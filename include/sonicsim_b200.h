@@ -13,9 +13,13 @@
  *   - `*_host` entry points take HOST pointers (pinned memory gives full PCIe rate), copy in,
  *     render and copy out; they return after the results are in host memory.
  *   - an ss_ctx is NOT thread-safe: use one context per host thread (one process per GPU is the
- *     intended deployment); calls on one context are serialised by the caller.  The context's scratch and
- *     descriptor buffers are ordered against earlier work only through the stream a call is given: give
- *     all `*_dev` calls of one context the same stream, or synchronise between calls that use different ones.
+ *     intended deployment); calls on one context are serialised by the caller.
+ *   - streams: a call on one stream may follow a call on another (or a host call) at once.  The library orders its
+ *     own buffers - scratch, descriptor blocks, a bank or pool under construction - behind their earlier users on
+ *     every stream, on the device (only a descriptor block's pinned staging copy, reused every 6 calls or chunks, may
+ *     hold the host until its previous upload is done).  The caller orders only its own buffers: an input written or an output
+ *     read on another stream needs the caller's event or synchronisation, as for any CUDA work.  Two runs of one plan
+ *     write the same outputs, so they are the caller's to order.
  *   - every function returns 0 (SS_OK) or a negative ss_status; ss_strerror() describes it.  The
  *     Python shim turns these into the exception types the reference raises (IndexError /
  *     ValueError), see INTEGRATION.md.
@@ -240,7 +244,8 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * the device: bit 0 = an interp_index outside [0, P - 2], bit 1 = a device-side bounds table that is not ascending from
  * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
  * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped).  The Python device API raises IndexError / ValueError from it on request
- * (Renderer.check_device_errors). */
+ * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
+ * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
 int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
 
 /* A batch of device-resident sources bound once (the generation loop of SonicSet.py:180-214 renders the same

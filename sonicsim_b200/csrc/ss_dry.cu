@@ -80,7 +80,7 @@ extern "C" int ss_dry_assemble_dev(ss_ctx* c, const ss_dry_clip* clips, int n_cl
     if (n_clips == 0) return SS_OK;
     const size_t bytes = sizeof(DryClip) * (size_t)n_clips;
     int slot; char *hblk, *dblk;
-    { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
+    { int st = ring_acquire(c, bytes, stream, &slot, &hblk, &dblk); if (st) return st; }
     DryClip* h = (DryClip*)hblk;
     long long max_count = 1;
     for (int i = 0; i < n_clips; ++i) {
@@ -97,5 +97,5 @@ extern "C" int ss_dry_assemble_dev(ss_ctx* c, const ss_dry_clip* clips, int n_cl
     k_dry_assemble<<<dim3(gx, (unsigned)n_clips), 256, 0, stream>>>((const DryClip*)dblk, out);
     CK(cudaGetLastError());
     c->launches += 1;
-    return SS_OK;
+    return ring_release(c, slot, stream);
 }

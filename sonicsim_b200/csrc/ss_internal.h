@@ -23,12 +23,15 @@ struct ss_ctx {
     char* d_scratch[kAux] = {}; size_t scratch_cap[kAux] = {};
     cudaStream_t s_aux[kAux] = {};
     cudaEvent_t ev_fork = nullptr, ev_join[kAux] = {};
-    // descriptor ring (pinned host + device)
-    static const int kRing = 2 * SS_AUX_STREAMS;      // multiple of kAux: a slot is always reused on the same stream
+    // descriptor ring (pinned host + device).  Any stream may reuse a slot (ring_acquire orders the reuse after the
+    // slot's previous readers); kRing is a multiple of kAux so that ss_render_dev's forked chunks reuse each slot on
+    // the stream that last used it, where that ordering costs nothing
+    static const int kRing = 2 * SS_AUX_STREAMS;
     char* h_desc[kRing] = {};
     char* d_desc[kRing] = {};
     size_t desc_cap[kRing] = {};
-    cudaEvent_t desc_ev[kRing] = {};
+    cudaEvent_t desc_ev[kRing] = {};     // behind the slot's host->device copy: the pinned block may be refilled
+    cudaEvent_t desc_done[kRing] = {};   // behind the last launch that reads the slot's device block
     int ring_pos = 0;
     // host path
     cudaStream_t s_in = nullptr, s_cmp = nullptr, s_out = nullptr;
@@ -83,12 +86,15 @@ struct MixItem {
 // The four mixture kernels over the n descriptors at `d` (device memory), asynchronous on `stream`.
 int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream);
 
-// Take the next slot of the descriptor ring (pinned host block + its device twin), grown to `bytes`.
-// Blocks the host until the slot's previous host->device copy has completed.  The caller fills `*h`,
-// copies it to `*d` on its stream and records c->desc_ev[*slot] right after the copy.
-inline int ring_acquire(ss_ctx* c, size_t bytes, int* slot_out, char** h, char** d) {
+// Take the next slot of the descriptor ring (pinned host block + its device twin), grown to `bytes`, for work on
+// `stream`.  Blocks the host until the slot's previous host->device copy has completed (the pinned block is free), and
+// makes `stream` wait for the slot's previous readers, whatever stream they ran on (the device block is free; a no-op
+// wait when they ran on `stream`).  The caller fills `*h`, copies it to `*d` on `stream`, records c->desc_ev[*slot]
+// right after the copy and c->desc_done[*slot] (ring_release) after the last launch that reads the slot.
+inline int ring_acquire(ss_ctx* c, size_t bytes, cudaStream_t stream, int* slot_out, char** h, char** d) {
     const int slot = c->ring_pos; c->ring_pos = (c->ring_pos + 1) % ss_ctx::kRing;
     CK(cudaEventSynchronize(c->desc_ev[slot]));
+    CK(cudaStreamWaitEvent(stream, c->desc_done[slot], 0));
     if (bytes > c->desc_cap[slot]) {
         if (c->h_desc[slot]) CK(cudaFreeHost(c->h_desc[slot]));
         if (c->d_desc[slot]) { CK(cudaDeviceSynchronize()); CK(cudaFree(c->d_desc[slot])); }
@@ -99,5 +105,10 @@ inline int ring_acquire(ss_ctx* c, size_t bytes, int* slot_out, char** h, char**
         c->desc_cap[slot] = cap;
     }
     *slot_out = slot; *h = c->h_desc[slot]; *d = c->d_desc[slot];
+    return SS_OK;
+}
+// Mark the end of the launches on `stream` that read ring slot `slot`.
+inline int ring_release(ss_ctx* c, int slot, cudaStream_t stream) {
+    CK(cudaEventRecord(c->desc_done[slot], stream));
     return SS_OK;
 }

@@ -646,7 +646,10 @@ static int init_ctx(ss_ctx* c, int device) {
     CK(cudaFuncSetAttribute(k_render<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
     CK(cudaFuncSetAttribute(k_render_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
     CK(cudaFuncSetAttribute(k_render<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
-    for (int i = 0; i < ss_ctx::kRing; ++i) CK(cudaEventCreateWithFlags(&c->desc_ev[i], cudaEventDisableTiming));
+    for (int i = 0; i < ss_ctx::kRing; ++i) {
+        CK(cudaEventCreateWithFlags(&c->desc_ev[i], cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&c->desc_done[i], cudaEventDisableTiming));
+    }
     for (int i = 0; i < ss_ctx::kAux; ++i) {
         CK(cudaStreamCreateWithFlags(&c->s_aux[i], cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&c->ev_join[i], cudaEventDisableTiming));
@@ -693,6 +696,7 @@ extern "C" void ss_destroy(ss_ctx* c) {
         if (c->h_desc[i]) cudaFreeHost(c->h_desc[i]);
         if (c->d_desc[i]) cudaFree(c->d_desc[i]);
         if (c->desc_ev[i]) cudaEventDestroy(c->desc_ev[i]);
+        if (c->desc_done[i]) cudaEventDestroy(c->desc_done[i]);
     }
     for (int i = 0; i < ss_ctx::kSlots; ++i) {
         if (c->slot[i].d_in) cudaFree(c->slot[i].d_in);
@@ -1445,12 +1449,14 @@ static int launch_chunk(ss_ctx* c, const ss_source* items, const Shape* shapes, 
     }
     const size_t bytes = chunk_desc_bytes(items, shapes, first, last);
     int slot; char *hblk, *dblk;
-    { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
+    { int st = ring_acquire(c, bytes, stream, &slot, &hblk, &dblk); if (st) return st; }
     static thread_local ChunkLaunch L;                  // holds 3.2 KB of kernel parameters: not on the stack
     chunk_describe(items, shapes, first, last, hblk, dblk, c->d_scratch[buf], c->sm_count, &L);
     CK(cudaMemcpyAsync(dblk, hblk, bytes, cudaMemcpyHostToDevice, stream));
     CK(cudaEventRecord(c->desc_ev[slot], stream));
-    return chunk_enqueue(c, L, stream, c->profiling);
+    const int st = chunk_enqueue(c, L, stream, c->profiling);
+    const int rs = ring_release(c, slot, stream);
+    return st ? st : rs;
 }
 
 // split [0, n) into chunks whose spectra fit the L2-sized budget
@@ -1583,6 +1589,8 @@ extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, voi
     std::vector<Shape> shapes;
     { int st = shape_dev_items(c, items, n_items, shapes, false); if (st) return st; }
     { int st = wait_banks(items, n_items, stream); if (st) return st; }   // before the fork: every chunk
+    // the scratch buffers' last users, on whatever stream the previous call ran (a no-op wait on the same stream)
+    for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(stream, c->ev_join[i], 0));
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
     std::vector<Shape> arranged_shapes;

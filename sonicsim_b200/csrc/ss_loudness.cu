@@ -241,7 +241,7 @@ extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items
     const size_t off_p = align_up(sizeof(LoudItem) * n_items, 16);
     const size_t bytes = off_p + align_up(sizeof(int) * (n_items + 1), 16);
     int slot; char *hblk, *dblk;
-    { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
+    { int st = ring_acquire(c, bytes, stream, &slot, &hblk, &dblk); if (st) return st; }
     LoudItem* h = (LoudItem*)c->h_desc[slot];
     int* hp = (int*)(c->h_desc[slot] + off_p);
     int tot = 0; bool any_out = false;
@@ -272,7 +272,7 @@ extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items
         CK(cudaGetLastError());
         c->launches += 1;
     }
-    return SS_OK;
+    return ring_release(c, slot, stream);
 }
 
 // Internal (ss_internal.h): k_loud_scale alone, for stems that take the gain measured on another stem.
@@ -280,7 +280,7 @@ int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t 
     if (n_items == 0) return SS_OK;
     const size_t bytes = sizeof(LoudItem) * n_items;
     int slot; char *hblk, *dblk;
-    { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
+    { int st = ring_acquire(c, bytes, stream, &slot, &hblk, &dblk); if (st) return st; }
     LoudItem* h = (LoudItem*)hblk;
     for (int i = 0; i < n_items; ++i) {
         memset(&h[i], 0, sizeof(LoudItem));
@@ -293,7 +293,7 @@ int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t 
     k_loud_scale<<<dim3(c->sm_count * 2, n_items), 256, 0, stream>>>((const LoudItem*)dblk);
     CK(cudaGetLastError());
     c->launches += 1;
-    return SS_OK;
+    return ring_release(c, slot, stream);
 }
 
 // Single stem, host arrays (the drop-in lufs_norm): data / out hold N*C floats in the caller's layout, which is copied

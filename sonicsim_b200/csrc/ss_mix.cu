@@ -259,7 +259,7 @@ extern "C" int ss_mix_dev(ss_ctx* c, const ss_mix_item* items, int n_items, void
     cudaStream_t stream = (cudaStream_t)stream_;
     const size_t bytes = align_up(sizeof(MixItem) * n_items, 16);
     int slot; char *hblk, *dblk;
-    { int st = ring_acquire(c, bytes, &slot, &hblk, &dblk); if (st) return st; }
+    { int st = ring_acquire(c, bytes, stream, &slot, &hblk, &dblk); if (st) return st; }
     MixItem* h = (MixItem*)c->h_desc[slot];
     for (int i = 0; i < n_items; ++i) {
         const ss_mix_item& a = items[i];
@@ -274,7 +274,9 @@ extern "C" int ss_mix_dev(ss_ctx* c, const ss_mix_item* items, int n_items, void
     }
     CK(cudaMemcpyAsync(c->d_desc[slot], c->h_desc[slot], bytes, cudaMemcpyHostToDevice, stream));
     CK(cudaEventRecord(c->desc_ev[slot], stream));
-    return mix_enqueue(c, (const MixItem*)c->d_desc[slot], n_items, stream);
+    const int st = mix_enqueue(c, (const MixItem*)c->d_desc[slot], n_items, stream);   // k_mix_write reads the SNR here
+    const int rs = ring_release(c, slot, stream);
+    return st ? st : rs;
 }
 
 int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream) {

@@ -465,13 +465,13 @@ class Renderer:
         """`sources`: MovingSource / StaticSource whose fields are CUDA float32 / int32 tensors;
         `outs`: preallocated CUDA (C, N) tensors - (C, length) for a source with a `window`; `direct_outs`: the same
         for the direct-path stems of sources with direct_taps > 0, None for the others.  Asynchronous on `stream`
-        (torch current stream).  A window's start may be a CUDA int32 tensor (see MovingSource.window); a crop that
+        (default: torch's current stream of this renderer's device).  A window's start may be a CUDA int32 tensor (see MovingSource.window); a crop that
         moves every step is cheaper through a plan_device whose start tensors are rewritten between runs."""
         _refuse_pooled(sources, "render_device")
         items, n, keep = self._device_items(sources, outs, direct_outs)
         if stream is None:
             import torch
-            stream = torch.cuda.current_stream().cuda_stream
+            stream = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.lib.ss_render_dev(self.ctx, items, n, ctypes.c_void_p(stream)))
 
     def plan_device(self, sources, outs, direct_outs=None, mixtures=None) -> "DevicePlan":
@@ -711,12 +711,12 @@ class DevicePlan:
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
-        """Asynchronous on `stream` (default: torch's current stream)."""
+        """Asynchronous on `stream` (default: torch's current stream of the renderer's device)."""
         if self.n == 0:
             return
         if stream is None:
             import torch
-            stream = torch.cuda.current_stream().cuda_stream
+            stream = torch.cuda.current_stream(self.renderer.device).cuda_stream
         _lib.check(self.renderer.lib.ss_plan_run(self._plan, ctypes.c_void_p(stream)))
 
     def is_graph(self) -> bool:
@@ -855,6 +855,6 @@ def render_mixtures(utterances: T.Sequence[dict], device: T.Optional[int] = None
                              speakers_out=spk.data_ptr(), scratch=scr.data_ptr(), E=C * N, S=S, M=M,
                              snr=float(np.asarray(u.get("snr", 15.0)).reshape(-1)[0]))
         keep.append((mix, sirs, scr))
-    _lib.check(lib.ss_mix_dev(R.ctx, items, n, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
-    torch.cuda.synchronize()
+    _lib.check(lib.ss_mix_dev(R.ctx, items, n, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    torch.cuda.synchronize(dev)
     return [{"mix": keep[k][0].cpu().numpy(), "speakers": plan[k][0].cpu().numpy()} for k in range(n)]
