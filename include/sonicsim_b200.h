@@ -214,11 +214,30 @@ void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their cont
  * plan is created, for the largest any candidate needs: 3 kernel launches per chunk, as with a moving window.
  * Lifetime: a pool must outlive every plan that uses it; ss_pool_destroy waits for the device before it frees it. */
 int ss_pool_create(ss_ctx* ctx, const ss_source* candidates, int n, ss_pool** out);
-int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact candidate entries */
+int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact candidate entries (40 B each), and the
+                                               * level tables with their pointer array once ss_pool_levels built them */
 void ss_pool_destroy(ss_pool* pool);          /* destroy pools after the plans that use them, before their context */
 
+/* ---- level tables of a pool (version 107), for the start draws of plans (ss_plan_draw below).  Gives every candidate
+ * of the pool a table from which the energy of any crop is two loads:
+ *   Q[0] = 0, Q[n + 1] = Q[n] + e[n] for n < N, in float64 (N + 1 doubles), where e[n] is computed from the candidate's
+ *   whole reverberant stem as ss_render_dev renders it (the candidate as a whole banked source, bounds_host included):
+ *     - flags = SS_MIX_MONO: e[n] = (double)(v * v), v the channel fold of the mixture kernels at n (SS_MIX_MONO of
+ *       ss_plan_mix: the float32 sum of the C rows in channel order, then an IEEE division by C), with the same bits;
+ *     - flags = 0: e[n] = sum over c of (double)(y[c, n] * y[c, n]), in channel order.
+ *   These are the terms a mixture's rms_db sums, so a crop's level from a table differs from the plan's rms_db of the
+ *   same crop only by the order of the float64 sums.  The scan has a fixed order: identical bits at every build.
+ * The candidates are rendered in groups through the device path into one transient buffer of at most 256 MB (or one
+ * candidate's stem, when larger), after the pool's banks are complete.  Returns when the tables are in device memory.
+ * The tables cost 8 bytes per sample (3.84 MB for a 30 s candidate at 16 kHz) and describe the candidates' dry signals
+ * as they are at this call: a pool whose `x` buffers change afterwards needs a new pool for new tables.
+ * Refused (SS_ERR_INVALID): a NULL pool, flags other than 0 / SS_MIX_MONO, a pool that already has tables. */
+int ss_pool_levels(ss_pool* pool, uint32_t flags);
+/* Device pointer of candidate i's table (N + 1 doubles), or NULL without tables or with i outside [0, n). */
+const double* ss_pool_level_table(const ss_pool* pool, int i);
+
 /* library / build identification */
-int ss_version(void);        /* 106: source pools (ss_pool_create, pooled slots in plans) */
+int ss_version(void);        /* 107: level tables of pools (ss_pool_levels) and start draws in plans (ss_plan_create_ex) */
 const char* ss_strerror(int status);
 int ss_last_cuda_error(void);
 
@@ -286,7 +305,7 @@ void ss_plan_destroy(ss_plan* plan);
  *   - Outputs: mix (E), speakers_out (S, E) = each speaker after its gain (speaker 0's gain is 1), rms_db (S) =
  *     compute_mch_rms_dB (:29-32) of every speaker stem before its gain, after the fold with SS_MIX_MONO, rounded to
  *     float32 (-200 for a silent stem, from the 1e-20 floor).  rms_db lets a caller apply the dataloader's silence rule
- *     (:84-101, redraw when a speaker's crop is below -40 dB) by masking or redrawing; the plan itself does not loop.
+ *     (:84-101, redraw when a speaker's crop is below -40 dB) by masking or redrawing, or draw the starts on the device (ss_plan_draw below).
  *   - sirs, snr (and every win_start_dev of the plan's sources) are read on the device at every run: write them on the
  *     run's stream before the run, or in an order that is guaranteed to come before it.
  * Refused at creation, before anything is allocated and with no plan created:
@@ -313,6 +332,42 @@ typedef struct {
 } ss_plan_mix;
 int ss_plan_create_mix(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                        ss_plan** out);
+
+/* ---- start draws in plans (version 107): the crop start loop of the separation dataloader
+ * (separation/look2hear/datas/movingdatamodule.py:81-99), which draws up to 101 starts and rejects each one while any
+ * speaker's crop is below -40 dB (compute_mch_rms_dB, :29-32), keeping the last one when every draw fails - made on the
+ * device at every run, from uniform variates the caller supplies.
+ *   - The readers of a draw are the plan's items whose win_start_dev is the draw's `start`; len is their win_len; M is
+ *     the least over the readers of (picked candidate's N) - len + 1, the picks clamped into [0, n) as k_blocks clamps
+ *     them.
+ *   - Try t (0 <= t < tries) has the start s_t = min(floor(u[t] * M), M - 1) in float64 (u >= 1 gives M - 1, u < 0 or
+ *     NaN gives 0); speaker k is silent at s_t when 10 log10(max(1e-20, (Q_k[s_t + len] - Q_k[s_t]) / D_k)) <
+ *     threshold_db, Q_k the level table (ss_pool_levels) of speaker k's picked candidate, D_k = len for a mono table
+ *     and C * len otherwise.
+ *   - The draw takes the first try at which no speaker is silent, or s_{tries - 1} when there is none, and writes it to
+ *     `start` (and to `used` the 1-based index of that try, or 0).
+ * All draws run in one kernel launch at the head of every run (the graph's first node), before anything reads a start:
+ * a run with draws launches exactly one kernel more than the same plan without them.  u and the picks are read at every
+ * run: write them on the run's stream, or in an order that is guaranteed to come before it.  No error bit is added: a
+ * clamped pick is reported as bit 3 by k_blocks.
+ * Refused at creation, before anything is allocated:
+ *   - S > 8, tries > 4096, more than 16 readers, more than 65535 draws: SS_ERR_UNSUPPORTED;
+ *   - S < 1, tries < 1, a NULL start or u, a threshold that is not finite, u not 8-byte or used not 4-byte aligned, a
+ *     speaker index outside [0, n_items) or repeated, a speaker that is not a pooled slot of a pool with level tables or
+ *     whose win_start_dev is not `start`, a reader that is not a pooled slot, readers whose win_len differ, two draws
+ *     with one `start`, and a `start` or `used` range that meets any other range the plan reads or writes (other than
+ *     the readers' own reads of `start`; u counts as read): SS_ERR_INVALID. */
+typedef struct {
+    int32_t* start;           /* device int32 that this draw's readers read (their win_start_dev); written at every run */
+    const double* u;          /* device, `tries` doubles in [0, 1), read at every run                                  */
+    int32_t* used;            /* device int32 or NULL: 1-based index of the accepted try, 0 if every try was silent   */
+    int32_t speakers[8];      /* indices into `items`: the crops that must not be silent                               */
+    int32_t S, tries;         /* 1..8; 1..4096 (the dataloader's loop is 101)                                          */
+    float threshold_db;       /* -40 in the dataloader                                                                 */
+} ss_plan_draw;
+/* n_draws == 0 makes it ss_plan_create_mix */
+int ss_plan_create_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                      const ss_plan_draw* draws, int n_draws, ss_plan** out);
 
 /* Same, host pointers: H2D -> render -> D2H, pipelined over chunks on internal streams.  Returns
  * when every `out` is complete.  This is what the drop-in Python functions call. */

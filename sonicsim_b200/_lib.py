@@ -48,6 +48,13 @@ class SsPlanMix(ctypes.Structure):
                 ("noise_delay", ctypes.c_int32)]
 
 
+class SsPlanDraw(ctypes.Structure):
+    """`ss_plan_draw` of include/sonicsim_b200.h."""
+    _fields_ = [("start", ctypes.c_void_p), ("u", ctypes.c_void_p), ("used", ctypes.c_void_p),
+                ("speakers", ctypes.c_int32 * 8), ("S", ctypes.c_int32), ("tries", ctypes.c_int32),
+                ("threshold_db", ctypes.c_float)]
+
+
 class SsDryClip(ctypes.Structure):
     """`ss_dry_clip` of include/sonicsim_b200.h."""
     _fields_ = [("src", ctypes.c_void_p), ("kernel_t", ctypes.c_void_p), ("dst_start", ctypes.c_int64),
@@ -133,6 +140,8 @@ def load():
         lib.ss_plan_create.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_plan_create_mix.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPlanMix),
                                             ctypes.c_int, ctypes.POINTER(vp)]
+        lib.ss_plan_create_ex.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPlanMix),
+                                          ctypes.c_int, ctypes.POINTER(SsPlanDraw), ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_plan_run.argtypes = [vp, vp]
         lib.ss_plan_is_graph.argtypes = [vp]
         lib.ss_plan_destroy.argtypes = [vp]
@@ -148,6 +157,9 @@ def load():
         lib.ss_pool_bytes.restype = i64
         lib.ss_pool_destroy.argtypes = [vp]
         lib.ss_pool_destroy.restype = None
+        lib.ss_pool_levels.argtypes = [vp, ctypes.c_uint32]
+        lib.ss_pool_level_table.argtypes = [vp, ctypes.c_int]
+        lib.ss_pool_level_table.restype = vp
         lib.ss_render_host.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int]
         lib.ss_render_host_ex.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPostLufs)]
         lib.ss_convolve_fixed_receiver.argtypes = [vp, vp, vp, vp, i32, i32, i32]
@@ -180,7 +192,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_destroy", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

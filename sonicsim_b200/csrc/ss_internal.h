@@ -86,6 +86,12 @@ struct MixItem {
 // The four mixture kernels over the n descriptors at `d` (device memory), asynchronous on `stream`.
 int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream);
 
+// One level table of a pool candidate (ss_pool_levels): from the (C, N) stem y, q[0] = 0 and q[n + 1] = q[n] + e[n] in
+// float64, e[n] the square of the mixture kernels' channel fold at n (mono) or the float64 sum of the C channels' squares.
+struct LevelItem { const float* y; double* q; long long N; int C; int pad; };
+// k_levels over the n descriptors at `d` (device memory), one CTA per table, asynchronous on `stream`.
+int levels_enqueue(ss_ctx* c, const LevelItem* d, int n, bool mono, cudaStream_t stream);
+
 // Take the next slot of the descriptor ring (pinned host block + its device twin), grown to `bytes`, for work on
 // `stream`.  Blocks the host until the slot's previous host->device copy has completed (the pinned block is free), and
 // makes `stream` wait for the slot's previous readers, whatever stream they ran on (the device block is free; a no-op

@@ -598,7 +598,7 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 106; }
+extern "C" int ss_version(void) { return 107; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -805,7 +805,13 @@ struct ss_pool {
     std::vector<int32_t> bounds_host;     // every moving candidate's bounds, back to back
     std::vector<int64_t> bounds_off;      // candidate i's bounds at bounds_host[bounds_off[i]]
     std::vector<std::pair<int, int>> caps;  // (win_len, table size) already worked out (pool_table_cap)
+    std::vector<const ss_bank*> banks;    // candidate i's bank (ss_pool_levels renders the candidates)
     cudaEvent_t ready = nullptr;          // behind the construction of every candidate's bank
+    // level tables (ss_pool_levels): every candidate's N + 1 doubles back to back, and a device array of n pointers
+    double* levels = nullptr;
+    const double** level_ptr = nullptr;
+    std::vector<int64_t> level_off;       // candidate i's table at levels + level_off[i]
+    int level_flags = -1;                 // SS_MIX_MONO or 0 once the tables exist
 };
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
@@ -1367,10 +1373,20 @@ extern "C" void ss_pool_destroy(ss_pool* pl) {
     cudaSetDevice(pl->c->device);
     cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
     if (pl->table) cudaFree(pl->table);
+    if (pl->levels) cudaFree(pl->levels);
+    if (pl->level_ptr) cudaFree(pl->level_ptr);
     if (pl->ready) cudaEventDestroy(pl->ready);
     delete pl;
 }
-extern "C" int64_t ss_pool_bytes(const ss_pool* pl) { return pl ? (int64_t)sizeof(PoolEntry) * pl->n : 0; }
+extern "C" int64_t ss_pool_bytes(const ss_pool* pl) {
+    if (!pl) return 0;
+    int64_t b = (int64_t)sizeof(PoolEntry) * pl->n;
+    if (pl->levels) b += (int64_t)sizeof(double) * pl->level_off[pl->n] + (int64_t)sizeof(double*) * pl->n;
+    return b;
+}
+extern "C" const double* ss_pool_level_table(const ss_pool* pl, int i) {
+    return pl && pl->levels && i >= 0 && i < pl->n ? pl->levels + pl->level_off[i] : nullptr;
+}
 
 static int pool_build(ss_pool* pl, const ss_source* cand) {
     ss_ctx* c = pl->c;
@@ -1396,6 +1412,7 @@ static int pool_build(ss_pool* pl, const ss_source* cand) {
             pl->bounds_host.insert(pl->bounds_host.end(), it.bounds_host, it.bounds_host + it.P);
         }
         if (std::find(banks.begin(), banks.end(), b) == banks.end()) banks.push_back(const_cast<ss_bank*>(b));
+        pl->banks.push_back(b);
     }
     CK(cudaMalloc((void**)&pl->table, sizeof(PoolEntry) * (size_t)pl->n));
     CK(cudaMemcpy(pl->table, pl->host.data(), sizeof(PoolEntry) * (size_t)pl->n, cudaMemcpyHostToDevice));
@@ -1603,12 +1620,91 @@ extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, voi
     });
 }
 
+// ----------------------------------------------------------------------------- level tables of a pool
+// Candidates are rendered whole by ss_render_dev into one transient buffer, in groups of consecutive candidates whose
+// stems fit kLevelStemBytes (a larger candidate is a group of its own), and k_levels turns each group into its tables.
+constexpr size_t kLevelStemBytes = 256ull << 20;
+
+static int levels_build(ss_pool* pl, bool mono, cudaStream_t s, float** tmp, LevelItem** d_items) {
+    ss_ctx* c = pl->c;
+    const int n = pl->n;
+    pl->level_off.assign(n + 1, 0);
+    size_t cap = kLevelStemBytes;
+    for (int i = 0; i < n; ++i) {
+        pl->level_off[i + 1] = pl->level_off[i] + pl->host[i].N + 1;
+        cap = std::max(cap, align_up(4 * (size_t)pl->C * pl->host[i].N, 256));
+    }
+    CK(cudaMalloc((void**)&pl->levels, sizeof(double) * (size_t)pl->level_off[n]));
+    CK(cudaMalloc((void**)&pl->level_ptr, sizeof(double*) * (size_t)n));
+    std::vector<const double*> ptr(n);
+    for (int i = 0; i < n; ++i) ptr[i] = pl->levels + pl->level_off[i];
+    CK(cudaMemcpy(pl->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
+    // groups [first[g], first[g + 1]) and every candidate's stem in the transient buffer
+    std::vector<int> first(1, 0);
+    std::vector<size_t> at(n);
+    size_t used = 0;
+    for (int i = 0; i < n; ++i) {
+        const size_t b = align_up(4 * (size_t)pl->C * pl->host[i].N, 256);
+        if (used > 0 && used + b > cap) { first.push_back(i); used = 0; }
+        at[i] = used;
+        used += b;
+    }
+    first.push_back(n);
+    CK(cudaMalloc((void**)tmp, cap));
+    std::vector<LevelItem> li(n);
+    for (int i = 0; i < n; ++i)
+        li[i] = {(const float*)((char*)*tmp + at[i]), pl->levels + pl->level_off[i], pl->host[i].N, pl->C, 0};
+    CK(cudaMalloc((void**)d_items, sizeof(LevelItem) * (size_t)n));
+    CK(cudaMemcpy(*d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
+    CK(cudaStreamWaitEvent(s, pl->ready, 0));           // banks may still be building
+    std::vector<ss_source> items;
+    for (size_t g = 0; g + 1 < first.size(); ++g) {
+        items.clear();
+        for (int i = first[g]; i < first[g + 1]; ++i) {
+            const PoolEntry& e = pl->host[i];
+            ss_source it; memset(&it, 0, sizeof(it));
+            it.x = e.x; it.out = (float*)li[i].y; it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->L; it.mode = pl->mode;
+            it.rir_bank = pl->banks[i];
+            if (pl->mode == SS_MOVING_BOUNDS) { it.bounds = e.bounds; it.bounds_host = pl->bounds_host.data() + pl->bounds_off[i]; }
+            items.push_back(it);
+        }
+        int st = ss_render_dev(c, items.data(), (int)items.size(), (void*)s);     // the next group waits on `s` for
+        if (st == SS_OK) st = levels_enqueue(c, *d_items + first[g], first[g + 1] - first[g], mono, s);   // k_levels
+        if (st) return st;
+    }
+    CK(cudaStreamSynchronize(s));
+    return SS_OK;
+}
+
+extern "C" int ss_pool_levels(ss_pool* pl, uint32_t flags) {
+    if (!pl || (flags & ~SS_MIX_MONO) || pl->level_flags >= 0 || pl->levels) return SS_ERR_INVALID;
+    CK(cudaSetDevice(pl->c->device));
+    cudaStream_t s = nullptr;
+    CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    float* tmp = nullptr;
+    LevelItem* d_items = nullptr;
+    int st = levels_build(pl, (flags & SS_MIX_MONO) != 0, s, &tmp, &d_items);
+    if (st != SS_OK) cudaStreamSynchronize(s);
+    if (tmp) cudaFree(tmp);
+    if (d_items) cudaFree(d_items);
+    cudaStreamDestroy(s);
+    if (st != SS_OK) {                                  // no tables: the pool is as it was
+        if (pl->levels) cudaFree(pl->levels);
+        if (pl->level_ptr) cudaFree(pl->level_ptr);
+        pl->levels = nullptr; pl->level_ptr = nullptr;
+        return st;
+    }
+    pl->level_flags = (int)flags;
+    return SS_OK;
+}
+
 // ----------------------------------------------------------------------------- plans (device path)
 // A batch of device-resident sources bound once: validation, chunking, block tables and descriptor blocks are done at
 // creation and stay resident in device memory together with the plan's own scratch, so a run is kernel launches only -
 // captured into a CUDA graph on the first run (fork onto the context's internal streams, join back), one
 // cudaGraphLaunch per run afterwards instead of ~25 runtime calls.  The pointers in `items` (and the contents of
 // bounds_host) must stay valid and unchanged for the plan's life; buffer *contents* may change between runs.
+struct DrawDesc;
 struct ss_plan {
     ss_ctx* c = nullptr;
     std::vector<ChunkLaunch> chunks;
@@ -1625,7 +1721,82 @@ struct ss_plan {
     std::vector<ss_pool*> pools;       // pools of its pooled slots: every run waits for each pool's `ready` event
     const MixItem* d_mix = nullptr;   // the mixtures' descriptors, in d_desc behind the chunk descriptors
     int n_mix = 0;
+    const DrawDesc* d_draw = nullptr;  // the start draws' descriptors (k_draw), in d_desc behind the mixture scratch
+    int n_draw = 0;
 };
+
+// ----------------------------------------------------------------------------- k_draw
+// Crop start draws of a plan (ss_plan_draw).  A reader is a pooled slot whose win_start_dev is the draw's start; the
+// speakers are readers with level tables.  The picks are clamped as k_blocks clamps them (which reports bit 3).
+constexpr int kDrawReaders = 16, kDrawSpeakers = 8, kDrawTries = 4096, kMaxDraws = 65535;
+struct DrawReader {
+    const PoolEntry* pool;            // the slot's pool table ...
+    const int* pick;                  // ... and pick
+    const double* const* levels;      // the pool's level table pointers (speakers), else null
+    int n;                            // candidates in the pool
+    double D;                         // elements of one crop in a table: len (mono) or C * len
+};
+struct DrawDesc {
+    int* start;
+    const double* u;
+    int* used;
+    int tries, len, n_readers, S;
+    float threshold_db;
+    int spk[kDrawSpeakers];           // speaker k is reader spk[k]
+    DrawReader r[kDrawReaders];
+};
+
+// One warp per draw: the readers' picked N give M (a lane per reader), then 32 tries at a time, a lane per try, and a
+// ballot takes the first try at which no speaker is silent; after the last try without one, the last try's start.
+__global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws, int n) {
+    const int lane = threadIdx.x & 31, di = blockIdx.x * 4 + (threadIdx.x >> 5);
+    if (di >= n) return;
+    const DrawDesc& d = draws[di];
+    bool bad;
+    int M = 0x7fffffff;
+    if (lane < d.n_readers) {
+        const DrawReader& r = d.r[lane];
+        M = draw_span(r.pool[clamp_pick(*r.pick, r.n, bad)].N, d.len);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) M = min(M, __shfl_xor_sync(0xffffffffu, M, o));
+    const double* Q[kDrawSpeakers];
+    double D[kDrawSpeakers];
+#pragma unroll
+    for (int k = 0; k < kDrawSpeakers; ++k) {
+        Q[k] = nullptr; D[k] = 1.0;
+        if (k < d.S) {
+            const DrawReader& r = d.r[d.spk[k]];
+            Q[k] = r.levels[clamp_pick(*r.pick, r.n, bad)];
+            D[k] = r.D;
+        }
+    }
+    int start = 0, used = 0;
+    for (int base = 0; base < d.tries; base += 32) {
+        const int t = base + lane;
+        int s = 0;
+        bool pass = false;
+        if (t < d.tries) {
+            s = draw_start(d.u[t], M);
+            pass = true;
+#pragma unroll
+            for (int k = 0; k < kDrawSpeakers; ++k)
+                if (k < d.S && pass && draw_silent(Q[k], s, d.len, D[k], d.threshold_db)) pass = false;
+        }
+        const unsigned ok = __ballot_sync(0xffffffffu, pass);
+        if (ok) {
+            const int f = __ffs(ok) - 1;
+            start = __shfl_sync(0xffffffffu, s, f);
+            used = base + f + 1;
+            break;
+        }
+        if (base + 32 >= d.tries) start = __shfl_sync(0xffffffffu, s, d.tries - 1 - base);
+    }
+    if (lane == 0) {
+        *d.start = start;
+        if (d.used) *d.used = used;
+    }
+}
 
 extern "C" void ss_plan_destroy(ss_plan* p) {
     if (!p) return;
@@ -1654,8 +1825,24 @@ static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double
     return d;
 }
 
+// The descriptor of draw d of a plan: its readers in the callers' order of `items`
+static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan_draw& d) {
+    DrawDesc g; memset(&g, 0, sizeof(g));
+    g.start = d.start; g.u = d.u; g.used = d.used; g.tries = d.tries; g.S = d.S; g.threshold_db = d.threshold_db;
+    for (int i = 0; i < n_items; ++i) {
+        const ss_source& it = items[i];
+        if (it.win_start_dev != d.start) continue;
+        for (int k = 0; k < d.S; ++k) if (d.speakers[k] == i) g.spk[k] = g.n_readers;
+        const ss_pool* pl = it.pool;
+        g.len = it.win_len;
+        g.r[g.n_readers++] = {pl->table, it.pick_dev, pl->level_ptr, pl->n,
+                              (double)it.win_len * ((pl->level_flags & SS_MIX_MONO) ? 1 : pl->C)};
+    }
+    return g;
+}
+
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
-                      const ss_plan_mix* mixes, int n_mixes) {
+                      const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws) {
     ss_ctx* c = p->c;
     std::vector<int> cuts;
     std::vector<ss_source> arranged;
@@ -1677,7 +1864,8 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     // behind the chunk descriptors: the mixtures' descriptors, then one mixture scratch block each
     const size_t mix_off = off[n_chunks], scr_off = mix_off + align_up(sizeof(MixItem) * n_mixes, 256);
     const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
-    const size_t desc_bytes = scr_off + scr_bytes * n_mixes;
+    const size_t draw_off = align_up(scr_off + scr_bytes * n_mixes, 256);
+    const size_t desc_bytes = draw_off + sizeof(DrawDesc) * n_draws;
     CK(cudaMalloc((void**)&p->d_desc, desc_bytes + 256));
     for (int i = 0; i < ss_ctx::kAux; ++i)
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
@@ -1694,6 +1882,13 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         p->n_mix = n_mixes;
     }
     CK(cudaMemcpy(p->d_desc, host.data(), scr_off, cudaMemcpyHostToDevice));
+    if (n_draws > 0) {
+        std::vector<DrawDesc> g(n_draws);
+        for (int k = 0; k < n_draws; ++k) g[k] = draw_describe(caller_items, n_items, draws[k]);
+        CK(cudaMemcpy(p->d_desc + draw_off, g.data(), sizeof(DrawDesc) * n_draws, cudaMemcpyHostToDevice));
+        p->d_draw = (const DrawDesc*)(p->d_desc + draw_off);
+        p->n_draw = n_draws;
+    }
     return SS_OK;
 }
 
@@ -1714,9 +1909,45 @@ static bool written_ranges_disjoint(std::vector<ByteRange>& r) {
     return true;
 }
 
-static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes) {
+// A plan's start draws (include/sonicsim_b200.h, ss_plan_draw), all but the byte ranges (validate_mixes)
+static int validate_draws(const ss_source* items, int n_items, const ss_plan_draw* draws, int n_draws) {
+    if (n_draws > kMaxDraws) return SS_ERR_UNSUPPORTED;
+    for (int k = 0; k < n_draws; ++k) {
+        const ss_plan_draw& d = draws[k];
+        if (d.S > kDrawSpeakers || d.tries > kDrawTries) return SS_ERR_UNSUPPORTED;
+        if (d.S < 1 || d.tries < 1 || !d.start || !d.u || !isfinite(d.threshold_db)) return SS_ERR_INVALID;
+        if (((uintptr_t)d.u & 7) || ((uintptr_t)d.used & 3)) return SS_ERR_INVALID;
+        for (int j = 0; j < k; ++j) if (draws[j].start == d.start) return SS_ERR_INVALID;
+        for (int s = 0; s < d.S; ++s) {
+            const int i = d.speakers[s];
+            if (i < 0 || i >= n_items) return SS_ERR_INVALID;
+            for (int j = 0; j < s; ++j) if (d.speakers[j] == i) return SS_ERR_INVALID;
+            const ss_source& it = items[i];
+            if (!it.pool || !it.pool->levels || it.win_start_dev != d.start) return SS_ERR_INVALID;
+        }
+        int readers = 0, len = -1;
+        for (int i = 0; i < n_items; ++i) {
+            const ss_source& it = items[i];
+            if (it.win_start_dev != d.start) continue;
+            if (!it.pool || (len >= 0 && it.win_len != len)) return SS_ERR_INVALID;
+            len = it.win_len;
+            ++readers;
+        }
+        if (readers > kDrawReaders) return SS_ERR_UNSUPPORTED;
+    }
+    return SS_OK;
+}
+
+static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                          const ss_plan_draw* draws, int n_draws) {
     if (n_mixes > 65535) return SS_ERR_UNSUPPORTED;         // one gridDim.y row per mixture
     std::vector<ByteRange> r;
+    // a draw writes its start (which only its readers read) and `used`, and reads its u
+    for (int k = 0; k < n_draws; ++k) {
+        add_range(r, draws[k].start, 4, true);
+        add_range(r, draws[k].used, 4, true);
+        add_range(r, draws[k].u, 8 * (uint64_t)draws[k].tries, false);
+    }
     for (int k = 0; k < n_mixes; ++k) {
         const ss_plan_mix& m = mixes[k];
         if (m.S < 1 || m.M < 1 || m.S > kMixStems || m.M > kMixStems) return SS_ERR_UNSUPPORTED;
@@ -1754,7 +1985,9 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
             add_range(r, it.idx, 4 * (uint64_t)it.N, false);
             add_range(r, it.w, 4 * (uint64_t)it.N, false);
         }
-        add_range(r, it.win_start_dev, 4, false);
+        bool drawn = false;
+        for (int k = 0; k < n_draws; ++k) drawn = drawn || draws[k].start == it.win_start_dev;
+        if (!drawn) add_range(r, it.win_start_dev, 4, false);
         add_range(r, it.pick_dev, 4, false);
     }
     // a pooled slot may read any candidate: every candidate's x and bounds, once per pool
@@ -1770,13 +2003,14 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
 }
 
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
-                       ss_plan** out) {
+                       const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
-    { int st = validate_mixes(items, n_items, mixes, n_mixes); if (st) return st; }
+    { int st = validate_draws(items, n_items, draws, n_draws); if (st) return st; }
+    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
@@ -1786,25 +2020,41 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes);
+    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     *out = p;
     return SS_OK;
 }
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
-    return plan_create(c, items, n_items, nullptr, 0, out);
+    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, out);
 }
 
-// the launches of every chunk (run_chunks), then the mixtures (which read every chunk's outputs) on `stream`
+extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                 int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
+    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws)) return SS_ERR_INVALID;
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, out);
+}
+
+// The start draws (k_draw) on `stream`, ahead of everything that reads a start
+static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, cudaStream_t stream) {
+    k_draw<<<(n + 3) / 4, 128, 0, stream>>>(d, n);
+    CK(cudaGetLastError());
+    c->launches += 1;
+    return SS_OK;
+}
+
+// the start draws, the launches of every chunk (run_chunks), then the mixtures (which read every chunk's outputs) on
+// `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
+    if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, stream); if (st) return st; }
     const int rc = run_chunks(c, p->chunks.size(), stream, p->ev_fork, p->ev_join, [&](size_t k, cudaStream_t s, int) {
         return chunk_enqueue(c, p->chunks[k], s, c->profiling);
     });

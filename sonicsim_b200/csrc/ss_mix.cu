@@ -217,6 +217,52 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
     }
 }
 
+// Level tables of pool candidates (ss_pool_levels): one CTA per table walks the stem in tiles of kLevelThreads *
+// kLevelPer samples.  Each thread sums its kLevelPer consecutive terms in order, a warp shuffle scan and the warps'
+// totals in warp order place them in the tile, and a carry runs from tile to tile, so the bits depend on N alone: not
+// on the grouping, the launch or the run.  The mono term is fold() itself, the term k_mix_energy squares.
+constexpr int kLevelThreads = 256, kLevelPer = 8;
+__global__ void __launch_bounds__(kLevelThreads) k_levels(const LevelItem* __restrict__ items, int mono) {
+    __shared__ double sh[kLevelThreads / 32];
+    const LevelItem L = items[blockIdx.x];
+    MixItem it;
+    it.Cf = L.C; it.T = L.N;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) L.q[0] = 0.0;
+    double carry = 0.0;
+    for (long long base = 0; base < L.N; base += (long long)kLevelThreads * kLevelPer) {
+        const long long n0 = base + (long long)threadIdx.x * kLevelPer;
+        double run[kLevelPer];
+        double acc = 0.0;
+#pragma unroll
+        for (int j = 0; j < kLevelPer; ++j) {
+            const long long n = n0 + j;
+            double e = 0.0;
+            if (n < L.N) {
+                if (mono) { const float v = fold(it, L.y, n); e = (double)(v * v); }
+                else for (int c = 0; c < L.C; ++c) { const float v = L.y[(long long)c * L.N + n]; e += (double)(v * v); }
+            }
+            acc += e;
+            run[j] = acc;
+        }
+        double incl = acc;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const double v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+        double excl = __shfl_up_sync(0xffffffffu, incl, 1);
+        if (lane == 0) excl = 0.0;
+        if (lane == 31) sh[warp] = incl;
+        __syncthreads();
+        double wpre = 0.0, tile = 0.0;
+        for (int w = 0; w < kLevelThreads / 32; ++w) { if (w < warp) wpre += sh[w]; tile += sh[w]; }
+        const double pre = carry + (wpre + excl);
+#pragma unroll
+        for (int j = 0; j < kLevelPer; ++j)
+            if (n0 + j < L.N) L.q[n0 + j + 1] = pre + run[j];
+        carry += tile;
+        __syncthreads();                                  // sh is rewritten by the next tile
+    }
+}
+
 // true when the byte ranges [a, a + na) and [b, b + nb) share a byte
 bool ranges_meet(const void* a, size_t na, const void* b, size_t nb) {
     const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
@@ -287,6 +333,13 @@ int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream) {
     k_mix_write<<<grid, 256, 0, stream>>>(d);
     CK(cudaGetLastError());
     c->launches += 4;
+    return SS_OK;
+}
+
+int levels_enqueue(ss_ctx* c, const LevelItem* d, int n, bool mono, cudaStream_t stream) {
+    k_levels<<<n, kLevelThreads, 0, stream>>>(d, mono ? 1 : 0);
+    CK(cudaGetLastError());
+    c->launches += 1;
     return SS_OK;
 }
 

@@ -275,6 +275,25 @@ SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, co
     }
     return best;
 }
+// ---- crop start draws of device plans (ss_plan_draw, include/sonicsim_b200.h): the dataloader's start loop
+// (movingdatamodule.py:81-99) over level tables Q (ss_pool_levels: Q[0] = 0, Q[n + 1] = Q[n] + e[n], float64).
+// Starts a crop of len samples can take in a candidate of N samples: the M of a draw is the least of these over its readers
+SS_HD int draw_span(int N, int len) { return N - len + 1; }
+// Try t's start: min(floor(u * M), M - 1), in float64 (randint(0, M - 1) with its uniform variate given); a u outside
+// [0, 1) maps into range: u >= 1 to M - 1, u < 0 or NaN to 0
+SS_HD int draw_start(double u, int M) {
+    const double v = floor(u * (double)M);
+    if (!(v > 0.0)) return 0;
+    return v < (double)(M - 1) ? (int)v : M - 1;
+}
+// compute_mch_rms_dB (:29-32) of the crop [s, s + len) of a table below the threshold: silent.  D = len (mono table) or
+// C * len (channel table): the crop's element count
+SS_HD bool draw_silent(const double* Q, int s, int len, double D, float threshold_db) {
+    double ms = (Q[s + len] - Q[s]) / D;
+    if (ms < 1e-20) ms = 1e-20;
+    return 10.0 * log10(ms) < (double)threshold_db;
+}
+
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
 SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }

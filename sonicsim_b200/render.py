@@ -84,6 +84,26 @@ class Pooled(T.NamedTuple):
     direct_taps: int = 0
 
 
+class CropDraw(T.NamedTuple):
+    """A crop start drawn on the device at every run of a device plan (Renderer.plan_device(draws=...)): the dataloader's
+    start loop (movingdatamodule.py:81-99).  `start`: the one-element CUDA int32 tensor that the windows of this
+    example's pooled slots use as their start (those slots are the draw's readers, all of one window length).  `speakers`:
+    indices into the plan's sources, 1 to 8 pooled slots among the readers whose pools have level tables
+    (Renderer.source_pool(levels=...)).  `u`: a CUDA float64 tensor of 1 to 4096 uniform variates in [0, 1) (e.g. a row
+    of torch.rand((B, 101), dtype=torch.float64)), read at every run.  Try t starts at min(floor(u[t] * M), M - 1), M
+    the number of starts every reader's picked candidate holds; the draw keeps the first try at which no speaker's crop is
+    below `threshold_db` (compute_mch_rms_dB of the crop), else the last try.  `used`, if given (one-element CUDA int32),
+    receives the 1-based index of the kept try, or 0 when every try was silent."""
+    start: T.Any
+    speakers: T.Sequence[int]
+    u: T.Any
+    used: T.Any = None
+    threshold_db: float = -40.0
+
+
+LEVELS = {None: None, "mono": _lib.SS_MIX_MONO, "channels": 0}
+
+
 def _is_tensor(v) -> bool:
     return type(v).__module__.split(".")[0] == "torch"
 
@@ -191,15 +211,30 @@ class SourcePool(_Held):
     pooled slots (render.Pooled) of device plans pick from at every run.  `n` candidates of one `mode`, `C` and `L`;
     `n_min` is the shortest candidate's N (the longest window a slot may take); `direct_taps` > 0 when every candidate's
     bank holds a direct set with these taps.  The pool holds its candidates' banks and keeps their tensors alive; plans
-    hold the pool, which is freed once it is closed (or collected) and no live plan uses it any more."""
+    hold the pool, which is freed once it is closed (or collected) and no live plan uses it any more.  `levels` is None,
+    "mono" or "channels": the level tables the pool holds for start draws (CropDraw), included in `nbytes`."""
 
-    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps):
+    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None):
         self.renderer, self._h = renderer, handle
         self.candidates = list(candidates)
         self.n, self.mode, self.C, self.L = len(self.candidates), mode, C, L
-        self.n_min, self.direct_taps = n_min, direct_taps
+        self.n_min, self.direct_taps, self.levels = n_min, direct_taps, levels
         self.nbytes = int(renderer.lib.ss_pool_bytes(handle))
         self._banks = _hold_banks(self, self.candidates)
+
+    def level_table(self, i):
+        """A float64 CUDA copy of candidate i's level table (N + 1 values: Q[0] = 0, Q[n + 1] = Q[n] + e[n]), see
+        ss_pool_levels; None without tables."""
+        import torch
+        if self.closed or self.levels is None or not 0 <= i < self.n:
+            return None
+        ptr = self.renderer.lib.ss_pool_level_table(self._h, int(i))
+        n = self.candidates[i].dry.numel() + 1
+
+        class _View:
+            __cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (ptr, False), "version": 3}
+        with torch.cuda.device(self.renderer.device):
+            return torch.as_tensor(_View(), device="cuda:%d" % self.renderer.device).clone()
 
     def _free(self):
         if self._h:
@@ -305,13 +340,21 @@ class Renderer:
         return RirBank(self, h, shape, normalize, taps)
 
     # ------------------------------------------------------------------ source pools
-    def source_pool(self, candidates: T.Sequence[T.Union[MovingSource, StaticSource]]) -> SourcePool:
+    def source_pool(self, candidates: T.Sequence[T.Union[MovingSource, StaticSource]],
+                    levels: T.Optional[str] = None) -> SourcePool:
         """Validate and upload a set of candidate sources once, for pooled slots (render.Pooled) of device plans to pick
         from at every run.  Every candidate is a MovingSource or StaticSource whose RIRs are a RirBank of this renderer
         (`dry`, `bounds`: contiguous CUDA tensors of its device; a moving candidate needs `bounds_host`), with no window,
         normalize_rirs or direct_taps (those belong to the slot and the bank); all share one kind (moving or static), C
-        and L.  The candidates' tensors and banks are kept alive by the pool."""
+        and L.  The candidates' tensors and banks are kept alive by the pool.
+
+        `levels` = "mono" or "channels" also builds every candidate's level table (ss_pool_levels: the float64 prefix
+        sums of the squares of its whole rendered stem, channel-folded like Mixture(mono=True) for "mono"), which
+        CropDraw reads to test crops for silence; 8 bytes per sample.  The call then returns when the tables are
+        complete.  They describe the dry signals as they are now: new signals need a new pool."""
         import torch
+        if levels not in LEVELS:
+            raise ValueError("source_pool: levels must be None, 'mono' or 'channels', got %r" % (levels,))
         n = len(candidates)
         if not 1 <= n <= 1 << 24:
             raise ValueError("source_pool: a pool holds 1 to 2^24 candidates, got %d" % n)
@@ -363,10 +406,15 @@ class Renderer:
                 items[i].bounds, items[i].bounds_host = s.bounds.data_ptr(), bh.ctypes.data
         h = ctypes.c_void_p()
         _lib.check(self.lib.ss_pool_create(self.ctx, items, n, ctypes.byref(h)))
+        if levels is not None:
+            st = self.lib.ss_pool_levels(h, LEVELS[levels])
+            if st != _lib.SS_OK:
+                self.lib.ss_pool_destroy(h)
+                _lib.check(st)
         banks = [s.rir if isinstance(s, StaticSource) else s.rirs for s in candidates]
         taps = {b.direct_taps for b in banks}
         return SourcePool(self, h, candidates, first[0], first[1], first[2], min(s.dry.numel() for s in candidates),
-                          taps.pop() if len(taps) == 1 else 0)
+                          taps.pop() if len(taps) == 1 else 0, levels)
 
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
@@ -474,7 +522,7 @@ class Renderer:
             stream = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.lib.ss_render_dev(self.ctx, items, n, ctypes.c_void_p(stream)))
 
-    def plan_device(self, sources, outs, direct_outs=None, mixtures=None) -> "DevicePlan":
+    def plan_device(self, sources, outs, direct_outs=None, mixtures=None, draws=None) -> "DevicePlan":
         """Bind a batch of device-resident sources to its output tensors once; `plan.run()` then renders it with a
         single C-ABI call - one CUDA graph launch (ss_plan_run; a generation loop overwrites the same tensors and
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
@@ -492,11 +540,78 @@ class Renderer:
             starts.copy_(torch.randint(...)); sirs.uniform_(-6, 6); snr.uniform_(10, 20)   # movingdatamodule.py:106, :119
             plan.run()                                          # crops, gains and mixtures of every scene
 
-        and the model takes (mix, speakers_out) from there; rms_db (Mixture) carries each speaker's level for the
-        dataloader's silence rule."""
+        and the model takes (mix, speakers_out) from there; rms_db (Mixture) carries each speaker's level.
+
+        `draws`: CropDraw entries, the dataloader's silence rule on the device: at the head of every run (one more
+        kernel launch), each draw picks its readers' start from its `u`, rejecting starts at which a speaker's crop is
+        below the threshold, before anything reads that start.  A step is then
+
+            u.uniform_(); picks.copy_(...); sirs.uniform_(-6, 6); snr.uniform_(10, 20)
+            plan.run()"""
         items, n, keep = self._device_items(sources, outs, direct_outs)
         mixes = self._device_mixes(mixtures, outs, keep) if mixtures else None
-        return DevicePlan(self, items, n, keep, mixes)
+        drw = self._device_draws(draws, sources, keep) if draws else None
+        return DevicePlan(self, items, n, keep, mixes, drw)
+
+    def _device_draws(self, draws, sources, keep):
+        """Validated ss_plan_draw array of a plan's start draws; their tensors are appended to `keep`."""
+        import torch
+        n = len(sources)
+        arr = (_lib.SsPlanDraw * len(draws))()
+        seen = set()
+        for k, d in enumerate(draws):
+            def chk(t, name, dtype, lo, hi):
+                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
+                    raise ValueError("plan_device: %s of draw %d must be a CUDA tensor on cuda:%d" % (name, k, self.device))
+                if t.dtype != dtype or not t.is_contiguous():
+                    raise ValueError("plan_device: %s of draw %d must be a contiguous %s tensor" % (name, k, dtype))
+                if not lo <= t.numel() <= hi:
+                    raise ValueError("plan_device: %s of draw %d must hold %s elements, got %d"
+                                     % (name, k, lo if lo == hi else "%d to %d" % (lo, hi), t.numel()))
+                return t.data_ptr()
+
+            start = chk(d.start, "start", torch.int32, 1, 1)
+            u = chk(d.u, "u", torch.float64, 1, 4096)
+            used = chk(d.used, "used", torch.int32, 1, 1) if d.used is not None else None
+            if start in seen:
+                raise ValueError("plan_device: draw %d shares its start tensor with another draw" % k)
+            seen.add(start)
+            if used is not None and used == start:
+                raise ValueError("plan_device: used of draw %d is its start tensor" % k)
+            thr = float(d.threshold_db)
+            if not np.isfinite(thr):
+                raise ValueError("plan_device: threshold_db of draw %d must be finite, got %r" % (k, thr))
+            spk = [int(v) for v in d.speakers]
+            if not 1 <= len(spk) <= 8:
+                raise ValueError("plan_device: draw %d must name 1 to 8 speakers, got %d" % (k, len(spk)))
+            if len(set(spk)) != len(spk):
+                raise ValueError("plan_device: draw %d names a speaker more than once" % k)
+            readers = [i for i, s in enumerate(sources)
+                       if s.window is not None and _is_tensor(s.window[0]) and s.window[0].data_ptr() == start]
+            for i in readers:
+                if not isinstance(sources[i], Pooled):
+                    raise ValueError("plan_device: source %d reads the start of draw %d but is not a pooled slot "
+                                     "(render.Pooled)" % (i, k))
+            if len({int(sources[i].window[1]) for i in readers}) > 1:
+                raise ValueError("plan_device: the readers of draw %d (sources %s) have different window lengths"
+                                 % (k, readers))
+            if len(readers) > 16:
+                raise ValueError("plan_device: draw %d has %d readers, at most 16" % (k, len(readers)))
+            for v in spk:
+                if not 0 <= v < n:
+                    raise ValueError("plan_device: draw %d names source %d of %d" % (k, v, n))
+                if v not in readers:
+                    raise ValueError("plan_device: speaker %d of draw %d does not take its window start from the "
+                                     "draw's start tensor" % (v, k))
+                if sources[v].pool.levels is None:
+                    raise ValueError("plan_device: speaker %d of draw %d: its SourcePool has no level tables "
+                                     "(source_pool(levels=...))" % (v, k))
+            e = arr[k]
+            for i, v in enumerate(spk):
+                e.speakers[i] = v
+            e.start, e.u, e.used, e.S, e.tries, e.threshold_db = start, u, used, len(spk), d.u.numel(), thr
+        keep.append(list(draws))
+        return arr
 
     def _device_mixes(self, mixtures, outs, keep):
         """Validated ss_plan_mix array of a plan's mixtures; their tensors are appended to `keep`."""
@@ -698,12 +813,17 @@ class Renderer:
 class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
-    mixtures, the plan also assembles them at every run (ss_plan_create_mix)."""
+    mixtures, the plan also assembles them at every run (ss_plan_create_mix); with draws, it first draws their starts
+    (ss_plan_create_ex)."""
 
-    def __init__(self, renderer, items, n, keep, mixes=None):
+    def __init__(self, renderer, items, n, keep, mixes=None, draws=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
+        self.draws = draws
         self._plan = ctypes.c_void_p()
-        if n > 0 and mixes:
+        if n > 0 and draws:
+            _lib.check(renderer.lib.ss_plan_create_ex(renderer.ctx, items, n, mixes, len(mixes) if mixes else 0,
+                                                      draws, len(draws), ctypes.byref(self._plan)))
+        elif n > 0 and mixes:
             _lib.check(renderer.lib.ss_plan_create_mix(renderer.ctx, items, n, mixes, len(mixes),
                                                        ctypes.byref(self._plan)))
         elif n > 0:
