@@ -108,6 +108,39 @@ def _is_tensor(v) -> bool:
     return type(v).__module__.split(".")[0] == "torch"
 
 
+def _tensor(t, api, owner, field, dtype, device, shape=None, count=None):
+    """Checks a tensor argument before any C call and returns its data_ptr(): a contiguous `dtype` CUDA tensor on
+    cuda:`device`, of `count` = (lo, hi) elements and of shape `shape` (a str entry such as "C" takes any size) when
+    given.  `owner` ("source 3", "mixture 1", ...) names what holds the tensor; None for an argument of `api` itself."""
+    import torch
+    what = "%s: %s" % (api, field) if owner is None else "%s: %s of %s" % (api, field, owner)
+    if not isinstance(t, torch.Tensor) or not t.is_cuda:
+        raise ValueError("%s must be a CUDA tensor on cuda:%d" % (what, device))
+    if t.device.index != device:
+        raise ValueError("%s is on cuda:%s, the renderer on cuda:%d" % (what, t.device.index, device))
+    if t.dtype != dtype:
+        raise ValueError("%s must be %s, got %s" % (what, dtype, t.dtype))
+    if not t.is_contiguous():
+        raise ValueError("%s must be contiguous" % what)
+    if count is not None and not count[0] <= t.numel() <= count[1]:
+        lo, hi = count
+        raise ValueError("%s must hold %s element%s, got %d" % (what, lo if lo == hi else "%d to %d" % count,
+                                                                  "" if hi == 1 else "s", t.numel()))
+    if shape is not None and (t.dim() != len(shape) or
+                              any(w != g for w, g in zip(shape, t.shape) if not isinstance(w, str))):
+        raise ValueError("%s must have shape %s, got %s" % (what, str(tuple(shape)).replace("'", ""), tuple(t.shape)))
+    return t.data_ptr()
+
+
+def _bounds(b, P, what, keep):
+    """A host bounds table as a contiguous int32 array of P entries, kept alive in `keep`; `what` names it."""
+    a = np.ascontiguousarray(b, dtype=np.int32)
+    if a.shape != (P,):
+        raise ValueError("%s must have P = %d entries, got shape %s" % (what, P, a.shape))
+    keep.append(a)
+    return a
+
+
 def _window(s, i, N):
     """(win_start, win_len, samples per output row) of source i; a window must lie inside [0, N] and not be empty."""
     if s.window is None:
@@ -243,13 +276,37 @@ class SourcePool(_Held):
             self._banks()                      # the pool no longer reads its banks
 
 
+def _rirs(s, conv=None):
+    """Where a MovingSource / StaticSource takes its RIRs from: (RirBank or None, raw RIRs or None, P, C, L, mode).
+    Raw RIRs go through conv(raw, field name, shape), the caller's conversion or check, and their shape is read from
+    what it returns (a NumPy array or a tensor); without `conv` they are returned as given, with P, C, L None."""
+    static = isinstance(s, StaticSource)
+    r, mode = (s.rir, _lib.SS_STATIC) if static else (s.rirs, _lib.SS_MOVING_BOUNDS)
+    if isinstance(r, RirBank):
+        return (r, None) + ((1,) + r.pcl[1:] if static else r.pcl) + (mode,)
+    if conv is None:
+        return None, r, None, None, None, mode
+    if static:
+        r = conv(r, "rir", ("C", "L"))
+        (C, L), P = r.shape, 1
+    else:
+        r = conv(r, "rirs", ("P", "C", "L"))
+        P, C, L = r.shape
+    return None, r, P, C, L, mode
+
+
+def _check_usable(held, renderer, what):
+    """Refuses a closed RirBank / SourcePool, or one of another renderer's context; `what` names it."""
+    if held.closed:
+        raise ValueError("%s is closed" % what)
+    if held.renderer.ctx.value != renderer.ctx.value:
+        raise ValueError("%s belongs to another renderer's context" % what)
+
+
 def _bank_of(renderer, s, i, P, C, L):
     """Checks a banked source against its bank before any C call; returns the ss_bank handle."""
-    b = s.rir if isinstance(s, StaticSource) else s.rirs
-    if b.closed:
-        raise ValueError("source %d: its RirBank is closed" % i)
-    if b.renderer.ctx.value != renderer.ctx.value:
-        raise ValueError("source %d: its RirBank belongs to another renderer's context" % i)
+    b = _rirs(s)[0]
+    _check_usable(b, renderer, "source %d: its RirBank" % i)
     if b.pcl != (P, C, L):
         raise ValueError("source %d: its RirBank holds (P, C, L) = %s, the source has %s" % (i, b.pcl, (P, C, L)))
     if s.normalize_rirs:
@@ -283,7 +340,7 @@ def _hold_banks(plan, sources):
     releases them at once, once)."""
     banks = []
     for s in sources:
-        b = s.pool if isinstance(s, Pooled) else (s.rir if isinstance(s, StaticSource) else s.rirs)
+        b = s.pool if isinstance(s, Pooled) else _rirs(s)[0]
         if isinstance(b, (RirBank, SourcePool)) and all(b is not o for o in banks):
             banks.append(b)
     for b in banks:
@@ -319,23 +376,20 @@ class Renderer:
             raise ValueError("direct_taps must be >= 0, got %d" % taps)
         flags = (_lib.SS_RIR_NORMALIZE if normalize else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
         h = ctypes.c_void_p()
-        if type(rirs).__module__.split(".")[0] == "torch":
+        dev = _is_tensor(rirs)
+        if dev:
             import torch
-            if not rirs.is_cuda or rirs.device.index != self.device:
-                raise ValueError("rir_bank: a tensor must be on cuda:%d" % self.device)
-            if rirs.dtype != torch.float32 or not rirs.is_contiguous() or rirs.dim() not in (2, 3):
-                raise ValueError("rir_bank: rirs must be a contiguous float32 (P, C, L) or (C, L) tensor")
-            shape = tuple(rirs.shape)
-            P, C, L = shape if len(shape) == 3 else (1,) + shape
+            _tensor(rirs, "rir_bank", None, "rirs", torch.float32, self.device)
+        a = rirs if dev else _as_f32(rirs)
+        shape = tuple(a.shape)
+        if len(shape) not in (2, 3):
+            raise ValueError("rir_bank: rirs must be (P, C, L) or (C, L), got shape %s" % (shape,))
+        P, C, L = shape if len(shape) == 3 else (1,) + shape
+        if dev:
             stream = torch.cuda.current_stream(rirs.device).cuda_stream
             _lib.check(self.lib.ss_bank_create_dev(self.ctx, rirs.data_ptr(), P, C, L, flags, taps,
                                                    ctypes.c_void_p(stream), ctypes.byref(h)))
         else:
-            a = _as_f32(rirs)
-            if a.ndim not in (2, 3):
-                raise ValueError("rir_bank: rirs must be (P, C, L) or (C, L), got shape %s" % (a.shape,))
-            shape = a.shape
-            P, C, L = shape if len(shape) == 3 else (1,) + shape
             _lib.check(self.lib.ss_bank_create_host(self.ctx, a.ctypes.data, P, C, L, flags, taps, ctypes.byref(h)))
         return RirBank(self, h, shape, normalize, taps)
 
@@ -365,45 +419,28 @@ class Renderer:
             if not isinstance(s, (MovingSource, StaticSource)):
                 raise ValueError("source_pool: candidate %d must be a MovingSource or StaticSource, got %s"
                                  % (i, type(s).__name__))
-            static = isinstance(s, StaticSource)
-            rb = s.rir if static else s.rirs
-            if not isinstance(rb, RirBank):
+            rb, _, P, C, L, mode = _rirs(s)
+            if rb is None:
                 raise ValueError("source_pool: candidate %d must take its RIRs from a RirBank" % i)
-            if rb.closed:
-                raise ValueError("source_pool: the RirBank of candidate %d is closed" % i)
-            if rb.renderer.ctx.value != self.ctx.value:
-                raise ValueError("source_pool: the RirBank of candidate %d belongs to another renderer's context" % i)
+            _check_usable(rb, self, "source_pool: the RirBank of candidate %d" % i)
             if s.window is not None or s.normalize_rirs or int(s.direct_taps):
                 raise ValueError("source_pool: candidate %d has a window, normalize_rirs or direct_taps; those belong to "
                                  "the pooled slot (render.Pooled) and the bank" % i)
-            P, C, L = rb.pcl
-            kind = (_lib.SS_STATIC if static else _lib.SS_MOVING_BOUNDS, C, L)
+            kind = (mode, C, L)
             if first is None:
                 first = kind
             elif kind != first:
                 raise ValueError("source_pool: candidate %d is (%s, C=%d, L=%d), candidate 0 (%s, C=%d, L=%d): every "
                                  "candidate has one kind, C and L" % ((i,) + _kind(kind) + _kind(first)))
-
-            def chk(t, name, dtype, shape):
-                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
-                    raise ValueError("source_pool: %s of candidate %d must be a CUDA tensor on cuda:%d"
-                                     % (name, i, self.device))
-                if t.dtype != dtype or not t.is_contiguous() or (shape is not None and tuple(t.shape) != shape):
-                    raise ValueError("source_pool: %s of candidate %d must be a contiguous %s tensor%s"
-                                     % (name, i, dtype, "" if shape is None else " of shape %s" % (shape,)))
-
-            chk(s.dry, "dry", torch.float32, None)
-            N = s.dry.numel()
-            items[i] = SsSource(x=s.dry.data_ptr(), N=N, P=P, C=C, L=L, mode=kind[0], rir_bank=rb._h.value)
-            if not static:
-                chk(s.bounds, "bounds", torch.int32, (P,))
+            own = "candidate %d" % i
+            x = _tensor(s.dry, "source_pool", own, "dry", torch.float32, self.device)
+            items[i] = SsSource(x=x, N=s.dry.numel(), P=P, C=C, L=L, mode=mode, rir_bank=rb._h.value)
+            if mode == _lib.SS_MOVING_BOUNDS:
+                items[i].bounds = _tensor(s.bounds, "source_pool", own, "bounds", torch.int32, self.device, (P,))
                 if s.bounds_host is None:
                     raise ValueError("source_pool: moving candidate %d needs bounds_host" % i)
-                bh = np.ascontiguousarray(s.bounds_host, dtype=np.int32)
-                if bh.shape != (P,):
-                    raise ValueError("source_pool: bounds_host of candidate %d must have P = %d entries" % (i, P))
-                keep.append(bh)
-                items[i].bounds, items[i].bounds_host = s.bounds.data_ptr(), bh.ctypes.data
+                bh = _bounds(s.bounds_host, P, "source_pool: bounds_host of %s" % own, keep)
+                items[i].bounds_host = bh.ctypes.data
         h = ctypes.c_void_p()
         _lib.check(self.lib.ss_pool_create(self.ctx, items, n, ctypes.byref(h)))
         if levels is not None:
@@ -411,8 +448,7 @@ class Renderer:
             if st != _lib.SS_OK:
                 self.lib.ss_pool_destroy(h)
                 _lib.check(st)
-        banks = [s.rir if isinstance(s, StaticSource) else s.rirs for s in candidates]
-        taps = {b.direct_taps for b in banks}
+        taps = {_rirs(s)[0].direct_taps for s in candidates}
         return SourcePool(self, h, candidates, first[0], first[1], first[2], min(s.dry.numel() for s in candidates),
                           taps.pop() if len(taps) == 1 else 0, levels)
 
@@ -435,26 +471,8 @@ class Renderer:
         results = []
         for i, s in enumerate(sources):
             x = _as_f32(s.dry).reshape(-1)
-            rb = s.rir if isinstance(s, StaticSource) else s.rirs
-            rb = rb if isinstance(rb, RirBank) else None
-            h = None
-            if isinstance(s, StaticSource):
-                if rb is None:
-                    h = _as_f32(s.rir)
-                    C, L = h.shape
-                else:
-                    C, L = rb.pcl[1:]
-                P, mode, bounds = 1, _lib.SS_STATIC, None
-            else:
-                if rb is None:
-                    h = _as_f32(s.rirs)
-                    P, C, L = h.shape
-                else:
-                    P, C, L = rb.pcl
-                bounds = np.ascontiguousarray(s.bounds, dtype=np.int32)
-                mode = _lib.SS_MOVING_BOUNDS
-                if bounds.shape != (P,):
-                    raise ValueError("bounds must have P entries (cumulative segment bounds with leading 0)")
+            rb, h, P, C, L, mode = _rirs(s, lambda a, *_: _as_f32(a))
+            bounds = _bounds(s.bounds, P, "bounds of source %d" % i, keep) if mode == _lib.SS_MOVING_BOUNDS else None
             N = x.shape[0]
             ws, wl, n_out = _window(s, i, N)
             shape = "(C, N)" if s.window is None else "(C, length) of its window"
@@ -472,7 +490,7 @@ class Renderer:
                                 out_direct=dout.ctypes.data if dout is not None else None,
                                 direct_taps=int(s.direct_taps), win_start=ws, win_len=wl,
                                 rir_bank=_bank_of(self, s, i, P, C, L) if rb is not None else None)
-            keep.append((x, h, bounds, out, dout, rb))
+            keep.append((x, h, out, dout, rb))
             results.append(out)
             if post is not None and lufs_targets[i] is not None:
                 if s.window is not None:
@@ -560,19 +578,11 @@ class Renderer:
         arr = (_lib.SsPlanDraw * len(draws))()
         seen = set()
         for k, d in enumerate(draws):
-            def chk(t, name, dtype, lo, hi):
-                if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != self.device:
-                    raise ValueError("plan_device: %s of draw %d must be a CUDA tensor on cuda:%d" % (name, k, self.device))
-                if t.dtype != dtype or not t.is_contiguous():
-                    raise ValueError("plan_device: %s of draw %d must be a contiguous %s tensor" % (name, k, dtype))
-                if not lo <= t.numel() <= hi:
-                    raise ValueError("plan_device: %s of draw %d must hold %s elements, got %d"
-                                     % (name, k, lo if lo == hi else "%d to %d" % (lo, hi), t.numel()))
-                return t.data_ptr()
-
-            start = chk(d.start, "start", torch.int32, 1, 1)
-            u = chk(d.u, "u", torch.float64, 1, 4096)
-            used = chk(d.used, "used", torch.int32, 1, 1) if d.used is not None else None
+            own = "draw %d" % k
+            start = _tensor(d.start, "plan_device", own, "start", torch.int32, self.device, count=(1, 1))
+            u = _tensor(d.u, "plan_device", own, "u", torch.float64, self.device, count=(1, 4096))
+            used = (_tensor(d.used, "plan_device", own, "used", torch.int32, self.device, count=(1, 1))
+                    if d.used is not None else None)
             if start in seen:
                 raise ValueError("plan_device: draw %d shares its start tensor with another draw" % k)
             seen.add(start)
@@ -636,32 +646,17 @@ class Renderer:
                                      "source %d has %s" % (k, spk[0], (C, Tn), v, tuple(outs[v].shape)))
             mono = bool(m.mono)
             row = (Tn,) if mono else (C, Tn)
-
-            def chk(t, name, shape, numel=None):
-                if not isinstance(t, torch.Tensor) or not t.is_cuda:
-                    raise ValueError("plan_device: %s of mixture %d must be a CUDA tensor" % (name, k))
-                if t.device.index != self.device:
-                    raise ValueError("plan_device: %s of mixture %d is on cuda:%s, the renderer on cuda:%d"
-                                     % (name, k, t.device.index, self.device))
-                if t.dtype != torch.float32:
-                    raise ValueError("plan_device: %s of mixture %d must be torch.float32, got %s" % (name, k, t.dtype))
-                if not t.is_contiguous():
-                    raise ValueError("plan_device: %s of mixture %d must be contiguous" % (name, k))
-                if numel is not None and t.numel() != numel:
-                    raise ValueError("plan_device: %s of mixture %d must hold %d elements, got %d"
-                                     % (name, k, numel, t.numel()))
-                if shape is not None and tuple(t.shape) != tuple(shape):
-                    raise ValueError("plan_device: %s of mixture %d must have shape %s, got %s"
-                                     % (name, k, tuple(shape), tuple(t.shape)))
-                return t.data_ptr()
-
             if S == 1 and m.sirs is not None:
                 raise ValueError("plan_device: mixture %d has one speaker: its sirs must be None" % k)
-            sirs = chk(m.sirs, "sirs", None, S - 1) if S > 1 else None
-            snr = chk(m.snr, "snr", None, 1)
-            mix = chk(m.mix, "mix", row)
-            sp_out = chk(m.speakers_out, "speakers_out", (S,) + row) if m.speakers_out is not None else None
-            rms = chk(m.rms_db, "rms_db", (S,)) if m.rms_db is not None else None
+            own, f32 = "mixture %d" % k, torch.float32
+            sirs = (_tensor(m.sirs, "plan_device", own, "sirs", f32, self.device, count=(S - 1, S - 1))
+                    if S > 1 else None)
+            snr = _tensor(m.snr, "plan_device", own, "snr", f32, self.device, count=(1, 1))
+            mix = _tensor(m.mix, "plan_device", own, "mix", f32, self.device, row)
+            sp_out = (_tensor(m.speakers_out, "plan_device", own, "speakers_out", f32, self.device, (S,) + row)
+                      if m.speakers_out is not None else None)
+            rms = (_tensor(m.rms_db, "plan_device", own, "rms_db", f32, self.device, (S,))
+                   if m.rms_db is not None else None)
             delay = int(m.noise_delay)
             if delay < 0:
                 raise ValueError("plan_device: noise_delay of mixture %d must be >= 0, got %d" % (k, delay))
@@ -684,34 +679,15 @@ class Renderer:
         direct_outs = _check_direct_outs(direct_outs, n)
         items = (SsSource * n)()
         keep = [sources, outs, direct_outs]
-
-        def chk(t, name, i, dtype, shape=None):
-            if not isinstance(t, torch.Tensor) or not t.is_cuda:
-                raise ValueError("plan_device: %s of source %d must be a CUDA tensor" % (name, i))
-            if self.device is not None and t.device.index != self.device:
-                raise ValueError("plan_device: %s of source %d is on cuda:%s, the renderer on cuda:%d"
-                                 % (name, i, t.device.index, self.device))
-            if t.dtype != dtype:
-                raise ValueError("plan_device: %s of source %d must be %s, got %s" % (name, i, dtype, t.dtype))
-            if not t.is_contiguous():
-                raise ValueError("plan_device: %s of source %d must be contiguous" % (name, i))
-            if shape is not None and tuple(t.shape) != tuple(shape):
-                raise ValueError("plan_device: %s of source %d must have shape %s, got %s"
-                                 % (name, i, tuple(shape), tuple(t.shape)))
-
+        f32 = torch.float32
         for i, s in enumerate(sources):
+            own = "source %d" % i
             if isinstance(s, Pooled):
                 pl = s.pool
                 if not isinstance(pl, SourcePool):
                     raise ValueError("plan_device: the pool of source %d must be a SourcePool" % i)
-                if pl.closed:
-                    raise ValueError("plan_device: the SourcePool of source %d is closed" % i)
-                if pl.renderer.ctx.value != self.ctx.value:
-                    raise ValueError("plan_device: the SourcePool of source %d belongs to another renderer's context" % i)
-                chk(s.pick, "pick", i, torch.int32)
-                if s.pick.numel() != 1:
-                    raise ValueError("plan_device: pick of source %d must hold one int32, got %d elements"
-                                     % (i, s.pick.numel()))
+                _check_usable(pl, self, "plan_device: the SourcePool of source %d" % i)
+                pick = _tensor(s.pick, "plan_device", own, "pick", torch.int32, self.device, count=(1, 1))
                 if s.window is None:
                     raise ValueError("plan_device: pooled source %d needs a window (start, length)" % i)
                 ws, wl, n_out, start = _window_dev(s, i, pl.n_min, self.device)
@@ -719,57 +695,35 @@ class Renderer:
                 if taps > 0 and taps != pl.direct_taps:
                     raise ValueError("plan_device: pooled source %d has direct_taps = %d, but not every candidate's bank "
                                      "holds a direct set with these taps" % (i, taps))
-                C, L = pl.C, pl.L
-                chk(outs[i], "out", i, torch.float32, (C, n_out))
-                items[i] = SsSource(out=outs[i].data_ptr(), C=C, L=L, mode=pl.mode, pool=pl._h.value,
-                                    pick_dev=s.pick.data_ptr())
-                rb = None
+                C = pl.C
+                out = _tensor(outs[i], "plan_device", own, "out", f32, self.device, (C, n_out))
+                items[i] = SsSource(out=out, C=C, L=pl.L, mode=pl.mode, pool=pl._h.value, pick_dev=pick)
             else:
-                chk(s.dry, "dry", i, torch.float32)
+                x = _tensor(s.dry, "plan_device", own, "dry", f32, self.device)
                 N = s.dry.numel()
                 ws, wl, n_out, start = _window_dev(s, i, N, self.device)
-                rb = s.rir if isinstance(s, StaticSource) else s.rirs
-                rb = rb if isinstance(rb, RirBank) else None
-            if isinstance(s, StaticSource):
-                if rb is None:
-                    chk(s.rir, "rir", i, torch.float32)
-                    if s.rir.dim() != 2:
-                        raise ValueError("plan_device: rir of static source %d must be (C, L)" % i)
-                    C, L = s.rir.shape
-                else:
-                    C, L = rb.pcl[1:]
-                chk(outs[i], "out", i, torch.float32, (C, n_out))
-                items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rir.data_ptr() if rb is None else None,
-                                    out=outs[i].data_ptr(), N=N, P=1, C=C, L=L, mode=_lib.SS_STATIC)
-                P = 1
-            elif not isinstance(s, Pooled):
-                if rb is None:
-                    chk(s.rirs, "rirs", i, torch.float32)
-                    if s.rirs.dim() != 3:
-                        raise ValueError("plan_device: rirs of moving source %d must be (P, C, L)" % i)
-                    P, C, L = s.rirs.shape
-                else:
-                    P, C, L = rb.pcl
-                chk(outs[i], "out", i, torch.float32, (C, n_out))
-                chk(s.bounds, "bounds", i, torch.int32, (P,))
-                bh = None
-                if s.bounds_host is not None:
-                    bh = np.ascontiguousarray(s.bounds_host, dtype=np.int32)
-                    if bh.shape != (P,):
-                        raise ValueError("plan_device: bounds_host of source %d must have P entries" % i)
-                    keep.append(bh)
-                items[i] = SsSource(x=s.dry.data_ptr(), rir=s.rirs.data_ptr() if rb is None else None,
-                                    out=outs[i].data_ptr(), bounds=s.bounds.data_ptr(), N=N, P=P, C=C, L=L,
-                                    mode=_lib.SS_MOVING_BOUNDS, bounds_host=bh.ctypes.data if bh is not None else None)
-            if rb is not None:
-                items[i].rir_bank = _bank_of(self, s, i, P, C, L)
+
+                def raw(t, field, shape):                  # raw RIRs: checked before _rirs reads their shape
+                    _tensor(t, "plan_device", own, field, f32, self.device, shape)
+                    return t
+                rb, h, P, C, L, mode = _rirs(s, raw)
+                out = _tensor(outs[i], "plan_device", own, "out", f32, self.device, (C, n_out))
+                items[i] = SsSource(x=x, rir=h.data_ptr() if h is not None else None, out=out, N=N, P=P, C=C, L=L,
+                                    mode=mode)
+                if mode == _lib.SS_MOVING_BOUNDS:
+                    items[i].bounds = _tensor(s.bounds, "plan_device", own, "bounds", torch.int32, self.device, (P,))
+                    if s.bounds_host is not None:
+                        items[i].bounds_host = _bounds(s.bounds_host, P, "plan_device: bounds_host of %s" % own,
+                                                       keep).ctypes.data
+                if rb is not None:
+                    items[i].rir_bank = _bank_of(self, s, i, P, C, L)
             items[i].flags = _flags(s, i, direct_outs[i])
             items[i].win_start, items[i].win_len = ws, wl
             if start is not None:
                 items[i].win_start_dev = start.data_ptr()         # kept alive with `sources`
             if direct_outs[i] is not None:
-                chk(direct_outs[i], "direct_out", i, torch.float32, (C, n_out))
-                items[i].out_direct = direct_outs[i].data_ptr()
+                items[i].out_direct = _tensor(direct_outs[i], "plan_device", own, "direct_out", f32, self.device,
+                                              (C, n_out))
                 items[i].direct_taps = int(s.direct_taps)
         return items, n, keep
 
@@ -813,21 +767,15 @@ class Renderer:
 class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
-    mixtures, the plan also assembles them at every run (ss_plan_create_mix); with draws, it first draws their starts
-    (ss_plan_create_ex)."""
+    mixtures, the plan also assembles them at every run; with draws, it first draws their starts (ss_plan_create_ex)."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws = draws
         self._plan = ctypes.c_void_p()
-        if n > 0 and draws:
+        if n > 0:
             _lib.check(renderer.lib.ss_plan_create_ex(renderer.ctx, items, n, mixes, len(mixes) if mixes else 0,
-                                                      draws, len(draws), ctypes.byref(self._plan)))
-        elif n > 0 and mixes:
-            _lib.check(renderer.lib.ss_plan_create_mix(renderer.ctx, items, n, mixes, len(mixes),
-                                                       ctypes.byref(self._plan)))
-        elif n > 0:
-            _lib.check(renderer.lib.ss_plan_create(renderer.ctx, items, n, ctypes.byref(self._plan)))
+                                                      draws, len(draws) if draws else 0, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
@@ -866,11 +814,7 @@ class HostPlan:
 
     def run(self) -> T.List[np.ndarray]:
         """H2D -> render [-> loudness] -> D2H of the whole batch; returns the (C, N) output arrays."""
-        lib, ctx = self.renderer.lib, self.renderer.ctx
-        if self.post is None:
-            _lib.check(lib.ss_render_host(ctx, self.items, self.n))
-        else:
-            _lib.check(lib.ss_render_host_ex(ctx, self.items, self.n, self.post))
+        _lib.check(self.renderer.lib.ss_render_host_ex(self.renderer.ctx, self.items, self.n, self.post))
         return self.results
 
     def loudness(self) -> T.List[T.Tuple[float, float]]:
@@ -939,7 +883,7 @@ def render_mixtures(utterances: T.Sequence[dict], device: T.Optional[int] = None
     import torch
     from ._lib import SsMixItem
     R = default_renderer() if device is None else Renderer(device)
-    dev = torch.device("cuda", R.device if R.device is not None else torch.cuda.current_device())
+    dev = torch.device("cuda", R.device)
     lib = R.lib
     srcs, outs, plan = [], [], []
     for u in utterances:
