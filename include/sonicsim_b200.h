@@ -214,14 +214,17 @@ void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their cont
  * plan is created, for the largest any candidate needs: 3 kernel launches per chunk, as with a moving window.
  * Lifetime: a pool must outlive every plan that uses it; ss_pool_destroy waits for the device before it frees it. */
 int ss_pool_create(ss_ctx* ctx, const ss_source* candidates, int n, ss_pool** out);
-int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact candidate entries (40 B each), and the
+int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact candidate entries (40 B each), the n
+                                               * float gains (4 B each) once ss_pool_loudness measured them, and the
                                                * level tables with their pointer array once ss_pool_levels built them */
 void ss_pool_destroy(ss_pool* pool);          /* destroy pools after the plans that use them, before their context */
 
 /* ---- level tables of a pool (version 107), for the start draws of plans (ss_plan_draw below).  Gives every candidate
  * of the pool a table from which the energy of any crop is two loads:
  *   Q[0] = 0, Q[n + 1] = Q[n] + e[n] for n < N, in float64 (N + 1 doubles), where e[n] is computed from the candidate's
- *   whole reverberant stem as ss_render_dev renders it (the candidate as a whole banked source, bounds_host included):
+ *   whole reverberant stem as ss_render_dev renders it (the candidate as a whole banked source, bounds_host included),
+ *   the normalised stem - that stem times (float)gain, with k_loud_scale's arithmetic - in a pool with gains
+ *   (ss_pool_loudness below):
  *     - flags = SS_MIX_MONO: e[n] = (double)(v * v), v the channel fold of the mixture kernels at n (SS_MIX_MONO of
  *       ss_plan_mix: the float32 sum of the C rows in channel order, then an IEEE division by C), with the same bits;
  *     - flags = 0: e[n] = sum over c of (double)(y[c, n] * y[c, n]), in channel order.
@@ -237,7 +240,7 @@ int ss_pool_levels(ss_pool* pool, uint32_t flags);
 const double* ss_pool_level_table(const ss_pool* pool, int i);
 
 /* library / build identification */
-int ss_version(void);        /* 107: level tables of pools (ss_pool_levels) and start draws in plans (ss_plan_create_ex) */
+int ss_version(void);        /* 108: loudness gains of pools (ss_pool_loudness) */
 const char* ss_strerror(int status);
 int ss_last_cuda_error(void);
 
@@ -431,6 +434,30 @@ typedef struct {
  * with a target must have C <= 8 and the rate of the first source that has one; otherwise the call returns
  * SS_ERR_INVALID before anything is copied. */
 int ss_render_host_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss_post_lufs* post);
+
+/* ---- loudness gains of a pool (version 108): SonicSet's files hold every stem loudness-normalised over the whole stem
+ * (SonicSet.py:97-101, get_lufs_norm_audio: speakers to U(-19, -15) LUFS, the noise to U(-26, -22), the music to
+ * U(-31, -27)), and the dataloader crops those files.  A candidate is fixed when its pool is built, so its whole-stem
+ * loudness is a constant: measured here once, it makes every pooled slot that picks the candidate render the crop of the
+ * normalised stem, with no loudness kernel in any plan run.
+ *   - post: n entries, one per candidate, as for ss_render_host_ex (host gating plan brk / blk_lo / blk_hi, rate,
+ *     block_size, target_lufs, result).  brk == NULL leaves that candidate unmeasured, with gain 1.
+ *   - Every measured candidate is rendered whole, exactly as ss_pool_levels renders it (same groups, same transient
+ *     buffer), and measured by the launches of ss_loudness_dev (k_kweight, k_kw_scan, k_loud_gate, -inf LUFS measured as
+ *     -40): result[0..1] receives the float64 loudness and gain that ss_render_host_ex returns for the candidate rendered
+ *     on its own with that target.
+ *   - The pool keeps (float)gain per candidate in device memory (n floats, in ss_pool_bytes).  A pooled slot that picks
+ *     candidate i stores every sample of its reverberant and of its direct stem as y * (float)gain_i, one float32
+ *     multiply rounded once - the arithmetic of k_loud_scale, and the direct stem takes the reverberant stem's gain, as
+ *     in ss_render_host_ex.  The gain is fused into the render kernels' stores (k_blocks reads it with the pick): a plan
+ *     over pools with gains launches as many kernels per run as the same plan over the same pools without them.
+ *   - ss_pool_levels afterwards builds the tables of the normalised stems (each stem scaled by (float)gain with
+ *     k_loud_scale first), so that start draws test the crops the slots render.
+ * Returns when the gains are in device memory.  Refused before anything is allocated, with the pool unchanged: a NULL
+ * pool or post (SS_ERR_INVALID); C > 8 (SS_ERR_UNSUPPORTED, as ss_loudness_dev); measured candidates whose rates
+ * differ, a gating plan with brk but without blk_lo / blk_hi, n_e <= 0, n_blocks < 0, rate or block_size <= 0; a pool
+ * that already has gains or level tables, or that a plan has been created over (SS_ERR_INVALID). */
+int ss_pool_loudness(ss_pool* pool, const ss_post_lufs* post);   /* n entries, one per candidate */
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

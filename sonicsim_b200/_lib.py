@@ -158,6 +158,7 @@ def load():
         lib.ss_pool_destroy.argtypes = [vp]
         lib.ss_pool_destroy.restype = None
         lib.ss_pool_levels.argtypes = [vp, ctypes.c_uint32]
+        lib.ss_pool_loudness.argtypes = [vp, ctypes.POINTER(SsPostLufs)]
         lib.ss_pool_level_table.argtypes = [vp, ctypes.c_int]
         lib.ss_pool_level_table.restype = vp
         lib.ss_render_host.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int]
@@ -192,7 +193,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

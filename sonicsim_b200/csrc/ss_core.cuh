@@ -92,6 +92,32 @@ SS_HD void red_add(float* p, float v) {
 #endif
 }
 
+// v * g rounded once: the scale k_loud_scale applies to a stored stem (a pooled slot's loudness gain, ss_pool_loudness),
+// never contracted into a neighbouring add.  g = 1 returns v's bits.
+SS_HD float gain_mul(float v, float g) {
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(v, g);
+#else
+    volatile float r = v * g;
+    return r;
+#endif
+}
+// The last addend of a sample under a gain g: *p = (*p + v) * g, where *p holds what this thread stored and red_add-ed
+// there before.  The sum is rounded as red.global.add.f32 rounds it - to nearest even, subnormal inputs and results
+// flushed to sign-preserving zero (add.rn.ftz.f32) - so the result has the bits of red_add(p, v) followed by a scale by
+// g.  The load is relaxed at gpu scope, like the RED, so it observes this thread's earlier RED to the same address.
+SS_HD void red_add_last(float* p, float v, float g) {
+#if defined(__CUDA_ARCH__)
+    float a, s;
+    asm volatile("ld.relaxed.gpu.global.f32 %0, [%1];" : "=f"(a) : "l"(p) : "memory");
+    asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(s) : "f"(a), "f"(v));
+    *p = __fmul_rn(s, g);
+#else
+    volatile float s = *p + v;
+    *p = gain_mul(s, g);
+#endif
+}
+
 // (1 - w) * a + w * b with every product and the sum rounded separately, like NumPy evaluates
 // SonicSim_moving.py:94 (no FMA contraction), so both trajectory forms give identical bits.
 SS_HD float lerp_terms(float fa, float a, float fb, float b) {

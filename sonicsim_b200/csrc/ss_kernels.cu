@@ -112,8 +112,9 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 // full plan; a windowed one's holds the full plan's blocks [g0, g1) (window_span, cut to the table size).  A moving
 // window first reads its start from device memory, clamps it (bit 2 of g_dev_err) and stores it as counts[4], where
 // the window search here and k_prepare's range warps take it; its table is sized for every start (window_table_cap).
-// A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate into its Source in the
-// descriptor block, which is why k_prepare then reads the Source table from global memory (k_prepare<false>).
+// A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate - and its loudness gain,
+// counts[11] - into its Source in the descriptor block (pick_slot), which is why k_prepare then reads the Source table
+// from global memory (k_prepare<false>).
 __global__ void __launch_bounds__(256)
 k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -121,10 +122,9 @@ k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
         Source& S = srcs[si];
         int g0 = 0, g1 = S.nblk_max;
         if (S.h_rows) {
-            const PoolEntry* const pool = pool_table(S);
-            if (pool && lane == 0) {
+            if (pool_table(S) && lane == 0) {
                 bool bad;
-                pick_candidate(S, pool[clamp_pick(*pick_ptr(S), pool_size(S), bad)]);
+                pick_slot(S, *pick_ptr(S), bad);
                 if (bad) atomicOr(&g_dev_err, 8u);
             }
             __syncwarp();
@@ -275,7 +275,7 @@ k_prepare(const Source* __restrict__ srcs_g, const int* __restrict__ prefix_g, i
             // the reference raises IndexError for idx + 1 >= P (checked on the host path); block_positions clamps, leave a mark
             if (lane == 0 && (pmin < 0 || pmax + 1 > S.P - 1)) atomicOr(&g_dev_err, 1u);
         }
-        fill_items(S, items, blk, block_positions(S, bk, pmin, pmax), lane, 32);
+        fill_items(S, items, blk, block_positions(S, bk, pmin, pmax), lane, 32, stem_gain(S));
         return;
     }
     if (local < nh) rows_of_pair_h(S, local, ra, rb);
@@ -506,6 +506,7 @@ __device__ __forceinline__ void load2_ab(int t, const float2* s, Regs32& R) {
 #pragma unroll
     for (int r = 0; r < 16; ++r) R.b[r] = p[544 * r + 272];
 }
+template <bool GAIN>
 __global__ void __launch_bounds__(kThreads, SS_RENDER_MINB)
 k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_ptr, int n_items_host) {
     extern __shared__ __align__(128) float2 smem[];
@@ -591,14 +592,14 @@ k_render_fast(const RItem* __restrict__ items, const int* __restrict__ n_items_p
         fft16_w<true>(R.a, w);                            // pass C
         fft16_w<true>(R.b, w);
         render_phase3_close(t, R, T);
-        render_epilogue_item(t, s_item[k % 3], R);
+        render_epilogue_item<GAIN>(t, s_item[k % 3], R);
     }
 }
 
 // ============================================================================= host side
 thread_local int g_last_cuda = 0;
 
-extern "C" int ss_version(void) { return 107; }
+extern "C" int ss_version(void) { return 108; }
 extern "C" int ss_last_cuda_error(void) { return g_last_cuda; }
 extern "C" const char* ss_strerror(int st) {
     switch (st) {
@@ -644,7 +645,8 @@ static int init_ctx(ss_ctx* c, int device) {
     CK(cudaFuncSetAttribute(k_prepare<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPadF * (int)sizeof(float2)));
     CK(cudaFuncSetAttribute(k_prepare<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPadF * (int)sizeof(float2)));
     CK(cudaFuncSetAttribute(k_render<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
-    CK(cudaFuncSetAttribute(k_render_fast, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
+    CK(cudaFuncSetAttribute(k_render_fast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
+    CK(cudaFuncSetAttribute(k_render_fast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
     CK(cudaFuncSetAttribute(k_render<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRenderSmem));
     for (int i = 0; i < ss_ctx::kRing; ++i) {
         CK(cudaEventCreateWithFlags(&c->desc_ev[i], cudaEventDisableTiming));
@@ -812,6 +814,11 @@ struct ss_pool {
     const double** level_ptr = nullptr;
     std::vector<int64_t> level_off;       // candidate i's table at levels + level_off[i]
     int level_flags = -1;                 // SS_MIX_MONO or 0 once the tables exist
+    // loudness gains (ss_pool_loudness): n floats (float)gain on the device, 1 for an unmeasured candidate, and the
+    // measured (LUFS, gain) pairs on the host
+    float* gains = nullptr;
+    std::vector<double> loud;
+    bool planned = false;                 // a plan has been created over the pool: its gains may no longer change
 };
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
@@ -1076,6 +1083,7 @@ struct ChunkLaunch {
     int n = 0, ps = 0, grid_r = 0, n_known = -1;
     int grid_direct = 0;                  // k_rir_direct CTAs per source (8 rows each), 0: no direct target in the chunk
     bool host_tables = true, any_long = false, all_aligned = true, any_norm = false;
+    bool any_gain = false;                // a pooled slot of a pool with gains: k_render_fast<true>
     const Source* ds = nullptr; const int* dps = nullptr; RItem* d_items = nullptr; int* d_total = nullptr;
     PrepParams pp;
 };
@@ -1096,6 +1104,7 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
 // block table, so that they always travel in the descriptor block
 static size_t counts_bytes(const Shape& sh) { return sh.win ? 64 : 16; }
+static const float kUnitGain = 1.0f;      // counts[11] of every windowed source until a pooled slot picks (stem_gain)
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
 // counts (windowed source, device-built tables)
 static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int first, int last) {
@@ -1126,6 +1135,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
     size_t tab_off = off_tot + 16;
     bool any_long = false, all_aligned = true, any_norm = false, any_pooled = false;
     int grid_direct = 0;
+    L->any_gain = false;
     for (int i = 0; i < n; ++i) {
         const ss_source& it = items[first + i];
         const Shape& sh = shapes[first + i];
@@ -1142,6 +1152,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
             // candidate 0 until k_blocks writes the pick of each run over it
             pick_candidate(s, it.pool->host[0]);
             any_pooled = true;
+            L->any_gain = L->any_gain || it.pool->gains;
         } else if (it.rir_bank) {
             // spectra (and cuts) from the bank: no RIR rows, no cut table, no k_rir_absmax / k_rir_direct work
             set_banked(s, it.rir_bank->spec, (it.flags & SS_DIRECT_TARGET) ? it.rir_bank->cut : nullptr, sh.win != 0);
@@ -1169,6 +1180,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
             if (sh.win) {
                 hb_counts[2] = sh.k0 - sh.g0; hb_counts[3] = sh.k1 - sh.k0;
                 hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
+                memcpy(hb_counts + 11, &kUnitGain, sizeof(kUnitGain));                  // stem_gain
             }
             total_items += (sh.win ? sh.k1 - sh.k0 : nblk) * sh.per;
         } else {
@@ -1180,10 +1192,12 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                 memset(hb_counts, 0, counts_bytes(sh));
                 hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
                 memcpy(hb_counts + 6, &it.win_start_dev, sizeof(it.win_start_dev));      // win_start_ptr
-                if (it.pool) {                                                           // pool_table, pool_size, pick_ptr
+                memcpy(hb_counts + 11, &kUnitGain, sizeof(kUnitGain));                  // stem_gain until k_blocks picks
+                if (it.pool) {                                          // pool_table, pool_size, pick_ptr, pool_gains
                     memcpy(hb_counts + 8, &it.pool->table, sizeof(it.pool->table));
                     hb_counts[10] = it.pool->n;
                     memcpy(hb_counts + 12, &it.pick_dev, sizeof(it.pick_dev));
+                    memcpy(hb_counts + 14, &it.pool->gains, sizeof(it.pool->gains));
                 }
             } else {
                 s.counts = (int*)scratch;
@@ -1249,7 +1263,10 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, b
     if (timed) CK(cudaEventRecord(pf.e1, stream));
     if (L.grid_r > 0) {
         if (L.any_long) k_render<true, false><<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
-        else if (L.all_aligned && !c->no_fast) k_render_fast<<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
+        else if (L.all_aligned && !c->no_fast) {
+            if (L.any_gain) k_render_fast<true><<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
+            else k_render_fast<false><<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
+        }
         else k_render<false, false><<<L.grid_r, kThreads, kRenderSmem, stream>>>(L.d_items, L.d_total, L.n_known);
         CK(cudaGetLastError());
     }
@@ -1375,6 +1392,7 @@ extern "C" void ss_pool_destroy(ss_pool* pl) {
     if (pl->table) cudaFree(pl->table);
     if (pl->levels) cudaFree(pl->levels);
     if (pl->level_ptr) cudaFree(pl->level_ptr);
+    if (pl->gains) cudaFree(pl->gains);
     if (pl->ready) cudaEventDestroy(pl->ready);
     delete pl;
 }
@@ -1382,6 +1400,7 @@ extern "C" int64_t ss_pool_bytes(const ss_pool* pl) {
     if (!pl) return 0;
     int64_t b = (int64_t)sizeof(PoolEntry) * pl->n;
     if (pl->levels) b += (int64_t)sizeof(double) * pl->level_off[pl->n] + (int64_t)sizeof(double*) * pl->n;
+    if (pl->gains) b += (int64_t)sizeof(float) * pl->n;
     return b;
 }
 extern "C" const double* ss_pool_level_table(const ss_pool* pl, int i) {
@@ -1620,74 +1639,234 @@ extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, voi
     });
 }
 
-// ----------------------------------------------------------------------------- level tables of a pool
-// Candidates are rendered whole by ss_render_dev into one transient buffer, in groups of consecutive candidates whose
-// stems fit kLevelStemBytes (a larger candidate is a group of its own), and k_levels turns each group into its tables.
+// ----------------------------------------------------------------------------- whole stems of a pool's candidates
+// ss_pool_loudness and ss_pool_levels read every candidate's whole reverberant stem as ss_render_dev renders it (the
+// candidate as a whole banked source, bounds_host included).  The candidates are rendered in groups of consecutive
+// candidates whose stems fit kLevelStemBytes (a larger candidate is a group of its own) into one transient buffer.
 constexpr size_t kLevelStemBytes = 256ull << 20;
 
-static int levels_build(ss_pool* pl, bool mono, cudaStream_t s, float** tmp, LevelItem** d_items) {
-    ss_ctx* c = pl->c;
+struct StemGroups {
+    size_t cap = kLevelStemBytes;         // bytes of the transient buffer
+    std::vector<int> first;               // group g holds candidates [first[g], first[g + 1])
+    std::vector<size_t> at;               // candidate i's (C, N) stem at byte at[i] of the buffer
+};
+static StemGroups stem_groups(const ss_pool* pl) {
+    StemGroups G;
     const int n = pl->n;
-    pl->level_off.assign(n + 1, 0);
-    size_t cap = kLevelStemBytes;
-    for (int i = 0; i < n; ++i) {
-        pl->level_off[i + 1] = pl->level_off[i] + pl->host[i].N + 1;
-        cap = std::max(cap, align_up(4 * (size_t)pl->C * pl->host[i].N, 256));
-    }
-    CK(cudaMalloc((void**)&pl->levels, sizeof(double) * (size_t)pl->level_off[n]));
-    CK(cudaMalloc((void**)&pl->level_ptr, sizeof(double*) * (size_t)n));
-    std::vector<const double*> ptr(n);
-    for (int i = 0; i < n; ++i) ptr[i] = pl->levels + pl->level_off[i];
-    CK(cudaMemcpy(pl->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
-    // groups [first[g], first[g + 1]) and every candidate's stem in the transient buffer
-    std::vector<int> first(1, 0);
-    std::vector<size_t> at(n);
+    for (int i = 0; i < n; ++i) G.cap = std::max(G.cap, align_up(4 * (size_t)pl->C * pl->host[i].N, 256));
+    G.first.assign(1, 0);
+    G.at.resize(n);
     size_t used = 0;
     for (int i = 0; i < n; ++i) {
         const size_t b = align_up(4 * (size_t)pl->C * pl->host[i].N, 256);
-        if (used > 0 && used + b > cap) { first.push_back(i); used = 0; }
-        at[i] = used;
+        if (used > 0 && used + b > G.cap) { G.first.push_back(i); used = 0; }
+        G.at[i] = used;
         used += b;
     }
-    first.push_back(n);
-    CK(cudaMalloc((void**)tmp, cap));
-    std::vector<LevelItem> li(n);
-    for (int i = 0; i < n; ++i)
-        li[i] = {(const float*)((char*)*tmp + at[i]), pl->levels + pl->level_off[i], pl->host[i].N, pl->C, 0};
-    CK(cudaMalloc((void**)d_items, sizeof(LevelItem) * (size_t)n));
-    CK(cudaMemcpy(*d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
+    G.first.push_back(n);
+    return G;
+}
+// Render every group into `tmp` on `s` (after the pool's banks are complete), and after each group's render enqueue
+// group(first, last) on `s`, whatever reads those stems before the next group overwrites them.  Returns when `s` is idle.
+template <class Group>
+static int render_stem_groups(ss_pool* pl, const StemGroups& G, char* tmp, cudaStream_t s, Group group) {
     CK(cudaStreamWaitEvent(s, pl->ready, 0));           // banks may still be building
     std::vector<ss_source> items;
-    for (size_t g = 0; g + 1 < first.size(); ++g) {
+    for (size_t g = 0; g + 1 < G.first.size(); ++g) {
         items.clear();
-        for (int i = first[g]; i < first[g + 1]; ++i) {
+        for (int i = G.first[g]; i < G.first[g + 1]; ++i) {
             const PoolEntry& e = pl->host[i];
             ss_source it; memset(&it, 0, sizeof(it));
-            it.x = e.x; it.out = (float*)li[i].y; it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->L; it.mode = pl->mode;
-            it.rir_bank = pl->banks[i];
+            it.x = e.x; it.out = (float*)(tmp + G.at[i]); it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->L;
+            it.mode = pl->mode; it.rir_bank = pl->banks[i];
             if (pl->mode == SS_MOVING_BOUNDS) { it.bounds = e.bounds; it.bounds_host = pl->bounds_host.data() + pl->bounds_off[i]; }
             items.push_back(it);
         }
-        int st = ss_render_dev(c, items.data(), (int)items.size(), (void*)s);     // the next group waits on `s` for
-        if (st == SS_OK) st = levels_enqueue(c, *d_items + first[g], first[g + 1] - first[g], mono, s);   // k_levels
+        int st = ss_render_dev(pl->c, items.data(), (int)items.size(), (void*)s);   // the next group waits on `s`
+        if (st == SS_OK) st = group(G.first[g], G.first[g + 1]);
         if (st) return st;
     }
     CK(cudaStreamSynchronize(s));
     return SS_OK;
 }
+// One transient stream per build call, synchronised and destroyed on every return path
+struct BuildStream {
+    cudaStream_t s = nullptr;
+    ~BuildStream() { if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
+};
+
+// ----------------------------------------------------------------------------- loudness gains of a pool
+extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items, void* stream);
+
+// Device memory of one ss_pool_loudness call: the gating tables of the measured candidates (one copy per distinct set of
+// host arrays), their results, and one group's scratch
+static int loudness_build(ss_pool* pl, const ss_post_lufs* post, cudaStream_t s, std::vector<void*>& owned,
+                          std::vector<double>& res) {
+    const int n = pl->n;
+    struct Tab { const int32_t *brk, *lo, *hi; int n_e, n_blocks; size_t o_brk, o_lo, o_hi; };   // o_*: in d_tab
+    std::vector<Tab> tabs;
+    std::vector<int> tab_of(n, -1);
+    std::vector<char> host;
+    for (int i = 0; i < n; ++i) {
+        const ss_post_lufs& q = post[i];
+        if (!q.brk) continue;
+        int t = -1;
+        for (size_t k = 0; k < tabs.size(); ++k)
+            if (tabs[k].brk == q.brk && tabs[k].lo == q.blk_lo && tabs[k].hi == q.blk_hi && tabs[k].n_e == q.n_e &&
+                tabs[k].n_blocks == q.n_blocks) { t = (int)k; break; }
+        if (t < 0) {
+            const size_t off = host.size(), nb = 4 * (size_t)q.n_blocks;
+            const size_t o_lo = off + align_up(4 * (size_t)(q.n_e + 1), 256), o_hi = o_lo + align_up(nb + 4, 256);
+            host.resize(o_hi + align_up(nb + 4, 256));
+            memcpy(host.data() + off, q.brk, 4 * (size_t)(q.n_e + 1));
+            if (nb) { memcpy(host.data() + o_lo, q.blk_lo, nb); memcpy(host.data() + o_hi, q.blk_hi, nb); }
+            tabs.push_back(Tab{q.brk, q.blk_lo, q.blk_hi, q.n_e, q.n_blocks, off, o_lo, o_hi});
+            t = (int)tabs.size() - 1;
+        }
+        tab_of[i] = t;
+    }
+    const StemGroups G = stem_groups(pl);
+    size_t scratch = 0;                                 // the largest group's loudness scratch
+    for (size_t g = 0; g + 1 < G.first.size(); ++g) {
+        size_t b = 0;
+        for (int i = G.first[g]; i < G.first[g + 1]; ++i)
+            if (post[i].brk) b += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * pl->C * post[i].n_e, 256);
+        scratch = std::max(scratch, b);
+    }
+    char *d_tab = nullptr, *d_scr = nullptr, *tmp = nullptr;
+    double* d_res = nullptr;
+    CK(cudaMalloc((void**)&d_tab, std::max(host.size(), (size_t)256))); owned.push_back(d_tab);
+    CK(cudaMalloc((void**)&d_res, 2 * sizeof(double) * (size_t)n)); owned.push_back(d_res);
+    CK(cudaMalloc((void**)&d_scr, std::max(scratch, (size_t)256))); owned.push_back(d_scr);
+    CK(cudaMalloc((void**)&tmp, G.cap)); owned.push_back(tmp);
+    if (!host.empty()) CK(cudaMemcpy(d_tab, host.data(), host.size(), cudaMemcpyHostToDevice));
+    std::vector<ss_loud_item> li;
+    const int st = render_stem_groups(pl, G, tmp, s, [&](int first, int last) -> int {
+        // every measured candidate of the group: the launches of ss_loudness_dev on its (C, N) stem, measure only
+        li.clear();
+        char* scr = d_scr;
+        for (int i = first; i < last; ++i) {
+            if (!post[i].brk) continue;
+            const ss_post_lufs& q = post[i];
+            const Tab& tb = tabs[tab_of[i]];
+            ss_loud_item it; memset(&it, 0, sizeof(it));
+            it.data = (const float*)(tmp + G.at[i]);
+            it.brk = (const int32_t*)(d_tab + tb.o_brk);
+            it.blk_lo = (const int32_t*)(d_tab + tb.o_lo); it.blk_hi = (const int32_t*)(d_tab + tb.o_hi);
+            it.scratch = (double*)scr; scr += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * pl->C * q.n_e, 256);
+            it.result = d_res + 2 * (size_t)i;
+            it.stride_n = 1; it.stride_c = pl->host[i].N; it.N = pl->host[i].N; it.C = pl->C;
+            it.n_e = q.n_e; it.n_blocks = q.n_blocks;
+            it.rate = q.rate; it.block_size = q.block_size; it.target_lufs = q.target_lufs;
+            li.push_back(it);
+        }
+        for (size_t k = 0; k < li.size(); k += 65535) {   // ss_loudness_dev's item limit
+            const int st2 = ss_loudness_dev(pl->c, li.data() + k, (int)std::min(li.size() - k, (size_t)65535), (void*)s);
+            if (st2) return st2;
+        }
+        return SS_OK;
+    });
+    if (st) return st;
+    res.resize(2 * (size_t)n);
+    CK(cudaMemcpy(res.data(), d_res, 2 * sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
+    return SS_OK;
+}
+
+extern "C" int ss_pool_loudness(ss_pool* pl, const ss_post_lufs* post) {
+    if (!pl || !post) return SS_ERR_INVALID;
+    if (pl->C > 8) return SS_ERR_UNSUPPORTED;           // as ss_loudness_dev
+    if (pl->gains || pl->levels || pl->planned) return SS_ERR_INVALID;
+    const ss_post_lufs* first = nullptr;
+    for (int i = 0; i < pl->n; ++i) {
+        const ss_post_lufs& q = post[i];
+        if (!q.brk) continue;
+        if (!q.blk_lo || !q.blk_hi || q.n_e <= 0 || q.n_blocks < 0 || !(q.rate > 0) || !(q.block_size > 0))
+            return SS_ERR_INVALID;
+        if (!first) first = &q;
+        else if (q.rate != first->rate) return SS_ERR_INVALID;
+    }
+    CK(cudaSetDevice(pl->c->device));
+    std::vector<void*> owned;
+    std::vector<double> res;
+    int st;
+    {
+        BuildStream bs;
+        CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
+        st = loudness_build(pl, post, bs.s, owned, res);
+    }
+    for (void* q : owned) cudaFree(q);
+    if (st != SS_OK) return st;                         // no gains: the pool is as it was
+    const int n = pl->n;
+    std::vector<float> g(n, 1.0f);
+    std::vector<double> loud(2 * (size_t)n, NAN);
+    for (int i = 0; i < n; ++i) {
+        if (!post[i].brk) continue;
+        loud[2 * i] = res[2 * i]; loud[2 * i + 1] = res[2 * i + 1];
+        g[i] = (float)res[2 * i + 1];                   // what k_loud_scale multiplies by
+    }
+    float* d_g = nullptr;
+    CK(cudaMalloc((void**)&d_g, sizeof(float) * (size_t)n));
+    const cudaError_t e = cudaMemcpy(d_g, g.data(), sizeof(float) * (size_t)n, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { cudaFree(d_g); g_last_cuda = (int)e; return SS_ERR_CUDA; }
+    pl->gains = d_g;
+    pl->loud.swap(loud);
+    for (int i = 0; i < n; ++i)
+        if (post[i].brk && post[i].result) { post[i].result[0] = res[2 * i]; post[i].result[1] = res[2 * i + 1]; }
+    return SS_OK;
+}
+
+// ----------------------------------------------------------------------------- level tables of a pool
+// k_levels turns each group of whole stems into its tables; a pool with gains first scales each stem by its candidate's
+// (float)gain with k_loud_scale itself, so that the tables describe the normalised stems its slots render.
+static int levels_build(ss_pool* pl, bool mono, cudaStream_t s, std::vector<void*>& owned) {
+    const int n = pl->n;
+    pl->level_off.assign(n + 1, 0);
+    for (int i = 0; i < n; ++i) pl->level_off[i + 1] = pl->level_off[i] + pl->host[i].N + 1;
+    CK(cudaMalloc((void**)&pl->levels, sizeof(double) * (size_t)pl->level_off[n]));
+    CK(cudaMalloc((void**)&pl->level_ptr, sizeof(double*) * (size_t)n));
+    std::vector<const double*> ptr(n);
+    for (int i = 0; i < n; ++i) ptr[i] = pl->levels + pl->level_off[i];
+    CK(cudaMemcpy(pl->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
+    const StemGroups G = stem_groups(pl);
+    char* tmp = nullptr;
+    LevelItem* d_items = nullptr;
+    double* d_res = nullptr;                            // the (LUFS, gain) pairs k_loud_scale reads its gain from
+    CK(cudaMalloc((void**)&tmp, G.cap)); owned.push_back(tmp);
+    std::vector<LevelItem> li(n);
+    for (int i = 0; i < n; ++i) li[i] = {(const float*)(tmp + G.at[i]), pl->levels + pl->level_off[i], pl->host[i].N, pl->C, 0};
+    CK(cudaMalloc((void**)&d_items, sizeof(LevelItem) * (size_t)n)); owned.push_back(d_items);
+    CK(cudaMemcpy(d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
+    if (pl->gains) {
+        std::vector<double> r(pl->loud);
+        for (int i = 0; i < n; ++i) if (isnan(r[2 * i + 1])) r[2 * i + 1] = 1.0;      // unmeasured: gain 1
+        CK(cudaMalloc((void**)&d_res, sizeof(double) * r.size())); owned.push_back(d_res);
+        CK(cudaMemcpy(d_res, r.data(), sizeof(double) * r.size(), cudaMemcpyHostToDevice));
+    }
+    std::vector<ScaleItem> sc;
+    return render_stem_groups(pl, G, tmp, s, [&](int first, int last) -> int {
+        if (d_res) {
+            sc.clear();
+            for (int i = first; i < last; ++i) sc.push_back(ScaleItem{(float*)li[i].y, d_res + 2 * (size_t)i, pl->host[i].N, pl->C});
+            for (size_t k = 0; k < sc.size(); k += 65535) {   // one gridDim.y row per stem
+                const int st = loud_scale_dev(pl->c, sc.data() + k, (int)std::min(sc.size() - k, (size_t)65535), s);
+                if (st) return st;
+            }
+        }
+        return levels_enqueue(pl->c, d_items + first, last - first, mono, s);
+    });
+}
 
 extern "C" int ss_pool_levels(ss_pool* pl, uint32_t flags) {
     if (!pl || (flags & ~SS_MIX_MONO) || pl->level_flags >= 0 || pl->levels) return SS_ERR_INVALID;
     CK(cudaSetDevice(pl->c->device));
-    cudaStream_t s = nullptr;
-    CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    float* tmp = nullptr;
-    LevelItem* d_items = nullptr;
-    int st = levels_build(pl, (flags & SS_MIX_MONO) != 0, s, &tmp, &d_items);
-    if (st != SS_OK) cudaStreamSynchronize(s);
-    if (tmp) cudaFree(tmp);
-    if (d_items) cudaFree(d_items);
-    cudaStreamDestroy(s);
+    std::vector<void*> owned;
+    int st;
+    {
+        BuildStream bs;
+        CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
+        st = levels_build(pl, (flags & SS_MIX_MONO) != 0, bs.s, owned);
+    }
+    for (void* q : owned) cudaFree(q);
     if (st != SS_OK) {                                  // no tables: the pool is as it was
         if (pl->levels) cudaFree(pl->levels);
         if (pl->level_ptr) cudaFree(pl->level_ptr);
@@ -2022,6 +2201,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     }
     const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
+    for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
     return SS_OK;
 }

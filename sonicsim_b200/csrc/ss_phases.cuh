@@ -92,7 +92,7 @@ struct RItem {
     double step;           // ... and 1 / (samples in that segment), so that k_render_fast's output stage loads no table
     int n_lo;              // samples [n_lo, n_end) are stored (n_lo > n0: a window starts inside the block); the
                            // epilogues tie register r to sample n0 + t + 256 r, so n0 stays the block start
-    int pad_;
+    float gain;            // every stored sample is scaled by it (gain_mul): a pooled slot's loudness gain, else 1
 };
 static_assert(sizeof(RItem) == 112, "RItem is copied as 7 x 16 B");
 
@@ -113,8 +113,10 @@ struct XDesc {
     int mode;
     int kparts;
     int n_lo;              // as RItem::n_lo
+    float gain;            // as RItem::gain
+    int pad_;
 };
-static_assert(sizeof(XDesc) == 112, "XDesc layout");
+static_assert(sizeof(XDesc) == 120, "XDesc layout");
 
 // RIR rows are transformed two per complex FFT, and the bits of a half spectrum depend on its partner row: the direct
 // rows are paired among themselves exactly as a separate source's rows would be, never with a reverberant row.
@@ -261,6 +263,20 @@ SS_HD void pick_candidate(Source& s, const PoolEntry& e) {
     s.x = e.x; s.bounds = e.bounds; s.N = e.N; s.P = e.P; s.nb = (e.N + kB - 1) / kB;
     set_banked(s, e.spec, s.out_direct ? e.cut : nullptr, true);
 }
+// Loudness gains (ss_pool_loudness): a windowed source's counts[11] holds the float bits of the gain its stems are
+// stored with - 1 (written by the host) unless a pooled slot picked a candidate of a pool with gains - and a pooled slot's
+// [14..15] the device pointer of its pool's n float gains, or null
+SS_HD const float* pool_gains(const Source& s) { return *reinterpret_cast<const float* const*>(s.counts + 14); }
+SS_HD float stem_gain(const Source& s) { return s.h_rows ? *reinterpret_cast<const float*>(s.counts + 11) : 1.0f; }
+SS_HD void set_stem_gain(Source& s, float g) { *reinterpret_cast<float*>(s.counts + 11) = g; }
+// The head of k_blocks for a pooled slot: the pick v read from device memory, clamped into [0, n) (bad = it was not
+// there), the picked candidate written into the slot's Source and its gain into counts[11] (1 for a pool without gains)
+SS_HD void pick_slot(Source& s, int v, bool& bad) {
+    const int i = clamp_pick(v, pool_size(s), bad);
+    pick_candidate(s, pool_table(s)[i]);
+    const float* const g = pool_gains(s);
+    set_stem_gain(s, g ? g[i] : 1.0f);
+}
 // Table size of a pooled slot with windows of win_len: the largest window_table_cap over the candidates' full plans under
 // the pool's blocking (bounds[i]: candidate i's host bounds, null for a static pool), so that the table holds the blocks
 // of every candidate at every start.  `full` holds table_cap(aligned, nb, P) blocks of the largest candidate.
@@ -320,8 +336,9 @@ SS_HD Block block_positions(const Source& S, Block bk, int pmin, int pmax) {
 // fill the work items of block `blk` once its position range is known (lanes split the channels).  A direct-target
 // source's block has the reverberant items first, then as many direct items (direct spectra, `out_direct`): all of
 // them carry the block's X, so k_render_fast stages it once for both stems.  Windowed source: only blocks that meet
-// the window have items; output rows have stride win_len and sample n of the stem lands at row[n - win_start].
-SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, int lane, int nlanes) {
+// the window have items; output rows have stride win_len and sample n of the stem lands at row[n - win_start].  Every
+// item carries `gain` (k_prepare passes stem_gain), direct items too: a direct stem takes its reverberant stem's gain.
+SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, int lane, int nlanes, float gain = 1.0f) {
     RItem it;
     it.X = s.xspec + (size_t)blk * kSpec;
     it.bounds = s.bounds; it.rstep = s.rstep; it.idx = s.idx; it.w = s.w;
@@ -335,7 +352,7 @@ SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, i
     it.mode = s.mode;
     const int reach = bk.start / kB + 1;
     it.kparts = reach < s.K ? reach : s.K;
-    it.b0 = 0; it.step = 0.0; it.pad_ = 0;
+    it.b0 = 0; it.step = 0.0; it.gain = gain;
     if (s.aligned) { it.b0 = s.bounds[bk.p_lo]; it.step = s.rstep[bk.p_lo]; }
     const int per = items_per_set(s);
     RItem* dst = items + s.counts[1] + (size_t)(blk - win_first(s)) * items_per_block(s);
@@ -385,6 +402,7 @@ SS_HD XDesc make_xdesc(const RItem& it, int p) {
     d.valid = 1;
     d.mode = it.mode;
     d.kparts = it.kparts;
+    d.gain = it.gain; d.pad_ = 0;
     return d;
 }
 
@@ -759,7 +777,9 @@ SS_HD void hat_pair(int sg, float w, int p, float& fa, float& fb) {
 // Output stage of one thread: samples n = n0 + t + 256 r, r = 0..15, visited in order.  `first` = first
 // transform of its block (plain store); the second transform of a block that straddles a waypoint
 // (grid blocking only) accumulates with a fire-and-forget RED - two addends per address, the first
-// stored by this very thread, so the sum is order-free.
+// stored by this very thread, so the sum is order-free.  Every stored sample is v * gain (gain_mul).  Under a gain
+// other than 1 a straddling block's first transform stores v unscaled and the last one (p + 2 > p_hi) replaces its RED
+// by red_add_last, which scales the finished sum: the bits of accumulating first and scaling after (k_loud_scale).
 template <bool FAST = false>
 SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
     // `d` lives in shared memory: copy what the loop needs into registers once - after every global
@@ -770,6 +790,7 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
     const unsigned span = (unsigned)(n_end - n_lo);
     float* const row = d.row;
     const bool first = d.first != 0;
+    const float g = d.gain;
     if (nbase >= n_end) return;
     if (!FAST && mode == MODE_STATIC) {                      // Re -> channel c, Im -> channel c + 1
         float* const row1 = d.row1;
@@ -778,8 +799,8 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
             const int n = nbase + 256 * r;
             if ((unsigned)(n - n_lo) < span) {
                 const float2 z = R.a[out16(r)];
-                row[n] = z.x;
-                if (row1) row1[n] = z.y;
+                row[n] = gain_mul(z.x, g);
+                if (row1) row1[n] = gain_mul(z.y, g);
             }
         }
     } else if (FAST || (mode == MODE_MOVING_BOUNDS && d.p_lo + 1 == d.p_hi)) {
@@ -796,10 +817,11 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
         for (int r = 0; r < 16; ++r) {
             const int n = nbase + 256 * r;
             const float2 z = R.a[out16(r)];
-            const float v = lerp_terms(one_minus(w[r]), z.x, w[r], z.y);
+            const float v = gain_mul(lerp_terms(one_minus(w[r]), z.x, w[r], z.y), g);
             if ((unsigned)(n - n_lo) < span) row[n] = v;
         }
     } else if (mode == MODE_MOVING_BOUNDS) {
+        const bool last = p + 2 > d.p_hi, fuse = last && g != 1.0f;
         const int* const bounds = d.bounds;
         const double* const rstep = d.rstep;
         int sg = d.p_lo;
@@ -820,10 +842,13 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
                 hat_pair(sg, w, p, fa, fb);
                 const float2 z = R.a[out16(r)];
                 const float v = lerp_terms(fa, z.x, fb, z.y);
-                if (first) row[n] = v; else red_add(row + n, v);
+                if (first) row[n] = last ? gain_mul(v, g) : v;
+                else if (fuse) red_add_last(row + n, v, g);
+                else red_add(row + n, v);
             }
         }
     } else {
+        const bool last = p + 2 > d.p_hi, fuse = last && g != 1.0f;
         const int* const idx = d.idx;
         const float* const wv = d.w;
 #pragma unroll
@@ -834,7 +859,9 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
                 hat_pair(idx[n], wv[n], p, fa, fb);
                 const float2 z = R.a[out16(r)];
                 const float v = lerp_terms(fa, z.x, fb, z.y);
-                if (first) row[n] = v; else red_add(row + n, v);
+                if (first) row[n] = last ? gain_mul(v, g) : v;
+                else if (fuse) red_add_last(row + n, v, g);
+                else red_add(row + n, v);
             }
         }
     }
@@ -842,11 +869,15 @@ SS_HD void render_epilogue(int t, const XDesc& d, const Regs32& R) {
 
 // Output stage of k_render_fast (aligned blocking: the block lies in segment p_lo, one transform per item): as the
 // single-segment branch above, with the segment's first sample and 1 / length taken from the work item itself.
+// GAIN = false (chunks without a pooled slot of a pool with gains, where every item's gain is 1) stores without the
+// multiply, which costs the issue-bound kernel about 2 %.
+template <bool GAIN = true>
 SS_HD void render_epilogue_item(int t, const RItem& it, const Regs32& R) {
     const int nbase = it.n0 + t, n_end = it.n_end;
     const int n_lo = it.n_lo;                                // stored: [n_lo, n_end), as in render_epilogue
     const unsigned span = (unsigned)(n_end - n_lo);
     float* const row = it.row;
+    const float g = it.gain;
     if (nbase >= n_end) return;
     if (it.mode == MODE_STATIC) {                            // Re -> channel c, Im -> channel c + 1 (item-uniform branch)
         float* const row1 = it.row1;
@@ -855,8 +886,8 @@ SS_HD void render_epilogue_item(int t, const RItem& it, const Regs32& R) {
             const int n = nbase + 256 * r;
             if ((unsigned)(n - n_lo) < span) {
                 const float2 z = R.a[out16(r)];
-                row[n] = z.x;
-                if (row1) row1[n] = z.y;
+                row[n] = GAIN ? gain_mul(z.x, g) : z.x;
+                if (row1) row1[n] = GAIN ? gain_mul(z.y, g) : z.y;
             }
         }
         return;
@@ -869,7 +900,7 @@ SS_HD void render_epilogue_item(int t, const RItem& it, const Regs32& R) {
 #pragma unroll
     for (int r = 0; r < 16; ++r) {
         const int n = nbase + 256 * r;
-        const float v = lerp_pair(w[r], R.a[out16(r)]);
+        const float v = GAIN ? gain_mul(lerp_pair(w[r], R.a[out16(r)]), g) : lerp_pair(w[r], R.a[out16(r)]);
         if ((unsigned)(n - n_lo) < span) row[n] = v;
     }
 }

@@ -6,6 +6,7 @@ has no such symbols.  They render many (utterance, source) units with one C-ABI 
 (SonicSet.py:77-94).  Host arrays in / out by default; `Renderer.render_device` takes CUDA tensors.
 """
 import ctypes
+import math
 import typing as T
 import weakref
 
@@ -245,15 +246,23 @@ class SourcePool(_Held):
     `n_min` is the shortest candidate's N (the longest window a slot may take); `direct_taps` > 0 when every candidate's
     bank holds a direct set with these taps.  The pool holds its candidates' banks and keeps their tensors alive; plans
     hold the pool, which is freed once it is closed (or collected) and no live plan uses it any more.  `levels` is None,
-    "mono" or "channels": the level tables the pool holds for start draws (CropDraw), included in `nbytes`."""
+    "mono" or "channels": the level tables the pool holds for start draws (CropDraw), included in `nbytes`.
+    `loudness` is an (n, 2) float64 array of every candidate's measured integrated loudness (LUFS) and linear gain
+    (ss_pool_loudness), NaN for a candidate without a target; `nbytes` includes the gains (4 bytes per candidate)."""
 
-    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None):
+    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None, loudness=None):
         self.renderer, self._h = renderer, handle
         self.candidates = list(candidates)
         self.n, self.mode, self.C, self.L = len(self.candidates), mode, C, L
         self.n_min, self.direct_taps, self.levels = n_min, direct_taps, levels
+        self._loudness = loudness if loudness is not None else np.full((self.n, 2), np.nan)
         self.nbytes = int(renderer.lib.ss_pool_bytes(handle))
         self._banks = _hold_banks(self, self.candidates)
+
+    @property
+    def loudness(self) -> np.ndarray:
+        """(n, 2) float64: measured LUFS and linear gain of every candidate (ss_pool_loudness), NaN when unmeasured."""
+        return self._loudness.copy()
 
     def level_table(self, i):
         """A float64 CUDA copy of candidate i's level table (N + 1 values: Q[0] = 0, Q[n + 1] = Q[n] + e[n]), see
@@ -395,7 +404,8 @@ class Renderer:
 
     # ------------------------------------------------------------------ source pools
     def source_pool(self, candidates: T.Sequence[T.Union[MovingSource, StaticSource]],
-                    levels: T.Optional[str] = None) -> SourcePool:
+                    levels: T.Optional[str] = None,
+                    lufs_targets: T.Optional[T.Sequence[T.Optional[float]]] = None, sr: float = 16000) -> SourcePool:
         """Validate and upload a set of candidate sources once, for pooled slots (render.Pooled) of device plans to pick
         from at every run.  Every candidate is a MovingSource or StaticSource whose RIRs are a RirBank of this renderer
         (`dry`, `bounds`: contiguous CUDA tensors of its device; a moving candidate needs `bounds_host`), with no window,
@@ -405,13 +415,28 @@ class Renderer:
         `levels` = "mono" or "channels" also builds every candidate's level table (ss_pool_levels: the float64 prefix
         sums of the squares of its whole rendered stem, channel-folded like Mixture(mono=True) for "mono"), which
         CropDraw reads to test crops for silence; 8 bytes per sample.  The call then returns when the tables are
-        complete.  They describe the dry signals as they are now: new signals need a new pool."""
+        complete.  They describe the dry signals as they are now: new signals need a new pool.
+
+        `lufs_targets` (one float per candidate, or None to leave that candidate unscaled) loudness-normalises every
+        candidate's whole stem as SonicSet stored it (get_lufs_norm_audio, SonicSet.py:97-101; `sr` the sample rate):
+        each candidate is rendered whole once, measured like render_host(..., lufs_targets=) measures it, and every
+        pooled slot that picks it stores its crops, direct stem included, times that (float32) gain.  The level tables
+        then describe the normalised stems.  `loudness` holds the measured (LUFS, gain) pairs."""
         import torch
+        from .SonicSim_audio import gating_plan
         if levels not in LEVELS:
             raise ValueError("source_pool: levels must be None, 'mono' or 'channels', got %r" % (levels,))
         n = len(candidates)
         if not 1 <= n <= 1 << 24:
             raise ValueError("source_pool: a pool holds 1 to 2^24 candidates, got %d" % n)
+        if lufs_targets is not None:
+            if len(lufs_targets) != n:
+                raise ValueError("source_pool: %d candidates but %d entries in lufs_targets" % (n, len(lufs_targets)))
+            for i, t in enumerate(lufs_targets):
+                if t is not None and not math.isfinite(float(t)):
+                    raise ValueError("source_pool: the loudness target of candidate %d is not finite: %r" % (i, t))
+            if not float(sr) > 0:
+                raise ValueError("source_pool: sr must be > 0, got %r" % (sr,))
         items = (SsSource * n)()
         keep = []
         first = None
@@ -441,16 +466,37 @@ class Renderer:
                     raise ValueError("source_pool: moving candidate %d needs bounds_host" % i)
                 bh = _bounds(s.bounds_host, P, "source_pool: bounds_host of %s" % own, keep)
                 items[i].bounds_host = bh.ctypes.data
+        loud, post = None, None
+        if lufs_targets is not None:
+            if first[1] > 8:
+                raise ValueError("source_pool: loudness normalisation supports at most 8 channels, the candidates have %d"
+                                 % first[1])
+            loud = np.full((n, 2), np.nan, dtype=np.float64)
+            post = (SsPostLufs * n)()
+            plans = {}                                   # one gating plan per length
+            for i, t in enumerate(lufs_targets):
+                if t is None:
+                    continue
+                N = int(items[i].N)
+                block = 0.4 if N / sr >= 0.4 else N / sr                      # SonicSim_audio.py:69, as plan_host
+                if N not in plans:
+                    plans[N] = gating_plan(N, float(sr), float(block))
+                brk, blo, bhi = plans[N]
+                post[i] = SsPostLufs(brk=brk.ctypes.data, blk_lo=blo.ctypes.data, blk_hi=bhi.ctypes.data,
+                                     n_e=len(brk) - 1, n_blocks=len(blo), rate=float(sr), block_size=float(block),
+                                     target_lufs=float(t), result=loud[i].ctypes.data)
+            keep.append(plans)
         h = ctypes.c_void_p()
         _lib.check(self.lib.ss_pool_create(self.ctx, items, n, ctypes.byref(h)))
-        if levels is not None:
-            st = self.lib.ss_pool_levels(h, LEVELS[levels])
-            if st != _lib.SS_OK:
-                self.lib.ss_pool_destroy(h)
-                _lib.check(st)
+        st = self.lib.ss_pool_loudness(h, post) if post is not None else _lib.SS_OK
+        if st == _lib.SS_OK and levels is not None:
+            st = self.lib.ss_pool_levels(h, LEVELS[levels])        # tables of the normalised stems
+        if st != _lib.SS_OK:
+            self.lib.ss_pool_destroy(h)
+            _lib.check(st)
         taps = {_rirs(s)[0].direct_taps for s in candidates}
         return SourcePool(self, h, candidates, first[0], first[1], first[2], min(s.dry.numel() for s in candidates),
-                          taps.pop() if len(taps) == 1 else 0, levels)
+                          taps.pop() if len(taps) == 1 else 0, levels, loud)
 
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
