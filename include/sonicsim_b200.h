@@ -414,7 +414,8 @@ int ss_loudness_dev(ss_ctx* ctx, const ss_loud_item* items, int n_items, void* s
 
 /* One stem in host memory, N*C floats in a dense (N, C) or (C, N) layout given by the strides (other
  * strides return SS_ERR_INVALID, even when measuring only: the block is copied as it is); returns when
- * `out` (if given, same layout), the measured loudness and the linear gain are available. */
+ * `out` (if given, same layout), the measured loudness and the linear gain are available.  A NULL brk, and
+ * gating arguments that the checks of ss_post_lufs below refuse, return SS_ERR_INVALID. */
 int ss_lufs_norm_host(ss_ctx* ctx, const float* data, float* out, int32_t N, int32_t C,
                       int64_t stride_n, int64_t stride_c, double rate, double block_size,
                       double target_lufs, const int32_t* brk, int32_t n_e, const int32_t* blk_lo,
@@ -422,7 +423,10 @@ int ss_lufs_norm_host(ss_ctx* ctx, const float* data, float* out, int32_t N, int
 
 /* Optional per-source post-processing of ss_render_host_ex: measure the rendered (C, N) stem and
  * normalise it to `target_lufs` on the device before it is copied out (SonicSet.py:97-101 applies
- * get_lufs_norm_audio to every stem right after rendering it).  brk == NULL skips the source. */
+ * get_lufs_norm_audio to every stem right after rendering it).  brk == NULL skips the source.
+ * An array of entries is refused (SS_ERR_INVALID, before anything is copied) unless every entry with a
+ * brk has non-NULL blk_lo and blk_hi, n_e > 0, n_blocks >= 0, rate > 0 and block_size > 0 (NaN is
+ * refused), and the rate of the first entry that has a brk. */
 typedef struct {
     const int32_t* brk; const int32_t* blk_lo; const int32_t* blk_hi;   /* host arrays, see ss_loud_item */
     int32_t n_e, n_blocks;
@@ -431,8 +435,8 @@ typedef struct {
 } ss_post_lufs;
 
 /* ss_render_host + optional loudness normalisation of each stem while it is still in HBM.  Every source
- * with a target must have C <= 8 and the rate of the first source that has one; otherwise the call returns
- * SS_ERR_INVALID before anything is copied. */
+ * with a target must have C <= 8, and `post` must pass the checks of ss_post_lufs; otherwise the call
+ * returns SS_ERR_INVALID before anything is copied. */
 int ss_render_host_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss_post_lufs* post);
 
 /* ---- loudness gains of a pool (version 108): SonicSet's files hold every stem loudness-normalised over the whole stem
@@ -454,9 +458,9 @@ int ss_render_host_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss
  *   - ss_pool_levels afterwards builds the tables of the normalised stems (each stem scaled by (float)gain with
  *     k_loud_scale first), so that start draws test the crops the slots render.
  * Returns when the gains are in device memory.  Refused before anything is allocated, with the pool unchanged: a NULL
- * pool or post (SS_ERR_INVALID); C > 8 (SS_ERR_UNSUPPORTED, as ss_loudness_dev); measured candidates whose rates
- * differ, a gating plan with brk but without blk_lo / blk_hi, n_e <= 0, n_blocks < 0, rate or block_size <= 0; a pool
- * that already has gains or level tables, or that a plan has been created over (SS_ERR_INVALID). */
+ * pool or post (SS_ERR_INVALID); C > 8 (SS_ERR_UNSUPPORTED, as ss_loudness_dev); entries that the checks of
+ * ss_post_lufs refuse; a pool that already has gains or level tables, or that a plan has been created over
+ * (SS_ERR_INVALID). */
 int ss_pool_loudness(ss_pool* pool, const ss_post_lufs* post);   /* n entries, one per candidate */
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py

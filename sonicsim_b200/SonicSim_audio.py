@@ -51,6 +51,11 @@ def gating_plan(num_samples: int, rate: float, block_size: float, refine: int = 
     return brk.astype(np.int32), blk_lo, blk_hi
 
 
+def gating_block_size(num_samples, rate):
+    """SonicSim_audio.py:69: lufs_norm's gating block in seconds, 0.4 or the whole stem when that is shorter."""
+    return 0.4 if num_samples / rate >= 0.4 else num_samples / rate
+
+
 def _valid_audio(data, rate, block_size):
     """pyloudnorm.util.valid_audio."""
     if not isinstance(data, np.ndarray):
@@ -83,8 +88,7 @@ def integrated_loudness_and_norm(data: np.ndarray, sr, block_size, target, want_
 
 def lufs_norm(data, sr, norm=-6):
     """SonicSim_audio.py:68-81 -> (norm_data, gain)."""
-    block_size = 0.4 if len(data) / sr >= 0.4 else len(data) / sr                   # :69
-    loudness, _, out = integrated_loudness_and_norm(np.asarray(data), sr, block_size, norm)
+    loudness, _, out = integrated_loudness_and_norm(np.asarray(data), sr, gating_block_size(len(data), sr), norm)
     if math.isinf(loudness):                                                        # :73-75 (applied on the device too)
         print("loudness is inf")
     norm_data = out if np.asarray(data).dtype == np.float32 else out.astype(np.asarray(data).dtype)

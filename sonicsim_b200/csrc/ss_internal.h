@@ -64,6 +64,20 @@ inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 struct ScaleItem { float* data; const double* result; int32_t N, C; };
 int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t stream);
 
+// Loudness targets of n stems (ss_render_host_ex, ss_pool_loudness).  check_post_lufs: the checks of ss_post_lufs in
+// include/sonicsim_b200.h, SS_OK or SS_ERR_INVALID.  gating_tables: every distinct (brk, blk_lo, blk_hi, n_e, n_blocks)
+// of the entries with a target once, in one host block for one upload; entry i's set at bytes[at[i]].
+int check_post_lufs(const ss_post_lufs* post, int n);
+struct GatingTables { std::vector<char> bytes; std::vector<size_t> at; };
+GatingTables gating_tables(const ss_post_lufs* post, int n);
+// The item that measures entry q's (C, N) stem at `data`, with its set of gating_tables at `tab` on the device;
+// out = data normalises the stem in place, NULL measures only.  `scratch`: loud_scratch_bytes(q, C).
+ss_loud_item loud_item(const ss_post_lufs& q, const char* tab, const float* data, float* out, int32_t N, int32_t C,
+                       double* scratch, double* result);
+inline size_t loud_scratch_bytes(const ss_post_lufs& q, int32_t C) {
+    return align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * C * q.n_e, 256);
+}
+
 // One mixture of the dataloader's arithmetic (ss_mix.cu), as ss_mix_dev and plans with mixtures describe it on the
 // device.  A stem is Cf rows of E floats at row stride T (Cf = 1: the stem's E floats as they are; Cf = C under
 // SS_MIX_MONO: its (C, T) channels, folded to their mean at every element).

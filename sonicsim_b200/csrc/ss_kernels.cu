@@ -1696,50 +1696,27 @@ struct BuildStream {
 };
 
 // ----------------------------------------------------------------------------- loudness gains of a pool
-extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items, void* stream);
-
 // Device memory of one ss_pool_loudness call: the gating tables of the measured candidates (one copy per distinct set of
 // host arrays), their results, and one group's scratch
 static int loudness_build(ss_pool* pl, const ss_post_lufs* post, cudaStream_t s, std::vector<void*>& owned,
                           std::vector<double>& res) {
     const int n = pl->n;
-    struct Tab { const int32_t *brk, *lo, *hi; int n_e, n_blocks; size_t o_brk, o_lo, o_hi; };   // o_*: in d_tab
-    std::vector<Tab> tabs;
-    std::vector<int> tab_of(n, -1);
-    std::vector<char> host;
-    for (int i = 0; i < n; ++i) {
-        const ss_post_lufs& q = post[i];
-        if (!q.brk) continue;
-        int t = -1;
-        for (size_t k = 0; k < tabs.size(); ++k)
-            if (tabs[k].brk == q.brk && tabs[k].lo == q.blk_lo && tabs[k].hi == q.blk_hi && tabs[k].n_e == q.n_e &&
-                tabs[k].n_blocks == q.n_blocks) { t = (int)k; break; }
-        if (t < 0) {
-            const size_t off = host.size(), nb = 4 * (size_t)q.n_blocks;
-            const size_t o_lo = off + align_up(4 * (size_t)(q.n_e + 1), 256), o_hi = o_lo + align_up(nb + 4, 256);
-            host.resize(o_hi + align_up(nb + 4, 256));
-            memcpy(host.data() + off, q.brk, 4 * (size_t)(q.n_e + 1));
-            if (nb) { memcpy(host.data() + o_lo, q.blk_lo, nb); memcpy(host.data() + o_hi, q.blk_hi, nb); }
-            tabs.push_back(Tab{q.brk, q.blk_lo, q.blk_hi, q.n_e, q.n_blocks, off, o_lo, o_hi});
-            t = (int)tabs.size() - 1;
-        }
-        tab_of[i] = t;
-    }
+    const GatingTables tabs = gating_tables(post, n);
     const StemGroups G = stem_groups(pl);
     size_t scratch = 0;                                 // the largest group's loudness scratch
     for (size_t g = 0; g + 1 < G.first.size(); ++g) {
         size_t b = 0;
         for (int i = G.first[g]; i < G.first[g + 1]; ++i)
-            if (post[i].brk) b += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * pl->C * post[i].n_e, 256);
+            if (post[i].brk) b += loud_scratch_bytes(post[i], pl->C);
         scratch = std::max(scratch, b);
     }
     char *d_tab = nullptr, *d_scr = nullptr, *tmp = nullptr;
     double* d_res = nullptr;
-    CK(cudaMalloc((void**)&d_tab, std::max(host.size(), (size_t)256))); owned.push_back(d_tab);
+    CK(cudaMalloc((void**)&d_tab, std::max(tabs.bytes.size(), (size_t)256))); owned.push_back(d_tab);
     CK(cudaMalloc((void**)&d_res, 2 * sizeof(double) * (size_t)n)); owned.push_back(d_res);
     CK(cudaMalloc((void**)&d_scr, std::max(scratch, (size_t)256))); owned.push_back(d_scr);
     CK(cudaMalloc((void**)&tmp, G.cap)); owned.push_back(tmp);
-    if (!host.empty()) CK(cudaMemcpy(d_tab, host.data(), host.size(), cudaMemcpyHostToDevice));
+    if (!tabs.bytes.empty()) CK(cudaMemcpy(d_tab, tabs.bytes.data(), tabs.bytes.size(), cudaMemcpyHostToDevice));
     std::vector<ss_loud_item> li;
     const int st = render_stem_groups(pl, G, tmp, s, [&](int first, int last) -> int {
         // every measured candidate of the group: the launches of ss_loudness_dev on its (C, N) stem, measure only
@@ -1747,18 +1724,9 @@ static int loudness_build(ss_pool* pl, const ss_post_lufs* post, cudaStream_t s,
         char* scr = d_scr;
         for (int i = first; i < last; ++i) {
             if (!post[i].brk) continue;
-            const ss_post_lufs& q = post[i];
-            const Tab& tb = tabs[tab_of[i]];
-            ss_loud_item it; memset(&it, 0, sizeof(it));
-            it.data = (const float*)(tmp + G.at[i]);
-            it.brk = (const int32_t*)(d_tab + tb.o_brk);
-            it.blk_lo = (const int32_t*)(d_tab + tb.o_lo); it.blk_hi = (const int32_t*)(d_tab + tb.o_hi);
-            it.scratch = (double*)scr; scr += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * pl->C * q.n_e, 256);
-            it.result = d_res + 2 * (size_t)i;
-            it.stride_n = 1; it.stride_c = pl->host[i].N; it.N = pl->host[i].N; it.C = pl->C;
-            it.n_e = q.n_e; it.n_blocks = q.n_blocks;
-            it.rate = q.rate; it.block_size = q.block_size; it.target_lufs = q.target_lufs;
-            li.push_back(it);
+            li.push_back(loud_item(post[i], d_tab + tabs.at[i], (const float*)(tmp + G.at[i]), nullptr, pl->host[i].N,
+                                   pl->C, (double*)scr, d_res + 2 * (size_t)i));
+            scr += loud_scratch_bytes(post[i], pl->C);
         }
         for (size_t k = 0; k < li.size(); k += 65535) {   // ss_loudness_dev's item limit
             const int st2 = ss_loudness_dev(pl->c, li.data() + k, (int)std::min(li.size() - k, (size_t)65535), (void*)s);
@@ -1775,16 +1743,7 @@ static int loudness_build(ss_pool* pl, const ss_post_lufs* post, cudaStream_t s,
 extern "C" int ss_pool_loudness(ss_pool* pl, const ss_post_lufs* post) {
     if (!pl || !post) return SS_ERR_INVALID;
     if (pl->C > 8) return SS_ERR_UNSUPPORTED;           // as ss_loudness_dev
-    if (pl->gains || pl->levels || pl->planned) return SS_ERR_INVALID;
-    const ss_post_lufs* first = nullptr;
-    for (int i = 0; i < pl->n; ++i) {
-        const ss_post_lufs& q = post[i];
-        if (!q.brk) continue;
-        if (!q.blk_lo || !q.blk_hi || q.n_e <= 0 || q.n_blocks < 0 || !(q.rate > 0) || !(q.block_size > 0))
-            return SS_ERR_INVALID;
-        if (!first) first = &q;
-        else if (q.rate != first->rate) return SS_ERR_INVALID;
-    }
+    if (pl->gains || pl->levels || pl->planned || check_post_lufs(post, pl->n)) return SS_ERR_INVALID;
     CK(cudaSetDevice(pl->c->device));
     std::vector<void*> owned;
     std::vector<double> res;
@@ -2305,17 +2264,13 @@ static int ensure(char** p, size_t* cap, size_t need) {
     return SS_OK;
 }
 
-extern "C" int ss_loudness_dev(ss_ctx* c, const ss_loud_item* items, int n_items, void* stream);
-
 // Host path: H2D -> k_spectra -> k_render [-> loudness measure + in-place gain] -> D2H, pipelined
 // over chunks on three streams with two device slots.
 extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_post_lufs* post) {
     if (!c || (!items && n_items > 0) || n_items < 0) return SS_ERR_INVALID;
     if (n_items == 0) return SS_OK;
     CK(cudaSetDevice(c->device));
-    // every stem with a target shares one sample rate (ss_loudness_dev runs one set of filter coefficients per call);
-    // checked against the first source that has a target, so that the answer does not depend on the chunking
-    const ss_post_lufs* first_post = nullptr;
+    if (post && check_post_lufs(post, n_items)) return SS_ERR_INVALID;
     std::vector<Shape> shapes(n_items);
     std::vector<ReadSet> rset(n_items);
     for (int i = 0; i < n_items; ++i) {
@@ -2331,11 +2286,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         shapes[i] = shape_of(h);
         rset[i] = read_set(items[i], shapes[i]);
         st = check_idx_host(items[i], rset[i]); if (st) return st;
-        if (post && post[i].brk) {
-            if (!post[i].blk_lo || !post[i].blk_hi || post[i].n_e <= 0 || post[i].rate <= 0 || items[i].C > 8) return SS_ERR_INVALID;
-            if (!first_post) first_post = &post[i];
-            if (post[i].rate != first_post->rate) return SS_ERR_INVALID;
-        }
+        if (post && post[i].brk && items[i].C > 8) return SS_ERR_INVALID;
     }
     // an earlier asynchronous ss_render_dev may still be using scratch buffer 0 on its internal streams
     for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaStreamWaitEvent(c->s_cmp, c->ev_join[i], 0));
@@ -2353,25 +2304,11 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     // there and serialise the whole pipeline; (c) the loudness kernels of consecutive chunks run on rotating side
     // streams: their grids are small and latency-bound, three of them overlap each other, the
     // next chunk's render and the copies
-    struct Tab { const int32_t *brk, *lo, *hi; int n_e, n_blocks; const int32_t *d_brk, *d_lo, *d_hi; };
-    std::vector<Tab> tabs;
-    std::vector<int> tab_of(n_items, -1);
+    GatingTables tabs;
+    const size_t res_bytes = align_up(2 * sizeof(double) * (size_t)n_items, 256);   // [0, res_bytes): results
     if (post) {
-        size_t tab_bytes = 0;
-        for (int i = 0; i < n_items; ++i) {
-            if (!post[i].brk) continue;
-            int t = -1;
-            for (size_t q = 0; q < tabs.size(); ++q)
-                if (tabs[q].brk == post[i].brk && tabs[q].lo == post[i].blk_lo && tabs[q].hi == post[i].blk_hi &&
-                    tabs[q].n_e == post[i].n_e && tabs[q].n_blocks == post[i].n_blocks) { t = (int)q; break; }
-            if (t < 0) {
-                Tab nt = {post[i].brk, post[i].blk_lo, post[i].blk_hi, post[i].n_e, post[i].n_blocks, nullptr, nullptr, nullptr};
-                tabs.push_back(nt); t = (int)tabs.size() - 1;
-                tab_bytes += align_up(4 * (size_t)(nt.n_e + 1), 256) + 2 * align_up(4 * (size_t)(nt.n_blocks + 1), 256);
-            }
-            tab_of[i] = t;
-        }
-        const size_t res_bytes = align_up(2 * sizeof(double) * (size_t)n_items, 256);
+        tabs = gating_tables(post, n_items);
+        const size_t tab_bytes = tabs.bytes.size();
         if (tab_bytes + res_bytes > c->h_post_cap) {
             CK(cudaDeviceSynchronize());
             if (c->h_post) CK(cudaFreeHost(c->h_post));
@@ -2382,20 +2319,14 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
             CK(cudaMalloc((void**)&c->d_post, cap));
             c->h_post_cap = cap;
         }
-        size_t off = res_bytes;                              // [0, res_bytes): results (host side only)
-        for (auto& t : tabs) {
-            size_t nb = 4 * (size_t)(t.n_e + 1);
-            memcpy(c->h_post + off, t.brk, nb); t.d_brk = (const int32_t*)(c->d_post + off); off += align_up(nb, 256);
-            nb = 4 * (size_t)t.n_blocks;
-            if (nb) memcpy(c->h_post + off, t.lo, nb);
-            t.d_lo = (const int32_t*)(c->d_post + off); off += align_up(nb + 4, 256);
-            if (nb) memcpy(c->h_post + off, t.hi, nb);
-            t.d_hi = (const int32_t*)(c->d_post + off); off += align_up(nb + 4, 256);
+        char* const h_tab = c->h_post + res_bytes;
+        if (tab_bytes) {
+            memcpy(h_tab, tabs.bytes.data(), tab_bytes);
+            CK(cudaMemcpyAsync(c->d_post + res_bytes, h_tab, tab_bytes, cudaMemcpyHostToDevice, c->s_in));
         }
-        if (off > res_bytes)
-            CK(cudaMemcpyAsync(c->d_post + res_bytes, c->h_post + res_bytes, off - res_bytes, cudaMemcpyHostToDevice, c->s_in));
     }
     double* const h_res = post ? (double*)c->h_post : nullptr;
+    const char* const d_tab = post ? c->d_post + res_bytes : nullptr;
     // the pipeline proper; any failure falls through to the stream synchronisation below, so that no copy is
     // still reading or writing the caller's buffers when this function returns
     auto pipeline = [&]() -> int {
@@ -2412,8 +2343,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
             if (it.mode == SS_MOVING_BOUNDS) in_b += align_up(sizeof(int32_t) * (size_t)it.P, 256);
             if (it.mode == SS_MOVING_INDEXED) in_b += 2 * align_up(4 * (size_t)(rs.ib - rs.ia), 256);
             out_b += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256) * direct_sets(it);
-            if (post && post[i].brk)
-                out_b += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * it.C * post[i].n_e, 256) + 256;
+            if (post && post[i].brk) out_b += loud_scratch_bytes(post[i], it.C) + 256;
         }
         if (k >= (size_t)ss_ctx::kSlots) CK(cudaEventSynchronize(sl.ev_free));      // slot's previous chunk fully drained
         if ((rc = ensure(&sl.d_in, &sl.in_cap, in_b)) != SS_OK) break;
@@ -2447,18 +2377,10 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
             if (it.flags & SS_DIRECT_TARGET) { d.out_direct = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256); }
             dev[i] = d;
             if (post && post[i].brk) {
-                const ss_post_lufs& pl = post[i];
-                ss_loud_item li; memset(&li, 0, sizeof(li));
-                const Tab& tb = tabs[tab_of[i]];
-                li.brk = tb.d_brk; li.blk_lo = tb.d_lo; li.blk_hi = tb.d_hi;
-                li.scratch = (double*)po; po += align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * it.C * pl.n_e, 256);
-                li.result = (double*)po; po += 256;
-                res_dev[i] = li.result;
-                li.data = d.out; li.out = d.out;                 // (C, N) stem, normalised in place
-                li.stride_n = 1; li.stride_c = it.N; li.N = it.N; li.C = it.C; li.n_e = pl.n_e; li.n_blocks = pl.n_blocks;
-                li.rate = pl.rate; li.block_size = pl.block_size; li.target_lufs = pl.target_lufs;
-                loud.push_back(li);
-                if (it.flags & SS_DIRECT_TARGET) direct_gain.push_back(ScaleItem{d.out_direct, li.result, it.N, it.C});
+                double* scratch = (double*)po; po += loud_scratch_bytes(post[i], it.C);
+                res_dev[i] = (double*)po; po += 256;
+                loud.push_back(loud_item(post[i], d_tab + tabs.at[i], d.out, d.out, it.N, it.C, scratch, res_dev[i]));
+                if (it.flags & SS_DIRECT_TARGET) direct_gain.push_back(ScaleItem{d.out_direct, res_dev[i], it.N, it.C});
             }
         }
         CK(cudaEventRecord(sl.ev_in, c->s_in));

@@ -7,6 +7,8 @@
 #include <math.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "ss_internal.h"
 #include "ss_loud.cuh"
 
@@ -296,13 +298,71 @@ int loud_scale_dev(ss_ctx* c, const ScaleItem* items, int n_items, cudaStream_t 
     return ring_release(c, slot, stream);
 }
 
+// Every stem with a target shares one sample rate (ss_loudness_dev runs one set of filter coefficients per call),
+// checked against the first entry that has a target, so that the answer does not depend on how a caller groups stems.
+// The `!(x > 0)` tests refuse NaN.
+int check_post_lufs(const ss_post_lufs* post, int n) {
+    const ss_post_lufs* first = nullptr;
+    for (int i = 0; i < n; ++i) {
+        const ss_post_lufs& q = post[i];
+        if (!q.brk) continue;
+        if (!q.blk_lo || !q.blk_hi || q.n_e <= 0 || q.n_blocks < 0 || !(q.rate > 0) || !(q.block_size > 0))
+            return SS_ERR_INVALID;
+        if (!first) first = &q;
+        else if (q.rate != first->rate) return SS_ERR_INVALID;
+    }
+    return SS_OK;
+}
+
+// A table set: brk, then blk_lo at lo_at(q), then blk_hi at hi_at(q), each 256-aligned.  Stems of one clip length
+// share the caller's host arrays (the normal case): their set is copied once.
+static size_t lo_at(const ss_post_lufs& q) { return align_up(4 * (size_t)(q.n_e + 1), 256); }
+static size_t hi_at(const ss_post_lufs& q) { return lo_at(q) + align_up(4 * (size_t)q.n_blocks + 4, 256); }
+
+GatingTables gating_tables(const ss_post_lufs* post, int n) {
+    GatingTables T;
+    T.at.assign(n, 0);
+    std::vector<int> sets;                               // the first entry of each distinct set
+    for (int i = 0; i < n; ++i) {
+        const ss_post_lufs& q = post[i];
+        if (!q.brk) continue;
+        const auto k = std::find_if(sets.begin(), sets.end(), [&](int j) {
+            const ss_post_lufs& p = post[j];
+            return p.brk == q.brk && p.blk_lo == q.blk_lo && p.blk_hi == q.blk_hi && p.n_e == q.n_e &&
+                   p.n_blocks == q.n_blocks;
+        });
+        if (k != sets.end()) { T.at[i] = T.at[*k]; continue; }
+        sets.push_back(i);
+        const size_t off = T.bytes.size(), nb = 4 * (size_t)q.n_blocks;
+        T.at[i] = off;
+        T.bytes.resize(off + hi_at(q) + align_up(nb + 4, 256));
+        memcpy(&T.bytes[off], q.brk, 4 * (size_t)(q.n_e + 1));
+        if (nb) { memcpy(&T.bytes[off + lo_at(q)], q.blk_lo, nb); memcpy(&T.bytes[off + hi_at(q)], q.blk_hi, nb); }
+    }
+    return T;
+}
+
+ss_loud_item loud_item(const ss_post_lufs& q, const char* tab, const float* data, float* out, int32_t N, int32_t C,
+                       double* scratch, double* result) {
+    ss_loud_item it;
+    memset(&it, 0, sizeof(it));
+    it.data = data; it.out = out;
+    it.brk = (const int32_t*)tab;
+    it.blk_lo = (const int32_t*)(tab + lo_at(q)); it.blk_hi = (const int32_t*)(tab + hi_at(q));
+    it.scratch = scratch; it.result = result;
+    it.stride_n = 1; it.stride_c = N; it.N = N; it.C = C; it.n_e = q.n_e; it.n_blocks = q.n_blocks;
+    it.rate = q.rate; it.block_size = q.block_size; it.target_lufs = q.target_lufs;
+    return it;
+}
+
 // Single stem, host arrays (the drop-in lufs_norm): data / out hold N*C floats in the caller's layout, which is copied
 // to the device as one block, so the strides must describe a dense layout even when only measuring.
 extern "C" int ss_lufs_norm_host(ss_ctx* c, const float* data, float* out, int32_t N, int32_t C,
                                  int64_t stride_n, int64_t stride_c, double rate, double block_size,
                                  double target_lufs, const int32_t* brk, int32_t n_e, const int32_t* blk_lo,
                                  const int32_t* blk_hi, int32_t n_blocks, double* loudness, double* gain) {
-    if (!c || !data || !brk || !blk_lo || !blk_hi || N <= 0 || C <= 0 || n_e <= 0) return SS_ERR_INVALID;
+    const ss_post_lufs q = {brk, blk_lo, blk_hi, n_e, n_blocks, rate, block_size, target_lufs, nullptr};
+    if (!c || !data || !brk || N <= 0 || C <= 0 || check_post_lufs(&q, 1)) return SS_ERR_INVALID;
     if (!dense_layout(N, C, stride_n, stride_c)) return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     const size_t nel = (size_t)N * C;

@@ -363,6 +363,43 @@ def _check_direct_outs(direct_outs, n):
     return direct_outs if direct_outs is not None else [None] * n
 
 
+def _check_lufs(api, what, targets, n, sr):
+    """Refuses, before any C call, loudness targets (when given) other than one finite value or None for each of the n
+    stems, and sr <= 0; `what` names a stem ("source", "candidate")."""
+    if targets is None:
+        return
+    if len(targets) != n:
+        raise ValueError("%s: %d %ss but %d entries in lufs_targets" % (api, n, what, len(targets)))
+    for i, t in enumerate(targets):
+        if t is not None and not math.isfinite(float(t)):
+            raise ValueError("%s: the loudness target of %s %d is not finite: %r" % (api, what, i, t))
+    if not float(sr) > 0:
+        raise ValueError("%s: sr must be > 0, got %r" % (api, sr))
+
+
+def _post_lufs(targets, items, sr, results, keep):
+    """The ss_post_lufs array of checked targets for the SsSource `items` (None without targets): stem i is measured
+    like SonicSim_audio.lufs_norm into results[i].  The gating plans it points into, one per length, go to `keep`."""
+    if targets is None:
+        return None
+    from .SonicSim_audio import gating_block_size, gating_plan
+    post = (SsPostLufs * len(targets))()
+    plans = {}
+    for i, t in enumerate(targets):
+        if t is None:
+            continue
+        N = items[i].N
+        block = float(gating_block_size(N, sr))
+        if N not in plans:
+            plans[N] = gating_plan(N, float(sr), block)
+        brk, blo, bhi = plans[N]
+        post[i] = SsPostLufs(brk=brk.ctypes.data, blk_lo=blo.ctypes.data, blk_hi=bhi.ctypes.data, n_e=len(brk) - 1,
+                             n_blocks=len(blo), rate=float(sr), block_size=block, target_lufs=float(t),
+                             result=results[i].ctypes.data)
+    keep.append(plans)
+    return post
+
+
 class Renderer:
     """Owns the per-device ss_ctx.  One process per GPU (LOCAL_RANK picks the device by default)."""
 
@@ -423,20 +460,12 @@ class Renderer:
         pooled slot that picks it stores its crops, direct stem included, times that (float32) gain.  The level tables
         then describe the normalised stems.  `loudness` holds the measured (LUFS, gain) pairs."""
         import torch
-        from .SonicSim_audio import gating_plan
         if levels not in LEVELS:
             raise ValueError("source_pool: levels must be None, 'mono' or 'channels', got %r" % (levels,))
         n = len(candidates)
         if not 1 <= n <= 1 << 24:
             raise ValueError("source_pool: a pool holds 1 to 2^24 candidates, got %d" % n)
-        if lufs_targets is not None:
-            if len(lufs_targets) != n:
-                raise ValueError("source_pool: %d candidates but %d entries in lufs_targets" % (n, len(lufs_targets)))
-            for i, t in enumerate(lufs_targets):
-                if t is not None and not math.isfinite(float(t)):
-                    raise ValueError("source_pool: the loudness target of candidate %d is not finite: %r" % (i, t))
-            if not float(sr) > 0:
-                raise ValueError("source_pool: sr must be > 0, got %r" % (sr,))
+        _check_lufs("source_pool", "candidate", lufs_targets, n, sr)
         items = (SsSource * n)()
         keep = []
         first = None
@@ -466,26 +495,11 @@ class Renderer:
                     raise ValueError("source_pool: moving candidate %d needs bounds_host" % i)
                 bh = _bounds(s.bounds_host, P, "source_pool: bounds_host of %s" % own, keep)
                 items[i].bounds_host = bh.ctypes.data
-        loud, post = None, None
-        if lufs_targets is not None:
-            if first[1] > 8:
-                raise ValueError("source_pool: loudness normalisation supports at most 8 channels, the candidates have %d"
-                                 % first[1])
-            loud = np.full((n, 2), np.nan, dtype=np.float64)
-            post = (SsPostLufs * n)()
-            plans = {}                                   # one gating plan per length
-            for i, t in enumerate(lufs_targets):
-                if t is None:
-                    continue
-                N = int(items[i].N)
-                block = 0.4 if N / sr >= 0.4 else N / sr                      # SonicSim_audio.py:69, as plan_host
-                if N not in plans:
-                    plans[N] = gating_plan(N, float(sr), float(block))
-                brk, blo, bhi = plans[N]
-                post[i] = SsPostLufs(brk=brk.ctypes.data, blk_lo=blo.ctypes.data, blk_hi=bhi.ctypes.data,
-                                     n_e=len(brk) - 1, n_blocks=len(blo), rate=float(sr), block_size=float(block),
-                                     target_lufs=float(t), result=loud[i].ctypes.data)
-            keep.append(plans)
+        if lufs_targets is not None and first[1] > 8:
+            raise ValueError("source_pool: loudness normalisation supports at most 8 channels, the candidates have %d"
+                             % first[1])
+        loud = np.full((n, 2), np.nan, dtype=np.float64)
+        post = _post_lufs(lufs_targets, items, sr, loud, keep)
         h = ctypes.c_void_p()
         _lib.check(self.lib.ss_pool_create(self.ctx, items, n, ctypes.byref(h)))
         st = self.lib.ss_pool_loudness(h, post) if post is not None else _lib.SS_OK
@@ -506,12 +520,11 @@ class Renderer:
         """Validate a batch once and bind it to its host buffers; `plan.run()` then renders it with a single
         C-ABI call (a generation loop refills the same pinned buffers and calls run() again).
         See render_host for the arguments."""
-        from .SonicSim_audio import gating_plan
         _refuse_pooled(sources, "plan_host")
         n = len(sources)
         direct_outs = _check_direct_outs(direct_outs, n)
+        _check_lufs("plan_host", "source", lufs_targets, n, sr)
         items = (SsSource * n)()
-        post = (SsPostLufs * n)() if lufs_targets is not None else None
         results_l = np.full((n, 2), np.nan, dtype=np.float64)
         keep = []
         results = []
@@ -538,18 +551,13 @@ class Renderer:
                                 rir_bank=_bank_of(self, s, i, P, C, L) if rb is not None else None)
             keep.append((x, h, out, dout, rb))
             results.append(out)
-            if post is not None and lufs_targets[i] is not None:
+            if lufs_targets is not None and lufs_targets[i] is not None:
                 if s.window is not None:
                     raise ValueError("source %d has a window and a loudness target: the loudness of a stem is "
                                      "measured over the whole stem" % i)
                 if C > 8:
                     raise ValueError("loudness normalisation supports at most 8 channels")
-                block = 0.4 if N / sr >= 0.4 else N / sr                      # SonicSim_audio.py:69
-                brk, blo, bhi = gating_plan(N, float(sr), float(block))
-                post[i] = SsPostLufs(brk=brk.ctypes.data, blk_lo=blo.ctypes.data, blk_hi=bhi.ctypes.data,
-                                     n_e=len(brk) - 1, n_blocks=len(blo), rate=float(sr), block_size=float(block),
-                                     target_lufs=float(lufs_targets[i]), result=results_l[i].ctypes.data)
-                keep.append((brk, blo, bhi))
+        post = _post_lufs(lufs_targets, items, sr, results_l, keep)
         return HostPlan(self, items, post, n, results, results_l, keep, sources)
 
     def render_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],

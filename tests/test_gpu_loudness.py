@@ -435,3 +435,66 @@ def test_render_host_ex_rejects_mixed_rates_and_wide_stems_before_any_copy():
     from sonicsim_b200 import SonicSim_audio as sa
     with pytest.raises(ValueError):
         sa.integrated_loudness_and_norm(np.zeros((16000, 9), np.float32), 16000, 0.4, -20.0)
+
+
+# one malformed field of an ss_post_lufs entry with a target (ctypes: None is a NULL pointer)
+MALFORMED = {"blk_lo NULL": ("blk_lo", None), "blk_hi NULL": ("blk_hi", None), "n_e 0": ("n_e", 0),
+             "n_blocks -1": ("n_blocks", -1), "rate 0": ("rate", 0.0), "rate NaN": ("rate", NAN),
+             "block_size 0": ("block_size", 0.0), "block_size NaN": ("block_size", NAN)}
+
+
+def _results(post, i):
+    return np.frombuffer((ctypes.c_double * 2).from_address(post[i].result), np.float64)
+
+
+@pytest.mark.parametrize("bad", list(MALFORMED))
+def test_render_host_ex_rejects_each_malformed_entry_before_any_copy(bad):
+    """The third of three sources (the first has no target) has one malformed field: ss_render_host_ex refuses the call
+    whether the sources share a chunk or not, and writes no output and no result.  ss_lufs_norm_host refuses the same
+    gating arguments."""
+    from sonicsim_b200 import _lib, render
+    R = render.default_renderer()
+    rng = np.random.default_rng(5)
+    field, value = MALFORMED[bad]
+    with small_host_budget_context() as small:
+        for ctx in (R.ctx, small):
+            items, post, outs, keep = _c_abi_items(rng, [None, 16000, 16000], N=96000)
+            setattr(post[2], field, value)
+            assert R.lib.ss_render_host_ex(ctx, items, 3, post) == _lib.SS_ERR_INVALID
+            assert all(np.all(np.isnan(o)) for o in outs)
+            assert all(np.all(np.isnan(_results(post, i))) for i in (1, 2))
+    q = post[2]
+    N, C = 96000, 2
+    x = so.synth_dry(rng, N * C)
+    out = np.full(N * C, NAN, np.float32)
+    lufs, gain = ctypes.c_double(NAN), ctypes.c_double(NAN)
+    st = R.lib.ss_lufs_norm_host(R.ctx, x.ctypes.data, out.ctypes.data, N, C, C, 1, q.rate, q.block_size, -20.0, q.brk,
+                                 q.n_e, q.blk_lo, q.blk_hi, q.n_blocks, ctypes.byref(lufs), ctypes.byref(gain))
+    assert st == _lib.SS_ERR_INVALID
+    assert np.isnan(lufs.value) and np.isnan(gain.value) and np.all(np.isnan(out))
+
+
+@pytest.mark.parametrize("targets, sr, match", [
+    ([-20.0], 16000, "entries in lufs_targets"),
+    ([-20.0, None, -20.0, -20.0], 16000, "entries in lufs_targets"),
+    ([-20.0, NAN, None], 16000, "not finite"),
+    ([float("inf"), -20.0, None], 16000, "not finite"),
+    ([-20.0, None, -20.0], 0, "sr must be > 0"),
+    ([-20.0, None, -20.0], NAN, "sr must be > 0"),
+])
+def test_plan_host_refuses_bad_targets_before_any_call(targets, sr, match):
+    """The wrong number of targets, a target that is not finite and sr <= 0 raise ValueError through plan_host,
+    render_host and render_scene, and nothing is rendered."""
+    from sonicsim_b200 import render
+    R = render.default_renderer()
+    rng = np.random.default_rng(6)
+    srcs = [render.StaticSource(so.synth_dry(rng, 16000), so.synth_rirs(rng, 1, 2, 300)[0]) for _ in range(3)]
+    outs = [np.full((2, 16000), NAN, np.float32) for _ in srcs]
+    with pytest.raises(ValueError, match=match):
+        R.plan_host(srcs, outs, targets, sr)
+    with pytest.raises(ValueError, match=match):
+        R.render_host(srcs, outs, targets, sr)
+    assert all(np.all(np.isnan(o)) for o in outs)
+    if match == "sr must be > 0":                            # render_scene draws its targets itself, one per stem
+        with pytest.raises(ValueError, match=match):
+            render.render_scene([], [(s.dry, s.rir) for s in srcs], sr=sr, static_lufs=[-20.0] * 3)

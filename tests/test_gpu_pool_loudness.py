@@ -13,7 +13,8 @@ the crop of that normalised stem.  Checked:
      slices of the normalised stems, and a quiet candidate whose gain turns a silent crop into an accepted one keeps a
      different start than the same plan without gains;
   5. a plan over gain pools launches exactly what the same plan over the pools without gains launches, as a graph;
-  6. every refusal, in Python and through the C ABI, leaves the pool unchanged."""
+  6. every refusal, in Python and through the C ABI (each malformed field of a target's entry included), leaves the
+     pool unchanged."""
 import ctypes
 
 import numpy as np
@@ -22,6 +23,7 @@ import torch
 
 from oracle import sonicsim_oracle as so
 import draw_reference as dr
+from test_gpu_loudness import MALFORMED
 from test_gpu_plan_draw import Step, check_snap, gappy_dry, TABLE_TOL, TRIES
 from test_gpu_plan_pool import Cand, _choice, _mix_dev, fold, to
 
@@ -402,5 +404,28 @@ def test_refusals_leave_the_pool_unchanged():
         before = state(pool)
         post, keep = _post(1, [9000], [-20.0], [16000])
         assert lib.ss_pool_loudness(pool._h, post) == UNS and state(pool) == before
+    finally:
+        pool.close()
+
+
+@pytest.mark.parametrize("bad", list(MALFORMED))
+def test_pool_loudness_refuses_each_malformed_entry(bad):
+    """The last of three entries (the second has no target) has one malformed field: SS_ERR_INVALID, the pool's bytes
+    and loudness unchanged, and the same pool then takes well-formed targets."""
+    from sonicsim_b200 import _lib
+    render, R = _R()
+    lib = R.lib
+    cands = noises(41)
+    N = [c.N for c in cands]
+    field, value = MALFORMED[bad]
+    pool = R.source_pool([c.src for c in cands])
+    try:
+        before = (lib.ss_pool_bytes(pool._h), pool.loudness.tobytes())
+        post, keep = _post(3, N, [-20.0, None, -22.0], [RATE] * 3)
+        setattr(post[2], field, value)
+        assert lib.ss_pool_loudness(pool._h, post) == _lib.SS_ERR_INVALID
+        assert (lib.ss_pool_bytes(pool._h), pool.loudness.tobytes()) == before
+        post, keep = _post(3, N, [-20.0, None, -22.0], [RATE] * 3)
+        assert lib.ss_pool_loudness(pool._h, post) == _lib.SS_OK
     finally:
         pool.close()
