@@ -187,13 +187,24 @@ void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their cont
  * Candidates (every violation is SS_ERR_INVALID, before anything is allocated):
  *   - 1 <= n <= 2^24;
  *   - banked: rir == NULL, rir_bank set, a bank of this context, with the candidate's P, C and L; `x` set;
- *   - one `mode` for all, SS_MOVING_BOUNDS or SS_STATIC (SS_MOVING_INDEXED is refused), one C, one L;
+ *   - one `mode` for all, SS_MOVING_BOUNDS or SS_STATIC (SS_MOVING_INDEXED is refused), one C; L may differ
+ *     (SonicSet gives every speaker of a scene its own RIR length): each candidate keeps its own bank, unpadded;
  *   - a moving candidate has `bounds` and `bounds_host` (ascending from 0 to N), so that the pool's blocking and table
  *     sizes are exact; idx and w are NULL;
  *   - out, out_direct, flags, direct_taps, win_start, win_len, win_start_dev, pool and pick_dev are zero.
  * Banks with and without a direct set may be mixed in one pool; the direct rule is enforced per slot.
- * Blocking: aligned if every candidate would choose aligned blocking on its own (ss_debug_plan), otherwise the
- * 4096-sample grid for all of them, so the kernel variant of a pooled slot is fixed when the pool is created.
+ * Blocking: aligned if every candidate would choose aligned blocking on its own (ss_debug_plan) with its own
+ * K = ceil(L / 4096), otherwise the 4096-sample grid for all of them.  The kernel variant of a pooled slot is fixed when
+ * the pool is created, from the pool's largest K: k_render<LONG> if any candidate has K > 1.  A slot that picks candidate
+ * i renders with that candidate's own K_i RIR partitions.  A pool's L is its longest candidate's.
+ * Bits of candidates of different L: a candidate that would choose the pool's blocking and variant on its own (every
+ * K_i > 1 candidate, and every candidate of a pool whose candidates share K) has the bits of ss_render_dev as above.  A
+ * K_i = 1 candidate of a pool with K > 1 candidates runs k_render<LONG> with one partition: its output equals, bit for
+ * bit, a render over its bank with exact-zero partitions appended, and the render of its RIRs zero-padded to the pool's
+ * L within float32 rounding only (a padded bank's zero partitions hold the rounding residue of the rows they are
+ * transformed with).  Level tables and gains (below) are computed from every candidate rendered whole on its own, so
+ * for such a candidate they differ from its pooled stems by float32 rounding, as for a candidate that chooses other
+ * blocking than its pool.
  * The pool copies what it needs (including the bounds_host values); the candidates' device buffers (x, bounds) and banks
  * must outlive the pool.  ss_pool_create returns when the pool's table is in device memory; the pool records one event
  * behind the construction of all its banks, which every plan run that uses the pool waits on.
@@ -201,7 +212,7 @@ void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their cont
  * A pooled slot (every violation is SS_ERR_INVALID, before anything is allocated):
  *   - x, rir, rir_bank, bounds, bounds_host, idx and w are NULL, N and P are 0; pool of this context; pick_dev a 4-byte
  *     aligned device pointer;
- *   - mode, C and L are the pool's;
+ *   - mode, C and L are the pool's (L: the longest candidate's);
  *   - win_len > 0 with a fixed win_start (win_start + win_len <= every candidate's N) or a win_start_dev (win_start == 0
  *     and win_len <= every candidate's N); the window start is clamped against the picked candidate's N (bit 2);
  *   - SS_DIRECT_TARGET only if every candidate's bank holds a direct set with the slot's direct_taps; no
@@ -215,6 +226,7 @@ void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their cont
  * Lifetime: a pool must outlive every plan that uses it; ss_pool_destroy waits for the device before it frees it. */
 int ss_pool_create(ss_ctx* ctx, const ss_source* candidates, int n, ss_pool** out);
 int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact candidate entries (40 B each), the n
+                                               * int32 partition counts (4 B each) when the candidates' K differ, the n
                                                * float gains (4 B each) once ss_pool_loudness measured them, and the
                                                * level tables with their pointer array once ss_pool_levels built them */
 void ss_pool_destroy(ss_pool* pool);          /* destroy pools after the plans that use them, before their context */

@@ -112,9 +112,9 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 // full plan; a windowed one's holds the full plan's blocks [g0, g1) (window_span, cut to the table size).  A moving
 // window first reads its start from device memory, clamps it (bit 2 of g_dev_err) and stores it as counts[4], where
 // the window search here and k_prepare's range warps take it; its table is sized for every start (window_table_cap).
-// A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate - and its loudness gain,
-// counts[11] - into its Source in the descriptor block (pick_slot), which is why k_prepare then reads the Source table
-// from global memory (k_prepare<false>).
+// A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate - its RIR partition count
+// when the pool's candidates differ in K (pick_parts), and its loudness gain, counts[11] - into its Source in the
+// descriptor block (pick_slot), which is why k_prepare then reads the Source table from global memory (k_prepare<false>).
 __global__ void __launch_bounds__(256)
 k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -124,7 +124,9 @@ k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
         if (S.h_rows) {
             if (pool_table(S) && lane == 0) {
                 bool bad;
-                pick_slot(S, *pick_ptr(S), bad);
+                const int v = *pick_ptr(S);
+                pick_parts(S, v);                       // the picked candidate's K first: set_banked reads it
+                pick_slot(S, v, bad);
                 if (bad) atomicOr(&g_dev_err, 8u);
             }
             __syncwarp();
@@ -800,7 +802,9 @@ struct ss_bank {
 struct ss_pool {
     ss_ctx* c = nullptr;
     PoolEntry* table = nullptr;           // device, n entries
-    int n = 0, mode = 0, C = 0, L = 0, K = 0, aligned = 0;
+    int n = 0, mode = 0, C = 0, L = 0, K = 0, aligned = 0;   // L, K: the longest candidate's
+    std::vector<int> parts_host;          // candidate i's RIR partition count K_i
+    int* parts = nullptr;                 // device copy of parts_host when the K_i differ (pool_parts), else null
     int n_min = 0, p_max = 0;             // shortest candidate (window rule), most positions (rstep table)
     int direct_taps = 0;                  // > 0: every candidate's bank holds a direct set with these taps
     std::vector<PoolEntry> host;          // the table's entries
@@ -878,7 +882,8 @@ static bool bounds_ok(const int32_t* b, int P, int N) {
     for (int q = 0; q + 1 < P; ++q) if (b[q + 1] < b[q]) return false;
     return true;
 }
-// A pooled slot against its pool (include/sonicsim_b200.h): no source fields of its own, the pool's mode / C / L, a
+// A pooled slot against its pool (include/sonicsim_b200.h): no source fields of its own, the pool's mode / C / L (the
+// longest candidate's), a
 // window every candidate holds, a direct target only when every candidate's bank has the slot's direct set.
 static int validate_pooled(const ss_ctx* c, const ss_source& it) {
     const ss_pool* pl = it.pool;
@@ -910,6 +915,7 @@ struct Shape {
     int p_max;                // rstep entries: P, or the largest candidate's P for a pooled slot
     // time window (win_len > 0); zero otherwise
     int win;
+    int pooled;               // a pooled slot (shape_pooled)
     int tab_host;             // the window's blocks are known here (all but aligned blocking over device-side bounds)
     int g0, g1, k0, k1;       // tab_host: full-table blocks in the table / meeting the window (window_span)
     int row0, rows;           // RIR rows transformed per set (window_rows)
@@ -1001,13 +1007,13 @@ static Shape shape_of(const ss_source& it) {
     return s;
 }
 // A pooled slot: a moving window (tables built by k_blocks, the whole candidate read) under the pool's blocking, sized
-// once for the largest table, position count and item count any candidate needs.  The table sizes are worked out once
-// per pool and window length.
+// once for the largest table (each candidate with its own K), position count and item count any candidate needs.  The
+// table sizes are worked out once per pool and window length.  K is the pool's largest: it picks the kernel variant.
 static Shape shape_pooled(const ss_source& it) {
     ss_pool* pl = const_cast<ss_pool*>(it.pool);
     Shape s;
     memset(&s, 0, sizeof(s));
-    s.K = pl->K; s.aligned = pl->aligned; s.win = 1; s.p_max = pl->p_max;
+    s.K = pl->K; s.aligned = pl->aligned; s.win = 1; s.pooled = 1; s.p_max = pl->p_max;
     s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
     s.nblk_max = -1;
     for (const auto& q : pl->caps) if (q.first == it.win_len) s.nblk_max = q.second;
@@ -1021,8 +1027,8 @@ static Shape shape_pooled(const ss_source& it) {
             if (pl->mode == SS_MOVING_BOUNDS) bounds.push_back(pl->bounds_host.data() + pl->bounds_off[i]);
         }
         std::vector<Block> full((size_t)cap_max);
-        s.nblk_max = pool_table_cap(pl->aligned, bounds.empty() ? nullptr : bounds.data(), N.data(), P.data(), pl->n,
-                                    it.win_len, pl->K, full.data());
+        s.nblk_max = pool_table_cap(pl->aligned, bounds.empty() ? nullptr : bounds.data(), N.data(), P.data(),
+                                    pl->parts_host.data(), pl->n, it.win_len, pl->K, full.data());
         pl->caps.push_back({it.win_len, s.nblk_max});
     }
     s.max_items = s.nblk_max * s.per;
@@ -1102,8 +1108,9 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
     return true;
 }
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
-// block table, so that they always travel in the descriptor block
-static size_t counts_bytes(const Shape& sh) { return sh.win ? 64 : 16; }
+// block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts),
+// padded to 80 bytes
+static size_t counts_bytes(const Shape& sh) { return sh.pooled ? 80 : sh.win ? 64 : 16; }
 static const float kUnitGain = 1.0f;      // counts[11] of every windowed source until a pooled slot picks (stem_gain)
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
 // counts (windowed source, device-built tables)
@@ -1149,7 +1156,9 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
         s.K = sh.K; s.nb = sh.nb; s.mode = it.mode; s.aligned = sh.aligned; s.nblk_max = sh.nblk_max;
         if (it.flags & SS_DIRECT_TARGET) { s.out_direct = it.out_direct; s.direct_taps = it.direct_taps; }
         if (it.pool) {
-            // candidate 0 until k_blocks writes the pick of each run over it
+            // candidate 0 until k_blocks writes the pick of each run over it (the kernel variant below stays the Shape's:
+            // the pool's largest K)
+            s.K = it.pool->parts_host[0];
             pick_candidate(s, it.pool->host[0]);
             any_pooled = true;
             L->any_gain = L->any_gain || it.pool->gains;
@@ -1193,11 +1202,12 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                 hb_counts[4] = it.win_start; hb_counts[5] = it.win_len;
                 memcpy(hb_counts + 6, &it.win_start_dev, sizeof(it.win_start_dev));      // win_start_ptr
                 memcpy(hb_counts + 11, &kUnitGain, sizeof(kUnitGain));                  // stem_gain until k_blocks picks
-                if (it.pool) {                                          // pool_table, pool_size, pick_ptr, pool_gains
+                if (it.pool) {                              // pool_table, pool_size, pick_ptr, pool_gains, pool_parts
                     memcpy(hb_counts + 8, &it.pool->table, sizeof(it.pool->table));
                     hb_counts[10] = it.pool->n;
                     memcpy(hb_counts + 12, &it.pick_dev, sizeof(it.pick_dev));
                     memcpy(hb_counts + 14, &it.pool->gains, sizeof(it.pool->gains));
+                    memcpy(hb_counts + 16, &it.pool->parts, sizeof(it.pool->parts));
                 }
             } else {
                 s.counts = (int*)scratch;
@@ -1208,8 +1218,8 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
         hps[i] = ps;
         ps += spectra_pairs_h(s) + spectra_pairs_x(s) + range_ctas(s);
         pr += sh.max_items;
-        any_long = any_long || s.K > 1;
-        all_aligned = all_aligned && one_transform_per_item(s.aligned, s.mode, s.K);
+        any_long = any_long || sh.K > 1;
+        all_aligned = all_aligned && one_transform_per_item(sh.aligned, it.mode, sh.K);
     }
     hps[n] = ps;
     // work-item table of the whole chunk (dense) + its length
@@ -1390,6 +1400,7 @@ extern "C" void ss_pool_destroy(ss_pool* pl) {
     cudaSetDevice(pl->c->device);
     cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
     if (pl->table) cudaFree(pl->table);
+    if (pl->parts) cudaFree(pl->parts);
     if (pl->levels) cudaFree(pl->levels);
     if (pl->level_ptr) cudaFree(pl->level_ptr);
     if (pl->gains) cudaFree(pl->gains);
@@ -1399,6 +1410,7 @@ extern "C" void ss_pool_destroy(ss_pool* pl) {
 extern "C" int64_t ss_pool_bytes(const ss_pool* pl) {
     if (!pl) return 0;
     int64_t b = (int64_t)sizeof(PoolEntry) * pl->n;
+    if (pl->parts) b += (int64_t)sizeof(int) * pl->n;
     if (pl->levels) b += (int64_t)sizeof(double) * pl->level_off[pl->n] + (int64_t)sizeof(double*) * pl->n;
     if (pl->gains) b += (int64_t)sizeof(float) * pl->n;
     return b;
@@ -1410,9 +1422,10 @@ extern "C" const double* ss_pool_level_table(const ss_pool* pl, int i) {
 static int pool_build(ss_pool* pl, const ss_source* cand) {
     ss_ctx* c = pl->c;
     const ss_source& a = cand[0];
-    pl->mode = a.mode; pl->C = a.C; pl->L = a.L; pl->K = (a.L + kB - 1) / kB; pl->aligned = 1;
+    pl->mode = a.mode; pl->C = a.C; pl->L = a.L; pl->K = a.rir_bank->K; pl->aligned = 1;
     pl->n_min = a.N; pl->direct_taps = a.rir_bank->cut ? a.rir_bank->direct_taps : 0;
     pl->host.resize(pl->n);
+    pl->parts_host.resize(pl->n);
     if (pl->mode == SS_MOVING_BOUNDS) pl->bounds_off.resize(pl->n);
     std::vector<ss_bank*> banks;
     for (int i = 0; i < pl->n; ++i) {
@@ -1423,9 +1436,10 @@ static int pool_build(ss_pool* pl, const ss_source* cand) {
         e.N = it.N; e.P = it.P;
         pl->host[i] = e;
         pl->n_min = std::min(pl->n_min, it.N); pl->p_max = std::max(pl->p_max, it.P);
+        pl->L = std::max(pl->L, it.L); pl->K = std::max(pl->K, b->K); pl->parts_host[i] = b->K;
         if (pl->direct_taps != (b->cut ? b->direct_taps : 0)) pl->direct_taps = 0;
-        // the pool's blocking: aligned only if every candidate would choose it
-        if (!choose_aligned(it, pl->K, (it.N + kB - 1) / kB)) pl->aligned = 0;
+        // the pool's blocking: aligned only if every candidate would choose it with its own K
+        if (!choose_aligned(it, b->K, (it.N + kB - 1) / kB)) pl->aligned = 0;
         if (pl->mode == SS_MOVING_BOUNDS) {
             pl->bounds_off[i] = (int64_t)pl->bounds_host.size();
             pl->bounds_host.insert(pl->bounds_host.end(), it.bounds_host, it.bounds_host + it.P);
@@ -1435,6 +1449,10 @@ static int pool_build(ss_pool* pl, const ss_source* cand) {
     }
     CK(cudaMalloc((void**)&pl->table, sizeof(PoolEntry) * (size_t)pl->n));
     CK(cudaMemcpy(pl->table, pl->host.data(), sizeof(PoolEntry) * (size_t)pl->n, cudaMemcpyHostToDevice));
+    if (std::any_of(pl->parts_host.begin(), pl->parts_host.end(), [&](int k) { return k != pl->K; })) {
+        CK(cudaMalloc((void**)&pl->parts, sizeof(int) * (size_t)pl->n));
+        CK(cudaMemcpy(pl->parts, pl->parts_host.data(), sizeof(int) * (size_t)pl->n, cudaMemcpyHostToDevice));
+    }
     // one event behind every bank's construction: a plan run waits once per pool, not once per candidate bank
     CK(cudaEventCreateWithFlags(&pl->ready, cudaEventDisableTiming));
     cudaStream_t s = nullptr;
@@ -1458,7 +1476,7 @@ extern "C" int ss_pool_create(ss_ctx* c, const ss_source* cand, int n, ss_pool**
     for (int i = 0; i < n; ++i) {
         const int st = validate_candidate(c, cand[i]);
         if (st) return st;
-        if (cand[i].mode != cand[0].mode || cand[i].C != cand[0].C || cand[i].L != cand[0].L) return SS_ERR_INVALID;
+        if (cand[i].mode != cand[0].mode || cand[i].C != cand[0].C) return SS_ERR_INVALID;   // any L
     }
     CK(cudaSetDevice(c->device));
     ss_pool* pl = new (std::nothrow) ss_pool();
@@ -1677,7 +1695,7 @@ static int render_stem_groups(ss_pool* pl, const StemGroups& G, char* tmp, cudaS
         for (int i = G.first[g]; i < G.first[g + 1]; ++i) {
             const PoolEntry& e = pl->host[i];
             ss_source it; memset(&it, 0, sizeof(it));
-            it.x = e.x; it.out = (float*)(tmp + G.at[i]); it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->L;
+            it.x = e.x; it.out = (float*)(tmp + G.at[i]); it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->banks[i]->L;
             it.mode = pl->mode; it.rir_bank = pl->banks[i];
             if (pl->mode == SS_MOVING_BOUNDS) { it.bounds = e.bounds; it.bounds_host = pl->bounds_host.data() + pl->bounds_off[i]; }
             items.push_back(it);

@@ -43,8 +43,8 @@ struct Source {
     int* counts;           // scratch: [0] = blocks in use, [1] = index of this source's first render item; windowed
                            // source (h_rows != 0): [2] = first block that meets the window, [3] = blocks that do,
                            // [4] = win_start, [5] = win_len, [6..7] = device pointer of a moving window's start or
-                           // null (win_start_ptr); tables built on the device: [8..13] the pool of a pooled slot
-                           // (pool_table, pool_size, pick_ptr)
+                           // null (win_start_ptr); tables built on the device: [8..17] the pool of a pooled slot
+                           // (pool_table, pool_size, pick_ptr, pool_gains, pool_parts)
     const float* norm_part;// scratch: kNormParts partial abs-maxima of the RIR tensor (k_rir_absmax), or null: taps used as given
     int* cut;              // scratch: P*C direct-path row lengths (k_rir_direct), or null: no direct target
     float* out_direct;     // (C, N) direct-path stem (with `cut`)
@@ -247,8 +247,8 @@ struct PoolEntry {
     int N, P;
 };
 static_assert(sizeof(PoolEntry) == 40, "PoolEntry layout");
-// A pooled slot's counts (counts_bytes = 64 for every windowed source whose tables k_blocks builds): [8..9] the pool's
-// device table or null (not pooled), [10] its candidate count, [12..13] the device pointer of the pick
+// A pooled slot's counts (counts_bytes = 64 for every windowed source whose tables k_blocks builds, 80 for a pooled slot):
+// [8..9] the pool's device table or null (not pooled), [10] its candidate count, [12..13] the device pointer of the pick
 SS_HD const PoolEntry* pool_table(const Source& s) { return *reinterpret_cast<const PoolEntry* const*>(s.counts + 8); }
 SS_HD int pool_size(const Source& s) { return s.counts[10]; }
 SS_HD const int* pick_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 12); }
@@ -277,19 +277,35 @@ SS_HD void pick_slot(Source& s, int v, bool& bad) {
     const float* const g = pool_gains(s);
     set_stem_gain(s, g ? g[i] : 1.0f);
 }
+// Candidates of one pool may differ in L.  A pool whose candidates differ in K (RIR partitions) keeps a device array of
+// their n partition counts; a pooled slot's counts block is 80 bytes, and [16..17] hold that array's device pointer, or
+// null (a uniform pool: the slot keeps the pool's K).  The head of k_blocks sets the slot's K to the picked candidate's
+// (pick_parts) before pick_slot, whose set_banked derives h_rows = P*C*K from it; the window search, the block table and
+// fill_items (kparts, pstride, the direct set's offset) then follow the picked K.
+SS_HD const int* pool_parts(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 16); }
+SS_HD void pick_parts(Source& s, int v) {
+    const int* const k = pool_parts(s);
+    bool bad;
+    if (k) s.K = k[clamp_pick(v, pool_size(s), bad)];
+}
 // Table size of a pooled slot with windows of win_len: the largest window_table_cap over the candidates' full plans under
 // the pool's blocking (bounds[i]: candidate i's host bounds, null for a static pool), so that the table holds the blocks
-// of every candidate at every start.  `full` holds table_cap(aligned, nb, P) blocks of the largest candidate.
-SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, const int* P, int n, int win_len, int K,
-                         Block* full) {
+// of every candidate at every start.  Candidate i has Ks[i] RIR partitions (g1 - g0 grows with K), or K when Ks is null.
+// `full` holds table_cap(aligned, nb, P) blocks of the largest candidate.
+SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, const int* P, const int* Ks, int n,
+                         int win_len, int K, Block* full) {
     int best = 0;
     for (int i = 0; i < n; ++i) {
         const int nb = (N[i] + kB - 1) / kB, cap = table_cap(aligned, nb, P[i]);
         const int nfull = plan_blocks(aligned, bounds ? bounds[i] : nullptr, P[i], N[i], nb, 0, cap, full);
-        const int c = window_table_cap(full, nfull < cap ? nfull : cap, N[i], win_len, K, P[i], cap);
+        const int c = window_table_cap(full, nfull < cap ? nfull : cap, N[i], win_len, Ks ? Ks[i] : K, P[i], cap);
         best = c > best ? c : best;
     }
     return best;
+}
+SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, const int* P, int n, int win_len, int K,
+                         Block* full) {
+    return pool_table_cap(aligned, bounds, N, P, nullptr, n, win_len, K, full);
 }
 // ---- crop start draws of device plans (ss_plan_draw, include/sonicsim_b200.h): the dataloader's start loop
 // (movingdatamodule.py:81-99) over level tables Q (ss_pool_levels: Q[0] = 0, Q[n + 1] = Q[n] + e[n], float64).

@@ -242,13 +242,14 @@ class RirBank(_Held):
 
 class SourcePool(_Held):
     """A set of banked candidate sources validated and uploaded once (Renderer.source_pool; ss_pool of the C ABI), which
-    pooled slots (render.Pooled) of device plans pick from at every run.  `n` candidates of one `mode`, `C` and `L`;
-    `n_min` is the shortest candidate's N (the longest window a slot may take); `direct_taps` > 0 when every candidate's
+    pooled slots (render.Pooled) of device plans pick from at every run.  `n` candidates of one `mode` and `C`; `L` is
+    the longest candidate's RIR length (candidates may differ in L, each keeps its own bank); `n_min` is the shortest candidate's N (the longest window a slot may take); `direct_taps` > 0 when every candidate's
     bank holds a direct set with these taps.  The pool holds its candidates' banks and keeps their tensors alive; plans
     hold the pool, which is freed once it is closed (or collected) and no live plan uses it any more.  `levels` is None,
     "mono" or "channels": the level tables the pool holds for start draws (CropDraw), included in `nbytes`.
     `loudness` is an (n, 2) float64 array of every candidate's measured integrated loudness (LUFS) and linear gain
-    (ss_pool_loudness), NaN for a candidate without a target; `nbytes` includes the gains (4 bytes per candidate)."""
+    (ss_pool_loudness), NaN for a candidate without a target; `nbytes` includes the gains (4 bytes per candidate), and
+    the candidates' partition counts (4 bytes per candidate) when their K = ceil(L / 4096) differ (ss_pool_bytes)."""
 
     def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None, loudness=None):
         self.renderer, self._h = renderer, handle
@@ -328,7 +329,7 @@ def _bank_of(renderer, s, i, P, C, L):
 
 
 def _kind(k):
-    return ("static" if k[0] == _lib.SS_STATIC else "moving", k[1], k[2])
+    return ("static" if k[0] == _lib.SS_STATIC else "moving", k[1])
 
 
 def _refuse_pooled(sources, where):
@@ -446,8 +447,10 @@ class Renderer:
         """Validate and upload a set of candidate sources once, for pooled slots (render.Pooled) of device plans to pick
         from at every run.  Every candidate is a MovingSource or StaticSource whose RIRs are a RirBank of this renderer
         (`dry`, `bounds`: contiguous CUDA tensors of its device; a moving candidate needs `bounds_host`), with no window,
-        normalize_rirs or direct_taps (those belong to the slot and the bank); all share one kind (moving or static), C
-        and L.  The candidates' tensors and banks are kept alive by the pool.
+        normalize_rirs or direct_taps (those belong to the slot and the bank); all share one kind (moving or static) and
+        C, and may differ in L (e.g. the speakers of one formats.load_rir_dump, each with its own length): a slot that
+        picks a candidate renders it with that candidate's own RIR partitions.  The pool's L, which its slots are given,
+        is the longest candidate's.  The candidates' tensors and banks are kept alive by the pool.
 
         `levels` = "mono" or "channels" also builds every candidate's level table (ss_pool_levels: the float64 prefix
         sums of the squares of its whole rendered stem, channel-folded like Mixture(mono=True) for "mono"), which
@@ -468,7 +471,7 @@ class Renderer:
         _check_lufs("source_pool", "candidate", lufs_targets, n, sr)
         items = (SsSource * n)()
         keep = []
-        first = None
+        first, L_max = None, 0
         for i, s in enumerate(candidates):
             if not isinstance(s, (MovingSource, StaticSource)):
                 raise ValueError("source_pool: candidate %d must be a MovingSource or StaticSource, got %s"
@@ -480,12 +483,13 @@ class Renderer:
             if s.window is not None or s.normalize_rirs or int(s.direct_taps):
                 raise ValueError("source_pool: candidate %d has a window, normalize_rirs or direct_taps; those belong to "
                                  "the pooled slot (render.Pooled) and the bank" % i)
-            kind = (mode, C, L)
+            kind = (mode, C)
             if first is None:
                 first = kind
             elif kind != first:
-                raise ValueError("source_pool: candidate %d is (%s, C=%d, L=%d), candidate 0 (%s, C=%d, L=%d): every "
-                                 "candidate has one kind, C and L" % ((i,) + _kind(kind) + _kind(first)))
+                raise ValueError("source_pool: candidate %d is (%s, C=%d), candidate 0 (%s, C=%d): every candidate has "
+                                 "one kind and C (L may differ)" % ((i,) + _kind(kind) + _kind(first)))
+            L_max = max(L_max, L)
             own = "candidate %d" % i
             x = _tensor(s.dry, "source_pool", own, "dry", torch.float32, self.device)
             items[i] = SsSource(x=x, N=s.dry.numel(), P=P, C=C, L=L, mode=mode, rir_bank=rb._h.value)
@@ -509,7 +513,7 @@ class Renderer:
             self.lib.ss_pool_destroy(h)
             _lib.check(st)
         taps = {_rirs(s)[0].direct_taps for s in candidates}
-        return SourcePool(self, h, candidates, first[0], first[1], first[2], min(s.dry.numel() for s in candidates),
+        return SourcePool(self, h, candidates, first[0], first[1], L_max, min(s.dry.numel() for s in candidates),
                           taps.pop() if len(taps) == 1 else 0, levels, loud)
 
     # ------------------------------------------------------------------ host buffers
