@@ -175,6 +175,15 @@ int ss_bank_create_host(ss_ctx* ctx, const float* rir, int32_t P, int32_t C, int
 int64_t ss_bank_bytes(const ss_bank* bank);   /* device bytes held */
 void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their context */
 
+/* ---- host banks: `flags` of ss_bank_create_dev / _host may add SS_BANK_HOST.  The bank is transformed by the same
+ * launches into a transient device buffer, then moved into pinned, mapped host memory (cudaHostAllocMapped) - spectra and
+ * cut table alike - and the device buffer is freed: its spectra are bit-identical to a device bank's of the same RIRs,
+ * ss_bank_bytes is 0 and ss_bank_host_bytes reports the 8 * 4096 * P * C * K bytes per set plus the cut table.  Both
+ * create calls return only when the bank is in host memory.  A host bank serves only as a candidate of a host pool
+ * (below): ss_render_dev, ss_render_host / _ex and ss_plan_create* refuse a source that names one (SS_ERR_INVALID). */
+#define SS_BANK_HOST 0x100
+int64_t ss_bank_host_bytes(const ss_bank* bank);   /* pinned host bytes held */
+
 /* ---- source pools (version 106): the dataloader's random choices of separation/look2hear/datas/movingdatamodule.py
  * :57-59 (`random.choice(self.data_dirs)`, `random.sample(range(1, 4), num_spks)`) and :68-77 (the scene's noise) made
  * on the device.  A pool is a set of banked candidate sources, validated and uploaded once.  A pooled slot of a plan
@@ -230,6 +239,28 @@ int64_t ss_pool_bytes(const ss_pool* pool);   /* device bytes held: n compact ca
                                                * float gains (4 B each) once ss_pool_loudness measured them, and the
                                                * level tables with their pointer array once ss_pool_levels built them */
 void ss_pool_destroy(ss_pool* pool);          /* destroy pools after the plans that use them, before their context */
+
+/* ---- host pools: a pool whose candidates all have host banks (SS_BANK_HOST) is a host pool; a pool that mixes host and
+ * device banks is SS_ERR_INVALID.  Its bulk stays in pinned host memory and every plan run copies only what its slots
+ * read into device memory, so that a pool's device footprint is O(n * P) bytes whatever its dry signals and banks hold.
+ *   - ss_pool_create copies every candidate's `x` (a host or a device pointer) into one pinned, mapped arena that the pool
+ *     owns, uploads each moving candidate's bounds_host into a device array of its own (`bounds` may then be NULL), and
+ *     uploads the direct-path cut tables (P * C ints per candidate whose bank has a direct set).  Unlike a device pool,
+ *     the caller's x and bounds buffers need not outlive the pool: only the banks must.
+ *   - ss_pool_levels puts the tables in pinned, mapped host memory (ss_pool_level_table then returns a mapped host
+ *     address, which the device reads over PCIe); ss_pool_levels and ss_pool_loudness render each stem group from
+ *     transient device copies of its banks and dry signals, in batches of at most 256 MB (or one candidate's, when
+ *     larger), so that a build's transient device memory is bounded whatever n is.
+ *   - In a plan, every pooled slot of a host pool gets a staging area in device memory, sized once at creation for the
+ *     most RIR rows (both sets with a direct target) and dry samples any candidate's window of this length reads at any
+ *     start.  At every run one more kernel, k_stage, launched after the start draws and before any render, reads each
+ *     such slot's pick (clamped, bit 3) and start, and copies the picked candidate's read set from host memory into the
+ *     staging area: the dry samples [ws - (K + 2) * 4096, ws + win_len + 2 * 4096) and the RIR rows of every position
+ *     they reach.  The slot then renders from the staged copies with the bits of the same slot over a device pool.
+ *   - ss_pool_bytes keeps counting device bytes: for a host pool the n entries, the partition counts and gains as for a
+ *     device pool, the device copies of the bounds (4 * P bytes per moving candidate) and cut tables, and the level
+ *     tables' pointer array; ss_pool_host_bytes counts the arena and the level tables. */
+int64_t ss_pool_host_bytes(const ss_pool* pool);   /* pinned host bytes held (0 for a device pool) */
 
 /* ---- level tables of a pool (version 107), for the start draws of plans (ss_plan_draw below).  Gives every candidate
  * of the pool a table from which the energy of any crop is two loads:

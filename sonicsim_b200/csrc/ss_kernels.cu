@@ -123,11 +123,16 @@ k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
         int g0 = 0, g1 = S.nblk_max;
         if (S.h_rows) {
             if (pool_table(S) && lane == 0) {
-                bool bad;
-                const int v = *pick_ptr(S);
-                pick_parts(S, v);                       // the picked candidate's K first: set_banked reads it
-                pick_slot(S, v, bad);
-                if (bad) atomicOr(&g_dev_err, 8u);
+                const StageView* const sv = stage_view(S);
+                if (sv) {
+                    take_view(S, *sv);                  // a host pool: k_stage picked (bit 3) and staged the candidate
+                } else {
+                    bool bad;
+                    const int v = *pick_ptr(S);
+                    pick_parts(S, v);                   // the picked candidate's K first: set_banked reads it
+                    pick_slot(S, v, bad);
+                    if (bad) atomicOr(&g_dev_err, 8u);
+                }
             }
             __syncwarp();
             const int* const ws_dev = win_start_ptr(S);
@@ -796,6 +801,9 @@ struct ss_bank {
     int* cut = nullptr;                   // P*C direct-path row lengths, or null: no direct set
     int P = 0, C = 0, L = 0, K = 0, flags = 0, direct_taps = 0;
     cudaEvent_t ready = nullptr;          // recorded behind the launches that build it; every use waits on it
+    // SS_BANK_HOST: spectra and cut table moved into pinned, mapped host memory (spec / cut: their device addresses)
+    char* h_mem = nullptr;
+    size_t host_bytes = 0;
 };
 // Source pool: the candidates' compact entries in one device allocation, and on the host what validation, sizing and the
 // mixture range checks need.
@@ -815,6 +823,7 @@ struct ss_pool {
     cudaEvent_t ready = nullptr;          // behind the construction of every candidate's bank
     // level tables (ss_pool_levels): every candidate's N + 1 doubles back to back, and a device array of n pointers
     double* levels = nullptr;
+    double* h_levels = nullptr;           // a host pool's tables: their host address (levels: their device address)
     const double** level_ptr = nullptr;
     std::vector<int64_t> level_off;       // candidate i's table at levels + level_off[i]
     int level_flags = -1;                 // SS_MIX_MONO or 0 once the tables exist
@@ -823,6 +832,14 @@ struct ss_pool {
     float* gains = nullptr;
     std::vector<double> loud;
     bool planned = false;                 // a plan has been created over the pool: its gains may no longer change
+    // host pool (every candidate's bank has SS_BANK_HOST): x in one pinned, mapped arena (host[i].x: its device address);
+    // the device copies of the bounds and cut tables in one device allocation (host[i].bounds / cut point into it)
+    bool host_res = false;
+    char* h_x = nullptr;
+    size_t h_x_bytes = 0;
+    int* d_aux = nullptr;
+    size_t aux_bytes = 0;
+    std::vector<std::pair<int, std::pair<int, int>>> stage_caps;  // (win_len, (rows, dry samples)) (stage_cap)
 };
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
@@ -840,13 +857,15 @@ static int wait_banks(const ss_source* items, int n, cudaStream_t stream) {
 // A banked source against its bank (include/sonicsim_b200.h): same shape, normalisation left to the bank, a direct
 // target only with the bank's direct set and taps.  (A static source has P == 1 and a moving one P >= 2, checked by
 // validate_item, so the shape check also gives the bank's P the source's mode.)
-static int validate_bank_use(const ss_source& it) {
+static int bank_fits(const ss_source& it) {
     const ss_bank* b = it.rir_bank;
     if (it.P != b->P || it.C != b->C || it.L != b->L) return SS_ERR_INVALID;
     if (it.flags & SS_RIR_NORMALIZE) return SS_ERR_INVALID;
     if ((it.flags & SS_DIRECT_TARGET) && (!b->cut || it.direct_taps != b->direct_taps)) return SS_ERR_INVALID;
     return SS_OK;
 }
+// a source rendered from a bank: a host bank (SS_BANK_HOST) serves only as a candidate of a host pool
+static int validate_bank_use(const ss_source& it) { return it.rir_bank->h_mem ? SS_ERR_INVALID : bank_fits(it); }
 static int validate_item(const ss_source& it) {
     if (it.pool || it.pick_dev) return SS_ERR_INVALID;              // pooled slots: plans only (validate_pooled)
     if (!it.x || !it.out || (it.rir != nullptr) == (it.rir_bank != nullptr)) return SS_ERR_INVALID;   // rir xor bank
@@ -1108,8 +1127,8 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
     return true;
 }
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
-// block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts),
-// padded to 80 bytes
+// block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts) and
+// [18..19] (stage_view), 80 bytes
 static size_t counts_bytes(const Shape& sh) { return sh.pooled ? 80 : sh.win ? 64 : 16; }
 static const float kUnitGain = 1.0f;      // counts[11] of every windowed source until a pooled slot picks (stem_gain)
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
@@ -1131,7 +1150,7 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
 // Fill the descriptor block of items[first, last) at `hbase` (host memory) for its device address `dbase`, carve the
 // chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.
 static void chunk_describe(const ss_source* items, const Shape* shapes, int first, int last, char* hbase, char* dbase,
-                           char* scratch, int sm_count, ChunkLaunch* L) {
+                           char* scratch, int sm_count, ChunkLaunch* L, StageView* const* views = nullptr) {
     const int n = last - first;
     const bool host_tables = chunk_host_tables(items, first, last);
     const size_t off_ps = align_up(sizeof(Source) * n, 16);
@@ -1208,6 +1227,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                     memcpy(hb_counts + 12, &it.pick_dev, sizeof(it.pick_dev));
                     memcpy(hb_counts + 14, &it.pool->gains, sizeof(it.pool->gains));
                     memcpy(hb_counts + 16, &it.pool->parts, sizeof(it.pool->parts));
+                    if (views) memcpy(hb_counts + 18, &views[first + i], sizeof(StageView*));   // stage_view
                 }
             } else {
                 s.counts = (int*)scratch;
@@ -1292,7 +1312,7 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, b
 // chunk scratch.  Its spectra therefore have the bits a render would transform itself.
 static int bank_args(const ss_ctx* c, const float* rir, int P, int C, int L, int flags, int direct_taps, ss_bank** out) {
     if (!c || !rir || !out || P < 1 || C < 1 || L < 1) return SS_ERR_INVALID;
-    if (flags & ~(SS_RIR_NORMALIZE | SS_DIRECT_TARGET)) return SS_ERR_INVALID;
+    if (flags & ~(SS_RIR_NORMALIZE | SS_DIRECT_TARGET | SS_BANK_HOST)) return SS_ERR_INVALID;
     if ((flags & SS_DIRECT_TARGET) && direct_taps < 1) return SS_ERR_INVALID;
     if ((int64_t)P * C * ((L + kB - 1) / kB) > (int64_t)1 << 28) return SS_ERR_UNSUPPORTED;    // as validate_item
     return SS_OK;
@@ -1329,6 +1349,24 @@ static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stre
     CK(cudaEventRecord(b->ready, stream));
     return SS_OK;
 }
+// SS_BANK_HOST: the built spectra and cut table into pinned, mapped host memory, then the device buffer freed.  Returns
+// when the bank is in host memory.
+static int bank_to_host(ss_bank* b, cudaStream_t stream) {
+    const size_t spec_b = ((b->flags & SS_DIRECT_TARGET) ? 2 : 1) * (size_t)b->P * b->C * b->K * kSpec * sizeof(float2);
+    const size_t cut_b = b->cut ? sizeof(int) * (size_t)b->P * b->C : 0;
+    CK(cudaHostAlloc((void**)&b->h_mem, spec_b + cut_b, cudaHostAllocMapped | cudaHostAllocPortable));
+    b->host_bytes = spec_b + cut_b;
+    CK(cudaMemcpyAsync(b->h_mem, b->spec, spec_b, cudaMemcpyDeviceToHost, stream));
+    if (cut_b) CK(cudaMemcpyAsync(b->h_mem + spec_b, b->cut, cut_b, cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    CK(cudaFree(b->d_mem));
+    b->d_mem = nullptr; b->bytes = 0;
+    char* dev = nullptr;
+    CK(cudaHostGetDevicePointer((void**)&dev, b->h_mem, 0));
+    b->spec = (float2*)dev;
+    b->cut = cut_b ? (int*)(dev + spec_b) : nullptr;
+    return SS_OK;
+}
 
 // Waits for the whole device: a render that used the bank may run on any stream of the caller (cudaFree would wait for
 // the device anyway).
@@ -1337,10 +1375,12 @@ extern "C" void ss_bank_destroy(ss_bank* b) {
     cudaSetDevice(b->c->device);
     cudaDeviceSynchronize();
     if (b->d_mem) cudaFree(b->d_mem);
+    if (b->h_mem) cudaFreeHost(b->h_mem);
     if (b->ready) cudaEventDestroy(b->ready);
     delete b;
 }
 extern "C" int64_t ss_bank_bytes(const ss_bank* b) { return b ? (int64_t)b->bytes : 0; }
+extern "C" int64_t ss_bank_host_bytes(const ss_bank* b) { return b ? (int64_t)b->host_bytes : 0; }
 
 extern "C" int ss_bank_create_dev(ss_ctx* c, const float* rir, int32_t P, int32_t C, int32_t L, int32_t flags,
                                   int32_t direct_taps, void* stream, ss_bank** out) {
@@ -1351,7 +1391,8 @@ extern "C" int ss_bank_create_dev(ss_ctx* c, const float* rir, int32_t P, int32_
     if (!b) return SS_ERR_NOMEM;
     b->c = c; b->P = P; b->C = C; b->L = L; b->K = (L + kB - 1) / kB; b->flags = flags;
     b->direct_taps = (flags & SS_DIRECT_TARGET) ? direct_taps : 0;
-    const int st = bank_build(c, b, rir, (cudaStream_t)stream);
+    int st = bank_build(c, b, rir, (cudaStream_t)stream);
+    if (st == SS_OK && (flags & SS_BANK_HOST)) st = bank_to_host(b, (cudaStream_t)stream);
     if (st != SS_OK) { ss_bank_destroy(b); return st; }
     *out = b;
     return SS_OK;
@@ -1390,33 +1431,83 @@ static int validate_candidate(const ss_ctx* c, const ss_source& it) {
     if (it.N > 0x7fffffff - 2 * kF) return SS_ERR_INVALID;                 // as validate_item
     if (it.mode == SS_STATIC) { if (it.P != 1 || it.bounds || it.bounds_host) return SS_ERR_INVALID; }
     else if (it.mode == SS_MOVING_BOUNDS) {
-        if (it.P < 2 || !it.bounds || !it.bounds_host || !bounds_ok(it.bounds_host, it.P, it.N)) return SS_ERR_INVALID;
+        // (a host pool uploads bounds_host itself: its candidates need no device bounds)
+        if (it.P < 2 || (!it.bounds && !it.rir_bank->h_mem) || !it.bounds_host || !bounds_ok(it.bounds_host, it.P, it.N))
+            return SS_ERR_INVALID;
     } else return SS_ERR_INVALID;
-    return validate_bank_use(it);
+    return bank_fits(it);
 }
 
+// the level tables (pinned, mapped host memory in a host pool) and their pointer array
+static void free_levels(ss_pool* pl) {
+    if (pl->levels) { if (pl->host_res) cudaFreeHost(pl->h_levels); else cudaFree(pl->levels); }
+    if (pl->level_ptr) cudaFree(pl->level_ptr);
+    pl->levels = nullptr; pl->h_levels = nullptr; pl->level_ptr = nullptr;
+}
 extern "C" void ss_pool_destroy(ss_pool* pl) {
     if (!pl) return;
     cudaSetDevice(pl->c->device);
     cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
     if (pl->table) cudaFree(pl->table);
     if (pl->parts) cudaFree(pl->parts);
-    if (pl->levels) cudaFree(pl->levels);
-    if (pl->level_ptr) cudaFree(pl->level_ptr);
+    free_levels(pl);
     if (pl->gains) cudaFree(pl->gains);
     if (pl->ready) cudaEventDestroy(pl->ready);
+    if (pl->h_x) cudaFreeHost(pl->h_x);
+    if (pl->d_aux) cudaFree(pl->d_aux);
     delete pl;
 }
+static size_t level_bytes(const ss_pool* pl) { return sizeof(double) * (size_t)pl->level_off[pl->n]; }
 extern "C" int64_t ss_pool_bytes(const ss_pool* pl) {
     if (!pl) return 0;
     int64_t b = (int64_t)sizeof(PoolEntry) * pl->n;
     if (pl->parts) b += (int64_t)sizeof(int) * pl->n;
-    if (pl->levels) b += (int64_t)sizeof(double) * pl->level_off[pl->n] + (int64_t)sizeof(double*) * pl->n;
+    if (pl->levels) b += (pl->host_res ? 0 : (int64_t)level_bytes(pl)) + (int64_t)sizeof(double*) * pl->n;
     if (pl->gains) b += (int64_t)sizeof(float) * pl->n;
-    return b;
+    return b + (int64_t)pl->aux_bytes;
+}
+extern "C" int64_t ss_pool_host_bytes(const ss_pool* pl) {
+    return pl && pl->host_res ? (int64_t)(pl->h_x_bytes + (pl->levels ? level_bytes(pl) : 0)) : 0;
 }
 extern "C" const double* ss_pool_level_table(const ss_pool* pl, int i) {
     return pl && pl->levels && i >= 0 && i < pl->n ? pl->levels + pl->level_off[i] : nullptr;
+}
+
+// Host pool: the candidates' x into the pool's pinned, mapped arena (each at a 64-byte boundary, zero-padded to a multiple
+// of 4 samples: k_stage copies whole float4s), bounds_host and the banks' cut tables into one device allocation; the
+// entries point at the device addresses of both.
+static int pool_host_copies(ss_pool* pl, const ss_source* cand) {
+    const int n = pl->n;
+    std::vector<size_t> xo(n + 1, 0), ao(n + 1, 0);
+    for (int i = 0; i < n; ++i) {
+        xo[i + 1] = xo[i] + align_up(sizeof(float) * (size_t)cand[i].N, 64);
+        const ss_bank* b = cand[i].rir_bank;
+        ao[i + 1] = ao[i] + (pl->mode == SS_MOVING_BOUNDS ? (size_t)cand[i].P : 0) + (b->cut ? (size_t)b->P * b->C : 0);
+    }
+    pl->h_x_bytes = xo[n];
+    CK(cudaHostAlloc((void**)&pl->h_x, pl->h_x_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+    memset(pl->h_x, 0, pl->h_x_bytes);
+    char* dx = nullptr;
+    CK(cudaHostGetDevicePointer((void**)&dx, pl->h_x, 0));
+    std::vector<int> aux(ao[n]);
+    for (int i = 0; i < n; ++i) {
+        const ss_bank* b = cand[i].rir_bank;
+        int* a = aux.data() + ao[i];
+        if (pl->mode == SS_MOVING_BOUNDS) { memcpy(a, cand[i].bounds_host, sizeof(int) * (size_t)cand[i].P); a += cand[i].P; }
+        if (b->cut) memcpy(a, b->h_mem + (size_t)((char*)b->cut - (char*)b->spec), sizeof(int) * (size_t)b->P * b->C);
+        CK(cudaMemcpy(pl->h_x + xo[i], cand[i].x, sizeof(float) * (size_t)cand[i].N, cudaMemcpyDefault));
+    }
+    pl->aux_bytes = sizeof(int) * std::max(ao[n], (size_t)1);
+    CK(cudaMalloc((void**)&pl->d_aux, pl->aux_bytes));
+    if (ao[n]) CK(cudaMemcpy(pl->d_aux, aux.data(), sizeof(int) * ao[n], cudaMemcpyHostToDevice));
+    for (int i = 0; i < n; ++i) {
+        PoolEntry& e = pl->host[i];
+        int* a = pl->d_aux + ao[i];
+        e.x = (const float*)(dx + xo[i]);
+        if (pl->mode == SS_MOVING_BOUNDS) { e.bounds = a; a += cand[i].P; }
+        e.cut = e.cut ? a : nullptr;
+    }
+    return SS_OK;
 }
 
 static int pool_build(ss_pool* pl, const ss_source* cand) {
@@ -1447,6 +1538,7 @@ static int pool_build(ss_pool* pl, const ss_source* cand) {
         if (std::find(banks.begin(), banks.end(), b) == banks.end()) banks.push_back(const_cast<ss_bank*>(b));
         pl->banks.push_back(b);
     }
+    if (pl->host_res) { int st = pool_host_copies(pl, cand); if (st) return st; }
     CK(cudaMalloc((void**)&pl->table, sizeof(PoolEntry) * (size_t)pl->n));
     CK(cudaMemcpy(pl->table, pl->host.data(), sizeof(PoolEntry) * (size_t)pl->n, cudaMemcpyHostToDevice));
     if (std::any_of(pl->parts_host.begin(), pl->parts_host.end(), [&](int k) { return k != pl->K; })) {
@@ -1477,11 +1569,12 @@ extern "C" int ss_pool_create(ss_ctx* c, const ss_source* cand, int n, ss_pool**
         const int st = validate_candidate(c, cand[i]);
         if (st) return st;
         if (cand[i].mode != cand[0].mode || cand[i].C != cand[0].C) return SS_ERR_INVALID;   // any L
+        if (!cand[i].rir_bank->h_mem != !cand[0].rir_bank->h_mem) return SS_ERR_INVALID;  // host and device banks
     }
     CK(cudaSetDevice(c->device));
     ss_pool* pl = new (std::nothrow) ss_pool();
     if (!pl) return SS_ERR_NOMEM;
-    pl->c = c; pl->n = n;
+    pl->c = c; pl->n = n; pl->host_res = cand[0].rir_bank->h_mem != nullptr;
     const int st = pool_build(pl, cand);
     if (st != SS_OK) { ss_pool_destroy(pl); return st; }
     *out = pl;
@@ -1686,9 +1779,50 @@ static StemGroups stem_groups(const ss_pool* pl) {
 }
 // Render every group into `tmp` on `s` (after the pool's banks are complete), and after each group's render enqueue
 // group(first, last) on `s`, whatever reads those stems before the next group overwrites them.  Returns when `s` is idle.
+// A host pool's candidates [first, first + n) (items, rendered whole): their reverberant spectra and dry signals copied
+// into transient device memory and rendered from there, in batches of at most kLevelStemBytes of copies (or one
+// candidate's, when larger), each behind the previous batch's render on `s`.  `buf` holds `cap` = stem_copy_cap bytes.
+static size_t stem_copy_bytes(const ss_pool* pl, int i) {
+    const ss_bank* b = pl->banks[i];
+    return align_up((size_t)b->P * b->C * b->K * kSpec * sizeof(float2), 256) + align_up(sizeof(float) * (size_t)pl->host[i].N, 256);
+}
+static size_t stem_copy_cap(const ss_pool* pl) {
+    size_t cap = 0, total = 0;
+    for (int i = 0; i < pl->n; ++i) { cap = std::max(cap, stem_copy_bytes(pl, i)); total += stem_copy_bytes(pl, i); }
+    return std::max(cap, std::min(total, kLevelStemBytes));
+}
+static int render_host_stems(ss_pool* pl, ss_source* items, int first, int n, char* buf, size_t cap, cudaStream_t s) {
+    std::vector<ss_bank> shells(n);
+    for (int lo = 0; lo < n;) {
+        size_t used = 0;
+        int hi = lo;
+        while (hi < n && (hi == lo || used + stem_copy_bytes(pl, first + hi) <= cap)) {
+            const int i = first + hi;
+            const ss_bank* b = pl->banks[i];
+            const size_t spec_b = (size_t)b->P * b->C * b->K * kSpec * sizeof(float2);
+            ss_bank& sh = shells[hi];
+            sh = *b;                                    // the bank's shape and `ready`, spectra from the copy
+            sh.h_mem = nullptr; sh.d_mem = nullptr; sh.cut = nullptr; sh.spec = (float2*)(buf + used);
+            CK(cudaMemcpyAsync(sh.spec, b->spec, spec_b, cudaMemcpyDefault, s));
+            float* x = (float*)(buf + used + align_up(spec_b, 256));
+            CK(cudaMemcpyAsync(x, pl->host[i].x, sizeof(float) * (size_t)pl->host[i].N, cudaMemcpyDefault, s));
+            items[hi].x = x; items[hi].rir_bank = &sh;
+            used += stem_copy_bytes(pl, i);
+            ++hi;
+        }
+        const int st = ss_render_dev(pl->c, items + lo, hi - lo, (void*)s);   // the next batch's copies wait on `s`
+        if (st) return st;
+        lo = hi;
+    }
+    return SS_OK;
+}
 template <class Group>
 static int render_stem_groups(ss_pool* pl, const StemGroups& G, char* tmp, cudaStream_t s, Group group) {
     CK(cudaStreamWaitEvent(s, pl->ready, 0));           // banks may still be building
+    char* copies = nullptr;                             // a host pool's transient copies
+    const size_t copy_cap = pl->host_res ? stem_copy_cap(pl) : 0;
+    if (pl->host_res) CK(cudaMalloc((void**)&copies, copy_cap));
+    struct Free { char* p; ~Free() { if (p) cudaFree(p); } } free_copies{copies};   // (cudaFree waits for the device)
     std::vector<ss_source> items;
     for (size_t g = 0; g + 1 < G.first.size(); ++g) {
         items.clear();
@@ -1700,7 +1834,8 @@ static int render_stem_groups(ss_pool* pl, const StemGroups& G, char* tmp, cudaS
             if (pl->mode == SS_MOVING_BOUNDS) { it.bounds = e.bounds; it.bounds_host = pl->bounds_host.data() + pl->bounds_off[i]; }
             items.push_back(it);
         }
-        int st = ss_render_dev(pl->c, items.data(), (int)items.size(), (void*)s);   // the next group waits on `s`
+        int st = pl->host_res ? render_host_stems(pl, items.data(), G.first[g], (int)items.size(), copies, copy_cap, s)
+                              : ss_render_dev(pl->c, items.data(), (int)items.size(), (void*)s);   // the next group waits on `s`
         if (st == SS_OK) st = group(G.first[g], G.first[g + 1]);
         if (st) return st;
     }
@@ -1799,7 +1934,12 @@ static int levels_build(ss_pool* pl, bool mono, cudaStream_t s, std::vector<void
     const int n = pl->n;
     pl->level_off.assign(n + 1, 0);
     for (int i = 0; i < n; ++i) pl->level_off[i + 1] = pl->level_off[i] + pl->host[i].N + 1;
-    CK(cudaMalloc((void**)&pl->levels, sizeof(double) * (size_t)pl->level_off[n]));
+    if (pl->host_res) {                                 // a host pool: k_levels writes and k_draw reads them over PCIe
+        CK(cudaHostAlloc((void**)&pl->h_levels, level_bytes(pl), cudaHostAllocMapped | cudaHostAllocPortable));
+        CK(cudaHostGetDevicePointer((void**)&pl->levels, pl->h_levels, 0));
+    } else {
+        CK(cudaMalloc((void**)&pl->levels, level_bytes(pl)));
+    }
     CK(cudaMalloc((void**)&pl->level_ptr, sizeof(double*) * (size_t)n));
     std::vector<const double*> ptr(n);
     for (int i = 0; i < n; ++i) ptr[i] = pl->levels + pl->level_off[i];
@@ -1845,9 +1985,7 @@ extern "C" int ss_pool_levels(ss_pool* pl, uint32_t flags) {
     }
     for (void* q : owned) cudaFree(q);
     if (st != SS_OK) {                                  // no tables: the pool is as it was
-        if (pl->levels) cudaFree(pl->levels);
-        if (pl->level_ptr) cudaFree(pl->level_ptr);
-        pl->levels = nullptr; pl->level_ptr = nullptr;
+        free_levels(pl);
         return st;
     }
     pl->level_flags = (int)flags;
@@ -1861,6 +1999,7 @@ extern "C" int ss_pool_levels(ss_pool* pl, uint32_t flags) {
 // cudaGraphLaunch per run afterwards instead of ~25 runtime calls.  The pointers in `items` (and the contents of
 // bounds_host) must stay valid and unchanged for the plan's life; buffer *contents* may change between runs.
 struct DrawDesc;
+struct StageSlot;
 struct ss_plan {
     ss_ctx* c = nullptr;
     std::vector<ChunkLaunch> chunks;
@@ -1879,6 +2018,8 @@ struct ss_plan {
     int n_mix = 0;
     const DrawDesc* d_draw = nullptr;  // the start draws' descriptors (k_draw), in d_desc behind the mixture scratch
     int n_draw = 0;
+    const StageSlot* d_stage = nullptr;   // the host-pool slots' staging (k_stage), in d_desc behind the draws
+    int n_stage = 0;
 };
 
 // ----------------------------------------------------------------------------- k_draw
@@ -1954,6 +2095,71 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
     }
 }
 
+// ----------------------------------------------------------------------------- k_stage
+// Host pools: at the head of every run (after k_draw, so that drawn starts are final), each pooled slot of a host pool
+// gets its picked candidate's read set (stage_set) copied from pinned, mapped host memory into its staging area, and its
+// view of the candidate (StageView), which the head of k_blocks takes.  One gridDim.y row of kStageCtas CTAs per slot:
+// every CTA works out the read set, then the CTAs copy it in 16-byte loads, kStageUnroll of them in flight per thread.
+constexpr int kStageCtas = 16, kStageUnroll = 4;
+struct StageSlot {
+    const PoolEntry* pool;            // the pool's table: x and spec are mapped host addresses, bounds and cut device ones
+    const int* pick;
+    const int* ws_dev;                // the slot's moving start, or null: ws
+    const int* parts;                 // the candidates' K when they differ (pool_parts), else null: K
+    const float* gains;               // the pool's gains, or null
+    StageView* view;                  // staging area: the view, ...
+    float2* spec;                     // ... sets * rows_cap rows (used: sets * rows, back to back) ...
+    float* x;                         // ... and the dry samples, whole float4s from xa & ~3 on
+    int n, C, K, ws, len, sets;
+};
+__global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots) {
+    const StageSlot& g = slots[blockIdx.y];
+    __shared__ StageView s_v;
+    __shared__ int s_x[2];                              // dry samples copied: whole float4s [s_x[0], s_x[1])
+    if (threadIdx.x == 0) {
+        bool bad;
+        const int i = clamp_pick(*g.pick, g.n, bad);
+        if (bad && blockIdx.x == 0) atomicOr(&g_dev_err, 8u);
+        const PoolEntry e = g.pool[i];
+        const int K = g.parts ? g.parts[i] : g.K;
+        const int ws = g.ws_dev ? clamp_win_start(*g.ws_dev, e.N, g.len, bad) : g.ws;   // (bit 2 is k_blocks')
+        const StageSet r = stage_set(e.N, e.P, g.C, K, e.bounds, ws, g.len);
+        s_v.e = e; s_v.K = K; s_v.row0 = r.row0; s_v.rows = r.rows; s_v.gain = g.gains ? g.gains[i] : 1.0f;
+        s_x[0] = r.xa & ~3; s_x[1] = (r.xb + 3) & ~3;  // (the pool's arena pads every x to whole float4s)
+    }
+    __syncthreads();
+    const PoolEntry& e = s_v.e;
+    const size_t nx4 = (size_t)((s_x[1] - s_x[0]) >> 2);
+    const size_t per_set = (size_t)s_v.rows * (kSpec / 2);          // float4s per set
+    const size_t rows_h = (size_t)e.P * g.C * s_v.K;                 // rows per set of the bank
+    const size_t total = nx4 + (size_t)g.sets * per_set;
+    const float4* const xs = reinterpret_cast<const float4*>(e.x + s_x[0]);
+    float4* const xd = reinterpret_cast<float4*>(g.x);
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t q0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x; q0 < total; q0 += stride * kStageUnroll) {
+        float4 v[kStageUnroll];
+        float4* dst[kStageUnroll];
+#pragma unroll
+        for (int u = 0; u < kStageUnroll; ++u) {        // every load issued before the first store
+            const size_t q = q0 + u * stride;
+            dst[u] = nullptr;
+            if (q >= total) continue;
+            if (q < nx4) { v[u] = xs[q]; dst[u] = xd + q; continue; }
+            const size_t j = q - nx4, set = j / per_set;
+            v[u] = reinterpret_cast<const float4*>(e.spec + (set * rows_h + s_v.row0) * kSpec)[j - set * per_set];
+            dst[u] = reinterpret_cast<float4*>(g.spec) + j;
+        }
+#pragma unroll
+        for (int u = 0; u < kStageUnroll; ++u) if (dst[u]) *dst[u] = v[u];
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        StageView w = s_v;
+        w.e.x = g.x - s_x[0];                           // biased: sample n at x[n] (Source::x)
+        w.e.spec = g.spec;
+        *g.view = w;
+    }
+}
+
 extern "C" void ss_plan_destroy(ss_plan* p) {
     if (!p) return;
     cudaSetDevice(p->c->device);
@@ -1997,6 +2203,27 @@ static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan
     return g;
 }
 
+// Staging area of a pooled slot of a host pool with windows of win_len (stage_cap), worked out once per pool and length
+static std::pair<int, int> stage_cap(ss_pool* pl, int win_len) {
+    for (const auto& q : pl->stage_caps) if (q.first == win_len) return q.second;
+    std::vector<const int*> bounds;
+    std::vector<int> N(pl->n), P(pl->n);
+    for (int i = 0; i < pl->n; ++i) {
+        N[i] = pl->host[i].N; P[i] = pl->host[i].P;
+        if (pl->mode == SS_MOVING_BOUNDS) bounds.push_back(pl->bounds_host.data() + pl->bounds_off[i]);
+    }
+    int rows, nx;
+    stage_cap(bounds.empty() ? nullptr : bounds.data(), N.data(), P.data(), pl->parts_host.data(), pl->n, pl->C, win_len,
+              rows, nx);
+    pl->stage_caps.push_back({win_len, {rows, nx}});
+    return {rows, nx};
+}
+static size_t stage_bytes(const ss_source& it) {
+    const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(it.pool), it.win_len);
+    return align_up(sizeof(StageView), 256) + align_up((size_t)direct_sets(it) * cap.first * kSpec * sizeof(float2), 256) +
+           align_up(sizeof(float) * (size_t)cap.second, 256);
+}
+
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
                       const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws) {
     ss_ctx* c = p->c;
@@ -2022,14 +2249,38 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
     const size_t draw_off = align_up(scr_off + scr_bytes * n_mixes, 256);
     const size_t desc_bytes = draw_off + sizeof(DrawDesc) * n_draws;
-    CK(cudaMalloc((void**)&p->d_desc, desc_bytes + 256));
+    // behind the draws: the host-pool slots' k_stage descriptors, then their staging areas
+    std::vector<int> staged;                            // arranged items that are slots of host pools
+    for (int i = 0; i < (int)arranged.size(); ++i) if (items[i].pool && items[i].pool->host_res) staged.push_back(i);
+    if (staged.size() > 65535) return SS_ERR_UNSUPPORTED;   // one gridDim.y row of k_stage per slot
+    const size_t stage_off = align_up(desc_bytes, 256), area_off = align_up(stage_off + sizeof(StageSlot) * staged.size(), 256);
+    size_t total = area_off;
+    for (int i : staged) total += stage_bytes(items[i]);
+    CK(cudaMalloc((void**)&p->d_desc, total + 256));
     for (int i = 0; i < ss_ctx::kAux; ++i)
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
     std::vector<char> host(desc_bytes + 256);
+    std::vector<StageView*> views(arranged.size(), nullptr);
+    std::vector<StageSlot> stage(staged.size());
+    for (size_t k = 0, at = area_off; k < staged.size(); ++k) {
+        const ss_source& it = items[staged[k]];
+        const ss_pool* pl = it.pool;
+        StageSlot& g = stage[k];
+        memset(&g, 0, sizeof(g));
+        g.pool = pl->table; g.pick = it.pick_dev; g.ws_dev = it.win_start_dev; g.parts = pl->parts; g.gains = pl->gains;
+        g.n = pl->n; g.C = pl->C; g.K = pl->K; g.ws = it.win_start; g.len = it.win_len; g.sets = direct_sets(it);
+        const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
+        char* a = p->d_desc + at;
+        g.view = (StageView*)a; a += align_up(sizeof(StageView), 256);
+        g.spec = (float2*)a; a += align_up((size_t)g.sets * cap.first * kSpec * sizeof(float2), 256);
+        g.x = (float*)a;
+        at += stage_bytes(it);
+        views[staged[k]] = g.view;
+    }
     p->chunks.resize(n_chunks);
     for (size_t k = 0; k < n_chunks; ++k)
         chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
-                       p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k]);
+                       p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data());
     for (int k = 0; k < n_mixes; ++k)
         ((MixItem*)(host.data() + mix_off))[k] =
             mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
@@ -2044,6 +2295,11 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         CK(cudaMemcpy(p->d_desc + draw_off, g.data(), sizeof(DrawDesc) * n_draws, cudaMemcpyHostToDevice));
         p->d_draw = (const DrawDesc*)(p->d_desc + draw_off);
         p->n_draw = n_draws;
+    }
+    if (!stage.empty()) {
+        CK(cudaMemcpy(p->d_desc + stage_off, stage.data(), sizeof(StageSlot) * stage.size(), cudaMemcpyHostToDevice));
+        p->d_stage = (const StageSlot*)(p->d_desc + stage_off);
+        p->n_stage = (int)stage.size();
     }
     return SS_OK;
 }
@@ -2207,11 +2463,16 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, cudaStream_t stream
     return SS_OK;
 }
 
-// the start draws, the launches of every chunk (run_chunks), then the mixtures (which read every chunk's outputs) on
-// `stream`
+// the start draws, the host-pool staging, the launches of every chunk (run_chunks), then the mixtures (which read every
+// chunk's outputs) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
     if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, stream); if (st) return st; }
+    if (p->n_stage) {                                   // host pools: after the draws, before any chunk reads a slot
+        k_stage<<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
     const int rc = run_chunks(c, p->chunks.size(), stream, p->ev_fork, p->ev_join, [&](size_t k, cudaStream_t s, int) {
         return chunk_enqueue(c, p->chunks[k], s, c->profiling);
     });

@@ -307,6 +307,68 @@ SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, co
                          Block* full) {
     return pool_table_cap(aligned, bounds, N, P, nullptr, n, win_len, K, full);
 }
+// ---- host pools (SS_BANK_HOST, include/sonicsim_b200.h): banks and dry signals in pinned host memory.  At every run
+// k_stage copies the read set of each pooled slot's picked candidate into the slot's staging area in device memory and
+// writes the slot's view of it; the head of k_blocks then takes that view instead of the pool's entry.
+// Read set of a window [ws, ws + len) of a candidate of N samples, P positions (bounds: its trajectory, unread when
+// P == 1), C channels and K partitions - a superset of what k_blocks, k_prepare and the render kernels read:
+//   - dry samples [xa, xb) = [ws - (K + 2) * 4096, ws + len + 2 * 4096) clamped to [0, N).  The table's first block g0
+//     is at most K blocks in front of the block holding ws (window_span: K - 1 partition blocks, one more for the even
+//     start) and starts after ws - (K + 1) * 4096; its dry window reaches 4096 further back.  The last block, the
+//     partner of the last one that meets the window, starts before ws + len + 4096 and its window ends 4096 later.
+//   - RIR rows [row0, row0 + rows) of each set: every position whose segment holds a sample of [xa, xb) and the one
+//     after it (the blocks that meet the window lie inside [xa, xb)), widened to row pairs as window_rows does.
+struct StageSet { int xa, xb, row0, rows; };
+SS_HD StageSet stage_set(int N, int P, int C, int K, const int* bounds, int ws, int len) {
+    StageSet r;
+    const long long a = (long long)ws - (long long)(K + 2) * kB, b = (long long)ws + len + 2 * kB;
+    r.xa = a > 0 ? (int)a : 0;
+    r.xb = b < N ? (int)b : N;
+    int pa = 0, pb = 0;
+    if (P > 1) { pa = seg_of(bounds, P - 1, r.xa); pb = seg_of(bounds, P - 1, r.xb - 1) + 1; }
+    window_rows(P, C, K, pa, pb, r.row0, r.rows);
+    return r;
+}
+// Staging area of a pooled slot with windows of len over n candidates (candidate i: N[i], P[i], Ks[i] partitions,
+// trajectory bounds[i], or bounds == null for a static pool): the most RIR rows per set and dry samples any candidate's
+// read set holds at any start in [0, N[i] - len].  Both grow with the start while the first staged sample stays in one
+// segment, so the rows are largest at the last start of each such run - stage_set at P[i] + 1 starts, O(P log P) per
+// candidate - and the dry span at min(N[i] - len, (K + 2) * 4096).  The dry count has 8 samples to spare: k_stage
+// copies whole float4s around the read set.
+SS_HD void stage_cap(const int* const* bounds, const int* N, const int* P, const int* Ks, int n, int C, int len,
+                     int& rows, int& nx) {
+    rows = 0; nx = 0;
+    for (int i = 0; i < n; ++i) {
+        const int last = N[i] - len;
+        const long long d0 = (long long)(Ks[i] + 2) * kB;
+        const int* const b = bounds ? bounds[i] : nullptr;
+        for (int sg = -2; sg < (b ? P[i] - 1 : 0); ++sg) {
+            // the last start, the widest dry span, then the last start of each segment's run
+            const long long w = sg == -2 ? last : sg == -1 ? d0 : b[sg + 1] - 1 + d0;
+            const StageSet r = stage_set(N[i], P[i], C, Ks[i], b, w < last ? (int)w : last, len);
+            rows = r.rows > rows ? r.rows : rows;
+            nx = r.xb - r.xa + 8 > nx ? r.xb - r.xa + 8 : nx;
+        }
+    }
+}
+// A slot's view of its picked candidate, written by k_stage: the pool's entry with x (biased: sample n at x[n]) and spec
+// pointing into the staging area, whose sets hold rows [row0, row0 + rows) back to back; the candidate's K and gain.
+struct StageView {
+    PoolEntry e;
+    int K, row0, rows;
+    float gain;
+};
+static_assert(sizeof(StageView) == 56, "StageView layout");
+// A pooled slot's counts[18..19]: the device pointer of its StageView (a slot of a host pool), or null
+SS_HD const StageView* stage_view(const Source& s) { return *reinterpret_cast<const StageView* const*>(s.counts + 18); }
+// The head of k_blocks for a slot of a host pool: the staged view into the slot's Source, as pick_slot writes an entry of a
+// device pool, with the staged rows as the window's row origin (h_row0, h_rows; fill_items addresses rows through it)
+SS_HD void take_view(Source& s, const StageView& v) {
+    s.K = v.K;
+    pick_candidate(s, v.e);
+    s.h_row0 = v.row0; s.h_rows = v.rows;
+    set_stem_gain(s, v.gain);
+}
 // ---- crop start draws of device plans (ss_plan_draw, include/sonicsim_b200.h): the dataloader's start loop
 // (movingdatamodule.py:81-99) over level tables Q (ss_pool_levels: Q[0] = 0, Q[n + 1] = Q[n] + e[n], float64).
 // Starts a crop of len samples can take in a candidate of N samples: the M of a draw is the least of these over its readers

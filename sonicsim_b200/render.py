@@ -222,13 +222,16 @@ class RirBank(_Held):
     ABI).  Pass it as `MovingSource.rirs` / `StaticSource.rir`: the source renders bit-identically to the same source
     given the raw RIRs, which are never read again.  It belongs to the context of the renderer that made it.  Every
     render that uses it is ordered after its construction by the library, on every path, whatever stream built it.
-    Plans and source pools hold the bank: it is freed only once it is closed (or collected) and nothing alive uses it."""
+    Plans and source pools hold the bank: it is freed only once it is closed (or collected) and nothing alive uses it.
+    A host bank (`host` True, Renderer.rir_bank(..., host=True)) holds its spectra in pinned host memory
+    (`host_nbytes`; `nbytes` counts device bytes only) and serves only as a candidate of a host source pool."""
 
-    def __init__(self, renderer, handle, shape, normalize, direct_taps):
+    def __init__(self, renderer, handle, shape, normalize, direct_taps, host=False):
         self.renderer, self._h = renderer, handle
         self.shape = tuple(int(v) for v in shape)          # as given: (P, C, L) or (C, L)
-        self.normalize, self.direct_taps = bool(normalize), int(direct_taps)
+        self.normalize, self.direct_taps, self.host = bool(normalize), int(direct_taps), bool(host)
         self.nbytes = int(renderer.lib.ss_bank_bytes(handle))
+        self.host_nbytes = int(renderer.lib.ss_bank_host_bytes(handle))
 
     @property
     def pcl(self) -> T.Tuple[int, int, int]:
@@ -249,11 +252,18 @@ class SourcePool(_Held):
     "mono" or "channels": the level tables the pool holds for start draws (CropDraw), included in `nbytes`.
     `loudness` is an (n, 2) float64 array of every candidate's measured integrated loudness (LUFS) and linear gain
     (ss_pool_loudness), NaN for a candidate without a target; `nbytes` includes the gains (4 bytes per candidate), and
-    the candidates' partition counts (4 bytes per candidate) when their K = ceil(L / 4096) differ (ss_pool_bytes)."""
+    the candidates' partition counts (4 bytes per candidate) when their K = ceil(L / 4096) differ (ss_pool_bytes).
+    `resident` is "device", or "host" for a pool over host banks (RirBank.host): its dry signals, banks and level tables
+    stay in pinned host memory (`host_nbytes`, banks not included), `nbytes` counts its device bytes, and every plan run
+    copies only what its slots read (ss_pool_host_bytes, INTEGRATION.md)."""
 
-    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None, loudness=None):
+    def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None, loudness=None,
+                 sizes=None, resident="device"):
         self.renderer, self._h = renderer, handle
         self.candidates = list(candidates)
+        self.resident = resident
+        self._sizes = list(sizes) if sizes is not None else [int(s.dry.numel()) for s in self.candidates]
+        self.host_nbytes = int(renderer.lib.ss_pool_host_bytes(handle))
         self.n, self.mode, self.C, self.L = len(self.candidates), mode, C, L
         self.n_min, self.direct_taps, self.levels = n_min, direct_taps, levels
         self._loudness = loudness if loudness is not None else np.full((self.n, 2), np.nan)
@@ -272,7 +282,10 @@ class SourcePool(_Held):
         if self.closed or self.levels is None or not 0 <= i < self.n:
             return None
         ptr = self.renderer.lib.ss_pool_level_table(self._h, int(i))
-        n = self.candidates[i].dry.numel() + 1
+        n = self._sizes[i] + 1
+        if self.resident == "host":                        # pinned, mapped host memory: copied from the host side
+            host = np.ctypeslib.as_array((ctypes.c_double * n).from_address(ptr))
+            return torch.from_numpy(host.copy()).to("cuda:%d" % self.renderer.device)
 
         class _View:
             __cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (ptr, False), "version": 3}
@@ -305,6 +318,19 @@ def _rirs(s, conv=None):
     return None, r, P, C, L, mode
 
 
+def _pool_host_dry(dry, own, device, keep):
+    """(pointer, N) of the dry signal of a host pool's candidate, which the pool copies: a CUDA float32 tensor of the
+    renderer's device, or a 1-D NumPy array / CPU tensor (converted to contiguous float32, kept alive in `keep`)."""
+    if _is_tensor(dry) and dry.is_cuda:
+        import torch
+        return _tensor(dry, "source_pool", own, "dry", torch.float32, device), dry.numel()
+    a = np.ascontiguousarray(dry.numpy() if _is_tensor(dry) else dry, dtype=np.float32)
+    if a.ndim != 1 or a.size < 1:
+        raise ValueError("source_pool: dry of %s must be 1-D and not empty, got shape %s" % (own, a.shape))
+    keep.append(a)
+    return a.ctypes.data, a.size
+
+
 def _check_usable(held, renderer, what):
     """Refuses a closed RirBank / SourcePool, or one of another renderer's context; `what` names it."""
     if held.closed:
@@ -322,6 +348,9 @@ def _bank_of(renderer, s, i, P, C, L):
     if s.normalize_rirs:
         raise ValueError("source %d: normalisation is a property of its RirBank (normalize=%s); leave normalize_rirs "
                          "False" % (i, b.normalize))
+    if getattr(b, "host", False):
+        raise ValueError("source %d: its RirBank is a host bank (host=True), which serves only as a candidate of a "
+                         "source pool" % i)
     if int(s.direct_taps) not in (0, b.direct_taps):
         raise ValueError("source %d: direct_taps = %d, its RirBank holds %s" % (
             i, int(s.direct_taps), "direct_taps = %d" % b.direct_taps if b.direct_taps else "no direct set"))
@@ -410,18 +439,21 @@ class Renderer:
         self.ctx = _lib.context(self.device)
 
     # ------------------------------------------------------------------ RIR spectrum banks
-    def rir_bank(self, rirs, normalize: bool = False, direct_taps: int = 0) -> RirBank:
+    def rir_bank(self, rirs, normalize: bool = False, direct_taps: int = 0, host: bool = False) -> RirBank:
         """Transform an RIR set (P, C, L) - or (C, L) for a static source - once into a RirBank on this renderer's
         device: a NumPy array is copied in and the call returns when the bank is complete; a CUDA float32 tensor of this
         device is transformed asynchronously on the current stream (keep it unchanged until that stream gets there).
         Either way the bank can be used at once, on every path: every render that uses it - render_host / plan_host on
         the library's own streams, render_device / plan_device on any stream - waits for its construction first.
         `normalize` / `direct_taps` are the normalize_rirs / direct_taps every source of the bank renders with (a bank
-        with a direct set also serves sources with direct_taps = 0)."""
+        with a direct set also serves sources with direct_taps = 0).  `host` moves the transformed bank into pinned host
+        memory (SS_BANK_HOST; bit-identical spectra, the call returns once it is there): such a bank is only a candidate
+        of a host source pool (source_pool), whose plans copy the rows each run reads to the device."""
         taps = int(direct_taps)
         if taps < 0:
             raise ValueError("direct_taps must be >= 0, got %d" % taps)
-        flags = (_lib.SS_RIR_NORMALIZE if normalize else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0)
+        flags = (_lib.SS_RIR_NORMALIZE if normalize else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0) | \
+            (_lib.SS_BANK_HOST if host else 0)
         h = ctypes.c_void_p()
         dev = _is_tensor(rirs)
         if dev:
@@ -438,7 +470,7 @@ class Renderer:
                                                    ctypes.c_void_p(stream), ctypes.byref(h)))
         else:
             _lib.check(self.lib.ss_bank_create_host(self.ctx, a.ctypes.data, P, C, L, flags, taps, ctypes.byref(h)))
-        return RirBank(self, h, shape, normalize, taps)
+        return RirBank(self, h, shape, normalize, taps, host)
 
     # ------------------------------------------------------------------ source pools
     def source_pool(self, candidates: T.Sequence[T.Union[MovingSource, StaticSource]],
@@ -451,6 +483,11 @@ class Renderer:
         C, and may differ in L (e.g. the speakers of one formats.load_rir_dump, each with its own length): a slot that
         picks a candidate renders it with that candidate's own RIR partitions.  The pool's L, which its slots are given,
         is the longest candidate's.  The candidates' tensors and banks are kept alive by the pool.
+
+        Candidates whose banks are all host banks (rir_bank(..., host=True)) make a host pool (`resident` "host"): its
+        dry signals are copied into pinned host memory at once, so `dry` (and `bounds`, when `bounds_host` is not given)
+        may also be NumPy arrays or CPU tensors; every plan run then copies only the rows and samples its slots read to
+        the device (one more kernel launch per run).  A pool that mixes host and device banks is refused.
 
         `levels` = "mono" or "channels" also builds every candidate's level table (ss_pool_levels: the float64 prefix
         sums of the squares of its whole rendered stem, channel-folded like Mixture(mono=True) for "mono"), which
@@ -471,7 +508,7 @@ class Renderer:
         _check_lufs("source_pool", "candidate", lufs_targets, n, sr)
         items = (SsSource * n)()
         keep = []
-        first, L_max = None, 0
+        first, L_max, host, sizes = None, 0, None, []
         for i, s in enumerate(candidates):
             if not isinstance(s, (MovingSource, StaticSource)):
                 raise ValueError("source_pool: candidate %d must be a MovingSource or StaticSource, got %s"
@@ -489,15 +526,31 @@ class Renderer:
             elif kind != first:
                 raise ValueError("source_pool: candidate %d is (%s, C=%d), candidate 0 (%s, C=%d): every candidate has "
                                  "one kind and C (L may differ)" % ((i,) + _kind(kind) + _kind(first)))
+            if host is None:
+                host = rb.host
+            elif rb.host != host:
+                raise ValueError("source_pool: candidate %d has a %s bank, candidate 0 a %s one: a pool's banks are all "
+                                 "host banks or all device banks" % ((i,) + (("host", "device") if rb.host else
+                                                                           ("device", "host"))))
             L_max = max(L_max, L)
             own = "candidate %d" % i
-            x = _tensor(s.dry, "source_pool", own, "dry", torch.float32, self.device)
-            items[i] = SsSource(x=x, N=s.dry.numel(), P=P, C=C, L=L, mode=mode, rir_bank=rb._h.value)
+            bounds_host = s.bounds_host if mode == _lib.SS_MOVING_BOUNDS else None
+            if host:                                       # copied into the pool: NumPy, CPU or CUDA tensors
+                x, N = _pool_host_dry(s.dry, own, self.device, keep)
+                if mode == _lib.SS_MOVING_BOUNDS and bounds_host is None and s.bounds is not None and \
+                        not (_is_tensor(s.bounds) and s.bounds.is_cuda):
+                    bounds_host = s.bounds.numpy() if _is_tensor(s.bounds) else s.bounds
+            else:
+                x = _tensor(s.dry, "source_pool", own, "dry", torch.float32, self.device)
+                N = s.dry.numel()
+            sizes.append(N)
+            items[i] = SsSource(x=x, N=N, P=P, C=C, L=L, mode=mode, rir_bank=rb._h.value)
             if mode == _lib.SS_MOVING_BOUNDS:
-                items[i].bounds = _tensor(s.bounds, "source_pool", own, "bounds", torch.int32, self.device, (P,))
-                if s.bounds_host is None:
+                if not host:
+                    items[i].bounds = _tensor(s.bounds, "source_pool", own, "bounds", torch.int32, self.device, (P,))
+                if bounds_host is None:
                     raise ValueError("source_pool: moving candidate %d needs bounds_host" % i)
-                bh = _bounds(s.bounds_host, P, "source_pool: bounds_host of %s" % own, keep)
+                bh = _bounds(bounds_host, P, "source_pool: bounds_host of %s" % own, keep)
                 items[i].bounds_host = bh.ctypes.data
         if lufs_targets is not None and first[1] > 8:
             raise ValueError("source_pool: loudness normalisation supports at most 8 channels, the candidates have %d"
@@ -513,8 +566,8 @@ class Renderer:
             self.lib.ss_pool_destroy(h)
             _lib.check(st)
         taps = {_rirs(s)[0].direct_taps for s in candidates}
-        return SourcePool(self, h, candidates, first[0], first[1], L_max, min(s.dry.numel() for s in candidates),
-                          taps.pop() if len(taps) == 1 else 0, levels, loud)
+        return SourcePool(self, h, candidates, first[0], first[1], L_max, min(sizes),
+                          taps.pop() if len(taps) == 1 else 0, levels, loud, sizes, "host" if host else "device")
 
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],

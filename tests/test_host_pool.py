@@ -1,0 +1,177 @@
+"""Host pools on the CPU, through the kernels' own helpers (exported by tests/emu/ss_emu_stage.cu): the read set k_stage
+copies for a pooled slot of a host pool (stage_set) and the staging area a plan sizes for it (stage_cap).
+  - the staged set holds every dry sample and RIR row the windowed render reads - the dry windows of the table's blocks
+    (window_blocks) and window_rows of the positions of the blocks that meet the window;
+  - it never exceeds the slot's staging area, which is the largest set of any candidate at any start;
+  - the head of k_blocks over the staged view (take_view) builds the same Source, block table, work items, h_row0 / h_rows
+    origin and direct-set rows as over the full candidate (pick_slot), and the slot renders the same bits from copies
+    that hold the read set and NaN everywhere else."""
+import ctypes
+import os
+import subprocess
+
+import numpy as np
+import pytest
+
+from conftest import ROOT
+from oracle import sonicsim_oracle as so
+from test_pool import _choice, _random_bounds
+from window_cases import B
+
+KSPEC = 4096
+
+
+@pytest.fixture(scope="module")
+def emu(tmp_path_factory):
+    src = os.path.join(ROOT, "tests", "emu", "ss_emu_stage.cu")
+    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_stage.so")
+    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
+           "-o", so_path, src]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
+    lib = ctypes.CDLL(so_path)
+    vp, i32 = ctypes.c_void_p, ctypes.c_int
+    lib.emu_stage_set.argtypes = [i32] * 4 + [vp] + [i32] * 2 + [vp]
+    lib.emu_stage_cap.argtypes = [vp] * 5 + [i32] * 3 + [vp]
+    lib.emu_stage_slot.argtypes = [vp] * 4 + [i32] * 10 + [vp] * 5
+    lib.emu_bank_create.argtypes = [vp] + [i32] * 5 + [vp, vp]
+    return lib
+
+
+def _p(a):
+    return None if a is None else ctypes.c_void_p(a.ctypes.data)
+
+
+def _k(L):
+    return (L + B - 1) // B
+
+
+class Cand:
+    """One candidate: dry x, trajectory (None: static), RIRs and their emulated bank (with a direct set when taps > 0)."""
+
+    def __init__(self, emu, rng, N, P, C, L, taps, short=False):
+        self.N, self.P, self.C, self.L, self.K = N, P, C, L, _k(L)
+        self.x = so.synth_dry(rng, N)
+        self.bounds = None if P == 1 else _random_bounds(rng, P, N, short)
+        h = so.synth_rirs(rng, P, C, L)
+        sets = 2 if taps else 1
+        self.spec = np.full((sets * P * C * self.K, KSPEC), np.nan, np.complex64)
+        self.cut = np.zeros(P * C, np.int32) if taps else None
+        emu.emu_bank_create(_p(h), P, C, L, 0, taps, _p(self.spec), _p(self.cut))
+        self.direct = 1 if taps else 0
+
+    def aligned_alone(self):
+        return 0 if self.P == 1 else _choice(self.bounds, self.N, self.P, self.L)
+
+
+def _slot(emu, c, aligned, k_pool, ws, wl, render):
+    outs = [np.full((c.C, wl), np.nan, np.float32) for _ in range(4)]
+    info = np.zeros(15, np.int32)
+    emu.emu_stage_slot(_p(c.x), _p(c.spec), _p(c.cut), _p(c.bounds), c.N, c.P, c.C, c.L, 0 if c.P == 1 else 1,
+                       aligned, k_pool, ws, wl, c.direct, int(render), *[_p(o) for o in outs], _p(info))
+    return info, outs
+
+
+def _cap(emu, cands, wl):
+    N = np.array([c.N for c in cands], np.int32)
+    P = np.array([c.P for c in cands], np.int32)
+    K = np.array([c.K for c in cands], np.int32)
+    out = np.zeros(2, np.int32)
+    if cands[0].P == 1:
+        emu.emu_stage_cap(None, None, _p(N), _p(P), _p(K), len(cands), cands[0].C, wl, _p(out))
+    else:
+        off = np.cumsum([0] + [c.P for c in cands[:-1]]).astype(np.int64)
+        flat = np.ascontiguousarray(np.concatenate([c.bounds for c in cands]), np.int32)
+        emu.emu_stage_cap(_p(flat), _p(off), _p(N), _p(P), _p(K), len(cands), cands[0].C, wl, _p(out))
+    return int(out[0]), int(out[1])
+
+
+def _check_tables(info, c, ws, wl):
+    xa, xb, row0, rows = (int(v) for v in info[:4])
+    # the staged set holds the read set
+    assert xa <= info[4] and info[5] <= xb, (ws, wl, info[:8].tolist())
+    assert row0 <= info[6] and info[6] + info[7] <= row0 + rows, (ws, wl, info[:8].tolist())
+    assert row0 % 2 == 0 and 0 <= row0 and row0 + rows <= c.P * c.C * c.K
+    # the staged view builds the same Source, table and items; the full run's rows start at 0, the staged at row0
+    assert info[8] == 1, (ws, wl)
+    assert info[9:13].tolist() == [0, c.P * c.C * c.K, row0, rows], (ws, wl, info[9:13].tolist())
+    assert info[13:15].tolist() == ([c.P * c.C * c.K, rows] if c.direct else [-1, -1])
+    return xb - xa, rows
+
+
+def _starts(c, wl, every):
+    last = c.N - wl
+    if every:
+        return list(range(last + 1))
+    s = {0, last, last // 2, min(last, (c.K + 2) * B)}
+    for b in ([] if c.bounds is None else c.bounds[1:-1]):      # segment edges, on both sides
+        for d in (-1, 0, 1):
+            if 0 <= b + d <= last:
+                s.add(int(b + d))
+    for q in range(0, c.N, B):                                  # grid block edges
+        for d in (-1, 0):
+            if 0 <= q + d <= last:
+                s.add(q + d)
+    return sorted(s)
+
+
+CASES = [  # (P, C, L list, taps, N range, wl, every start)
+    (1, 3, [1000], 0, (9000, 13000), 3000, True),
+    (1, 2, [9000, 16384], 40, (20000, 30000), 6000, False),
+    (4, 2, [4096], 0, (9000, 12000), 2500, True),
+    (5, 3, [3000], 40, (20000, 40000), 7000, False),
+    (3, 1, [4097, 9000, 16000], 0, (20000, 40000), 9000, False),
+    (6, 2, [2000, 8192, 12289], 40, (25000, 40000), 5000, False),
+]
+
+
+@pytest.mark.parametrize("case", range(len(CASES)))
+def test_staged_set_holds_the_read_set_within_capacity(emu, case):
+    """Aligned and grid blocking, K = 1..4, static and moving, with and without a direct set: at every start of the small
+    cases and at the first, last, segment- and block-edge starts of the larger ones, the staged set holds what the slot
+    reads, and the slot's staging area (stage_cap over the pool) holds the staged set; the capacity is reached."""
+    P, C, Ls, taps, (n_lo, n_hi), wl, every = CASES[case]
+    rng = np.random.default_rng(100 + case)
+    cands = [Cand(emu, rng, int(rng.integers(n_lo, n_hi)), P, C, L, taps, short=i % 2 == 1)
+             for i, L in enumerate(Ls * 2)]
+    k_pool = max(c.K for c in cands)
+    aligned = int(all(c.aligned_alone() for c in cands)) if P > 1 else 0
+    cap_rows, cap_x = _cap(emu, cands, wl)
+    most_rows, most_x = 0, 0
+    for c in cands:
+        for ws in _starts(c, wl, every):
+            info, _ = _slot(emu, c, aligned, k_pool, ws, wl, render=False)
+            nx, rows = _check_tables(info, c, ws, wl)
+            assert rows <= cap_rows and nx + 8 <= cap_x, (ws, rows, cap_rows, nx, cap_x)
+            most_rows, most_x = max(most_rows, rows), max(most_x, nx + 8)
+    if every:                                                   # every start was tried: the capacity is exact
+        assert (most_rows, most_x) == (cap_rows, cap_x)
+
+
+def test_both_blockings_and_every_k_are_covered():
+    seen = set()
+    rng_cases = [(P, Ls) for P, C, Ls, *_ in CASES]
+    for P, Ls in rng_cases:
+        for L in Ls:
+            seen.add(("static" if P == 1 else "moving", _k(L)))
+    assert {k for _, k in seen} == {1, 2, 3, 4} and {"static", "moving"} <= {m for m, _ in seen}
+
+
+@pytest.mark.parametrize("case", range(len(CASES)))
+def test_staged_slot_renders_the_same_bits(emu, case):
+    """The slot rendered from copies of the read set (NaN everywhere else) against the slot over the full candidate:
+    the same bits for the reverberant and the direct stem, at the first, last and edge starts and a few others."""
+    P, C, Ls, taps, (n_lo, n_hi), wl, _ = CASES[case]
+    rng = np.random.default_rng(200 + case)
+    cands = [Cand(emu, rng, int(rng.integers(n_lo, n_hi)), P, C, L, taps, short=i % 2 == 1) for i, L in enumerate(Ls)]
+    k_pool = max(c.K for c in cands)
+    aligned = int(all(c.aligned_alone() for c in cands)) if P > 1 else 0
+    for c in cands:
+        starts = _starts(c, wl, False)
+        pick = sorted({starts[0], starts[-1]} | set(rng.choice(starts, size=min(4, len(starts)), replace=False).tolist()))
+        for ws in pick:
+            info, (yf, ys, df, ds) = _slot(emu, c, aligned, k_pool, int(ws), wl, render=True)
+            _check_tables(info, c, ws, wl)
+            assert not np.isnan(yf).any() and np.array_equal(yf, ys), (case, ws)
+            if taps:
+                assert not np.isnan(df).any() and np.array_equal(df, ds), (case, ws)
