@@ -36,6 +36,7 @@ extern "C" {
 typedef struct ss_ctx ss_ctx;
 typedef struct ss_bank ss_bank;
 typedef struct ss_pool ss_pool;
+typedef struct ss_dry_pool ss_dry_pool;
 
 typedef enum {
     SS_OK = 0,
@@ -308,7 +309,9 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * offending samples as silence (clamped positions) and set a bit that this call returns and clears after waiting for
  * the device: bit 0 = an interp_index outside [0, P - 2], bit 1 = a device-side bounds table that is not ascending from
  * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
- * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped).  The Python device API raises IndexError / ValueError from it on request
+ * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped), bit 4 (dry
+ * pools, below) = a dry pick outside [0, n) of its dry pool (clamped).  The Python device API raises IndexError /
+ * ValueError from it on request
  * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
  * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
 int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
@@ -414,6 +417,60 @@ typedef struct {
 /* n_draws == 0 makes it ss_plan_create_mix */
 int ss_plan_create_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                       const ss_plan_draw* draws, int n_draws, ss_plan** out);
+
+/* ---- dry pools: SonicSet renders 3 utterance streams per scene, but a trajectory's RIRs do not depend on what is said
+ * along it: any dry utterance rendered through a banked trajectory is physically consistent.  A dry pool is a set of n
+ * dry signals that pooled slots take their dry signal from, picked on the device at every run independently of the
+ * trajectory pick, so that (#dry signals x #trajectories) combinations are reachable with no host work.
+ *   - ss_dry_pool_create: x[i] is a DEVICE pointer (4-byte aligned) to signal i, float32, lengths[i] samples (1 <=
+ *     lengths[i] <= 2^31 - 1 - 16384, the bound of ss_source.N); 1 <= n <= 2^24.  The pool references the signals, which
+ *     must outlive it; their contents may change between runs, as a candidate's x may.  flags = SS_DRY_LEVELS also builds
+ *     every signal's level table: Q[0] = 0, Q[n + 1] = Q[n] + (double)(x[n] * x[n]) in float64 (lengths[i] + 1 doubles,
+ *     8 bytes per sample), by the scan of ss_pool_levels over the signal as a one-channel stem (whose mono fold is the
+ *     signal itself), on a stream of the library's own: the signals must be complete when the call is made (synchronise
+ *     the stream that wrote them), and the tables describe them as they are then.  Returns when the pool (and its
+ *     tables) is in device memory.  Refused (SS_ERR_INVALID): NULL arguments, n or a length out of range, a NULL or unaligned x[i],
+ *     unknown flags.
+ *   - ss_dry_pick names a pooled slot of a plan (`slot`, an index into `items`), a dry pool of the plan's context and a
+ *     4-byte aligned DEVICE int32 `pick_dev`, read at every run like the slot's pick.  At every run the slot renders the
+ *     candidate its own pick names - bank, bounds, N, P, K, blocking, kernel variant unchanged - with dry signal
+ *     pick_dev's signal of the dry pool in place of the candidate's x.  Only samples [0, N) of it are read (the read set
+ *     of a pooled slot), N the picked candidate's.  A dry pick outside [0, n) is clamped into that range and
+ *     ss_device_errors reports bit 4.
+ *   - Bits: a dry-picked slot's stem (and its direct stem) equals ss_render_dev of the picked candidate with x = the
+ *     picked signal's first N samples, with the same fixed window, bit for bit, whenever the pooled slot has the bits of
+ *     ss_render_dev at all (every candidate would choose the pool's blocking on its own, see source pools).
+ *   - Start draws (ss_plan_draw): a speaker with a dry pick tests the DRY crop, not the reverberant one: silent when
+ *     10 log10(max(1e-20, (Q[s + len] - Q[s]) / len)) < threshold_db, Q its dry pool's table of the picked signal.  This
+ *     is the dataloader's rule applied to the dry speech: no table of the rendered stem exists for a pair drawn at run
+ *     time.  The gaps create_long_audio leaves between utterances are exact zeros of the dry stream, so the rule still
+ *     rejects crops that fall in a gap.  M is unchanged (the readers' picked candidates' N); speakers with and without a
+ *     dry pick may share a draw.  A run with dry picks launches exactly as many kernels as the same plan without them.
+ *   - Mixtures take dry-picked stems like any other; a static pool (noise) takes dry picks as a moving one does.
+ * Refused by ss_plan_create_dry, before anything is allocated and with no plan created (SS_ERR_INVALID): n_picks < 0, a
+ * NULL picks with n_picks > 0; a slot outside [0, n_items), or named by two dry picks; a slot that is not pooled, or whose
+ * pool is a host pool (k_stage stages the candidate's own x) or has loudness gains (measured with the candidates' own
+ * dry signals); a NULL pool or one of another context; a dry pool with a signal shorter than the slot pool's longest
+ * candidate N; a NULL or unaligned pick_dev; a draw speaker with a dry pick whose dry pool has no level tables; a range a
+ * plan writes that meets a dry pick or a signal of a dry pool it uses.  A destroyed dry pool cannot be detected: a dry
+ * pool must outlive every plan that uses it; ss_dry_pool_destroy waits for the device before it frees it.
+ * n_picks == 0 makes ss_plan_create_dry exactly ss_plan_create_ex.  ss_version stays 108: these exports mark the
+ * capability. */
+#define SS_DRY_LEVELS 1u
+typedef struct {
+    int32_t slot;                     /* index into `items` of a pooled slot                                           */
+    const ss_dry_pool* pool;          /* the dry pool it takes its dry signal from                                     */
+    const int32_t* pick_dev;          /* device int32: the signal, read at every run                                   */
+} ss_dry_pick;
+int ss_dry_pool_create(ss_ctx* ctx, const float* const* x, const int32_t* lengths, int n, uint32_t flags,
+                       ss_dry_pool** out);
+int64_t ss_dry_pool_bytes(const ss_dry_pool* pool);   /* device bytes held: n signal pointers (8 B each), and with level
+                                                       * tables the tables (8 B per sample + 8) and their n pointers */
+/* Device pointer of signal i's level table (lengths[i] + 1 doubles), or NULL without tables or with i outside [0, n). */
+const double* ss_dry_pool_level_table(const ss_dry_pool* pool, int i);
+void ss_dry_pool_destroy(ss_dry_pool* pool);          /* destroy dry pools after the plans that use them */
+int ss_plan_create_dry(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                       const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks, ss_plan** out);
 
 /* Same, host pointers: H2D -> render -> D2H, pipelined over chunks on internal streams.  Returns
  * when every `out` is complete.  This is what the drop-in Python functions call. */

@@ -22,6 +22,7 @@ SS_STATIC, SS_MOVING_BOUNDS, SS_MOVING_INDEXED = 0, 1, 2
 SS_RIR_NORMALIZE, SS_DIRECT_TARGET = 1, 2
 SS_BANK_HOST = 0x100
 SS_MIX_MONO = 1
+SS_DRY_LEVELS = 1
 
 
 class SsLoudItem(ctypes.Structure):
@@ -54,6 +55,11 @@ class SsPlanDraw(ctypes.Structure):
     _fields_ = [("start", ctypes.c_void_p), ("u", ctypes.c_void_p), ("used", ctypes.c_void_p),
                 ("speakers", ctypes.c_int32 * 8), ("S", ctypes.c_int32), ("tries", ctypes.c_int32),
                 ("threshold_db", ctypes.c_float)]
+
+
+class SsDryPick(ctypes.Structure):
+    """`ss_dry_pick` of include/sonicsim_b200.h."""
+    _fields_ = [("slot", ctypes.c_int32), ("pool", ctypes.c_void_p), ("pick_dev", ctypes.c_void_p)]
 
 
 class SsDryClip(ctypes.Structure):
@@ -143,6 +149,9 @@ def load():
                                             ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_plan_create_ex.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPlanMix),
                                           ctypes.c_int, ctypes.POINTER(SsPlanDraw), ctypes.c_int, ctypes.POINTER(vp)]
+        lib.ss_plan_create_dry.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPlanMix),
+                                           ctypes.c_int, ctypes.POINTER(SsPlanDraw), ctypes.c_int,
+                                           ctypes.POINTER(SsDryPick), ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_plan_run.argtypes = [vp, vp]
         lib.ss_plan_is_graph.argtypes = [vp]
         lib.ss_plan_destroy.argtypes = [vp]
@@ -166,6 +175,13 @@ def load():
         lib.ss_pool_loudness.argtypes = [vp, ctypes.POINTER(SsPostLufs)]
         lib.ss_pool_level_table.argtypes = [vp, ctypes.c_int]
         lib.ss_pool_level_table.restype = vp
+        lib.ss_dry_pool_create.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(vp)]
+        lib.ss_dry_pool_bytes.argtypes = [vp]
+        lib.ss_dry_pool_bytes.restype = i64
+        lib.ss_dry_pool_level_table.argtypes = [vp, ctypes.c_int]
+        lib.ss_dry_pool_level_table.restype = vp
+        lib.ss_dry_pool_destroy.argtypes = [vp]
+        lib.ss_dry_pool_destroy.restype = None
         lib.ss_render_host.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int]
         lib.ss_render_host_ex.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPostLufs)]
         lib.ss_convolve_fixed_receiver.argtypes = [vp, vp, vp, vp, i32, i32, i32]
@@ -198,7 +214,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_plan_create_dry", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

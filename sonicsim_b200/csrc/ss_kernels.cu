@@ -42,7 +42,8 @@ using namespace ss;
 // Device-path trajectory check: the kernels cannot raise, so a source whose device-side trajectory breaks the contract
 // of ss_render_dev (idx outside [0, P - 2]; bounds not ascending from 0 to N) sets a bit here; ss_device_errors reads
 // and clears it.  bit 0: index out of range, bit 1: bounds not monotone / not ending at N, bit 2: a moving window's
-// start outside [0, N - win_len] (clamped), bit 3: a pooled slot's pick outside [0, n) (clamped).
+// start outside [0, N - win_len] (clamped), bit 3: a pooled slot's pick outside [0, n) (clamped), bit 4: a dry pick
+// outside [0, n) of its dry pool (clamped).
 __device__ unsigned g_dev_err;
 
 // twiddle tables, filled from the host in double precision (ss_create)
@@ -115,6 +116,7 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 // A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate - its RIR partition count
 // when the pool's candidates differ in K (pick_parts), and its loudness gain, counts[11] - into its Source in the
 // descriptor block (pick_slot), which is why k_prepare then reads the Source table from global memory (k_prepare<false>).
+// A dry-picked slot then reads its dry pick, clamps it (bit 4) and puts the picked dry signal in place of x (pick_dry).
 __global__ void __launch_bounds__(256)
 k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -127,11 +129,8 @@ k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
                 if (sv) {
                     take_view(S, *sv);                  // a host pool: k_stage picked (bit 3) and staged the candidate
                 } else {
-                    bool bad;
-                    const int v = *pick_ptr(S);
-                    pick_parts(S, v);                   // the picked candidate's K first: set_banked reads it
-                    pick_slot(S, v, bad);
-                    if (bad) atomicOr(&g_dev_err, 8u);
+                    const unsigned err = pick_pooled(S);   // the pick (bit 3), and a dry pick (bit 4)
+                    if (err) atomicOr(&g_dev_err, err);
                 }
             }
             __syncwarp();
@@ -841,6 +840,18 @@ struct ss_pool {
     size_t aux_bytes = 0;
     std::vector<std::pair<int, std::pair<int, int>>> stage_caps;  // (win_len, (rows, dry samples)) (stage_cap)
 };
+// Dry pool: n dry signals referenced by their device pointers (the caller's buffers), the device array of those pointers
+// that dry-picked slots index (dry_table), and with SS_DRY_LEVELS every signal's level table.
+struct ss_dry_pool {
+    ss_ctx* c = nullptr;
+    int n = 0, n_min = 0;                 // n_min: the shortest signal (the longest candidate N it serves)
+    const float** ptrs = nullptr;         // device, n signal pointers
+    std::vector<const float*> x;          // the same pointers on the host
+    std::vector<int32_t> N;
+    double* levels = nullptr;             // device: every signal's N + 1 doubles back to back
+    const double** level_ptr = nullptr;   // device, n table pointers
+    std::vector<int64_t> level_off;       // signal i's table at levels + level_off[i]
+};
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
 static int wait_banks(const ss_source* items, int n, cudaStream_t stream) {
@@ -1127,9 +1138,9 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
     return true;
 }
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
-// block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts) and
-// [18..19] (stage_view), 80 bytes
-static size_t counts_bytes(const Shape& sh) { return sh.pooled ? 80 : sh.win ? 64 : 16; }
+// block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts),
+// [18..19] (stage_view) and [20..24] (dry_table, dry_pick_ptr, dry_size), 112 bytes
+static size_t counts_bytes(const Shape& sh) { return sh.pooled ? 112 : sh.win ? 64 : 16; }
 static const float kUnitGain = 1.0f;      // counts[11] of every windowed source until a pooled slot picks (stem_gain)
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
 // counts (windowed source, device-built tables)
@@ -1150,7 +1161,8 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
 // Fill the descriptor block of items[first, last) at `hbase` (host memory) for its device address `dbase`, carve the
 // chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.
 static void chunk_describe(const ss_source* items, const Shape* shapes, int first, int last, char* hbase, char* dbase,
-                           char* scratch, int sm_count, ChunkLaunch* L, StageView* const* views = nullptr) {
+                           char* scratch, int sm_count, ChunkLaunch* L, StageView* const* views = nullptr,
+                           const ss_dry_pick* const* dry = nullptr) {
     const int n = last - first;
     const bool host_tables = chunk_host_tables(items, first, last);
     const size_t off_ps = align_up(sizeof(Source) * n, 16);
@@ -1228,6 +1240,12 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                     memcpy(hb_counts + 14, &it.pool->gains, sizeof(it.pool->gains));
                     memcpy(hb_counts + 16, &it.pool->parts, sizeof(it.pool->parts));
                     if (views) memcpy(hb_counts + 18, &views[first + i], sizeof(StageView*));   // stage_view
+                    if (dry && dry[first + i]) {            // dry_table, dry_pick_ptr, dry_size
+                        const ss_dry_pick& d = *dry[first + i];
+                        memcpy(hb_counts + 20, &d.pool->ptrs, sizeof(d.pool->ptrs));
+                        memcpy(hb_counts + 22, &d.pick_dev, sizeof(d.pick_dev));
+                        hb_counts[24] = d.pool->n;
+                    }
                 }
             } else {
                 s.counts = (int*)scratch;
@@ -1643,18 +1661,23 @@ static void make_chunks(const ss_source* items, const Shape* shapes, int n, int6
 // else (k_render<0, 0>) - and each group
 // is chunked on its own: one static source no longer sends the moving sources of its chunk through the generic kernel
 // (a SonicSet scene is 3 moving + 2 static sources).  `arranged` / `arranged_shapes` receive the regrouped items and
-// their shapes, `cuts` the chunk bounds.
+// their shapes, `cuts` the chunk bounds, and `order` (when given) the caller's index of every arranged item.
 static void arrange_chunks(const ss_ctx* c, const ss_source* items, const Shape* shapes, int n,
-                           std::vector<ss_source>& arranged, std::vector<Shape>& arranged_shapes, std::vector<int>& cuts) {
+                           std::vector<ss_source>& arranged, std::vector<Shape>& arranged_shapes, std::vector<int>& cuts,
+                           std::vector<int>* order = nullptr) {
     arranged.clear(); arranged.reserve(n);
     arranged_shapes.clear(); arranged_shapes.reserve(n);
     cuts.clear(); cuts.push_back(0);
+    if (order) order->clear();
     for (int cls = 0; cls < 3; ++cls) {
         const int lo = (int)arranged.size();
         for (int i = 0; i < n; ++i) {
             const Shape& sh = shapes[i];
             const int k = sh.K > 1 ? 1 : (one_transform_per_item(sh.aligned, items[i].mode, sh.K) ? 0 : 2);
-            if (k == cls) { arranged.push_back(items[i]); arranged_shapes.push_back(sh); }
+            if (k == cls) {
+                arranged.push_back(items[i]); arranged_shapes.push_back(sh);
+                if (order) order->push_back(i);
+            }
         }
         const int cnt = (int)arranged.size() - lo;
         if (cnt == 0) continue;
@@ -1992,6 +2015,75 @@ extern "C" int ss_pool_levels(ss_pool* pl, uint32_t flags) {
     return SS_OK;
 }
 
+// ----------------------------------------------------------------------------- dry pools
+extern "C" void ss_dry_pool_destroy(ss_dry_pool* dp) {
+    if (!dp) return;
+    cudaSetDevice(dp->c->device);
+    cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
+    if (dp->ptrs) cudaFree(dp->ptrs);
+    if (dp->levels) cudaFree(dp->levels);
+    if (dp->level_ptr) cudaFree(dp->level_ptr);
+    delete dp;
+}
+extern "C" int64_t ss_dry_pool_bytes(const ss_dry_pool* dp) {
+    if (!dp) return 0;
+    int64_t b = (int64_t)sizeof(float*) * dp->n;
+    if (dp->levels) b += (int64_t)sizeof(double) * dp->level_off[dp->n] + (int64_t)sizeof(double*) * dp->n;
+    return b;
+}
+extern "C" const double* ss_dry_pool_level_table(const ss_dry_pool* dp, int i) {
+    return dp && dp->levels && i >= 0 && i < dp->n ? dp->levels + dp->level_off[i] : nullptr;
+}
+// The signals' pointer array, and with level tables the tables - k_levels over each signal as a one-channel stem, whose
+// mono fold is the signal itself - built on a transient stream; returns when they are in device memory.
+static int dry_pool_build(ss_dry_pool* dp, bool levels) {
+    const int n = dp->n;
+    CK(cudaMalloc((void**)&dp->ptrs, sizeof(float*) * (size_t)n));
+    CK(cudaMemcpy(dp->ptrs, dp->x.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice));
+    if (!levels) return SS_OK;
+    dp->level_off.assign(n + 1, 0);
+    for (int i = 0; i < n; ++i) dp->level_off[i + 1] = dp->level_off[i] + dp->N[i] + 1;
+    CK(cudaMalloc((void**)&dp->levels, sizeof(double) * (size_t)dp->level_off[n]));
+    CK(cudaMalloc((void**)&dp->level_ptr, sizeof(double*) * (size_t)n));
+    std::vector<const double*> ptr(n);
+    std::vector<LevelItem> li(n);
+    for (int i = 0; i < n; ++i) {
+        ptr[i] = dp->levels + dp->level_off[i];
+        li[i] = {dp->x[i], dp->levels + dp->level_off[i], dp->N[i], 1, 0};
+    }
+    CK(cudaMemcpy(dp->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
+    LevelItem* d_items = nullptr;
+    CK(cudaMalloc((void**)&d_items, sizeof(LevelItem) * (size_t)n));
+    struct Free { void* p; ~Free() { cudaFree(p); } } free_items{d_items};   // (cudaFree waits for the device)
+    CK(cudaMemcpy(d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
+    BuildStream bs;
+    CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
+    for (int k = 0; k < n; k += 65535) {
+        const int st = levels_enqueue(dp->c, d_items + k, std::min(n - k, 65535), true, bs.s);
+        if (st) return st;
+    }
+    CK(cudaStreamSynchronize(bs.s));
+    return SS_OK;
+}
+extern "C" int ss_dry_pool_create(ss_ctx* c, const float* const* x, const int32_t* lengths, int n, uint32_t flags,
+                                  ss_dry_pool** out) {
+    if (!c || !x || !lengths || !out || n < 1 || n > (1 << 24) || (flags & ~SS_DRY_LEVELS)) return SS_ERR_INVALID;
+    *out = nullptr;
+    for (int i = 0; i < n; ++i)                         // (the bound of validate_item on N)
+        if (!x[i] || ((uintptr_t)x[i] & 3) || lengths[i] < 1 || lengths[i] > 0x7fffffff - 2 * kF) return SS_ERR_INVALID;
+    CK(cudaSetDevice(c->device));
+    ss_dry_pool* dp = new (std::nothrow) ss_dry_pool();
+    if (!dp) return SS_ERR_NOMEM;
+    dp->c = c; dp->n = n;
+    dp->x.assign(x, x + n);
+    dp->N.assign(lengths, lengths + n);
+    dp->n_min = *std::min_element(lengths, lengths + n);
+    const int st = dry_pool_build(dp, (flags & SS_DRY_LEVELS) != 0);
+    if (st != SS_OK) { ss_dry_pool_destroy(dp); return st; }
+    *out = dp;
+    return SS_OK;
+}
+
 // ----------------------------------------------------------------------------- plans (device path)
 // A batch of device-resident sources bound once: validation, chunking, block tables and descriptor blocks are done at
 // creation and stay resident in device memory together with the plan's own scratch, so a run is kernel launches only -
@@ -2024,14 +2116,18 @@ struct ss_plan {
 
 // ----------------------------------------------------------------------------- k_draw
 // Crop start draws of a plan (ss_plan_draw).  A reader is a pooled slot whose win_start_dev is the draw's start; the
-// speakers are readers with level tables.  The picks are clamped as k_blocks clamps them (which reports bit 3).
+// speakers are readers with level tables: their pool's, or their dry pool's for a dry-picked speaker (speaker_table).  The
+// picks are clamped as k_blocks clamps them (which reports bits 3 and 4).
 constexpr int kDrawReaders = 16, kDrawSpeakers = 8, kDrawTries = 4096, kMaxDraws = 65535;
 struct DrawReader {
     const PoolEntry* pool;            // the slot's pool table ...
     const int* pick;                  // ... and pick
-    const double* const* levels;      // the pool's level table pointers (speakers), else null
+    const double* const* levels;      // the pool's level table pointers (speakers without a dry pick), else null
     int n;                            // candidates in the pool
-    double D;                         // elements of one crop in a table: len (mono) or C * len
+    double D;                         // elements of one crop in a table: len (mono or dry) or C * len
+    const double* const* dry_levels;  // a dry-picked speaker: its dry pool's table pointers, else null ...
+    const int* dry_pick;              // ... its dry pick ...
+    int n_dry;                        // ... and the dry pool's signal count
 };
 struct DrawDesc {
     int* start;
@@ -2064,7 +2160,7 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
         Q[k] = nullptr; D[k] = 1.0;
         if (k < d.S) {
             const DrawReader& r = d.r[d.spk[k]];
-            Q[k] = r.levels[clamp_pick(*r.pick, r.n, bad)];
+            Q[k] = speaker_table(r.levels, r.pick, r.n, r.dry_levels, r.dry_pick, r.n_dry);
             D[k] = r.D;
         }
     }
@@ -2188,7 +2284,8 @@ static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double
 }
 
 // The descriptor of draw d of a plan: its readers in the callers' order of `items`
-static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan_draw& d) {
+// (dry[i]: item i's dry pick, or null; a dry-picked speaker tests its dry pool's one-channel tables, D = len)
+static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan_draw& d, const ss_dry_pick* const* dry) {
     DrawDesc g; memset(&g, 0, sizeof(g));
     g.start = d.start; g.u = d.u; g.used = d.used; g.tries = d.tries; g.S = d.S; g.threshold_db = d.threshold_db;
     for (int i = 0; i < n_items; ++i) {
@@ -2197,8 +2294,10 @@ static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan
         for (int k = 0; k < d.S; ++k) if (d.speakers[k] == i) g.spk[k] = g.n_readers;
         const ss_pool* pl = it.pool;
         g.len = it.win_len;
-        g.r[g.n_readers++] = {pl->table, it.pick_dev, pl->level_ptr, pl->n,
-                              (double)it.win_len * ((pl->level_flags & SS_MIX_MONO) ? 1 : pl->C)};
+        DrawReader r = {pl->table, it.pick_dev, pl->level_ptr, pl->n,
+                        (double)it.win_len * ((pl->level_flags & SS_MIX_MONO) ? 1 : pl->C), nullptr, nullptr, 0};
+        if (dry[i]) { r.dry_levels = dry[i]->pool->level_ptr; r.dry_pick = dry[i]->pick_dev; r.n_dry = dry[i]->pool->n; r.D = it.win_len; }
+        g.r[g.n_readers++] = r;
     }
     return g;
 }
@@ -2224,13 +2323,17 @@ static size_t stage_bytes(const ss_source& it) {
            align_up(sizeof(float) * (size_t)cap.second, 256);
 }
 
+// (dry[i]: caller item i's dry pick, or null)
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
-                      const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws) {
+                      const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws,
+                      const ss_dry_pick* const* dry) {
     ss_ctx* c = p->c;
-    std::vector<int> cuts;
+    std::vector<int> cuts, order;
     std::vector<ss_source> arranged;
     std::vector<Shape> arranged_shapes;
-    arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts);
+    arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
+    std::vector<const ss_dry_pick*> dry_arranged(arranged.size());
+    for (size_t i = 0; i < arranged.size(); ++i) dry_arranged[i] = dry[order[i]];
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     const size_t n_chunks = cuts.size() - 1;
     std::vector<size_t> off(n_chunks + 1, 0);
@@ -2280,7 +2383,8 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     p->chunks.resize(n_chunks);
     for (size_t k = 0; k < n_chunks; ++k)
         chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
-                       p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data());
+                       p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data(),
+                       dry_arranged.data());
     for (int k = 0; k < n_mixes; ++k)
         ((MixItem*)(host.data() + mix_off))[k] =
             mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
@@ -2291,7 +2395,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     CK(cudaMemcpy(p->d_desc, host.data(), scr_off, cudaMemcpyHostToDevice));
     if (n_draws > 0) {
         std::vector<DrawDesc> g(n_draws);
-        for (int k = 0; k < n_draws; ++k) g[k] = draw_describe(caller_items, n_items, draws[k]);
+        for (int k = 0; k < n_draws; ++k) g[k] = draw_describe(caller_items, n_items, draws[k], dry);
         CK(cudaMemcpy(p->d_desc + draw_off, g.data(), sizeof(DrawDesc) * n_draws, cudaMemcpyHostToDevice));
         p->d_draw = (const DrawDesc*)(p->d_desc + draw_off);
         p->n_draw = n_draws;
@@ -2322,7 +2426,8 @@ static bool written_ranges_disjoint(std::vector<ByteRange>& r) {
 }
 
 // A plan's start draws (include/sonicsim_b200.h, ss_plan_draw), all but the byte ranges (validate_mixes)
-static int validate_draws(const ss_source* items, int n_items, const ss_plan_draw* draws, int n_draws) {
+static int validate_draws(const ss_source* items, int n_items, const ss_plan_draw* draws, int n_draws,
+                          const ss_dry_pick* const* dry) {
     if (n_draws > kMaxDraws) return SS_ERR_UNSUPPORTED;
     for (int k = 0; k < n_draws; ++k) {
         const ss_plan_draw& d = draws[k];
@@ -2335,7 +2440,9 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
             if (i < 0 || i >= n_items) return SS_ERR_INVALID;
             for (int j = 0; j < s; ++j) if (d.speakers[j] == i) return SS_ERR_INVALID;
             const ss_source& it = items[i];
-            if (!it.pool || !it.pool->levels || it.win_start_dev != d.start) return SS_ERR_INVALID;
+            // level tables to test: the dry pool's for a dry-picked speaker, else the pool's
+            if (!it.pool || it.win_start_dev != d.start) return SS_ERR_INVALID;
+            if (dry[i] ? !dry[i]->pool->levels : !it.pool->levels) return SS_ERR_INVALID;
         }
         int readers = 0, len = -1;
         for (int i = 0; i < n_items; ++i) {
@@ -2351,7 +2458,7 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
 }
 
 static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
-                          const ss_plan_draw* draws, int n_draws) {
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks) {
     if (n_mixes > 65535) return SS_ERR_UNSUPPORTED;         // one gridDim.y row per mixture
     std::vector<ByteRange> r;
     // a draw writes its start (which only its readers read) and `used`, and reads its u
@@ -2411,18 +2518,47 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
             add_range(r, e.x, 4 * (uint64_t)e.N, false);
             add_range(r, e.bounds, 4 * (uint64_t)e.P, false);
         }
+    // a dry-picked slot may read any signal of its dry pool, and reads its dry pick
+    std::vector<const ss_dry_pool*> dpools;
+    for (int k = 0; k < n_picks; ++k) {
+        add_range(r, picks[k].pick_dev, 4, false);
+        if (std::find(dpools.begin(), dpools.end(), picks[k].pool) == dpools.end()) dpools.push_back(picks[k].pool);
+    }
+    for (const ss_dry_pool* dp : dpools)
+        for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
 
+// A plan's dry picks (include/sonicsim_b200.h, ss_dry_pick), all but the byte ranges (validate_mixes): dry[i] receives
+// item i's pick, or null
+static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_items, const ss_dry_pick* picks,
+                              int n_picks, std::vector<const ss_dry_pick*>& dry) {
+    dry.assign(n_items, nullptr);
+    for (int k = 0; k < n_picks; ++k) {
+        const ss_dry_pick& d = picks[k];
+        if (d.slot < 0 || d.slot >= n_items || dry[d.slot]) return SS_ERR_INVALID;      // one dry pick per slot
+        if (!d.pool || d.pool->c != c || !d.pick_dev || ((uintptr_t)d.pick_dev & 3)) return SS_ERR_INVALID;
+        const ss_pool* pl = items[d.slot].pool;
+        // a pooled slot of a device pool without gains (k_stage stages the candidate's own x; the gains were measured
+        // with it), whose every candidate's N the dry pool's shortest signal covers
+        if (!pl || pl->host_res || pl->gains) return SS_ERR_INVALID;
+        for (const PoolEntry& e : pl->host) if (e.N > d.pool->n_min) return SS_ERR_INVALID;
+        dry[d.slot] = &d;
+    }
+    return SS_OK;
+}
+
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
-                       const ss_plan_draw* draws, int n_draws, ss_plan** out) {
+                       const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks, ss_plan** out) {
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
+    std::vector<const ss_dry_pick*> dry;
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
-    { int st = validate_draws(items, n_items, draws, n_draws); if (st) return st; }
-    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws); if (st) return st; }
+    { int st = validate_dry_picks(c, items, n_items, picks, n_picks, dry); if (st) return st; }
+    { int st = validate_draws(items, n_items, draws, n_draws, dry.data()); if (st) return st; }
+    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
@@ -2432,7 +2568,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws);
+    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data());
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -2440,19 +2576,28 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 }
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
-    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                  int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                  int n_picks, ss_plan** out) {
+    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
+        (n_picks > 0 && !picks))
+        return SS_ERR_INVALID;
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start

@@ -44,7 +44,8 @@ struct Source {
                            // source (h_rows != 0): [2] = first block that meets the window, [3] = blocks that do,
                            // [4] = win_start, [5] = win_len, [6..7] = device pointer of a moving window's start or
                            // null (win_start_ptr); tables built on the device: [8..17] the pool of a pooled slot
-                           // (pool_table, pool_size, pick_ptr, pool_gains, pool_parts)
+                           // (pool_table, pool_size, pick_ptr, pool_gains, pool_parts), [18..19] its stage view,
+                           // [20..24] its dry pick (dry_table, dry_pick_ptr, dry_size)
     const float* norm_part;// scratch: kNormParts partial abs-maxima of the RIR tensor (k_rir_absmax), or null: taps used as given
     int* cut;              // scratch: P*C direct-path row lengths (k_rir_direct), or null: no direct target
     float* out_direct;     // (C, N) direct-path stem (with `cut`)
@@ -369,6 +370,32 @@ SS_HD void take_view(Source& s, const StageView& v) {
     s.h_row0 = v.row0; s.h_rows = v.rows;
     set_stem_gain(s, v.gain);
 }
+// ---- dry pools (ss_dry_pool, include/sonicsim_b200.h).  A dry-picked slot of a device pool renders its picked
+// candidate with the dry signal its own pick names in a dry pool.  Its counts block is 112 bytes, as every pooled slot's:
+// [20..21] the device pointer of the dry pool's n signal pointers, or null (no dry pick), [22..23] the device pointer of
+// the dry pick, [24] the dry pool's signal count.
+SS_HD const float* const* dry_table(const Source& s) { return *reinterpret_cast<const float* const* const*>(s.counts + 20); }
+SS_HD const int* dry_pick_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 22); }
+SS_HD int dry_size(const Source& s) { return s.counts[24]; }
+// The dry pick v read from device memory, clamped into [0, n) (bad = it was not there): the picked signal replaces the
+// candidate's own x.  Everything else - N, P, bounds, K, spectra, cuts, gain - stays the trajectory candidate's, and only
+// samples [0, N) of x are read, so a dry signal at least N long renders as that candidate with the signal's first N.
+SS_HD void pick_dry(Source& s, int v, bool& bad) { s.x = dry_table(s)[clamp_pick(v, dry_size(s), bad)]; }
+// The head of k_blocks for a pooled slot of a device pool: the trajectory pick (its K, then its candidate and gain), then
+// the dry pick of a dry-picked slot.  Returns the error bits to report: 8 for a clamped pick, 16 for a clamped dry pick.
+SS_HD unsigned pick_pooled(Source& s) {
+    bool bad;
+    unsigned err = 0;
+    const int v = *pick_ptr(s);
+    pick_parts(s, v);                       // the picked candidate's K first: set_banked reads it
+    pick_slot(s, v, bad);
+    if (bad) err |= 8u;
+    if (dry_table(s)) {
+        pick_dry(s, *dry_pick_ptr(s), bad);
+        if (bad) err |= 16u;
+    }
+    return err;
+}
 // ---- crop start draws of device plans (ss_plan_draw, include/sonicsim_b200.h): the dataloader's start loop
 // (movingdatamodule.py:81-99) over level tables Q (ss_pool_levels: Q[0] = 0, Q[n + 1] = Q[n] + e[n], float64).
 // Starts a crop of len samples can take in a candidate of N samples: the M of a draw is the least of these over its readers
@@ -386,6 +413,14 @@ SS_HD bool draw_silent(const double* Q, int s, int len, double D, float threshol
     double ms = (Q[s + len] - Q[s]) / D;
     if (ms < 1e-20) ms = 1e-20;
     return 10.0 * log10(ms) < (double)threshold_db;
+}
+// The level table a draw tests for one speaker: a dry-picked speaker's (dry_levels non-null) is its dry pool's table of
+// the picked dry signal, whose crops have D = len; any other's is its pool's table of the picked candidate.  Both picks
+// are clamped as k_blocks clamps them.
+SS_HD const double* speaker_table(const double* const* levels, const int* pick, int n, const double* const* dry_levels,
+                                  const int* dry_pick, int n_dry) {
+    bool bad;
+    return dry_levels ? dry_levels[clamp_pick(*dry_pick, n_dry, bad)] : levels[clamp_pick(*pick, n, bad)];
 }
 
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed

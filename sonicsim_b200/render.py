@@ -78,11 +78,27 @@ class Pooled(T.NamedTuple):
     `window` = (start, length) as MovingSource.window: the start an int or a one-element CUDA int32 tensor; the length
     at most every candidate's N.  The output is (C, length).  `direct_taps` > 0 also renders the direct-path stem, which
     needs every candidate's bank to hold a direct set with these taps.  A pick outside [0, n) is clamped into range and a
-    start beyond the picked candidate's N - length is clamped too (check_device_errors).  Only plan_device takes it."""
+    start beyond the picked candidate's N - length is clamped too (check_device_errors).  Only plan_device takes it.
+    `dry`, a DryPick, makes it a dry-picked slot: the picked candidate renders with the dry signal the DryPick names in
+    place of its own."""
     pool: T.Any
     pick: T.Any
     window: T.Tuple[T.Any, int]
     direct_taps: int = 0
+    dry: T.Any = None
+
+
+class DryPick(T.NamedTuple):
+    """The dry signal of a pooled slot (Pooled.dry), picked on the device at every run independently of the slot's
+    candidate: `pool` a DryPool (Renderer.dry_pool), `pick` a one-element CUDA int32 tensor (e.g. dry_picks[b, k] of a
+    (B, S) tensor) naming one of its signals.  At every run the slot renders its picked candidate - RIRs, trajectory, N,
+    blocking unchanged - with the first N samples of that signal as its dry signal, bit for bit what render_device gives
+    for the candidate with that dry signal and the same window.  A pick outside [0, n) is clamped into range
+    (check_device_errors raises IndexError).  Every signal of the pool must be at least as long as the slot pool's longest
+    candidate; host pools and pools with loudness gains take no dry picks.  In a CropDraw, a dry-picked speaker is tested
+    on its dry crop, from the dry pool's level tables (dry_pool(..., levels=True))."""
+    pool: T.Any
+    pick: T.Any
 
 
 class CropDraw(T.NamedTuple):
@@ -258,8 +274,9 @@ class SourcePool(_Held):
     copies only what its slots read (ss_pool_host_bytes, INTEGRATION.md)."""
 
     def __init__(self, renderer, handle, candidates, mode, C, L, n_min, direct_taps, levels=None, loudness=None,
-                 sizes=None, resident="device"):
+                 sizes=None, resident="device", gains=False):
         self.renderer, self._h = renderer, handle
+        self.gains = bool(gains)                           # loudness gains (lufs_targets): no dry picks
         self.candidates = list(candidates)
         self.resident = resident
         self._sizes = list(sizes) if sizes is not None else [int(s.dry.numel()) for s in self.candidates]
@@ -297,6 +314,41 @@ class SourcePool(_Held):
             self.renderer.lib.ss_pool_destroy(self._h)
             self._h = ctypes.c_void_p()
             self._banks()                      # the pool no longer reads its banks
+
+
+class DryPool(_Held):
+    """A set of `n` float32 dry signals on the device (Renderer.dry_pool; ss_dry_pool of the C ABI), which dry-picked
+    slots (DryPick) take their dry signal from at every run.  `n_min` is the shortest signal's length: the longest
+    candidate N a pool of slots that pick from it may have.  With `levels` True it holds every signal's level table
+    (float64 prefix sums of its squares, 8 bytes per sample, in `nbytes`), which CropDraw reads for dry-picked speakers.
+    The pool references the signals' tensors and keeps them alive; plans hold the pool, which is freed once it is closed
+    (or collected) and no live plan uses it."""
+
+    def __init__(self, renderer, handle, signals, levels):
+        self.renderer, self._h = renderer, handle
+        self.signals = list(signals)
+        self.n, self.levels = len(self.signals), bool(levels)
+        self.n_min = min(int(x.numel()) for x in self.signals)
+        self.nbytes = int(renderer.lib.ss_dry_pool_bytes(handle))
+
+    def level_table(self, i):
+        """A float64 CUDA copy of signal i's level table (N + 1 values: Q[0] = 0, Q[n + 1] = Q[n] + x[n]^2), or None
+        without tables."""
+        import torch
+        if self.closed or not self.levels or not 0 <= i < self.n:
+            return None
+        ptr = self.renderer.lib.ss_dry_pool_level_table(self._h, int(i))
+        n = int(self.signals[i].numel()) + 1
+
+        class _View:
+            __cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (ptr, False), "version": 3}
+        with torch.cuda.device(self.renderer.device):
+            return torch.as_tensor(_View(), device="cuda:%d" % self.renderer.device).clone()
+
+    def _free(self):
+        if self._h:
+            self.renderer.lib.ss_dry_pool_destroy(self._h)
+            self._h = ctypes.c_void_p()
 
 
 def _rirs(s, conv=None):
@@ -379,9 +431,10 @@ def _hold_banks(plan, sources):
     releases them at once, once)."""
     banks = []
     for s in sources:
-        b = s.pool if isinstance(s, Pooled) else _rirs(s)[0]
-        if isinstance(b, (RirBank, SourcePool)) and all(b is not o for o in banks):
-            banks.append(b)
+        held = [s.pool, s.dry.pool if isinstance(s.dry, DryPick) else None] if isinstance(s, Pooled) else [_rirs(s)[0]]
+        for b in held:
+            if isinstance(b, (RirBank, SourcePool, DryPool)) and all(b is not o for o in banks):
+                banks.append(b)
     for b in banks:
         b._hold()
     return weakref.finalize(plan, _release_banks, banks)
@@ -567,7 +620,35 @@ class Renderer:
             _lib.check(st)
         taps = {_rirs(s)[0].direct_taps for s in candidates}
         return SourcePool(self, h, candidates, first[0], first[1], L_max, min(sizes),
-                          taps.pop() if len(taps) == 1 else 0, levels, loud, sizes, "host" if host else "device")
+                          taps.pop() if len(taps) == 1 else 0, levels, loud, sizes, "host" if host else "device",
+                          post is not None)
+
+    # ------------------------------------------------------------------ dry pools
+    def dry_pool(self, signals: T.Sequence[T.Any], levels: bool = False) -> DryPool:
+        """A DryPool over `signals`: 1 to 2^24 contiguous 1-D CUDA float32 tensors of this renderer's device, referenced
+        (not copied) and kept alive by the pool, for dry-picked pooled slots (DryPick) of device plans.  `levels` also
+        builds every signal's level table, which start draws (CropDraw) test dry-picked speakers with; the call then
+        returns when the tables are complete, and they describe the signals as they are now."""
+        import torch
+        n = len(signals)
+        if not 1 <= n <= 1 << 24:
+            raise ValueError("dry_pool: a dry pool holds 1 to 2^24 signals, got %d" % n)
+        ptrs = (ctypes.c_void_p * n)()
+        lengths = np.empty(n, np.int32)
+        for i, x in enumerate(signals):
+            own = "signal %d" % i
+            ptrs[i] = _tensor(x, "dry_pool", own, "dry", torch.float32, self.device)
+            if x.dim() != 1 or x.numel() < 1:
+                raise ValueError("dry_pool: %s must be 1-D and not empty, got shape %s" % (own, tuple(x.shape)))
+            if x.numel() > 0x7fffffff - 16384:
+                raise ValueError("dry_pool: %s has %d samples, at most %d" % (own, x.numel(), 0x7fffffff - 16384))
+            lengths[i] = x.numel()
+        if levels:                             # the tables are built on the library's own stream: finish the writes
+            torch.cuda.current_stream(self.device).synchronize()
+        h = ctypes.c_void_p()
+        _lib.check(self.lib.ss_dry_pool_create(self.ctx, ptrs, lengths.ctypes.data, n,
+                                               _lib.SS_DRY_LEVELS if levels else 0, ctypes.byref(h)))
+        return DryPool(self, h, signals, levels)
 
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
@@ -676,11 +757,48 @@ class Renderer:
         below the threshold, before anything reads that start.  A step is then
 
             u.uniform_(); picks.copy_(...); sirs.uniform_(-6, 6); snr.uniform_(10, 20)
-            plan.run()"""
+            plan.run()
+
+        A Pooled slot with `dry` = DryPick(dry_pool, pick) also takes its dry signal from a DryPool at every run, so
+        that every (dry signal, trajectory) pair is reachable in the same single graph launch
+        (dry_picks.random_(0, n) before the run)."""
+        dry = self._device_dry(sources)
         items, n, keep = self._device_items(sources, outs, direct_outs)
         mixes = self._device_mixes(mixtures, outs, keep) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
-        return DevicePlan(self, items, n, keep, mixes, drw)
+        return DevicePlan(self, items, n, keep, mixes, drw, dry)
+
+    def _device_dry(self, sources):
+        """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
+        import torch
+        picks = []
+        for i, s in enumerate(sources):
+            d = getattr(s, "dry", None)
+            if not isinstance(s, Pooled):
+                if isinstance(d, DryPick):
+                    raise ValueError("plan_device: source %d has a DryPick but is not a pooled slot (render.Pooled)" % i)
+                continue
+            if d is None:
+                continue
+            if not isinstance(d, DryPick):
+                raise ValueError("plan_device: the dry of pooled source %d must be a DryPick or None" % i)
+            if not isinstance(d.pool, DryPool):
+                raise ValueError("plan_device: the dry pool of source %d must be a DryPool" % i)
+            _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
+            pl = s.pool
+            if isinstance(pl, SourcePool):
+                if pl.resident == "host":
+                    raise ValueError("plan_device: pooled source %d has a dry pick over a host pool, whose runs stage "
+                                     "each candidate's own dry signal" % i)
+                if pl.gains:
+                    raise ValueError("plan_device: pooled source %d has a dry pick over a pool with loudness gains, "
+                                     "which were measured with the candidates' own dry signals" % i)
+                if d.pool.n_min < max(pl._sizes):
+                    raise ValueError("plan_device: the DryPool of source %d holds a signal of %d samples, shorter than "
+                                     "its pool's longest candidate (N = %d)" % (i, d.pool.n_min, max(pl._sizes)))
+            pick = _tensor(d.pick, "plan_device", "source %d" % i, "dry pick", torch.int32, self.device, count=(1, 1))
+            picks.append(_lib.SsDryPick(slot=i, pool=d.pool._h.value, pick_dev=pick))
+        return (_lib.SsDryPick * len(picks))(*picks) if picks else None
 
     def _device_draws(self, draws, sources, keep):
         """Validated ss_plan_draw array of a plan's start draws; their tensors are appended to `keep`."""
@@ -724,7 +842,12 @@ class Renderer:
                 if v not in readers:
                     raise ValueError("plan_device: speaker %d of draw %d does not take its window start from the "
                                      "draw's start tensor" % (v, k))
-                if sources[v].pool.levels is None:
+                dry = sources[v].dry
+                if isinstance(dry, DryPick):
+                    if not dry.pool.levels:
+                        raise ValueError("plan_device: speaker %d of draw %d: its DryPool has no level tables "
+                                         "(dry_pool(levels=True))" % (v, k))
+                elif sources[v].pool.levels is None:
                     raise ValueError("plan_device: speaker %d of draw %d: its SourcePool has no level tables "
                                      "(source_pool(levels=...))" % (v, k))
             e = arr[k]
@@ -850,6 +973,9 @@ class Renderer:
         if bits.value & 8:
             raise IndexError("a pick on the device was out of range for the candidates of its SourcePool; it was clamped "
                              "into [0, n)")
+        if bits.value & 16:
+            raise IndexError("a dry pick on the device was out of range for the signals of its DryPool; it was clamped "
+                             "into [0, n)")
         if bits.value & 2:
             raise ValueError("a device-side trajectory bounds table is not ascending from 0 to N")
         if bits.value & 4:
@@ -878,15 +1004,17 @@ class Renderer:
 class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
-    mixtures, the plan also assembles them at every run; with draws, it first draws their starts (ss_plan_create_ex)."""
+    mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
+    dry-picked slots take their dry signals from dry pools (ss_plan_create_dry)."""
 
-    def __init__(self, renderer, items, n, keep, mixes=None, draws=None):
+    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
-        self.draws = draws
+        self.draws, self.dry = draws, dry
         self._plan = ctypes.c_void_p()
         if n > 0:
-            _lib.check(renderer.lib.ss_plan_create_ex(renderer.ctx, items, n, mixes, len(mixes) if mixes else 0,
-                                                      draws, len(draws) if draws else 0, ctypes.byref(self._plan)))
+            _lib.check(renderer.lib.ss_plan_create_dry(renderer.ctx, items, n, mixes, len(mixes) if mixes else 0,
+                                                       draws, len(draws) if draws else 0, dry, len(dry) if dry else 0,
+                                                       ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
