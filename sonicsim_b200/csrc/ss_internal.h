@@ -58,6 +58,33 @@ extern thread_local int g_last_cuda;
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// Grow-on-demand buffers of a context.  Growing waits for the whole device first: the old buffer may still be read by
+// work on any stream.  ensure: the device buffer *p of *cap bytes to at least `need` (need + need / 4, in whole MB, so
+// that slowly growing calls reallocate rarely).  ensure_pair: a pinned host block *h and its device twin *d, *cap bytes
+// each, to at least `need` (twice `need`, in whole 4 KB pages).
+inline int ensure(char** p, size_t* cap, size_t need) {
+    if (need <= *cap) return SS_OK;
+    CK(cudaDeviceSynchronize());
+    if (*p) CK(cudaFree(*p));
+    *p = nullptr; *cap = 0;
+    const size_t grown = align_up(need + need / 4, 1 << 20);
+    CK(cudaMalloc((void**)p, grown));
+    *cap = grown;
+    return SS_OK;
+}
+inline int ensure_pair(char** h, char** d, size_t* cap, size_t need) {
+    if (need <= *cap) return SS_OK;
+    CK(cudaDeviceSynchronize());
+    if (*h) CK(cudaFreeHost(*h));
+    if (*d) CK(cudaFree(*d));
+    *h = nullptr; *d = nullptr; *cap = 0;
+    const size_t grown = align_up(need * 2, 4096);
+    CK(cudaHostAlloc((void**)h, grown, cudaHostAllocDefault));
+    CK(cudaMalloc((void**)d, grown));
+    *cap = grown;
+    return SS_OK;
+}
+
 // data[i] *= (float)result[1] over the N * C floats of each item, with k_loud_scale's arithmetic: a stem that takes the
 // linear gain another stem's loudness measurement left in `result` (ss_render_host_ex: the direct-path stem takes its
 // reverberant stem's gain, so that target and mixture stay consistent).  Device pointers, asynchronous on `stream`.
@@ -115,15 +142,7 @@ inline int ring_acquire(ss_ctx* c, size_t bytes, cudaStream_t stream, int* slot_
     const int slot = c->ring_pos; c->ring_pos = (c->ring_pos + 1) % ss_ctx::kRing;
     CK(cudaEventSynchronize(c->desc_ev[slot]));
     CK(cudaStreamWaitEvent(stream, c->desc_done[slot], 0));
-    if (bytes > c->desc_cap[slot]) {
-        if (c->h_desc[slot]) CK(cudaFreeHost(c->h_desc[slot]));
-        if (c->d_desc[slot]) { CK(cudaDeviceSynchronize()); CK(cudaFree(c->d_desc[slot])); }
-        c->h_desc[slot] = nullptr; c->d_desc[slot] = nullptr; c->desc_cap[slot] = 0;
-        const size_t cap = align_up(bytes * 2, 4096);
-        CK(cudaHostAlloc((void**)&c->h_desc[slot], cap, cudaHostAllocDefault));
-        CK(cudaMalloc((void**)&c->d_desc[slot], cap));
-        c->desc_cap[slot] = cap;
-    }
+    { const int st = ensure_pair(&c->h_desc[slot], &c->d_desc[slot], &c->desc_cap[slot], bytes); if (st) return st; }
     *slot_out = slot; *h = c->h_desc[slot]; *d = c->d_desc[slot];
     return SS_OK;
 }

@@ -791,7 +791,7 @@ extern "C" void ss_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 // RIR spectrum bank: one device allocation = [reverberant set | direct set] (P*C*K rows of kSpec float2 each, the layout
 // k_prepare writes into chunk scratch) | cut table (direct set) | descriptor of the blockless source that built it |
-// its norm_part slots (SS_RIR_NORMALIZE).
+// its norm_part slots (SS_RIR_NORMALIZE).  A host bank's block (SS_BANK_HOST) is [spectra | cut table], unpadded.
 struct ss_bank {
     ss_ctx* c = nullptr;                  // the context that made it; sources of other contexts are refused
     char* d_mem = nullptr;
@@ -803,6 +803,10 @@ struct ss_bank {
     // SS_BANK_HOST: spectra and cut table moved into pinned, mapped host memory (spec / cut: their device addresses)
     char* h_mem = nullptr;
     size_t host_bytes = 0;
+    // bytes of one set of spectra, of every set, and of the cut table, which follows the spectra in both layouts
+    size_t set_bytes() const { return (size_t)P * C * K * kSpec * sizeof(float2); }
+    size_t spec_bytes() const { return ((flags & SS_DIRECT_TARGET) ? 2 : 1) * set_bytes(); }
+    size_t cut_bytes() const { return (flags & SS_DIRECT_TARGET) ? sizeof(int) * (size_t)P * C : 0; }
 };
 // Source pool: the candidates' compact entries in one device allocation, and on the host what validation, sizing and the
 // mixture range checks need.
@@ -1335,11 +1339,9 @@ static int bank_args(const ss_ctx* c, const float* rir, int P, int C, int L, int
     if ((int64_t)P * C * ((L + kB - 1) / kB) > (int64_t)1 << 28) return SS_ERR_UNSUPPORTED;    // as validate_item
     return SS_OK;
 }
-static int ensure(char** p, size_t* cap, size_t need);      // (host path, below)
 static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stream) {
     const bool direct = (b->flags & SS_DIRECT_TARGET) != 0, norm = (b->flags & SS_RIR_NORMALIZE) != 0;
-    const size_t spec_b = (direct ? 2 : 1) * (size_t)b->P * b->C * b->K * kSpec * sizeof(float2);
-    const size_t cut_b = direct ? align_up(sizeof(int) * (size_t)b->P * b->C, 256) : 0;
+    const size_t spec_b = b->spec_bytes(), cut_b = align_up(b->cut_bytes(), 256);
     const size_t src_b = align_up(sizeof(Source), 256);
     b->bytes = spec_b + cut_b + src_b + (norm ? 512 : 0);
     CK(cudaMalloc((void**)&b->d_mem, b->bytes));
@@ -1370,8 +1372,7 @@ static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stre
 // SS_BANK_HOST: the built spectra and cut table into pinned, mapped host memory, then the device buffer freed.  Returns
 // when the bank is in host memory.
 static int bank_to_host(ss_bank* b, cudaStream_t stream) {
-    const size_t spec_b = ((b->flags & SS_DIRECT_TARGET) ? 2 : 1) * (size_t)b->P * b->C * b->K * kSpec * sizeof(float2);
-    const size_t cut_b = b->cut ? sizeof(int) * (size_t)b->P * b->C : 0;
+    const size_t spec_b = b->spec_bytes(), cut_b = b->cut_bytes();
     CK(cudaHostAlloc((void**)&b->h_mem, spec_b + cut_b, cudaHostAllocMapped | cudaHostAllocPortable));
     b->host_bytes = spec_b + cut_b;
     CK(cudaMemcpyAsync(b->h_mem, b->spec, spec_b, cudaMemcpyDeviceToHost, stream));
@@ -1500,7 +1501,7 @@ static int pool_host_copies(ss_pool* pl, const ss_source* cand) {
     for (int i = 0; i < n; ++i) {
         xo[i + 1] = xo[i] + align_up(sizeof(float) * (size_t)cand[i].N, 64);
         const ss_bank* b = cand[i].rir_bank;
-        ao[i + 1] = ao[i] + (pl->mode == SS_MOVING_BOUNDS ? (size_t)cand[i].P : 0) + (b->cut ? (size_t)b->P * b->C : 0);
+        ao[i + 1] = ao[i] + (pl->mode == SS_MOVING_BOUNDS ? (size_t)cand[i].P : 0) + b->cut_bytes() / sizeof(int);
     }
     pl->h_x_bytes = xo[n];
     CK(cudaHostAlloc((void**)&pl->h_x, pl->h_x_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
@@ -1512,7 +1513,7 @@ static int pool_host_copies(ss_pool* pl, const ss_source* cand) {
         const ss_bank* b = cand[i].rir_bank;
         int* a = aux.data() + ao[i];
         if (pl->mode == SS_MOVING_BOUNDS) { memcpy(a, cand[i].bounds_host, sizeof(int) * (size_t)cand[i].P); a += cand[i].P; }
-        if (b->cut) memcpy(a, b->h_mem + (size_t)((char*)b->cut - (char*)b->spec), sizeof(int) * (size_t)b->P * b->C);
+        if (b->cut) memcpy(a, b->h_mem + b->spec_bytes(), b->cut_bytes());
         CK(cudaMemcpy(pl->h_x + xo[i], cand[i].x, sizeof(float) * (size_t)cand[i].N, cudaMemcpyDefault));
     }
     pl->aux_bytes = sizeof(int) * std::max(ao[n], (size_t)1);
@@ -1604,14 +1605,7 @@ extern "C" int ss_pool_create(ss_ctx* c, const ss_source* cand, int n, ss_pool**
 static int launch_chunk(ss_ctx* c, const ss_source* items, const Shape* shapes, int first, int last,
                         cudaStream_t stream, int buf) {
     const size_t need = chunk_scratch_bytes(items, shapes, first, last);
-    if (need > c->scratch_cap[buf]) {
-        CK(cudaDeviceSynchronize());
-        if (c->d_scratch[buf]) CK(cudaFree(c->d_scratch[buf]));
-        c->d_scratch[buf] = nullptr; c->scratch_cap[buf] = 0;
-        size_t cap = align_up(need + need / 4, 1 << 20);
-        CK(cudaMalloc(&c->d_scratch[buf], cap));
-        c->scratch_cap[buf] = cap;
-    }
+    { const int st = ensure(&c->d_scratch[buf], &c->scratch_cap[buf], need); if (st) return st; }
     const size_t bytes = chunk_desc_bytes(items, shapes, first, last);
     int slot; char *hblk, *dblk;
     { int st = ring_acquire(c, bytes, stream, &slot, &hblk, &dblk); if (st) return st; }
@@ -1806,8 +1800,7 @@ static StemGroups stem_groups(const ss_pool* pl) {
 // into transient device memory and rendered from there, in batches of at most kLevelStemBytes of copies (or one
 // candidate's, when larger), each behind the previous batch's render on `s`.  `buf` holds `cap` = stem_copy_cap bytes.
 static size_t stem_copy_bytes(const ss_pool* pl, int i) {
-    const ss_bank* b = pl->banks[i];
-    return align_up((size_t)b->P * b->C * b->K * kSpec * sizeof(float2), 256) + align_up(sizeof(float) * (size_t)pl->host[i].N, 256);
+    return align_up(pl->banks[i]->set_bytes(), 256) + align_up(sizeof(float) * (size_t)pl->host[i].N, 256);
 }
 static size_t stem_copy_cap(const ss_pool* pl) {
     size_t cap = 0, total = 0;
@@ -1822,12 +1815,11 @@ static int render_host_stems(ss_pool* pl, ss_source* items, int first, int n, ch
         while (hi < n && (hi == lo || used + stem_copy_bytes(pl, first + hi) <= cap)) {
             const int i = first + hi;
             const ss_bank* b = pl->banks[i];
-            const size_t spec_b = (size_t)b->P * b->C * b->K * kSpec * sizeof(float2);
             ss_bank& sh = shells[hi];
             sh = *b;                                    // the bank's shape and `ready`, spectra from the copy
             sh.h_mem = nullptr; sh.d_mem = nullptr; sh.cut = nullptr; sh.spec = (float2*)(buf + used);
-            CK(cudaMemcpyAsync(sh.spec, b->spec, spec_b, cudaMemcpyDefault, s));
-            float* x = (float*)(buf + used + align_up(spec_b, 256));
+            CK(cudaMemcpyAsync(sh.spec, b->spec, b->set_bytes(), cudaMemcpyDefault, s));   // the reverberant set
+            float* x = (float*)(buf + used + align_up(b->set_bytes(), 256));
             CK(cudaMemcpyAsync(x, pl->host[i].x, sizeof(float) * (size_t)pl->host[i].N, cudaMemcpyDefault, s));
             items[hi].x = x; items[hi].rir_bank = &sh;
             used += stem_copy_bytes(pl, i);
@@ -2677,15 +2669,22 @@ static int check_idx_host(const ss_source& it, const ReadSet& rs) {
     return SS_OK;
 }
 
-static int ensure(char** p, size_t* cap, size_t need) {
-    if (need <= *cap) return SS_OK;
-    CK(cudaDeviceSynchronize());
-    if (*p) CK(cudaFree(*p));
-    *p = nullptr; *cap = 0;
-    size_t c2 = align_up(need + need / 8, 1 << 20);
-    CK(cudaMalloc((void**)p, c2));
-    *cap = c2;
-    return SS_OK;
+// Where one source's arrays go in its chunk's slot: its inputs (x, rir, bounds or idx, w) in d_in and its outputs
+// (out, out_direct, loudness scratch and result) in d_out, each at a 256-byte boundary after the chunk's earlier
+// arrays, which end at *in / *out.  An array the source does not stage has 0 bytes.
+struct Span { size_t at, bytes; };
+struct Staged { Span x, rir, tab, w, out, direct, scratch, res; };
+static Staged stage_source(const ss_source& it, const ReadSet& rs, const ss_post_lufs* q, size_t* in, size_t* out) {
+    auto take = [](size_t* end, size_t bytes) { const Span s = {*end, bytes}; *end += align_up(bytes, 256); return s; };
+    Staged s = {};
+    s.x = take(in, sizeof(float) * (size_t)(rs.xb - rs.xa));
+    if (!it.rir_bank) s.rir = take(in, sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L);
+    if (it.mode == SS_MOVING_BOUNDS) s.tab = take(in, sizeof(int32_t) * (size_t)it.P);
+    if (it.mode == SS_MOVING_INDEXED) { s.tab = take(in, 4 * (size_t)(rs.ib - rs.ia)); s.w = take(in, s.tab.bytes); }
+    s.out = take(out, sizeof(float) * (size_t)it.C * rs.wl);
+    if (it.flags & SS_DIRECT_TARGET) s.direct = take(out, s.out.bytes);
+    if (q) { s.scratch = take(out, loud_scratch_bytes(*q, it.C)); s.res = take(out, 2 * sizeof(double)); }
+    return s;
 }
 
 // Host path: H2D -> k_spectra -> k_render [-> loudness measure + in-place gain] -> D2H, pipelined
@@ -2719,6 +2718,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     std::vector<int> cuts;
     make_chunks(items, shapes.data(), n_items, c->chunk_bytes_host, cuts);
     std::vector<ss_source> dev(n_items);
+    std::vector<Staged> staged(n_items);
     std::vector<ss_loud_item> loud;
     std::vector<ScaleItem> direct_gain;                  // direct-path stems scaled by their reverberant stem's gain
     std::vector<double*> res_dev(n_items, nullptr);
@@ -2733,16 +2733,7 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
     if (post) {
         tabs = gating_tables(post, n_items);
         const size_t tab_bytes = tabs.bytes.size();
-        if (tab_bytes + res_bytes > c->h_post_cap) {
-            CK(cudaDeviceSynchronize());
-            if (c->h_post) CK(cudaFreeHost(c->h_post));
-            if (c->d_post) CK(cudaFree(c->d_post));
-            c->h_post = nullptr; c->d_post = nullptr; c->h_post_cap = 0;
-            const size_t cap = align_up((tab_bytes + res_bytes) * 2, 4096);
-            CK(cudaHostAlloc((void**)&c->h_post, cap, cudaHostAllocDefault));
-            CK(cudaMalloc((void**)&c->d_post, cap));
-            c->h_post_cap = cap;
-        }
+        { const int st = ensure_pair(&c->h_post, &c->d_post, &c->h_post_cap, tab_bytes + res_bytes); if (st) return st; }
         char* const h_tab = c->h_post + res_bytes;
         if (tab_bytes) {
             memcpy(h_tab, tabs.bytes.data(), tab_bytes);
@@ -2759,50 +2750,42 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         const int first = cuts[k], last = cuts[k + 1];
         ss_ctx::Slot& sl = c->slot[k % ss_ctx::kSlots];
         size_t in_b = 0, out_b = 0;
-        for (int i = first; i < last; ++i) {
-            const ss_source& it = items[i];
-            const ReadSet& rs = rset[i];
-            in_b += align_up(sizeof(float) * (size_t)(rs.xb - rs.xa), 256);
-            if (!it.rir_bank) in_b += align_up(sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L, 256);
-            if (it.mode == SS_MOVING_BOUNDS) in_b += align_up(sizeof(int32_t) * (size_t)it.P, 256);
-            if (it.mode == SS_MOVING_INDEXED) in_b += 2 * align_up(4 * (size_t)(rs.ib - rs.ia), 256);
-            out_b += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256) * direct_sets(it);
-            if (post && post[i].brk) out_b += loud_scratch_bytes(post[i], it.C) + 256;
-        }
+        for (int i = first; i < last; ++i)
+            staged[i] = stage_source(items[i], rset[i], post && post[i].brk ? &post[i] : nullptr, &in_b, &out_b);
         if (k >= (size_t)ss_ctx::kSlots) CK(cudaEventSynchronize(sl.ev_free));      // slot's previous chunk fully drained
         if ((rc = ensure(&sl.d_in, &sl.in_cap, in_b)) != SS_OK) break;
         if ((rc = ensure(&sl.d_out, &sl.out_cap, out_b)) != SS_OK) break;
-        char* pi = sl.d_in; char* po = sl.d_out;
+        char* const pi = sl.d_in; char* const po = sl.d_out;
         loud.clear();
         direct_gain.clear();
         for (int i = first; i < last; ++i) {
             const ss_source& it = items[i];
             const ReadSet& rs = rset[i];
+            const Staged& s = staged[i];
             ss_source d = it;
-            size_t nb;
             // only the read set is copied; the device pointers are offset so that the kernels index the full arrays
-            nb = sizeof(float) * (size_t)(rs.xb - rs.xa);
-            CK(cudaMemcpyAsync(pi, it.x + rs.xa, nb, cudaMemcpyHostToDevice, c->s_in)); d.x = (const float*)pi - rs.xa; pi += align_up(nb, 256);
+            CK(cudaMemcpyAsync(pi + s.x.at, it.x + rs.xa, s.x.bytes, cudaMemcpyHostToDevice, c->s_in));
+            d.x = (const float*)(pi + s.x.at) - rs.xa;
             if (!it.rir_bank) {                              // a banked source's spectra are on the device already
                 const size_t pos0 = (size_t)rs.pa * it.C * it.L;
-                nb = sizeof(float) * (size_t)(rs.pb - rs.pa + 1) * it.C * it.L;
-                CK(cudaMemcpyAsync(pi, it.rir + pos0, nb, cudaMemcpyHostToDevice, c->s_in)); d.rir = (const float*)pi - pos0; pi += align_up(nb, 256);
+                CK(cudaMemcpyAsync(pi + s.rir.at, it.rir + pos0, s.rir.bytes, cudaMemcpyHostToDevice, c->s_in));
+                d.rir = (const float*)(pi + s.rir.at) - pos0;
             }
             if (it.mode == SS_MOVING_BOUNDS) {
-                nb = sizeof(int32_t) * (size_t)it.P;
-                CK(cudaMemcpyAsync(pi, it.bounds, nb, cudaMemcpyHostToDevice, c->s_in)); d.bounds = (const int32_t*)pi; pi += align_up(nb, 256);
+                CK(cudaMemcpyAsync(pi + s.tab.at, it.bounds, s.tab.bytes, cudaMemcpyHostToDevice, c->s_in));
+                d.bounds = (const int32_t*)(pi + s.tab.at);
                 d.bounds_host = it.bounds;
             } else if (it.mode == SS_MOVING_INDEXED) {
-                nb = 4 * (size_t)(rs.ib - rs.ia);
-                CK(cudaMemcpyAsync(pi, it.idx + rs.ia, nb, cudaMemcpyHostToDevice, c->s_in)); d.idx = (const int32_t*)pi - rs.ia; pi += align_up(nb, 256);
-                CK(cudaMemcpyAsync(pi, it.w + rs.ia, nb, cudaMemcpyHostToDevice, c->s_in)); d.w = (const float*)pi - rs.ia; pi += align_up(nb, 256);
+                CK(cudaMemcpyAsync(pi + s.tab.at, it.idx + rs.ia, s.tab.bytes, cudaMemcpyHostToDevice, c->s_in));
+                CK(cudaMemcpyAsync(pi + s.w.at, it.w + rs.ia, s.w.bytes, cudaMemcpyHostToDevice, c->s_in));
+                d.idx = (const int32_t*)(pi + s.tab.at) - rs.ia; d.w = (const float*)(pi + s.w.at) - rs.ia;
             }
-            d.out = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256);
-            if (it.flags & SS_DIRECT_TARGET) { d.out_direct = (float*)po; po += align_up(sizeof(float) * (size_t)it.C * rs.wl, 256); }
+            d.out = (float*)(po + s.out.at);
+            if (it.flags & SS_DIRECT_TARGET) d.out_direct = (float*)(po + s.direct.at);
             dev[i] = d;
             if (post && post[i].brk) {
-                double* scratch = (double*)po; po += loud_scratch_bytes(post[i], it.C);
-                res_dev[i] = (double*)po; po += 256;
+                double* const scratch = (double*)(po + s.scratch.at);
+                res_dev[i] = (double*)(po + s.res.at);
                 loud.push_back(loud_item(post[i], d_tab + tabs.at[i], d.out, d.out, it.N, it.C, scratch, res_dev[i]));
                 if (it.flags & SS_DIRECT_TARGET) direct_gain.push_back(ScaleItem{d.out_direct, res_dev[i], it.N, it.C});
             }
@@ -2825,12 +2808,12 @@ extern "C" int ss_render_host_ex(ss_ctx* c, const ss_source* items, int n_items,
         }
         CK(cudaStreamWaitEvent(c->s_out, sl.ev_done, 0));
         for (int i = first; i < last; ++i) {
-            const size_t ob = sizeof(float) * (size_t)items[i].C * rset[i].wl;
-            CK(cudaMemcpyAsync(items[i].out, dev[i].out, ob, cudaMemcpyDeviceToHost, c->s_out));
+            const Staged& s = staged[i];
+            CK(cudaMemcpyAsync(items[i].out, dev[i].out, s.out.bytes, cudaMemcpyDeviceToHost, c->s_out));
             if (items[i].flags & SS_DIRECT_TARGET)
-                CK(cudaMemcpyAsync(items[i].out_direct, dev[i].out_direct, ob, cudaMemcpyDeviceToHost, c->s_out));
+                CK(cudaMemcpyAsync(items[i].out_direct, dev[i].out_direct, s.direct.bytes, cudaMemcpyDeviceToHost, c->s_out));
             if (res_dev[i])
-                CK(cudaMemcpyAsync(h_res + 2 * i, res_dev[i], 2 * sizeof(double), cudaMemcpyDeviceToHost, c->s_out));
+                CK(cudaMemcpyAsync(h_res + 2 * i, res_dev[i], s.res.bytes, cudaMemcpyDeviceToHost, c->s_out));
         }
         CK(cudaEventRecord(sl.ev_free, c->s_out));
         // the next chunk's H2D into the *other* slot may start now; it must not overtake the

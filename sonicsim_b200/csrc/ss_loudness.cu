@@ -365,44 +365,27 @@ extern "C" int ss_lufs_norm_host(ss_ctx* c, const float* data, float* out, int32
     if (!c || !data || !brk || N <= 0 || C <= 0 || check_post_lufs(&q, 1)) return SS_ERR_INVALID;
     if (!dense_layout(N, C, stride_n, stride_c)) return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
+    // one block in the first input slot: the stem, its gating tables, the loudness scratch and the two result doubles
+    const GatingTables tabs = gating_tables(&q, 1);
     const size_t nel = (size_t)N * C;
-    const size_t o_data = 0;
-    const size_t o_brk = align_up(nel * 4, 256);
-    const size_t o_lo = o_brk + align_up(4 * (size_t)(n_e + 1), 256);
-    const size_t o_hi = o_lo + align_up(4 * (size_t)(n_blocks + 1), 256);
-    const size_t o_E = o_hi + align_up(4 * (size_t)(n_blocks + 1), 256);
-    const size_t o_res = o_E + align_up(8 * (size_t)kLoudScratch * C * n_e, 256);
-    const size_t total = o_res + 256;
+    const size_t o_tab = align_up(nel * 4, 256), o_scr = o_tab + tabs.bytes.size();
+    const size_t o_res = o_scr + loud_scratch_bytes(q, C), total = o_res + 256;
     ss_ctx::Slot& sl = c->slot[0];
     CK(cudaStreamSynchronize(c->s_cmp));
-    if (total > sl.in_cap) {
-        CK(cudaDeviceSynchronize());
-        if (sl.d_in) CK(cudaFree(sl.d_in));
-        sl.d_in = nullptr; sl.in_cap = 0;
-        CK(cudaMalloc((void**)&sl.d_in, align_up(total, 1 << 20)));
-        sl.in_cap = align_up(total, 1 << 20);
-    }
+    { const int rc = ensure(&sl.d_in, &sl.in_cap, total); if (rc) return rc; }
     char* base = sl.d_in;
     cudaStream_t st = c->s_cmp;
-    CK(cudaMemcpyAsync(base + o_data, data, nel * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(base + o_brk, brk, 4 * (size_t)(n_e + 1), cudaMemcpyHostToDevice, st));
-    if (n_blocks > 0) {
-        CK(cudaMemcpyAsync(base + o_lo, blk_lo, 4 * (size_t)n_blocks, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(base + o_hi, blk_hi, 4 * (size_t)n_blocks, cudaMemcpyHostToDevice, st));
-    }
-    ss_loud_item it;
-    memset(&it, 0, sizeof(it));
-    it.data = (const float*)(base + o_data);
-    it.out = out ? (float*)(base + o_data) : nullptr;       // scaled in place on the device
-    it.brk = (const int32_t*)(base + o_brk); it.blk_lo = (const int32_t*)(base + o_lo); it.blk_hi = (const int32_t*)(base + o_hi);
-    it.scratch = (double*)(base + o_E); it.result = (double*)(base + o_res);
-    it.stride_n = stride_n; it.stride_c = stride_c; it.N = N; it.C = C; it.n_e = n_e; it.n_blocks = n_blocks;
-    it.rate = rate; it.block_size = block_size; it.target_lufs = target_lufs;
+    CK(cudaMemcpyAsync(base, data, nel * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(base + o_tab, tabs.bytes.data(), tabs.bytes.size(), cudaMemcpyHostToDevice, st));
+    // scaled in place on the device; the copy keeps the caller's (dense) layout
+    ss_loud_item it = loud_item(q, base + o_tab, (const float*)base, out ? (float*)base : nullptr, N, C,
+                                (double*)(base + o_scr), (double*)(base + o_res));
+    it.stride_n = stride_n; it.stride_c = stride_c;
     int rc = ss_loudness_dev(c, &it, 1, (void*)st);
     if (rc) return rc;
     double res[2];
     CK(cudaMemcpyAsync(res, base + o_res, sizeof(res), cudaMemcpyDeviceToHost, st));
-    if (out) CK(cudaMemcpyAsync(out, base + o_data, nel * 4, cudaMemcpyDeviceToHost, st));
+    if (out) CK(cudaMemcpyAsync(out, base, nel * 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (loudness) *loudness = res[0];
     if (gain) *gain = res[1];

@@ -357,13 +357,7 @@ extern "C" int ss_mix_host_ex(ss_ctx* c, const float* speakers, const float* noi
     ss_ctx::Slot& sl = c->slot[0];
     cudaStream_t st = c->s_cmp;
     CK(cudaStreamSynchronize(st));
-    if (total > sl.in_cap) {
-        CK(cudaDeviceSynchronize());
-        if (sl.d_in) CK(cudaFree(sl.d_in));
-        sl.d_in = nullptr; sl.in_cap = 0;
-        CK(cudaMalloc((void**)&sl.d_in, align_up(total, 1 << 20)));
-        sl.in_cap = align_up(total, 1 << 20);
-    }
+    { const int rc = ensure(&sl.d_in, &sl.in_cap, total); if (rc) return rc; }
     char* b = sl.d_in;
     CK(cudaMemcpyAsync(b + o_spk, speakers, 4 * (size_t)S * E, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(b + o_noise, noises, 4 * (size_t)M * E, cudaMemcpyHostToDevice, st));
@@ -423,13 +417,7 @@ extern "C" int ss_overlap_host(ss_ctx* c, const float* x, float* y, int32_t rows
     ss_ctx::Slot& sl = c->slot[0];
     cudaStream_t st = c->s_cmp;
     CK(cudaStreamSynchronize(st));
-    if (total > sl.in_cap) {
-        CK(cudaDeviceSynchronize());
-        if (sl.d_in) CK(cudaFree(sl.d_in));
-        sl.d_in = nullptr; sl.in_cap = 0;
-        CK(cudaMalloc((void**)&sl.d_in, align_up(total, 1 << 20)));
-        sl.in_cap = align_up(total, 1 << 20);
-    }
+    { const int rc = ensure(&sl.d_in, &sl.in_cap, total); if (rc) return rc; }
     char* b = sl.d_in;
     CK(cudaMemcpyAsync(b, x, bytes, cudaMemcpyHostToDevice, st));
     int rc = ss_overlap_dev(c, (const float*)b, (float*)(b + o_y), rows, T, delay, (void*)st);
