@@ -1,0 +1,828 @@
+"""Host pools (SS_BANK_HOST) at training scale against float64.  A slot of a host pool renders from what k_stage copied
+into its staging area at that run (stage_set's dry samples and RIR rows, StageView), so a staging overrun, a wrong row
+origin (h_row0) or a view given to the wrong slot gives plausible audio.  Every output here is checked (i) bit for bit
+against the same plan over device pools of the same candidates, and (ii) sample by sample against float64
+(render_reference.check_render; a pool with loudness gains scales the reference by its float32 gain; direct stems
+against direct_path_rirs).  Outputs lie in NaN-filled buffers with sentinels on both sides (test_gpu_plan_scale.Out).
+  A. staged crops on both blockings: grid, aligned (direct targets), mixed-K and static host pools with N % 4 in
+     {1, 2, 3}, pure-delay RIRs and graded dry signals; starts 0 and N - len, the maximisers of stage_cap, both clamps of
+     the read set and starts with ws % 4 in {1, 2, 3}, for windows of 64 000, 3 * 4096 + 5 and 3001 samples and fixed
+     starts; the slots whose read sets fill the staging area run side by side;
+  B. training scale: configs[1] speakers with direct targets (default budget and one chunk), P = 60 speakers with random
+     cuts over 32 shared RIR sets with loudness gains, and K = 1..4 speakers in 48 slots; mixtures against
+     mix_reference, draws against draw_reference on the pool's own tables;
+  C. a plan that interleaves host-pool, device-pool, dry-picked and unpooled slots and a static source over every kernel
+     variant (launches: the device-pool plan's plus one; one graph; a side stream), and a plan of 1056 host-pool slots;
+  D. host-pool builds whose copy batches split stem groups (48 P = 60 speakers) and a candidate whose copy alone exceeds
+     256 MiB: LUFS, gains and tables against the device-pool twin, render_host, the float64 BS.1770 oracle and the
+     long-double prefix; a training plan with draws over the speaker pool.
+No test holds more than 2 GB of pinned host memory in banks and pools (as counted by their host_nbytes)."""
+import numpy as np
+import pytest
+import torch
+
+import draw_reference as dr
+from chunk_budget import DEFAULT_CHUNK_BYTES, chunk_budget  # noqa: F401  (fixture)
+from direct_path import direct_path_rirs
+from oracle import sonicsim_oracle as so
+from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, delay_rirs, graded_dry, render_check_inputs
+from test_gpu_plan_draw import NEAR_DB, TABLE_TOL, gappy_dry
+from test_gpu_plan_pool import _choice
+from test_gpu_plan_scale import Out, check_mixture, fold
+from test_gpu_pool_builds import STEM_BYTES, align_up, stem_groups, table_error
+from test_host_pool import stage_set_np
+
+pytestmark = pytest.mark.gpu
+
+RATE = 16000
+B = 4096
+TAPS = 40
+TRIES = 101
+ONE_CHUNK = 1 << 30
+PINNED_MAX = 2 << 30
+STATS = {}                       # section / variant -> [worst local ratio, worst global relative RMS]
+QUIET = {}                       # section / variant -> labels of crops whose global error is taken against the scale
+
+
+def _R():
+    from sonicsim_b200 import render
+    return render, render.default_renderer()
+
+
+def to(a):
+    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+
+def _report(title):
+    print("\n%s:" % title)
+    for k in sorted(STATS):
+        if k.startswith(title.split(":")[0]):
+            print("  %-40s worst per-sample ratio %.3g, worst global relative RMS %.3g; %d quiet crops%s" % (
+                k, *STATS[k], len(QUIET.get(k, [])), (" (first: %s)" % QUIET[k][0]) if k in QUIET else ""))
+
+
+def _rms(v):
+    return float(np.sqrt(np.mean(np.square(v, dtype=np.float64))))
+
+
+def _note(key, worst, g):
+    s = STATS.setdefault(key, [0.0, 0.0])
+    s[0], s[1] = max(s[0], worst), max(s[1], g)
+
+
+class Cand:
+    """One candidate: dry x (N,), RIRs h (P, C, L) (P = 1: static), bounds (P,) or None, K partitions."""
+
+    def __init__(self, x, h, b):
+        self.x, self.h, self.b = np.ascontiguousarray(x, np.float32), np.ascontiguousarray(h, np.float32), b
+        self.N, (self.P, self.C, self.L) = len(x), h.shape
+        self.K = (self.L + B - 1) // B
+        self.mode = 0 if b is None else 1
+
+    def check(self, y, a, wl, direct=False, gain=1.0, key="", label=""):
+        """Sample by sample against float64 at window start a (times the float32 gain of the pool), and as a whole for
+        crops of at least one block: relative RMS against the crop's RMS, or, for a quiet crop (RMS under 2^-6 of its
+        rounding scale's: quiet graded blocks next to loud ones), against the scale's RMS.  Such a crop carries the
+        rounding of its loud neighbours' transforms, which its own RMS does not measure - e.g. the direct stem of the
+        aligned pool's candidate 0 at 42001 + 12293 samples: RMS 6.8e-4 of its scale's, error 1.3e-4 of its RMS and
+        8.6e-8 of the scale's."""
+        h = direct_path_rirs(self.h, TAPS) if direct else self.h
+        y64, scale = render_check_inputs(self.x, h if self.P > 1 else h[0], self.mode, bounds=self.b, window=(a, wl))
+        g = float(np.float32(gain))
+        y64, scale = y64 * g, scale * g
+        key = key + (" direct" if direct else "")
+        quiet = wl >= B and _rms(y64) < _rms(scale) / 64
+        worst, gl = check_render(y, y64, scale, TAU_LOCAL, TAU_GLOBAL if wl >= B and not quiet else np.inf, n0=a,
+                                 label=label)
+        if quiet:
+            gl = _rms(np.asarray(y, np.float64) - y64) / _rms(scale)
+            assert gl <= TAU_GLOBAL, "%s: quiet crop, global RMS %.3g of the scale's > %.3g" % (label, gl, TAU_GLOBAL)
+            QUIET.setdefault(key, []).append(label)
+        _note(key, worst, gl if wl >= B else 0.0)
+
+
+def pool_variant(cands):
+    """The render kernel every slot of a pool of these candidates runs: static pools k_render_fast, pools of K > 1
+    k_render<1,0>, moving pools whose every candidate picks aligned blocking on its own k_render_fast, and every other
+    moving pool (mixed blocking renders on the grid) k_render<0,0>."""
+    if cands[0].P == 1:
+        return "k_render_fast static"
+    if max(c.K for c in cands) > 1:
+        return "k_render<1,0>"
+    return "k_render_fast" if all(_choice(c.b, c.N, c.P, c.L) for c in cands) else "k_render<0,0>"
+
+
+class Pools:
+    """One set of candidates as a device pool and as a host pool (banks shared between candidates when `share` names
+    the RIR set of each), with direct sets of TAPS taps when `taps`, level tables and loudness targets.  Counts the
+    pinned bytes it holds."""
+
+    def __init__(self, cands, taps=False, levels=None, lufs=None, share=None, host_only=False):
+        render, R = _R()
+        self.cands, self.taps = cands, taps
+        self.pools, self.banks = {}, []
+        sets = share if share is not None else list(range(len(cands)))
+        for host in ((True,) if host_only else (False, True)):
+            banks = {}
+            for c, r in zip(cands, sets):
+                if r not in banks:
+                    banks[r] = R.rir_bank(c.h if c.P > 1 else c.h[0], direct_taps=TAPS if taps else 0, host=host)
+            self.banks += list(banks.values())
+            srcs = []
+            for c, r in zip(cands, sets):
+                if c.P == 1:
+                    srcs.append(render.StaticSource(c.x if host else to(c.x), banks[r]))
+                elif host:
+                    srcs.append(render.MovingSource(c.x, banks[r], c.b))
+                else:
+                    srcs.append(render.MovingSource(to(c.x), banks[r], to(c.b), bounds_host=c.b))
+            self.pools[host] = R.source_pool(srcs, levels=levels, lufs_targets=lufs, sr=RATE)
+        self.variant = pool_variant(cands)
+        pinned = sum(k.host_nbytes for k in self.banks) + self.pools[True].host_nbytes
+        self.pinned = pinned
+        self.gains = self.pools[True].loudness[:, 1]
+
+    def gain(self, i):
+        g = self.gains[i]
+        return 1.0 if np.isnan(g) else float(g)
+
+    def close(self):
+        for p in self.pools.values():
+            p.close()
+        for k in self.banks:
+            k.close()
+
+
+def _hold(*pools):
+    """The pinned host bytes the test's banks and pools hold, as the library counts them (host_nbytes; the renderer's own
+    host staging buffers not included), printed and kept under 2 GB."""
+    total = sum(p.pinned for p in pools)
+    print("\npinned host memory of the banks and pools held (host_nbytes): %.1f MB" % (total / 1e6))
+    assert total <= PINNED_MAX, total
+    return total
+
+
+def _bounds_of(idx, P):
+    return np.concatenate([[0], np.cumsum(np.bincount(idx, minlength=P - 1))]).astype(np.int32)
+
+
+# ----------------------------------------------------------------------------------------- A. staged crops
+A_LENS = [64000, 3 * B + 5, 3001]
+
+
+def a_grid(rng):
+    """Moving candidates with 59 segments of 0.3 to 3.8 k samples (grid blocking), pure-delay RIRs, graded dry
+    signals."""
+    out = []
+    for j, N in enumerate((70001, 83002)):
+        P = 60
+        np.random.seed(500 + j)
+        b = _bounds_of(so.setup_dynamic_interp(so.synth_path(rng, P), N)[0], P)
+        assert _choice(b, N, P, 4096) == 0
+        out.append(Cand(graded_dry(rng, N), delay_rirs(rng, P, 3, 4096)[0], b))
+    return out
+
+
+def a_aligned(rng):
+    out = []
+    for j, N in enumerate((65001, 90002, 130003)):
+        P = 4 + j
+        b = np.round(np.linspace(0, N, P)).astype(np.int32)
+        assert _choice(b, N, P, 4096) == 1
+        out.append(Cand(graded_dry(rng, N), so.synth_rirs(rng, P, 2, 4096), b))
+    return out
+
+
+def a_mixed_k(rng):
+    out = []
+    for j, (N, L) in enumerate(((70001, 3000), (81002, 4097), (66003, 9000), (90000, 16384))):
+        P = 3 + j % 3
+        b = np.round(np.linspace(0, N, P)).astype(np.int32)
+        out.append(Cand(graded_dry(rng, N), delay_rirs(rng, P, 1, L)[0], b))
+    return out
+
+
+def a_static(rng):
+    return [Cand(graded_dry(rng, N), so.synth_rirs(rng, 1, 5, L), None)
+            for N, L in ((66001, 2048), (70002, 4096), (80003, 3000))]
+
+
+A_POOLS = {"grid": (a_grid, False, "k_render<0,0>"), "aligned": (a_aligned, True, "k_render_fast"),
+           "mixed-K": (a_mixed_k, False, "k_render<1,0>"), "static": (a_static, False, "k_render_fast static")}
+
+
+def probe_starts(c, wl, rng):
+    """0 and N - len; the maximisers of stage_cap, (K + 2) 4096 and b[s + 1] - 1 + (K + 2) 4096; starts where xa clamps
+    to 0 and where xb clamps to N; starts with ws % 4 in {1, 2, 3}; all inside [0, N - len]."""
+    last = c.N - wl
+    d0 = (c.K + 2) * B
+    s = {0, last, d0, d0 - 1, 1, last - 1, max(0, c.N - wl - 2 * B + 1)}
+    for q in ([] if c.b is None else c.b[1:-1]):
+        s.add(int(q) - 1 + d0)
+    for m in (1, 2, 3):
+        v = int(rng.integers(0, last + 1))
+        s.add(v - v % 4 + m)
+    return sorted(v for v in s if 0 <= v <= last)
+
+
+def read_set(c, ws, wl, sets):
+    """(bytes k_stage copies - whole float4s of dry samples and the rows of every set -, rows, dry samples)."""
+    xa, xb, _, rows = (int(v[0]) for v in stage_set_np(c.N, c.P, c.C, c.K, c.b, [ws], wl))
+    return 4 * (((xb + 3) & ~3) - (xa & ~3)) + sets * rows * B * 8, rows, xb - xa
+
+
+class Probes:
+    """A plan over both pools of `pl`: for every window length, `k` slots with device starts and one with a fixed
+    start, all over the same pick and start tensors, NaN-filled guarded outputs."""
+
+    def __init__(self, pl, lens, k, fixed):
+        render, R = _R()
+        self.pl, self.lens, self.k = pl, lens, k
+        n = len(lens) * (k + 1)
+        self.picks = torch.zeros(n, dtype=torch.int32, device="cuda")
+        self.starts = torch.zeros(n, dtype=torch.int32, device="cuda")
+        self.slots = []                               # (wl, fixed start or None)
+        for wl, f in zip(lens, fixed):
+            self.slots += [(wl, None)] * k + [(wl, f)]
+        C = pl.cands[0].C
+        self.plans, self.outs, self.douts = {}, {}, {}
+        for host, pool in pl.pools.items():
+            srcs = [render.Pooled(pool, self.picks[j], (self.starts[j] if f is None else f, wl), TAPS if pl.taps else 0)
+                    for j, (wl, f) in enumerate(self.slots)]
+            self.outs[host] = [Out(C, wl) for wl, _ in self.slots]
+            self.douts[host] = [Out(C, wl) for wl, _ in self.slots] if pl.taps else []
+            self.plans[host] = R.plan_device(srcs, [o.view() for o in self.outs[host]],
+                                             direct_outs=[o.view() for o in self.douts[host]] if pl.taps else None)
+
+    def run(self, pk, st):
+        self.pk, self.st = list(pk), [s if f is None else f for s, (_, f) in zip(st, self.slots)]
+        self.picks.copy_(torch.tensor(self.pk, dtype=torch.int32))
+        self.starts.copy_(torch.tensor(st, dtype=torch.int32))
+        R = _R()[1]
+        self.launches = {}
+        for host in self.plans:
+            for o in self.outs[host] + self.douts[host]:
+                o.reset()
+            R.reset_stats()
+            self.plans[host].run()
+            self.launches[host] = R.launch_count()
+        torch.cuda.synchronize()
+        for j in range(len(self.slots)):                  # (i) bit for bit the device-pool plan
+            a, b = self.outs[False][j].get(), self.outs[True][j].get()
+            assert np.array_equal(a, b), ("device twin", j, self.pk[j], self.st[j])
+            if self.pl.taps:
+                assert np.array_equal(self.douts[False][j].get(), self.douts[True][j].get()), ("direct twin", j)
+
+    def check(self, key, label):
+        for j, (wl, _) in enumerate(self.slots):          # (ii) float64
+            c = self.pl.cands[self.pk[j]]
+            g = self.pl.gain(self.pk[j])
+            what = "%s slot %d cand %d start %d len %d" % (label, j, self.pk[j], self.st[j], wl)
+            c.check(self.outs[True][j].get(), self.st[j], wl, gain=g, key=key, label=what)
+            if self.pl.taps:
+                c.check(self.douts[True][j].get(), self.st[j], wl, direct=True, gain=g, key=key, label=what + " direct")
+
+    def close(self):
+        for p in self.plans.values():
+            p.close()
+
+
+@pytest.mark.parametrize("kind", list(A_POOLS))
+def test_staged_crops_at_every_read_set_edge(kind):
+    make, taps, variant = A_POOLS[kind]
+    render, R = _R()
+    rng = np.random.default_rng(600 + len(kind))
+    cands = make(rng)
+    assert {c.N % 4 for c in cands} >= ({1, 2, 3} if len(cands) >= 3 else {1, 2})
+    pl = Pools(cands, taps=taps)
+    assert pl.variant == variant, (kind, pl.variant)
+    _hold(pl)
+    k = 8
+    n_min = min(c.N for c in cands)
+    fixed = [n_min - wl for wl in A_LENS]
+    pr = Probes(pl, A_LENS, k, fixed)
+    sets = 2 if taps else 1
+    try:
+        R.check_device_errors()
+        queues = []
+        for wl in A_LENS:                      # the largest read sets first, so that the full areas run side by side
+            q = [read_set(c, s, wl, sets) + (i, s) for i, c in enumerate(cands) for s in probe_starts(c, wl, rng)]
+            q.sort(key=lambda t: -t[0])
+            queues.append(q)
+        # the staging area: the most rows and dry samples of any read set (the probes hold stage_cap's maximisers)
+        cap = {wl: (max(t[1] for t in q), max(t[2] for t in q)) for wl, q in zip(A_LENS, queues)}
+        runs = max(-(-len(q) // k) for q in queues)
+        full_together = 0
+        for r in range(runs):
+            pk, st = [], []
+            for wl, q in zip(A_LENS, queues):
+                take = q[r * k:(r + 1) * k]
+                while len(take) < k:                   # the rest: random picks and starts
+                    i = int(rng.integers(0, len(cands)))
+                    take.append((0, -1, -1, i, int(rng.integers(0, cands[i].N - wl + 1))))
+                full_together = max(full_together, sum(t[1] == cap[wl][0] or t[2] == cap[wl][1] for t in take))
+                pk += [t[3] for t in take] + [int(rng.integers(0, len(cands)))]
+                st += [t[4] for t in take] + [0]
+            pr.run(pk, st)
+            pr.check("A %s" % variant, "%s run %d" % (kind, r))
+        assert full_together >= 2, full_together                        # full staging areas side by side
+        R.check_device_errors()
+        print("\n%s: %d runs of %d slots; staging capacity reached by %d adjacent slots" %
+              (kind, runs, len(pr.slots), full_together))
+        _report("A")
+    finally:
+        pr.close()
+        pl.close()
+
+
+# ----------------------------------------------------------------------------------------- B. training scale
+def b_configs1(rng):
+    """bench.make_inputs(16, 0): 32 configs[1] speakers (P = 40, C = 6, 30 s; every other dry signal gappy) and 16
+    static 6-channel noises."""
+    import bench
+    items = bench.make_inputs(16, 0)
+    spk = [Cand(gappy_dry(rng, len(x)) if j % 2 else x, h, b) for j, (x, h, b) in enumerate(items)]
+    N, C = bench.CFG["N"], bench.CFG["C"]
+    noi = [Cand((rng.standard_normal(N) * 0.05).astype(np.float32),
+                (rng.standard_normal((1, C, 4096)) * np.exp(-np.arange(4096) / 800.0)).astype(np.float32), None)
+           for _ in range(16)]
+    return spk, noi
+
+
+def _random_cuts(rng, P, N, span=None):
+    """Random cuts over [0, N], or over a random stretch of `span` samples (short segments: grid blocking)."""
+    at = 0 if span is None else int(rng.integers(0, N - span))
+    cuts = at + np.sort(rng.integers(0, (N if span is None else span) + 1, P - 2))
+    return np.concatenate([[0], cuts, [N]]).astype(np.int32)
+
+
+class Training:
+    """16 scenes: `layout` a list of (pools key, taps) per scene, the first two the mixture's speakers and the draw's,
+    the rest its noises; one start per scene drawn by a 101-try CropDraw over mono level tables; one mono Mixture."""
+
+    def __init__(self, pools, layout, U=16):
+        render, R = _R()
+        self.pools, self.layout, self.U = pools, layout, U
+        S = len(layout)
+        self.picks = torch.zeros((U, S), dtype=torch.int32, device="cuda")
+        self.starts = torch.zeros(U, dtype=torch.int32, device="cuda")
+        self.u = torch.zeros((U, TRIES), dtype=torch.float64, device="cuda")
+        self.used = torch.zeros(U, dtype=torch.int32, device="cuda")
+        self.sirs = torch.zeros((U, 1), device="cuda")
+        self.snr = torch.zeros(U, device="cuda")
+        self.T = 4 * RATE
+        self.plans, self.o = {}, {}
+        for host in (False, True):
+            srcs, outs, douts, mixes, draws = [], [], [], [], []
+            o = dict(outs=[], douts=[], mix=[], spk=[], rms=[])
+            for u in range(U):
+                base = len(srcs)
+                for k, (key, taps) in enumerate(layout):
+                    pl = pools[key]
+                    srcs.append(render.Pooled(pl.pools[host], self.picks[u, k], (self.starts[u], self.T),
+                                              TAPS if taps else 0))
+                    o["outs"].append(Out(pl.cands[0].C, self.T))
+                    o["douts"].append(Out(pl.cands[0].C, self.T) if taps else None)
+                o["mix"].append(Out(1, self.T))
+                o["spk"].append(Out(2, self.T))
+                o["rms"].append(Out(1, 2))
+                mixes.append(render.Mixture([base, base + 1], list(range(base + 2, base + S)), self.sirs[u],
+                                            self.snr[u], o["mix"][-1].view(self.T), o["spk"][-1].view(2, self.T),
+                                            o["rms"][-1].view(2), mono=True))
+                draws.append(render.CropDraw(self.starts[u], [base, base + 1], self.u[u], self.used[u]))
+            self.o[host] = o
+            self.plans[host] = R.plan_device(srcs, [x.view() for x in o["outs"]],
+                                             direct_outs=[None if x is None else x.view() for x in o["douts"]],
+                                             mixtures=mixes, draws=draws)
+
+    def bufs(self, host):
+        o = self.o[host]
+        return o["outs"] + [x for x in o["douts"] if x is not None] + o["mix"] + o["spk"] + o["rms"]
+
+    def draw(self, gen):
+        for k, (key, _) in enumerate(self.layout):
+            n = self.pools[key].pools[True].n
+            self.picks[:, k].copy_(torch.randint(0, n, (self.U,), generator=gen, device="cuda", dtype=torch.int32))
+        self.u.uniform_(generator=gen)
+        self.sirs.uniform_(-6, 6, generator=gen)
+        self.snr.uniform_(10, 20, generator=gen)
+
+    def run(self, gen, tables, run, full_check, what):
+        """One run of both plans; returns the number of draws checked against draw_reference."""
+        self.draw(gen)
+        for host in (False, True):
+            for x in self.bufs(host):
+                x.reset()
+            self.plans[host].run()
+        torch.cuda.synchronize()
+        for a, b in zip(self.bufs(False), self.bufs(True)):            # (i)
+            assert np.array_equal(a.get(), b.get()), what
+        pk, st = self.picks.cpu().numpy(), self.starts.cpu().numpy()
+        used, u = self.used.cpu().numpy(), self.u.cpu().numpy()
+        sirs, snr = self.sirs.cpu().numpy(), self.snr.cpu().numpy()
+        o, S, checked = self.o[True], len(self.layout), 0
+        for e in range(self.U):
+            a = int(st[e])
+            stems = []
+            for k, (key, taps) in enumerate(self.layout):
+                pl = self.pools[key]
+                i = int(pk[e, k])
+                y = o["outs"][S * e + k].get()
+                stems.append(y)
+                if full_check or e in (0, 7, 15):                       # (ii)
+                    c = pl.cands[i]
+                    label = "%s run %d scene %d stem %d cand %d start %d" % (what, run, e, k, i, a)
+                    c.check(y, a, self.T, gain=pl.gain(i), key="B %s %s" % (what, pl.variant), label=label)
+                    if taps:
+                        c.check(o["douts"][S * e + k].get(), a, self.T, direct=True, gain=pl.gain(i),
+                                key="B %s %s" % (what, pl.variant), label=label + " direct")
+            check_mixture(np.stack([fold(s) for s in stems[:2]]), np.stack([fold(s) for s in stems[2:]]), sirs[e],
+                          snr[e], o["mix"][e].get().reshape(-1), o["spk"][e].get().reshape(2, -1),
+                          o["rms"][e].get().reshape(-1), "%s run %d scene %d" % (what, run, e))
+            tabs = [tables[self.layout[k][0]][int(pk[e, k])] for k in range(2)]
+            Nr = [self.pools[key].cands[int(pk[e, k])].N for k, (key, _) in enumerate(self.layout)]
+            if dr.margins(tabs, [self.T, self.T], Nr, self.T, u[e]) < NEAR_DB:
+                continue
+            assert (a, int(used[e])) == dr.draw(tabs, [self.T, self.T], Nr, self.T, u[e]), (what, run, e)
+            checked += 1
+        return checked
+
+    def close(self):
+        for p in self.plans.values():
+            p.close()
+
+
+def _tables(pl):
+    return [pl.pools[True].level_table(i).cpu().numpy() for i in range(pl.pools[True].n)]
+
+
+def _training(pools, layout, what, runs=3, min_draws=30):
+    R = _R()[1]
+    tr = Training(pools, layout)
+    gen = torch.Generator(device="cuda")
+    gen.manual_seed(77)
+    tables = {k: _tables(p) for k, p in pools.items() if p.pools[True].levels is not None}
+    for k, p in pools.items():
+        if p.pools[True].levels is not None:
+            for i in range(p.pools[True].n):
+                assert torch.equal(p.pools[True].level_table(i), p.pools[False].level_table(i)), (what, k, i)
+    try:
+        R.check_device_errors()
+        checked = sum(tr.run(gen, tables, r, r == 0, what) for r in range(runs))
+        assert checked >= min_draws, checked
+        for p in tr.plans.values():
+            assert p.is_graph()
+        R.check_device_errors()
+        print("\n%s: %d draws checked against draw_reference" % (what, checked))
+    finally:
+        tr.close()
+
+
+@pytest.mark.parametrize("budget", ["default", "one-chunk"])
+def test_training_configs1_pool(budget, chunk_budget):
+    R = chunk_budget(DEFAULT_CHUNK_BYTES if budget == "default" else ONE_CHUNK)
+    rng = np.random.default_rng(701)
+    spk, noi = b_configs1(rng)
+    pools = {"spk": Pools(spk, taps=True, levels="mono"), "noi": Pools(noi)}
+    _hold(*pools.values())
+    try:
+        _training(pools, [("spk", True), ("spk", True), ("noi", False)], "configs1 %s" % budget)
+        _report("B configs1 %s" % budget)
+    finally:
+        for p in pools.values():
+            p.close()
+    assert R
+
+
+def test_training_p60_pool_with_gains():
+    """P = 60 with random cuts (some candidates on the grid) over 32 shared RIR sets, loudness targets; 2 speakers, a
+    noise and a music per example."""
+    rng = np.random.default_rng(702)
+    N, P, C = 30 * RATE, 60, 6
+    rirs = [so.synth_rirs(rng, P, C, 4096) for _ in range(32)]
+    spk = [Cand(gappy_dry(rng, N) if j % 3 == 0 else so.synth_dry(rng, N), rirs[j % 32],
+                _random_cuts(rng, P, N, None if j % 4 else 60000))
+           for j in range(40)]
+    assert {_choice(c.b, N, P, 4096) for c in spk} == {0, 1}
+    stat = [Cand(so.synth_dry(rng, N - 1000 * j),
+                 (rng.standard_normal((1, C, 4096)) * np.exp(-np.arange(4096) / 800.0)).astype(np.float32), None)
+            for j in range(16)]
+    targets = [float(rng.uniform(-30, -16)) if j % 5 else None for j in range(len(spk))]
+    pools = {"spk": Pools(spk, levels="mono", lufs=targets, share=[j % 32 for j in range(len(spk))]),
+             "noi": Pools(stat[:8]), "mus": Pools(stat[8:])}
+    _hold(*pools.values())
+    try:
+        assert np.array_equal(pools["spk"].pools[False].loudness, pools["spk"].pools[True].loudness, equal_nan=True)
+        _training(pools, [("spk", False), ("spk", False), ("noi", False), ("mus", False)], "P=60 gains")
+        _report("B P=60 gains")
+    finally:
+        for p in pools.values():
+            p.close()
+
+
+def test_training_mixed_k_pool():
+    """32 configs[1]-shaped speakers with K = 1..4 in 48 slots (3 per scene)."""
+    import bench
+    rng = np.random.default_rng(703)
+    items = bench.make_inputs(16, 0)
+    Ls = (4096, 8192, 12288, 16384)
+    spk = []
+    for j, (x, h, b) in enumerate(items):
+        L = Ls[j % 4]
+        hh = h if L == 4096 else so.synth_rirs(rng, h.shape[0], h.shape[1], L)
+        spk.append(Cand(gappy_dry(rng, len(x)) if j % 2 else x, hh, b))
+    pools = {"spk": Pools(spk, levels="mono")}
+    _hold(*pools.values())
+    try:
+        _training(pools, [("spk", False)] * 3, "mixed-K")
+        _report("B mixed-K")
+    finally:
+        for p in pools.values():
+            p.close()
+
+
+# ----------------------------------------------------------------------------------------- C. mixed plans
+def test_mixed_plan_of_host_device_dry_and_unpooled_slots():
+    """Caller order interleaves host-pool slots (grid and aligned), device-pool slots, dry-picked device-pool slots,
+    unpooled banked moving sources (fast, long) and a static source; arrange_chunks regroups them by kernel variant."""
+    render, R = _R()
+    rng = np.random.default_rng(801)
+    grid, aligned = Pools(a_grid(rng)), Pools(a_aligned(rng), taps=True)
+    dev = Pools(a_aligned(rng))
+    longs = [Cand(so.synth_dry(rng, 40000 + 3 * j), so.synth_rirs(rng, 3, 2, 9000),
+                  np.array([0, 15000 + j, 40000 + 3 * j], np.int32)) for j in range(2)]
+    static = Cand(so.synth_dry(rng, 50001), so.synth_rirs(rng, 1, 2, 2048), None)
+    _hold(grid, aligned, dev)
+    dry = [so.synth_dry(rng, 140000) for _ in range(3)]
+    dpool = R.dry_pool([to(x) for x in dry])
+    banks = [R.rir_bank(to(c.h)) for c in longs] + [R.rir_bank(to(static.h[0]))]
+    wl = 20001
+    kinds = ["host grid", "device", "unpooled long", "host aligned", "dry", "static", "host grid", "unpooled long",
+             "device", "host aligned", "dry", "host grid"]
+    n = len(kinds)
+    picks = torch.zeros(n, dtype=torch.int32, device="cuda")
+    dpicks = torch.zeros(n, dtype=torch.int32, device="cuda")
+    starts = torch.zeros(n, dtype=torch.int32, device="cuda")
+
+    def sources(host):
+        srcs, unp = [], 0
+        for j, k in enumerate(kinds):
+            w = (starts[j], wl)
+            if k == "host grid":
+                srcs.append(render.Pooled(grid.pools[host], picks[j], w))
+            elif k == "host aligned":
+                srcs.append(render.Pooled(aligned.pools[host], picks[j], w, TAPS))
+            elif k == "device":
+                srcs.append(render.Pooled(dev.pools[False], picks[j], w))
+            elif k == "dry":
+                srcs.append(render.Pooled(dev.pools[False], picks[j], w, dry=render.DryPick(dpool, dpicks[j])))
+            elif k == "unpooled long":
+                c = longs[unp]
+                srcs.append(render.MovingSource(to(c.x), banks[unp], to(c.b), c.b, window=w))
+                unp += 1
+            else:
+                srcs.append(render.StaticSource(to(static.x), banks[2], window=w))
+        return srcs
+
+    C = [3 if k == "host grid" else 2 for k in kinds]
+    outs = {h: [Out(c, wl) for c in C] for h in (False, True)}
+    douts = {h: [Out(2, wl) if k == "host aligned" else None for k in kinds] for h in (False, True)}
+    plans = {h: R.plan_device(sources(h), [o.view() for o in outs[h]],
+                              direct_outs=[None if o is None else o.view() for o in douts[h]]) for h in (False, True)}
+    try:
+        R.check_device_errors()
+        counts = {}
+        for run in range(4):
+            pk, dp, st = [], [], []
+            for j, k in enumerate(kinds):
+                if k.startswith("host"):
+                    cs = (grid if "grid" in k else aligned).cands
+                elif k in ("device", "dry"):
+                    cs = dev.cands
+                else:
+                    cs = longs if "long" in k else [static]
+                i = int(rng.integers(0, len(cs))) if k != "unpooled long" else kinds[:j].count(k)
+                N = cs[i].N if k != "static" else static.N
+                pk.append(i if k != "static" else 0)
+                dp.append(int(rng.integers(0, len(dry))))
+                st.append((0, N - wl, int(rng.integers(0, N - wl + 1)), N - wl - 2 * B + 1)[(run + j) % 4])
+            picks.copy_(torch.tensor(pk, dtype=torch.int32))
+            dpicks.copy_(torch.tensor(dp, dtype=torch.int32))
+            starts.copy_(torch.tensor(st, dtype=torch.int32))
+            for h in (False, True):
+                for o in outs[h] + [x for x in douts[h] if x is not None]:
+                    o.reset()
+                R.reset_stats()
+                plans[h].run()
+                counts[h] = R.launch_count()
+            torch.cuda.synchronize()
+            if run > 0:
+                assert counts[True] == counts[False] + 1, counts
+            for j, k in enumerate(kinds):
+                y = outs[True][j].get()
+                assert np.array_equal(y, outs[False][j].get()), (run, j, k)
+                label = "mixed plan run %d slot %d (%s)" % (run, j, k)
+                if k.startswith("host"):
+                    c = (grid if "grid" in k else aligned).cands[pk[j]]
+                elif k == "device":
+                    c = dev.cands[pk[j]]
+                elif k == "dry":
+                    d = dev.cands[pk[j]]
+                    c = Cand(dry[dp[j]][:d.N], d.h, d.b)
+                elif k == "unpooled long":
+                    c = longs[pk[j]]
+                else:
+                    c = static
+                c.check(y, st[j], wl, key="C mixed %s" % k, label=label)
+                if douts[True][j] is not None:
+                    yd = douts[True][j].get()
+                    assert np.array_equal(yd, douts[False][j].get()), (run, j, k)
+                    c.check(yd, st[j], wl, direct=True, key="C mixed %s" % k, label=label + " direct")
+        for p in plans.values():
+            assert p.is_graph()
+        # a side stream, behind queued work
+        ref = [o.get().copy() for o in outs[True]]
+        for o in outs[True]:
+            o.reset()
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            torch.cuda._sleep(int(2e7))
+            plans[True].run(s.cuda_stream)
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        for j, o in enumerate(outs[True]):
+            assert np.array_equal(o.get(), ref[j]), ("side stream", j)
+        R.check_device_errors()
+        _report("C mixed")
+    finally:
+        for p in plans.values():
+            p.close()
+        for k in banks:
+            k.close()
+        dpool.close()
+        for p in (grid, aligned, dev):
+            p.close()
+
+
+def stage_bytes(cands, wl, sets):
+    """stage_bytes of ss_kernels.cu: the view, sets * rows_cap rows and nx_cap dry floats, each 256-aligned, with the
+    capacity (stage_cap) the largest read set over every start of every candidate."""
+    rows = nx = 0
+    for c in cands:
+        xa, xb, _, r = stage_set_np(c.N, c.P, c.C, c.K, c.b, np.arange(c.N - wl + 1), wl)
+        rows, nx = max(rows, int(r.max())), max(nx, int((xb - xa).max()) + 8)
+    return align_up(56, 256) + align_up(sets * rows * B * 8, 256) + align_up(4 * nx, 256)
+
+
+def test_many_staged_slots():
+    """1056 host-pool slots with 1500-sample windows over small candidates: a k_stage grid of 1056 rows and several
+    chunks under the default budget."""
+    render, R = _R()
+    rng = np.random.default_rng(802)
+    cands = []
+    for j in range(6):
+        N, P = 20001 + 1001 * j, 3 + j % 3
+        cands.append(Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 1, 2000), _random_cuts(rng, P, N)))
+    pl = Pools(cands)
+    _hold(pl)
+    n, wl = 1056, 1500
+    pr = Probes(pl, [wl], n - 1, [123])
+    try:
+        for run in range(2):
+            pk = rng.integers(0, len(cands), n)
+            st = [int(rng.integers(0, cands[p].N - wl + 1)) for p in pk]
+            pr.run(pk, st)
+            # every slot in the first run (so the first and last staged slots, whatever order arrange_chunks gives
+            # them), the first, last and 40 others in the second
+            sample = range(n) if run == 0 else sorted({0, n - 1} | set(rng.choice(n, 40, replace=False).tolist()))
+            for j in sample:
+                c = cands[pr.pk[j]]
+                c.check(pr.outs[True][j].get(), pr.st[j], wl, key="C many", label="many run %d slot %d" % (run, j))
+        launches = pr.launches
+        chunks = launches[False] / 3                     # k_blocks, k_prepare and the render per chunk
+        print("\nmany slots: %d host-pool slots, %g chunks, launches per run %s (device, host pools), %d bytes of "
+              "staging (restated stage_bytes)" % (n, chunks, launches, n * stage_bytes(cands, wl, 1)))
+        assert launches[True] == launches[False] + 1 and chunks == int(chunks) and chunks > 1, launches
+        R.check_device_errors()
+        _report("C many")
+    finally:
+        pr.close()
+        pl.close()
+
+
+# ----------------------------------------------------------------------------------------- D. builds across batches
+def copy_batches(C, cands, first):
+    """render_host_stems' batching restated: candidate i's copy is its reverberant spectra and dry signal, each
+    256-aligned (stem_copy_bytes); the buffer holds max(largest copy, min(all copies, 256 MiB)) (stem_copy_cap); inside
+    every stem group a batch takes candidates while they fit, and always at least one.  Returns every batch's first
+    candidate."""
+    cb = [align_up(8 * B * c.P * C * c.K, 256) + align_up(4 * c.N, 256) for c in cands]
+    cap = max(max(cb), min(sum(cb), STEM_BYTES))
+    starts = []
+    for g in range(len(first) - 1):
+        lo = first[g]
+        while lo < first[g + 1]:
+            starts.append(lo)
+            used, hi = 0, lo
+            while hi < first[g + 1] and (hi == lo or used + cb[hi] <= cap):
+                used += cb[hi]
+                hi += 1
+            lo = hi
+    return starts, cap
+
+
+def d_speakers(rng):
+    import bench
+    items = bench.make_inputs(24, 0)
+    N, P, C = 30 * RATE, 60, 6
+    cut = {5: 1, 18: 7, 30: 13, 47: 29}
+    out = []
+    for j, (x, _, _) in enumerate(items):
+        n = N - cut.get(j, 0)
+        b = _random_cuts(rng, P, n)
+        out.append(Cand(gappy_dry(rng, n) * np.float32(4.0) if j % 2 else x[:n].copy(), so.synth_rirs(rng, P, C, 4096), b))
+    return out
+
+
+def d_giant(rng):
+    """A moving 8-channel pool: one candidate with P = 400 and L = 12288 (315 MB of spectra) between ordinary ones."""
+    out = []
+    for j in range(5):
+        if j == 2:
+            P, L, N = 400, 12288, 400003
+        else:
+            P, L, N = 5, 4096, 300001 + 7 * j
+        out.append(Cand(so.synth_dry(rng, N) * np.float32(0.5 + 0.25 * (j % 3)), so.synth_rirs(rng, P, 8, L),
+                        np.round(np.linspace(0, N, P)).astype(np.int32)))
+    return out
+
+
+def host_alone(R, render, c, target):
+    """render_host of the candidate alone over a device bank: the (C, N) stem and, with a target, (LUFS, gain)."""
+    bank = R.rir_bank(c.h)
+    try:
+        lo = []
+        y = R.render_host([render.MovingSource(c.x, bank, c.b)], lufs_targets=None if target is None else [target],
+                          loudness_out=lo, sr=RATE)[0]
+    finally:
+        bank.close()
+    return y, (tuple(lo[0]) if target is not None else None)
+
+
+@pytest.mark.parametrize("kind", ["speakers", "giant"])
+def test_host_builds_across_copy_batches(kind):
+    render, R = _R()
+    rng = np.random.default_rng(901 if kind == "speakers" else 902)
+    cands = d_speakers(rng) if kind == "speakers" else d_giant(rng)
+    C = cands[0].C
+    first, _ = stem_groups(C, [c.N for c in cands])
+    batches, cap = copy_batches(C, cands, first)
+    inside = [s for s in batches if s not in first]
+    print("\n%s: stem groups %s, copy batches %s, copy buffer %d bytes" % (kind, first, batches, cap))
+    if kind == "speakers":
+        assert inside, (first, batches)                   # a batch boundary strictly inside a stem group
+        unmeasured = {inside[0], first[1], first[1] - 1}
+        silent = {inside[0] - 1}
+    else:
+        assert cap > STEM_BYTES and 2 in batches and 3 in batches, (batches, cap)
+        unmeasured, silent = {1}, {3}                      # on each side of the giant
+    for j in silent:
+        cands[j].x[:] = 0.0
+    trng = np.random.default_rng(903)
+    targets = [None if j in unmeasured else float(trng.uniform(-30, -14)) for j in range(len(cands))]
+    refs = [host_alone(R, render, c, t) for c, t in zip(cands, targets)]
+    oracle = [None if t is None or j in silent else
+              so.bs1770_integrated_loudness(host_alone(R, render, c, None)[0].T.astype(np.float64), RATE, 0.4,
+                                            up_to_8_channels=True) for j, (c, t) in enumerate(zip(cands, targets))]
+    worst_tab = worst_db = 0.0
+    for levels in ("mono", "channels"):
+        pl = Pools(cands, levels=levels, lufs=targets)
+        _hold(pl)
+        try:
+            Ld, Lh = pl.pools[False].loudness, pl.pools[True].loudness
+            assert Ld.tobytes() == Lh.tobytes(), (kind, levels)
+            for i, (c, t) in enumerate(zip(cands, targets)):
+                what = (kind, levels, i)
+                q = pl.pools[True].level_table(i)
+                assert torch.equal(q, pl.pools[False].level_table(i)), what
+                y, lo = refs[i]
+                if t is None:
+                    assert np.isnan(Lh[i]).all(), what
+                else:
+                    assert (Lh[i, 0], Lh[i, 1]) == lo, (what, Lh[i], lo)
+                    if i in silent:
+                        assert np.isneginf(Lh[i, 0]), what
+                    else:
+                        d = abs(Lh[i, 0] - oracle[i])
+                        assert d < 1e-6, (what, Lh[i, 0], oracle[i])
+                        worst_db = max(worst_db, d)
+                r = table_error(q.cpu().numpy(), y, levels == "mono")
+                assert r <= TABLE_TOL, (what, r / TABLE_TOL)
+                worst_tab = max(worst_tab, r)
+            if kind == "speakers" and levels == "mono":
+                _training({"spk": pl}, [("spk", False)] * 3, "D speakers", runs=2, min_draws=20)
+        finally:
+            pl.close()
+    print("%s: worst table error %.3g x TABLE_TOL, worst loudness vs the oracle %.3g dB" %
+          (kind, worst_tab / TABLE_TOL, worst_db))

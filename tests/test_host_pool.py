@@ -5,7 +5,10 @@ copies for a pooled slot of a host pool (stage_set) and the staging area a plan 
   - it never exceeds the slot's staging area, which is the largest set of any candidate at any start;
   - the head of k_blocks over the staged view (take_view) builds the same Source, block table, work items, h_row0 / h_rows
     origin and direct-set rows as over the full candidate (pick_slot), and the slot renders the same bits from copies
-    that hold the read set and NaN everywhere else."""
+    that hold the read set and NaN everywhere else;
+  - a NumPy restatement of stage_set matches the kernels' at sampled starts, and over every start of training-shaped
+    candidates (N = 480 000, P in {40, 60} with runs of short segments, K = 1..4, static and moving) stage_cap equals
+    the largest read set exactly."""
 import ctypes
 import os
 import subprocess
@@ -155,6 +158,112 @@ def test_both_blockings_and_every_k_are_covered():
         for L in Ls:
             seen.add(("static" if P == 1 else "moving", _k(L)))
     assert {k for _, k in seen} == {1, 2, 3, 4} and {"static", "moving"} <= {m for m, _ in seen}
+
+
+def stage_set_np(N, P, C, K, bounds, ws, wl):
+    """stage_set (ss_phases.cuh) in NumPy over an array of starts ws: (xa, xb, row0, rows) as int64 arrays.  The dry span
+    [ws - (K + 2) 4096, ws + wl + 2 * 4096) clamped to [0, N); the rows of every position whose segment holds a sample of
+    it and the one after, widened to row pairs and clipped to the bank (window_rows)."""
+    ws = np.asarray(ws, np.int64)
+    xa = np.maximum(ws - (K + 2) * B, 0)
+    xb = np.minimum(ws + wl + 2 * B, N)
+    if P > 1:
+        inner = np.asarray(bounds, np.int64)[1:P]             # seg_of: bounds[1..P-1] <= n, clamped to P - 2
+        pa = np.minimum(np.searchsorted(inner, xa, side="right"), P - 2)
+        pb = np.minimum(np.searchsorted(inner, xb - 1, side="right"), P - 2) + 1
+    else:
+        pa, pb = np.zeros_like(ws), np.zeros_like(ws)
+    ck = C * K
+    r0 = (pa * ck) & ~1
+    r1 = np.minimum(((pb + 1) * ck + 1) & ~1, P * ck)
+    return xa, xb, r0, r1 - r0
+
+
+def _emu_stage_set(emu, c, ws, wl):
+    out = np.zeros(4, np.int32)
+    emu.emu_stage_set(c.N, c.P, c.C, c.K, _p(c.bounds), int(ws), wl, _p(out))
+    return out.tolist()
+
+
+class Shape:
+    """A candidate's shape alone (no signals): N, P, C, K and its trajectory."""
+
+    def __init__(self, N, P, C, K, bounds):
+        self.N, self.P, self.C, self.K, self.bounds = N, P, C, K, bounds
+
+
+def training_bounds(rng, P, N):
+    """Random cuts over [0, N) with a run of segments shorter than 4096 (some empty) somewhere inside."""
+    k = P // 3
+    at = int(rng.integers(0, N - 12000))
+    short = at + np.sort(rng.integers(0, 12000, k))
+    cuts = np.sort(np.concatenate([short, rng.integers(0, N + 1, P - 2 - k)]))
+    return np.ascontiguousarray(np.concatenate([[0], cuts, [N]]), np.int32)
+
+
+TRAIN_N = 480000
+TRAIN_LENS = [64000, 3 * B + 5, 1000]
+
+
+def training_shapes(seed):
+    """Static and moving (P = 40, 60) training-shaped candidates with K = 1..4 and C in {6, 1, 3}."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for K in (1, 2, 3, 4):
+        for P, C in ((1, 6), (40, 6), (60, 6), (40, 1), (60, 3)):
+            out.append(Shape(TRAIN_N, P, C, K, None if P == 1 else training_bounds(rng, P, TRAIN_N)))
+    return out
+
+
+def test_numpy_stage_set_matches_the_kernels(emu):
+    """The NumPy restatement against emu_stage_set (the kernels' own stage_set) at every segment edge +-1, the
+    maximisers of stage_cap, both clamps and random starts of the training shapes and of short candidates."""
+    lib = emu
+    rng = np.random.default_rng(31)
+    shapes = training_shapes(30) + [Shape(n, P, C, K, None if P == 1 else training_bounds(rng, P, n))
+                                    for n, P, C, K in ((13001, 4, 2, 1), (20003, 6, 3, 3), (9002, 1, 5, 4))]
+    n = 0
+    for c in shapes:
+        for wl in TRAIN_LENS:
+            last = c.N - wl
+            if last < 0:
+                continue
+            ws = {0, last, min(last, (c.K + 2) * B), min(last, (c.K + 2) * B - 1)}
+            ws |= {int(v) for v in rng.integers(0, last + 1, 60)}
+            for b in ([] if c.bounds is None else c.bounds[1:-1]):
+                for d in (-1, 0, 1):
+                    for v in (b + d, b + d + (c.K + 2) * B, b + d - wl - 2 * B):
+                        if 0 <= v <= last:
+                            ws.add(int(v))
+            ws = np.array(sorted(ws), np.int64)
+            got = np.stack(stage_set_np(c.N, c.P, c.C, c.K, c.bounds, ws, wl), axis=1)
+            for w, g in zip(ws, got):
+                assert g.tolist() == _emu_stage_set(lib, c, w, wl), (c.P, c.C, c.K, wl, int(w))
+            n += len(ws)
+    assert n > 10000
+
+
+@pytest.mark.parametrize("wl", TRAIN_LENS)
+def test_stage_cap_is_the_maximum_over_every_start(emu, wl):
+    """N = 480 000, P in {40, 60} with random cuts that include segments shorter than 4096, K = 1..4, static and moving:
+    stage_cap of each candidate alone, and of all the moving (and all the static) candidates of one C as one pool,
+    equals the largest read set over every start in [0, N - len] exactly - rows, and dry samples + 8."""
+    lib = emu
+    shapes = training_shapes(40 + wl % 97)
+    ws = np.arange(TRAIN_N - wl + 1, dtype=np.int64)
+    most = []
+    for c in shapes:
+        xa, xb, _, rows = stage_set_np(c.N, c.P, c.C, c.K, c.bounds, ws, wl)
+        m = (int(rows.max()), int((xb - xa).max()) + 8)
+        assert _cap(lib, [c], wl) == m, (c.P, c.C, c.K, wl, _cap(lib, [c], wl), m)
+        most.append(m)
+    for static in (True, False):
+        for C in {c.C for c in shapes}:
+            group = [i for i, c in enumerate(shapes) if c.C == C and (c.P == 1) == static]
+            if not group:
+                continue
+            want = (max(most[i][0] for i in group), max(most[i][1] for i in group))
+            assert _cap(lib, [shapes[i] for i in group], wl) == want, (static, C, wl)
 
 
 @pytest.mark.parametrize("case", range(len(CASES)))
