@@ -260,7 +260,9 @@ void ss_pool_destroy(ss_pool* pool);          /* destroy pools after the plans t
  *     they reach.  The slot then renders from the staged copies with the bits of the same slot over a device pool.
  *   - ss_pool_bytes keeps counting device bytes: for a host pool the n entries, the partition counts and gains as for a
  *     device pool, the device copies of the bounds (4 * P bytes per moving candidate) and cut tables, and the level
- *     tables' pointer array; ss_pool_host_bytes counts the arena and the level tables. */
+ *     tables' pointer array; ss_pool_host_bytes counts the arena and the level tables.
+ *   - Dry picks (ss_dry_pick, below) on a host pool's slots take a host dry pool (SS_DRY_HOST): k_stage then copies the
+ *     same dry samples from the picked dry signal instead of the candidate's x.  A device dry pool is refused there. */
 int64_t ss_pool_host_bytes(const ss_pool* pool);   /* pinned host bytes held (0 for a device pool) */
 
 /* ---- level tables of a pool (version 107), for the start draws of plans (ss_plan_draw below).  Gives every candidate
@@ -423,8 +425,8 @@ int ss_plan_create_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss
  * dry signals that pooled slots take their dry signal from, picked on the device at every run independently of the
  * trajectory pick, so that (#dry signals x #trajectories) combinations are reachable with no host work.
  *   - ss_dry_pool_create: x[i] is a DEVICE pointer (4-byte aligned) to signal i, float32, lengths[i] samples (1 <=
- *     lengths[i] <= 2^31 - 1 - 16384, the bound of ss_source.N); 1 <= n <= 2^24.  The pool references the signals, which
- *     must outlive it; their contents may change between runs, as a candidate's x may.  flags = SS_DRY_LEVELS also builds
+ *     lengths[i] <= 2^31 - 1 - 16384, the bound of ss_source.N); 1 <= n <= 2^24.  The pool (unless SS_DRY_HOST, below)
+ *     references the signals, which must outlive it; their contents may change between runs, as a candidate's x may.  flags = SS_DRY_LEVELS also builds
  *     every signal's level table: Q[0] = 0, Q[n + 1] = Q[n] + (double)(x[n] * x[n]) in float64 (lengths[i] + 1 doubles,
  *     8 bytes per sample), by the scan of ss_pool_levels over the signal as a one-channel stem (whose mono fold is the
  *     signal itself), on a stream of the library's own: the signals must be complete when the call is made (synchronise
@@ -445,18 +447,35 @@ int ss_plan_create_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss
  *     is the dataloader's rule applied to the dry speech: no table of the rendered stem exists for a pair drawn at run
  *     time.  The gaps create_long_audio leaves between utterances are exact zeros of the dry stream, so the rule still
  *     rejects crops that fall in a gap.  M is unchanged (the readers' picked candidates' N); speakers with and without a
- *     dry pick may share a draw.  A run with dry picks launches exactly as many kernels as the same plan without them.
+ *     dry pick may share a draw.  A run with dry picks from a device dry pool launches exactly as many kernels as the
+ *     same plan without them.
  *   - Mixtures take dry-picked stems like any other; a static pool (noise) takes dry picks as a moving one does.
+ *   - Host dry pools: with flags | SS_DRY_HOST, x[i] may be a HOST pointer (pageable or pinned) or a device pointer.  The
+ *     pool copies every signal into one pinned, mapped arena it owns (each at a 64-byte boundary, zero-padded to a whole
+ *     number of float4s; 64-bit offsets), so the caller's buffers need not outlive the call.  With SS_DRY_LEVELS the
+ *     tables are built as above from transient device copies of the signals, in batches of at most 256 MB (or one
+ *     signal's, when larger), and kept in pinned, mapped host memory, bit for bit a device dry pool's tables; k_draw reads
+ *     them over PCIe.  ss_dry_pool_bytes counts the device bytes only (the n signal pointers, and the n table pointers);
+ *     ss_dry_pool_host_bytes counts the arena and the tables; ss_dry_pool_level_table returns a mapped host address.
+ *     In a plan every slot with a host dry pick is staged, as a host pool's slots are: at every run k_stage reads its
+ *     pick (bit 3) and its dry pick (clamped, bit 4), and copies the dry samples the picked candidate's window reads,
+ *     [ws - (K + 2) * 4096, ws + win_len + 2 * 4096) clamped to [0, N), of the PICKED SIGNAL into a staging area sized
+ *     once per pool and window length.  A slot of a device pool stages nothing else (its spectra stay the bank's), so a
+ *     plan over device pools launches one kernel more per run than with a device dry pool; a host pool's slot stages its
+ *     rows as before, so a host-pool plan launches as many kernels with host dry picks as without.  Bits, draws and
+ *     errors are those of the same plan over a device dry pool of the same signals.
  * Refused by ss_plan_create_dry, before anything is allocated and with no plan created (SS_ERR_INVALID): n_picks < 0, a
- * NULL picks with n_picks > 0; a slot outside [0, n_items), or named by two dry picks; a slot that is not pooled, or whose
- * pool is a host pool (k_stage stages the candidate's own x) or has loudness gains (measured with the candidates' own
- * dry signals); a NULL pool or one of another context; a dry pool with a signal shorter than the slot pool's longest
- * candidate N; a NULL or unaligned pick_dev; a draw speaker with a dry pick whose dry pool has no level tables; a range a
- * plan writes that meets a dry pick or a signal of a dry pool it uses.  A destroyed dry pool cannot be detected: a dry
- * pool must outlive every plan that uses it; ss_dry_pool_destroy waits for the device before it frees it.
- * n_picks == 0 makes ss_plan_create_dry exactly ss_plan_create_ex.  ss_version stays 108: these exports mark the
- * capability. */
+ * NULL picks with n_picks > 0; a slot outside [0, n_items), or named by two dry picks; a slot that is not pooled, or
+ * whose pool has loudness gains (measured with the candidates' own dry signals), or is a host pool while the dry pool is
+ * a device one (k_stage copies whole float4s, which only a host dry pool's padded arena guarantees); a NULL pool or one
+ * of another context; a dry pool with a signal shorter than the slot pool's longest candidate N; a NULL or unaligned
+ * pick_dev; a draw speaker with a dry pick whose dry pool has no level tables; a range a plan writes that meets a dry
+ * pick or a signal of a device dry pool it uses (a host dry pool owns its arena).  A destroyed dry pool cannot be
+ * detected: a dry pool must outlive every plan that uses it; ss_dry_pool_destroy waits for the device before it frees it.
+ * n_picks == 0 makes ss_plan_create_dry exactly ss_plan_create_ex.  ss_version stays 108: these exports (and
+ * ss_dry_pool_host_bytes for host dry pools) mark the capability. */
 #define SS_DRY_LEVELS 1u
+#define SS_DRY_HOST 0x100u
 typedef struct {
     int32_t slot;                     /* index into `items` of a pooled slot                                           */
     const ss_dry_pool* pool;          /* the dry pool it takes its dry signal from                                     */
@@ -465,8 +484,12 @@ typedef struct {
 int ss_dry_pool_create(ss_ctx* ctx, const float* const* x, const int32_t* lengths, int n, uint32_t flags,
                        ss_dry_pool** out);
 int64_t ss_dry_pool_bytes(const ss_dry_pool* pool);   /* device bytes held: n signal pointers (8 B each), and with level
-                                                       * tables the tables (8 B per sample + 8) and their n pointers */
-/* Device pointer of signal i's level table (lengths[i] + 1 doubles), or NULL without tables or with i outside [0, n). */
+                                                       * tables the tables (8 B per sample + 8, not for a host dry
+                                                       * pool) and their n pointers */
+int64_t ss_dry_pool_host_bytes(const ss_dry_pool* pool);   /* pinned host bytes held: the arena and the tables (0 for a
+                                                            * device dry pool) */
+/* Device pointer of signal i's level table (lengths[i] + 1 doubles; a mapped host address for a host dry pool), or NULL
+ * without tables or with i outside [0, n). */
 const double* ss_dry_pool_level_table(const ss_dry_pool* pool, int i);
 void ss_dry_pool_destroy(ss_dry_pool* pool);          /* destroy dry pools after the plans that use them */
 int ss_plan_create_dry(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,

@@ -845,7 +845,9 @@ struct ss_pool {
     std::vector<std::pair<int, std::pair<int, int>>> stage_caps;  // (win_len, (rows, dry samples)) (stage_cap)
 };
 // Dry pool: n dry signals referenced by their device pointers (the caller's buffers), the device array of those pointers
-// that dry-picked slots index (dry_table), and with SS_DRY_LEVELS every signal's level table.
+// that dry-picked slots index (dry_table), and with SS_DRY_LEVELS every signal's level table.  A host dry pool
+// (SS_DRY_HOST) owns its signals, copied into one pinned, mapped arena, and keeps its tables in pinned, mapped host
+// memory: x, ptrs, levels and level_ptr then hold mapped device addresses.
 struct ss_dry_pool {
     ss_ctx* c = nullptr;
     int n = 0, n_min = 0;                 // n_min: the shortest signal (the longest candidate N it serves)
@@ -855,6 +857,10 @@ struct ss_dry_pool {
     double* levels = nullptr;             // device: every signal's N + 1 doubles back to back
     const double** level_ptr = nullptr;   // device, n table pointers
     std::vector<int64_t> level_off;       // signal i's table at levels + level_off[i]
+    bool host = false;                    // SS_DRY_HOST
+    char* h_x = nullptr;                  // the arena (host address) and its bytes
+    size_t h_x_bytes = 0;
+    double* h_levels = nullptr;           // the tables' host address
 };
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
@@ -2013,29 +2019,99 @@ extern "C" void ss_dry_pool_destroy(ss_dry_pool* dp) {
     cudaSetDevice(dp->c->device);
     cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
     if (dp->ptrs) cudaFree(dp->ptrs);
-    if (dp->levels) cudaFree(dp->levels);
+    if (dp->h_levels) cudaFreeHost(dp->h_levels); else if (dp->levels) cudaFree(dp->levels);
     if (dp->level_ptr) cudaFree(dp->level_ptr);
+    if (dp->h_x) cudaFreeHost(dp->h_x);
     delete dp;
+}
+static int64_t dry_level_bytes(const ss_dry_pool* dp) {
+    return dp->levels ? (int64_t)sizeof(double) * dp->level_off[dp->n] : 0;
 }
 extern "C" int64_t ss_dry_pool_bytes(const ss_dry_pool* dp) {
     if (!dp) return 0;
     int64_t b = (int64_t)sizeof(float*) * dp->n;
-    if (dp->levels) b += (int64_t)sizeof(double) * dp->level_off[dp->n] + (int64_t)sizeof(double*) * dp->n;
+    if (dp->levels) b += (dp->host ? 0 : dry_level_bytes(dp)) + (int64_t)sizeof(double*) * dp->n;
     return b;
 }
-extern "C" const double* ss_dry_pool_level_table(const ss_dry_pool* dp, int i) {
-    return dp && dp->levels && i >= 0 && i < dp->n ? dp->levels + dp->level_off[i] : nullptr;
+extern "C" int64_t ss_dry_pool_host_bytes(const ss_dry_pool* dp) {
+    return dp && dp->host ? (int64_t)dp->h_x_bytes + dry_level_bytes(dp) : 0;
 }
-// The signals' pointer array, and with level tables the tables - k_levels over each signal as a one-channel stem, whose
-// mono fold is the signal itself - built on a transient stream; returns when they are in device memory.
+extern "C" const double* ss_dry_pool_level_table(const ss_dry_pool* dp, int i) {
+    if (!dp || !dp->levels || i < 0 || i >= dp->n) return nullptr;
+    return (dp->host ? dp->h_levels : dp->levels) + dp->level_off[i];
+}
+// A host dry pool: the signals into its pinned, mapped arena, each at a 64-byte boundary and zero-padded to whole
+// float4s (k_stage copies whole float4s around a read set); x[i] becomes the signal's mapped device address
+static int dry_host_copies(ss_dry_pool* dp) {
+    const int n = dp->n;
+    std::vector<size_t> xo(n + 1, 0);
+    for (int i = 0; i < n; ++i) xo[i + 1] = xo[i] + align_up(sizeof(float) * (size_t)dp->N[i], 64);
+    dp->h_x_bytes = xo[n];
+    CK(cudaHostAlloc((void**)&dp->h_x, dp->h_x_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+    char* dx = nullptr;
+    CK(cudaHostGetDevicePointer((void**)&dx, dp->h_x, 0));
+    for (int i = 0; i < n; ++i) {
+        const size_t b = sizeof(float) * (size_t)dp->N[i];
+        CK(cudaMemcpy(dp->h_x + xo[i], dp->x[i], b, cudaMemcpyDefault));
+        memset(dp->h_x + xo[i] + b, 0, xo[i + 1] - xo[i] - b);
+        dp->x[i] = (const float*)(dx + xo[i]);
+    }
+    return SS_OK;
+}
+// A host dry pool's level tables: k_levels over transient device copies of the signals, in batches of at most
+// kLevelStemBytes of copies (or one signal's, when larger), each batch's copies behind the previous batch's scan on `s`;
+// k_levels writes the tables into pinned, mapped host memory.  `li` holds every signal's descriptor with its table.
+static int dry_host_levels(ss_dry_pool* dp, std::vector<LevelItem>& li, cudaStream_t s) {
+    const int n = dp->n;
+    std::vector<size_t> at(n);
+    std::vector<int> first(1, 0);
+    size_t used = 0, cap = kLevelStemBytes;
+    for (int i = 0; i < n; ++i) cap = std::max(cap, align_up(sizeof(float) * (size_t)dp->N[i], 256));
+    for (int i = 0; i < n; ++i) {
+        const size_t b = align_up(sizeof(float) * (size_t)dp->N[i], 256);
+        if (used > 0 && used + b > cap) { first.push_back(i); used = 0; }
+        at[i] = used;
+        used += b;
+    }
+    first.push_back(n);
+    if (first.size() == 2) cap = used;                  // one batch: no more than it needs
+    char* buf = nullptr;
+    CK(cudaMalloc((void**)&buf, cap));
+    struct Free { void* p; ~Free() { cudaFree(p); } } free_buf{buf};   // (cudaFree waits for the device)
+    for (int i = 0; i < n; ++i) li[i].y = (const float*)(buf + at[i]);
+    LevelItem* d_items = nullptr;
+    CK(cudaMalloc((void**)&d_items, sizeof(LevelItem) * (size_t)n));
+    struct Free free_items{d_items};
+    CK(cudaMemcpy(d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
+    for (size_t g = 0; g + 1 < first.size(); ++g) {
+        for (int i = first[g]; i < first[g + 1]; ++i)
+            CK(cudaMemcpyAsync((void*)li[i].y, dp->x[i], sizeof(float) * (size_t)dp->N[i], cudaMemcpyDefault, s));
+        for (int k = first[g]; k < first[g + 1]; k += 65535) {
+            const int st = levels_enqueue(dp->c, d_items + k, std::min(first[g + 1] - k, 65535), true, s);
+            if (st) return st;
+        }
+    }
+    CK(cudaStreamSynchronize(s));
+    return SS_OK;
+}
+// The signals' pointer array (a host dry pool's after its arena copies), and with level tables the tables - k_levels over
+// each signal as a one-channel stem, whose mono fold is the signal itself - built on a transient stream; returns when
+// they are complete.
 static int dry_pool_build(ss_dry_pool* dp, bool levels) {
     const int n = dp->n;
+    if (dp->host) { const int st = dry_host_copies(dp); if (st) return st; }
     CK(cudaMalloc((void**)&dp->ptrs, sizeof(float*) * (size_t)n));
     CK(cudaMemcpy(dp->ptrs, dp->x.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice));
     if (!levels) return SS_OK;
     dp->level_off.assign(n + 1, 0);
     for (int i = 0; i < n; ++i) dp->level_off[i + 1] = dp->level_off[i] + dp->N[i] + 1;
-    CK(cudaMalloc((void**)&dp->levels, sizeof(double) * (size_t)dp->level_off[n]));
+    const size_t tb = sizeof(double) * (size_t)dp->level_off[n];
+    if (dp->host) {                                     // k_levels writes and k_draw reads them over PCIe
+        CK(cudaHostAlloc((void**)&dp->h_levels, tb, cudaHostAllocMapped | cudaHostAllocPortable));
+        CK(cudaHostGetDevicePointer((void**)&dp->levels, dp->h_levels, 0));
+    } else {
+        CK(cudaMalloc((void**)&dp->levels, tb));
+    }
     CK(cudaMalloc((void**)&dp->level_ptr, sizeof(double*) * (size_t)n));
     std::vector<const double*> ptr(n);
     std::vector<LevelItem> li(n);
@@ -2044,12 +2120,13 @@ static int dry_pool_build(ss_dry_pool* dp, bool levels) {
         li[i] = {dp->x[i], dp->levels + dp->level_off[i], dp->N[i], 1, 0};
     }
     CK(cudaMemcpy(dp->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
+    BuildStream bs;
+    CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
+    if (dp->host) return dry_host_levels(dp, li, bs.s);
     LevelItem* d_items = nullptr;
     CK(cudaMalloc((void**)&d_items, sizeof(LevelItem) * (size_t)n));
     struct Free { void* p; ~Free() { cudaFree(p); } } free_items{d_items};   // (cudaFree waits for the device)
     CK(cudaMemcpy(d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
-    BuildStream bs;
-    CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
     for (int k = 0; k < n; k += 65535) {
         const int st = levels_enqueue(dp->c, d_items + k, std::min(n - k, 65535), true, bs.s);
         if (st) return st;
@@ -2059,14 +2136,15 @@ static int dry_pool_build(ss_dry_pool* dp, bool levels) {
 }
 extern "C" int ss_dry_pool_create(ss_ctx* c, const float* const* x, const int32_t* lengths, int n, uint32_t flags,
                                   ss_dry_pool** out) {
-    if (!c || !x || !lengths || !out || n < 1 || n > (1 << 24) || (flags & ~SS_DRY_LEVELS)) return SS_ERR_INVALID;
+    if (!c || !x || !lengths || !out || n < 1 || n > (1 << 24) || (flags & ~(SS_DRY_LEVELS | SS_DRY_HOST)))
+        return SS_ERR_INVALID;
     *out = nullptr;
     for (int i = 0; i < n; ++i)                         // (the bound of validate_item on N)
         if (!x[i] || ((uintptr_t)x[i] & 3) || lengths[i] < 1 || lengths[i] > 0x7fffffff - 2 * kF) return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     ss_dry_pool* dp = new (std::nothrow) ss_dry_pool();
     if (!dp) return SS_ERR_NOMEM;
-    dp->c = c; dp->n = n;
+    dp->c = c; dp->n = n; dp->host = (flags & SS_DRY_HOST) != 0;
     dp->x.assign(x, x + n);
     dp->N.assign(lengths, lengths + n);
     dp->n_min = *std::min_element(lengths, lengths + n);
@@ -2102,7 +2180,7 @@ struct ss_plan {
     int n_mix = 0;
     const DrawDesc* d_draw = nullptr;  // the start draws' descriptors (k_draw), in d_desc behind the mixture scratch
     int n_draw = 0;
-    const StageSlot* d_stage = nullptr;   // the host-pool slots' staging (k_stage), in d_desc behind the draws
+    const StageSlot* d_stage = nullptr;   // the staged slots' k_stage descriptors, in d_desc behind the draws
     int n_stage = 0;
 };
 
@@ -2184,36 +2262,37 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
 }
 
 // ----------------------------------------------------------------------------- k_stage
-// Host pools: at the head of every run (after k_draw, so that drawn starts are final), each pooled slot of a host pool
-// gets its picked candidate's read set (stage_set) copied from pinned, mapped host memory into its staging area, and its
-// view of the candidate (StageView), which the head of k_blocks takes.  One gridDim.y row of kStageCtas CTAs per slot:
-// every CTA works out the read set, then the CTAs copy it in 16-byte loads, kStageUnroll of them in flight per thread.
+// Staged slots: at the head of every run (after k_draw, so that drawn starts are final), each pooled slot of a host pool
+// and each slot with a dry pick from a host dry pool gets its picked candidate's read set (stage_set) copied from pinned,
+// mapped host memory into its staging area, and its view of the candidate (StageView), which the head of k_blocks takes.
+// A slot of a host pool stages the RIR rows and the dry samples; a slot of a device pool stages only the dry samples of
+// its dry pick.  One gridDim.y row of kStageCtas CTAs per slot: every CTA works out the read set (stage_head), then the
+// CTAs copy it in 16-byte loads, kStageUnroll of them in flight per thread.
 constexpr int kStageCtas = 16, kStageUnroll = 4;
 struct StageSlot {
-    const PoolEntry* pool;            // the pool's table: x and spec are mapped host addresses, bounds and cut device ones
+    const PoolEntry* pool;            // the pool's table (a host pool's: x and spec are mapped host addresses)
     const int* pick;
     const int* ws_dev;                // the slot's moving start, or null: ws
     const int* parts;                 // the candidates' K when they differ (pool_parts), else null: K
     const float* gains;               // the pool's gains, or null
+    const float* const* dry;          // a host dry pool's signal table (mapped host addresses), or null: no dry pick ...
+    const int* dry_pick;              // ... the slot's dry pick ...
     StageView* view;                  // staging area: the view, ...
     float2* spec;                     // ... sets * rows_cap rows (used: sets * rows, back to back) ...
     float* x;                         // ... and the dry samples, whole float4s from xa & ~3 on
-    int n, C, K, ws, len, sets;
+    int n, C, K, ws, len;
+    int sets;                         // spectra sets staged: 1, 2 with a direct target, 0 for a slot of a device pool
+    int n_dry;                        // ... and the dry pool's signal count
 };
 __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots) {
     const StageSlot& g = slots[blockIdx.y];
     __shared__ StageView s_v;
+    __shared__ const float* s_src;                      // the signal the dry samples come from
     __shared__ int s_x[2];                              // dry samples copied: whole float4s [s_x[0], s_x[1])
     if (threadIdx.x == 0) {
-        bool bad;
-        const int i = clamp_pick(*g.pick, g.n, bad);
-        if (bad && blockIdx.x == 0) atomicOr(&g_dev_err, 8u);
-        const PoolEntry e = g.pool[i];
-        const int K = g.parts ? g.parts[i] : g.K;
-        const int ws = g.ws_dev ? clamp_win_start(*g.ws_dev, e.N, g.len, bad) : g.ws;   // (bit 2 is k_blocks')
-        const StageSet r = stage_set(e.N, e.P, g.C, K, e.bounds, ws, g.len);
-        s_v.e = e; s_v.K = K; s_v.row0 = r.row0; s_v.rows = r.rows; s_v.gain = g.gains ? g.gains[i] : 1.0f;
-        s_x[0] = r.xa & ~3; s_x[1] = (r.xb + 3) & ~3;  // (the pool's arena pads every x to whole float4s)
+        const unsigned err = stage_head(g.pool, g.n, *g.pick, g.parts, g.K, g.gains, g.ws_dev, g.ws, g.len, g.C,
+                                        g.sets != 0, g.dry, g.dry ? *g.dry_pick : 0, g.n_dry, s_v, s_src, s_x[0], s_x[1]);
+        if (err && blockIdx.x == 0) atomicOr(&g_dev_err, err);
     }
     __syncthreads();
     const PoolEntry& e = s_v.e;
@@ -2221,7 +2300,7 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
     const size_t per_set = (size_t)s_v.rows * (kSpec / 2);          // float4s per set
     const size_t rows_h = (size_t)e.P * g.C * s_v.K;                 // rows per set of the bank
     const size_t total = nx4 + (size_t)g.sets * per_set;
-    const float4* const xs = reinterpret_cast<const float4*>(e.x + s_x[0]);
+    const float4* const xs = reinterpret_cast<const float4*>(s_src + s_x[0]);
     float4* const xd = reinterpret_cast<float4*>(g.x);
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (size_t q0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x; q0 < total; q0 += stride * kStageUnroll) {
@@ -2243,7 +2322,7 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         StageView w = s_v;
         w.e.x = g.x - s_x[0];                           // biased: sample n at x[n] (Source::x)
-        w.e.spec = g.spec;
+        if (g.sets) w.e.spec = g.spec;                  // (a device pool's slot keeps its bank's spectra)
         *g.view = w;
     }
 }
@@ -2309,9 +2388,11 @@ static std::pair<int, int> stage_cap(ss_pool* pl, int win_len) {
     pl->stage_caps.push_back({win_len, {rows, nx}});
     return {rows, nx};
 }
+// (spectra sets it stages: direct_sets for a slot of a host pool, 0 for a slot of a device pool, which stages dry samples only)
+static int stage_sets(const ss_source& it) { return it.pool->host_res ? direct_sets(it) : 0; }
 static size_t stage_bytes(const ss_source& it) {
     const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(it.pool), it.win_len);
-    return align_up(sizeof(StageView), 256) + align_up((size_t)direct_sets(it) * cap.first * kSpec * sizeof(float2), 256) +
+    return align_up(sizeof(StageView), 256) + align_up((size_t)stage_sets(it) * cap.first * kSpec * sizeof(float2), 256) +
            align_up(sizeof(float) * (size_t)cap.second, 256);
 }
 
@@ -2326,6 +2407,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
     std::vector<const ss_dry_pick*> dry_arranged(arranged.size());
     for (size_t i = 0; i < arranged.size(); ++i) dry_arranged[i] = dry[order[i]];
+    std::vector<const ss_dry_pick*> dry_describe(dry_arranged);   // the dry picks k_blocks makes (pick_pooled)
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     const size_t n_chunks = cuts.size() - 1;
     std::vector<size_t> off(n_chunks + 1, 0);
@@ -2344,9 +2426,13 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
     const size_t draw_off = align_up(scr_off + scr_bytes * n_mixes, 256);
     const size_t desc_bytes = draw_off + sizeof(DrawDesc) * n_draws;
-    // behind the draws: the host-pool slots' k_stage descriptors, then their staging areas
-    std::vector<int> staged;                            // arranged items that are slots of host pools
-    for (int i = 0; i < (int)arranged.size(); ++i) if (items[i].pool && items[i].pool->host_res) staged.push_back(i);
+    // behind the draws: the staged slots' k_stage descriptors, then their staging areas
+    std::vector<int> staged;                            // arranged items that are slots of host pools or host dry picks
+    for (int i = 0; i < (int)arranged.size(); ++i)
+        if (items[i].pool && (items[i].pool->host_res || (dry_arranged[i] && dry_arranged[i]->pool->host))) {
+            staged.push_back(i);
+            dry_describe[i] = nullptr;                  // k_stage stages the dry pick: the counts hold none (take_view)
+        }
     if (staged.size() > 65535) return SS_ERR_UNSUPPORTED;   // one gridDim.y row of k_stage per slot
     const size_t stage_off = align_up(desc_bytes, 256), area_off = align_up(stage_off + sizeof(StageSlot) * staged.size(), 256);
     size_t total = area_off;
@@ -2363,11 +2449,12 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         StageSlot& g = stage[k];
         memset(&g, 0, sizeof(g));
         g.pool = pl->table; g.pick = it.pick_dev; g.ws_dev = it.win_start_dev; g.parts = pl->parts; g.gains = pl->gains;
-        g.n = pl->n; g.C = pl->C; g.K = pl->K; g.ws = it.win_start; g.len = it.win_len; g.sets = direct_sets(it);
+        g.n = pl->n; g.C = pl->C; g.K = pl->K; g.ws = it.win_start; g.len = it.win_len; g.sets = stage_sets(it);
+        if (const ss_dry_pick* d = dry_arranged[staged[k]]) { g.dry = d->pool->ptrs; g.dry_pick = d->pick_dev; g.n_dry = d->pool->n; }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
         char* a = p->d_desc + at;
         g.view = (StageView*)a; a += align_up(sizeof(StageView), 256);
-        g.spec = (float2*)a; a += align_up((size_t)g.sets * cap.first * kSpec * sizeof(float2), 256);
+        g.spec = g.sets ? (float2*)a : nullptr; a += align_up((size_t)g.sets * cap.first * kSpec * sizeof(float2), 256);
         g.x = (float*)a;
         at += stage_bytes(it);
         views[staged[k]] = g.view;
@@ -2376,7 +2463,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     for (size_t k = 0; k < n_chunks; ++k)
         chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
                        p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data(),
-                       dry_arranged.data());
+                       dry_describe.data());
     for (int k = 0; k < n_mixes; ++k)
         ((MixItem*)(host.data() + mix_off))[k] =
             mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
@@ -2516,8 +2603,9 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
         add_range(r, picks[k].pick_dev, 4, false);
         if (std::find(dpools.begin(), dpools.end(), picks[k].pool) == dpools.end()) dpools.push_back(picks[k].pool);
     }
-    for (const ss_dry_pool* dp : dpools)
-        for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
+    for (const ss_dry_pool* dp : dpools)                    // (a host dry pool owns its arena: nothing a plan writes)
+        if (!dp->host)
+            for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
 
@@ -2531,9 +2619,10 @@ static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_ite
         if (d.slot < 0 || d.slot >= n_items || dry[d.slot]) return SS_ERR_INVALID;      // one dry pick per slot
         if (!d.pool || d.pool->c != c || !d.pick_dev || ((uintptr_t)d.pick_dev & 3)) return SS_ERR_INVALID;
         const ss_pool* pl = items[d.slot].pool;
-        // a pooled slot of a device pool without gains (k_stage stages the candidate's own x; the gains were measured
-        // with it), whose every candidate's N the dry pool's shortest signal covers
-        if (!pl || pl->host_res || pl->gains) return SS_ERR_INVALID;
+        // a pooled slot without gains (they were measured with the candidates' own x) whose every candidate's N the dry
+        // pool's shortest signal covers; a slot of a host pool only from a host dry pool, whose arena pads every signal
+        // to the whole float4s k_stage copies
+        if (!pl || (pl->host_res && !d.pool->host) || pl->gains) return SS_ERR_INVALID;
         for (const PoolEntry& e : pl->host) if (e.N > d.pool->n_min) return SS_ERR_INVALID;
         dry[d.slot] = &d;
     }
@@ -2605,7 +2694,7 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, cudaStream_t stream
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
     if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, stream); if (st) return st; }
-    if (p->n_stage) {                                   // host pools: after the draws, before any chunk reads a slot
+    if (p->n_stage) {                                   // staged slots: after the draws, before any chunk reads a slot
         k_stage<<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
         CK(cudaGetLastError());
         c->launches += 1;

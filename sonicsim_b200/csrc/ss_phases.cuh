@@ -396,6 +396,36 @@ SS_HD unsigned pick_pooled(Source& s) {
     }
     return err;
 }
+// The head of k_stage for one staged slot (a slot of a host pool, or a slot with a dry pick from a host dry pool): the
+// pick (clamped into [0, n), bit 3), the picked candidate's K (parts[i], or K) and start (ws_dev's, clamped - bit 2 is
+// k_blocks' - or ws), its read set (stage_set) and the view the head of k_blocks takes.  A slot of a host pool (rows)
+// stages rows [row0, row0 + rows) of each set; a slot of a device pool keeps its bank's spectra, row0 = 0 and rows =
+// P*C*K, what set_banked gives it.  A dry-picked slot (dry: the dry pool's signal table, in mapped host memory) then
+// reads its dry pick (clamped into [0, n_dry), bit 16) and stages that signal's samples instead of the candidate's x:
+// the read set stays the candidate's, inside [0, N).  src receives the signal to copy, [x0, x1) the whole float4s around
+// [xa, xb) (a host arena pads every signal to whole float4s).  Returns the error bits.
+SS_HD unsigned stage_head(const PoolEntry* pool, int n, int v, const int* parts, int K, const float* gains,
+                          const int* ws_dev, int ws, int len, int C, bool rows, const float* const* dry, int dv,
+                          int n_dry, StageView& view, const float*& src, int& x0, int& x1) {
+    bool bad;
+    unsigned err = 0;
+    const int i = clamp_pick(v, n, bad);
+    if (bad) err |= 8u;
+    const PoolEntry e = pool[i];
+    const int k = parts ? parts[i] : K;
+    if (ws_dev) ws = clamp_win_start(*ws_dev, e.N, len, bad);
+    const StageSet r = stage_set(e.N, e.P, C, k, e.bounds, ws, len);
+    view.e = e; view.K = k; view.gain = gains ? gains[i] : 1.0f;
+    view.row0 = rows ? r.row0 : 0;
+    view.rows = rows ? r.rows : e.P * C * k;
+    src = e.x;
+    if (dry) {
+        src = dry[clamp_pick(dv, n_dry, bad)];
+        if (bad) err |= 16u;
+    }
+    x0 = r.xa & ~3; x1 = (r.xb + 3) & ~3;
+    return err;
+}
 // ---- crop start draws of device plans (ss_plan_draw, include/sonicsim_b200.h): the dataloader's start loop
 // (movingdatamodule.py:81-99) over level tables Q (ss_pool_levels: Q[0] = 0, Q[n + 1] = Q[n] + e[n], float64).
 // Starts a crop of len samples can take in a candidate of N samples: the M of a draw is the least of these over its readers

@@ -318,18 +318,24 @@ class SourcePool(_Held):
 
 class DryPool(_Held):
     """A set of `n` float32 dry signals on the device (Renderer.dry_pool; ss_dry_pool of the C ABI), which dry-picked
-    slots (DryPick) take their dry signal from at every run.  `n_min` is the shortest signal's length: the longest
-    candidate N a pool of slots that pick from it may have.  With `levels` True it holds every signal's level table
-    (float64 prefix sums of its squares, 8 bytes per sample, in `nbytes`), which CropDraw reads for dry-picked speakers.
-    The pool references the signals' tensors and keeps them alive; plans hold the pool, which is freed once it is closed
-    (or collected) and no live plan uses it."""
+    slots (DryPick) take their dry signal from at every run.  `sizes` are the signals' lengths and `n_min` the shortest:
+    the longest candidate N a pool of slots that pick from it may have.  With `levels` True it holds every signal's level
+    table (float64 prefix sums of its squares, 8 bytes per sample, in `nbytes`), which CropDraw reads for dry-picked
+    speakers.  A device dry pool (`resident` "device") references the signals' tensors (`signals`) and keeps them alive;
+    a host dry pool (`resident` "host") copied them into pinned host memory, where its level tables also stay
+    (`host_nbytes`; `nbytes` then counts only its pointer arrays), and every plan run copies only the samples its slots
+    read (ss_dry_pool_host_bytes, INTEGRATION.md).  Plans hold the pool, which is freed once it is closed (or collected)
+    and no live plan uses it."""
+    resident = "device"
 
-    def __init__(self, renderer, handle, signals, levels):
+    def __init__(self, renderer, handle, signals, sizes, levels, resident="device"):
         self.renderer, self._h = renderer, handle
         self.signals = list(signals)
-        self.n, self.levels = len(self.signals), bool(levels)
-        self.n_min = min(int(x.numel()) for x in self.signals)
+        self.sizes = [int(v) for v in sizes]
+        self.n, self.levels, self.resident = len(self.sizes), bool(levels), resident
+        self.n_min = min(self.sizes)
         self.nbytes = int(renderer.lib.ss_dry_pool_bytes(handle))
+        self.host_nbytes = int(renderer.lib.ss_dry_pool_host_bytes(handle))
 
     def level_table(self, i):
         """A float64 CUDA copy of signal i's level table (N + 1 values: Q[0] = 0, Q[n + 1] = Q[n] + x[n]^2), or None
@@ -338,7 +344,10 @@ class DryPool(_Held):
         if self.closed or not self.levels or not 0 <= i < self.n:
             return None
         ptr = self.renderer.lib.ss_dry_pool_level_table(self._h, int(i))
-        n = int(self.signals[i].numel()) + 1
+        n = self.sizes[i] + 1
+        if self.resident == "host":                        # pinned, mapped host memory: copied from the host side
+            host = np.ctypeslib.as_array((ctypes.c_double * n).from_address(ptr))
+            return torch.from_numpy(host.copy()).to("cuda:%d" % self.renderer.device)
 
         class _View:
             __cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (ptr, False), "version": 3}
@@ -370,15 +379,16 @@ def _rirs(s, conv=None):
     return None, r, P, C, L, mode
 
 
-def _pool_host_dry(dry, own, device, keep):
-    """(pointer, N) of the dry signal of a host pool's candidate, which the pool copies: a CUDA float32 tensor of the
-    renderer's device, or a 1-D NumPy array / CPU tensor (converted to contiguous float32, kept alive in `keep`)."""
+def _pool_host_dry(dry, api, own, device, keep):
+    """(pointer, N) of a dry signal that a host pool (a candidate's) or a host dry pool copies (`api` names the call):
+    a CUDA float32 tensor of the renderer's device, or a 1-D NumPy array / CPU tensor (converted to contiguous float32,
+    kept alive in `keep`)."""
     if _is_tensor(dry) and dry.is_cuda:
         import torch
-        return _tensor(dry, "source_pool", own, "dry", torch.float32, device), dry.numel()
+        return _tensor(dry, api, own, "dry", torch.float32, device), dry.numel()
     a = np.ascontiguousarray(dry.numpy() if _is_tensor(dry) else dry, dtype=np.float32)
     if a.ndim != 1 or a.size < 1:
-        raise ValueError("source_pool: dry of %s must be 1-D and not empty, got shape %s" % (own, a.shape))
+        raise ValueError("%s: dry of %s must be 1-D and not empty, got shape %s" % (api, own, a.shape))
     keep.append(a)
     return a.ctypes.data, a.size
 
@@ -589,7 +599,7 @@ class Renderer:
             own = "candidate %d" % i
             bounds_host = s.bounds_host if mode == _lib.SS_MOVING_BOUNDS else None
             if host:                                       # copied into the pool: NumPy, CPU or CUDA tensors
-                x, N = _pool_host_dry(s.dry, own, self.device, keep)
+                x, N = _pool_host_dry(s.dry, "source_pool", own, self.device, keep)
                 if mode == _lib.SS_MOVING_BOUNDS and bounds_host is None and s.bounds is not None and \
                         not (_is_tensor(s.bounds) and s.bounds.is_cuda):
                     bounds_host = s.bounds.numpy() if _is_tensor(s.bounds) else s.bounds
@@ -624,31 +634,40 @@ class Renderer:
                           post is not None)
 
     # ------------------------------------------------------------------ dry pools
-    def dry_pool(self, signals: T.Sequence[T.Any], levels: bool = False) -> DryPool:
+    def dry_pool(self, signals: T.Sequence[T.Any], levels: bool = False, host: bool = False) -> DryPool:
         """A DryPool over `signals`: 1 to 2^24 contiguous 1-D CUDA float32 tensors of this renderer's device, referenced
         (not copied) and kept alive by the pool, for dry-picked pooled slots (DryPick) of device plans.  `levels` also
         builds every signal's level table, which start draws (CropDraw) test dry-picked speakers with; the call then
-        returns when the tables are complete, and they describe the signals as they are now."""
+        returns when the tables are complete, and they describe the signals as they are now.
+
+        With `host` True the pool is host-resident (`resident` "host"): the signals, which may also be 1-D NumPy arrays
+        or CPU tensors, are copied into pinned host memory at once and not held, the level tables stay there too, and
+        every plan run copies only the samples its dry-picked slots' crops read to the device.  Slots of host source
+        pools take dry picks only from a host dry pool."""
         import torch
         n = len(signals)
         if not 1 <= n <= 1 << 24:
             raise ValueError("dry_pool: a dry pool holds 1 to 2^24 signals, got %d" % n)
         ptrs = (ctypes.c_void_p * n)()
         lengths = np.empty(n, np.int32)
+        keep = []
         for i, x in enumerate(signals):
             own = "signal %d" % i
-            ptrs[i] = _tensor(x, "dry_pool", own, "dry", torch.float32, self.device)
-            if x.dim() != 1 or x.numel() < 1:
+            if host:                                       # copied into the pool: NumPy, CPU or CUDA tensors
+                ptrs[i], N = _pool_host_dry(x, "dry_pool", own, self.device, keep)
+            else:
+                ptrs[i], N = _tensor(x, "dry_pool", own, "dry", torch.float32, self.device), x.numel()
+            if _is_tensor(x) and x.is_cuda and (x.dim() != 1 or N < 1):
                 raise ValueError("dry_pool: %s must be 1-D and not empty, got shape %s" % (own, tuple(x.shape)))
-            if x.numel() > 0x7fffffff - 16384:
-                raise ValueError("dry_pool: %s has %d samples, at most %d" % (own, x.numel(), 0x7fffffff - 16384))
-            lengths[i] = x.numel()
-        if levels:                             # the tables are built on the library's own stream: finish the writes
+            if N > 0x7fffffff - 16384:
+                raise ValueError("dry_pool: %s has %d samples, at most %d" % (own, N, 0x7fffffff - 16384))
+            lengths[i] = N
+        if levels or host:                     # tables and copies are made on the library's own streams: finish the writes
             torch.cuda.current_stream(self.device).synchronize()
+        flags = (_lib.SS_DRY_LEVELS if levels else 0) | (_lib.SS_DRY_HOST if host else 0)
         h = ctypes.c_void_p()
-        _lib.check(self.lib.ss_dry_pool_create(self.ctx, ptrs, lengths.ctypes.data, n,
-                                               _lib.SS_DRY_LEVELS if levels else 0, ctypes.byref(h)))
-        return DryPool(self, h, signals, levels)
+        _lib.check(self.lib.ss_dry_pool_create(self.ctx, ptrs, lengths.ctypes.data, n, flags, ctypes.byref(h)))
+        return DryPool(self, h, [] if host else signals, lengths, levels, "host" if host else "device")
 
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
@@ -787,7 +806,7 @@ class Renderer:
             _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
             pl = s.pool
             if isinstance(pl, SourcePool):
-                if pl.resident == "host":
+                if pl.resident == "host" and d.pool.resident == "device":
                     raise ValueError("plan_device: pooled source %d has a dry pick over a host pool, whose runs stage "
                                      "each candidate's own dry signal" % i)
                 if pl.gains:
