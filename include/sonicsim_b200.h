@@ -37,6 +37,7 @@ typedef struct ss_ctx ss_ctx;
 typedef struct ss_bank ss_bank;
 typedef struct ss_pool ss_pool;
 typedef struct ss_dry_pool ss_dry_pool;
+typedef struct ss_pair_gains ss_pair_gains;
 
 typedef enum {
     SS_OK = 0,
@@ -466,7 +467,8 @@ int ss_plan_create_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss
  *     errors are those of the same plan over a device dry pool of the same signals.
  * Refused by ss_plan_create_dry, before anything is allocated and with no plan created (SS_ERR_INVALID): n_picks < 0, a
  * NULL picks with n_picks > 0; a slot outside [0, n_items), or named by two dry picks; a slot that is not pooled, or
- * whose pool has loudness gains (measured with the candidates' own dry signals), or is a host pool while the dry pool is
+ * whose pool has loudness gains (measured with the candidates' own dry signals; ss_plan_create_pair accepts it with pair
+ * gains, below), or is a host pool while the dry pool is
  * a device one (k_stage copies whole float4s, which only a host dry pool's padded arena guarantees); a NULL pool or one
  * of another context; a dry pool with a signal shorter than the slot pool's longest candidate N; a NULL or unaligned
  * pick_dev; a draw speaker with a dry pick whose dry pool has no level tables; a range a plan writes that meets a dry
@@ -585,6 +587,45 @@ int ss_render_host_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss
  * ss_post_lufs refuse; a pool that already has gains or level tables, or that a plan has been created over
  * (SS_ERR_INVALID). */
 int ss_pool_loudness(ss_pool* pool, const ss_post_lufs* post);   /* n entries, one per candidate */
+
+/* ---- pair gains: a dry-picked slot (ss_dry_pick) renders a pair (dry signal d, candidate i) drawn at run time, whose
+ * whole-stem loudness depends only on the pair.  A pair-gain table measures it once for every pair of a pool of n
+ * candidates and a dry pool of n_dry signals, so that each dry-picked slot stores its crops at SonicSet's loudness
+ * (get_lufs_norm_audio, as for ss_pool_loudness) with no loudness kernel and no extra launch in any plan run.
+ *   - post: n entries, one per candidate of `pool`: its gating plan (brk / blk_lo / blk_hi, n_e, n_blocks), rate and
+ *     block_size, as for ss_pool_loudness; target_lufs and result are ignored; brk == NULL leaves every pair of that
+ *     candidate unmeasured.
+ *   - targets: n_dry * n doubles, pair (d, i) at [d * n + i]; NaN leaves the pair unmeasured (gain 1).
+ *   - results: NULL, or 2 * n_dry * n doubles that receive (LUFS, linear gain) of pair (d, i) at [2 * (d * n + i)], NaN
+ *     for an unmeasured pair.
+ *   - Each measured pair is candidate i rendered whole, with x = the first N samples of signal d (N the candidate's), as
+ *     ss_pool_loudness renders a candidate (same groups of at most 256 MB of stems, candidate-major: a host pool's bank
+ *     is copied to the device once per batch of its pairs; a host dry pool's signals are read from transient device
+ *     copies), and measured by the same launches: results receive the float64 loudness and gain that ss_render_host_ex
+ *     returns for the pair rendered on its own with that target.  Any residency of the pool and the dry pool works.
+ *   - The table keeps (float)gain per pair in device memory (4 bytes per pair, ss_pair_gains_bytes).  It waits for the
+ *     pool's banks and returns when the table is in device memory.
+ * Refused before anything is allocated: NULL arguments (other than results), a pool or dry pool of another context, a
+ * dry pool with a signal shorter than the pool's longest candidate N, entries that the checks of ss_post_lufs refuse, or
+ * a target that is neither NaN nor finite (SS_ERR_INVALID); C > 8 or n_dry * n > 2^26 (SS_ERR_UNSUPPORTED).
+ *
+ * ss_plan_create_pair is ss_plan_create_dry with pair_gains: NULL (exactly ss_plan_create_dry), or n_picks entries, entry
+ * k for picks[k], each a table or NULL (no pair gains).  A dry pick with a table stores every sample of its slot's
+ * reverberant and direct stem as y * table[d * n + i], one float32 multiply rounded once, d the clamped dry pick and i
+ * the clamped pick: k_blocks (or k_stage for a staged slot) reads the pair's gain with the picks, as it reads a pool's
+ * gain, so a plan launches as many kernels per run with pair gains as without them.  The pair's gain replaces the
+ * candidate's pool gain (ss_pool_loudness), never multiplies it, so such a dry pick is accepted on a pool with gains; a
+ * dry pick without a table is still refused there.  Start draws (ss_plan_draw) are unchanged: they test a dry-picked
+ * speaker's dry crop, so starts and `used` are the same with and without pair gains.  A table measured over another pool
+ * than the slot's or another dry pool than the pick's is SS_ERR_INVALID.  A table must outlive every plan that uses it. */
+int ss_pair_gains_create(ss_ctx* ctx, const ss_pool* pool, const ss_dry_pool* dry, const ss_post_lufs* post,
+                         const double* targets, double* results, ss_pair_gains** out);
+int64_t ss_pair_gains_bytes(const ss_pair_gains* g);       /* device bytes held: 4 per pair                            */
+void ss_pair_gains_destroy(ss_pair_gains* g);              /* waits for the device, like ss_pool_destroy               */
+int ss_plan_create_pair(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                        const ss_pair_gains* const* pair_gains /* NULL or n_picks entries, NULL = none */,
+                        int n_picks, ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

@@ -116,7 +116,8 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 // A pooled slot reads its pick before that, clamps it (bit 3) and writes the picked candidate - its RIR partition count
 // when the pool's candidates differ in K (pick_parts), and its loudness gain, counts[11] - into its Source in the
 // descriptor block (pick_slot), which is why k_prepare then reads the Source table from global memory (k_prepare<false>).
-// A dry-picked slot then reads its dry pick, clamps it (bit 4) and puts the picked dry signal in place of x (pick_dry).
+// A dry-picked slot then reads its dry pick, clamps it (bit 4) and puts the picked dry signal in place of x (pick_dry);
+// with pair gains (ss_pair_gains) it takes the pair's gain in place of the candidate's.
 __global__ void __launch_bounds__(256)
 k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -1129,7 +1130,7 @@ struct ChunkLaunch {
     int n = 0, ps = 0, grid_r = 0, n_known = -1;
     int grid_direct = 0;                  // k_rir_direct CTAs per source (8 rows each), 0: no direct target in the chunk
     bool host_tables = true, any_long = false, all_aligned = true, any_norm = false;
-    bool any_gain = false;                // a pooled slot of a pool with gains: k_render_fast<true>
+    bool any_gain = false;                // a pooled slot of a pool with gains or with pair gains: k_render_fast<true>
     const Source* ds = nullptr; const int* dps = nullptr; RItem* d_items = nullptr; int* d_total = nullptr;
     PrepParams pp;
 };
@@ -1149,7 +1150,7 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
 }
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
 // block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts),
-// [18..19] (stage_view) and [20..24] (dry_table, dry_pick_ptr, dry_size), 112 bytes
+// [18..19] (stage_view), [20..24] (dry_table, dry_pick_ptr, dry_size) and [26..27] (pair_table), 112 bytes
 static size_t counts_bytes(const Shape& sh) { return sh.pooled ? 112 : sh.win ? 64 : 16; }
 static const float kUnitGain = 1.0f;      // counts[11] of every windowed source until a pooled slot picks (stem_gain)
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
@@ -1172,7 +1173,7 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
 // chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.
 static void chunk_describe(const ss_source* items, const Shape* shapes, int first, int last, char* hbase, char* dbase,
                            char* scratch, int sm_count, ChunkLaunch* L, StageView* const* views = nullptr,
-                           const ss_dry_pick* const* dry = nullptr) {
+                           const ss_dry_pick* const* dry = nullptr, const float* const* pair = nullptr) {
     const int n = last - first;
     const bool host_tables = chunk_host_tables(items, first, last);
     const size_t off_ps = align_up(sizeof(Source) * n, 16);
@@ -1202,7 +1203,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
             s.K = it.pool->parts_host[0];
             pick_candidate(s, it.pool->host[0]);
             any_pooled = true;
-            L->any_gain = L->any_gain || it.pool->gains;
+            L->any_gain = L->any_gain || it.pool->gains || (pair && pair[first + i]);
         } else if (it.rir_bank) {
             // spectra (and cuts) from the bank: no RIR rows, no cut table, no k_rir_absmax / k_rir_direct work
             set_banked(s, it.rir_bank->spec, (it.flags & SS_DIRECT_TARGET) ? it.rir_bank->cut : nullptr, sh.win != 0);
@@ -1250,11 +1251,12 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                     memcpy(hb_counts + 14, &it.pool->gains, sizeof(it.pool->gains));
                     memcpy(hb_counts + 16, &it.pool->parts, sizeof(it.pool->parts));
                     if (views) memcpy(hb_counts + 18, &views[first + i], sizeof(StageView*));   // stage_view
-                    if (dry && dry[first + i]) {            // dry_table, dry_pick_ptr, dry_size
+                    if (dry && dry[first + i]) {            // dry_table, dry_pick_ptr, dry_size, pair_table
                         const ss_dry_pick& d = *dry[first + i];
                         memcpy(hb_counts + 20, &d.pool->ptrs, sizeof(d.pool->ptrs));
                         memcpy(hb_counts + 22, &d.pick_dev, sizeof(d.pick_dev));
                         hb_counts[24] = d.pool->n;
+                        if (pair) memcpy(hb_counts + 26, &pair[first + i], sizeof(pair[first + i]));
                     }
                 }
             } else {
@@ -1774,27 +1776,46 @@ extern "C" int ss_render_dev(ss_ctx* c, const ss_source* items, int n_items, voi
 }
 
 // ----------------------------------------------------------------------------- whole stems of a pool's candidates
-// ss_pool_loudness and ss_pool_levels read every candidate's whole reverberant stem as ss_render_dev renders it (the
-// candidate as a whole banked source, bounds_host included).  The candidates are rendered in groups of consecutive
-// candidates whose stems fit kLevelStemBytes (a larger candidate is a group of its own) into one transient buffer.
+// ss_pool_loudness, ss_pool_levels and ss_pair_gains_create read whole reverberant stems as ss_render_dev renders them
+// (the candidate as a whole banked source, bounds_host included).  A stem is a candidate rendered with one dry signal:
+// its own x, or (ss_pair_gains_create) the first N samples of a dry pool's signal.  The stems are rendered in groups of
+// consecutive stems whose outputs fit kLevelStemBytes (a larger stem is a group of its own) into one transient buffer.
 constexpr size_t kLevelStemBytes = 256ull << 20;
+
+struct Stem { int cand, sig; };           // candidate `cand` with signal `sig` of the dry pool, or sig < 0: its own x
+struct StemSet {
+    const ss_pool* pl = nullptr;
+    const ss_dry_pool* dry = nullptr;     // the pool the signals come from, or null: every stem takes its own x
+    std::vector<Stem> stems;
+    int N(size_t k) const { return pl->host[stems[k].cand].N; }
+    const float* x(size_t k) const { return stems[k].sig < 0 ? pl->host[stems[k].cand].x : dry->x[stems[k].sig]; }
+    // rendered from transient device copies: a host pool's banks and dry signals, a host dry pool's signals
+    bool copied() const { return pl->host_res || (dry && dry->host); }
+};
+// every candidate of a pool with its own x, in candidate order (stem i is candidate i)
+static StemSet own_stems(const ss_pool* pl) {
+    StemSet S;
+    S.pl = pl;
+    for (int i = 0; i < pl->n; ++i) S.stems.push_back({i, -1});
+    return S;
+}
 
 struct StemGroups {
     size_t cap = kLevelStemBytes;         // bytes of the transient buffer
-    std::vector<int> first;               // group g holds candidates [first[g], first[g + 1])
-    std::vector<size_t> at;               // candidate i's (C, N) stem at byte at[i] of the buffer
+    std::vector<int> first;               // group g holds stems [first[g], first[g + 1])
+    std::vector<size_t> at;               // stem k's (C, N) output at byte at[k] of the buffer
 };
-static StemGroups stem_groups(const ss_pool* pl) {
+static StemGroups stem_groups(const StemSet& S) {
     StemGroups G;
-    const int n = pl->n;
-    for (int i = 0; i < n; ++i) G.cap = std::max(G.cap, align_up(4 * (size_t)pl->C * pl->host[i].N, 256));
+    const int n = (int)S.stems.size();
+    for (int k = 0; k < n; ++k) G.cap = std::max(G.cap, align_up(4 * (size_t)S.pl->C * S.N(k), 256));
     G.first.assign(1, 0);
     G.at.resize(n);
     size_t used = 0;
-    for (int i = 0; i < n; ++i) {
-        const size_t b = align_up(4 * (size_t)pl->C * pl->host[i].N, 256);
-        if (used > 0 && used + b > G.cap) { G.first.push_back(i); used = 0; }
-        G.at[i] = used;
+    for (int k = 0; k < n; ++k) {
+        const size_t b = align_up(4 * (size_t)S.pl->C * S.N(k), 256);
+        if (used > 0 && used + b > G.cap) { G.first.push_back(k); used = 0; }
+        G.at[k] = used;
         used += b;
     }
     G.first.push_back(n);
@@ -1802,61 +1823,79 @@ static StemGroups stem_groups(const ss_pool* pl) {
 }
 // Render every group into `tmp` on `s` (after the pool's banks are complete), and after each group's render enqueue
 // group(first, last) on `s`, whatever reads those stems before the next group overwrites them.  Returns when `s` is idle.
-// A host pool's candidates [first, first + n) (items, rendered whole): their reverberant spectra and dry signals copied
-// into transient device memory and rendered from there, in batches of at most kLevelStemBytes of copies (or one
-// candidate's, when larger), each behind the previous batch's render on `s`.  `buf` holds `cap` = stem_copy_cap bytes.
-static size_t stem_copy_bytes(const ss_pool* pl, int i) {
-    return align_up(pl->banks[i]->set_bytes(), 256) + align_up(sizeof(float) * (size_t)pl->host[i].N, 256);
+// Copied stems [first, first + n) (items, rendered whole): a host pool's reverberant spectra - once per run of
+// consecutive stems of one candidate - and every stem's dry signal copied into transient device memory and rendered from
+// there, in batches of at most kLevelStemBytes of copies (or one stem's, when larger), each behind the previous batch's
+// render on `s`.  `buf` holds `cap` = stem_copy_cap bytes.
+static size_t stem_bank_bytes(const StemSet& S, size_t k) {
+    return S.pl->host_res ? align_up(S.pl->banks[S.stems[k].cand]->set_bytes(), 256) : 0;
 }
-static size_t stem_copy_cap(const ss_pool* pl) {
+static size_t stem_x_bytes(const StemSet& S, size_t k) { return align_up(sizeof(float) * (size_t)S.N(k), 256); }
+static bool stem_new_bank(const StemSet& S, size_t k, bool batch_start) {
+    return S.pl->host_res && (batch_start || S.stems[k - 1].cand != S.stems[k].cand);
+}
+static size_t stem_copy_cap(const StemSet& S) {
     size_t cap = 0, total = 0;
-    for (int i = 0; i < pl->n; ++i) { cap = std::max(cap, stem_copy_bytes(pl, i)); total += stem_copy_bytes(pl, i); }
+    for (size_t k = 0; k < S.stems.size(); ++k) {
+        cap = std::max(cap, stem_bank_bytes(S, k) + stem_x_bytes(S, k));
+        total += (stem_new_bank(S, k, k == 0) ? stem_bank_bytes(S, k) : 0) + stem_x_bytes(S, k);
+    }
     return std::max(cap, std::min(total, kLevelStemBytes));
 }
-static int render_host_stems(ss_pool* pl, ss_source* items, int first, int n, char* buf, size_t cap, cudaStream_t s) {
+static int render_copied_stems(const StemSet& S, ss_source* items, int first, int n, char* buf, size_t cap,
+                               cudaStream_t s) {
     std::vector<ss_bank> shells(n);
     for (int lo = 0; lo < n;) {
         size_t used = 0;
         int hi = lo;
-        while (hi < n && (hi == lo || used + stem_copy_bytes(pl, first + hi) <= cap)) {
-            const int i = first + hi;
-            const ss_bank* b = pl->banks[i];
-            ss_bank& sh = shells[hi];
-            sh = *b;                                    // the bank's shape and `ready`, spectra from the copy
-            sh.h_mem = nullptr; sh.d_mem = nullptr; sh.cut = nullptr; sh.spec = (float2*)(buf + used);
-            CK(cudaMemcpyAsync(sh.spec, b->spec, b->set_bytes(), cudaMemcpyDefault, s));   // the reverberant set
-            float* x = (float*)(buf + used + align_up(b->set_bytes(), 256));
-            CK(cudaMemcpyAsync(x, pl->host[i].x, sizeof(float) * (size_t)pl->host[i].N, cudaMemcpyDefault, s));
-            items[hi].x = x; items[hi].rir_bank = &sh;
-            used += stem_copy_bytes(pl, i);
-            ++hi;
+        const ss_bank* shell = nullptr;
+        for (; hi < n; ++hi) {
+            const size_t k = (size_t)(first + hi);
+            const bool new_bank = stem_new_bank(S, k, hi == lo);
+            if (hi > lo && used + (new_bank ? stem_bank_bytes(S, k) : 0) + stem_x_bytes(S, k) > cap) break;
+            if (new_bank) {
+                const ss_bank* b = S.pl->banks[S.stems[k].cand];
+                ss_bank& sh = shells[hi];
+                sh = *b;                                // the bank's shape and `ready`, spectra from the copy
+                sh.h_mem = nullptr; sh.d_mem = nullptr; sh.cut = nullptr; sh.spec = (float2*)(buf + used);
+                CK(cudaMemcpyAsync(sh.spec, b->spec, b->set_bytes(), cudaMemcpyDefault, s));   // the reverberant set
+                used += stem_bank_bytes(S, k);
+                shell = &sh;
+            }
+            float* x = (float*)(buf + used);
+            CK(cudaMemcpyAsync(x, S.x(k), sizeof(float) * (size_t)S.N(k), cudaMemcpyDefault, s));
+            used += stem_x_bytes(S, k);
+            items[hi].x = x;
+            if (S.pl->host_res) items[hi].rir_bank = shell;
         }
-        const int st = ss_render_dev(pl->c, items + lo, hi - lo, (void*)s);   // the next batch's copies wait on `s`
+        const int st = ss_render_dev(S.pl->c, items + lo, hi - lo, (void*)s);   // the next batch's copies wait on `s`
         if (st) return st;
         lo = hi;
     }
     return SS_OK;
 }
 template <class Group>
-static int render_stem_groups(ss_pool* pl, const StemGroups& G, char* tmp, cudaStream_t s, Group group) {
+static int render_stem_groups(const StemSet& S, const StemGroups& G, char* tmp, cudaStream_t s, Group group) {
+    const ss_pool* pl = S.pl;
     CK(cudaStreamWaitEvent(s, pl->ready, 0));           // banks may still be building
-    char* copies = nullptr;                             // a host pool's transient copies
-    const size_t copy_cap = pl->host_res ? stem_copy_cap(pl) : 0;
-    if (pl->host_res) CK(cudaMalloc((void**)&copies, copy_cap));
+    char* copies = nullptr;                             // transient copies of banks and dry signals
+    const size_t copy_cap = S.copied() ? stem_copy_cap(S) : 0;
+    if (S.copied()) CK(cudaMalloc((void**)&copies, copy_cap));
     struct Free { char* p; ~Free() { if (p) cudaFree(p); } } free_copies{copies};   // (cudaFree waits for the device)
     std::vector<ss_source> items;
     for (size_t g = 0; g + 1 < G.first.size(); ++g) {
         items.clear();
-        for (int i = G.first[g]; i < G.first[g + 1]; ++i) {
+        for (int k = G.first[g]; k < G.first[g + 1]; ++k) {
+            const int i = S.stems[k].cand;
             const PoolEntry& e = pl->host[i];
             ss_source it; memset(&it, 0, sizeof(it));
-            it.x = e.x; it.out = (float*)(tmp + G.at[i]); it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->banks[i]->L;
+            it.x = S.x(k); it.out = (float*)(tmp + G.at[k]); it.N = e.N; it.P = e.P; it.C = pl->C; it.L = pl->banks[i]->L;
             it.mode = pl->mode; it.rir_bank = pl->banks[i];
             if (pl->mode == SS_MOVING_BOUNDS) { it.bounds = e.bounds; it.bounds_host = pl->bounds_host.data() + pl->bounds_off[i]; }
             items.push_back(it);
         }
-        int st = pl->host_res ? render_host_stems(pl, items.data(), G.first[g], (int)items.size(), copies, copy_cap, s)
-                              : ss_render_dev(pl->c, items.data(), (int)items.size(), (void*)s);   // the next group waits on `s`
+        int st = S.copied() ? render_copied_stems(S, items.data(), G.first[g], (int)items.size(), copies, copy_cap, s)
+                            : ss_render_dev(pl->c, items.data(), (int)items.size(), (void*)s);   // the next group waits on `s`
         if (st == SS_OK) st = group(G.first[g], G.first[g + 1]);
         if (st) return st;
     }
@@ -1870,37 +1909,43 @@ struct BuildStream {
 };
 
 // ----------------------------------------------------------------------------- loudness gains of a pool
-// Device memory of one ss_pool_loudness call: the gating tables of the measured candidates (one copy per distinct set of
-// host arrays), their results, and one group's scratch
-static int loudness_build(ss_pool* pl, const ss_post_lufs* post, cudaStream_t s, std::vector<void*>& owned,
-                          std::vector<double>& res) {
-    const int n = pl->n;
-    const GatingTables tabs = gating_tables(post, n);
-    const StemGroups G = stem_groups(pl);
+// Device memory of one loudness build (ss_pool_loudness, ss_pair_gains_create): the gating tables of the measured
+// candidates (post[i]: candidate i's gating plan; one copy per distinct set of host arrays), every stem's result, and
+// one group's scratch.  entry(k, q) fills q with stem k's entry - its candidate's plan and its target - and returns
+// whether stem k is measured.  res receives (LUFS, gain) per stem, in stem order.
+template <class Entry>
+static int loudness_build(const StemSet& S, const ss_post_lufs* post, Entry entry, cudaStream_t s,
+                          std::vector<void*>& owned, std::vector<double>& res) {
+    const ss_pool* pl = S.pl;
+    const size_t n = S.stems.size();
+    const GatingTables tabs = gating_tables(post, pl->n);
+    const StemGroups G = stem_groups(S);
+    ss_post_lufs q;
     size_t scratch = 0;                                 // the largest group's loudness scratch
     for (size_t g = 0; g + 1 < G.first.size(); ++g) {
         size_t b = 0;
-        for (int i = G.first[g]; i < G.first[g + 1]; ++i)
-            if (post[i].brk) b += loud_scratch_bytes(post[i], pl->C);
+        for (int k = G.first[g]; k < G.first[g + 1]; ++k)
+            if (entry(k, q)) b += loud_scratch_bytes(q, pl->C);
         scratch = std::max(scratch, b);
     }
     char *d_tab = nullptr, *d_scr = nullptr, *tmp = nullptr;
     double* d_res = nullptr;
     CK(cudaMalloc((void**)&d_tab, std::max(tabs.bytes.size(), (size_t)256))); owned.push_back(d_tab);
-    CK(cudaMalloc((void**)&d_res, 2 * sizeof(double) * (size_t)n)); owned.push_back(d_res);
+    CK(cudaMalloc((void**)&d_res, 2 * sizeof(double) * n)); owned.push_back(d_res);
     CK(cudaMalloc((void**)&d_scr, std::max(scratch, (size_t)256))); owned.push_back(d_scr);
     CK(cudaMalloc((void**)&tmp, G.cap)); owned.push_back(tmp);
     if (!tabs.bytes.empty()) CK(cudaMemcpy(d_tab, tabs.bytes.data(), tabs.bytes.size(), cudaMemcpyHostToDevice));
     std::vector<ss_loud_item> li;
-    const int st = render_stem_groups(pl, G, tmp, s, [&](int first, int last) -> int {
-        // every measured candidate of the group: the launches of ss_loudness_dev on its (C, N) stem, measure only
+    const int st = render_stem_groups(S, G, tmp, s, [&](int first, int last) -> int {
+        // every measured stem of the group: the launches of ss_loudness_dev on its (C, N) output, measure only
         li.clear();
         char* scr = d_scr;
-        for (int i = first; i < last; ++i) {
-            if (!post[i].brk) continue;
-            li.push_back(loud_item(post[i], d_tab + tabs.at[i], (const float*)(tmp + G.at[i]), nullptr, pl->host[i].N,
-                                   pl->C, (double*)scr, d_res + 2 * (size_t)i));
-            scr += loud_scratch_bytes(post[i], pl->C);
+        for (int k = first; k < last; ++k) {
+            if (!entry(k, q)) continue;
+            const int i = S.stems[k].cand;
+            li.push_back(loud_item(q, d_tab + tabs.at[i], (const float*)(tmp + G.at[k]), nullptr, pl->host[i].N, pl->C,
+                                   (double*)scr, d_res + 2 * (size_t)k));
+            scr += loud_scratch_bytes(q, pl->C);
         }
         for (size_t k = 0; k < li.size(); k += 65535) {   // ss_loudness_dev's item limit
             const int st2 = ss_loudness_dev(pl->c, li.data() + k, (int)std::min(li.size() - k, (size_t)65535), (void*)s);
@@ -1909,8 +1954,8 @@ static int loudness_build(ss_pool* pl, const ss_post_lufs* post, cudaStream_t s,
         return SS_OK;
     });
     if (st) return st;
-    res.resize(2 * (size_t)n);
-    CK(cudaMemcpy(res.data(), d_res, 2 * sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
+    res.resize(2 * n);
+    CK(cudaMemcpy(res.data(), d_res, 2 * sizeof(double) * n, cudaMemcpyDeviceToHost));
     return SS_OK;
 }
 
@@ -1925,7 +1970,8 @@ extern "C" int ss_pool_loudness(ss_pool* pl, const ss_post_lufs* post) {
     {
         BuildStream bs;
         CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
-        st = loudness_build(pl, post, bs.s, owned, res);
+        st = loudness_build(own_stems(pl), post, [&](int i, ss_post_lufs& q) { q = post[i]; return post[i].brk != nullptr; },
+                            bs.s, owned, res);
     }
     for (void* q : owned) cudaFree(q);
     if (st != SS_OK) return st;                         // no gains: the pool is as it was
@@ -1965,7 +2011,8 @@ static int levels_build(ss_pool* pl, bool mono, cudaStream_t s, std::vector<void
     std::vector<const double*> ptr(n);
     for (int i = 0; i < n; ++i) ptr[i] = pl->levels + pl->level_off[i];
     CK(cudaMemcpy(pl->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
-    const StemGroups G = stem_groups(pl);
+    const StemSet S = own_stems(pl);
+    const StemGroups G = stem_groups(S);
     char* tmp = nullptr;
     LevelItem* d_items = nullptr;
     double* d_res = nullptr;                            // the (LUFS, gain) pairs k_loud_scale reads its gain from
@@ -1981,7 +2028,7 @@ static int levels_build(ss_pool* pl, bool mono, cudaStream_t s, std::vector<void
         CK(cudaMemcpy(d_res, r.data(), sizeof(double) * r.size(), cudaMemcpyHostToDevice));
     }
     std::vector<ScaleItem> sc;
-    return render_stem_groups(pl, G, tmp, s, [&](int first, int last) -> int {
+    return render_stem_groups(S, G, tmp, s, [&](int first, int last) -> int {
         if (d_res) {
             sc.clear();
             for (int i = first; i < last; ++i) sc.push_back(ScaleItem{(float*)li[i].y, d_res + 2 * (size_t)i, pl->host[i].N, pl->C});
@@ -2154,6 +2201,77 @@ extern "C" int ss_dry_pool_create(ss_ctx* c, const float* const* x, const int32_
     return SS_OK;
 }
 
+// ----------------------------------------------------------------------------- pair gains
+// The (float)gain of every (dry signal d, candidate i) pair of a pool and a dry pool, at [d * n + i] in device memory,
+// which dry-picked slots take in place of their candidate's gain (pair_table).  The pools are kept only to check that a
+// plan's slot names the pool and the dry pool the table was measured over.
+constexpr int64_t kMaxPairs = 1 << 26;
+struct ss_pair_gains {
+    ss_ctx* c = nullptr;
+    const ss_pool* pool = nullptr;
+    const ss_dry_pool* dry = nullptr;
+    float* gains = nullptr;
+    int64_t pairs = 0;
+};
+extern "C" void ss_pair_gains_destroy(ss_pair_gains* g) {
+    if (!g) return;
+    cudaSetDevice(g->c->device);
+    cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
+    if (g->gains) cudaFree(g->gains);
+    delete g;
+}
+extern "C" int64_t ss_pair_gains_bytes(const ss_pair_gains* g) { return g ? (int64_t)sizeof(float) * g->pairs : 0; }
+extern "C" int ss_pair_gains_create(ss_ctx* c, const ss_pool* pl, const ss_dry_pool* dp, const ss_post_lufs* post,
+                                    const double* targets, double* results, ss_pair_gains** out) {
+    if (!c || !pl || !dp || !post || !targets || !out || pl->c != c || dp->c != c) return SS_ERR_INVALID;
+    if (pl->C > 8) return SS_ERR_UNSUPPORTED;           // as ss_loudness_dev
+    const int n = pl->n;
+    const int64_t pairs = (int64_t)dp->n * n;
+    if (pairs > kMaxPairs) return SS_ERR_UNSUPPORTED;
+    for (const PoolEntry& e : pl->host) if (e.N > dp->n_min) return SS_ERR_INVALID;   // (ss_plan_create_dry's rule)
+    if (check_post_lufs(post, n)) return SS_ERR_INVALID;
+    for (int64_t k = 0; k < pairs; ++k) if (!isnan(targets[k]) && !isfinite(targets[k])) return SS_ERR_INVALID;
+    CK(cudaSetDevice(c->device));
+    // the measured pairs, candidate-major: a host pool's bank is copied once per batch of its pairs
+    StemSet S;
+    S.pl = pl; S.dry = dp;
+    for (int i = 0; i < n; ++i)
+        if (post[i].brk)
+            for (int d = 0; d < dp->n; ++d) if (!isnan(targets[(int64_t)d * n + i])) S.stems.push_back({i, d});
+    std::vector<void*> owned;
+    std::vector<double> res;
+    int st = SS_OK;
+    if (!S.stems.empty()) {
+        BuildStream bs;
+        CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
+        st = loudness_build(S, post, [&](int k, ss_post_lufs& q) {
+            q = post[S.stems[k].cand];
+            q.target_lufs = targets[(int64_t)S.stems[k].sig * n + S.stems[k].cand];
+            return true;
+        }, bs.s, owned, res);
+    }
+    for (void* q : owned) cudaFree(q);
+    if (st != SS_OK) return st;
+    std::vector<float> g((size_t)pairs, 1.0f);
+    for (size_t k = 0; k < S.stems.size(); ++k)
+        g[(size_t)S.stems[k].sig * n + S.stems[k].cand] = (float)res[2 * k + 1];   // what k_loud_scale multiplies by
+    ss_pair_gains* pg = new (std::nothrow) ss_pair_gains();
+    if (!pg) return SS_ERR_NOMEM;
+    pg->c = c; pg->pool = pl; pg->dry = dp; pg->pairs = pairs;
+    cudaError_t e = cudaMalloc((void**)&pg->gains, sizeof(float) * (size_t)pairs);
+    if (e == cudaSuccess) e = cudaMemcpy(pg->gains, g.data(), sizeof(float) * (size_t)pairs, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) { ss_pair_gains_destroy(pg); g_last_cuda = (int)e; return SS_ERR_CUDA; }
+    if (results) {
+        std::fill(results, results + 2 * pairs, (double)NAN);
+        for (size_t k = 0; k < S.stems.size(); ++k) {
+            double* const r = results + 2 * ((int64_t)S.stems[k].sig * n + S.stems[k].cand);
+            r[0] = res[2 * k]; r[1] = res[2 * k + 1];
+        }
+    }
+    *out = pg;
+    return SS_OK;
+}
+
 // ----------------------------------------------------------------------------- plans (device path)
 // A batch of device-resident sources bound once: validation, chunking, block tables and descriptor blocks are done at
 // creation and stay resident in device memory together with the plan's own scratch, so a run is kernel launches only -
@@ -2277,6 +2395,7 @@ struct StageSlot {
     const float* gains;               // the pool's gains, or null
     const float* const* dry;          // a host dry pool's signal table (mapped host addresses), or null: no dry pick ...
     const int* dry_pick;              // ... the slot's dry pick ...
+    const float* pair;                // ... and its pair gains, or null
     StageView* view;                  // staging area: the view, ...
     float2* spec;                     // ... sets * rows_cap rows (used: sets * rows, back to back) ...
     float* x;                         // ... and the dry samples, whole float4s from xa & ~3 on
@@ -2291,7 +2410,8 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
     __shared__ int s_x[2];                              // dry samples copied: whole float4s [s_x[0], s_x[1])
     if (threadIdx.x == 0) {
         const unsigned err = stage_head(g.pool, g.n, *g.pick, g.parts, g.K, g.gains, g.ws_dev, g.ws, g.len, g.C,
-                                        g.sets != 0, g.dry, g.dry ? *g.dry_pick : 0, g.n_dry, s_v, s_src, s_x[0], s_x[1]);
+                                        g.sets != 0, g.dry, g.dry ? *g.dry_pick : 0, g.n_dry, s_v, s_src, s_x[0], s_x[1],
+                                        g.pair);
         if (err && blockIdx.x == 0) atomicOr(&g_dev_err, err);
     }
     __syncthreads();
@@ -2396,17 +2516,18 @@ static size_t stage_bytes(const ss_source& it) {
            align_up(sizeof(float) * (size_t)cap.second, 256);
 }
 
-// (dry[i]: caller item i's dry pick, or null)
+// (dry[i]: caller item i's dry pick, or null; pair[i]: its pair gains' device table, or null)
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
                       const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws,
-                      const ss_dry_pick* const* dry) {
+                      const ss_dry_pick* const* dry, const float* const* pair) {
     ss_ctx* c = p->c;
     std::vector<int> cuts, order;
     std::vector<ss_source> arranged;
     std::vector<Shape> arranged_shapes;
     arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
     std::vector<const ss_dry_pick*> dry_arranged(arranged.size());
-    for (size_t i = 0; i < arranged.size(); ++i) dry_arranged[i] = dry[order[i]];
+    std::vector<const float*> pair_arranged(arranged.size());
+    for (size_t i = 0; i < arranged.size(); ++i) { dry_arranged[i] = dry[order[i]]; pair_arranged[i] = pair[order[i]]; }
     std::vector<const ss_dry_pick*> dry_describe(dry_arranged);   // the dry picks k_blocks makes (pick_pooled)
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     const size_t n_chunks = cuts.size() - 1;
@@ -2450,7 +2571,9 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         memset(&g, 0, sizeof(g));
         g.pool = pl->table; g.pick = it.pick_dev; g.ws_dev = it.win_start_dev; g.parts = pl->parts; g.gains = pl->gains;
         g.n = pl->n; g.C = pl->C; g.K = pl->K; g.ws = it.win_start; g.len = it.win_len; g.sets = stage_sets(it);
-        if (const ss_dry_pick* d = dry_arranged[staged[k]]) { g.dry = d->pool->ptrs; g.dry_pick = d->pick_dev; g.n_dry = d->pool->n; }
+        if (const ss_dry_pick* d = dry_arranged[staged[k]]) {
+            g.dry = d->pool->ptrs; g.dry_pick = d->pick_dev; g.n_dry = d->pool->n; g.pair = pair_arranged[staged[k]];
+        }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
         char* a = p->d_desc + at;
         g.view = (StageView*)a; a += align_up(sizeof(StageView), 256);
@@ -2463,7 +2586,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     for (size_t k = 0; k < n_chunks; ++k)
         chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
                        p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data(),
-                       dry_describe.data());
+                       dry_describe.data(), pair_arranged.data());
     for (int k = 0; k < n_mixes; ++k)
         ((MixItem*)(host.data() + mix_off))[k] =
             mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
@@ -2610,34 +2733,41 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
 }
 
 // A plan's dry picks (include/sonicsim_b200.h, ss_dry_pick), all but the byte ranges (validate_mixes): dry[i] receives
-// item i's pick, or null
+// item i's pick, or null, and pair[i] the device table of its pair gains (pair_gains[k] of pick k), or null
 static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_items, const ss_dry_pick* picks,
-                              int n_picks, std::vector<const ss_dry_pick*>& dry) {
+                              const ss_pair_gains* const* pair_gains, int n_picks, std::vector<const ss_dry_pick*>& dry,
+                              std::vector<const float*>& pair) {
     dry.assign(n_items, nullptr);
+    pair.assign(n_items, nullptr);
     for (int k = 0; k < n_picks; ++k) {
         const ss_dry_pick& d = picks[k];
         if (d.slot < 0 || d.slot >= n_items || dry[d.slot]) return SS_ERR_INVALID;      // one dry pick per slot
         if (!d.pool || d.pool->c != c || !d.pick_dev || ((uintptr_t)d.pick_dev & 3)) return SS_ERR_INVALID;
         const ss_pool* pl = items[d.slot].pool;
-        // a pooled slot without gains (they were measured with the candidates' own x) whose every candidate's N the dry
-        // pool's shortest signal covers; a slot of a host pool only from a host dry pool, whose arena pads every signal
-        // to the whole float4s k_stage copies
-        if (!pl || (pl->host_res && !d.pool->host) || pl->gains) return SS_ERR_INVALID;
+        const ss_pair_gains* const t = pair_gains ? pair_gains[k] : nullptr;
+        // a pooled slot whose every candidate's N the dry pool's shortest signal covers, on a pool with gains only with
+        // pair gains (the pool's were measured with the candidates' own x) of this pool and dry pool; a slot of a host
+        // pool only from a host dry pool, whose arena pads every signal to the whole float4s k_stage copies
+        if (!pl || (pl->host_res && !d.pool->host) || (pl->gains && !t)) return SS_ERR_INVALID;
+        if (t && (t->pool != pl || t->dry != d.pool)) return SS_ERR_INVALID;
         for (const PoolEntry& e : pl->host) if (e.N > d.pool->n_min) return SS_ERR_INVALID;
         dry[d.slot] = &d;
+        pair[d.slot] = t ? t->gains : nullptr;
     }
     return SS_OK;
 }
 
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
-                       const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks, ss_plan** out) {
+                       const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                       const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
     std::vector<const ss_dry_pick*> dry;
+    std::vector<const float*> pair;
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
-    { int st = validate_dry_picks(c, items, n_items, picks, n_picks, dry); if (st) return st; }
+    { int st = validate_dry_picks(c, items, n_items, picks, pair_gains, n_picks, dry, pair); if (st) return st; }
     { int st = validate_draws(items, n_items, draws, n_draws, dry.data()); if (st) return st; }
     { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
@@ -2649,7 +2779,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data());
+    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data(), pair.data());
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -2657,28 +2787,34 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 }
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
-    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                   const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
+    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
+        (n_picks > 0 && !picks))
+        return SS_ERR_INVALID;
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
-    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
-        (n_picks > 0 && !picks))
-        return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks, out);
+    return ss_plan_create_pair(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start

@@ -373,16 +373,27 @@ SS_HD void take_view(Source& s, const StageView& v) {
 // ---- dry pools (ss_dry_pool, include/sonicsim_b200.h).  A dry-picked slot of a device pool renders its picked
 // candidate with the dry signal its own pick names in a dry pool.  Its counts block is 112 bytes, as every pooled slot's:
 // [20..21] the device pointer of the dry pool's n signal pointers, or null (no dry pick), [22..23] the device pointer of
-// the dry pick, [24] the dry pool's signal count.
+// the dry pick, [24] the dry pool's signal count, [26..27] the device pointer of the slot's pair gains (ss_pair_gains),
+// or null.
 SS_HD const float* const* dry_table(const Source& s) { return *reinterpret_cast<const float* const* const*>(s.counts + 20); }
 SS_HD const int* dry_pick_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 22); }
 SS_HD int dry_size(const Source& s) { return s.counts[24]; }
+SS_HD const float* pair_table(const Source& s) { return *reinterpret_cast<const float* const*>(s.counts + 26); }
 // The dry pick v read from device memory, clamped into [0, n) (bad = it was not there): the picked signal replaces the
 // candidate's own x.  Everything else - N, P, bounds, K, spectra, cuts, gain - stays the trajectory candidate's, and only
 // samples [0, N) of x are read, so a dry signal at least N long renders as that candidate with the signal's first N.
-SS_HD void pick_dry(Source& s, int v, bool& bad) { s.x = dry_table(s)[clamp_pick(v, dry_size(s), bad)]; }
+// Returns the clamped pick.
+SS_HD int pick_dry(Source& s, int v, bool& bad) {
+    const int d = clamp_pick(v, dry_size(s), bad);
+    s.x = dry_table(s)[d];
+    return d;
+}
+// Pair gains (ss_pair_gains): the (float)gain of dry signal d through candidate i of a pool of n, measured on the pair's
+// whole stem; it replaces the candidate's own gain
+SS_HD float pair_gain(const float* table, int d, int i, int n) { return table[(long long)d * n + i]; }
 // The head of k_blocks for a pooled slot of a device pool: the trajectory pick (its K, then its candidate and gain), then
-// the dry pick of a dry-picked slot.  Returns the error bits to report: 8 for a clamped pick, 16 for a clamped dry pick.
+// the dry pick of a dry-picked slot, and with pair gains the pair's gain.  Returns the error bits to report: 8 for a
+// clamped pick, 16 for a clamped dry pick.
 SS_HD unsigned pick_pooled(Source& s) {
     bool bad;
     unsigned err = 0;
@@ -391,8 +402,10 @@ SS_HD unsigned pick_pooled(Source& s) {
     pick_slot(s, v, bad);
     if (bad) err |= 8u;
     if (dry_table(s)) {
-        pick_dry(s, *dry_pick_ptr(s), bad);
+        const int d = pick_dry(s, *dry_pick_ptr(s), bad);
         if (bad) err |= 16u;
+        if (const float* const t = pair_table(s))
+            set_stem_gain(s, pair_gain(t, d, clamp_pick(v, pool_size(s), bad), pool_size(s)));
     }
     return err;
 }
@@ -402,11 +415,12 @@ SS_HD unsigned pick_pooled(Source& s) {
 // stages rows [row0, row0 + rows) of each set; a slot of a device pool keeps its bank's spectra, row0 = 0 and rows =
 // P*C*K, what set_banked gives it.  A dry-picked slot (dry: the dry pool's signal table, in mapped host memory) then
 // reads its dry pick (clamped into [0, n_dry), bit 16) and stages that signal's samples instead of the candidate's x:
-// the read set stays the candidate's, inside [0, N).  src receives the signal to copy, [x0, x1) the whole float4s around
+// the read set stays the candidate's, inside [0, N).  With pair gains (pair: a dry-picked slot's table) the view takes
+// the pair's gain in place of the candidate's.  src receives the signal to copy, [x0, x1) the whole float4s around
 // [xa, xb) (a host arena pads every signal to whole float4s).  Returns the error bits.
 SS_HD unsigned stage_head(const PoolEntry* pool, int n, int v, const int* parts, int K, const float* gains,
                           const int* ws_dev, int ws, int len, int C, bool rows, const float* const* dry, int dv,
-                          int n_dry, StageView& view, const float*& src, int& x0, int& x1) {
+                          int n_dry, StageView& view, const float*& src, int& x0, int& x1, const float* pair = nullptr) {
     bool bad;
     unsigned err = 0;
     const int i = clamp_pick(v, n, bad);
@@ -420,8 +434,10 @@ SS_HD unsigned stage_head(const PoolEntry* pool, int n, int v, const int* parts,
     view.rows = rows ? r.rows : e.P * C * k;
     src = e.x;
     if (dry) {
-        src = dry[clamp_pick(dv, n_dry, bad)];
+        const int d = clamp_pick(dv, n_dry, bad);
+        src = dry[d];
         if (bad) err |= 16u;
+        if (pair) view.gain = pair_gain(pair, d, i, n);
     }
     x0 = r.xa & ~3; x1 = (r.xb + 3) & ~3;
     return err;

@@ -95,10 +95,13 @@ class DryPick(T.NamedTuple):
     blocking unchanged - with the first N samples of that signal as its dry signal, bit for bit what render_device gives
     for the candidate with that dry signal and the same window.  A pick outside [0, n) is clamped into range
     (check_device_errors raises IndexError).  Every signal of the pool must be at least as long as the slot pool's longest
-    candidate; host pools and pools with loudness gains take no dry picks.  In a CropDraw, a dry-picked speaker is tested
-    on its dry crop, from the dry pool's level tables (dry_pool(..., levels=True))."""
+    candidate; host pools take dry picks only from a host dry pool.  In a CropDraw, a dry-picked speaker is tested on its
+    dry crop, from the dry pool's level tables (dry_pool(..., levels=True)).  `gains`, a PairGains of the slot's pool and
+    this dry pool (Renderer.pair_gains), stores the slot's stems at the picked pair's measured loudness gain, in place of
+    the candidate's own; a pool with loudness gains takes only dry picks with `gains`."""
     pool: T.Any
     pick: T.Any
+    gains: T.Any = None
 
 
 class CropDraw(T.NamedTuple):
@@ -360,6 +363,30 @@ class DryPool(_Held):
             self._h = ctypes.c_void_p()
 
 
+class PairGains(_Held):
+    """The loudness gain of every (dry signal, candidate) pair of a SourcePool and a DryPool (Renderer.pair_gains;
+    ss_pair_gains of the C ABI), which dry-picked slots (DryPick(..., gains=)) store their stems with.  `loudness` is an
+    (n_dry, n, 2) float64 array of every pair's measured integrated loudness (LUFS) and linear gain, NaN for a pair
+    without a target; `nbytes` counts its device bytes (4 per pair).  Plans hold it: it is freed once it is closed (or
+    collected) and no live plan uses it."""
+
+    def __init__(self, renderer, handle, pool, dry_pool, loudness):
+        self.renderer, self._h = renderer, handle
+        self.pool, self.dry_pool = pool, dry_pool
+        self._loudness = loudness
+        self.nbytes = int(renderer.lib.ss_pair_gains_bytes(handle))
+
+    @property
+    def loudness(self) -> np.ndarray:
+        """(n_dry, n, 2) float64: measured LUFS and linear gain of pair (d, i), NaN when unmeasured."""
+        return self._loudness.copy()
+
+    def _free(self):
+        if self._h:
+            self.renderer.lib.ss_pair_gains_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+
 def _rirs(s, conv=None):
     """Where a MovingSource / StaticSource takes its RIRs from: (RirBank or None, raw RIRs or None, P, C, L, mode).
     Raw RIRs go through conv(raw, field name, shape), the caller's conversion or check, and their shape is read from
@@ -441,9 +468,10 @@ def _hold_banks(plan, sources):
     releases them at once, once)."""
     banks = []
     for s in sources:
-        held = [s.pool, s.dry.pool if isinstance(s.dry, DryPick) else None] if isinstance(s, Pooled) else [_rirs(s)[0]]
+        dry = s.dry if isinstance(s, Pooled) and isinstance(s.dry, DryPick) else None
+        held = [s.pool] + ([dry.pool, dry.gains] if dry else []) if isinstance(s, Pooled) else [_rirs(s)[0]]
         for b in held:
-            if isinstance(b, (RirBank, SourcePool, DryPool)) and all(b is not o for o in banks):
+            if isinstance(b, (RirBank, SourcePool, DryPool, PairGains)) and all(b is not o for o in banks):
                 banks.append(b)
     for b in banks:
         b._hold()
@@ -669,6 +697,63 @@ class Renderer:
         _lib.check(self.lib.ss_dry_pool_create(self.ctx, ptrs, lengths.ctypes.data, n, flags, ctypes.byref(h)))
         return DryPool(self, h, [] if host else signals, lengths, levels, "host" if host else "device")
 
+    def pair_gains(self, pool: SourcePool, dry_pool: DryPool, lufs_targets, sr: float = 16000) -> PairGains:
+        """Measure the whole-stem loudness of every (dry signal d, candidate i) pair of `pool` and `dry_pool` once, for
+        dry-picked slots (DryPick(dry_pool, pick, gains=...)) to store their stems at SonicSet's loudness
+        (get_lufs_norm_audio, SonicSet.py:97-101) with no work per run.  `lufs_targets`: one float for every pair, or an
+        (n_dry, n) array whose entry [d, i] is pair (d, i)'s target, NaN to leave that pair at gain 1 - SonicSet's
+        per-stem draw is np.random.uniform(-19, -15, (n_dry, n)).  Each measured pair is candidate i rendered whole with
+        the first N samples of signal d, measured like render_host(..., lufs_targets=) measures it: `loudness` holds
+        the (LUFS, gain) pairs, bit for bit what render_host reports for that pair.  The call returns when the table is
+        on the device (4 bytes per pair)."""
+        import torch
+        if not isinstance(pool, SourcePool):
+            raise ValueError("pair_gains: pool must be a SourcePool, got %s" % type(pool).__name__)
+        if not isinstance(dry_pool, DryPool):
+            raise ValueError("pair_gains: dry_pool must be a DryPool, got %s" % type(dry_pool).__name__)
+        _check_usable(pool, self, "pair_gains: the SourcePool")
+        _check_usable(dry_pool, self, "pair_gains: the DryPool")
+        n, n_dry = pool.n, dry_pool.n
+        if n * n_dry > 1 << 26:
+            raise ValueError("pair_gains: %d x %d pairs, at most 2^26" % (n_dry, n))
+        if pool.C > 8:
+            raise ValueError("pair_gains: loudness normalisation supports at most 8 channels, the pool has %d" % pool.C)
+        if dry_pool.n_min < max(pool._sizes):
+            raise ValueError("pair_gains: the DryPool holds a signal of %d samples, shorter than the pool's longest "
+                             "candidate (N = %d)" % (dry_pool.n_min, max(pool._sizes)))
+        t = np.asarray(lufs_targets, dtype=np.float64)
+        if t.ndim == 0:
+            t = np.full((n_dry, n), float(t))
+        if t.shape != (n_dry, n):
+            raise ValueError("pair_gains: lufs_targets must be a float or an (n_dry, n) = (%d, %d) array, got shape %s"
+                             % (n_dry, n, t.shape))
+        bad = np.argwhere(np.isinf(t))
+        if len(bad):
+            d, i = (int(v) for v in bad[0])
+            raise ValueError("pair_gains: the loudness target of pair (%d, %d) is not finite: %r" % (d, i, t[d, i]))
+        if not float(sr) > 0:
+            raise ValueError("pair_gains: sr must be > 0, got %r" % (sr,))
+        t = np.ascontiguousarray(t)
+        from .SonicSim_audio import gating_block_size, gating_plan
+        post = (SsPostLufs * n)()
+        plans = {}
+        for i, N in enumerate(pool._sizes):
+            if np.isnan(t[:, i]).all():
+                continue                                   # no measured pair: no gating plan
+            block = float(gating_block_size(N, sr))
+            if N not in plans:
+                plans[N] = gating_plan(N, float(sr), block)
+            brk, blo, bhi = plans[N]
+            post[i] = SsPostLufs(brk=brk.ctypes.data, blk_lo=blo.ctypes.data, blk_hi=bhi.ctypes.data,
+                                 n_e=len(brk) - 1, n_blocks=len(blo), rate=float(sr), block_size=block)
+        loud = np.full((n_dry, n, 2), np.nan, dtype=np.float64)
+        if dry_pool.resident == "device":                  # measured on the library's own stream: finish the writes
+            torch.cuda.current_stream(self.device).synchronize()
+        h = ctypes.c_void_p()
+        _lib.check(self.lib.ss_pair_gains_create(self.ctx, pool._h, dry_pool._h, post, t.ctypes.data,
+                                                 loud.ctypes.data, ctypes.byref(h)))
+        return PairGains(self, h, pool, dry_pool, loud)
+
     # ------------------------------------------------------------------ host buffers
     def plan_host(self, sources: T.Sequence[T.Union[MovingSource, StaticSource]],
                   outs: T.Optional[T.Sequence[np.ndarray]] = None,
@@ -785,7 +870,7 @@ class Renderer:
         items, n, keep = self._device_items(sources, outs, direct_outs)
         mixes = self._device_mixes(mixtures, outs, keep) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
-        return DevicePlan(self, items, n, keep, mixes, drw, dry)
+        return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -809,15 +894,32 @@ class Renderer:
                 if pl.resident == "host" and d.pool.resident == "device":
                     raise ValueError("plan_device: pooled source %d has a dry pick over a host pool, whose runs stage "
                                      "each candidate's own dry signal" % i)
-                if pl.gains:
+                if pl.gains and d.gains is None:
                     raise ValueError("plan_device: pooled source %d has a dry pick over a pool with loudness gains, "
-                                     "which were measured with the candidates' own dry signals" % i)
+                                     "which were measured with the candidates' own dry signals; give the DryPick "
+                                     "pair gains (Renderer.pair_gains)" % i)
                 if d.pool.n_min < max(pl._sizes):
                     raise ValueError("plan_device: the DryPool of source %d holds a signal of %d samples, shorter than "
                                      "its pool's longest candidate (N = %d)" % (i, d.pool.n_min, max(pl._sizes)))
+            if d.gains is not None:
+                g = d.gains
+                if not isinstance(g, PairGains):
+                    raise ValueError("plan_device: the gains of the DryPick of source %d must be a PairGains" % i)
+                _check_usable(g, self, "plan_device: the PairGains of source %d" % i)
+                if g.pool is not pl or g.dry_pool is not d.pool:
+                    raise ValueError("plan_device: the PairGains of source %d were measured over another SourcePool "
+                                     "or DryPool than the slot's pool and its DryPick's" % i)
             pick = _tensor(d.pick, "plan_device", "source %d" % i, "dry pick", torch.int32, self.device, count=(1, 1))
             picks.append(_lib.SsDryPick(slot=i, pool=d.pool._h.value, pick_dev=pick))
         return (_lib.SsDryPick * len(picks))(*picks) if picks else None
+
+    @staticmethod
+    def _device_pair_gains(sources):
+        """The ss_pair_gains handles of a plan's dry picks (the order of _device_dry), or None when no pick has gains."""
+        picks = [s.dry for s in sources if isinstance(s, Pooled) and isinstance(s.dry, DryPick)]
+        if all(d.gains is None for d in picks):
+            return None
+        return (ctypes.c_void_p * len(picks))(*[d.gains._h.value if d.gains is not None else None for d in picks])
 
     def _device_draws(self, draws, sources, keep):
         """Validated ss_plan_draw array of a plan's start draws; their tensors are appended to `keep`."""
@@ -1024,16 +1126,20 @@ class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
-    dry-picked slots take their dry signals from dry pools (ss_plan_create_dry)."""
+    dry-picked slots take their dry signals from dry pools (ss_plan_create_dry), and with pair gains their gains from
+    pair-gain tables (ss_plan_create_pair)."""
 
-    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None):
+    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
-        self.draws, self.dry = draws, dry
+        self.draws, self.dry, self.pair_gains = draws, dry, pair_gains
         self._plan = ctypes.c_void_p()
         if n > 0:
-            _lib.check(renderer.lib.ss_plan_create_dry(renderer.ctx, items, n, mixes, len(mixes) if mixes else 0,
-                                                       draws, len(draws) if draws else 0, dry, len(dry) if dry else 0,
-                                                       ctypes.byref(self._plan)))
+            args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry)
+            if pair_gains is None:
+                st = renderer.lib.ss_plan_create_dry(*args, len(dry) if dry else 0, ctypes.byref(self._plan))
+            else:
+                st = renderer.lib.ss_plan_create_pair(*args, pair_gains, len(dry), ctypes.byref(self._plan))
+            _lib.check(st)
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
