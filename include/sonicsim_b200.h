@@ -469,7 +469,8 @@ int ss_plan_create_ex(ss_ctx* ctx, const ss_source* items, int n_items, const ss
  * NULL picks with n_picks > 0; a slot outside [0, n_items), or named by two dry picks; a slot that is not pooled, or
  * whose pool has loudness gains (measured with the candidates' own dry signals; ss_plan_create_pair accepts it with pair
  * gains, below), or is a host pool while the dry pool is
- * a device one (k_stage copies whole float4s, which only a host dry pool's padded arena guarantees); a NULL pool or one
+ * a device float32 one (k_stage copies whole float4s, which only a host or 16-bit dry pool's padded arena guarantees); a
+ * NULL pool or one
  * of another context; a dry pool with a signal shorter than the slot pool's longest candidate N; a NULL or unaligned
  * pick_dev; a draw speaker with a dry pick whose dry pool has no level tables; a range a plan writes that meets a dry
  * pick or a signal of a device dry pool it uses (a host dry pool owns its arena).  A destroyed dry pool cannot be
@@ -494,6 +495,42 @@ int64_t ss_dry_pool_host_bytes(const ss_dry_pool* pool);   /* pinned host bytes 
  * without tables or with i outside [0, n). */
 const double* ss_dry_pool_level_table(const ss_dry_pool* pool, int i);
 void ss_dry_pool_destroy(ss_dry_pool* pool);          /* destroy dry pools after the plans that use them */
+/* ---- 16-bit dry pools: a speech corpus of 16-bit PCM (LibriSpeech; SonicSet's streams place whole utterances into
+ * zeros, so every sample is k / 32768 with k an int16) held as its int16 samples, about 2.125 B per sample with level
+ * tables instead of 12.  A 16-bit pool behaves bit for bit as the float32 dry pool of the values k / 32768: stems,
+ * direct stems, mixtures, rms_db, drawn starts, `used`, pair gains and level tables are the same, in every residency.
+ *   - ss_dry_pool_create_i16: x[i] is a host or device pointer (2-byte aligned) to signal i's lengths[i] int16 samples.
+ *     flags: SS_DRY_LEVELS and SS_DRY_HOST as for ss_dry_pool_create.  The pool always copies the signals into one arena
+ *     it owns - device memory, or pinned, mapped host memory with SS_DRY_HOST - each at a 64-byte boundary and
+ *     zero-padded to the next, so the caller's buffers may go once the call returns.
+ *   - Level tables (SS_DRY_LEVELS) are kept at stride 64 (ss_dry_pool_level_stride): signal i's table holds q[j] =
+ *     Q[min(64 j, lengths[i])] for j = 0..ceil(lengths[i] / 64), ceil(lengths[i] / 64) + 1 doubles, at the pool's
+ *     residency; Q is the float pool's full table.  The float32 square of k / 32768 is a multiple of 2^-30 and at most
+ *     1, so with lengths[i] <= 2^23 every partial sum of Q is exact in float64 in any order: Q[s] = q[s / 64] plus the
+ *     float64 sum of the float32 squares of samples [64 (s / 64), s), bit for bit.  The tables are built by the scan of
+ *     ss_pool_levels over transient float32 expansions of the signals, in batches of at most 256 MB of expansions.
+ *   - Plans (ss_plan_create_dry / _pair): every slot with a 16-bit dry pick is staged, whatever the residency of its dry
+ *     pool and its pool: at every run k_stage reads the picks (bits 3 and 4, clamped) and stores the picked signal's
+ *     samples [xa & ~3, (xb + 3) & ~3) of the candidate's read set as exact float32 into the slot's staging area, sized
+ *     as for a host dry pool.  A 16-bit pool serves slots of device and of host pools alike.  A draw speaker with a
+ *     16-bit dry pick forms Q[s] and Q[s + len] from the sparse table and at most 63 samples each (k_draw reads them over
+ *     PCIe for a host pool); speakers of float and 16-bit pools may share a draw.
+ *   - Pair gains (ss_pair_gains_create) render each pair from a transient float32 expansion of the dry signal.
+ *   - ss_dry_pool_bytes = 8 n (signal pointers) + the arena without SS_DRY_HOST (sum of 2 lengths[i] rounded up to 64)
+ *     + with tables 8 n (table pointers) + the tables without SS_DRY_HOST (8 (ceil(lengths[i] / 64) + 1) each);
+ *     ss_dry_pool_host_bytes = the arena and the tables with SS_DRY_HOST, else 0.  ss_dry_pool_level_table returns the
+ *     sparse table (a mapped host address with SS_DRY_HOST).
+ * Refused before anything is allocated: NULL arguments, n outside [1, 2^24], a NULL or odd x[i], unknown flags
+ * (SS_ERR_INVALID); a length outside [1, 2^23] (SS_ERR_UNSUPPORTED: beyond 2^23 samples the tables' sums, and so the
+ * bit contract, need not be exact).  ss_version stays 108: these exports mark the capability. */
+int ss_dry_pool_create_i16(ss_ctx* ctx, const int16_t* const* x, const int32_t* lengths, int n, uint32_t flags,
+                           ss_dry_pool** out);
+/* Samples per level table entry of a dry pool: 1 (ss_dry_pool_create: entry s is Q[s]) or 64 (a 16-bit pool), 0 for
+ * NULL. */
+int ss_dry_pool_level_stride(const ss_dry_pool* pool);
+/* Signal i of a 16-bit pool in its arena (a device pointer, or a host address with SS_DRY_HOST), or NULL for another
+ * pool or i outside [0, n). */
+const int16_t* ss_dry_pool_signal_i16(const ss_dry_pool* pool, int i);
 int ss_plan_create_dry(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks, ss_plan** out);
 

@@ -185,6 +185,10 @@ def load():
         lib.ss_dry_pool_level_table.restype = vp
         lib.ss_dry_pool_destroy.argtypes = [vp]
         lib.ss_dry_pool_destroy.restype = None
+        lib.ss_dry_pool_create_i16.argtypes = [vp, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.POINTER(vp)]
+        lib.ss_dry_pool_level_stride.argtypes = [vp]
+        lib.ss_dry_pool_signal_i16.argtypes = [vp, ctypes.c_int]
+        lib.ss_dry_pool_signal_i16.restype = vp
         lib.ss_pair_gains_create.argtypes = [vp, vp, vp, ctypes.POINTER(SsPostLufs), vp, vp, ctypes.POINTER(vp)]
         lib.ss_pair_gains_bytes.argtypes = [vp]
         lib.ss_pair_gains_bytes.restype = i64
@@ -225,7 +229,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_host_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_plan_create_dry", "ss_pair_gains_create", "ss_pair_gains_bytes", "ss_pair_gains_destroy", "ss_plan_create_pair", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_host_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_dry_pool_create_i16", "ss_dry_pool_level_stride", "ss_dry_pool_signal_i16", "ss_plan_create_dry", "ss_pair_gains_create", "ss_pair_gains_bytes", "ss_pair_gains_destroy", "ss_plan_create_pair", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

@@ -849,6 +849,10 @@ struct ss_pool {
 // that dry-picked slots index (dry_table), and with SS_DRY_LEVELS every signal's level table.  A host dry pool
 // (SS_DRY_HOST) owns its signals, copied into one pinned, mapped arena, and keeps its tables in pinned, mapped host
 // memory: x, ptrs, levels and level_ptr then hold mapped device addresses.
+// A 16-bit dry pool (ss_dry_pool_create_i16) owns one arena of int16 signals, in device memory or (SS_DRY_HOST) pinned,
+// mapped host memory; ptrs and x16 hold int16 addresses, x is empty, and its tables are sparse (kLevelStride): signal
+// i's ceil(N / 64) + 1 entries at levels + level_off[i].  With tables, ptrs holds 2n pointers, the n signals' and then
+// the n tables' (level_ptr = ptrs + n, not allocated on its own), which k_draw reads both of (speaker_signal_i16).
 struct ss_dry_pool {
     ss_ctx* c = nullptr;
     int n = 0, n_min = 0;                 // n_min: the shortest signal (the longest candidate N it serves)
@@ -862,6 +866,12 @@ struct ss_dry_pool {
     char* h_x = nullptr;                  // the arena (host address) and its bytes
     size_t h_x_bytes = 0;
     double* h_levels = nullptr;           // the tables' host address
+    bool i16 = false;                     // a 16-bit pool ...
+    std::vector<const int16_t*> x16;      // ... its signals' device (or mapped) addresses ...
+    char* d_x = nullptr;                  // ... and its device arena and its bytes (without SS_DRY_HOST)
+    size_t d_x_bytes = 0;
+    int stride() const { return i16 ? kLevelStride : 1; }
+    bool padded() const { return host || i16; }   // owns an arena padded for k_stage's wide loads
 };
 // Order `stream` after the construction of every bank the items use (a bank built from device memory is built
 // asynchronously on its creator's stream, which a render may not share: the host path runs on the context's own streams).
@@ -1788,10 +1798,25 @@ struct StemSet {
     const ss_dry_pool* dry = nullptr;     // the pool the signals come from, or null: every stem takes its own x
     std::vector<Stem> stems;
     int N(size_t k) const { return pl->host[stems[k].cand].N; }
-    const float* x(size_t k) const { return stems[k].sig < 0 ? pl->host[stems[k].cand].x : dry->x[stems[k].sig]; }
-    // rendered from transient device copies: a host pool's banks and dry signals, a host dry pool's signals
-    bool copied() const { return pl->host_res || (dry && dry->host); }
+    // (null for a 16-bit signal, which is only read through its float32 expansion: render_copied_stems)
+    const float* x(size_t k) const {
+        return stems[k].sig < 0 ? pl->host[stems[k].cand].x : dry->i16 ? nullptr : dry->x[stems[k].sig];
+    }
+    // rendered from transient device copies: a host pool's banks and dry signals, a host or 16-bit dry pool's signals
+    bool copied() const { return pl->host_res || (dry && dry->padded()); }
 };
+// A 16-bit signal's float32 expansion y[n] = x[n] / 32768, exact (x: device or mapped host memory)
+__global__ void __launch_bounds__(256) k_expand_i16(const int16_t* __restrict__ x, float* __restrict__ y, long long N) {
+    for (long long n = (long long)blockIdx.x * blockDim.x + threadIdx.x; n < N; n += (long long)gridDim.x * blockDim.x)
+        y[n] = i16_sample(x[n]);
+}
+static int expand_i16(ss_ctx* c, const int16_t* x, float* y, long long N, cudaStream_t s) {
+    const long long blocks = std::min((N + 255) / 256, (long long)c->sm_count * 8);
+    k_expand_i16<<<(unsigned)blocks, 256, 0, s>>>(x, y, N);
+    CK(cudaGetLastError());
+    c->launches += 1;
+    return SS_OK;
+}
 // every candidate of a pool with its own x, in candidate order (stem i is candidate i)
 static StemSet own_stems(const ss_pool* pl) {
     StemSet S;
@@ -1863,7 +1888,12 @@ static int render_copied_stems(const StemSet& S, ss_source* items, int first, in
                 shell = &sh;
             }
             float* x = (float*)(buf + used);
-            CK(cudaMemcpyAsync(x, S.x(k), sizeof(float) * (size_t)S.N(k), cudaMemcpyDefault, s));
+            if (S.stems[k].sig >= 0 && S.dry->i16) {
+                const int st = expand_i16(S.pl->c, S.dry->x16[S.stems[k].sig], x, S.N(k), s);
+                if (st) return st;
+            } else {
+                CK(cudaMemcpyAsync(x, S.x(k), sizeof(float) * (size_t)S.N(k), cudaMemcpyDefault, s));
+            }
             used += stem_x_bytes(S, k);
             items[hi].x = x;
             if (S.pl->host_res) items[hi].rir_bank = shell;
@@ -2067,8 +2097,9 @@ extern "C" void ss_dry_pool_destroy(ss_dry_pool* dp) {
     cudaDeviceSynchronize();                            // (a plan that used it may run on any stream)
     if (dp->ptrs) cudaFree(dp->ptrs);
     if (dp->h_levels) cudaFreeHost(dp->h_levels); else if (dp->levels) cudaFree(dp->levels);
-    if (dp->level_ptr) cudaFree(dp->level_ptr);
+    if (dp->level_ptr && !dp->i16) cudaFree(dp->level_ptr);   // (a 16-bit pool's lie in ptrs)
     if (dp->h_x) cudaFreeHost(dp->h_x);
+    if (dp->d_x) cudaFree(dp->d_x);
     delete dp;
 }
 static int64_t dry_level_bytes(const ss_dry_pool* dp) {
@@ -2076,7 +2107,7 @@ static int64_t dry_level_bytes(const ss_dry_pool* dp) {
 }
 extern "C" int64_t ss_dry_pool_bytes(const ss_dry_pool* dp) {
     if (!dp) return 0;
-    int64_t b = (int64_t)sizeof(float*) * dp->n;
+    int64_t b = (int64_t)sizeof(float*) * dp->n + (int64_t)dp->d_x_bytes;
     if (dp->levels) b += (dp->host ? 0 : dry_level_bytes(dp)) + (int64_t)sizeof(double*) * dp->n;
     return b;
 }
@@ -2086,6 +2117,44 @@ extern "C" int64_t ss_dry_pool_host_bytes(const ss_dry_pool* dp) {
 extern "C" const double* ss_dry_pool_level_table(const ss_dry_pool* dp, int i) {
     if (!dp || !dp->levels || i < 0 || i >= dp->n) return nullptr;
     return (dp->host ? dp->h_levels : dp->levels) + dp->level_off[i];
+}
+extern "C" int ss_dry_pool_level_stride(const ss_dry_pool* dp) { return dp ? dp->stride() : 0; }
+extern "C" const int16_t* ss_dry_pool_signal_i16(const ss_dry_pool* dp, int i) {
+    if (!dp || !dp->i16 || i < 0 || i >= dp->n) return nullptr;
+    return dp->host ? (const int16_t*)(dp->h_x + ((const char*)dp->x16[i] - (const char*)dp->x16[0])) : dp->x16[i];
+}
+// A 16-bit dry pool: the signals into its arena (device memory, or pinned, mapped host memory with SS_DRY_HOST), each at
+// a 64-byte boundary and zero-padded to the next (k_stage reads whole groups of 4 samples around a read set); x16[i]
+// receives the signal's device (or mapped device) address
+static int dry_i16_copies(ss_dry_pool* dp, const int16_t* const* x) {
+    const int n = dp->n;
+    std::vector<size_t> xo(n + 1, 0);
+    for (int i = 0; i < n; ++i) xo[i + 1] = xo[i] + align_up(sizeof(int16_t) * (size_t)dp->N[i], 64);
+    char* dx = nullptr;
+    if (dp->host) {
+        dp->h_x_bytes = xo[n];
+        CK(cudaHostAlloc((void**)&dp->h_x, dp->h_x_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+        CK(cudaHostGetDevicePointer((void**)&dx, dp->h_x, 0));
+    } else {
+        dp->d_x_bytes = xo[n];
+        CK(cudaMalloc((void**)&dp->d_x, dp->d_x_bytes));
+        CK(cudaMemset(dp->d_x, 0, dp->d_x_bytes));
+        dx = dp->d_x;
+    }
+    dp->x16.resize(n);
+    for (int i = 0; i < n; ++i) {
+        const size_t b = sizeof(int16_t) * (size_t)dp->N[i];
+        CK(cudaMemcpy((dp->host ? dp->h_x : dp->d_x) + xo[i], x[i], b, cudaMemcpyDefault));
+        if (dp->host) memset(dp->h_x + xo[i] + b, 0, xo[i + 1] - xo[i] - b);
+        dp->x16[i] = (const int16_t*)(dx + xo[i]);
+    }
+    return SS_OK;
+}
+// A 16-bit pool's sparse tables from full ones: q[j] = Q[min(64 j, N)], j = 0..ceil(N / 64)
+__global__ void __launch_bounds__(256) k_level_sample(const double* __restrict__ Q, double* __restrict__ q, long long N) {
+    const long long m = (N + kLevelStride - 1) / kLevelStride;
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j <= m; j += (long long)gridDim.x * blockDim.x)
+        q[j] = Q[j * kLevelStride < N ? j * kLevelStride : N];
 }
 // A host dry pool: the signals into its pinned, mapped arena, each at a 64-byte boundary and zero-padded to whole
 // float4s (k_stage copies whole float4s around a read set); x[i] becomes the signal's mapped device address
@@ -2105,38 +2174,65 @@ static int dry_host_copies(ss_dry_pool* dp) {
     }
     return SS_OK;
 }
-// A host dry pool's level tables: k_levels over transient device copies of the signals, in batches of at most
-// kLevelStemBytes of copies (or one signal's, when larger), each batch's copies behind the previous batch's scan on `s`;
-// k_levels writes the tables into pinned, mapped host memory.  `li` holds every signal's descriptor with its table.
-static int dry_host_levels(ss_dry_pool* dp, std::vector<LevelItem>& li, cudaStream_t s) {
+// The level tables of a host or 16-bit dry pool: k_levels over transient device copies of the signals (a 16-bit pool's:
+// their float32 expansions), in batches of at most kLevelStemBytes of copies (or one signal's, when larger), each
+// batch's copies behind the previous batch's scan on `s`.  k_levels writes a host dry pool's tables into pinned, mapped
+// host memory; a 16-bit pool's full tables go to transient device memory too, and k_level_sample keeps every 64th entry
+// and the last in the pool's tables, which are therefore the float pool's entries bit for bit.  `li` holds every
+// signal's descriptor with its table.
+static int dry_copied_levels(ss_dry_pool* dp, std::vector<LevelItem>& li, cudaStream_t s) {
     const int n = dp->n;
-    std::vector<size_t> at(n);
+    std::vector<size_t> at(n), tat(n);
     std::vector<int> first(1, 0);
-    size_t used = 0, cap = kLevelStemBytes;
+    size_t used = 0, cap = kLevelStemBytes, tused = 0, tcap = 0;
     for (int i = 0; i < n; ++i) cap = std::max(cap, align_up(sizeof(float) * (size_t)dp->N[i], 256));
     for (int i = 0; i < n; ++i) {
         const size_t b = align_up(sizeof(float) * (size_t)dp->N[i], 256);
-        if (used > 0 && used + b > cap) { first.push_back(i); used = 0; }
+        if (used > 0 && used + b > cap) { first.push_back(i); used = 0; tused = 0; }
         at[i] = used;
         used += b;
+        tat[i] = tused;                                 // (a 16-bit pool: the signal's full table in the batch's)
+        tused += align_up(sizeof(double) * ((size_t)dp->N[i] + 1), 256);
+        tcap = std::max(tcap, tused);
     }
     first.push_back(n);
     if (first.size() == 2) cap = used;                  // one batch: no more than it needs
-    char* buf = nullptr;
+    char *buf = nullptr, *tabs = nullptr;
     CK(cudaMalloc((void**)&buf, cap));
-    struct Free { void* p; ~Free() { cudaFree(p); } } free_buf{buf};   // (cudaFree waits for the device)
-    for (int i = 0; i < n; ++i) li[i].y = (const float*)(buf + at[i]);
+    struct Free { void* p; ~Free() { if (p) cudaFree(p); } } free_buf{buf};   // (cudaFree waits for the device)
+    if (dp->i16) CK(cudaMalloc((void**)&tabs, tcap));
+    struct Free free_tabs{tabs};
+    std::vector<double*> q(n);                          // the pool's tables
+    for (int i = 0; i < n; ++i) {
+        q[i] = li[i].q;
+        li[i].y = (const float*)(buf + at[i]);
+        if (dp->i16) li[i].q = (double*)(tabs + tat[i]);
+    }
     LevelItem* d_items = nullptr;
     CK(cudaMalloc((void**)&d_items, sizeof(LevelItem) * (size_t)n));
     struct Free free_items{d_items};
     CK(cudaMemcpy(d_items, li.data(), sizeof(LevelItem) * (size_t)n, cudaMemcpyHostToDevice));
     for (size_t g = 0; g + 1 < first.size(); ++g) {
-        for (int i = first[g]; i < first[g + 1]; ++i)
-            CK(cudaMemcpyAsync((void*)li[i].y, dp->x[i], sizeof(float) * (size_t)dp->N[i], cudaMemcpyDefault, s));
+        for (int i = first[g]; i < first[g + 1]; ++i) {
+            if (dp->i16) {
+                const int st = expand_i16(dp->c, dp->x16[i], (float*)li[i].y, dp->N[i], s);
+                if (st) return st;
+            } else {
+                CK(cudaMemcpyAsync((void*)li[i].y, dp->x[i], sizeof(float) * (size_t)dp->N[i], cudaMemcpyDefault, s));
+            }
+        }
         for (int k = first[g]; k < first[g + 1]; k += 65535) {
             const int st = levels_enqueue(dp->c, d_items + k, std::min(first[g + 1] - k, 65535), true, s);
             if (st) return st;
         }
+        if (dp->i16)
+            for (int i = first[g]; i < first[g + 1]; ++i) {
+                const long long m = ((long long)dp->N[i] + kLevelStride - 1) / kLevelStride + 1;
+                k_level_sample<<<(unsigned)std::min((m + 255) / 256, (long long)dp->c->sm_count * 8), 256, 0, s>>>(
+                    li[i].q, q[i], dp->N[i]);
+                CK(cudaGetLastError());
+                dp->c->launches += 1;
+            }
     }
     CK(cudaStreamSynchronize(s));
     return SS_OK;
@@ -2146,12 +2242,16 @@ static int dry_host_levels(ss_dry_pool* dp, std::vector<LevelItem>& li, cudaStre
 // they are complete.
 static int dry_pool_build(ss_dry_pool* dp, bool levels) {
     const int n = dp->n;
-    if (dp->host) { const int st = dry_host_copies(dp); if (st) return st; }
-    CK(cudaMalloc((void**)&dp->ptrs, sizeof(float*) * (size_t)n));
-    CK(cudaMemcpy(dp->ptrs, dp->x.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice));
+    if (dp->host && !dp->i16) { const int st = dry_host_copies(dp); if (st) return st; }
+    // the signal pointers, and a 16-bit pool's table pointers behind them
+    const size_t n_ptr = (dp->i16 && levels ? 2 : 1) * (size_t)n;
+    CK(cudaMalloc((void**)&dp->ptrs, sizeof(float*) * n_ptr));
+    if (dp->i16) CK(cudaMemcpy(dp->ptrs, dp->x16.data(), sizeof(int16_t*) * (size_t)n, cudaMemcpyHostToDevice));
+    else CK(cudaMemcpy(dp->ptrs, dp->x.data(), sizeof(float*) * (size_t)n, cudaMemcpyHostToDevice));
     if (!levels) return SS_OK;
     dp->level_off.assign(n + 1, 0);
-    for (int i = 0; i < n; ++i) dp->level_off[i + 1] = dp->level_off[i] + dp->N[i] + 1;
+    const int r = dp->stride();
+    for (int i = 0; i < n; ++i) dp->level_off[i + 1] = dp->level_off[i] + (dp->N[i] + r - 1) / r + 1;
     const size_t tb = sizeof(double) * (size_t)dp->level_off[n];
     if (dp->host) {                                     // k_levels writes and k_draw reads them over PCIe
         CK(cudaHostAlloc((void**)&dp->h_levels, tb, cudaHostAllocMapped | cudaHostAllocPortable));
@@ -2159,17 +2259,18 @@ static int dry_pool_build(ss_dry_pool* dp, bool levels) {
     } else {
         CK(cudaMalloc((void**)&dp->levels, tb));
     }
-    CK(cudaMalloc((void**)&dp->level_ptr, sizeof(double*) * (size_t)n));
+    if (dp->i16) dp->level_ptr = (const double**)(dp->ptrs + n);
+    else CK(cudaMalloc((void**)&dp->level_ptr, sizeof(double*) * (size_t)n));
     std::vector<const double*> ptr(n);
     std::vector<LevelItem> li(n);
     for (int i = 0; i < n; ++i) {
         ptr[i] = dp->levels + dp->level_off[i];
-        li[i] = {dp->x[i], dp->levels + dp->level_off[i], dp->N[i], 1, 0};
+        li[i] = {dp->i16 ? nullptr : dp->x[i], dp->levels + dp->level_off[i], dp->N[i], 1, 0};
     }
     CK(cudaMemcpy(dp->level_ptr, ptr.data(), sizeof(double*) * (size_t)n, cudaMemcpyHostToDevice));
     BuildStream bs;
     CK(cudaStreamCreateWithFlags(&bs.s, cudaStreamNonBlocking));
-    if (dp->host) return dry_host_levels(dp, li, bs.s);
+    if (dp->padded()) return dry_copied_levels(dp, li, bs.s);
     LevelItem* d_items = nullptr;
     CK(cudaMalloc((void**)&d_items, sizeof(LevelItem) * (size_t)n));
     struct Free { void* p; ~Free() { cudaFree(p); } } free_items{d_items};   // (cudaFree waits for the device)
@@ -2196,6 +2297,26 @@ extern "C" int ss_dry_pool_create(ss_ctx* c, const float* const* x, const int32_
     dp->N.assign(lengths, lengths + n);
     dp->n_min = *std::min_element(lengths, lengths + n);
     const int st = dry_pool_build(dp, (flags & SS_DRY_LEVELS) != 0);
+    if (st != SS_OK) { ss_dry_pool_destroy(dp); return st; }
+    *out = dp;
+    return SS_OK;
+}
+extern "C" int ss_dry_pool_create_i16(ss_ctx* c, const int16_t* const* x, const int32_t* lengths, int n, uint32_t flags,
+                                      ss_dry_pool** out) {
+    if (!c || !x || !lengths || !out || n < 1 || n > (1 << 24) || (flags & ~(SS_DRY_LEVELS | SS_DRY_HOST)))
+        return SS_ERR_INVALID;
+    *out = nullptr;
+    for (int i = 0; i < n; ++i) if (!x[i] || ((uintptr_t)x[i] & 1)) return SS_ERR_INVALID;
+    for (int i = 0; i < n; ++i)                         // (beyond 2^23 samples a table's sums need not be exact)
+        if (lengths[i] < 1 || lengths[i] > (1 << 23)) return SS_ERR_UNSUPPORTED;
+    CK(cudaSetDevice(c->device));
+    ss_dry_pool* dp = new (std::nothrow) ss_dry_pool();
+    if (!dp) return SS_ERR_NOMEM;
+    dp->c = c; dp->n = n; dp->host = (flags & SS_DRY_HOST) != 0; dp->i16 = true;
+    dp->N.assign(lengths, lengths + n);
+    dp->n_min = *std::min_element(lengths, lengths + n);
+    int st = dry_i16_copies(dp, x);
+    if (st == SS_OK) st = dry_pool_build(dp, (flags & SS_DRY_LEVELS) != 0);
     if (st != SS_OK) { ss_dry_pool_destroy(dp); return st; }
     *out = dp;
     return SS_OK;
@@ -2300,6 +2421,7 @@ struct ss_plan {
     int n_draw = 0;
     const StageSlot* d_stage = nullptr;   // the staged slots' k_stage descriptors, in d_desc behind the draws
     int n_stage = 0;
+    bool draw16 = false, stage16 = false; // a draw speaker / a staged slot has a 16-bit dry pick: k_draw<true> / k_stage<true>
 };
 
 // ----------------------------------------------------------------------------- k_draw
@@ -2316,7 +2438,9 @@ struct DrawReader {
     const double* const* dry_levels;  // a dry-picked speaker: its dry pool's table pointers, else null ...
     const int* dry_pick;              // ... its dry pick ...
     int n_dry;                        // ... and the dry pool's signal count
+    int dry16;                        // 1: the dry pool is 16-bit (sparse tables, speaker_signal_i16; k_draw<true> only)
 };
+static_assert(sizeof(DrawReader) == 64, "DrawReader layout");
 struct DrawDesc {
     int* start;
     const double* u;
@@ -2329,6 +2453,9 @@ struct DrawDesc {
 
 // One warp per draw: the readers' picked N give M (a lane per reader), then 32 tries at a time, a lane per try, and a
 // ballot takes the first try at which no speaker is silent; after the last try without one, the last try's start.
+// k_draw<true> (a plan with a 16-bit dry-picked speaker) tests such a speaker from its sparse table and its signal's
+// samples (draw_silent_i16): at most 2 * 63 samples and two table entries per try, over PCIe for a host pool.
+template <bool I16>
 __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws, int n) {
     const int lane = threadIdx.x & 31, di = blockIdx.x * 4 + (threadIdx.x >> 5);
     if (di >= n) return;
@@ -2343,13 +2470,15 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
     for (int o = 16; o > 0; o >>= 1) M = min(M, __shfl_xor_sync(0xffffffffu, M, o));
     const double* Q[kDrawSpeakers];
     double D[kDrawSpeakers];
+    const int16_t* X[kDrawSpeakers];                    // (k_draw<true>) a 16-bit speaker's signal, else null
 #pragma unroll
     for (int k = 0; k < kDrawSpeakers; ++k) {
-        Q[k] = nullptr; D[k] = 1.0;
+        Q[k] = nullptr; D[k] = 1.0; X[k] = nullptr;
         if (k < d.S) {
             const DrawReader& r = d.r[d.spk[k]];
             Q[k] = speaker_table(r.levels, r.pick, r.n, r.dry_levels, r.dry_pick, r.n_dry);
             D[k] = r.D;
+            if (I16 && r.dry16) X[k] = speaker_signal_i16(r.dry_levels, r.dry_pick, r.n_dry);
         }
     }
     int start = 0, used = 0;
@@ -2362,7 +2491,9 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
             pass = true;
 #pragma unroll
             for (int k = 0; k < kDrawSpeakers; ++k)
-                if (k < d.S && pass && draw_silent(Q[k], s, d.len, D[k], d.threshold_db)) pass = false;
+                if (k < d.S && pass && (I16 && X[k] ? draw_silent_i16(Q[k], X[k], s, d.len, d.threshold_db)
+                                                    : draw_silent(Q[k], s, d.len, D[k], d.threshold_db)))
+                    pass = false;
         }
         const unsigned ok = __ballot_sync(0xffffffffu, pass);
         if (ok) {
@@ -2381,8 +2512,9 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
 
 // ----------------------------------------------------------------------------- k_stage
 // Staged slots: at the head of every run (after k_draw, so that drawn starts are final), each pooled slot of a host pool
-// and each slot with a dry pick from a host dry pool gets its picked candidate's read set (stage_set) copied from pinned,
-// mapped host memory into its staging area, and its view of the candidate (StageView), which the head of k_blocks takes.
+// and each slot with a dry pick from a host or 16-bit dry pool gets its picked candidate's read set (stage_set) copied
+// (from pinned, mapped host memory, or a 16-bit pool's arena) into its staging area, and its view of the candidate
+// (StageView), which the head of k_blocks takes.
 // A slot of a host pool stages the RIR rows and the dry samples; a slot of a device pool stages only the dry samples of
 // its dry pick.  One gridDim.y row of kStageCtas CTAs per slot: every CTA works out the read set (stage_head), then the
 // CTAs copy it in 16-byte loads, kStageUnroll of them in flight per thread.
@@ -2402,7 +2534,13 @@ struct StageSlot {
     int n, C, K, ws, len;
     int sets;                         // spectra sets staged: 1, 2 with a direct target, 0 for a slot of a device pool
     int n_dry;                        // ... and the dry pool's signal count
+    int i16;                          // 1: the dry pool is 16-bit, `dry` holds int16 addresses (k_stage<true> only)
 };
+static_assert(sizeof(StageSlot) == 120, "StageSlot layout");
+// k_stage<true> (a plan with a 16-bit dry pick) reads such a slot's dry samples as 4 int16 at a time from the whole
+// groups [xa & ~3, (xb + 3) & ~3) of the picked signal (inside its padded arena) and stores their exact float32 values,
+// so that the staging area holds what a float pool's slot stages.
+template <bool I16>
 __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots) {
     const StageSlot& g = slots[blockIdx.y];
     __shared__ StageView s_v;
@@ -2421,6 +2559,8 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
     const size_t rows_h = (size_t)e.P * g.C * s_v.K;                 // rows per set of the bank
     const size_t total = nx4 + (size_t)g.sets * per_set;
     const float4* const xs = reinterpret_cast<const float4*>(s_src + s_x[0]);
+    const short4* const xs16 = I16 && g.i16 ? reinterpret_cast<const short4*>(reinterpret_cast<const int16_t*>(s_src) + s_x[0])
+                                            : nullptr;
     float4* const xd = reinterpret_cast<float4*>(g.x);
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (size_t q0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x; q0 < total; q0 += stride * kStageUnroll) {
@@ -2431,7 +2571,7 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
             const size_t q = q0 + u * stride;
             dst[u] = nullptr;
             if (q >= total) continue;
-            if (q < nx4) { v[u] = xs[q]; dst[u] = xd + q; continue; }
+            if (q < nx4) { v[u] = I16 && xs16 ? i16x4_samples(xs16[q]) : xs[q]; dst[u] = xd + q; continue; }
             const size_t j = q - nx4, set = j / per_set;
             v[u] = reinterpret_cast<const float4*>(e.spec + (set * rows_h + s_v.row0) * kSpec)[j - set * per_set];
             dst[u] = reinterpret_cast<float4*>(g.spec) + j;
@@ -2487,7 +2627,10 @@ static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan
         g.len = it.win_len;
         DrawReader r = {pl->table, it.pick_dev, pl->level_ptr, pl->n,
                         (double)it.win_len * ((pl->level_flags & SS_MIX_MONO) ? 1 : pl->C), nullptr, nullptr, 0};
-        if (dry[i]) { r.dry_levels = dry[i]->pool->level_ptr; r.dry_pick = dry[i]->pick_dev; r.n_dry = dry[i]->pool->n; r.D = it.win_len; }
+        if (dry[i]) {
+            r.dry_levels = dry[i]->pool->level_ptr; r.dry_pick = dry[i]->pick_dev; r.n_dry = dry[i]->pool->n; r.D = it.win_len;
+            r.dry16 = dry[i]->pool->i16 ? 1 : 0;
+        }
         g.r[g.n_readers++] = r;
     }
     return g;
@@ -2548,9 +2691,9 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     const size_t draw_off = align_up(scr_off + scr_bytes * n_mixes, 256);
     const size_t desc_bytes = draw_off + sizeof(DrawDesc) * n_draws;
     // behind the draws: the staged slots' k_stage descriptors, then their staging areas
-    std::vector<int> staged;                            // arranged items that are slots of host pools or host dry picks
+    std::vector<int> staged;                            // arranged items that are slots of host pools, host or 16-bit dry picks
     for (int i = 0; i < (int)arranged.size(); ++i)
-        if (items[i].pool && (items[i].pool->host_res || (dry_arranged[i] && dry_arranged[i]->pool->host))) {
+        if (items[i].pool && (items[i].pool->host_res || (dry_arranged[i] && dry_arranged[i]->pool->padded()))) {
             staged.push_back(i);
             dry_describe[i] = nullptr;                  // k_stage stages the dry pick: the counts hold none (take_view)
         }
@@ -2573,6 +2716,8 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         g.n = pl->n; g.C = pl->C; g.K = pl->K; g.ws = it.win_start; g.len = it.win_len; g.sets = stage_sets(it);
         if (const ss_dry_pick* d = dry_arranged[staged[k]]) {
             g.dry = d->pool->ptrs; g.dry_pick = d->pick_dev; g.n_dry = d->pool->n; g.pair = pair_arranged[staged[k]];
+            g.i16 = d->pool->i16 ? 1 : 0;
+            p->stage16 = p->stage16 || d->pool->i16;
         }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
         char* a = p->d_desc + at;
@@ -2597,7 +2742,10 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     CK(cudaMemcpy(p->d_desc, host.data(), scr_off, cudaMemcpyHostToDevice));
     if (n_draws > 0) {
         std::vector<DrawDesc> g(n_draws);
-        for (int k = 0; k < n_draws; ++k) g[k] = draw_describe(caller_items, n_items, draws[k], dry);
+        for (int k = 0; k < n_draws; ++k) {
+            g[k] = draw_describe(caller_items, n_items, draws[k], dry);
+            for (int j = 0; j < g[k].S; ++j) p->draw16 = p->draw16 || g[k].r[g[k].spk[j]].dry16;
+        }
         CK(cudaMemcpy(p->d_desc + draw_off, g.data(), sizeof(DrawDesc) * n_draws, cudaMemcpyHostToDevice));
         p->d_draw = (const DrawDesc*)(p->d_desc + draw_off);
         p->n_draw = n_draws;
@@ -2726,8 +2874,8 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
         add_range(r, picks[k].pick_dev, 4, false);
         if (std::find(dpools.begin(), dpools.end(), picks[k].pool) == dpools.end()) dpools.push_back(picks[k].pool);
     }
-    for (const ss_dry_pool* dp : dpools)                    // (a host dry pool owns its arena: nothing a plan writes)
-        if (!dp->host)
+    for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
+        if (!dp->padded())
             for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
@@ -2747,8 +2895,8 @@ static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_ite
         const ss_pair_gains* const t = pair_gains ? pair_gains[k] : nullptr;
         // a pooled slot whose every candidate's N the dry pool's shortest signal covers, on a pool with gains only with
         // pair gains (the pool's were measured with the candidates' own x) of this pool and dry pool; a slot of a host
-        // pool only from a host dry pool, whose arena pads every signal to the whole float4s k_stage copies
-        if (!pl || (pl->host_res && !d.pool->host) || (pl->gains && !t)) return SS_ERR_INVALID;
+        // pool only from a host or 16-bit dry pool, whose arena pads every signal to the whole groups k_stage reads
+        if (!pl || (pl->host_res && !d.pool->padded()) || (pl->gains && !t)) return SS_ERR_INVALID;
         if (t && (t->pool != pl || t->dry != d.pool)) return SS_ERR_INVALID;
         for (const PoolEntry& e : pl->host) if (e.N > d.pool->n_min) return SS_ERR_INVALID;
         dry[d.slot] = &d;
@@ -2818,8 +2966,9 @@ extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
-static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, cudaStream_t stream) {
-    k_draw<<<(n + 3) / 4, 128, 0, stream>>>(d, n);
+static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, cudaStream_t stream) {
+    if (i16) k_draw<true><<<(n + 3) / 4, 128, 0, stream>>>(d, n);
+    else k_draw<false><<<(n + 3) / 4, 128, 0, stream>>>(d, n);
     CK(cudaGetLastError());
     c->launches += 1;
     return SS_OK;
@@ -2829,9 +2978,10 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, cudaStream_t stream
 // chunk's outputs) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
-    if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, stream); if (st) return st; }
+    if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, p->draw16, stream); if (st) return st; }
     if (p->n_stage) {                                   // staged slots: after the draws, before any chunk reads a slot
-        k_stage<<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
+        if (p->stage16) k_stage<true><<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
+        else k_stage<false><<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
         CK(cudaGetLastError());
         c->launches += 1;
     }

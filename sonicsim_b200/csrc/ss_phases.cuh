@@ -455,10 +455,39 @@ SS_HD int draw_start(double u, int M) {
 }
 // compute_mch_rms_dB (:29-32) of the crop [s, s + len) of a table below the threshold: silent.  D = len (mono table) or
 // C * len (channel table): the crop's element count
-SS_HD bool draw_silent(const double* Q, int s, int len, double D, float threshold_db) {
-    double ms = (Q[s + len] - Q[s]) / D;
+SS_HD bool draw_silent_sums(double q0, double q1, double D, float threshold_db) {
+    double ms = (q1 - q0) / D;
     if (ms < 1e-20) ms = 1e-20;
     return 10.0 * log10(ms) < (double)threshold_db;
+}
+SS_HD bool draw_silent(const double* Q, int s, int len, double D, float threshold_db) {
+    const double q1 = Q[s + len];
+    return draw_silent_sums(Q[s], q1, D, threshold_db);
+}
+// ---- 16-bit dry pools (ss_dry_pool_create_i16): sample k of a signal stands for k / 32768, exactly a float32.  Its
+// float32 square is a multiple of 2^-30 and at most 1, so for N <= 2^23 every partial sum of the level table is a
+// multiple of 2^-30 below 2^53 * 2^-30: exact in float64, whatever the order of the sum.  The pool keeps the table at
+// stride kLevelStride, q[j] = Q[min(64 j, N)] for j = 0..ceil(N / 64), and any Q[s] is q[s / 64] plus the exact sum of
+// the at most 63 squares behind it: bit for bit the full table's entry.
+constexpr int kLevelStride = 64;
+SS_HD float i16_sample(int16_t v) { return (float)v * (1.0f / 32768.0f); }
+// four samples of a 16-bit signal as k_stage stores them into a staging area of float32 samples
+SS_HD float4 i16x4_samples(short4 v) {
+    return make_float4(i16_sample(v.x), i16_sample(v.y), i16_sample(v.z), i16_sample(v.w));
+}
+// Q[s] (0 <= s <= N) of a 16-bit signal x from its sparse table q
+SS_HD double sparse_level(const double* q, const int16_t* x, int s) {
+    const int j = s / kLevelStride;
+    double a = q[j];
+    for (int n = j * kLevelStride; n < s; ++n) {
+        const float v = i16_sample(x[n]);
+        a += (double)(v * v);                           // the term k_levels adds
+    }
+    return a;
+}
+// draw_silent of a 16-bit dry-picked speaker (D = len)
+SS_HD bool draw_silent_i16(const double* q, const int16_t* x, int s, int len, float threshold_db) {
+    return draw_silent_sums(sparse_level(q, x, s), sparse_level(q, x, s + len), (double)len, threshold_db);
 }
 // The level table a draw tests for one speaker: a dry-picked speaker's (dry_levels non-null) is its dry pool's table of
 // the picked dry signal, whose crops have D = len; any other's is its pool's table of the picked candidate.  Both picks
@@ -467,6 +496,12 @@ SS_HD const double* speaker_table(const double* const* levels, const int* pick, 
                                   const int* dry_pick, int n_dry) {
     bool bad;
     return dry_levels ? dry_levels[clamp_pick(*dry_pick, n_dry, bad)] : levels[clamp_pick(*pick, n, bad)];
+}
+// The picked signal of a dry-picked speaker whose dry pool is 16-bit, clamped as speaker_table clamps it: such a pool's
+// device pointer array holds its n_dry signal pointers and then its n_dry table pointers, dry_levels.
+SS_HD const int16_t* speaker_signal_i16(const double* const* dry_levels, const int* dry_pick, int n_dry) {
+    bool bad;
+    return reinterpret_cast<const int16_t* const*>(dry_levels - n_dry)[clamp_pick(*dry_pick, n_dry, bad)];
 }
 
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed

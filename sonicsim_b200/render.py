@@ -95,8 +95,8 @@ class DryPick(T.NamedTuple):
     blocking unchanged - with the first N samples of that signal as its dry signal, bit for bit what render_device gives
     for the candidate with that dry signal and the same window.  A pick outside [0, n) is clamped into range
     (check_device_errors raises IndexError).  Every signal of the pool must be at least as long as the slot pool's longest
-    candidate; host pools take dry picks only from a host dry pool.  In a CropDraw, a dry-picked speaker is tested on its
-    dry crop, from the dry pool's level tables (dry_pool(..., levels=True)).  `gains`, a PairGains of the slot's pool and
+    candidate; host pools take dry picks only from a host or a 16-bit dry pool.  In a CropDraw, a dry-picked speaker is
+    tested on its dry crop, from the dry pool's level tables (dry_pool(..., levels=True)).  `gains`, a PairGains of the slot's pool and
     this dry pool (Renderer.pair_gains), stores the slot's stems at the picked pair's measured loudness gain, in place of
     the candidate's own; a pool with loudness gains takes only dry picks with `gains`."""
     pool: T.Any
@@ -320,40 +320,59 @@ class SourcePool(_Held):
 
 
 class DryPool(_Held):
-    """A set of `n` float32 dry signals on the device (Renderer.dry_pool; ss_dry_pool of the C ABI), which dry-picked
+    """A set of `n` dry signals (Renderer.dry_pool; ss_dry_pool of the C ABI), which dry-picked
     slots (DryPick) take their dry signal from at every run.  `sizes` are the signals' lengths and `n_min` the shortest:
     the longest candidate N a pool of slots that pick from it may have.  With `levels` True it holds every signal's level
     table (float64 prefix sums of its squares, 8 bytes per sample, in `nbytes`), which CropDraw reads for dry-picked
     speakers.  A device dry pool (`resident` "device") references the signals' tensors (`signals`) and keeps them alive;
     a host dry pool (`resident` "host") copied them into pinned host memory, where its level tables also stay
     (`host_nbytes`; `nbytes` then counts only its pointer arrays), and every plan run copies only the samples its slots
-    read (ss_dry_pool_host_bytes, INTEGRATION.md).  Plans hold the pool, which is freed once it is closed (or collected)
-    and no live plan uses it."""
+    read (ss_dry_pool_host_bytes, INTEGRATION.md).  A 16-bit pool (`dtype` "int16") holds every signal as its int16
+    samples k, standing for k / 32768, in an arena it owns (2 bytes per sample), and its level tables at `level_stride`
+    64 (one float64 per 64 samples); it behaves bit for bit as the float32 pool of the same values.  Plans hold the
+    pool, which is freed once it is closed (or collected) and no live plan uses it."""
     resident = "device"
+    dtype = "float32"
 
-    def __init__(self, renderer, handle, signals, sizes, levels, resident="device"):
+    def __init__(self, renderer, handle, signals, sizes, levels, resident="device", dtype="float32"):
         self.renderer, self._h = renderer, handle
         self.signals = list(signals)
         self.sizes = [int(v) for v in sizes]
-        self.n, self.levels, self.resident = len(self.sizes), bool(levels), resident
+        self.n, self.levels, self.resident, self.dtype = len(self.sizes), bool(levels), resident, dtype
         self.n_min = min(self.sizes)
         self.nbytes = int(renderer.lib.ss_dry_pool_bytes(handle))
         self.host_nbytes = int(renderer.lib.ss_dry_pool_host_bytes(handle))
+        self.level_stride = int(renderer.lib.ss_dry_pool_level_stride(handle))
+
+    def _read(self, ptr, n, typestr, ctype):
+        """A NumPy copy of n elements at `ptr`, in this pool's residency (a host address for a host pool)."""
+        import torch
+        if self.resident == "host":                        # pinned, mapped host memory: copied from the host side
+            return np.ctypeslib.as_array((ctype * n).from_address(ptr)).copy()
+
+        class _View:
+            __cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 3}
+        with torch.cuda.device(self.renderer.device):
+            return torch.as_tensor(_View(), device="cuda:%d" % self.renderer.device).cpu().numpy()
 
     def level_table(self, i):
         """A float64 CUDA copy of signal i's level table (N + 1 values: Q[0] = 0, Q[n + 1] = Q[n] + x[n]^2), or None
-        without tables."""
+        without tables.  A 16-bit pool's is rebuilt on the host from its sparse table and the signal's samples, bit for
+        bit the float32 pool's (_levels_from_sparse)."""
         import torch
         if self.closed or not self.levels or not 0 <= i < self.n:
             return None
-        ptr = self.renderer.lib.ss_dry_pool_level_table(self._h, int(i))
-        n = self.sizes[i] + 1
-        if self.resident == "host":                        # pinned, mapped host memory: copied from the host side
-            host = np.ctypeslib.as_array((ctypes.c_double * n).from_address(ptr))
-            return torch.from_numpy(host.copy()).to("cuda:%d" % self.renderer.device)
+        lib, N = self.renderer.lib, self.sizes[i]
+        ptr = lib.ss_dry_pool_level_table(self._h, int(i))
+        if self.dtype == "int16":
+            q = self._read(ptr, -(-N // self.level_stride) + 1, "<f8", ctypes.c_double)
+            x = self._read(lib.ss_dry_pool_signal_i16(self._h, int(i)), N, "<i2", ctypes.c_int16)
+            return torch.from_numpy(_levels_from_sparse(q, x)).to("cuda:%d" % self.renderer.device)
+        if self.resident == "host":
+            return torch.from_numpy(self._read(ptr, N + 1, "<f8", ctypes.c_double)).to("cuda:%d" % self.renderer.device)
 
         class _View:
-            __cuda_array_interface__ = {"shape": (n,), "typestr": "<f8", "data": (ptr, False), "version": 3}
+            __cuda_array_interface__ = {"shape": (N + 1,), "typestr": "<f8", "data": (ptr, False), "version": 3}
         with torch.cuda.device(self.renderer.device):
             return torch.as_tensor(_View(), device="cuda:%d" % self.renderer.device).clone()
 
@@ -416,6 +435,73 @@ def _pool_host_dry(dry, api, own, device, keep):
     a = np.ascontiguousarray(dry.numpy() if _is_tensor(dry) else dry, dtype=np.float32)
     if a.ndim != 1 or a.size < 1:
         raise ValueError("%s: dry of %s must be 1-D and not empty, got shape %s" % (api, own, a.shape))
+    keep.append(a)
+    return a.ctypes.data, a.size
+
+
+I16_MAX_SAMPLES = 1 << 23                  # a 16-bit dry signal's longest (ss_dry_pool_create_i16)
+I16_STRIDE = 64                            # its level tables' stride
+
+
+def _levels_from_sparse(q, x):
+    """The full level table (N + 1 float64) of a 16-bit signal x (N int16 samples, k standing for k / 32768) from its
+    sparse table q (q[j] = Q[min(64 j, N)]): Q[s] = q[s // 64] plus the float64 sum of the float32 squares of samples
+    [64 (s // 64), s).  Every partial sum is a multiple of 2^-30 below 2^23, exact in float64, so the result is the
+    float32 pool's table bit for bit whatever the order of the sums."""
+    N = x.size
+    m = -(-N // I16_STRIDE)
+    v = x.astype(np.float32) * np.float32(1.0 / 32768.0)
+    sq = np.zeros(m * I16_STRIDE, np.float64)
+    sq[:N] = (v * v).astype(np.float64)                # the float32 square k_levels adds
+    blocks = sq.reshape(m, I16_STRIDE)
+    part = np.cumsum(blocks, axis=1) - blocks          # exclusive, within each block
+    Q = np.empty(N + 1, np.float64)
+    Q[:N] = (q[:m, None] + part).reshape(-1)[:N]
+    Q[N] = q[m]
+    return Q
+
+
+def _as_i16(x, own, device, keep):
+    """(pointer, N) of a signal for a 16-bit dry pool: an int16 NumPy array or CPU / CUDA tensor, or a float one whose
+    every sample is exactly k / 32768 with -32768 <= k <= 32767 (converted; the first sample off that grid is named).
+    Anything else - other dtypes, a sample off the grid or +1.0, an empty or longer than 2^23 signal - is a ValueError.
+    Converted or host arrays are kept alive in `keep`; a CUDA tensor must be on cuda:`device`."""
+    tensor = _is_tensor(x)
+    cuda = tensor and x.is_cuda
+    if cuda and x.device.index != device:
+        raise ValueError("dry_pool: %s is on cuda:%s, the renderer on cuda:%d" % (own, x.device.index, device))
+    a = x if cuda else x.numpy() if tensor else np.asarray(x)
+    if a.ndim != 1 or a.shape[0] < 1 or a.shape[0] > I16_MAX_SAMPLES:
+        raise ValueError("dry_pool: %s must be 1-D with 1 to 2^23 samples for dtype int16, got shape %s"
+                         % (own, tuple(a.shape)))
+    if cuda:
+        import torch
+        if a.dtype == torch.int16:
+            a = a.contiguous()
+        elif a.dtype.is_floating_point:
+            k = a.double() * 32768.0
+            bad = ~((k == torch.floor(k)) & (k >= -32768.0) & (k <= 32767.0))   # (NaN and inf fail too)
+            if bool(bad.any()):
+                j = int(torch.nonzero(bad)[0, 0])
+                raise ValueError("dry_pool: %s has sample %d = %r, not k / 32768 with k an int16"
+                                 % (own, j, float(a[j])))
+            a = k.to(torch.int16)
+        else:
+            raise ValueError("dry_pool: %s must be int16 or float on the int16 grid, got %s" % (own, a.dtype))
+        keep.append(a)
+        return a.data_ptr(), a.numel()
+    if a.dtype == np.int16:
+        a = np.ascontiguousarray(a)
+    elif np.issubdtype(a.dtype, np.floating):
+        k = a.astype(np.float64) * 32768.0
+        with np.errstate(invalid="ignore"):
+            bad = ~((k == np.floor(k)) & (k >= -32768.0) & (k <= 32767.0))
+        if bad.any():
+            j = int(np.argmax(bad))
+            raise ValueError("dry_pool: %s has sample %d = %r, not k / 32768 with k an int16" % (own, j, float(a[j])))
+        a = k.astype(np.int16)
+    else:
+        raise ValueError("dry_pool: %s must be int16 or float on the int16 grid, got %s" % (own, a.dtype))
     keep.append(a)
     return a.ctypes.data, a.size
 
@@ -662,7 +748,8 @@ class Renderer:
                           post is not None)
 
     # ------------------------------------------------------------------ dry pools
-    def dry_pool(self, signals: T.Sequence[T.Any], levels: bool = False, host: bool = False) -> DryPool:
+    def dry_pool(self, signals: T.Sequence[T.Any], levels: bool = False, host: bool = False,
+                 dtype: str = "float32") -> DryPool:
         """A DryPool over `signals`: 1 to 2^24 contiguous 1-D CUDA float32 tensors of this renderer's device, referenced
         (not copied) and kept alive by the pool, for dry-picked pooled slots (DryPick) of device plans.  `levels` also
         builds every signal's level table, which start draws (CropDraw) test dry-picked speakers with; the call then
@@ -671,14 +758,30 @@ class Renderer:
         With `host` True the pool is host-resident (`resident` "host"): the signals, which may also be 1-D NumPy arrays
         or CPU tensors, are copied into pinned host memory at once and not held, the level tables stay there too, and
         every plan run copies only the samples its dry-picked slots' crops read to the device.  Slots of host source
-        pools take dry picks only from a host dry pool."""
+        pools take dry picks only from a host or a 16-bit dry pool.
+
+        With `dtype` "int16" the pool is 16-bit: every signal, an int16 NumPy array or CPU / CUDA tensor, or a float one
+        whose every sample is exactly k / 32768 (-32768 <= k <= 32767; 16-bit PCM as torchaudio or soundfile load it),
+        of 1 to 2^23 samples, is copied as its int16 samples into an arena the pool owns (device memory, or pinned host
+        memory with `host`), and its level tables are kept at one entry per 64 samples.  The pool renders, draws and
+        measures bit for bit as the float32 pool of the same values, and serves slots of host source pools too."""
         import torch
         n = len(signals)
         if not 1 <= n <= 1 << 24:
             raise ValueError("dry_pool: a dry pool holds 1 to 2^24 signals, got %d" % n)
+        if dtype not in ("float32", "int16"):
+            raise ValueError("dry_pool: dtype must be \"float32\" or \"int16\", got %r" % (dtype,))
         ptrs = (ctypes.c_void_p * n)()
         lengths = np.empty(n, np.int32)
         keep = []
+        if dtype == "int16":
+            for i, x in enumerate(signals):
+                ptrs[i], lengths[i] = _as_i16(x, "signal %d" % i, self.device, keep)
+            torch.cuda.current_stream(self.device).synchronize()   # copied on the library's own streams
+            flags = (_lib.SS_DRY_LEVELS if levels else 0) | (_lib.SS_DRY_HOST if host else 0)
+            h = ctypes.c_void_p()
+            _lib.check(self.lib.ss_dry_pool_create_i16(self.ctx, ptrs, lengths.ctypes.data, n, flags, ctypes.byref(h)))
+            return DryPool(self, h, [], lengths, levels, "host" if host else "device", "int16")
         for i, x in enumerate(signals):
             own = "signal %d" % i
             if host:                                       # copied into the pool: NumPy, CPU or CUDA tensors
@@ -891,7 +994,7 @@ class Renderer:
             _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
             pl = s.pool
             if isinstance(pl, SourcePool):
-                if pl.resident == "host" and d.pool.resident == "device":
+                if pl.resident == "host" and d.pool.resident == "device" and d.pool.dtype == "float32":
                     raise ValueError("plan_device: pooled source %d has a dry pick over a host pool, whose runs stage "
                                      "each candidate's own dry signal" % i)
                 if pl.gains and d.gains is None:
