@@ -186,6 +186,27 @@ void ss_bank_destroy(ss_bank* bank);          /* destroy banks before their cont
 #define SS_BANK_HOST 0x100
 int64_t ss_bank_host_bytes(const ss_bank* bank);   /* pinned host bytes held */
 
+/* ---- tap-form host banks: `flags` may add SS_BANK_TAPS together with SS_BANK_HOST (without it the create calls return
+ * SS_ERR_INVALID before any allocation); it combines with SS_RIR_NORMALIZE and SS_DIRECT_TARGET as the spectral form
+ * does.  Such a bank keeps the taps instead of their spectra: pinned, mapped host memory holds P * C * K rows of 4096
+ * float32, row (p * C + c) * K + part at float offset row * 4096 holding taps [part * 4096, part * 4096 + 4096) of RIR
+ * (p, c), zero past L, then the cut table as in a spectral host bank.  With SS_RIR_NORMALIZE the stored taps are the
+ * IEEE quotients h / m, m the abs-max of the whole RIR tensor (k_rir_absmax), and the raw taps when m == 0.  The build runs
+ * k_rir_absmax and k_rir_direct as for a spectral bank, then writes the rows; nothing is transformed.
+ * ss_bank_host_bytes = 16384 * P * C * K plus 4 * P * C with a direct set (half a spectral host bank's bytes, a quarter
+ * with a direct set); ss_bank_bytes is 0.  A tap-form bank serves only as a candidate of a host pool whose banks are all
+ * tap-form (a pool that mixes forms is SS_ERR_INVALID).  Such a pool stages, at every run, the rows [row0, row0 + rows)
+ * of its slots' read sets as rows * 16 KB - one set whatever the slot's direct target - instead of sets * rows * 32 KB of
+ * spectra, and one more kernel per run, a k_prepare launch behind k_stage and before any chunk, transforms them on the
+ * device into the staging area's spectra, rows paired (2r, 2r + 1) as a bank build pairs them.
+ * Bit contract: a plan over tap-form host pools gives the bits of the same plan over spectral host pools of the same RIRs
+ * - and so of device pools - in stems, direct stems, mixtures, speakers_out, rms_db, drawn starts, `used` and
+ * ss_device_errors, for dry picks and pair gains too; level tables, loudness results and pair gains are identical.  The
+ * transform loads the values a spectral build loads (pre-divided taps, zeros past L for its zero fill, direct rows cut at
+ * the same cut[p, c]), through the same code.  ss_version stays 108: ss_bank_flags marks the capability. */
+#define SS_BANK_TAPS 0x200
+int32_t ss_bank_flags(const ss_bank* bank);        /* the flags the bank was created with (0 for NULL) */
+
 /* ---- source pools (version 106): the dataloader's random choices of separation/look2hear/datas/movingdatamodule.py
  * :57-59 (`random.choice(self.data_dirs)`, `random.sample(range(1, 4), num_spks)`) and :68-77 (the scene's noise) made
  * on the device.  A pool is a set of banked candidate sources, validated and uploaded once.  A pooled slot of a plan

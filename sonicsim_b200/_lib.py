@@ -21,6 +21,7 @@ SS_OK, SS_ERR_INVALID, SS_ERR_INDEX, SS_ERR_CUDA, SS_ERR_NOMEM, SS_ERR_UNSUPPORT
 SS_STATIC, SS_MOVING_BOUNDS, SS_MOVING_INDEXED = 0, 1, 2
 SS_RIR_NORMALIZE, SS_DIRECT_TARGET = 1, 2
 SS_BANK_HOST = 0x100
+SS_BANK_TAPS = 0x200
 SS_MIX_MONO = 1
 SS_DRY_LEVELS = 1
 SS_DRY_HOST = 0x100
@@ -163,6 +164,7 @@ def load():
         lib.ss_bank_bytes.restype = i64
         lib.ss_bank_host_bytes.argtypes = [vp]
         lib.ss_bank_host_bytes.restype = i64
+        lib.ss_bank_flags.argtypes = [vp]
         lib.ss_bank_destroy.argtypes = [vp]
         lib.ss_bank_destroy.restype = None
         lib.ss_pool_create.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(vp)]
@@ -229,7 +231,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_host_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_dry_pool_create_i16", "ss_dry_pool_level_stride", "ss_dry_pool_signal_i16", "ss_plan_create_dry", "ss_pair_gains_create", "ss_pair_gains_bytes", "ss_pair_gains_destroy", "ss_plan_create_pair", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_flags", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_host_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_dry_pool_create_i16", "ss_dry_pool_level_stride", "ss_dry_pool_signal_i16", "ss_plan_create_dry", "ss_pair_gains_create", "ss_pair_gains_bytes", "ss_pair_gains_destroy", "ss_plan_create_pair", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

@@ -792,7 +792,8 @@ extern "C" void ss_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 // RIR spectrum bank: one device allocation = [reverberant set | direct set] (P*C*K rows of kSpec float2 each, the layout
 // k_prepare writes into chunk scratch) | cut table (direct set) | descriptor of the blockless source that built it |
-// its norm_part slots (SS_RIR_NORMALIZE).  A host bank's block (SS_BANK_HOST) is [spectra | cut table], unpadded.
+// its norm_part slots (SS_RIR_NORMALIZE).  A host bank's block (SS_BANK_HOST) is [spectra | cut table], unpadded; a
+// tap-form host bank (SS_BANK_TAPS) holds the padded tap rows (tap_value) in place of the spectra, in both places.
 struct ss_bank {
     ss_ctx* c = nullptr;                  // the context that made it; sources of other contexts are refused
     char* d_mem = nullptr;
@@ -808,6 +809,9 @@ struct ss_bank {
     size_t set_bytes() const { return (size_t)P * C * K * kSpec * sizeof(float2); }
     size_t spec_bytes() const { return ((flags & SS_DIRECT_TARGET) ? 2 : 1) * set_bytes(); }
     size_t cut_bytes() const { return (flags & SS_DIRECT_TARGET) ? sizeof(int) * (size_t)P * C : 0; }
+    // SS_BANK_TAPS: the P*C*K rows of kB taps, one set whatever the flags (`spec` then holds their address)
+    size_t tap_bytes() const { return (size_t)P * C * K * kB * sizeof(float); }
+    size_t head_bytes() const { return (flags & SS_BANK_TAPS) ? tap_bytes() : spec_bytes(); }   // in front of the cuts
 };
 // Source pool: the candidates' compact entries in one device allocation, and on the host what validation, sizing and the
 // mixture range checks need.
@@ -839,6 +843,7 @@ struct ss_pool {
     // host pool (every candidate's bank has SS_BANK_HOST): x in one pinned, mapped arena (host[i].x: its device address);
     // the device copies of the bounds and cut tables in one device allocation (host[i].bounds / cut point into it)
     bool host_res = false;
+    bool taps = false;                    // a host pool of tap-form banks (SS_BANK_TAPS): entries' spec hold tap rows
     char* h_x = nullptr;
     size_t h_x_bytes = 0;
     int* d_aux = nullptr;
@@ -1352,14 +1357,23 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, b
 // chunk scratch.  Its spectra therefore have the bits a render would transform itself.
 static int bank_args(const ss_ctx* c, const float* rir, int P, int C, int L, int flags, int direct_taps, ss_bank** out) {
     if (!c || !rir || !out || P < 1 || C < 1 || L < 1) return SS_ERR_INVALID;
-    if (flags & ~(SS_RIR_NORMALIZE | SS_DIRECT_TARGET | SS_BANK_HOST)) return SS_ERR_INVALID;
+    if (flags & ~(SS_RIR_NORMALIZE | SS_DIRECT_TARGET | SS_BANK_HOST | SS_BANK_TAPS)) return SS_ERR_INVALID;
+    if ((flags & SS_BANK_TAPS) && !(flags & SS_BANK_HOST)) return SS_ERR_INVALID;     // tap rows: host banks only
     if ((flags & SS_DIRECT_TARGET) && direct_taps < 1) return SS_ERR_INVALID;
     if ((int64_t)P * C * ((L + kB - 1) / kB) > (int64_t)1 << 28) return SS_ERR_UNSUPPORTED;    // as validate_item
     return SS_OK;
 }
+// SS_BANK_TAPS: the n = P*C*K * kB stored taps (tap_value) from bank_build's blockless source, after k_rir_absmax
+__global__ void __launch_bounds__(256) k_bank_taps(const Source* __restrict__ src, float* __restrict__ taps, long long n) {
+    const Source& S = *src;
+    const float m = S.norm_part ? rir_absmax(S) : 0.f;
+    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x)
+        taps[q] = tap_value(S, (int)(q / kB), (int)(q % kB), m);
+}
 static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stream) {
     const bool direct = (b->flags & SS_DIRECT_TARGET) != 0, norm = (b->flags & SS_RIR_NORMALIZE) != 0;
-    const size_t spec_b = b->spec_bytes(), cut_b = align_up(b->cut_bytes(), 256);
+    const bool taps = (b->flags & SS_BANK_TAPS) != 0;
+    const size_t spec_b = b->head_bytes(), cut_b = align_up(b->cut_bytes(), 256);
     const size_t src_b = align_up(sizeof(Source), 256);
     b->bytes = spec_b + cut_b + src_b + (norm ? 512 : 0);
     CK(cudaMalloc((void**)&b->d_mem, b->bytes));
@@ -1377,20 +1391,26 @@ static int bank_build(ss_ctx* c, ss_bank* b, const float* rir, cudaStream_t stre
     if (direct) { s.cut = b->cut; s.direct_taps = b->direct_taps; }
     static thread_local ChunkLaunch L;                  // kernel parameters, as in launch_chunk
     L = ChunkLaunch();
-    L.n = 1; L.ps = spectra_pairs_h(s); L.grid_r = 0; L.n_known = 0;
+    L.n = 1; L.ps = taps ? 0 : spectra_pairs_h(s); L.grid_r = 0; L.n_known = 0;   // (tap rows: no transform)
     L.any_norm = norm; L.grid_direct = direct ? (s.P * s.C + 7) / 8 : 0;
     L.ds = d_src;
     L.pp.n_inline = 1; L.pp.prefix[0] = 0; L.pp.prefix[1] = L.ps; L.pp.srcs[0] = s;
     CK(cudaEventCreateWithFlags(&b->ready, cudaEventDisableTiming));
     CK(cudaMemcpyAsync(d_src, &s, sizeof(s), cudaMemcpyHostToDevice, stream));  // k_rir_absmax / k_rir_direct read it
     { int st = chunk_enqueue(c, L, stream, false); if (st) return st; }
+    if (taps) {
+        const long long n = (long long)b->P * b->C * b->K * kB;
+        k_bank_taps<<<(unsigned)std::min(n / 256, (long long)c->sm_count * 8), 256, 0, stream>>>(d_src, (float*)b->spec, n);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
     CK(cudaEventRecord(b->ready, stream));
     return SS_OK;
 }
-// SS_BANK_HOST: the built spectra and cut table into pinned, mapped host memory, then the device buffer freed.  Returns
-// when the bank is in host memory.
+// SS_BANK_HOST: the built spectra (SS_BANK_TAPS: tap rows) and cut table into pinned, mapped host memory, then the
+// device buffer freed.  Returns when the bank is in host memory.
 static int bank_to_host(ss_bank* b, cudaStream_t stream) {
-    const size_t spec_b = b->spec_bytes(), cut_b = b->cut_bytes();
+    const size_t spec_b = b->head_bytes(), cut_b = b->cut_bytes();
     CK(cudaHostAlloc((void**)&b->h_mem, spec_b + cut_b, cudaHostAllocMapped | cudaHostAllocPortable));
     b->host_bytes = spec_b + cut_b;
     CK(cudaMemcpyAsync(b->h_mem, b->spec, spec_b, cudaMemcpyDeviceToHost, stream));
@@ -1418,6 +1438,7 @@ extern "C" void ss_bank_destroy(ss_bank* b) {
 }
 extern "C" int64_t ss_bank_bytes(const ss_bank* b) { return b ? (int64_t)b->bytes : 0; }
 extern "C" int64_t ss_bank_host_bytes(const ss_bank* b) { return b ? (int64_t)b->host_bytes : 0; }
+extern "C" int32_t ss_bank_flags(const ss_bank* b) { return b ? b->flags : 0; }
 
 extern "C" int ss_bank_create_dev(ss_ctx* c, const float* rir, int32_t P, int32_t C, int32_t L, int32_t flags,
                                   int32_t direct_taps, void* stream, ss_bank** out) {
@@ -1531,7 +1552,7 @@ static int pool_host_copies(ss_pool* pl, const ss_source* cand) {
         const ss_bank* b = cand[i].rir_bank;
         int* a = aux.data() + ao[i];
         if (pl->mode == SS_MOVING_BOUNDS) { memcpy(a, cand[i].bounds_host, sizeof(int) * (size_t)cand[i].P); a += cand[i].P; }
-        if (b->cut) memcpy(a, b->h_mem + b->spec_bytes(), b->cut_bytes());
+        if (b->cut) memcpy(a, b->h_mem + b->head_bytes(), b->cut_bytes());
         CK(cudaMemcpy(pl->h_x + xo[i], cand[i].x, sizeof(float) * (size_t)cand[i].N, cudaMemcpyDefault));
     }
     pl->aux_bytes = sizeof(int) * std::max(ao[n], (size_t)1);
@@ -1607,11 +1628,13 @@ extern "C" int ss_pool_create(ss_ctx* c, const ss_source* cand, int n, ss_pool**
         if (st) return st;
         if (cand[i].mode != cand[0].mode || cand[i].C != cand[0].C) return SS_ERR_INVALID;   // any L
         if (!cand[i].rir_bank->h_mem != !cand[0].rir_bank->h_mem) return SS_ERR_INVALID;  // host and device banks
+        if ((cand[i].rir_bank->flags ^ cand[0].rir_bank->flags) & SS_BANK_TAPS) return SS_ERR_INVALID;   // two forms
     }
     CK(cudaSetDevice(c->device));
     ss_pool* pl = new (std::nothrow) ss_pool();
     if (!pl) return SS_ERR_NOMEM;
     pl->c = c; pl->n = n; pl->host_res = cand[0].rir_bank->h_mem != nullptr;
+    pl->taps = (cand[0].rir_bank->flags & SS_BANK_TAPS) != 0;
     const int st = pool_build(pl, cand);
     if (st != SS_OK) { ss_pool_destroy(pl); return st; }
     *out = pl;
@@ -1851,9 +1874,12 @@ static StemGroups stem_groups(const StemSet& S) {
 // Copied stems [first, first + n) (items, rendered whole): a host pool's reverberant spectra - once per run of
 // consecutive stems of one candidate - and every stem's dry signal copied into transient device memory and rendered from
 // there, in batches of at most kLevelStemBytes of copies (or one stem's, when larger), each behind the previous batch's
-// render on `s`.  `buf` holds `cap` = stem_copy_cap bytes.
+// render on `s`.  `buf` holds `cap` = stem_copy_cap bytes.  A tap-form pool's candidate is copied as its tap rows and
+// rendered as a whole source with those RIRs (L = K * 4096, no flags): k_prepare then transforms the rows bank_build
+// transforms for a spectral bank of the same RIRs, paired alike, into the same spectra.
 static size_t stem_bank_bytes(const StemSet& S, size_t k) {
-    return S.pl->host_res ? align_up(S.pl->banks[S.stems[k].cand]->set_bytes(), 256) : 0;
+    const ss_bank* b = S.pl->banks[S.stems[k].cand];
+    return S.pl->host_res ? align_up(S.pl->taps ? b->tap_bytes() : b->set_bytes(), 256) : 0;
 }
 static size_t stem_x_bytes(const StemSet& S, size_t k) { return align_up(sizeof(float) * (size_t)S.N(k), 256); }
 static bool stem_new_bank(const StemSet& S, size_t k, bool batch_start) {
@@ -1874,11 +1900,17 @@ static int render_copied_stems(const StemSet& S, ss_source* items, int first, in
         size_t used = 0;
         int hi = lo;
         const ss_bank* shell = nullptr;
+        const float* taps = nullptr;                    // (a tap-form pool) the candidate's copied rows
         for (; hi < n; ++hi) {
             const size_t k = (size_t)(first + hi);
             const bool new_bank = stem_new_bank(S, k, hi == lo);
             if (hi > lo && used + (new_bank ? stem_bank_bytes(S, k) : 0) + stem_x_bytes(S, k) > cap) break;
-            if (new_bank) {
+            if (new_bank && S.pl->taps) {
+                const ss_bank* b = S.pl->banks[S.stems[k].cand];
+                taps = (const float*)(buf + used);
+                CK(cudaMemcpyAsync(buf + used, b->spec, b->tap_bytes(), cudaMemcpyDefault, s));
+                used += stem_bank_bytes(S, k);
+            } else if (new_bank) {
                 const ss_bank* b = S.pl->banks[S.stems[k].cand];
                 ss_bank& sh = shells[hi];
                 sh = *b;                                // the bank's shape and `ready`, spectra from the copy
@@ -1896,7 +1928,11 @@ static int render_copied_stems(const StemSet& S, ss_source* items, int first, in
             }
             used += stem_x_bytes(S, k);
             items[hi].x = x;
-            if (S.pl->host_res) items[hi].rir_bank = shell;
+            if (S.pl->taps) {
+                items[hi].rir = taps; items[hi].rir_bank = nullptr; items[hi].L = S.pl->banks[S.stems[k].cand]->K * kB;
+            } else if (S.pl->host_res) {
+                items[hi].rir_bank = shell;
+            }
         }
         const int st = ss_render_dev(S.pl->c, items + lo, hi - lo, (void*)s);   // the next batch's copies wait on `s`
         if (st) return st;
@@ -2422,6 +2458,12 @@ struct ss_plan {
     const StageSlot* d_stage = nullptr;   // the staged slots' k_stage descriptors, in d_desc behind the draws
     int n_stage = 0;
     bool draw16 = false, stage16 = false; // a draw speaker / a staged slot has a 16-bit dry pick: k_draw<true> / k_stage<true>
+    // slots of tap-form pools: k_stage<I16, true> reads d_taps (n_stage entries) and writes n_tap transform Sources
+    // (d_tap_src, CTA ranges d_tap_prefix), which one k_prepare<false> of tap_ctas CTAs transforms behind it
+    const StageTap* d_taps = nullptr;
+    const Source* d_tap_src = nullptr;
+    const int* d_tap_prefix = nullptr;
+    int n_tap = 0, tap_ctas = 0;
 };
 
 // ----------------------------------------------------------------------------- k_draw
@@ -2540,9 +2582,13 @@ static_assert(sizeof(StageSlot) == 120, "StageSlot layout");
 // k_stage<true> (a plan with a 16-bit dry pick) reads such a slot's dry samples as 4 int16 at a time from the whole
 // groups [xa & ~3, (xb + 3) & ~3) of the picked signal (inside its padded arena) and stores their exact float32 values,
 // so that the staging area holds what a float pool's slot stages.
-template <bool I16>
-__global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots) {
+// k_stage<I16, true> (a plan with a slot of a tap-form pool) copies such a slot's tap rows [row0, row0 + rows), one
+// contiguous span of the candidate's rows, instead of sets * rows spectra rows, and writes the Source over them that the
+// plan's transform launch (k_prepare<false>) turns into the spectra the slot's view names: those k_stage<I16> copies.
+template <bool I16, bool TAPS = false>
+__global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots, const StageTap* __restrict__ taps) {
     const StageSlot& g = slots[blockIdx.y];
+    const StageTap* const tp = TAPS && taps[blockIdx.y].taps ? &taps[blockIdx.y] : nullptr;
     __shared__ StageView s_v;
     __shared__ const float* s_src;                      // the signal the dry samples come from
     __shared__ int s_x[2];                              // dry samples copied: whole float4s [s_x[0], s_x[1])
@@ -2557,7 +2603,7 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
     const size_t nx4 = (size_t)((s_x[1] - s_x[0]) >> 2);
     const size_t per_set = (size_t)s_v.rows * (kSpec / 2);          // float4s per set
     const size_t rows_h = (size_t)e.P * g.C * s_v.K;                 // rows per set of the bank
-    const size_t total = nx4 + (size_t)g.sets * per_set;
+    const size_t total = nx4 + (TAPS && tp ? (size_t)s_v.rows * (kB / 4) : (size_t)g.sets * per_set);
     const float4* const xs = reinterpret_cast<const float4*>(s_src + s_x[0]);
     const short4* const xs16 = I16 && g.i16 ? reinterpret_cast<const short4*>(reinterpret_cast<const int16_t*>(s_src) + s_x[0])
                                             : nullptr;
@@ -2572,6 +2618,12 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
             dst[u] = nullptr;
             if (q >= total) continue;
             if (q < nx4) { v[u] = I16 && xs16 ? i16x4_samples(xs16[q]) : xs[q]; dst[u] = xd + q; continue; }
+            if (TAPS && tp) {
+                const size_t j = q - nx4;
+                v[u] = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(e.spec) + (size_t)s_v.row0 * kB)[j];
+                dst[u] = reinterpret_cast<float4*>(tp->taps) + j;
+                continue;
+            }
             const size_t j = q - nx4, set = j / per_set;
             v[u] = reinterpret_cast<const float4*>(e.spec + (set * rows_h + s_v.row0) * kSpec)[j - set * per_set];
             dst[u] = reinterpret_cast<float4*>(g.spec) + j;
@@ -2584,6 +2636,9 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
         w.e.x = g.x - s_x[0];                           // biased: sample n at x[n] (Source::x)
         if (g.sets) w.e.spec = g.spec;                  // (a device pool's slot keeps its bank's spectra)
         *g.view = w;
+        if (TAPS && tp)
+            *tp->src = tap_source(tp->taps, g.spec, g.sets > 1 ? e.cut : nullptr, e.P, g.C, s_v.K, s_v.row0, s_v.rows,
+                                  tp->zero);
     }
 }
 
@@ -2653,10 +2708,10 @@ static std::pair<int, int> stage_cap(ss_pool* pl, int win_len) {
 }
 // (spectra sets it stages: direct_sets for a slot of a host pool, 0 for a slot of a device pool, which stages dry samples only)
 static int stage_sets(const ss_source& it) { return it.pool->host_res ? direct_sets(it) : 0; }
-static size_t stage_bytes(const ss_source& it) {
+// A slot's staging area (stage_area): view | spectra | dry samples | (a slot of a tap-form pool) tap rows
+static StageArea stage_area_of(const ss_source& it) {
     const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(it.pool), it.win_len);
-    return align_up(sizeof(StageView), 256) + align_up((size_t)stage_sets(it) * cap.first * kSpec * sizeof(float2), 256) +
-           align_up(sizeof(float) * (size_t)cap.second, 256);
+    return stage_area(stage_sets(it), cap.first, cap.second, it.pool->taps);
 }
 
 // (dry[i]: caller item i's dry pick, or null; pair[i]: its pair gains' device table, or null)
@@ -2700,8 +2755,13 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     if (staged.size() > 65535) return SS_ERR_UNSUPPORTED;   // one gridDim.y row of k_stage per slot
     const size_t stage_off = align_up(desc_bytes, 256), area_off = align_up(stage_off + sizeof(StageSlot) * staged.size(), 256);
     size_t total = area_off;
-    for (int i : staged) total += stage_bytes(items[i]);
+    int n_tap = 0;
+    for (int i : staged) { total += stage_area_of(items[i]).end; n_tap += items[i].pool->taps ? 1 : 0; }
+    const TapBlock tb = tap_block(total, (int)staged.size(), n_tap);   // (slots of tap-form pools)
+    const size_t tap_off = tb.taps, tsrc_off = tb.src, tpre_off = tb.prefix, zero_off = tb.zero;
+    if (n_tap) total = tb.end;
     CK(cudaMalloc((void**)&p->d_desc, total + 256));
+    std::vector<char> tap_host(n_tap ? total - tap_off : 0, 0);
     for (int i = 0; i < ss_ctx::kAux; ++i)
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
     std::vector<char> host(desc_bytes + 256);
@@ -2720,12 +2780,29 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
             p->stage16 = p->stage16 || d->pool->i16;
         }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
-        char* a = p->d_desc + at;
-        g.view = (StageView*)a; a += align_up(sizeof(StageView), 256);
-        g.spec = g.sets ? (float2*)a : nullptr; a += align_up((size_t)g.sets * cap.first * kSpec * sizeof(float2), 256);
-        g.x = (float*)a;
-        at += stage_bytes(it);
+        const StageArea sa = stage_area_of(it);
+        char* const a = p->d_desc + at;
+        g.view = (StageView*)(a + sa.view);
+        g.spec = g.sets ? (float2*)(a + sa.spec) : nullptr;
+        g.x = (float*)(a + sa.x);
+        at += sa.end;
         views[staged[k]] = g.view;
+        if (pl->taps) {                                 // its tap rows, transform Source and CTA range
+            const int t = p->n_tap++;
+            StageTap& q = ((StageTap*)tap_host.data())[k];
+            q.taps = (float*)(a + sa.taps);
+            q.src = (Source*)(p->d_desc + tsrc_off) + t;
+            q.zero = (int*)(p->d_desc + zero_off);
+            int* const prefix = (int*)(tap_host.data() + (tpre_off - tap_off));
+            prefix[t + 1] = prefix[t] + g.sets * ((cap.first + 1) >> 1);   // pairs of the most rows any run stages
+        }
+    }
+    if (n_tap) {
+        p->tap_ctas = ((const int*)(tap_host.data() + (tpre_off - tap_off)))[n_tap];
+        CK(cudaMemcpy(p->d_desc + tap_off, tap_host.data(), tap_host.size(), cudaMemcpyHostToDevice));
+        p->d_taps = (const StageTap*)(p->d_desc + tap_off);
+        p->d_tap_src = (const Source*)(p->d_desc + tsrc_off);
+        p->d_tap_prefix = (const int*)(p->d_desc + tpre_off);
     }
     p->chunks.resize(n_chunks);
     for (size_t k = 0; k < n_chunks; ++k)
@@ -2980,8 +3057,18 @@ static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
     if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, p->draw16, stream); if (st) return st; }
     if (p->n_stage) {                                   // staged slots: after the draws, before any chunk reads a slot
-        if (p->stage16) k_stage<true><<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
-        else k_stage<false><<<dim3(kStageCtas, p->n_stage), 256, 0, stream>>>(p->d_stage);
+        const dim3 grid(kStageCtas, p->n_stage);
+        if (p->n_tap && p->stage16) k_stage<true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
+        else if (p->n_tap) k_stage<false, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
+        else if (p->stage16) k_stage<true><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);
+        else k_stage<false><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
+    if (p->n_tap) {                                     // the staged tap rows into the spectra the slots' views name
+        static const PrepParams global_tables = {};     // (n_inline = 0: the Sources k_stage wrote, from global memory)
+        k_prepare<false><<<p->tap_ctas, kThreads, kPadF * (int)sizeof(float2), stream>>>(
+            p->d_tap_src, p->d_tap_prefix, p->n_tap, nullptr, global_tables);
         CK(cudaGetLastError());
         c->launches += 1;
     }

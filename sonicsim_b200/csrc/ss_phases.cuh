@@ -689,6 +689,65 @@ SS_HD PeakAt peak_scan(const float* h, int L, float div, int lane, int nlanes) {
 }
 SS_HD int direct_cut(int peak, int L, int taps) { return peak < L - taps ? peak + taps : L; }   // min(L, peak + taps)
 
+// ---- tap-form host banks (SS_BANK_TAPS, include/sonicsim_b200.h): a host bank that keeps each candidate's RIR taps as
+// P*C*K rows of kB floats, row (p * C + c) * K + part holding taps [part * kB, part * kB + kB) of RIR (p, c), zero past
+// L.  Tap j of row `row` as k_bank_taps stores it from bank_build's blockless source S (m: rir_absmax(S) of a normalised
+// bank, else 0): divided as spectra_phase1 divides its row loads, never when m == 0, so that k_prepare over the stored
+// rows without norm_part loads the values it loads over S with it - make_row's zero fill past L included (0 / m = +0).
+SS_HD float tap_value(const Source& S, int row, int j, float m) {
+    const int pc = row / S.K, t = (row % S.K) * kB + j;
+    if (t >= S.L) return 0.f;
+    const float h = S.rir[(size_t)pc * S.L + t];
+    return m != 0.f ? div_rn(h, m) : h;
+}
+// The Source k_prepare's RIR CTAs transform a tap slot's staged rows [row0, row0 + rows) with: bank_build's blockless
+// source over the stored rows (L = K * kB, so row r starts at rir + r * kB; rir biased: row r of the bank at
+// staged + (r - row0) * kB), windowed onto the staged rows, which land in `spec` with set stride `rows` - the layout
+// k_stage copies a spectral bank's rows into.  cut: the candidate's cut table for a slot with a direct stem, else null.
+// `zero` is a zero word: CTAs past this run's spectra_pairs_h read counts[0] == 0 and return.
+SS_HD Source tap_source(const float* staged, float2* spec, int* cut, int P, int C, int K, int row0, int rows,
+                        int* zero) {
+    Source s{};
+    s.rir = staged - (ptrdiff_t)row0 * kB; s.N = 1; s.P = P; s.C = C; s.L = K * kB; s.K = K; s.nb = 1;
+    s.mode = P == 1 ? MODE_STATIC : MODE_MOVING_BOUNDS;
+    s.hspec = spec; s.cut = cut; s.counts = zero;
+    s.h_row0 = row0; s.h_rows = rows;
+    return s;
+}
+// What a slot of a tap-form pool stages besides its StageSlot (ss_kernels.cu), at the same index (k_stage<I16, true>):
+struct StageTap {
+    float* taps;                      // the staging area's tap rows (rows_cap * 4096 floats), or null: not a tap slot
+    Source* src;                      // its transform Source (tap_source), written by CTA 0 at every run
+    int* zero;                        // a zero word, the Source's counts
+};
+// A staged slot's area in a plan's descriptor allocation, every region at a 256-byte boundary from the area's start: its
+// StageView, `sets` sets of rows_cap spectra rows, nx dry samples and, for a slot of a tap-form pool (taps), rows_cap
+// rows of taps - the rows its transform turns into those spectra.  `end` is the area's size.
+struct StageArea { size_t view, spec, x, taps, end; };
+SS_HD size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+SS_HD StageArea stage_area(int sets, int rows_cap, int nx, bool taps) {
+    StageArea a;
+    a.view = 0;
+    a.spec = align256(sizeof(StageView));
+    a.x = a.spec + align256((size_t)sets * rows_cap * kSpec * sizeof(float2));
+    a.taps = a.x + align256(sizeof(float) * (size_t)nx);
+    a.end = a.taps + (taps ? align256(sizeof(float) * (size_t)rows_cap * kB) : 0);
+    return a;
+}
+// Behind a plan's staging areas, from the 256-aligned offset `at`, when it has slots of tap-form pools: one StageTap per
+// staged slot, the n_tap transform Sources, their k_prepare CTA prefix (n_tap + 1 ints) and a zero word (the Sources'
+// counts), each at a 256-byte boundary.  Offsets from the start of the allocation; `end` is where the block ends.
+struct TapBlock { size_t taps, src, prefix, zero, end; };
+SS_HD TapBlock tap_block(size_t at, int n_staged, int n_tap) {
+    TapBlock t;
+    t.taps = align256(at);
+    t.src = t.taps + align256(sizeof(StageTap) * (size_t)n_staged);
+    t.prefix = t.src + align256(sizeof(Source) * (size_t)n_tap);
+    t.zero = t.prefix + align256(sizeof(int) * (size_t)(n_tap + 1));
+    t.end = t.zero + 256;
+    return t;
+}
+
 struct Regs32 { float2 a[16]; float2 b[16]; };
 
 // S1: pass A of the forward transform straight from global memory: all 64 loads of the thread's two

@@ -243,12 +243,15 @@ class RirBank(_Held):
     render that uses it is ordered after its construction by the library, on every path, whatever stream built it.
     Plans and source pools hold the bank: it is freed only once it is closed (or collected) and nothing alive uses it.
     A host bank (`host` True, Renderer.rir_bank(..., host=True)) holds its spectra in pinned host memory
-    (`host_nbytes`; `nbytes` counts device bytes only) and serves only as a candidate of a host source pool."""
+    (`host_nbytes`; `nbytes` counts device bytes only) and serves only as a candidate of a host source pool.  `form` is
+    "spectra", or "taps" for a tap-form host bank (SS_BANK_TAPS), which holds the (normalised) taps in rows of 4096
+    instead, half the pinned bytes, and whose pools transform the rows each run stages on the device."""
 
-    def __init__(self, renderer, handle, shape, normalize, direct_taps, host=False):
+    def __init__(self, renderer, handle, shape, normalize, direct_taps, host=False, form="spectra"):
         self.renderer, self._h = renderer, handle
         self.shape = tuple(int(v) for v in shape)          # as given: (P, C, L) or (C, L)
         self.normalize, self.direct_taps, self.host = bool(normalize), int(direct_taps), bool(host)
+        self.form = form
         self.nbytes = int(renderer.lib.ss_bank_bytes(handle))
         self.host_nbytes = int(renderer.lib.ss_bank_host_bytes(handle))
 
@@ -616,7 +619,8 @@ class Renderer:
         self.ctx = _lib.context(self.device)
 
     # ------------------------------------------------------------------ RIR spectrum banks
-    def rir_bank(self, rirs, normalize: bool = False, direct_taps: int = 0, host: bool = False) -> RirBank:
+    def rir_bank(self, rirs, normalize: bool = False, direct_taps: int = 0, host: bool = False,
+                 form: str = "spectra") -> RirBank:
         """Transform an RIR set (P, C, L) - or (C, L) for a static source - once into a RirBank on this renderer's
         device: a NumPy array is copied in and the call returns when the bank is complete; a CUDA float32 tensor of this
         device is transformed asynchronously on the current stream (keep it unchanged until that stream gets there).
@@ -625,12 +629,19 @@ class Renderer:
         `normalize` / `direct_taps` are the normalize_rirs / direct_taps every source of the bank renders with (a bank
         with a direct set also serves sources with direct_taps = 0).  `host` moves the transformed bank into pinned host
         memory (SS_BANK_HOST; bit-identical spectra, the call returns once it is there): such a bank is only a candidate
-        of a host source pool (source_pool), whose plans copy the rows each run reads to the device."""
+        of a host source pool (source_pool), whose plans copy the rows each run reads to the device.  `form` = "taps"
+        (host banks only, SS_BANK_TAPS) keeps the taps instead of their spectra - zero-padded rows of 4096, divided by the
+        abs-max with `normalize` - at half the pinned bytes, a quarter with a direct set; its pools copy half the RIR
+        bytes per run and transform them on the device, with the bits of a spectral host bank of the same RIRs."""
         taps = int(direct_taps)
         if taps < 0:
             raise ValueError("direct_taps must be >= 0, got %d" % taps)
+        if form not in ("spectra", "taps"):
+            raise ValueError("rir_bank: form must be 'spectra' or 'taps', got %r" % (form,))
+        if form == "taps" and not host:
+            raise ValueError("rir_bank: form='taps' is a host bank form: it needs host=True")
         flags = (_lib.SS_RIR_NORMALIZE if normalize else 0) | (_lib.SS_DIRECT_TARGET if taps > 0 else 0) | \
-            (_lib.SS_BANK_HOST if host else 0)
+            (_lib.SS_BANK_HOST if host else 0) | (_lib.SS_BANK_TAPS if form == "taps" else 0)
         h = ctypes.c_void_p()
         dev = _is_tensor(rirs)
         if dev:
@@ -647,7 +658,7 @@ class Renderer:
                                                    ctypes.c_void_p(stream), ctypes.byref(h)))
         else:
             _lib.check(self.lib.ss_bank_create_host(self.ctx, a.ctypes.data, P, C, L, flags, taps, ctypes.byref(h)))
-        return RirBank(self, h, shape, normalize, taps, host)
+        return RirBank(self, h, shape, normalize, taps, host, form)
 
     # ------------------------------------------------------------------ source pools
     def source_pool(self, candidates: T.Sequence[T.Union[MovingSource, StaticSource]],
@@ -664,7 +675,10 @@ class Renderer:
         Candidates whose banks are all host banks (rir_bank(..., host=True)) make a host pool (`resident` "host"): its
         dry signals are copied into pinned host memory at once, so `dry` (and `bounds`, when `bounds_host` is not given)
         may also be NumPy arrays or CPU tensors; every plan run then copies only the rows and samples its slots read to
-        the device (one more kernel launch per run).  A pool that mixes host and device banks is refused.
+        the device (one more kernel launch per run).  A pool that mixes host and device banks is refused.  Over tap-form
+        host banks (rir_bank(..., form="taps")) each run copies the staged rows' taps and transforms them on the device
+        (one more launch again), with the bits of the same pool over spectral host banks; a pool that mixes forms is
+        refused.
 
         `levels` = "mono" or "channels" also builds every candidate's level table (ss_pool_levels: the float64 prefix
         sums of the squares of its whole rendered stem, channel-folded like Mixture(mono=True) for "mono"), which
@@ -685,7 +699,7 @@ class Renderer:
         _check_lufs("source_pool", "candidate", lufs_targets, n, sr)
         items = (SsSource * n)()
         keep = []
-        first, L_max, host, sizes = None, 0, None, []
+        first, L_max, host, form, sizes = None, 0, None, None, []
         for i, s in enumerate(candidates):
             if not isinstance(s, (MovingSource, StaticSource)):
                 raise ValueError("source_pool: candidate %d must be a MovingSource or StaticSource, got %s"
@@ -709,6 +723,11 @@ class Renderer:
                 raise ValueError("source_pool: candidate %d has a %s bank, candidate 0 a %s one: a pool's banks are all "
                                  "host banks or all device banks" % ((i,) + (("host", "device") if rb.host else
                                                                            ("device", "host"))))
+            if form is None:
+                form = rb.form
+            elif rb.form != form:
+                raise ValueError("source_pool: candidate %d has a bank of form %r, candidate 0 one of form %r: a pool's "
+                                 "banks are all of one form" % (i, rb.form, form))
             L_max = max(L_max, L)
             own = "candidate %d" % i
             bounds_host = s.bounds_host if mode == _lib.SS_MOVING_BOUNDS else None
