@@ -368,7 +368,8 @@ void ss_plan_destroy(ss_plan* plan);
  *
  * T is a stem's output length (win_len, or N for a whole stem), E = C * T, or T with SS_MIX_MONO.
  *   - Indices name entries of the `items` passed to ss_plan_create_mix, in the caller's order.  A mixture reads the
- *     reverberant `out` of each named item (a direct-path stem is rendered as usual and is not a mixture input).  A stem
+ *     reverberant `out` of each named item (a direct-path stem is not a mixture input; ss_plan_create_target below makes
+ *     it a mixture's target).  A stem
  *     may appear in several mixtures (one noise stem shared by several scenes) but only once within one mixture.
  *   - SS_MIX_MONO: every stem, speakers and noises alike, is first folded to its channel mean (the dataloader's
  *     is_mono, :62-63, :76-77): at every element t, the float32 sum of its C rows in channel order 0..C-1, every add
@@ -684,6 +685,33 @@ int ss_plan_create_pair(ss_ctx* ctx, const ss_source* items, int n_items, const 
                         const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                         const ss_pair_gains* const* pair_gains /* NULL or n_picks entries, NULL = none */,
                         int n_picks, ss_plan** out);
+
+/* ---- dereverberation targets in plans: the training target of separation + dereverberation (WHAMR!-style: the mix is
+ * reverberant, the targets are the speakers' direct paths) and of the enhancement mixtures of configs[4].  A target of
+ * mixture k receives, at every run, each of its speakers' direct-path stems (SS_DIRECT_TARGET, `out_direct`) with the
+ * mixture's own treatment of that speaker:
+ *     direct_out[s] = fold(out_direct of speaker s) * (float)g_s
+ * with the fold of SS_MIX_MONO (or the stem as it is), the float32 gain g_s that scales speakers_out[s] (speaker 0: 1,
+ * so its target is exactly its folded direct stem) and the same single rounded float32 multiply, in the same launch
+ * that writes speakers_out (k_mix_write): a plan launches as many kernels per run with targets as without them.
+ *   - The gains stay defined on the reverberant crops, as the dataloader defines them (movingdatamodule.py:105-124):
+ *     mix, speakers_out, rms_db, the stems and the draws keep their bits, and the targets match the mix the model sees.
+ *   - direct_out: device, S * E floats laid out like speakers_out ((S, C, T), or (S, T) with SS_MIX_MONO).  A direct
+ *     set cut at the whole RIR (direct_taps >= L) makes the direct stem the reverberant stem's bits (SS_DIRECT_TARGET),
+ *     and then direct_out equals speakers_out bit for bit.
+ * ss_plan_create_target is ss_plan_create_pair with n_targets entries (n_targets == 0: exactly ss_plan_create_pair).
+ * Refused at creation with SS_ERR_INVALID, before anything is allocated and with no plan created: a `mix` outside
+ * [0, n_mixes) or named by two entries, n_targets < 0 or NULL targets with n_targets > 0, a NULL direct_out, a speaker
+ * of that mixture without SS_DIRECT_TARGET, and a direct_out range that meets another range (ss_plan_mix's rule for
+ * written ranges: the speakers' out_direct count as read).  ss_version stays 108: the export marks the capability. */
+typedef struct {
+    int32_t mix;                      /* index into `mixes`                                                           */
+    float* direct_out;                /* device, S * E floats, written at every run                                   */
+} ss_plan_target;
+int ss_plan_create_target(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                          const ss_pair_gains* const* pair_gains /* NULL or n_picks entries, NULL = none */,
+                          int n_picks, const ss_plan_target* targets, int n_targets, ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

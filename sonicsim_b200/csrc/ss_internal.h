@@ -123,9 +123,14 @@ struct MixItem {
     int S, M, Cf;
     int delay;                        // overlap_audio shift of the summed noise in elements (0 = none)
     float snr_val;                    // ss_mix_dev: the item's SNR, which `snr` points at in the uploaded descriptor
+    // dereverberation targets (ss_plan_create_target), null elsewhere: dir[s] is speaker s's direct-path stem, laid out
+    // as spk[s]; dir_out (S, E) receives each one folded and scaled by its speaker's gain, as spk_out does
+    const float* dir[kMixStems];
+    float* dir_out;
 };
-// The four mixture kernels over the n descriptors at `d` (device memory), asynchronous on `stream`.
-int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream);
+// The four mixture kernels over the n descriptors at `d` (device memory), asynchronous on `stream`; `direct`: some
+// descriptor has a dir_out (k_mix_write<true>).
+int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream, bool direct = false);
 
 // One level table of a pool candidate (ss_pool_levels): from the (C, N) stem y, q[0] = 0 and q[n + 1] = q[n] + e[n] in
 // float64, e[n] the square of the mixture kernels' channel fold at n (mono) or the float64 sum of the C channels' squares.

@@ -2453,6 +2453,7 @@ struct ss_plan {
     std::vector<ss_pool*> pools;       // pools of its pooled slots: every run waits for each pool's `ready` event
     const MixItem* d_mix = nullptr;   // the mixtures' descriptors, in d_desc behind the chunk descriptors
     int n_mix = 0;
+    bool mix_direct = false;           // some mixture has a dereverberation target: k_mix_write<true>
     const DrawDesc* d_draw = nullptr;  // the start draws' descriptors (k_draw), in d_desc behind the mixture scratch
     int n_draw = 0;
     const StageSlot* d_stage = nullptr;   // the staged slots' k_stage descriptors, in d_desc behind the draws
@@ -2655,8 +2656,9 @@ extern "C" void ss_plan_destroy(ss_plan* p) {
     delete p;
 }
 
-// The descriptor of mixture m of a plan: rows of the callers' `items` outputs (before arrange_chunks regroups them)
-static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double* scratch) {
+// The descriptor of mixture m of a plan: rows of the callers' `items` outputs (before arrange_chunks regroups them);
+// with dir_out, its speakers' direct-path stems and the (S, E) targets
+static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double* scratch, float* dir_out) {
     MixItem d; memset(&d, 0, sizeof(d));
     const ss_source& a = items[m.speakers[0]];
     const int64_t T = a.win_len > 0 ? a.win_len : a.N;
@@ -2666,6 +2668,10 @@ static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double
     d.sirs = m.sirs; d.snr = m.snr; d.mix = m.mix; d.spk_out = m.speakers_out; d.rms_out = m.rms_db; d.scratch = scratch;
     d.E = mono ? T : (int64_t)a.C * T; d.T = T; d.Cf = mono ? a.C : 1;
     d.S = m.S; d.M = m.M; d.delay = m.noise_delay;
+    if (dir_out) {
+        for (int s = 0; s < m.S; ++s) d.dir[s] = items[m.speakers[s]].out_direct;
+        d.dir_out = dir_out;
+    }
     return d;
 }
 
@@ -2714,10 +2720,11 @@ static StageArea stage_area_of(const ss_source& it) {
     return stage_area(stage_sets(it), cap.first, cap.second, it.pool->taps);
 }
 
-// (dry[i]: caller item i's dry pick, or null; pair[i]: its pair gains' device table, or null)
+// (dry[i]: caller item i's dry pick, or null; pair[i]: its pair gains' device table, or null; dir_out[k]: mixture k's
+// dereverberation targets, or null)
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
                       const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws,
-                      const ss_dry_pick* const* dry, const float* const* pair) {
+                      const ss_dry_pick* const* dry, const float* const* pair, float* const* dir_out) {
     ss_ctx* c = p->c;
     std::vector<int> cuts, order;
     std::vector<ss_source> arranged;
@@ -2809,9 +2816,11 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
                        p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data(),
                        dry_describe.data(), pair_arranged.data());
-    for (int k = 0; k < n_mixes; ++k)
+    for (int k = 0; k < n_mixes; ++k) {
         ((MixItem*)(host.data() + mix_off))[k] =
-            mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k));
+            mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k), dir_out[k]);
+        p->mix_direct = p->mix_direct || dir_out[k];
+    }
     if (n_mixes > 0) {
         p->d_mix = (const MixItem*)(p->d_desc + mix_off);
         p->n_mix = n_mixes;
@@ -2884,8 +2893,11 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
     return SS_OK;
 }
 
+// (dir_out[k]: mixture k's dereverberation targets, or null: S * E floats written, and every speaker of the mixture
+// needs a direct-path stem)
 static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
-                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks) {
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks,
+                          float* const* dir_out) {
     if (n_mixes > 65535) return SS_ERR_UNSUPPORTED;         // one gridDim.y row per mixture
     std::vector<ByteRange> r;
     // a draw writes its start (which only its readers read) and `used`, and reads its u
@@ -2912,8 +2924,11 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
             const ss_source& b = items[stems[j]];
             if (b.C != a.C || (b.win_len > 0 ? b.win_len : b.N) != T) return SS_ERR_INVALID;
         }
+        if (dir_out[k])
+            for (int s = 0; s < m.S; ++s) if (!(items[m.speakers[s]].flags & SS_DIRECT_TARGET)) return SS_ERR_INVALID;
         const uint64_t E = (m.flags & SS_MIX_MONO) ? (uint64_t)T : (uint64_t)a.C * T;
         add_range(r, m.mix, 4 * E, true);
+        add_range(r, dir_out[k], 4 * E * m.S, true);
         add_range(r, m.speakers_out, 4 * E * m.S, true);
         add_range(r, m.rms_db, 4 * (uint64_t)m.S, true);
         add_range(r, m.sirs, 4 * (uint64_t)(m.S - 1), false);
@@ -2982,19 +2997,35 @@ static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_ite
     return SS_OK;
 }
 
+// A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
+// and the byte ranges (validate_mixes): dir_out[k] receives mixture k's direct_out, or null
+static int validate_targets(int n_mixes, const ss_plan_target* targets, int n_targets, std::vector<float*>& dir_out) {
+    dir_out.assign(n_mixes, nullptr);
+    for (int j = 0; j < n_targets; ++j) {
+        const ss_plan_target& t = targets[j];
+        if (t.mix < 0 || t.mix >= n_mixes || dir_out[t.mix] || !t.direct_out) return SS_ERR_INVALID;
+        dir_out[t.mix] = t.direct_out;
+    }
+    return SS_OK;
+}
+
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
-                       const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
+                       const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                       int n_targets, ss_plan** out) {
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
     std::vector<const ss_dry_pick*> dry;
     std::vector<const float*> pair;
+    std::vector<float*> dir_out;
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
     { int st = validate_dry_picks(c, items, n_items, picks, pair_gains, n_picks, dry, pair); if (st) return st; }
     { int st = validate_draws(items, n_items, draws, n_draws, dry.data()); if (st) return st; }
-    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks); if (st) return st; }
+    { int st = validate_targets(n_mixes, targets, n_targets, dir_out); if (st) return st; }
+    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks, dir_out.data());
+      if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
@@ -3004,7 +3035,8 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data(), pair.data());
+    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data(), pair.data(),
+                              dir_out.data());
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -3012,19 +3044,19 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 }
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
-    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, out);
+    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3033,7 +3065,18 @@ extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_item
     if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
         (n_picks > 0 && !picks))
         return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                     int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                     const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                     int n_targets, ss_plan** out) {
+    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
+        (n_picks > 0 && !picks) || n_targets < 0 || (n_targets > 0 && !targets))
+        return SS_ERR_INVALID;
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3076,7 +3119,7 @@ static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
         return chunk_enqueue(c, p->chunks[k], s, c->profiling);
     });
     if (rc) return rc;
-    return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream) : SS_OK;
+    return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream, p->mix_direct) : SS_OK;
 }
 
 extern "C" int ss_plan_run(ss_plan* p, void* stream_) {

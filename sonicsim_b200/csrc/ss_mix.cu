@@ -175,7 +175,20 @@ __global__ void __launch_bounds__(256) k_mix_speech_energy(const MixItem* __rest
     if (threadIdx.x == 0) it.scratch[(long long)blockIdx.x * (kMaxStems + 2) + kMaxStems + 1] = r;
 }
 
-// pass 3: noise gain (:118-121), mixture and scaled speakers (:123-124)
+// The write pass's 16-byte test: mix_vec_ok, and with kDirect also a target's direct rows and dir_out.  The pass writes
+// every element on its own, so either path gives the same bits and the choice may differ from the energy passes'.
+template <bool kDirect>
+__device__ __forceinline__ bool write_vec_ok(const MixItem& it) {
+    if (!mix_vec_ok(it)) return false;
+    if (!kDirect || !it.dir_out) return true;
+    uintptr_t a = (uintptr_t)it.dir_out;
+    for (int s = 0; s < it.S; ++s) a |= (uintptr_t)it.dir[s];
+    return (a & 15) == 0;
+}
+
+// pass 3: noise gain (:118-121), mixture and scaled speakers (:123-124); with kDirect, a mixture with dir_out also
+// writes each speaker's folded direct-path stem times the speaker's gain gf[s], with the multiply of spk_out
+template <bool kDirect>
 __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ items) {
     const MixItem& it = items[blockIdx.y];
     const double* g = it.scratch + (long long)kMixBlocks * (kMaxStems + 2);
@@ -187,7 +200,7 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
     float gf[kMaxStems];
 #pragma unroll
     for (int s = 0; s < kMaxStems; ++s) gf[s] = s < it.S ? (float)g[s] : 0.f;
-    if (mix_vec_ok(it)) {
+    if (write_vec_ok<kDirect>(it)) {
         for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < (it.E >> 2); q += (long long)gridDim.x * blockDim.x) {
             float4 sp = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
@@ -196,6 +209,11 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
                 v.x = __fmul_rn(v.x, gf[s]); v.y = __fmul_rn(v.y, gf[s]); v.z = __fmul_rn(v.z, gf[s]); v.w = __fmul_rn(v.w, gf[s]);
                 if (it.spk_out) ((float4*)(it.spk_out + (long long)s * it.E))[q] = v;
                 sp.x += v.x; sp.y += v.y; sp.z += v.z; sp.w += v.w;
+                if (kDirect && it.dir_out) {
+                    float4 d = fold4(it, it.dir[s], q);
+                    d.x = __fmul_rn(d.x, gf[s]); d.y = __fmul_rn(d.y, gf[s]); d.z = __fmul_rn(d.z, gf[s]); d.w = __fmul_rn(d.w, gf[s]);
+                    ((float4*)(it.dir_out + (long long)s * it.E))[q] = d;
+                }
             }
             const float4 n = noise_sum4(it, q);
             float4 o;
@@ -212,6 +230,7 @@ __global__ void __launch_bounds__(256) k_mix_write(const MixItem* __restrict__ i
             float v = __fmul_rn(fold(it, it.spk[s], e), gf[s]);               // products and sums rounded separately, as torch does
             if (it.spk_out) it.spk_out[(long long)s * it.E + e] = v;
             sp += v;
+            if (kDirect && it.dir_out) it.dir_out[(long long)s * it.E + e] = __fmul_rn(fold(it, it.dir[s], e), gf[s]);
         }
         it.mix[e] = __fadd_rn(sp, __fmul_rn(noise_at(it, e), gn));
     }
@@ -325,12 +344,13 @@ extern "C" int ss_mix_dev(ss_ctx* c, const ss_mix_item* items, int n_items, void
     return st ? st : rs;
 }
 
-int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream) {
+int mix_enqueue(ss_ctx* c, const MixItem* d, int n, cudaStream_t stream, bool direct) {
     dim3 grid(kMixBlocks, n);
     k_mix_energy<<<grid, 256, 0, stream>>>(d);
     k_mix_gain<<<(n + 63) / 64, 64, 0, stream>>>(d, n);
     k_mix_speech_energy<<<grid, 256, 0, stream>>>(d);
-    k_mix_write<<<grid, 256, 0, stream>>>(d);
+    if (direct) k_mix_write<true><<<grid, 256, 0, stream>>>(d);
+    else k_mix_write<false><<<grid, 256, 0, stream>>>(d);
     CK(cudaGetLastError());
     c->launches += 4;
     return SS_OK;

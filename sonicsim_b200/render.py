@@ -59,7 +59,11 @@ class Mixture(T.NamedTuple):
     after their gains; `rms_db` (S,): compute_mch_rms_dB of every speaker stem before its gain (-200 for silence), for
     the dataloader's silence rule (redraw when a speaker is below -40 dB).  `mono`: fold every stem to its channel
     mean first (float32 sum in channel order, then a division by C).  `noise_delay`: overlap_audio's shift of the summed
-    noise, in elements (see ss_mix_item)."""
+    noise, in elements (see ss_mix_item).  `direct_out` (S, C, T) or (S, T), the dereverberation targets: each speaker's
+    direct-path stem (the speaker's source needs direct_taps and a direct_outs entry) folded like the mixture's stems
+    and scaled by that speaker's float32 gain with the multiply that gives speakers_out, so that target s is
+    speakers_out[s] with the direct path in place of the reverberant stem (speaker 0: its folded direct stem).  The
+    gains stay those of the reverberant crops, as the dataloader defines them."""
     speakers: T.Sequence[int]
     noises: T.Sequence[int]
     sirs: T.Any
@@ -69,6 +73,7 @@ class Mixture(T.NamedTuple):
     rms_db: T.Any = None
     mono: bool = False
     noise_delay: int = 0
+    direct_out: T.Any = None
 
 
 class Pooled(T.NamedTuple):
@@ -976,7 +981,9 @@ class Renderer:
             starts.copy_(torch.randint(...)); sirs.uniform_(-6, 6); snr.uniform_(10, 20)   # movingdatamodule.py:106, :119
             plan.run()                                          # crops, gains and mixtures of every scene
 
-        and the model takes (mix, speakers_out) from there; rms_db (Mixture) carries each speaker's level.
+        and the model takes (mix, speakers_out) from there; rms_db (Mixture) carries each speaker's level.  A Mixture
+        with `direct_out` also writes its speakers' dereverberation targets in the same launches (ss_plan_create_target):
+        the model then takes (mix, direct_out) for separation + dereverberation.
 
         `draws`: CropDraw entries, the dataloader's silence rule on the device: at the head of every run (one more
         kernel launch), each draw picks its readers' start from its `u`, rejecting starts at which a speaker's crop is
@@ -990,9 +997,11 @@ class Renderer:
         (dry_picks.random_(0, n) before the run)."""
         dry = self._device_dry(sources)
         items, n, keep = self._device_items(sources, outs, direct_outs)
-        mixes = self._device_mixes(mixtures, outs, keep) if mixtures else None
+        targets = []
+        mixes = self._device_mixes(mixtures, outs, keep, items, targets) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
-        return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None)
+        return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
+                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1100,8 +1109,10 @@ class Renderer:
         keep.append(list(draws))
         return arr
 
-    def _device_mixes(self, mixtures, outs, keep):
-        """Validated ss_plan_mix array of a plan's mixtures; their tensors are appended to `keep`."""
+    def _device_mixes(self, mixtures, outs, keep, items=None, targets=None):
+        """Validated ss_plan_mix array of a plan's mixtures; their tensors are appended to `keep`.  A mixture with a
+        direct_out needs `items` (the plan's SsSource array, whose speakers must render direct-path stems) and `targets`,
+        a list that receives its validated SsPlanTarget."""
         import torch
         n = len(outs)
         arr = (_lib.SsPlanMix * len(mixtures))()
@@ -1137,6 +1148,13 @@ class Renderer:
             delay = int(m.noise_delay)
             if delay < 0:
                 raise ValueError("plan_device: noise_delay of mixture %d must be >= 0, got %d" % (k, delay))
+            if m.direct_out is not None:
+                for v in spk:
+                    if not items[v].out_direct:
+                        raise ValueError("plan_device: mixture %d has a direct_out, but its speaker source %d renders no "
+                                         "direct-path stem (direct_taps and a direct_outs entry)" % (k, v))
+                d_out = _tensor(m.direct_out, "plan_device", own, "direct_out", f32, self.device, (S,) + row)
+                targets.append(_lib.SsPlanTarget(mix=k, direct_out=d_out))
             e = arr[k]
             for i, v in enumerate(spk):
                 e.speakers[i] = v
@@ -1248,16 +1266,20 @@ class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
-    dry-picked slots take their dry signals from dry pools (ss_plan_create_dry), and with pair gains their gains from
-    pair-gain tables (ss_plan_create_pair)."""
+    dry-picked slots take their dry signals from dry pools (ss_plan_create_dry), with pair gains their gains from
+    pair-gain tables (ss_plan_create_pair), and with dereverberation targets its mixtures also write those
+    (ss_plan_create_target)."""
 
-    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None):
+    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
-        self.draws, self.dry, self.pair_gains = draws, dry, pair_gains
+        self.draws, self.dry, self.pair_gains, self.targets = draws, dry, pair_gains, targets
         self._plan = ctypes.c_void_p()
         if n > 0:
             args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry)
-            if pair_gains is None:
+            if targets is not None:
+                st = renderer.lib.ss_plan_create_target(*args, pair_gains, len(dry) if dry else 0, targets,
+                                                        len(targets), ctypes.byref(self._plan))
+            elif pair_gains is None:
                 st = renderer.lib.ss_plan_create_dry(*args, len(dry) if dry else 0, ctypes.byref(self._plan))
             else:
                 st = renderer.lib.ss_plan_create_pair(*args, pair_gains, len(dry), ctypes.byref(self._plan))
