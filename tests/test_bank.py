@@ -5,31 +5,17 @@ given its raw RIRs - whole stems against the full and dual emulations, windows a
 normalised, direct and normalised + direct banks, with the raw RIR buffer NaN-filled once the bank is built.  Also the
 Python layer's refusals that need no device."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
-from window_cases import CASES, make_case, windows
-
-KSPEC = 4096
+from emu import build_emu
+from window_cases import CASES, KSPEC, _p, make_case, windows
 
 
 @pytest.fixture(scope="module")
-def bank_emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_bank.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_bank.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    return ctypes.CDLL(so_path)
-
-
-def _p(a):
-    return None if a is None else ctypes.c_void_p(a.ctypes.data)
+def bank_emu():
+    return build_emu.load("ss_emu_bank")
 
 
 def create(lib, h, normalize, taps):

@@ -13,13 +13,11 @@
     reading only whole groups of 4 inside the signal's 64-byte padded arena span.
   - The float -> int16 acceptance check of Renderer.dry_pool and its refusals, before any C call."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from emu import build_emu
 from sonicsim_b200 import render
 
 B = 4096
@@ -58,20 +56,8 @@ def reversed_prefix(t):
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_compact.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_compact.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_sparse_levels.argtypes = [vp, vp, vp, i32, vp]
-    lib.emu_draw_i16.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, i32, ctypes.c_float, ctypes.POINTER(ctypes.c_int32)]
-    lib.emu_speaker_i16.argtypes = [vp, vp, i32, i32, vp]
-    lib.emu_stage_i16.argtypes = [vp] + [i32] * 6 + [vp, vp] + [i32] * 3 + [vp, vp, vp]
-    return lib
+def emu():
+    return build_emu.load("ss_emu_compact")
 
 
 def long_audio(rng, N, n_utt, amp=(0.01, 0.9)):

@@ -2,27 +2,20 @@
 kernels (tests/emu, the same per-thread code as the CUDA kernels) rendering both stems of a source in one pass against
 rendering each RIR set as a source of its own, bit for bit."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT, TOL
+from conftest import TOL
 from direct_path import CASES, direct_path_rirs, make_case, normalized, oracle_render
+from emu import build_emu
 from oracle import sonicsim_oracle as so
 
 
 @pytest.fixture(scope="module")
-def render_dual(tmp_path_factory):
+def render_dual():
     """emu_render_dual of tests/emu/ss_emu_dual.cu, built with g++ like the other emulation library."""
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_dual.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_dual.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
+    lib = build_emu.load("ss_emu_dual")
     fp, ip = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int32)
 
     def ptr(a, t=fp):

@@ -12,24 +12,14 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
+from emu import build_emu
 import draw_reference as dr
 from sonicsim_b200 import _lib
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_dry_pool.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_dry_pool.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_pick_pooled.argtypes = [vp, vp, vp, i32, vp, i32] + [i32] * 7 + [vp]
-    lib.emu_draw_mixed.argtypes = [vp] * 9 + [i32, vp, vp, i32, i32, vp, i32, ctypes.c_float,
-                                              ctypes.POINTER(ctypes.c_int32)]
-    return lib
+def emu():
+    return build_emu.load("ss_emu_dry_pool")
 
 
 def pick(emu, N, P, Ks=None, gains=None, K=1, C=2, direct=0, n_dry=0, v=0, dv=0):

@@ -5,9 +5,7 @@ and windows, plain / normalised / direct / both.  The banked items carry rir = N
 is NaN once the bank is built, and every output lies between sentinels.  Also: one bank shared by many sources across
 chunks, host- and device-built banks, loudness targets, the launches an all-banked batch saves, configs[1] against the
 oracle, and every refusal."""
-import contextlib
 import ctypes
-import os
 
 import numpy as np
 import pytest
@@ -17,6 +15,7 @@ from chunk_budget import chunk_budget  # noqa: F401  (fixture)
 from conftest import TOL
 from oracle import sonicsim_oracle as so
 from window_cases import CASES, make_case, windows
+from gpu_plumbing import _lib, small_host_budget_context
 
 pytestmark = pytest.mark.gpu
 
@@ -24,31 +23,6 @@ SENT = np.float32(1234.5)
 PAD = 37
 FLAGS = [(False, False), (True, False), (False, True), (True, True)]
 FLAG_IDS = ["plain", "normalize", "direct", "normalize+direct"]
-
-
-def _lib():
-    from sonicsim_b200 import _lib as L, render
-    return L, render.default_renderer()
-
-
-@contextlib.contextmanager
-def small_host_budget_context():
-    """A context of its own whose host pipeline budget is 1 MB (SS_HOST_CHUNK_MB is read by ss_create)."""
-    L, R = _lib()
-    old = os.environ.get("SS_HOST_CHUNK_MB")
-    os.environ["SS_HOST_CHUNK_MB"] = "1"
-    ctx = ctypes.c_void_p()
-    try:
-        assert R.lib.ss_create(R.device, ctypes.byref(ctx)) == 0
-    finally:
-        if old is None:
-            del os.environ["SS_HOST_CHUNK_MB"]
-        else:
-            os.environ["SS_HOST_CHUNK_MB"] = old
-    try:
-        yield ctx
-    finally:
-        R.lib.ss_destroy(ctx)
 
 
 def make_bank(ctx, h, normalize, taps, dev=False):

@@ -19,10 +19,8 @@ import pytest
 import torch
 
 from oracle import sonicsim_oracle as so
-from test_gpu_dry_pool import Slots
-from test_gpu_host_dry_pool import _host_pool
-from test_gpu_plan_pool import longs, noises, speakers
-from test_gpu_pool_lengths import moving
+from gpu_plumbing import _R
+from pool_worlds import DrySlots, _host_pool, longs, moving, noises, speakers
 
 pytestmark = pytest.mark.gpu
 
@@ -30,11 +28,6 @@ TAPS = 40
 NAN = float("nan")
 RATE = 16000
 SLEEP = int(5e8)
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
 
 
 def gappy_i16(rng, N, burst=(0.2, 1.0), gap=(0.0, 1.5)):
@@ -113,7 +106,7 @@ def test_stems_equal_the_float_pool(world, kind, src_resident, i16_resident):
     ks = i16_signals(611, 5, n_max)
     fpool, ipool = twin_pools(R, ks, src_resident, i16_resident)
     wl = min(9000, min(c.N for c in cands) - 1) if kind != "noise" else 20000
-    A, Bs = Slots(pool, fpool, cands, wl, taps), Slots(pool, ipool, cands, wl, taps)
+    A, Bs = DrySlots(pool, fpool, cands, wl, taps), DrySlots(pool, ipool, cands, wl, taps)
     pa = R.plan_device(A.srcs, A.outs, direct_outs=A.douts)
     pb = R.plan_device(Bs.srcs, Bs.outs, direct_outs=Bs.douts)
     gen = torch.Generator(device="cuda")
@@ -286,8 +279,8 @@ def test_pair_gains_equal_the_float_pool(world, src_resident, i16_resident):
     assert np.array_equal(np.isnan(la), np.isnan(lb)) and np.array_equal(la[~np.isnan(la)], lb[~np.isnan(lb)])
     assert ga.nbytes == gb.nbytes == 4 * 3 * len(cands)
     wl = 9000
-    A = Slots(pool, fpool, cands, wl, taps)
-    Bs = Slots(pool, ipool, cands, wl, taps)
+    A = DrySlots(pool, fpool, cands, wl, taps)
+    Bs = DrySlots(pool, ipool, cands, wl, taps)
     A.srcs = [s._replace(dry=s.dry._replace(gains=ga)) for s in A.srcs]
     Bs.srcs = [s._replace(dry=s.dry._replace(gains=gb)) for s in Bs.srcs]
     pa = R.plan_device(A.srcs, A.outs, direct_outs=A.douts)
@@ -357,7 +350,7 @@ def test_clamped_dry_picks_report_bit_4(world, src_resident):
     ks = i16_signals(651, 3, max(c.N for c in cands))
     fpool, ipool = twin_pools(R, ks, src_resident, "device")
     pool = pools[src_resident]
-    A, Bs = Slots(pool, fpool, cands, 5000, taps), Slots(pool, ipool, cands, 5000, taps)
+    A, Bs = DrySlots(pool, fpool, cands, 5000, taps), DrySlots(pool, ipool, cands, 5000, taps)
     pa = R.plan_device(A.srcs, A.outs, direct_outs=A.douts)
     pb = R.plan_device(Bs.srcs, Bs.outs, direct_outs=Bs.douts)
     try:
@@ -405,12 +398,12 @@ def test_python_refusals(world):
     ip = R.dry_pool(i16_signals(661, 2, max(c.N for c in cands)), dtype="int16")
     fdev = R.dry_pool([torch.from_numpy(values(k)).cuda() for k in i16_signals(661, 2, max(c.N for c in cands))])
     try:
-        sl = Slots(pools["host"], ip, cands, 4000, taps, k=2)
+        sl = DrySlots(pools["host"], ip, cands, 4000, taps, k=2)
         R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts).close()
-        sl = Slots(pools["host"], fdev, cands, 4000, taps, k=2)
+        sl = DrySlots(pools["host"], fdev, cands, 4000, taps, k=2)
         with pytest.raises(ValueError, match="host pool"):
             R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
-        sl = Slots(pools["device"], ip, cands, 4000, taps, k=2)
+        sl = DrySlots(pools["device"], ip, cands, 4000, taps, k=2)
         st = torch.zeros(1, dtype=torch.int32, device="cuda")
         srcs = [s._replace(window=(st, 4000)) for s in sl.srcs]
         draw = render.CropDraw(st, [0, 1], torch.rand(5, dtype=torch.float64, device="cuda"))

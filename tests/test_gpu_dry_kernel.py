@@ -9,74 +9,14 @@ import numpy as np
 import pytest
 import torch
 
-from mix_reference import (F32, RESAMPLE_PAIRS, clip_lengths, max_rel, resample_abs_bound, resample_f64,
-                           resample_kernel)
+from mix_reference import F32, RESAMPLE_PAIRS, clip_lengths, max_rel, resample_kernel
+from mix_reference import Clip, DryBuf
 
 pytestmark = pytest.mark.gpu
 
 NAN = float("nan")
 SS_ERR_INVALID, SS_ERR_UNSUPPORTED = -1, -5
 MAX_REL = [0.0]         # largest per-clip max-relative resampling error seen
-
-
-class Buf:
-    """`n` floats at `off` past a NaN guard of `pad` floats, followed by `pad` NaNs."""
-
-    def __init__(self, n, off=0, data=None, pad=64):
-        self.n, self.lo = int(n), pad + off
-        self.t = torch.full((pad + off + self.n + pad,), NAN, device="cuda")
-        if data is not None:
-            self.t[self.lo:self.lo + self.n] = torch.from_numpy(np.ascontiguousarray(data, F32).reshape(-1)).cuda()
-
-    @property
-    def ptr(self):
-        return self.t.data_ptr() + 4 * self.lo
-
-    def get(self):
-        return self.t[self.lo:self.lo + self.n].cpu().numpy()
-
-    def guards_nan(self):
-        a = self.t.cpu().numpy()
-        return bool(np.all(np.isnan(a[:self.lo])) and np.all(np.isnan(a[self.lo + self.n:])))
-
-
-_banks = {}
-
-
-def bank(orig, new):
-    """(guarded (taps, new_g) filter bank, orig_g, new_g, width, taps) of Resample(orig, new); guards of `taps` floats."""
-    if (orig, new) not in _banks:
-        K, o, n, width = resample_kernel(orig, new)
-        taps = K.shape[1]
-        _banks[(orig, new)] = (Buf(taps * n, 0, K.T, pad=taps), o, n, width, taps)
-    return _banks[(orig, new)]
-
-
-class Clip:
-    """One ss_dry_clip: x (channels, L) at `orig` Hz placed into a `new` Hz stream (orig == new: no resampling)."""
-
-    def __init__(self, x, orig, new, src_start, count, dst_start, off=0):
-        from sonicsim_b200 import _lib as L
-        self.x, self.orig, self.new = np.asarray(x, F32), orig, new
-        self.ch, self.L = self.x.shape
-        self.src_start, self.count, self.dst_start = int(src_start), int(count), int(dst_start)
-        kt, o, n, width, taps = (None, 1, 1, 0, 1) if orig == new else bank(orig, new)
-        self.taps = taps
-        self.src = Buf(self.ch * self.L, off, self.x, pad=max(taps, 64))
-        self.c = L.SsDryClip(src=self.src.ptr, kernel_t=kt.ptr if kt else None, dst_start=self.dst_start,
-                             src_start=self.src_start, count=self.count, channels=self.ch, src_len=self.L, orig=o,
-                             new_rate=n, width=width, taps=taps)
-
-    def expected(self):
-        """(float64 clip, per-sample rounding bound) over [src_start, src_start + count); bound None: exact."""
-        sl = slice(self.src_start, self.src_start + self.count)
-        if self.orig == self.new:
-            y = self.x[0] if self.ch == 1 else (self.x[0] + self.x[1]) * F32(0.5)
-            return y[sl], None
-        y = sum(resample_f64(r, self.orig, self.new) for r in self.x) / self.ch
-        b = sum(resample_abs_bound(r, self.orig, self.new) for r in self.x) / self.ch
-        # fp32 accumulation of at most `taps` fused terms per channel, one more rounding for the stereo sum
-        return y[sl], (self.taps + self.ch - 1) * 2.0 ** -24 * b[sl]
 
 
 def res_len(L, orig, new):
@@ -140,7 +80,7 @@ def pair_clips(orig, new, ch, rng):
 def test_dry_clips_against_reference(orig, new, ch):
     rng = np.random.default_rng(orig * 3 + new + ch)
     clips, total = pair_clips(orig, new, ch, rng)
-    out = Buf(total)
+    out = DryBuf(total)
     assert assemble(clips, out) == 0
     check_stream(clips, out)
 
@@ -163,12 +103,12 @@ def _batch(rng):
 
 def test_dry_batch_equals_single_clips():
     clips, total = _batch(np.random.default_rng(40))
-    out = Buf(total)
+    out = DryBuf(total)
     assert assemble(clips, out) == 0
     y = check_stream(clips, out)
     assert clips[0].dst_start == 0 and clips[-1].dst_start + clips[-1].count == total
     for c in clips:
-        alone = Buf(total, 1)
+        alone = DryBuf(total, 1)
         assert assemble([c], alone) == 0
         a = alone.get()
         assert alone.guards_nan()
@@ -178,7 +118,7 @@ def test_dry_batch_equals_single_clips():
 
 
 def test_dry_no_clips_zero_fills_exactly_total():
-    out = Buf(4097, 3)
+    out = DryBuf(4097, 3)
     assert assemble([], out) == 0
     assert out.guards_nan() and np.array_equal(out.get(), np.zeros(4097, F32))
 
@@ -188,16 +128,16 @@ def test_dry_refusals_leave_the_stream_untouched():
     x = (rng.standard_normal((1, 500)) * 0.1).astype(F32)
     n = res_len(500, 44100, 16000)
     ok = [Clip(x, 16000, 16000, 0, 100, 0), Clip(x, 44100, 16000, 0, n, 100)]
-    out = Buf(1000)
+    out = DryBuf(1000)
     assert assemble(ok + [Clip(x, 16000, 16000, 0, 50, 100 + n)], out) == 0       # touching ranges are fine
-    assert assemble([Clip(x, 44100, 16000, 1, n, 0)], Buf(1000)) == SS_ERR_INVALID  # one sample past res_len
+    assert assemble([Clip(x, 44100, 16000, 1, n, 0)], DryBuf(1000)) == SS_ERR_INVALID  # one sample past res_len
     for bad in (Clip(x, 16000, 16000, 0, 50, 99),            # overlaps the first clip's last sample
                 Clip(x, 16000, 16000, 0, 10, 150),           # inside the second clip
                 Clip(x, 44100, 16000, 0, n, 0)):             # the same range as the first clip and more
-        out = Buf(1000)
+        out = DryBuf(1000)
         assert assemble(ok + [bad], out) == SS_ERR_INVALID
         assert np.all(np.isnan(out.t.cpu().numpy()))
-    out = Buf(1000)
+    out = DryBuf(1000)
     assert assemble([Clip(x, 16000, 16000, 0, 0, 5)] * 65536, out) == SS_ERR_UNSUPPORTED
     assert np.all(np.isnan(out.t.cpu().numpy()))
 

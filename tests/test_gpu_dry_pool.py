@@ -23,96 +23,17 @@ import torch
 
 from oracle import sonicsim_oracle as so
 import draw_reference as dr
-from test_gpu_plan_draw import gappy_dry
-from test_gpu_plan_pool import Cand, _mix_dev, noises, speakers
-from test_gpu_pool_lengths import moving
+from draw_reference import NEAR_DB, TABLE_TOL
+from gpu_plumbing import _R, to
+from pool_worlds import Cand, DrawStep, DrySlots, _mix_dev, dry_signals, reference
+from pool_worlds import draw_world, world  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
 TAPS = 40
 NAN = float("nan")
 RATE = 16000
-TABLE_TOL = 1e-13
-NEAR_DB = 1e-6
 SLEEP = int(5e8)
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def dry_signals(seed, n, length, tail):
-    """n dry signals of `length` finite samples followed by `tail` NaNs (never read by a slot)."""
-    rng = np.random.default_rng(seed)
-    out = []
-    for _ in range(n):
-        x = np.full(length + tail, np.nan, np.float32)
-        x[:length] = so.synth_dry(rng, length)
-        out.append(to(x))
-    return out
-
-
-@pytest.fixture(scope="module")
-def world():
-    spk = speakers(301, n=4, taps=TAPS)                       # aligned moving, direct sets
-    lng = moving(302, [5000, 9000, 13000, 6000])              # K = 2, 3, 4, 2: grid, k_render<LONG>
-    noi = noises(303, n=3)                                    # static
-    return {"speakers": (spk, TAPS), "long": (lng, 0), "noise": (noi, 0)}
-
-
-def reference(c, x, s, wl, taps):
-    """render_device of candidate c with dry x[:N] (a contiguous copy) at the fixed window (s, wl)."""
-    render, R = _R()
-    out = torch.empty((c.C, wl), device="cuda")
-    dout = torch.empty((c.C, wl), device="cuda") if taps else None
-    R.render_device([c.src._replace(dry=x[:c.N].contiguous(), window=(s, wl), direct_taps=taps)], [out],
-                    direct_outs=[dout] if taps else None)
-    return out, dout
-
-
-class Slots:
-    """k dry-picked pooled slots over one pool, each with its own pick, dry pick and start tensor; NaN-filled outputs."""
-
-    def __init__(self, pool, dpool, cands, wl, taps, k=4, dry=True):
-        render, _ = _R()
-        self.cands, self.wl, self.taps, self.k = cands, wl, taps, k
-        self.picks = torch.zeros(k, dtype=torch.int32, device="cuda")
-        self.dpicks = torch.zeros(k, dtype=torch.int32, device="cuda")
-        self.starts = torch.zeros(k, dtype=torch.int32, device="cuda")
-        C = cands[0].C
-        self.outs = [torch.empty((C, wl), device="cuda") for _ in range(k)]
-        self.douts = [torch.empty((C, wl), device="cuda") for _ in range(k)] if taps else None
-        self.srcs = [render.Pooled(pool, self.picks[j], (self.starts[j], wl), taps,
-                                   render.DryPick(dpool, self.dpicks[j]) if dry else None) for j in range(k)]
-
-    def fill(self, gen, n, n_dry, n_min):
-        self.picks.copy_(torch.randint(0, n, (self.k,), generator=gen, device="cuda", dtype=torch.int32))
-        self.dpicks.copy_(torch.randint(0, n_dry, (self.k,), generator=gen, device="cuda", dtype=torch.int32))
-        self.starts.copy_(torch.randint(0, n_min - self.wl + 1, (self.k,), generator=gen, device="cuda",
-                                        dtype=torch.int32))
-        for o in self.outs + (self.douts or []):
-            o.fill_(NAN)
-
-    def snap(self):
-        return dict(picks=self.picks.clone(), dpicks=self.dpicks.clone(), starts=self.starts.clone(),
-                    outs=[o.clone() for o in self.outs], douts=[o.clone() for o in self.douts or []])
-
-    def check(self, snap, signals, what):
-        for j in range(self.k):
-            c = self.cands[int(snap["picks"][j])]
-            x = signals[int(snap["dpicks"][j])]
-            s = int(snap["starts"][j])
-            ref, dref = reference(c, x, s, self.wl, self.taps)
-            y = snap["outs"][j]
-            assert torch.isfinite(y).all(), (what, j)
-            assert torch.equal(y, ref), (what, j, int(snap["picks"][j]), int(snap["dpicks"][j]), s)
-            if self.taps:
-                assert torch.isfinite(snap["douts"][j]).all() and torch.equal(snap["douts"][j], dref), (what, j)
 
 
 @pytest.mark.parametrize("kind", ["speakers", "long", "noise"])
@@ -125,7 +46,7 @@ def test_bits_equal_render_device(world, kind):
     dpool = R.dry_pool(signals)
     assert dpool.n == 5 and dpool.n_min == n_max + 3001 and not dpool.levels and dpool.nbytes == 8 * 5
     wl = 9000 if kind != "noise" else 20000
-    sl = Slots(pool, dpool, cands, wl, taps)
+    sl = DrySlots(pool, dpool, cands, wl, taps)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     gen = torch.Generator(device="cuda")
     gen.manual_seed(17)
@@ -200,81 +121,7 @@ def test_mixtures_over_dry_picked_slots(world):
             p.close()
 
 
-@pytest.fixture(scope="module")
-def draw_world():
-    """Moving speakers of 12.5 to 20 s (aligned, levels "mono" for the speaker without a dry pick), static noises, and
-    gappy dry streams of 26 s."""
-    rng = np.random.default_rng(321)
-    spk = []
-    for j in range(4):
-        P, N = 3 + j % 3, 200000 + 37003 * j
-        b = np.round(np.linspace(0, N, P)).astype(np.int32)
-        spk.append(Cand(gappy_dry(rng, N), so.synth_rirs(rng, P, 2, 4096), b))
-    noi = [Cand(so.synth_dry(rng, 180000 + 51001 * j), so.synth_rirs(rng, 1, 2, 4096)[0], None) for j in range(3)]
-    dry = [gappy_dry(rng, 26 * RATE) for _ in range(6)]
-    return spk, noi, dry
-
-
 LEN = 4 * RATE
-
-
-class DrawStep:
-    """B examples: speaker 0 dry-picked, speaker 1 dry-picked or not (`mixed`), a pooled noise; one CropDraw each."""
-
-    def __init__(self, R, render, sp, npool, dpool, B, mixed=True, thr=-40.0, tries=101, dry=True):
-        d = "cuda"
-        self.B, self.mixed, self.thr = B, mixed, thr
-        self.picks = torch.zeros((B, 3), dtype=torch.int32, device=d)
-        self.dpicks = torch.zeros((B, 2), dtype=torch.int32, device=d)
-        self.starts = torch.zeros(B, dtype=torch.int32, device=d)
-        self.u = torch.zeros((B, tries), dtype=torch.float64, device=d)
-        self.used = torch.full((B,), -7, dtype=torch.int32, device=d)
-        self.outs = [torch.empty((2, LEN), device=d) for _ in range(3 * B)]
-        self.srcs, self.draws = [], []
-        for b in range(B):
-            dp0 = render.DryPick(dpool, self.dpicks[b, 0]) if dry else None
-            dp1 = render.DryPick(dpool, self.dpicks[b, 1]) if dry and not mixed else None
-            self.srcs += [render.Pooled(sp, self.picks[b, 0], (self.starts[b], LEN), 0, dp0),
-                          render.Pooled(sp, self.picks[b, 1], (self.starts[b], LEN), 0, dp1),
-                          render.Pooled(npool, self.picks[b, 2], (self.starts[b], LEN))]
-            self.draws.append(render.CropDraw(self.starts[b], [3 * b, 3 * b + 1], self.u[b], self.used[b], thr))
-        self.plan = R.plan_device(self.srcs, self.outs, draws=self.draws)
-
-    def fill(self, gen, ns, nn, nd):
-        self.picks[:, :2].copy_(torch.randint(0, ns, (self.B, 2), generator=gen, device="cuda", dtype=torch.int32))
-        self.picks[:, 2].copy_(torch.randint(0, nn, (self.B,), generator=gen, device="cuda", dtype=torch.int32))
-        self.dpicks.copy_(torch.randint(0, nd, (self.B, 2), generator=gen, device="cuda", dtype=torch.int32))
-        self.u.uniform_(generator=gen)
-        for o in self.outs:
-            o.fill_(NAN)
-
-    def snap(self):
-        return dict(picks=self.picks.clone(), dpicks=self.dpicks.clone(), starts=self.starts.clone(),
-                    used=self.used.clone(), u=self.u.clone(), outs=[o.clone() for o in self.outs])
-
-    def check(self, snap, spk, noi, dry_dev, Tp, Td, what, stems=True):
-        """Every example against draw_reference on the device's tables; returns (checked, near)."""
-        picks, dpicks = snap["picks"].cpu().numpy(), snap["dpicks"].cpu().numpy()
-        starts, used, u = snap["starts"].cpu().numpy(), snap["used"].cpu().numpy(), snap["u"].cpu().numpy()
-        checked = near = 0
-        for b in range(self.B):
-            p0, p1, pn = (int(v) for v in picks[b])
-            d0, d1 = (int(v) for v in dpicks[b])
-            Nr = [spk[p0].N, spk[p1].N, noi[pn].N]
-            tabs = [Td[d0], Tp[p1] if self.mixed else Td[d1]]
-            s, k = int(starts[b]), int(used[b])
-            assert 0 <= s <= min(Nr) - LEN, (what, b, s, Nr)
-            if stems:
-                for j, (c, x) in enumerate(((spk[p0], dry_dev[d0]), (spk[p1], None if self.mixed else dry_dev[d1]),
-                                            (noi[pn], None))):
-                    want = reference(c, x, s, LEN, 0)[0] if x is not None else c.full[:, s:s + LEN]
-                    assert torch.equal(snap["outs"][3 * b + j], want), (what, b, j)
-            if dr.margins(tabs, [LEN, LEN], Nr, LEN, u[b], self.thr) < NEAR_DB:
-                near += 1
-                continue
-            assert (s, k) == dr.draw(tabs, [LEN, LEN], Nr, LEN, u[b], self.thr), (what, b, Nr)
-            checked += 1
-        return checked, near
 
 
 @pytest.fixture(scope="module")
@@ -365,7 +212,7 @@ def test_clamped_dry_pick(world):
     cands, taps = world["speakers"]
     signals = dry_signals(313, 3, max(c.N for c in cands), 7)
     pool, dpool = R.source_pool([c.src for c in cands]), R.dry_pool(signals)
-    sl = Slots(pool, dpool, cands, 5000, taps, k=2)
+    sl = DrySlots(pool, dpool, cands, 5000, taps, k=2)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     try:
         torch.cuda.synchronize()
@@ -398,8 +245,8 @@ def test_launches_paths_and_side_stream(world):
     cands, taps = world["speakers"]
     signals = dry_signals(314, 4, max(c.N for c in cands), 50)
     pool, dpool = R.source_pool([c.src for c in cands]), R.dry_pool(signals)
-    sl = Slots(pool, dpool, cands, 7000, taps)
-    bare_sl = Slots(pool, dpool, cands, 7000, taps, dry=False)
+    sl = DrySlots(pool, dpool, cands, 7000, taps)
+    bare_sl = DrySlots(pool, dpool, cands, 7000, taps, dry=False)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     bare = R.plan_device(bare_sl.srcs, bare_sl.outs, direct_outs=bare_sl.douts)
     gen = torch.Generator(device="cuda")
@@ -462,7 +309,7 @@ def test_launches_paths_and_side_stream(world):
     banks2 = [R2.rir_bank(to(c.h), direct_taps=taps) for c in cands]
     pool2 = R2.source_pool([render.MovingSource(to(c.x), bk, to(c.b), c.b) for c, bk in zip(cands, banks2)])
     dpool2 = R2.dry_pool(signals)
-    sl2 = Slots(pool2, dpool2, cands, 7000, taps)
+    sl2 = DrySlots(pool2, dpool2, cands, 7000, taps)
     plan2 = R2.plan_device(sl2.srcs, sl2.outs, direct_outs=sl2.douts)
     try:
         for a, b in ((sl2.picks, sl.picks), (sl2.dpicks, sl.dpicks), (sl2.starts, sl.starts)):

@@ -19,8 +19,6 @@ slot may read.  The float64 references run window by window (L - 1 samples of co
   E. dry level tables at k_levels tile edges and unaligned signals, and a pool of 65 542 signals (two k_levels launches);
   F. lifetimes: a dry pool closed under two live plans, its caller's tensors dropped, and its memory returned."""
 import gc
-import os
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pytest
@@ -31,11 +29,12 @@ from chunk_budget import DEFAULT_CHUNK_BYTES, chunk_budget  # noqa: F401  (fixtu
 from direct_path import direct_path_rirs
 from oracle import sonicsim_oracle as so
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, dry_signal, render_check_inputs, rir_set
-from test_gpu_host_pool_scale import Cand, _bounds_of, _random_cuts, a_aligned, a_mixed_k, a_static
-from test_gpu_plan_draw import NEAR_DB, TABLE_TOL, gappy_dry
-from test_gpu_plan_pool import _choice
-from test_gpu_plan_scale import Out, check_mixture, fold
-from test_gpu_pool_builds import EDGE, LARGE, NL, NN, NS, SMALL, TSTARS, WB, Z0, Z1, Case, _device_errors
+from draw_reference import NEAR_DB, TABLE_TOL, gappy_dry
+from gpu_plumbing import _R, _device_errors, _rms, pmap, to
+from mix_reference import Out, check_mixture, fold
+from pool_worlds import (Case, EDGE, LARGE, NL, NN, NS, SMALL, ScaleCand, TSTARS, WB, Z0, Z1, _bounds_of, _random_cuts,
+                         a_aligned, a_mixed_k, a_static)
+from window_cases import _choice
 
 pytestmark = pytest.mark.gpu
 
@@ -45,25 +44,6 @@ TAPS = 40
 NAN = float("nan")
 STATS = {}                       # section / variant -> [worst local ratio, worst global relative RMS]
 QUIET = {}                       # section / variant -> number of quiet crops held to the scale-relative rule
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _rms(v):
-    return float(np.sqrt(np.mean(np.square(v, dtype=np.float64))))
-
-
-def pmap(fn, jobs):
-    """fn over jobs on a thread pool (the float64 FFTs release the GIL); exceptions propagate."""
-    with ThreadPoolExecutor(max(1, min(16, os.cpu_count() or 1))) as ex:
-        return list(ex.map(fn, jobs))
 
 
 def _report(section):
@@ -203,18 +183,18 @@ def a_grid(rng):
         np.random.seed(510 + j)
         b = _bounds_of(so.setup_dynamic_interp(so.synth_path(rng, P), N)[0], P)
         assert _choice(b, N, P, B) == 0
-        out.append(Cand(so.synth_dry(rng, N), rir_set("delay" if j % 2 else "synth", rng, P, 3, B), b))
+        out.append(ScaleCand(so.synth_dry(rng, N), rir_set("delay" if j % 2 else "synth", rng, P, 3, B), b))
     return out
 
 
 def a_long(rng):
     """Long RIRs (L = 32768: K = 8, and K = 5) at reduced N."""
-    return [Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, L), np.round(np.linspace(0, N, P)).astype(np.int32))
+    return [ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, L), np.round(np.linspace(0, N, P)).astype(np.int32))
             for N, P, L in ((90001, 5, 32768), (100002, 4, 20000), (80003, 6, 32768))]
 
 
 def a_static_long(rng):
-    return [Cand(so.synth_dry(rng, N), so.synth_rirs(rng, 1, 2, L), None)
+    return [ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, 1, 2, L), None)
             for N, L in ((66001, 8192), (70002, 12000), (80003, 5000))]
 
 
@@ -379,7 +359,7 @@ C_KINDS = ["dry aligned", "plain grid", "dry long", "unpooled", "dry grid", "pla
 
 
 def c_pools(rng):
-    aligned = [Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, B), np.round(np.linspace(0, N, P)).astype(np.int32))
+    aligned = [ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, B), np.round(np.linspace(0, N, P)).astype(np.int32))
                for N, P in ((20001, 3), (24002, 4), (28003, 3))]
     assert all(_choice(c.b, c.N, c.P, B) == 1 for c in aligned)
     grid = []
@@ -387,8 +367,8 @@ def c_pools(rng):
         np.random.seed(530 + j)
         b = _bounds_of(so.setup_dynamic_interp(so.synth_path(rng, 30), N)[0], 30)
         assert _choice(b, N, 30, B) == 0
-        grid.append(Cand(so.synth_dry(rng, N), so.synth_rirs(rng, 30, 2, B), b))
-    longs = [Cand(so.synth_dry(rng, N), so.synth_rirs(rng, 3, 2, L), _random_cuts(rng, 3, N))
+        grid.append(ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, 30, 2, B), b))
+    longs = [ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, 3, 2, L), _random_cuts(rng, 3, N))
              for N, L in ((21001, 9000), (26002, 12288))]
     return {"aligned": DevPool(aligned), "grid": DevPool(grid), "long": DevPool(longs)}
 
@@ -466,8 +446,8 @@ def test_multi_chunk_plan_over_two_dry_pools(chunk_budget):
     sig = [dry_set(rng, n_max, 6), dry_set(rng, n_max + 11, 5, tails=(0, 3, 1, 2, 9))]
     sig = [(d, h) for h, d in sig]
     dps = [R.dry_pool(sig[0][0]), R.dry_pool(sig[1][0])]
-    ext = [Cand(so.synth_dry(rng, 30001), so.synth_rirs(rng, 4, 2, 6000), np.array([0, 9000, 20000, 30001], np.int32)),
-           Cand(so.synth_dry(rng, 27001), so.synth_rirs(rng, 1, 2, 3000), None)]
+    ext = [ScaleCand(so.synth_dry(rng, 30001), so.synth_rirs(rng, 4, 2, 6000), np.array([0, 9000, 20000, 30001], np.int32)),
+           ScaleCand(so.synth_dry(rng, 27001), so.synth_rirs(rng, 1, 2, 3000), None)]
     banks = [R.rir_bank(to(ext[0].h)), R.rir_bank(to(ext[1].h[0]))]
     extra = {"unpooled": (ext[0], render.MovingSource(to(ext[0].x), banks[0], to(ext[0].b), ext[0].b)),
              "static": (ext[1], render.StaticSource(to(ext[1].x), banks[1]))}
@@ -548,7 +528,7 @@ def traj_beacon(rng, N):
     h = np.zeros((1, 2, 64), np.float32)
     h[0, :, 0] = 1.0
     h[0, :, 1:] = rng.standard_normal((2, 63)) * 0.05 * np.exp(-np.arange(1, 64) / 16.0)
-    return Cand(so.synth_dry(rng, N) * np.float32(6.0), h, None)
+    return ScaleCand(so.synth_dry(rng, N) * np.float32(6.0), h, None)
 
 
 @pytest.fixture(scope="module")
@@ -710,9 +690,9 @@ def test_training_plan_of_dry_picked_examples():
     mixture each: stems against render_device, mixtures against mix_reference, draws against draw_reference."""
     render, R = _R()
     rng = np.random.default_rng(1402)
-    spk = DevPool([Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, B), np.round(np.linspace(0, N, P)).astype(np.int32))
+    spk = DevPool([ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, B), np.round(np.linspace(0, N, P)).astype(np.int32))
                    for N, P in ((150001, 4), (160002, 5), (170003, 6), (155004, 4), (165005, 5), (175006, 3))])
-    noi = DevPool([Cand(so.synth_dry(rng, N), so.synth_rirs(rng, 1, 2, 2048), None) for N in (160001, 170002, 180003)])
+    noi = DevPool([ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, 1, 2, 2048), None) for N in (160001, 170002, 180003)])
     n_max = max(spk.n_max, noi.n_max)
     dry_h = [gappy_dry(rng, n_max + 1000 * j) for j in range(24)]
     dry_d = [to(x) for x in dry_h]
@@ -852,8 +832,8 @@ def test_pool_past_one_levels_launch():
     dp = R.dry_pool(sig, levels=True)
     assert R.launch_count() == 2
     again = R.dry_pool(sig, levels=True)
-    tp = DevPool([Cand(so.synth_dry(rng, 40), so.synth_rirs(rng, 1, 1, 8), None),
-                  Cand(so.synth_dry(rng, 48), so.synth_rirs(rng, 1, 1, 8), None)], levels="mono")
+    tp = DevPool([ScaleCand(so.synth_dry(rng, 40), so.synth_rirs(rng, 1, 1, 8), None),
+                  ScaleCand(so.synth_dry(rng, 48), so.synth_rirs(rng, 1, 1, 8), None)], levels="mono")
     try:
         assert dp.nbytes == 8 * N_BIG + 8 * int((lens + 1).sum()) + 8 * N_BIG
         q = _tables_of(dp, lens)

@@ -26,10 +26,10 @@ import torch
 from oracle import sonicsim_oracle as so
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs
 from direct_path import direct_path_rirs
-from test_gpu_dry_pool import DrawStep, Slots, draw_world, reference  # noqa: F401  (draw_world: a fixture)
-from test_gpu_plan_draw import gappy_dry
-from test_gpu_plan_pool import _mix_dev, noises, speakers
-from test_gpu_pool_lengths import moving
+from draw_reference import gappy_dry
+from gpu_plumbing import _R, _rms, to
+from pool_worlds import DrawStep, DrySlots, _host_pool, _mix_dev, moving, noises, reference, speakers
+from pool_worlds import draw_world  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -37,24 +37,6 @@ TAPS = 40
 NAN = float("nan")
 RATE = 16000
 SLEEP = int(5e8)
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _host_pool(R, render, cands, taps=0, levels=None, lufs=None):
-    """The candidates over host banks, NumPy dry signals and bounds: the pool copies them."""
-    out = []
-    for c in cands:
-        bank = R.rir_bank(c.h, direct_taps=taps, host=True)
-        out.append(render.MovingSource(c.x, bank, c.b, c.b) if c.b is not None else render.StaticSource(c.x, bank))
-    return R.source_pool(out, levels=levels, lufs_targets=lufs)
 
 
 @pytest.fixture(scope="module")
@@ -107,11 +89,11 @@ def test_bits_equal_device_dry_pool_and_render_device(world, kind, resident):
     ddry = R.dry_pool(cuda)
     assert hdry.resident == "host" and hdry.n_min == n_max and hdry.sizes == [x.numel() for x in cuda]
     wl = 9000 if kind != "noise" else 20000
-    sl = Slots(pool, hdry, cands, wl, taps)
+    sl = DrySlots(pool, hdry, cands, wl, taps)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     twin = None
     if resident == "device":                                  # a device dry pool only on a device pool's slots
-        tw = Slots(pool, ddry, cands, wl, taps)
+        tw = DrySlots(pool, ddry, cands, wl, taps)
         twin = (tw, R.plan_device(tw.srcs, tw.outs, direct_outs=tw.douts))
     gen = torch.Generator(device="cuda")
     gen.manual_seed(41)
@@ -235,7 +217,7 @@ def test_clamped_dry_pick_on_a_staged_slot(world, resident):
     cands, taps, pools = world["speakers"]
     given, cuda = signal_set(413, max(c.N for c in cands))
     hdry = R.dry_pool(given[:3], host=True)
-    sl = Slots(pools[resident], hdry, cands, 5000, taps, k=2)
+    sl = DrySlots(pools[resident], hdry, cands, 5000, taps, k=2)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     try:
         torch.cuda.synchronize()
@@ -277,7 +259,7 @@ def test_launches_and_side_stream(world):
         sets = {}
         for name, pool, dpool, dry in (("dev+host", pools["device"], hdry, True), ("dev+dev", pools["device"], ddry, True),
                                        ("host+host", pools["host"], hdry, True), ("host", pools["host"], hdry, False)):
-            sl = Slots(pool, dpool, cands, 7000, taps, dry=dry)
+            sl = DrySlots(pool, dpool, cands, 7000, taps, dry=dry)
             plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
             plans.append(plan)
             sl.fill(gen, len(cands), hdry.n, n_min)
@@ -445,10 +427,6 @@ def test_refusals(world):
 LEN, U, S = 4 * RATE, 16, 2
 
 
-def _rms(v):
-    return float(np.sqrt(np.mean(np.square(np.asarray(v, np.float64)))))
-
-
 def test_training_scale(draw_world):
     """16 examples x (2 speakers + noise), every slot dry-picked from 64 gappy streams of 60 s held in host memory, one
     CropDraw over the dry tables and one mixture per example, on device and on host source pools.  Every stem, mixture,
@@ -544,7 +522,7 @@ def test_direct_stems_of_a_host_pool_against_float64(world):
     cands, taps, pools = world["speakers"]
     given, cuda = signal_set(418, max(c.N for c in cands))
     hdry = R.dry_pool(given, host=True)
-    sl = Slots(pools["host"], hdry, cands, 6000, taps, k=2)
+    sl = DrySlots(pools["host"], hdry, cands, 6000, taps, k=2)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     try:
         sl.picks.copy_(torch.tensor([0, 3], dtype=torch.int32))

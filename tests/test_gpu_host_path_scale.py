@@ -23,7 +23,6 @@ import contextlib
 import ctypes
 import os
 import time
-from concurrent.futures import ThreadPoolExecutor
 from types import SimpleNamespace
 
 import numpy as np
@@ -35,10 +34,10 @@ from direct_path import direct_path_rirs, normalized
 from mix_reference import F32, overlap_exact
 from oracle import sonicsim_oracle as so
 from render_reference import F, TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs
-from test_gpu_mix_kernels import check_mix
-from test_gpu_window import _host_aligned
-from test_loudness import EXACT_DB, assert_clear_of_gates, block_size_of
-from window_cases import poison, read_set
+from window_cases import _host_aligned, poison, read_set
+from gpu_plumbing import _R, _workers, pmap
+from loudness_cases import EXACT_DB, assert_clear_of_gates, block_size_of
+from mix_reference import check_mix
 
 pytestmark = pytest.mark.gpu
 
@@ -52,11 +51,6 @@ LOUD_SCRATCH_DOUBLES = 20        # SS_LOUD_SCRATCH_DOUBLES
 MB = 1 << 20
 STATS = {}                       # section -> [worst local ratio, worst global relative RMS]
 LUFS = {}                        # section -> worst |LUFS - float64 oracle|
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
 
 
 def _note(key, worst, g):
@@ -73,16 +67,6 @@ def _report(section):
         if k.startswith(section):
             print("\n%-28s worst |LUFS - float64| %.3g dB" % (k, LUFS[k]), end="")
     print()
-
-
-def _workers():
-    return max(1, min(16, os.cpu_count() or 1))
-
-
-def pmap(fn, jobs):
-    """fn over jobs on a thread pool (the float64 FFTs release the GIL); exceptions propagate."""
-    with ThreadPoolExecutor(_workers()) as ex:
-        return list(ex.map(fn, jobs))
 
 
 # ------------------------------------------------------------------------------------------------ references

@@ -23,14 +23,15 @@ import torch
 
 import draw_reference as dr
 from chunk_budget import DEFAULT_CHUNK_BYTES, chunk_budget  # noqa: F401  (fixture)
-from direct_path import direct_path_rirs
 from oracle import sonicsim_oracle as so
-from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, delay_rirs, graded_dry, render_check_inputs
-from test_gpu_plan_draw import NEAR_DB, TABLE_TOL, gappy_dry
-from test_gpu_plan_pool import _choice
-from test_gpu_plan_scale import Out, check_mixture, fold
-from test_gpu_pool_builds import STEM_BYTES, align_up, stem_groups, table_error
-from test_host_pool import stage_set_np
+from render_reference import delay_rirs, graded_dry
+from window_cases import stage_set_np
+from draw_reference import NEAR_DB, TABLE_TOL, gappy_dry
+from gpu_plumbing import _R, to
+from mix_reference import Out, check_mixture, fold
+from pool_worlds import (A_LENS, QUIET, STATS, STEM_BYTES, ScaleCand, _bounds_of, _random_cuts, a_aligned, a_mixed_k,
+                         a_static, align_up, stem_groups, table_error)
+from window_cases import _choice
 
 pytestmark = pytest.mark.gpu
 
@@ -40,17 +41,6 @@ TAPS = 40
 TRIES = 101
 ONE_CHUNK = 1 << 30
 PINNED_MAX = 2 << 30
-STATS = {}                       # section / variant -> [worst local ratio, worst global relative RMS]
-QUIET = {}                       # section / variant -> labels of crops whose global error is taken against the scale
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def _report(title):
@@ -59,46 +49,6 @@ def _report(title):
         if k.startswith(title.split(":")[0]):
             print("  %-40s worst per-sample ratio %.3g, worst global relative RMS %.3g; %d quiet crops%s" % (
                 k, *STATS[k], len(QUIET.get(k, [])), (" (first: %s)" % QUIET[k][0]) if k in QUIET else ""))
-
-
-def _rms(v):
-    return float(np.sqrt(np.mean(np.square(v, dtype=np.float64))))
-
-
-def _note(key, worst, g):
-    s = STATS.setdefault(key, [0.0, 0.0])
-    s[0], s[1] = max(s[0], worst), max(s[1], g)
-
-
-class Cand:
-    """One candidate: dry x (N,), RIRs h (P, C, L) (P = 1: static), bounds (P,) or None, K partitions."""
-
-    def __init__(self, x, h, b):
-        self.x, self.h, self.b = np.ascontiguousarray(x, np.float32), np.ascontiguousarray(h, np.float32), b
-        self.N, (self.P, self.C, self.L) = len(x), h.shape
-        self.K = (self.L + B - 1) // B
-        self.mode = 0 if b is None else 1
-
-    def check(self, y, a, wl, direct=False, gain=1.0, key="", label=""):
-        """Sample by sample against float64 at window start a (times the float32 gain of the pool), and as a whole for
-        crops of at least one block: relative RMS against the crop's RMS, or, for a quiet crop (RMS under 2^-6 of its
-        rounding scale's: quiet graded blocks next to loud ones), against the scale's RMS.  Such a crop carries the
-        rounding of its loud neighbours' transforms, which its own RMS does not measure - e.g. the direct stem of the
-        aligned pool's candidate 0 at 42001 + 12293 samples: RMS 6.8e-4 of its scale's, error 1.3e-4 of its RMS and
-        8.6e-8 of the scale's."""
-        h = direct_path_rirs(self.h, TAPS) if direct else self.h
-        y64, scale = render_check_inputs(self.x, h if self.P > 1 else h[0], self.mode, bounds=self.b, window=(a, wl))
-        g = float(np.float32(gain))
-        y64, scale = y64 * g, scale * g
-        key = key + (" direct" if direct else "")
-        quiet = wl >= B and _rms(y64) < _rms(scale) / 64
-        worst, gl = check_render(y, y64, scale, TAU_LOCAL, TAU_GLOBAL if wl >= B and not quiet else np.inf, n0=a,
-                                 label=label)
-        if quiet:
-            gl = _rms(np.asarray(y, np.float64) - y64) / _rms(scale)
-            assert gl <= TAU_GLOBAL, "%s: quiet crop, global RMS %.3g of the scale's > %.3g" % (label, gl, TAU_GLOBAL)
-            QUIET.setdefault(key, []).append(label)
-        _note(key, worst, gl if wl >= B else 0.0)
 
 
 def pool_variant(cands):
@@ -162,12 +112,7 @@ def _hold(*pools):
     return total
 
 
-def _bounds_of(idx, P):
-    return np.concatenate([[0], np.cumsum(np.bincount(idx, minlength=P - 1))]).astype(np.int32)
-
-
 # ----------------------------------------------------------------------------------------- A. staged crops
-A_LENS = [64000, 3 * B + 5, 3001]
 
 
 def a_grid(rng):
@@ -179,32 +124,8 @@ def a_grid(rng):
         np.random.seed(500 + j)
         b = _bounds_of(so.setup_dynamic_interp(so.synth_path(rng, P), N)[0], P)
         assert _choice(b, N, P, 4096) == 0
-        out.append(Cand(graded_dry(rng, N), delay_rirs(rng, P, 3, 4096)[0], b))
+        out.append(ScaleCand(graded_dry(rng, N), delay_rirs(rng, P, 3, 4096)[0], b))
     return out
-
-
-def a_aligned(rng):
-    out = []
-    for j, N in enumerate((65001, 90002, 130003)):
-        P = 4 + j
-        b = np.round(np.linspace(0, N, P)).astype(np.int32)
-        assert _choice(b, N, P, 4096) == 1
-        out.append(Cand(graded_dry(rng, N), so.synth_rirs(rng, P, 2, 4096), b))
-    return out
-
-
-def a_mixed_k(rng):
-    out = []
-    for j, (N, L) in enumerate(((70001, 3000), (81002, 4097), (66003, 9000), (90000, 16384))):
-        P = 3 + j % 3
-        b = np.round(np.linspace(0, N, P)).astype(np.int32)
-        out.append(Cand(graded_dry(rng, N), delay_rirs(rng, P, 1, L)[0], b))
-    return out
-
-
-def a_static(rng):
-    return [Cand(graded_dry(rng, N), so.synth_rirs(rng, 1, 5, L), None)
-            for N, L in ((66001, 2048), (70002, 4096), (80003, 3000))]
 
 
 A_POOLS = {"grid": (a_grid, False, "k_render<0,0>"), "aligned": (a_aligned, True, "k_render_fast"),
@@ -341,19 +262,12 @@ def b_configs1(rng):
     static 6-channel noises."""
     import bench
     items = bench.make_inputs(16, 0)
-    spk = [Cand(gappy_dry(rng, len(x)) if j % 2 else x, h, b) for j, (x, h, b) in enumerate(items)]
+    spk = [ScaleCand(gappy_dry(rng, len(x)) if j % 2 else x, h, b) for j, (x, h, b) in enumerate(items)]
     N, C = bench.CFG["N"], bench.CFG["C"]
-    noi = [Cand((rng.standard_normal(N) * 0.05).astype(np.float32),
+    noi = [ScaleCand((rng.standard_normal(N) * 0.05).astype(np.float32),
                 (rng.standard_normal((1, C, 4096)) * np.exp(-np.arange(4096) / 800.0)).astype(np.float32), None)
            for _ in range(16)]
     return spk, noi
-
-
-def _random_cuts(rng, P, N, span=None):
-    """Random cuts over [0, N], or over a random stretch of `span` samples (short segments: grid blocking)."""
-    at = 0 if span is None else int(rng.integers(0, N - span))
-    cuts = at + np.sort(rng.integers(0, (N if span is None else span) + 1, P - 2))
-    return np.concatenate([[0], cuts, [N]]).astype(np.int32)
 
 
 class Training:
@@ -500,11 +414,11 @@ def test_training_p60_pool_with_gains():
     rng = np.random.default_rng(702)
     N, P, C = 30 * RATE, 60, 6
     rirs = [so.synth_rirs(rng, P, C, 4096) for _ in range(32)]
-    spk = [Cand(gappy_dry(rng, N) if j % 3 == 0 else so.synth_dry(rng, N), rirs[j % 32],
+    spk = [ScaleCand(gappy_dry(rng, N) if j % 3 == 0 else so.synth_dry(rng, N), rirs[j % 32],
                 _random_cuts(rng, P, N, None if j % 4 else 60000))
            for j in range(40)]
     assert {_choice(c.b, N, P, 4096) for c in spk} == {0, 1}
-    stat = [Cand(so.synth_dry(rng, N - 1000 * j),
+    stat = [ScaleCand(so.synth_dry(rng, N - 1000 * j),
                  (rng.standard_normal((1, C, 4096)) * np.exp(-np.arange(4096) / 800.0)).astype(np.float32), None)
             for j in range(16)]
     targets = [float(rng.uniform(-30, -16)) if j % 5 else None for j in range(len(spk))]
@@ -530,7 +444,7 @@ def test_training_mixed_k_pool():
     for j, (x, h, b) in enumerate(items):
         L = Ls[j % 4]
         hh = h if L == 4096 else so.synth_rirs(rng, h.shape[0], h.shape[1], L)
-        spk.append(Cand(gappy_dry(rng, len(x)) if j % 2 else x, hh, b))
+        spk.append(ScaleCand(gappy_dry(rng, len(x)) if j % 2 else x, hh, b))
     pools = {"spk": Pools(spk, levels="mono")}
     _hold(*pools.values())
     try:
@@ -549,9 +463,9 @@ def test_mixed_plan_of_host_device_dry_and_unpooled_slots():
     rng = np.random.default_rng(801)
     grid, aligned = Pools(a_grid(rng)), Pools(a_aligned(rng), taps=True)
     dev = Pools(a_aligned(rng))
-    longs = [Cand(so.synth_dry(rng, 40000 + 3 * j), so.synth_rirs(rng, 3, 2, 9000),
+    longs = [ScaleCand(so.synth_dry(rng, 40000 + 3 * j), so.synth_rirs(rng, 3, 2, 9000),
                   np.array([0, 15000 + j, 40000 + 3 * j], np.int32)) for j in range(2)]
-    static = Cand(so.synth_dry(rng, 50001), so.synth_rirs(rng, 1, 2, 2048), None)
+    static = ScaleCand(so.synth_dry(rng, 50001), so.synth_rirs(rng, 1, 2, 2048), None)
     _hold(grid, aligned, dev)
     dry = [so.synth_dry(rng, 140000) for _ in range(3)]
     dpool = R.dry_pool([to(x) for x in dry])
@@ -628,7 +542,7 @@ def test_mixed_plan_of_host_device_dry_and_unpooled_slots():
                     c = dev.cands[pk[j]]
                 elif k == "dry":
                     d = dev.cands[pk[j]]
-                    c = Cand(dry[dp[j]][:d.N], d.h, d.b)
+                    c = ScaleCand(dry[dp[j]][:d.N], d.h, d.b)
                 elif k == "unpooled long":
                     c = longs[pk[j]]
                 else:
@@ -683,7 +597,7 @@ def test_many_staged_slots():
     cands = []
     for j in range(6):
         N, P = 20001 + 1001 * j, 3 + j % 3
-        cands.append(Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 1, 2000), _random_cuts(rng, P, N)))
+        cands.append(ScaleCand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 1, 2000), _random_cuts(rng, P, N)))
     pl = Pools(cands)
     _hold(pl)
     n, wl = 1056, 1500
@@ -741,7 +655,7 @@ def d_speakers(rng):
     for j, (x, _, _) in enumerate(items):
         n = N - cut.get(j, 0)
         b = _random_cuts(rng, P, n)
-        out.append(Cand(gappy_dry(rng, n) * np.float32(4.0) if j % 2 else x[:n].copy(), so.synth_rirs(rng, P, C, 4096), b))
+        out.append(ScaleCand(gappy_dry(rng, n) * np.float32(4.0) if j % 2 else x[:n].copy(), so.synth_rirs(rng, P, C, 4096), b))
     return out
 
 
@@ -753,7 +667,7 @@ def d_giant(rng):
             P, L, N = 400, 12288, 400003
         else:
             P, L, N = 5, 4096, 300001 + 7 * j
-        out.append(Cand(so.synth_dry(rng, N) * np.float32(0.5 + 0.25 * (j % 3)), so.synth_rirs(rng, P, 8, L),
+        out.append(ScaleCand(so.synth_dry(rng, N) * np.float32(0.5 + 0.25 * (j % 3)), so.synth_rirs(rng, P, 8, L),
                         np.round(np.linspace(0, N, P)).astype(np.int32)))
     return out
 

@@ -3,73 +3,20 @@ restatement of oracle/sonicsim_oracle.py, everywhere the library uses them: ss_l
 heterogeneous batches (1-8 channels, clips shorter than a gating block, both layouts, unaligned and odd-sized buffers,
 every output mode) at five sample rates, the gating edges, ss_render_host_ex split into many chunks, and the argument
 checks.  Loudness must match to 1e-6 dB, and every output must be exactly float32(gain) * input."""
-import contextlib
 import ctypes
-import os
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import sonicsim_oracle as so
-from test_loudness import (EXACT_DB, PARTITION_CASES, RATES, REFINES, assert_clear_of_gates, block_size_of,
-                           n_samples_for, stems)
+from gpu_plumbing import small_host_budget_context
+from loudness_cases import (EXACT_DB, MALFORMED, PARTITION_CASES, RATES, REFINES, Stem, _reference, _scene, _stem_shape,
+                            assert_clear_of_gates, block_size_of, n_samples_for, stems)
 
 pytestmark = pytest.mark.gpu
 
 NAN = float("nan")
-
-
-def _reference(x, sr):
-    return so.bs1770_integrated_loudness(x, sr, block_size_of(x.shape[0], sr), up_to_8_channels=True)
-
-
-class Stem:
-    """One ss_loud_item on the device.  `x` (N, C) float32; layout "nc" (interleaved) or "cn" (channel-major); `out`
-    "none" (measure only), "alias" (normalised in place) or "sep" (a separate NaN-filled buffer); `off` floats in
-    front of the data in its buffer (1 = not 16-byte aligned: k_loud_scale's scalar path); `refine` as gating_plan's."""
-
-    def __init__(self, x, sr, target, layout="cn", out="sep", off=0, pad=3, refine=1):
-        from sonicsim_b200.SonicSim_audio import gating_plan
-        self.x, self.sr, self.target, self.layout, self.mode, self.off = x, sr, target, layout, out, off
-        N, C = x.shape
-        self.N, self.C, self.n = N, C, N * C
-        self.block = block_size_of(N, sr)
-        brk, lo, hi = gating_plan(N, float(sr), float(self.block), refine)
-        dense = x.T.reshape(-1) if layout == "cn" else x.reshape(-1)
-        self.buf = torch.full((off + self.n + pad,), NAN, device="cuda")
-        self.buf[off:off + self.n] = torch.from_numpy(np.ascontiguousarray(dense)).cuda()
-        self.obuf = torch.full_like(self.buf, NAN) if out == "sep" else None
-        self.tabs = [torch.from_numpy(a.astype(np.int32)).cuda() for a in (brk, lo, hi)]
-        self.scratch = torch.empty(20 * C * (len(brk) - 1), dtype=torch.float64, device="cuda")
-        self.res = torch.full((2,), NAN, dtype=torch.float64, device="cuda")
-        sn, sc = (1, N) if layout == "cn" else (C, 1)
-        data = self.buf.data_ptr() + 4 * off
-        outp = {"none": None, "alias": data, "sep": None if self.obuf is None else self.obuf.data_ptr() + 4 * off}[out]
-        from sonicsim_b200 import _lib
-        self.item = _lib.SsLoudItem(data=data, out=outp, brk=self.tabs[0].data_ptr(), blk_lo=self.tabs[1].data_ptr(),
-                                    blk_hi=self.tabs[2].data_ptr(), scratch=self.scratch.data_ptr(),
-                                    result=self.res.data_ptr(), stride_n=sn, stride_c=sc, N=N, C=C, n_e=len(brk) - 1,
-                                    n_blocks=len(lo), rate=float(sr), block_size=float(self.block),
-                                    target_lufs=float(target))
-
-    def lufs_gain(self):
-        r = self.res.cpu().numpy()
-        return float(r[0]), float(r[1])
-
-    def output(self):
-        """The scaled stem as (N, C), or None when measuring only; checks that nothing around it was written."""
-        if self.mode == "none":
-            assert torch.equal(self.buf[self.off:self.off + self.n].cpu(),
-                               torch.from_numpy(np.ascontiguousarray(self.dense_input())))
-            return None
-        b = (self.obuf if self.mode == "sep" else self.buf).cpu().numpy()
-        assert np.all(np.isnan(b[:self.off])) and np.all(np.isnan(b[self.off + self.n:]))
-        flat = b[self.off:self.off + self.n]
-        return flat.reshape(self.C, self.N).T if self.layout == "cn" else flat.reshape(self.N, self.C)
-
-    def dense_input(self):
-        return self.x.T.reshape(-1) if self.layout == "cn" else self.x.reshape(-1)
 
 
 def loudness_dev(stems_):
@@ -279,54 +226,6 @@ def test_loudness_dev_gating_edges(sr, name):
 
 
 # ---- ss_render_host_ex split into many chunks
-@contextlib.contextmanager
-def small_host_budget_context():
-    """A context of its own whose host pipeline budget is 1 MB (SS_HOST_CHUNK_MB is read by ss_create), destroyed on
-    exit."""
-    from sonicsim_b200 import render
-    lib, device = render.default_renderer().lib, render.default_renderer().device
-    old = os.environ.get("SS_HOST_CHUNK_MB")
-    os.environ["SS_HOST_CHUNK_MB"] = "1"
-    ctx = ctypes.c_void_p()
-    try:
-        assert lib.ss_create(device, ctypes.byref(ctx)) == 0
-    finally:
-        if old is None:
-            del os.environ["SS_HOST_CHUNK_MB"]
-        else:
-            os.environ["SS_HOST_CHUNK_MB"] = old
-    try:
-        yield ctx
-    finally:
-        lib.ss_destroy(ctx)
-
-
-def _stem_shape(s):
-    return (s.rirs.shape[1] if hasattr(s, "rirs") else s.rir.shape[0]), s.dry.shape[0]
-
-
-def _scene(rng, n_sources=12):
-    """Moving, static and long-RIR sources with C = 1..8 and different N; some without targets, one with a direct
-    target.  Returns (sources, targets, direct index)."""
-    from sonicsim_b200 import render
-    srcs, targets = [], []
-    for i in range(n_sources):
-        C = 1 + i % 8
-        N = int(rng.integers(20000, 70000)) if i != 5 else 5000              # one clip shorter than a gating block
-        kind = i % 3
-        L = int(rng.integers(4097, 9000)) if kind == 2 else int(rng.integers(200, 3000))
-        x = so.synth_dry(rng, N)
-        if kind == 0:
-            srcs.append(render.StaticSource(x, so.synth_rirs(rng, 1, C, L)[0]))
-        else:
-            P = int(rng.integers(3, 9))
-            pos = so.synth_path(rng, P)
-            np.random.seed(i)
-            srcs.append(render.MovingSource(x, so.synth_rirs(rng, P, C, L), render.trajectory_bounds(pos, N)))
-        targets.append(None if i in (2, 7, 10) else float(rng.uniform(-33, -15)))
-    direct = 4
-    srcs[direct] = srcs[direct]._replace(direct_taps=40)
-    return srcs, targets, direct
 
 
 def _check_scene(srcs, targets, direct, run):
@@ -438,9 +337,6 @@ def test_render_host_ex_rejects_mixed_rates_and_wide_stems_before_any_copy():
 
 
 # one malformed field of an ss_post_lufs entry with a target (ctypes: None is a NULL pointer)
-MALFORMED = {"blk_lo NULL": ("blk_lo", None), "blk_hi NULL": ("blk_hi", None), "n_e 0": ("n_e", 0),
-             "n_blocks -1": ("n_blocks", -1), "rate 0": ("rate", 0.0), "rate NaN": ("rate", NAN),
-             "block_size 0": ("block_size", 0.0), "block_size NaN": ("block_size", NAN)}
 
 
 def _results(post, i):

@@ -9,112 +9,14 @@ import numpy as np
 import pytest
 import torch
 
-from mix_reference import (F32, assert_clear_of_f32_midpoint, compose_mix, f32_neighbours, mix_gains_f64,
-                           overlap_exact, ulps_f32)
+from mix_reference import F32, assert_clear_of_f32_midpoint, mix_gains_f64, overlap_exact
+from gpu_plumbing import _stream, renderer
+from mix_reference import MAX_ULPS, Mix, MixBuf, check_mix, mix_dev
 
 pytestmark = pytest.mark.gpu
 
 NAN = float("nan")
-PAD = 64
 SS_ERR_INVALID, SS_ERR_UNSUPPORTED = -1, -5
-MAX_ULPS = [0]          # largest gain error seen, in float32 steps from fl32(g64)
-
-
-def _lib():
-    from sonicsim_b200 import render
-    return render.default_renderer()
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-class Buf:
-    """`n` values at `off` elements past a NaN guard of PAD elements, followed by PAD NaNs."""
-
-    def __init__(self, n, off=0, data=None, dtype=torch.float32):
-        self.n, self.lo = int(n), PAD + off
-        self.t = torch.full((PAD + off + self.n + PAD,), NAN, dtype=dtype, device="cuda")
-        if data is not None:
-            self.t[self.lo:self.lo + self.n] = torch.from_numpy(np.ascontiguousarray(data).reshape(-1)).cuda()
-
-    @property
-    def ptr(self):
-        return self.t.data_ptr() + self.lo * self.t.element_size()
-
-    def get(self):
-        return self.t[self.lo:self.lo + self.n].cpu().numpy()
-
-    def guards_nan(self):
-        a = self.t.cpu().numpy()
-        return bool(np.all(np.isnan(a[:self.lo])) and np.all(np.isnan(a[self.lo + self.n:])))
-
-
-class Mix:
-    """One ss_mix_item over guarded buffers.  out: "null", "sep" (its own buffer) or "alias" (== speakers)."""
-
-    def __init__(self, spk, noise, sirs, snr, delay=0, out="sep", offs=(0, 0, 0, 0)):
-        from sonicsim_b200 import _lib as L
-        self.spk, self.noise = np.asarray(spk, F32), np.asarray(noise, F32)
-        self.S, self.E = self.spk.shape
-        self.M = self.noise.shape[0]
-        self.sirs = np.asarray(sirs, F32).reshape(-1)[:self.S - 1]
-        self.snr, self.delay, self.mode = F32(snr), int(delay), out
-        self.b_spk = Buf(self.S * self.E, offs[0], self.spk)
-        self.b_noise = Buf(self.M * self.E, offs[1], self.noise)
-        self.b_mix = Buf(self.E, offs[2])
-        self.b_out = Buf(self.S * self.E, offs[3]) if out == "sep" else None
-        self.b_sirs = Buf(max(self.S - 1, 1), 0, self.sirs if self.S > 1 else None)
-        self.b_scr = Buf(int(_lib().lib.ss_mix_scratch_doubles()), 0, dtype=torch.float64)
-        outp = {"null": None, "sep": self.b_out.ptr if self.b_out else None, "alias": self.b_spk.ptr}[out]
-        self.item = L.SsMixItem(speakers=self.b_spk.ptr, noises=self.b_noise.ptr, sirs=self.b_sirs.ptr,
-                                mix=self.b_mix.ptr, speakers_out=outp, scratch=self.b_scr.ptr, E=self.E, S=self.S,
-                                M=self.M, snr=float(self.snr), noise_delay=self.delay)
-
-    def bufs(self):
-        return [b for b in (self.b_spk, self.b_noise, self.b_mix, self.b_out, self.b_sirs, self.b_scr) if b]
-
-    def outputs(self):
-        """(mix, speakers_out or None); checks the guards and that the speakers are unchanged unless aliased."""
-        assert all(b.guards_nan() for b in self.bufs())
-        spk = self.b_spk.get().reshape(self.S, self.E)
-        if self.mode == "alias":
-            return self.b_mix.get(), spk
-        assert np.array_equal(spk, self.spk)
-        return self.b_mix.get(), None if self.b_out is None else self.b_out.get().reshape(self.S, self.E)
-
-
-def mix_dev(cases):
-    R = _lib()
-    arr = (type(cases[0].item) * len(cases))(*[c.item for c in cases])
-    st = R.lib.ss_mix_dev(R.ctx, arr, len(cases), _stream())
-    torch.cuda.synchronize()
-    return st
-
-
-def recover(out, x, g64):
-    """The float32 gains g among +-3 ulps of fl32(g64) with out == fl(x * g) everywhere."""
-    fits = [g for g in f32_neighbours(g64) if np.array_equal(out, x * g)]
-    assert fits, ("no float32 gain within 3 ulps reproduces the output", g64)
-    MAX_ULPS[0] = max(MAX_ULPS[0], min(ulps_f32(g, g64) for g in fits))
-    return fits[0]
-
-
-def check_mix(c, mix, spk_out):
-    """Gains within 3 ulps of mix_gains_f64, g_0 == 1, and mix / speakers_out bit for bit compose_mix with them.
-    Returns the recovered (g, gn)."""
-    g64, gn64 = mix_gains_f64(c.spk, c.noise, c.sirs, c.snr, c.delay)
-    assert spk_out is not None
-    assert np.array_equal(spk_out[0], c.spk[0])                            # g_0 is exactly 1
-    g = np.array([F32(1.0)] + [recover(spk_out[s], c.spk[s], g64[s]) for s in range(1, c.S)], F32)
-    speech, out = compose_mix(c.spk, np.zeros((1, c.E), F32), g, 0.0)
-    assert np.array_equal(out, spk_out)
-    noise = compose_mix(np.zeros((1, c.E), F32), c.noise, [1.0], 1.0, c.delay)[0]
-    fits = [gn for gn in f32_neighbours(gn64) if np.array_equal(mix, speech + noise * gn)]
-    assert fits, ("mix is not the composition with any noise gain within 3 ulps", gn64)
-    MAX_ULPS[0] = max(MAX_ULPS[0], min(ulps_f32(gn, gn64) for gn in fits))
-    assert np.array_equal(mix, compose_mix(c.spk, c.noise, g, fits[0], c.delay)[0])
-    return g, fits[0]
 
 
 def run_and_check(cases):
@@ -308,7 +210,7 @@ def test_mix_refuses_overlapping_ranges():
            item(speakers_out=mix - 4 * (S * E - 1)),            # speakers_out's last float is mix's first
            item(scratch=mix),                                   # scratch on the mix
            item(speakers_out=spk, mix=spk + 4 * (2 * E - 1))]   # in place, and mix meets the speakers
-    R = _lib()
+    R = renderer()
     before = arena.cpu().numpy()
     for it in bad:
         arr = (L.SsMixItem * 2)(item(), it)
@@ -325,7 +227,7 @@ def test_mix_limits():
     from sonicsim_b200 import _lib as L
     rng = np.random.default_rng(4)
     c = Mix(stems(rng, 1, 64), stems(rng, 1, 64), [], 10.0, 0, "null")
-    R = _lib()
+    R = renderer()
     arr = (L.SsMixItem * 65536)(*([c.item] * 65536))
     assert R.lib.ss_mix_dev(R.ctx, arr, 65536, _stream()) == SS_ERR_UNSUPPORTED
     torch.cuda.synchronize()
@@ -346,7 +248,7 @@ def test_mix_limits():
 
 # ---- ss_overlap_dev
 def overlap_dev(x, y, rows, T, D):
-    R = _lib()
+    R = renderer()
     st = R.lib.ss_overlap_dev(R.ctx, ctypes.c_void_p(x), ctypes.c_void_p(y), rows, T, D, _stream())
     torch.cuda.synchronize()
     return st
@@ -357,7 +259,7 @@ def test_overlap_matches_exact(rows, T):
     rng = np.random.default_rng(rows * 7 + T)
     x = rng.standard_normal((rows, T)).astype(F32)
     for i, D in enumerate((0, 1, T - 1, T, T + 3, 1 << 40)):
-        bx, by = Buf(rows * T, i % 4, x), Buf(rows * T, (i + 1) % 4)
+        bx, by = MixBuf(rows * T, i % 4, x), MixBuf(rows * T, (i + 1) % 4)
         assert overlap_dev(bx.ptr, by.ptr, rows, T, D) == 0
         assert bx.guards_nan() and by.guards_nan() and np.array_equal(bx.get(), x.reshape(-1))
         assert np.array_equal(by.get().reshape(rows, T), overlap_exact(x, D)), (rows, T, D)
@@ -366,13 +268,13 @@ def test_overlap_matches_exact(rows, T):
 def test_overlap_limits():
     rng = np.random.default_rng(1)
     x = rng.standard_normal(65536).astype(F32)
-    bx, by = Buf(65536, 0, x), Buf(65536, 1)
+    bx, by = MixBuf(65536, 0, x), MixBuf(65536, 1)
     assert overlap_dev(bx.ptr, by.ptr, 65535, 1, 0) == 0
     assert np.array_equal(by.get()[:65535], x[:65535] * F32(3)) and np.isnan(by.get()[65535])
-    by = Buf(65536)
+    by = MixBuf(65536)
     assert overlap_dev(bx.ptr, by.ptr, 65536, 1, 0) == SS_ERR_UNSUPPORTED
     # y overlapping x without being x: refused, y untouched (x in the middle of one buffer, every y inside it)
-    b = Buf(900, 0, rng.standard_normal(900).astype(F32))
+    b = MixBuf(900, 0, rng.standard_normal(900).astype(F32))
     before = b.t.cpu().numpy()
     x0 = b.ptr + 4 * 300
     for shift in (1, 4, 299, -1, -299):

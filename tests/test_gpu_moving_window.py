@@ -10,8 +10,8 @@ import numpy as np
 import pytest
 import torch
 
-from window_cases import CASES, full_blocks, make_case
-from test_gpu_window import _host_aligned
+from window_cases import CASES, _host_aligned, full_blocks, make_case
+from gpu_plumbing import _error_bits, _lib
 
 pytestmark = pytest.mark.gpu
 
@@ -21,18 +21,6 @@ PAD = 37
 # direct set, so that the source renders both stems from it
 FLAGS = {"plain": (False, False, False), "normalize": (True, False, False), "direct": (False, True, False),
          "bank": (True, True, True)}
-
-
-def _lib():
-    from sonicsim_b200 import _lib as L, render
-    return L, render.default_renderer()
-
-
-def _errors():
-    L_, R = _lib()
-    bits = ctypes.c_uint32()
-    L_.check(R.lib.ss_device_errors(R.ctx, ctypes.byref(bits)))
-    return bits.value
 
 
 class Out:
@@ -151,7 +139,7 @@ def _snap_all(outs):
 @pytest.mark.parametrize("name", list(CASES))
 def test_plan_with_moving_windows(name, flagset):
     L_, R = _lib()
-    _errors()
+    _error_bits()
     case = Case(name, flagset)
     try:
         lens = _lengths(case.N)
@@ -199,7 +187,7 @@ def test_plan_with_moving_windows(name, flagset):
                     a = int(table[k, j])
                     for o, r in zip(wouts[j], ref):
                         assert np.array_equal(Out.stem(o.buf, case.C, n, name), r[:, a:a + n]), ("dev", name, n, a)
-            assert _errors() == 0
+            assert _error_bits() == 0
         finally:
             R.lib.ss_plan_destroy(plan)
     finally:
@@ -209,7 +197,7 @@ def test_plan_with_moving_windows(name, flagset):
 @pytest.mark.parametrize("name", ["bounds", "indexed", "static2", "long8"])
 def test_out_of_range_starts_are_clamped(name):
     L_, R = _lib()
-    _errors()
+    _error_bits()
     case = Case(name, "plain")
     n = 5000
     N = case.N
@@ -227,8 +215,8 @@ def test_out_of_range_starts_are_clamped(name):
             wout[0].reset()
             L_.check(R.lib.ss_plan_run(plan, None))
             bad = v < 0 or v > N - n
-            assert _errors() == (4 if bad else 0), v            # reported once ...
-            assert _errors() == 0, v                            # ... and cleared by the read
+            assert _error_bits() == (4 if bad else 0), v            # reported once ...
+            assert _error_bits() == 0, v                            # ... and cleared by the read
             a = min(max(v, 0), N - n)
             assert np.array_equal(Out.stem(wout[0].buf, case.C, n, name), ref[:, a:a + n]), (name, v)
     finally:
@@ -242,7 +230,7 @@ def test_python_api_shared_starts_and_mixed_batch():
     clamped start."""
     from sonicsim_b200 import render
     R = render.default_renderer()
-    _errors()
+    _error_bits()
     x, h, idx, w, bounds, taps = make_case("bounds")
     N, C = x.shape[0], h.shape[1]
     to = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()

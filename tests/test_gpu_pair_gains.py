@@ -23,24 +23,15 @@ import pytest
 import torch
 
 from oracle import sonicsim_oracle as so
-from test_gpu_dry_pool import Slots, dry_signals, reference, world  # noqa: F401  (world: a fixture)
-from test_gpu_host_dry_pool import _host_pool
-from test_gpu_plan_draw import gappy_dry
-from test_gpu_plan_pool import Cand, _mix_dev
+from draw_reference import gappy_dry
+from gpu_plumbing import _R, to
+from pool_worlds import Cand, DrySlots, _host_pool, _mix_dev, dry_signals, reference
+from pool_worlds import world  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
 NAN = float("nan")
 RATE = 16000
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def host_pair(R, render, c, x, t):
@@ -150,7 +141,7 @@ def test_stems_are_the_plain_stems_times_the_pair_gain(world, kind):
     pool, dpool = R.source_pool([c.src for c in cands]), R.dry_pool(signals)
     pg = R.pair_gains(pool, dpool, targets_for(612, 5, len(cands)), sr=RATE)
     wl = 9000 if kind != "noise" else 20000
-    sl_g, sl_p = Slots(pool, dpool, cands, wl, taps), Slots(pool, dpool, cands, wl, taps)
+    sl_g, sl_p = DrySlots(pool, dpool, cands, wl, taps), DrySlots(pool, dpool, cands, wl, taps)
     plan_g = R.plan_device(with_gains(sl_g.srcs, pg), sl_g.outs, direct_outs=sl_g.douts)
     plan_p = R.plan_device(sl_p.srcs, sl_p.outs, direct_outs=sl_p.douts)
     gen = torch.Generator(device="cuda")
@@ -194,7 +185,7 @@ def test_host_forms_equal_the_device_form(world):
     try:
         for pr, dr_ in (("device", "device"), ("device", "host"), ("host", "host")):
             pg = R.pair_gains(pools[pr], dpools[dr_], t, sr=RATE)
-            sl = Slots(pools[pr], dpools[dr_], cands, wl, taps)
+            sl = DrySlots(pools[pr], dpools[dr_], cands, wl, taps)
             plan = R.plan_device(with_gains(sl.srcs, pg), sl.outs, direct_outs=sl.douts)
             held += [plan, pg]
             forms[(pr, dr_)] = (sl, plan)
@@ -249,7 +240,7 @@ def test_pair_gain_replaces_the_pool_gain(world):
     dpool = R.dry_pool(sig)
     pg_plain, pg_gain = R.pair_gains(plain, dpool, t, sr=RATE), R.pair_gains(gpool, dpool, t, sr=RATE)
     assert np.array_equal(pg_plain.loudness, pg_gain.loudness, equal_nan=True)
-    sl_a, sl_b = Slots(gpool, dpool, cands, 9000, taps), Slots(plain, dpool, cands, 9000, taps)
+    sl_a, sl_b = DrySlots(gpool, dpool, cands, 9000, taps), DrySlots(plain, dpool, cands, 9000, taps)
     held = [pg_plain, pg_gain, plain, gpool, dpool]
     try:
         with pytest.raises(ValueError, match="loudness gains"):
@@ -375,12 +366,12 @@ def test_refusals_write_nothing(world):
         pg = R.pair_gains(pool, dpool, -20.0, sr=RATE)
         held.insert(0, pg)
         # a PairGains of another pool, or of another dry pool, in a plan
-        sl = Slots(other, dpool, cands[:2], 3000, 0, k=2)
+        sl = DrySlots(other, dpool, cands[:2], 3000, 0, k=2)
         with pytest.raises(ValueError, match="another SourcePool or DryPool"):
             R.plan_device(with_gains(sl.srcs, pg), sl.outs)
         pg.close()
         with pytest.raises(ValueError, match="is closed"):
-            R.plan_device(with_gains(Slots(pool, dpool, cands, 3000, 0, k=2).srcs, pg), sl.outs)
+            R.plan_device(with_gains(DrySlots(pool, dpool, cands, 3000, 0, k=2).srcs, pg), sl.outs)
         pg = R.pair_gains(pool, dpool, -20.0, sr=RATE)
         held.insert(0, pg)
 
@@ -434,7 +425,7 @@ def test_refusals_write_nothing(world):
         held.append(wpool)
         c_call(p=wpool._h, ps=(L.SsPostLufs * 1)(post[0]), tg=np.full(2, -20.0), want=L.SS_ERR_UNSUPPORTED)
         # plans: a table of another pool or another dry pool than the pick's
-        sl = Slots(pool, dpool, cands, 3000, 0, k=2)
+        sl = DrySlots(pool, dpool, cands, 3000, 0, k=2)
         items, ni, keep = R._device_items(sl.srcs, sl.outs)
         arr = R._device_dry(sl.srcs)
         pg_other = R.pair_gains(other, dpool, -20.0, sr=RATE)

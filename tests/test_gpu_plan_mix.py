@@ -13,7 +13,8 @@ import pytest
 import torch
 
 from mix_reference import F32, _rms_db, compose_mix, mix_gains_f64
-from test_gpu_mix_kernels import Mix, check_mix, mix_dev
+from gpu_plumbing import renderer
+from mix_reference import Mix, check_mix, fold, mix_dev
 
 pytestmark = pytest.mark.gpu
 
@@ -21,11 +22,6 @@ SENT = 1234.5
 PAD = 32                # floats: a view at PAD is 16-byte aligned (the float4 path), at PAD + off it is not
 SR = 16000
 SS_ERR_INVALID, SS_ERR_UNSUPPORTED = -1, -5
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render.default_renderer()
 
 
 class Guarded:
@@ -59,7 +55,7 @@ class Stems:
     def __init__(self, rng, kind, banked=False, direct=False, C=2, N=48000, T=16000, L=900):
         from oracle import sonicsim_oracle as so
         from sonicsim_b200 import render
-        self.R, self.rng, self.kind, self.banked, self.direct = _R(), rng, kind, banked, direct
+        self.R, self.rng, self.kind, self.banked, self.direct = renderer(), rng, kind, banked, direct
         self.C, self.N, self.L = C, N, L
         self.T = N if kind == "whole" else T
         self.so, self.render = so, render
@@ -114,14 +110,6 @@ class Stems:
     def close(self):
         for b in self.banks:
             b.close()
-
-
-def fold(a):
-    a = np.asarray(a, F32)
-    acc = a[0].copy()
-    for c in range(1, a.shape[0]):
-        acc = acc + a[c]
-    return acc / F32(a.shape[0])
 
 
 class Scene:

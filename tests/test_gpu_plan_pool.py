@@ -19,75 +19,14 @@ import torch
 
 from oracle import sonicsim_oracle as so
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs
+from gpu_plumbing import _R, to
+from pool_worlds import (Cand, PooledSlots, TAPS, _draw_training, _mix_dev, _training_plan, fold_dev, longs, noises,
+                         speakers)
+from window_cases import _choice
 
 pytestmark = pytest.mark.gpu
 
-TAPS = 40
 NAN = float("nan")
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _choice(b, N, P, L):
-    """The blocking the library picks for one moving candidate on its own (ss_debug_plan): 1 = aligned."""
-    from sonicsim_b200 import _lib
-    item = _lib.SsSource(x=1, rir=1, out=1, bounds=b.ctypes.data, bounds_host=b.ctypes.data, N=N, P=P, C=1, L=L,
-                         mode=_lib.SS_MOVING_BOUNDS)
-    blk = np.zeros((N // 4096 + P + 8, 4), np.int32)
-    al = ctypes.c_int32()
-    assert _lib.load().ss_debug_plan(ctypes.byref(item), blk.ctypes.data, blk.shape[0], ctypes.byref(al)) > 0
-    return al.value
-
-
-class Cand:
-    """One candidate: host inputs, its banked source and its full stem(s) rendered by ss_render_dev."""
-
-    def __init__(self, x, h, b, taps=0):
-        render, R = _R()
-        self.x, self.h, self.b, self.N = x, h, b, len(x)
-        self.C, self.L = h.shape[-2], h.shape[-1]
-        self.bank = R.rir_bank(to(h), direct_taps=taps)
-        self.src = (render.MovingSource(to(x), self.bank, to(b), b) if b is not None
-                    else render.StaticSource(to(x), self.bank))
-        self.full = torch.empty((self.C, self.N), device="cuda")
-        self.full_d = torch.empty((self.C, self.N), device="cuda") if taps else None
-        R.render_device([self.src._replace(direct_taps=taps)], [self.full],
-                        direct_outs=[self.full_d] if taps else None)
-
-
-def speakers(seed, n=5, C=2, taps=TAPS):
-    """Moving candidates with a few long segments (aligned blocking on their own), all different P and N."""
-    rng = np.random.default_rng(seed)
-    out = []
-    for j in range(n):
-        P, N = 3 + j % 3, 30000 + 4099 * j
-        b = np.round(np.linspace(0, N, P)).astype(np.int32)
-        assert _choice(b, N, P, 4096) == 1
-        out.append(Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, C, 4096), b, taps))
-    return out
-
-
-def noises(seed, n=4, C=2):
-    rng = np.random.default_rng(seed)
-    return [Cand(so.synth_dry(rng, 26000 + 3001 * j), so.synth_rirs(rng, 1, C, 4096)[0], None) for j in range(n)]
-
-
-def longs(seed, n=3):
-    """Moving candidates with L > 4096 (K = 3): grid blocking, k_render<LONG>."""
-    rng = np.random.default_rng(seed)
-    out = []
-    for j in range(n):
-        P, N = 3 + j % 2, 24000 + 5003 * j
-        b = np.round(np.linspace(0, N, P)).astype(np.int32)
-        out.append(Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 1, 9000), b))
-    return out
 
 
 def mixed(seed):
@@ -107,48 +46,6 @@ def mixed(seed):
 POOLS = {"speakers": speakers, "noise": noises, "long": longs}
 
 
-class Slots:
-    """k pooled slots over one pool with device starts, plus one with a fixed start; NaN-filled outputs."""
-
-    def __init__(self, pool, cands, wl, k=4, fixed=123, taps=0):
-        render, _ = _R()
-        self.pool, self.cands, self.wl, self.fixed, self.taps = pool, cands, wl, fixed, taps
-        self.picks = torch.zeros(k + 1, dtype=torch.int32, device="cuda")
-        self.starts = torch.zeros(k, dtype=torch.int32, device="cuda")
-        self.srcs = [render.Pooled(pool, self.picks[j], (self.starts[j], wl), taps) for j in range(k)]
-        self.srcs.append(render.Pooled(pool, self.picks[k], (fixed, wl), taps))
-        C = cands[0].C
-        self.outs = [torch.empty((C, wl), device="cuda") for _ in self.srcs]
-        self.douts = [torch.empty((C, wl), device="cuda") for _ in self.srcs] if taps else None
-
-    def draw(self, rng, pk=None, st=None):
-        n = len(self.cands)
-        pk = rng.integers(0, n, len(self.srcs)) if pk is None else np.asarray(pk)
-        if st is None:
-            st = [int(rng.integers(0, self.cands[p].N - self.wl + 1)) for p in pk[:-1]]
-        self.pk, self.st = [int(v) for v in pk], [int(v) for v in st] + [self.fixed]
-        self.picks.copy_(torch.tensor(self.pk, dtype=torch.int32))
-        self.starts.copy_(torch.tensor(self.st[:-1], dtype=torch.int32))
-        for o in self.outs + (self.douts or []):
-            o.fill_(NAN)
-
-    def check(self, what):
-        """Every output against ss_render_dev of the picked candidate with a fixed window, and the full stem's slice."""
-        _, R = _R()
-        refs = [torch.empty_like(o) for o in self.outs]
-        drefs = [torch.empty_like(o) for o in self.outs] if self.taps else None
-        R.render_device([self.cands[p].src._replace(window=(a, self.wl), direct_taps=self.taps)
-                         for p, a in zip(self.pk, self.st)], refs, direct_outs=drefs)
-        torch.cuda.synchronize()
-        for j, (p, a) in enumerate(zip(self.pk, self.st)):
-            c = self.cands[p]
-            assert torch.equal(self.outs[j], refs[j]), (what, j, p, a)
-            assert torch.equal(self.outs[j], c.full[:, a:a + self.wl]), (what, j, p, a)
-            if self.taps:
-                assert torch.equal(self.douts[j], drefs[j]), (what, "direct", j, p, a)
-                assert torch.equal(self.douts[j], c.full_d[:, a:a + self.wl]), (what, "direct", j, p, a)
-
-
 @pytest.mark.parametrize("kind", list(POOLS))
 def test_pooled_outputs_equal_the_picked_candidate(kind):
     render, R = _R()
@@ -156,7 +53,7 @@ def test_pooled_outputs_equal_the_picked_candidate(kind):
     pool = R.source_pool([c.src for c in cands])
     taps = TAPS if kind == "speakers" else 0
     wl = 9000
-    sl = Slots(pool, cands, wl, taps=taps)
+    sl = PooledSlots(pool, cands, wl, taps=taps)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     rng = np.random.default_rng(1)
     try:
@@ -180,7 +77,7 @@ def test_launches_equal_fixed_moving_windows():
     render, R = _R()
     cands = speakers(8, taps=0)
     pool = R.source_pool([c.src for c in cands])
-    sl = Slots(pool, cands, 9000)
+    sl = PooledSlots(pool, cands, 9000)
     fixed = [c.src._replace(window=(sl.starts[j], 9000)) for j, c in enumerate(cands[:4])]
     fixed.append(cands[4].src._replace(window=(sl.fixed, 9000)))
     p_pool = R.plan_device(sl.srcs, sl.outs)
@@ -208,7 +105,7 @@ def test_mixed_blocking_against_float64():
     cands = mixed(9)
     pool = R.source_pool([c.src for c in cands])
     wl = 12000
-    sl = Slots(pool, cands, wl)
+    sl = PooledSlots(pool, cands, wl)
     plan = R.plan_device(sl.srcs, sl.outs)
     rng = np.random.default_rng(2)
     try:
@@ -235,7 +132,7 @@ def test_pool_shared_by_plans_and_closed_under_them():
     cands = noises(10)
     pool = R.source_pool([c.src for c in cands])
     assert pool.nbytes == 40 * len(cands)
-    a, b = Slots(pool, cands, 5000), Slots(pool, cands, 7000, k=6)
+    a, b = PooledSlots(pool, cands, 5000), PooledSlots(pool, cands, 7000, k=6)
     pa, pb = R.plan_device(a.srcs, a.outs), R.plan_device(b.srcs, b.outs)
     pool.close()                                          # both plans keep it alive
     assert pool.closed and pool._h
@@ -261,63 +158,6 @@ def test_pool_shared_by_plans_and_closed_under_them():
     assert not pool._h                                    # freed with the last plan
 
 
-def _mix_dev(R, spk, noi, sirs, snr):
-    """ss_mix_dev on stems already folded: spk (S, T), noi (M, T) -> mix (T,), speakers after their gains (S, T)."""
-    from sonicsim_b200 import _lib
-    S, M = spk.shape[0], noi.shape[0]
-    spk, noi = spk.contiguous().clone(), noi.contiguous()
-    mix = torch.empty(spk.shape[1], device="cuda")
-    scr = torch.empty(int(R.lib.ss_mix_scratch_doubles()), dtype=torch.float64, device="cuda")
-    it = _lib.SsMixItem(speakers=spk.data_ptr(), noises=noi.data_ptr(), sirs=sirs.data_ptr(), mix=mix.data_ptr(),
-                        speakers_out=spk.data_ptr(), scratch=scr.data_ptr(), E=spk.shape[1], S=S, M=M,
-                        snr=float(snr.item()))
-    _lib.check(R.lib.ss_mix_dev(R.ctx, ctypes.byref(it), 1, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
-    torch.cuda.synchronize()
-    return mix, spk
-
-
-def fold(t):
-    """SS_MIX_MONO's channel mean of a (C, T) tensor, in NumPy: float32 sum in channel order, then an IEEE division by C."""
-    a = t.cpu().numpy()
-    acc = a[0].copy()
-    for c in range(1, a.shape[0]):
-        acc = acc + a[c]
-    return torch.from_numpy(acc / np.float32(a.shape[0])).cuda()
-
-
-def _training_plan(R, render, spk_pool, noi_pool, U, S, T):
-    """U scenes: S pooled speakers and one pooled noise each, one device start per scene, one mono Mixture each."""
-    picks = torch.zeros((U, S), dtype=torch.int32, device="cuda")
-    scene = torch.zeros(U, dtype=torch.int32, device="cuda")
-    starts = torch.zeros(U, dtype=torch.int32, device="cuda")
-    sirs = torch.zeros((U, S - 1), device="cuda")
-    snr = torch.zeros(U, device="cuda")
-    srcs, outs = [], []
-    C = spk_pool.C
-    for u in range(U):
-        srcs += [render.Pooled(spk_pool, picks[u, k], (starts[u], T)) for k in range(S)]
-        srcs.append(render.Pooled(noi_pool, scene[u], (starts[u], T)))
-        outs += [torch.empty((C, T), device="cuda") for _ in range(S + 1)]
-    mix = torch.empty((U, T), device="cuda")
-    spk_out = torch.empty((U, S, T), device="cuda")
-    rms = torch.empty((U, S), device="cuda")
-    mixtures = [render.Mixture(list(range((S + 1) * u, (S + 1) * u + S)), [(S + 1) * u + S], sirs[u], snr[u], mix[u],
-                               spk_out[u], rms[u], mono=True) for u in range(U)]
-    plan = R.plan_device(srcs, outs, mixtures=mixtures)
-    return plan, dict(picks=picks, scene=scene, starts=starts, sirs=sirs, snr=snr, outs=outs, mix=mix,
-                      spk_out=spk_out, rms=rms)
-
-
-def _draw_training(st, n_scenes, S, n_min, T, g):
-    U = st["scene"].numel()
-    sc = torch.randint(0, n_scenes, (U,), device="cuda", dtype=torch.int32, generator=g)
-    st["picks"].copy_(S * sc[:, None] + torch.rand(U, S, device="cuda", generator=g).argsort(1).int())
-    st["scene"].copy_(sc)
-    st["starts"].copy_(torch.randint(0, n_min - T + 1, (U,), device="cuda", dtype=torch.int32, generator=g))
-    st["sirs"].uniform_(-6, 6, generator=g)
-    st["snr"].uniform_(10, 20, generator=g)
-
-
 def _check_training(R, st, spk_cands, noi_cands, S, T, what):
     """Every crop is the slice of its picked candidate's full stem; every mixture equals ss_mix_dev on the crops."""
     torch.cuda.synchronize()
@@ -330,7 +170,7 @@ def _check_training(R, st, spk_cands, noi_cands, S, T, what):
             c = spk_cands[int(picks[u, k])] if k < S else noi_cands[int(scene[u])]
             o = st["outs"][(S + 1) * u + k]
             assert torch.equal(o, c.full[:, a:a + T]), (what, u, k, a)
-            crops.append(fold(o))
+            crops.append(fold_dev(o))
         mix, out = _mix_dev(R, torch.stack(crops[:S]), torch.stack(crops[S:]), st["sirs"][u], st["snr"][u])
         assert torch.equal(mix, st["mix"][u]) and torch.equal(out, st["spk_out"][u]), (what, u)
 
@@ -361,7 +201,7 @@ def test_out_of_range_picks_and_starts_are_clamped():
     cands = noises(13)
     pool = R.source_pool([c.src for c in cands])
     wl = 6000
-    sl = Slots(pool, cands, wl, k=2)
+    sl = PooledSlots(pool, cands, wl, k=2)
     plan = R.plan_device(sl.srcs, sl.outs)
     n = len(cands)
     try:

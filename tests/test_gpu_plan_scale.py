@@ -22,65 +22,24 @@ import torch
 
 from chunk_budget import DEFAULT_CHUNK_BYTES, chunk_budget  # noqa: F401  (fixture)
 from direct_path import direct_path_rirs, normalized
-from mix_reference import F32, _rms_db, compose_mix, f32_neighbours, mix_gains_f64
 from oracle import sonicsim_oracle as so
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs, trajectory
 from window_cases import full_blocks
+from gpu_plumbing import _error_bits, _lib
+from mix_reference import Out, PAD, check_mixture, fold
 
 pytestmark = pytest.mark.gpu
 
-SENT = 1234.5
-PAD = 37
 B = 4096
 ONE_CHUNK = 1 << 30             # a chunk budget that holds every batch of this file in one chunk per kernel variant
 INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
 STATS = {}                      # label -> [worst local ratio, worst global relative RMS]
 
 
-def _lib():
-    from sonicsim_b200 import _lib as L, render
-    return L, render.default_renderer()
-
-
-def _errors():
-    L_, R = _lib()
-    bits = ctypes.c_uint32()
-    L_.check(R.lib.ss_device_errors(R.ctx, ctypes.byref(bits)))
-    return bits.value
-
-
 def _report(title):
     print("\n%s:" % title)
     for k in sorted(STATS):
         print("  %-22s worst per-sample ratio %.3g, worst global relative RMS %.3g" % (k, STATS[k][0], STATS[k][1]))
-
-
-class Out:
-    """A (rows, n) output inside a NaN-filled device buffer with sentinels on both sides."""
-
-    def __init__(self, rows, n):
-        self.rows, self.n = rows, n
-        self.buf = torch.full((rows * n + 2 * PAD,), float("nan"), device="cuda")
-        self.buf[:PAD] = SENT
-        self.buf[-PAD:] = SENT
-
-    def ptr(self):
-        return self.buf.data_ptr() + 4 * PAD
-
-    def view(self, *shape):
-        return self.buf[PAD:PAD + self.rows * self.n].view(*(shape or (self.rows, self.n)))
-
-    def reset(self):
-        self.buf[PAD:-PAD].fill_(float("nan"))
-
-    def get(self, snap=None):
-        """The output of a snapshot of the buffer (default: the buffer now) as (rows, n), sentinels and fill checked."""
-        s = self.buf if snap is None else snap
-        a = s.cpu().numpy() if isinstance(s, torch.Tensor) else s
-        assert np.all(a[:PAD] == SENT) and np.all(a[-PAD:] == SENT), "sentinel overwritten"
-        v = a[PAD:-PAD].reshape(self.rows, self.n)
-        assert not np.isnan(v).any(), "output not written"
-        return v
 
 
 class Src:
@@ -280,7 +239,7 @@ N_SOURCES = [1, 8, 9, 24, 25, 32, 33, 64, 65, 100]
 def test_device_table_chunk_of_n_sources(n, chunk_budget):
     L_, R = _lib()
     chunk_budget(ONE_CHUNK)
-    _errors()
+    _error_bits()
     sc = Scale(n, 100 + n)
     try:
         rng = np.random.default_rng(n)
@@ -321,7 +280,7 @@ def test_device_table_chunk_of_n_sources(n, chunk_budget):
             torch.cuda.synchronize()
             for j, o in enumerate(outs):
                 assert torch.equal(o.buf, snaps[k][j]), ("ss_render_dev", n, j, k)
-        assert _errors() == 0
+        assert _error_bits() == 0
         _report("%d sources in one device-table chunk" % n)
     finally:
         sc.close()
@@ -332,7 +291,7 @@ def test_clamped_starts_at_scale(chunk_budget):
     bit 2 of ss_device_errors, and every other stem keeps its bits."""
     L_, R = _lib()
     chunk_budget(ONE_CHUNK)
-    _errors()
+    _error_bits()
     n = 65
     sc = Scale(n, 100 + n)
     try:
@@ -342,7 +301,7 @@ def test_clamped_starts_at_scale(chunk_budget):
         sc.starts.copy_(torch.from_numpy(valid))
         L_.check(R.lib.ss_plan_run(sc.plan, None))
         before = [o.buf.clone() for o in outs]
-        assert _errors() == 0
+        assert _error_bits() == 0
         bad = valid.copy()
         clamped = {}
         for q, k in enumerate(range(1, len(sc.moving), 3)):
@@ -355,8 +314,8 @@ def test_clamped_starts_at_scale(chunk_budget):
         for o in outs:
             o.reset()
         L_.check(R.lib.ss_plan_run(sc.plan, None))
-        assert _errors() == 4                               # reported once ...
-        assert _errors() == 0                               # ... and cleared by the read
+        assert _error_bits() == 4                               # reported once ...
+        assert _error_bits() == 0                               # ... and cleared by the read
         for j, (s, o) in enumerate(zip(sc.srcs, outs)):
             if j in clamped:
                 s.check(o.get(), clamped[j], label="clamped source %d" % j)
@@ -369,36 +328,6 @@ def test_clamped_starts_at_scale(chunk_budget):
 
 
 # ------------------------------------------------------------------------------------------------ mixtures
-def fold(a):
-    """Channel mean of a (C, T) stem as SS_MIX_MONO computes it: float32 sum in channel order, then / C."""
-    a = np.asarray(a, F32)
-    acc = a[0].copy()
-    for c in range(1, a.shape[0]):
-        acc = acc + a[c]
-    return acc / F32(a.shape[0])
-
-
-def check_mixture(spk, noi, sirs, snr, mix, out, rms, label=""):
-    """A plan mixture against mix_reference: speaker 0 unscaled, every other speaker gain and the noise gain a float32
-    within 3 ulps of the float64 gain, speakers_out and mix bit for bit compose_mix with those gains, rms_db within
-    1e-6 dB of the float64 RMS, or within half a float32 step of it where that is larger (beyond 32 dB from 0 a float32
-    step is 3.8e-6 dB, and rms_db is the float64 value rounded to float32).  spk (S, E), noi (M, E) are the stems the
-    mixture must have read."""
-    S = spk.shape[0]
-    g64, gn64 = mix_gains_f64(spk, noi, sirs, snr)
-    assert np.array_equal(out[0], spk[0]), label
-    g = [F32(1.0)]
-    for s in range(1, S):
-        fits = [v for v in f32_neighbours(g64[s]) if np.array_equal(out[s], spk[s] * v)]
-        assert fits, (label, "speaker", s, g64[s])
-        g.append(fits[0])
-    fits = [v for v in f32_neighbours(gn64) if np.array_equal(mix, compose_mix(spk, noi, g, v)[0])]
-    assert fits, (label, "noise gain", gn64)
-    assert np.array_equal(out, compose_mix(spk, noi, g, fits[0])[1]), label
-    for s in range(S):
-        r64 = _rms_db(spk[s])
-        tol = max(1e-6, 0.5 * float(np.spacing(F32(abs(r64)))) + 1e-12)
-        assert abs(float(rms[s]) - r64) <= tol, (label, s, rms[s], r64)
 
 
 class PlanMix:
@@ -464,7 +393,7 @@ def test_kinds_and_flags_regrouped_in_one_plan(chunk_budget):
     mix_reference."""
     L_, R = _lib()
     chunk_budget(ONE_CHUNK)
-    _errors()
+    _error_bits()
     rng = np.random.default_rng(31)
     C, N, T = 2, 20000, 5000
     order = [(k, f) for f in ("norm", "direct", "bank") for k in ("grid", "fast", "long", "static", "indexed")]
@@ -527,7 +456,7 @@ def test_kinds_and_flags_regrouped_in_one_plan(chunk_budget):
             for q, m in enumerate(mixes):
                 m.check(stems, bufs[j:j + 3], sr_[q], sn_[q], "mixture %d run %d" % (q, k))
                 j += 3
-        assert _errors() == 0
+        assert _error_bits() == 0
         _report("kinds and flags regrouped in one plan")
     finally:
         R.lib.ss_plan_destroy(plan)
@@ -546,7 +475,7 @@ def test_training_step_at_full_scale(budget, chunk_budget):
     import bench
     from sonicsim_b200 import render
     R = chunk_budget(DEFAULT_CHUNK_BYTES)
-    _errors()
+    _error_bits()
     U, T = 16, 4 * 16000
     C, N, S = bench.CFG["C"], bench.CFG["N"], bench.CFG["speakers"]
     items = bench.make_inputs(U, 0)

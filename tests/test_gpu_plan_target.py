@@ -19,6 +19,7 @@ import torch
 
 from mix_reference import F32, f32_neighbours, mix_gains_f64
 from oracle import sonicsim_oracle as so
+from gpu_plumbing import _R, to
 
 pytestmark = pytest.mark.gpu
 
@@ -28,15 +29,6 @@ U = 16                      # examples per step: 2 speakers + 1 noise each
 TRIES = 101
 TAPS = 40
 SS_ERR_INVALID = -1
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 def fold_f32(a):

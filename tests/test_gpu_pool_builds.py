@@ -24,7 +24,6 @@ try's start from the last round.  Checked:
      `used` equals both the design and draw_reference, and every reader's crop the slice of its whole stem;
   C. k_levels tile edges: N from 1 to 2048 k + 1 around the 2048-sample tiles, C in {1, 3, 5, 8}, a silent stretch of
      whole tiles, both table kinds, against the long-double prefix."""
-import ctypes
 import types
 
 import numpy as np
@@ -34,39 +33,15 @@ import torch
 from oracle import sonicsim_oracle as so
 import draw_reference as dr
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs
-from test_gpu_plan_draw import NEAR_DB, TABLE_TOL, Step, check_snap, gappy_dry
-from test_gpu_plan_pool import Cand, _mix_dev, fold
-from test_gpu_pool_loudness import host_src
+from draw_reference import Step, TABLE_TOL, check_snap, gappy_dry
+from gpu_plumbing import _R, _device_errors
+from pool_worlds import (Cand, Case, EDGE, LARGE, LB, NL, NN, NS, SMALL, STEM_BYTES, TSTARS, WB, Z0, Z1, _mix_dev,
+                         align_up, fold_dev, host_src, stem_groups, table_error)
 
 pytestmark = pytest.mark.gpu
 
 RATE = 16000
-STEM_BYTES = 256 << 20         # the transient stem buffer of the pool builds (kLevelStemBytes)
 NAN = float("nan")
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def align_up(v, a):
-    return (v + a - 1) // a * a
-
-
-def stem_groups(C, Ns):
-    """The grouping of the pool builds restated: candidate i takes align_up(4 C N_i, 256) bytes of a buffer of
-    max(256 MiB, largest stem) bytes, and a candidate that does not fit behind the group's others starts a new group.
-    Returns (first candidate of every group + [n], buffer bytes)."""
-    b = [align_up(4 * C * N, 256) for N in Ns]
-    cap = max(STEM_BYTES, max(b))
-    first, used = [0], 0
-    for i, v in enumerate(b):
-        if used > 0 and used + v > cap:
-            first.append(i)
-            used = 0
-        used += v
-    return first + [len(Ns)], cap
 
 
 def host_stem(R, render, c, target=None):
@@ -79,18 +54,6 @@ def host_stem(R, render, c, target=None):
 
 def launches(prof, name):
     return sum(1 for e in prof.events() if name in e.name)
-
-
-def table_error(q, y, mono):
-    """|Q - Q_ref| / Q_ref[N] of a device table against the long-double prefix of stem y (0 when both are 0)."""
-    ref = dr.level_table(y, mono, np.longdouble)
-    assert q.shape == ref.shape and q[0] == 0.0
-    err = float(np.max(np.abs(q.astype(np.longdouble) - ref)))
-    top = float(ref[-1])
-    if top == 0.0:
-        assert err == 0.0
-        return 0.0
-    return err / top
 
 
 # ----------------------------------------------------------------------------------------- A. stem groups
@@ -268,8 +231,8 @@ def test_draws_over_a_multi_group_pool(big):
             for b in range(16):
                 s = int(starts[b])
                 crops = [x.full[:, s:s + LEN] for x in (nspk[picks[b, 0]], nspk[picks[b, 1]], nnoi[picks[b, 2]])]
-                spk_f = torch.stack([fold(crops[0]), fold(crops[1])])
-                mix, _ = _mix_dev(R, spk_f, fold(crops[2])[None], st.sirs[b], st.snr[b])
+                spk_f = torch.stack([fold_dev(crops[0]), fold_dev(crops[1])])
+                mix, _ = _mix_dev(R, spk_f, fold_dev(crops[2])[None], st.sirs[b], st.snr[b])
                 assert torch.equal(st.mix[b], mix), (run, b)
         print("multi-group draws: %d checked, %d near the threshold" % (total, near))
         assert set(edges) <= seen
@@ -283,16 +246,7 @@ def test_draws_over_a_multi_group_pool(big):
 
 
 # ----------------------------------------------------------------------------------------- B. k_draw's warp edges
-WB = 1024                      # window of the beacon draws
-LB = 64                        # RIR taps of the beacon candidates
-EDGE, Z0, Z1 = 3000, 10000, 20000
-NS, NL, NN = 36000, 44000, 32000
-SIL0 = Z0 + LB                 # crops [s, s + WB) with SIL0 <= s <= Z1 - WB render only the zone's zeros
-SIL_SPAN = Z1 - WB - SIL0 + 1
-PASS0, PASS_SPAN = EDGE + 100, Z0 - WB - EDGE - 200     # loud for every candidate
 TRIES_SET = [1, 2, 31, 32, 33, 63, 64, 65, 101, 4095, 4096]
-TSTARS = [0, 1, 30, 31, 32, 33, 63, 64]
-SPECIAL = [0.0, -0.25, NAN, 1.0 - 2.0 ** -53, 1.0]       # tries 32.. of a special case: start 0 (3) and M - 1 (2)
 
 
 def beacon(rng, N, zoned):
@@ -332,60 +286,6 @@ def beacons():
 
 
 # (readers, reader lane of speaker 0, 1, ..., the silent speaker, the shortest reader's lane or None: all long)
-LARGE = [(16, [0, 1, 2, 3, 4, 5, 6, 7], 0, 0),            # victim speaker 0 at lane 0, the shortest
-         (16, [8, 9, 10, 11, 12, 13, 14, 15], 7, 15),     # victim speaker 7 at lane 15, the shortest
-         (16, [0, 1, 2, 3, 4, 5, 6, 7], 7, 15),           # the shortest a noise reader at lane 15
-         (16, [15, 14, 13, 12, 11, 10, 9, 8], 0, 0),      # speaker 0 at lane 15; the shortest a noise reader at lane 0
-         (16, [3, 9, 12, 0, 6, 15, 1, 10], 7, 10),        # scattered speakers, the victim the shortest at lane 10
-         (9, [1, 3, 5, 7, 8], 4, 8),
-         (12, [11, 0, 4, 7], 0, 3),
-         (16, [0, 1, 2, 3, 4, 5, 6, 7], 3, None)]
-SMALL = [(1, [0], 0, 0),
-         (3, [0, 1], 1, None),
-         (3, [2, 0], 0, 2),
-         (2, [1, 0], 1, 1),
-         (3, [0, 1], 0, 2),
-         (3, [1, 2], 1, 0)]
-
-
-class Case:
-    """One designed draw: `lanes` (pool, candidate) per reader, `speakers` reader lanes in speaker order, `u`, and the
-    designed (start, used)."""
-
-    def __init__(self, layout, tries, tstar, special, seed):
-        nr, spk, victim, short = layout
-        self.layout, self.tries, self.tstar = layout, tries, tstar
-        self.speakers = list(spk)
-        self.lanes = []
-        for lane in range(nr):
-            s = lane == short
-            if lane in spk:
-                zoned = spk.index(lane) == victim
-                self.lanes.append(("spk", {(True, True): 0, (False, True): 1, (True, False): 2, (False, False): 3}[
-                    (zoned, s)]))
-            else:
-                self.lanes.append(("noi", 1 if s else 0))
-        self.bad_pick = None
-        self._design(special, seed, victim_shortest=short is not None and short == spk[victim])
-
-    def _design(self, special, seed, victim_shortest):
-        rng = np.random.default_rng(seed)
-        self.M = M = min(NS if p == "spk" and i < 2 else NN if p == "noi" and i == 1 else NL
-                         for p, i in self.lanes) - WB + 1
-        u = rng.random(self.tries)                               # tries after the kept one are never evaluated
-        last = self.tries if self.tstar is None else self.tstar
-        for t in range(last):
-            u[t] = (SIL0 + (t * 7919 + seed) % SIL_SPAN + 0.5) / M
-        if self.tstar is not None:
-            u[self.tstar] = (PASS0 + (seed * 131) % PASS_SPAN + 0.5) / M
-        if special:
-            vals = SPECIAL if victim_shortest else SPECIAL[:3]  # M - 1 is silent only in the shortest's end zone
-            for k, v in enumerate(vals):
-                assert 32 + k < min(last, self.tries - 1)
-                u[32 + k] = v
-        self.u = u
-        k = self.tries - 1 if self.tstar is None else self.tstar
-        self.start, self.used = dr.start_of(u[k], M), (0 if self.tstar is None else self.tstar + 1)
 
 
 def combos():
@@ -453,12 +353,6 @@ class DrawPlan:
 
     def close(self):
         self.plan.close()
-
-
-def _device_errors(R):
-    bits = ctypes.c_uint32()
-    assert R.lib.ss_device_errors(R.ctx, ctypes.byref(bits)) == 0
-    return bits.value
 
 
 def test_draw_warp_edges(beacons):

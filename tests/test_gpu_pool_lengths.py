@@ -20,20 +20,15 @@ from oracle import sonicsim_oracle as so
 import draw_reference as dr
 from direct_path import direct_path_rirs
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs
-from test_gpu_plan_draw import Step, TABLE_TOL
-from test_gpu_plan_pool import Cand, Slots, _choice, _draw_training, _training_plan
-from test_gpu_pool_loudness import gain_pool
+from draw_reference import Step, TABLE_TOL
+from gpu_plumbing import _R
+from pool_worlds import Cand, PooledSlots, _draw_training, _training_plan, gain_pool, moving
 
 pytestmark = pytest.mark.gpu
 
 B = 4096
 TAPS = 40
 NAN = float("nan")
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
 
 
 def _k(L):
@@ -45,18 +40,6 @@ def padded(c, L, taps=0):
     h = np.zeros(c.h.shape[:-1] + (L,), np.float32)
     h[..., :c.L] = c.h
     return Cand(c.x, h, c.b, taps)
-
-
-def moving(seed, Ls, taps=0, aligned=None):
-    rng = np.random.default_rng(seed)
-    out = []
-    for j, L in enumerate(Ls):
-        P, N = 3 + j % 3, 30000 + 4099 * j
-        b = np.round(np.linspace(0, N, P)).astype(np.int32)
-        if aligned is not None:
-            assert _choice(b, N, P, L) == aligned, (L, P, N)
-        out.append(Cand(so.synth_dry(rng, N), so.synth_rirs(rng, P, 2, L), b, taps))
-    return out
 
 
 def static(seed, Ls, N=26000):
@@ -73,7 +56,7 @@ def test_uniform_k_different_lengths(kind):
     pool = R.source_pool([c.src for c in cands])
     assert pool.L == 4096 and pool.nbytes == 40 * len(cands)
     wl = 9000
-    sl = Slots(pool, cands, wl, taps=taps)
+    sl = PooledSlots(pool, cands, wl, taps=taps)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     rng = np.random.default_rng(1)
     try:
@@ -110,7 +93,7 @@ def test_mixed_k(kind):
     pool = R.source_pool([c.src for c in cands])
     assert pool.L == 16384 and pool.nbytes == 44 * len(cands)
     wl = 7000
-    sl = Slots(pool, cands, wl, taps=taps)
+    sl = PooledSlots(pool, cands, wl, taps=taps)
     plan = R.plan_device(sl.srcs, sl.outs, direct_outs=sl.douts)
     n = len(cands)
     try:

@@ -15,7 +15,6 @@ the crop of that normalised stem.  Checked:
   5. a plan over gain pools launches exactly what the same plan over the pools without gains launches, as a graph;
   6. every refusal, in Python and through the C ABI (each malformed field of a target's entry included), leaves the
      pool unchanged."""
-import ctypes
 
 import numpy as np
 import pytest
@@ -23,49 +22,17 @@ import torch
 
 from oracle import sonicsim_oracle as so
 import draw_reference as dr
-from test_gpu_loudness import MALFORMED
-from test_gpu_plan_draw import Step, check_snap, gappy_dry, TABLE_TOL, TRIES
-from test_gpu_plan_pool import Cand, _choice, _mix_dev, fold, to
+from draw_reference import Step, TABLE_TOL, TRIES, check_snap, gappy_dry
+from gpu_plumbing import _R
+from loudness_cases import MALFORMED
+from pool_worlds import Cand, _mix_dev, fold_dev, gain_pool
+from window_cases import _choice
 
 pytestmark = pytest.mark.gpu
 
 RATE = 16000
 NAN = float("nan")
 B = 4096
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def host_src(render, c, taps=0):
-    """The candidate as a host-path source over the same bank."""
-    if c.b is None:
-        return render.StaticSource(c.x, c.bank, direct_taps=taps)
-    return render.MovingSource(c.x, c.bank, c.b, direct_taps=taps)
-
-
-def normalised(R, render, c, target, taps=0):
-    """render_host of the candidate alone with its target: (stem, direct stem or None, (LUFS, gain))."""
-    lo = []
-    d = [np.empty((c.C, c.N), np.float32)] if taps else None
-    out = R.render_host([host_src(render, c, taps)], lufs_targets=[target], loudness_out=lo, sr=RATE, direct_outs=d)[0]
-    return torch.from_numpy(out).cuda(), (torch.from_numpy(d[0]).cuda() if taps else None), lo[0]
-
-
-class NCand:
-    """A candidate's whole normalised stems (what check_snap and the draw reference read as `full`)."""
-
-    def __init__(self, c, full, full_d, loud):
-        self.c, self.N, self.full, self.full_d, self.loud = c, c.N, full, full_d, loud
-
-
-def gain_pool(R, render, cands, targets, taps=0, levels=None):
-    pool = R.source_pool([c.src for c in cands], levels=levels, lufs_targets=targets, sr=RATE)
-    norm = [NCand(c, *normalised(R, render, c, t, taps)) if t is not None else NCand(c, c.full, c.full_d, None)
-            for c, t in zip(cands, targets)]
-    return pool, norm
 
 
 def speakers(seed, n=4, taps=40):
@@ -263,8 +230,8 @@ def test_training_plan_over_gain_pools(world):
             for b in range(st.B):
                 s = int(starts[b])
                 crops = [n.full[:, s:s + LEN] for n in (nspk[picks[b, 0]], nspk[picks[b, 1]], nnoi[picks[b, 2]])]
-                spk_f = torch.stack([fold(crops[0]), fold(crops[1])])
-                mix, spk_out = _mix_dev(R, spk_f, fold(crops[2])[None], st.sirs[b], st.snr[b])
+                spk_f = torch.stack([fold_dev(crops[0]), fold_dev(crops[1])])
+                mix, spk_out = _mix_dev(R, spk_f, fold_dev(crops[2])[None], st.sirs[b], st.snr[b])
                 assert torch.equal(st.mix[b], mix), (run, b)
                 for k in range(2):
                     v = spk_f[k].double()

@@ -35,9 +35,10 @@ from direct_path import direct_path_rirs, normalized
 from mix_reference import F32, compose_mix, f32_neighbours, mix_gains_f64, overlap_exact
 from oracle import sonicsim_oracle as so
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, render_check_inputs
-from test_gpu_dry_kernel import Buf as DryBuf, Clip
-from test_gpu_loudness import Stem, _reference, _scene, _stem_shape, small_host_budget_context
-from test_loudness import EXACT_DB, assert_clear_of_gates, block_size_of, stems as loud_stems
+from gpu_plumbing import small_host_budget_context
+from loudness_cases import (EXACT_DB, Stem, _reference, _scene, _stem_shape, assert_clear_of_gates, block_size_of,
+                            stems as loud_stems)
+from mix_reference import Clip, DryBuf
 
 pytestmark = pytest.mark.gpu
 
@@ -47,12 +48,12 @@ SMALL = 1 << 20             # the smallest device chunk budget: about one source
 DEFAULT_CHUNK_BYTES = 32 << 20
 
 
-def _R():
+def _lib_render():
     from sonicsim_b200 import _lib, render
     return _lib, render, render.default_renderer()
 
 
-def to(a, device="cuda"):
+def to_device(a, device="cuda"):
     return torch.from_numpy(np.ascontiguousarray(a)).to(device)
 
 
@@ -149,15 +150,15 @@ class Source:
 
     def writes(self):
         """(dst, real, poison) of every input; draws a new start for a moving window."""
-        w = [(self.dx, to(self.x, self.dev), NAN), (self.dh, to(self.h, self.dev), NAN)]
+        w = [(self.dx, to_device(self.x, self.dev), NAN), (self.dh, to_device(self.h, self.dev), NAN)]
         if not self.static:
             linear = np.round(np.linspace(0, self.N, self.P)).astype(np.int32)
-            w.append((self.db, to(self.bounds, self.dev), to(linear, self.dev)))
+            w.append((self.db, to_device(self.bounds, self.dev), to_device(linear, self.dev)))
         if self.start is not None:
             hi = self.N - self.n
             self.a = int(self.rng.integers(0, hi + 1))
-            w.append((self.start, to(np.array([self.a], np.int32), self.dev),
-                      to(np.array([other_start(self.rng, self.a, hi)], np.int32), self.dev)))
+            w.append((self.start, to_device(np.array([self.a], np.int32), self.dev),
+                      to_device(np.array([other_start(self.rng, self.a, hi)], np.int32), self.dev)))
         return w
 
     def outs(self):
@@ -223,7 +224,7 @@ def warm(R, srcs):
 def test_render_dev_on_a_side_stream(chunks):
     """One chunk runs serially on s; many chunks fork onto the context's streams and must join back into s before the
     clones.  Whole stems, fixed windows and moving windows whose starts are written behind the sleep."""
-    _lib, render, R = _R()
+    _lib, render, R = _lib_render()
     R.set_chunk_bytes(SMALL if chunks == "many" else 1 << 30)
     try:
         grow_ring(R.lib, R.ctx)
@@ -248,7 +249,7 @@ def test_render_dev_on_a_side_stream(chunks):
 def renderer_for(mode):
     """The default renderer (graph; profiling switched on and off), or one whose own context runs plans without graphs
     (SS_NO_GRAPH is read by ss_create), with a device chunk budget of SMALL."""
-    _lib, render, R = _R()
+    _lib, render, R = _lib_render()
     if mode != "no_graph":
         R.set_chunk_bytes(SMALL)
         R.set_profiling(mode == "profiling")
@@ -284,8 +285,8 @@ class Candidate:
     def __init__(self, R, rng, N, C=2, L=600):
         from sonicsim_b200 import render
         self.x, self.h = so.synth_dry(rng, N), so.synth_rirs(rng, 1, C, L)
-        self.dx = to(self.x)
-        self.th = to(self.h[0])
+        self.dx = to_device(self.x)
+        self.th = to_device(self.h[0])
         self.bank = R.rir_bank(self.th)
         self.src = render.StaticSource(self.dx, self.bank)
 
@@ -343,11 +344,11 @@ def test_plan_runs_on_a_side_stream(mode):
                 ps = [int(v) for v in rng.integers(0, n_min - T + 1, 2)]
                 sv, nv = rng.uniform(-6, 6, (2, 1)).astype(np.float32), rng.uniform(10, 20, 2).astype(np.float32)
                 writes = [w for x in srcs for w in x.writes()]
-                writes += [(c.dx, to(c.x), NAN) for c in cands]
-                writes += [(picks, to(np.array(pk, np.int32)), to(np.array([(v + 1) % 3 for v in pk], np.int32))),
-                           (pstart, to(np.array(ps, np.int32)),
-                            to(np.array([other_start(rng, a, n_min - T) for a in ps], np.int32))),
-                           (sirs, to(sv), NAN), (snr, to(nv), NAN)]
+                writes += [(c.dx, to_device(c.x), NAN) for c in cands]
+                writes += [(picks, to_device(np.array(pk, np.int32)), to_device(np.array([(v + 1) % 3 for v in pk], np.int32))),
+                           (pstart, to_device(np.array(ps, np.int32)),
+                            to_device(np.array([other_start(rng, a, n_min - T) for a in ps], np.int32))),
+                           (sirs, to_device(sv), NAN), (snr, to_device(nv), NAN)]
                 snap_outs = [o for x in srcs for o in x.outs()] + pouts + [mix, spk_out]
                 stage(s, snap_outs, writes)
                 R.reset_stats()
@@ -379,7 +380,7 @@ def test_banks_and_pool_built_behind_queued_work_serve_a_plan_on_another_stream(
     """RIR tensors written behind the sleep on s, banks built from them there (and the tensors NaN-filled right after,
     still on s), a pool over those banks, then at once a plan over the pool and one more banked source run on a second
     stream s2: the run waits for the banks and the pool's `ready` event, recorded from a non-default stream."""
-    _lib, render, R = _R()
+    _lib, render, R = _lib_render()
     rng = np.random.default_rng(21)
     T, C, L = 6000, 2, 600
     xs = [so.synth_dry(rng, 15000 + 1000 * j) for j in range(4)]
@@ -387,11 +388,11 @@ def test_banks_and_pool_built_behind_queued_work_serve_a_plan_on_another_stream(
     hm = so.synth_rirs(rng, 4, C, L)
     N3 = xs[3].size
     bm = legal_bounds(rng, N3, 4)
-    dxs = [to(x) for x in xs]
-    dbm = to(bm)
+    dxs = [to_device(x) for x in xs]
+    dbm = to_device(bm)
     ths = [torch.empty((C, L), device="cuda") for _ in range(3)]
     thm = torch.empty((4, C, L), device="cuda")
-    writes = [(t, to(h[0]), NAN) for t, h in zip(ths, hs)] + [(thm, to(hm), NAN)]
+    writes = [(t, to_device(h[0]), NAN) for t, h in zip(ths, hs)] + [(thm, to_device(hm), NAN)]
     for staged in (False, True):                          # a warm-up on the default stream, then the case
         s, s2 = (side_stream(), side_stream()) if staged else (torch.cuda.default_stream(),) * 2
         if staged:
@@ -437,7 +438,7 @@ def _stream(s):
 
 def test_mix_dev_on_a_side_stream():
     from sonicsim_b200 import _lib
-    _, _, R = _R()
+    _, _, R = _lib_render()
     grow_ring(R.lib, R.ctx)
     rng = np.random.default_rng(31)
     cases = [(3, 2, 48001, 12.0), (2, 1, 65536, -3.0)]              # scalar path (odd E) and float4 path
@@ -451,7 +452,7 @@ def test_mix_dev_on_a_side_stream():
             torch.empty(S - 1, device="cuda")
         t_mix, t_out = torch.empty(E, device="cuda"), torch.empty((S, E), device="cuda")
         scr = torch.empty(scr_n, dtype=torch.float64, device="cuda")
-        writes += [(t_spk, to(spk), NAN), (t_noi, to(noi), NAN), (t_sir, to(sirs), NAN)]
+        writes += [(t_spk, to_device(spk), NAN), (t_noi, to_device(noi), NAN), (t_sir, to_device(sirs), NAN)]
         outs += [t_mix, t_out]
         bufs.append((spk, noi, sirs, snr, t_spk, t_noi, t_sir, scr))
         items.append(_lib.SsMixItem(speakers=t_spk.data_ptr(), noises=t_noi.data_ptr(), sirs=t_sir.data_ptr(),
@@ -469,16 +470,16 @@ def test_mix_dev_on_a_side_stream():
 
 
 def test_overlap_dev_on_a_side_stream():
-    _, _, R = _R()
+    _, _, R = _lib_render()
     rng = np.random.default_rng(32)
     rows, T, D = 3, 40001, 1777
     x = rng.standard_normal((rows, T)).astype(F32)
     tx, ty = torch.empty((rows, T), device="cuda"), torch.empty((rows, T), device="cuda")
-    unstaged([(tx, to(x), NAN)])
+    unstaged([(tx, to_device(x), NAN)])
     assert R.lib.ss_overlap_dev(R.ctx, ctypes.c_void_p(tx.data_ptr()), ctypes.c_void_p(ty.data_ptr()), rows, T, D,
                                 None) == 0                                  # warm-up
     s = side_stream()
-    stage(s, [ty], [(tx, to(x), NAN)])
+    stage(s, [ty], [(tx, to_device(x), NAN)])
     assert R.lib.ss_overlap_dev(R.ctx, ctypes.c_void_p(tx.data_ptr()), ctypes.c_void_p(ty.data_ptr()), rows, T, D,
                                 _stream(s)) == 0
     [y] = snapshot(s, [ty])
@@ -518,7 +519,7 @@ def _loud_check(stems_, snaps, what):
 
 def test_loudness_dev_on_a_side_stream():
     from sonicsim_b200 import _lib
-    _, _, R = _R()
+    _, _, R = _lib_render()
     grow_ring(R.lib, R.ctx)
     st = _loud_stems()
     outs, writes = _loud_stage(st)
@@ -532,7 +533,7 @@ def test_loudness_dev_on_a_side_stream():
 
 def test_dry_assemble_dev_on_a_side_stream():
     from sonicsim_b200 import _lib
-    _, _, R = _R()
+    _, _, R = _lib_render()
     grow_ring(R.lib, R.ctx)
     rng = np.random.default_rng(33)
     clips, cursor = [], 0
@@ -569,7 +570,7 @@ def test_render_on_one_stream_mixed_on_another_through_the_callers_event():
     """render_device on s (explicit stream argument) renders two speakers and a noise into one batch tensor; the caller
     records an event on s, a second stream s2 waits on it and ss_mix_dev mixes the stems there."""
     from sonicsim_b200 import _lib
-    _, render, R = _R()
+    _, render, R = _lib_render()
     grow_ring(R.lib, R.ctx)
     rng = np.random.default_rng(41)
     T = 9000
@@ -587,9 +588,9 @@ def test_render_on_one_stream_mixed_on_another_through_the_callers_event():
                           noise_delay=0)
     s, s2 = side_stream(), side_stream()
     sv = np.array([2.5], np.float32)
-    unstaged([(sirs, to(sv), NAN)])
+    unstaged([(sirs, to_device(sv), NAN)])
     _lib.check(R.lib.ss_mix_dev(R.ctx, ctypes.byref(item), 1, None))      # warm-up
-    stage(s, [spk, noi, mix, spk_out], [w for x in srcs for w in x.writes()] + [(sirs, to(sv), NAN)])
+    stage(s, [spk, noi, mix, spk_out], [w for x in srcs for w in x.writes()] + [(sirs, to_device(sv), NAN)])
     R.render_device([x.py() for x in srcs], [x.out for x in srcs], stream=s.cuda_stream)
     ev = torch.cuda.Event()
     ev.record(s)
@@ -613,7 +614,7 @@ def _host(x):
 def test_render_host_right_after_render_dev_on_a_side_stream():
     """A forked ss_render_dev on s, still queued behind the sleep, then at once render_host on the same context: its
     chunks take descriptor slots and scratch that the device render's chunks are still to read."""
-    _, render, R = _R()
+    _, render, R = _lib_render()
     R.set_chunk_bytes(SMALL)
     try:
         grow_ring(R.lib, R.ctx)
@@ -651,7 +652,7 @@ def test_render_host_ex_right_after_mix_and_loudness_on_a_side_stream():
     the oracle to 1e-6 dB and each direct stem takes its reverberant stem's gain; the device calls' results match
     theirs."""
     from sonicsim_b200 import _lib
-    _, render, R = _R()
+    _, render, R = _lib_render()
     rng = np.random.default_rng(61)
     srcs, targets, _ = _scene(np.random.default_rng(85), 12)
     direct = (1, 4, 8)
@@ -691,7 +692,7 @@ def test_render_host_ex_right_after_mix_and_loudness_on_a_side_stream():
         warm_outs, _, _ = host_ex(targets)                        # grows the host path's buffers before the staged run
         loud_outs, loud_writes = _loud_stage(st)
         dev_outs = [t_mix, t_out] + loud_outs
-        mix_writes = [(t_spk, to(spk), NAN), (t_noi, to(noi), NAN), (t_sir, to(sv), NAN)]
+        mix_writes = [(t_spk, to_device(spk), NAN), (t_noi, to_device(noi), NAN), (t_sir, to_device(sv), NAN)]
         unstaged(mix_writes)
         _lib.check(R.lib.ss_mix_dev(ctx, ctypes.byref(item), 1, None))                # warm-ups
         _lib.check(R.lib.ss_loudness_dev(ctx, larr, len(st), None))

@@ -23,6 +23,7 @@ import pytest
 import torch
 
 from oracle import sonicsim_oracle as so
+from gpu_plumbing import _R, _errors, to
 
 pytestmark = pytest.mark.gpu
 
@@ -31,15 +32,6 @@ LEN = 2 * RATE
 TRIES = 101
 TAPS = 40
 FORMS = ("spectra", "taps")
-
-
-def _R():
-    from sonicsim_b200 import render
-    return render, render.default_renderer()
-
-
-def to(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
 
 
 class Cand:
@@ -144,14 +136,6 @@ def _same(a, b, what):
         for i, (x, y) in enumerate(zip(a[k], b[k])):
             assert torch.equal(x, y), (what, k, i)
     assert torch.equal(a["starts"], b["starts"]) and torch.equal(a["used"], b["used"]), what
-
-
-def _errors(R):
-    try:
-        R.check_device_errors()
-    except (IndexError, ValueError) as e:
-        return type(e), str(e)
-    return None
 
 
 def test_pools_and_builds_equal(world):

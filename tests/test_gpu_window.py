@@ -4,9 +4,7 @@ bounds_host, and a device plan run twice with the dry signal changed in between,
 input outside the documented read set is NaN (or an out-of-range position), and every output lies inside a larger
 buffer with sentinels on both sides.  Also the Python API, windowed and unwindowed sources in one batch, BASELINE
 configs[1] speakers against the oracle, and the argument checks."""
-import contextlib
 import ctypes
-import os
 
 import numpy as np
 import pytest
@@ -14,51 +12,13 @@ import torch
 
 from conftest import TOL
 from oracle import sonicsim_oracle as so
-from window_cases import CASES, make_case, poison, read_set, windows
+from window_cases import CASES, _bad_bounds, _host_aligned, make_case, poison, read_set, windows
+from gpu_plumbing import _lib, small_host_budget_context
 
 pytestmark = pytest.mark.gpu
 
 SENT = np.float32(1234.5)
 PAD = 37
-
-
-def _lib():
-    from sonicsim_b200 import _lib as L, render
-    return L, render.default_renderer()
-
-
-@contextlib.contextmanager
-def small_host_budget_context():
-    """A context of its own whose host pipeline budget is 1 MB (SS_HOST_CHUNK_MB is read by ss_create)."""
-    L, R = _lib()
-    old = os.environ.get("SS_HOST_CHUNK_MB")
-    os.environ["SS_HOST_CHUNK_MB"] = "1"
-    ctx = ctypes.c_void_p()
-    try:
-        assert R.lib.ss_create(R.device, ctypes.byref(ctx)) == 0
-    finally:
-        if old is None:
-            del os.environ["SS_HOST_CHUNK_MB"]
-        else:
-            os.environ["SS_HOST_CHUNK_MB"] = old
-    try:
-        yield ctx
-    finally:
-        R.lib.ss_destroy(ctx)
-
-
-def _host_aligned(mode, P, C, L, N, bounds):
-    """The blocking the library picks with the trajectory on the host (ss_debug_plan)."""
-    L_, R = _lib()
-    if mode != 1:
-        return 0
-    b = np.ascontiguousarray(bounds, np.int32)
-    it = L_.SsSource(x=1, rir=1, out=1, bounds=b.ctypes.data, N=N, P=P, C=C, L=L, mode=1, bounds_host=b.ctypes.data)
-    cap = (N + 4095) // 4096 + P
-    out = np.zeros((cap, 4), np.int32)
-    al = ctypes.c_int32()
-    assert R.lib.ss_debug_plan(ctypes.byref(it), out.ctypes.data, cap, ctypes.byref(al)) > 0
-    return al.value
 
 
 class Batch:
@@ -349,7 +309,6 @@ def test_window_errors():
     assert R.lib.ss_render_host_ex(R.ctx, (L_.SsSource * 1)(it), 1, post) == L_.SS_ERR_INVALID
     assert np.all(sentinel == 7.0)
     # a windowed source whose bounds break the contract (ascending from 0 to N) is refused before anything is planned
-    from test_window import _bad_bounds
     Nb = 40960
     good, bad = _bad_bounds(Nb)
     Pb = len(good)

@@ -9,32 +9,17 @@ slot of a device pool whose dry samples k_stage stages from a host dry pool's ar
     starts at 0, at N - len and at segment and block edges;
   - the staged span holds every dry sample the render reads, stays inside the arena's padded signal, and fits the dry
     count of stage_cap over the pool - the slot's staging area."""
-import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
-from test_host_pool import Cand, _cap, _p
-from window_cases import B
+from emu import build_emu
+from window_cases import B, EmuCand, _p, stage_cap
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_dry_stage.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_dry_stage.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_stage_cap.argtypes = [vp] * 5 + [i32] * 3 + [vp]
-    lib.emu_bank_create.argtypes = [vp] + [i32] * 5 + [vp, vp]
-    lib.emu_dry_stage_slot.argtypes = [vp] * 4 + [i32] * 10 + [vp] + [i32] * 4 + [vp] * 5
-    return lib
+def emu():
+    return build_emu.load("ss_emu_dry_stage")
 
 
 def _dry_slot(emu, c, d, aligned, k_pool, ws, wl, render, n_dry=1, dv=0):
@@ -101,11 +86,11 @@ def test_dry_only_staged_slot_matches_the_device_dry_pick(emu, case):
     for i, L in enumerate(Ls):
         N = int(rng.integers(n_lo, n_hi))
         N += N % 4 == 0                                                 # N % 4 != 0
-        cands.append(Cand(emu, rng, N, P, C, L, taps, short=i % 2 == 1))
+        cands.append(EmuCand(emu, rng, N, P, C, L, taps, short=i % 2 == 1))
     assert all(c.N % 4 for c in cands)
     k_pool = max(c.K for c in cands)
     aligned = int(all(c.aligned_alone() for c in cands)) if P > 1 else 0
-    _, cap_x = _cap(emu, cands, wl)
+    _, cap_x = stage_cap(emu, cands, wl)
     rendered = 0
     for c in cands:
         starts = _starts(c, wl)
@@ -126,7 +111,7 @@ def test_dry_only_staged_slot_matches_the_device_dry_pick(emu, case):
 def test_out_of_range_dry_pick_is_clamped_as_k_blocks_clamps_it(emu):
     """A dry pick outside [0, n_dry) sets bit 16 in k_stage's head as in pick_pooled, and both take the same signal."""
     rng = np.random.default_rng(7)
-    c = Cand(emu, rng, 21001, 4, 2, 4096, 0)
+    c = EmuCand(emu, rng, 21001, 4, 2, 4096, 0)
     d = (rng.standard_normal(c.N + 3) * 0.1).astype(np.float32)
     for dv in (-1, 2, 1 << 30):
         info, outs = _dry_slot(emu, c, d, 0, 1, 5000, 3001, True, n_dry=2, dv=dv)

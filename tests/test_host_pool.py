@@ -9,62 +9,16 @@ copies for a pooled slot of a host pool (stage_set) and the staging area a plan 
   - a NumPy restatement of stage_set matches the kernels' at sampled starts, and over every start of training-shaped
     candidates (N = 480 000, P in {40, 60} with runs of short segments, K = 1..4, static and moving) stage_cap equals
     the largest read set exactly."""
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 
-from conftest import ROOT
-from oracle import sonicsim_oracle as so
-from test_pool import _choice, _random_bounds
-from window_cases import B
-
-KSPEC = 4096
+from emu import build_emu
+from window_cases import B, EmuCand, _k, _p, stage_cap, stage_set_np
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_stage.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_stage.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_stage_set.argtypes = [i32] * 4 + [vp] + [i32] * 2 + [vp]
-    lib.emu_stage_cap.argtypes = [vp] * 5 + [i32] * 3 + [vp]
-    lib.emu_stage_slot.argtypes = [vp] * 4 + [i32] * 10 + [vp] * 5
-    lib.emu_bank_create.argtypes = [vp] + [i32] * 5 + [vp, vp]
-    return lib
-
-
-def _p(a):
-    return None if a is None else ctypes.c_void_p(a.ctypes.data)
-
-
-def _k(L):
-    return (L + B - 1) // B
-
-
-class Cand:
-    """One candidate: dry x, trajectory (None: static), RIRs and their emulated bank (with a direct set when taps > 0)."""
-
-    def __init__(self, emu, rng, N, P, C, L, taps, short=False):
-        self.N, self.P, self.C, self.L, self.K = N, P, C, L, _k(L)
-        self.x = so.synth_dry(rng, N)
-        self.bounds = None if P == 1 else _random_bounds(rng, P, N, short)
-        h = so.synth_rirs(rng, P, C, L)
-        sets = 2 if taps else 1
-        self.spec = np.full((sets * P * C * self.K, KSPEC), np.nan, np.complex64)
-        self.cut = np.zeros(P * C, np.int32) if taps else None
-        emu.emu_bank_create(_p(h), P, C, L, 0, taps, _p(self.spec), _p(self.cut))
-        self.direct = 1 if taps else 0
-
-    def aligned_alone(self):
-        return 0 if self.P == 1 else _choice(self.bounds, self.N, self.P, self.L)
+def emu():
+    return build_emu.load("ss_emu_stage")
 
 
 def _slot(emu, c, aligned, k_pool, ws, wl, render):
@@ -73,20 +27,6 @@ def _slot(emu, c, aligned, k_pool, ws, wl, render):
     emu.emu_stage_slot(_p(c.x), _p(c.spec), _p(c.cut), _p(c.bounds), c.N, c.P, c.C, c.L, 0 if c.P == 1 else 1,
                        aligned, k_pool, ws, wl, c.direct, int(render), *[_p(o) for o in outs], _p(info))
     return info, outs
-
-
-def _cap(emu, cands, wl):
-    N = np.array([c.N for c in cands], np.int32)
-    P = np.array([c.P for c in cands], np.int32)
-    K = np.array([c.K for c in cands], np.int32)
-    out = np.zeros(2, np.int32)
-    if cands[0].P == 1:
-        emu.emu_stage_cap(None, None, _p(N), _p(P), _p(K), len(cands), cands[0].C, wl, _p(out))
-    else:
-        off = np.cumsum([0] + [c.P for c in cands[:-1]]).astype(np.int64)
-        flat = np.ascontiguousarray(np.concatenate([c.bounds for c in cands]), np.int32)
-        emu.emu_stage_cap(_p(flat), _p(off), _p(N), _p(P), _p(K), len(cands), cands[0].C, wl, _p(out))
-    return int(out[0]), int(out[1])
 
 
 def _check_tables(info, c, ws, wl):
@@ -135,11 +75,11 @@ def test_staged_set_holds_the_read_set_within_capacity(emu, case):
     reads, and the slot's staging area (stage_cap over the pool) holds the staged set; the capacity is reached."""
     P, C, Ls, taps, (n_lo, n_hi), wl, every = CASES[case]
     rng = np.random.default_rng(100 + case)
-    cands = [Cand(emu, rng, int(rng.integers(n_lo, n_hi)), P, C, L, taps, short=i % 2 == 1)
+    cands = [EmuCand(emu, rng, int(rng.integers(n_lo, n_hi)), P, C, L, taps, short=i % 2 == 1)
              for i, L in enumerate(Ls * 2)]
     k_pool = max(c.K for c in cands)
     aligned = int(all(c.aligned_alone() for c in cands)) if P > 1 else 0
-    cap_rows, cap_x = _cap(emu, cands, wl)
+    cap_rows, cap_x = stage_cap(emu, cands, wl)
     most_rows, most_x = 0, 0
     for c in cands:
         for ws in _starts(c, wl, every):
@@ -158,25 +98,6 @@ def test_both_blockings_and_every_k_are_covered():
         for L in Ls:
             seen.add(("static" if P == 1 else "moving", _k(L)))
     assert {k for _, k in seen} == {1, 2, 3, 4} and {"static", "moving"} <= {m for m, _ in seen}
-
-
-def stage_set_np(N, P, C, K, bounds, ws, wl):
-    """stage_set (ss_phases.cuh) in NumPy over an array of starts ws: (xa, xb, row0, rows) as int64 arrays.  The dry span
-    [ws - (K + 2) 4096, ws + wl + 2 * 4096) clamped to [0, N); the rows of every position whose segment holds a sample of
-    it and the one after, widened to row pairs and clipped to the bank (window_rows)."""
-    ws = np.asarray(ws, np.int64)
-    xa = np.maximum(ws - (K + 2) * B, 0)
-    xb = np.minimum(ws + wl + 2 * B, N)
-    if P > 1:
-        inner = np.asarray(bounds, np.int64)[1:P]             # seg_of: bounds[1..P-1] <= n, clamped to P - 2
-        pa = np.minimum(np.searchsorted(inner, xa, side="right"), P - 2)
-        pb = np.minimum(np.searchsorted(inner, xb - 1, side="right"), P - 2) + 1
-    else:
-        pa, pb = np.zeros_like(ws), np.zeros_like(ws)
-    ck = C * K
-    r0 = (pa * ck) & ~1
-    r1 = np.minimum(((pb + 1) * ck + 1) & ~1, P * ck)
-    return xa, xb, r0, r1 - r0
 
 
 def _emu_stage_set(emu, c, ws, wl):
@@ -255,7 +176,7 @@ def test_stage_cap_is_the_maximum_over_every_start(emu, wl):
     for c in shapes:
         xa, xb, _, rows = stage_set_np(c.N, c.P, c.C, c.K, c.bounds, ws, wl)
         m = (int(rows.max()), int((xb - xa).max()) + 8)
-        assert _cap(lib, [c], wl) == m, (c.P, c.C, c.K, wl, _cap(lib, [c], wl), m)
+        assert stage_cap(lib, [c], wl) == m, (c.P, c.C, c.K, wl, stage_cap(lib, [c], wl), m)
         most.append(m)
     for static in (True, False):
         for C in {c.C for c in shapes}:
@@ -263,7 +184,7 @@ def test_stage_cap_is_the_maximum_over_every_start(emu, wl):
             if not group:
                 continue
             want = (max(most[i][0] for i in group), max(most[i][1] for i in group))
-            assert _cap(lib, [shapes[i] for i in group], wl) == want, (static, C, wl)
+            assert stage_cap(lib, [shapes[i] for i in group], wl) == want, (static, C, wl)
 
 
 @pytest.mark.parametrize("case", range(len(CASES)))
@@ -272,7 +193,7 @@ def test_staged_slot_renders_the_same_bits(emu, case):
     the same bits for the reverberant and the direct stem, at the first, last and edge starts and a few others."""
     P, C, Ls, taps, (n_lo, n_hi), wl, _ = CASES[case]
     rng = np.random.default_rng(200 + case)
-    cands = [Cand(emu, rng, int(rng.integers(n_lo, n_hi)), P, C, L, taps, short=i % 2 == 1) for i, L in enumerate(Ls)]
+    cands = [EmuCand(emu, rng, int(rng.integers(n_lo, n_hi)), P, C, L, taps, short=i % 2 == 1) for i, L in enumerate(Ls)]
     k_pool = max(c.K for c in cands)
     aligned = int(all(c.aligned_alone() for c in cands)) if P > 1 else 0
     for c in cands:

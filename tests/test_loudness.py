@@ -4,16 +4,8 @@ import numpy as np
 import pytest
 
 from oracle import sonicsim_oracle as so
-
-
-def stems(seed, N, C, sr=16000):
-    rng = np.random.default_rng(seed)
-    t = np.arange(N) / sr
-    env = 0.5 + 0.5 * np.sin(2 * np.pi * 0.7 * t + rng.random() * 6)          # loud / quiet passages exercise the gates
-    x = rng.standard_normal((N, C)) * env[:, None] * 0.05
-    x[: N // 7] *= 1e-4                                                        # a near-silent lead-in (absolute gate)
-    x += 0.02 * np.sin(2 * np.pi * 30 * t)[:, None]                            # sub-38 Hz content (high-pass matters)
-    return x.astype(np.float32)
+from loudness_cases import (EXACT_DB, PARTITION_CASES, RATES, REFINES, assert_clear_of_gates, block_size_of,
+                            n_samples_for, stems)
 
 
 def test_oracle_kweighting_reference_values():
@@ -59,44 +51,6 @@ def test_gating_plan_matches_pyloudnorm_expressions():
         brk, blo, bhi = gating_plan(N, float(sr), float(bs))
         assert np.array_equal(brk[blo], np.minimum(lo, N)) and np.array_equal(brk[bhi], np.minimum(hi, N))
         assert np.all(np.diff(brk) > 0)
-
-
-def subsonic(seed, N, C, sr=16000):
-    """Noise over a strong 20 Hz tone: the 38 Hz high-pass carries a large state from one interval into the next."""
-    rng = np.random.default_rng(seed)
-    t = np.arange(N) / sr
-    return (0.6 * np.sin(2 * np.pi * 20 * t)[:, None] + 0.05 * rng.standard_normal((N, C))).astype(np.float32)
-
-
-RATES = [8000, 16000, 22050, 44100, 48000]
-EXACT_DB = 1e-6           # kernels vs the float64 restatement: they differ only by float64 rounding of the filter state
-
-
-def block_size_of(N, sr):
-    return 0.4 if N / sr >= 0.4 else N / sr                                   # SonicSim_audio.py:69
-
-
-def assert_clear_of_gates(x, sr, block, margin=1e-3):
-    """No gating block of `x` is within `margin` dB of the absolute (-70) or the relative gate, so rounding cannot
-    move a block across a gate and the comparison with the reference cannot turn on a near-tie."""
-    l, gamma_r = so.bs1770_block_loudness(x, sr, block, up_to_8_channels=True)
-    fin = l[np.isfinite(l)]
-    assert np.all(np.abs(fin + 70.0) > margin), np.min(np.abs(fin + 70.0))
-    if np.isfinite(gamma_r):
-        assert np.all(np.abs(fin - gamma_r) > margin), np.min(np.abs(fin - gamma_r))
-    return l, gamma_r
-
-
-def n_samples_for(n_e, sr):
-    """A clip length whose gating plan has exactly `n_e` elementary intervals (shortest such N from 0.05 s on)."""
-    from sonicsim_b200.SonicSim_audio import gating_plan
-    N = int(0.05 * sr)
-    while True:
-        brk = gating_plan(N, float(sr), float(block_size_of(N, sr)), 1)[0]
-        if len(brk) - 1 == n_e:
-            return N
-        assert len(brk) - 1 < n_e, "no clip length at %g Hz has %d intervals" % (sr, n_e)
-        N += max(1, int(0.01 * sr)) if len(brk) - 1 < n_e - 1 else 1
 
 
 def _emu_vs_reference(emu, x, sr):
@@ -159,11 +113,6 @@ def test_emulated_kernels_last_block_clipped_at_n(emu, sr):
     lo, hi = so.bs1770_block_bounds(N, sr, 0.4)
     assert hi[-1] > N and lo[-1] < N
     _emu_vs_reference(emu, stems(7, N, 3, sr), sr)
-
-
-PARTITION_CASES = [(16000, 100001, 2, stems), (48000, int(1.06 * 48000), 7, stems), (22050, 5000, 1, stems),
-                   (8000, int(0.41 * 8000), 2, subsonic), (48000, int(1.3 * 48000), 3, subsonic)]
-REFINES = (1, 2, 5, 32)
 
 
 def test_emulated_kernels_do_not_depend_on_the_partition(emu, monkeypatch):

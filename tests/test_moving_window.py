@@ -3,47 +3,22 @@ start (window_table_cap of ss_phases.cuh, exported by tests/emu/ss_emu_moving.cu
 for each start, swept over every start); k_blocks' clamp of a start read from device memory; and the refusals of the
 pure-host hook and of the Python layer."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
-from window_cases import B, CASES, full_blocks, make_case
+from emu import build_emu
+from window_cases import B, CASES, _needs_numpy, make_case
 from sonicsim_b200 import _lib
 
 
 @pytest.fixture(scope="module")
-def emu_moving(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_moving.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_moving.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_window_table_cap.argtypes = [vp] + [i32] * 6
-    lib.emu_window_tables.argtypes = [vp] + [i32] * 5 + [vp]
-    lib.emu_clamp_win_start.argtypes = [i32, i32, i32, ctypes.POINTER(ctypes.c_int32)]
-    return lib
+def emu_moving():
+    return build_emu.load("ss_emu_moving")
 
 
 def _lengths(N):
     return sorted({n for n in (1, 100, B - 1, B, B + 1, 3 * B + 5, 10000, N // 2, N - 1, N) if 1 <= n <= N})
-
-
-def _needs_numpy(N, bounds, aligned, K, wl):
-    """g1 - g0 of the table every start in [0, N - wl] needs, from the full plan (window_cases.full_blocks)."""
-    blk = np.array(full_blocks(N, bounds, aligned), np.int64)
-    starts, ends = blk[:, 0], blk[:, 0] + blk[:, 1]
-    ws = np.arange(N - wl + 1)
-    k0 = np.searchsorted(ends, ws, side="right")
-    k1 = np.searchsorted(starts, ws + wl, side="left")
-    g0 = np.maximum(k0 - (K - 1), 0) & ~1
-    g1 = np.minimum(len(blk), (k1 + 1) & ~1)
-    return g1 - g0
 
 
 @pytest.mark.parametrize("name", list(CASES))

@@ -3,28 +3,17 @@
 pool's gain, and a slot without a table keeps the pool's gain; the exports; and the Python refusals that need no
 device."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from emu import build_emu
 from sonicsim_b200 import _lib
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_pair.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_pair.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_pair_heads.argtypes = [vp, vp, i32, i32, i32, vp, i32, i32, i32, vp]
-    return lib
+def emu():
+    return build_emu.load("ss_emu_pair")
 
 
 def heads(emu, N, g, tab, n_dry, v, dv):

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
+from emu import build_emu
 import draw_reference as dr
 from sonicsim_b200 import _lib
 
@@ -18,18 +19,8 @@ GOLDEN = os.path.join(ROOT, "tests", "golden", "crop_draw.npz")
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_draw.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_draw.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_draw.argtypes = [vp, vp, i32, vp, i32, i32, vp, i32, ctypes.c_float, ctypes.POINTER(ctypes.c_int32)]
-    lib.emu_draw_start.argtypes = [ctypes.c_double, i32]
-    return lib
+def emu():
+    return build_emu.load("ss_emu_draw")
 
 
 def emu_draw(emu, tables, D, reader_N, length, u, thr=-40.0):

@@ -12,41 +12,14 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
-from test_moving_window import _needs_numpy
-from window_cases import B
+from emu import build_emu
+from window_cases import B, _choice, _needs_numpy, _random_bounds
 from sonicsim_b200 import _lib
 
 
 @pytest.fixture(scope="module")
-def emu_pool(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_pool.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_pool.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_pool_table_cap.argtypes = [vp, vp, vp, vp] + [i32] * 4
-    lib.emu_clamp_pick.argtypes = [i32, i32, ctypes.POINTER(ctypes.c_int32)]
-    lib.emu_pick_candidate.argtypes = [i32] * 5 + [vp]
-    return lib
-
-
-def _random_bounds(rng, P, N, short):
-    cuts = np.sort(rng.integers(0, (min(N, 3000) if short else N) + 1, P - 2))
-    return np.ascontiguousarray(np.concatenate([[0], cuts, [N]]), np.int32)
-
-
-def _choice(bounds, N, P, L):
-    """The blocking the library picks for one candidate on its own (ss_debug_plan), 1 = aligned."""
-    lib = _lib.load()
-    item = _lib.SsSource(x=1, out=1, bounds=bounds.ctypes.data, bounds_host=bounds.ctypes.data, N=N, P=P, C=1, L=L,
-                         mode=_lib.SS_MOVING_BOUNDS, rir=1)
-    blk = np.zeros((N // B + P + 8, 4), np.int32)
-    aligned = ctypes.c_int32()
-    assert lib.ss_debug_plan(ctypes.byref(item), blk.ctypes.data, blk.shape[0], ctypes.byref(aligned)) > 0
-    return aligned.value
+def emu_pool():
+    return build_emu.load("ss_emu_pool")
 
 
 def _cap(emu_pool, cands, aligned, L, wl, static=False):

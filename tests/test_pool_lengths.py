@@ -8,43 +8,18 @@ tests/emu/ss_emu_pool_lengths.cu):
     RIRs zero-padded to the pool's longest L: that bank's forward transforms pair each partition-0 row with a padded
     partition, whose half spectrum then holds the rounding residue of its partner rather than zeros (DESIGN section 3)."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from emu import build_emu
 from oracle import sonicsim_oracle as so
-from test_moving_window import _needs_numpy
-from test_pool import _choice, _random_bounds
-from window_cases import B
-
-KSPEC = 4096
+from window_cases import B, KSPEC, _choice, _k, _needs_numpy, _p, _random_bounds
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_pool_lengths.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_pool_lengths.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_pick_parts.argtypes = [i32, i32, vp, vp, vp] + [i32] * 5 + [vp]
-    lib.emu_pool_table_cap_parts.argtypes = [vp] * 5 + [i32] * 3
-    lib.emu_render_slot.argtypes = [vp] * 4 + [i32] * 8
-    return lib
-
-
-def _p(a):
-    return None if a is None else ctypes.c_void_p(a.ctypes.data)
-
-
-def _k(L):
-    return (L + B - 1) // B
+def emu():
+    return build_emu.load("ss_emu_pool_lengths")
 
 
 def test_pick_sets_the_picked_candidates_partitions(emu):

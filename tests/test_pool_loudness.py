@@ -5,47 +5,27 @@ blocks under aligned and grid blocking, blocks that straddle waypoints (the red_
 RIRs, windows and direct stems; with gain 1 every output keeps its bits; the head of k_blocks carries the picked
 candidate's gain into the slot; the export and version; and the refusals Python makes before any C call."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from emu import build_emu
 from sonicsim_b200 import _lib
 
 B = 4096
 
 
-def _build(tmp_path_factory, name):
-    src = os.path.join(ROOT, "tests", "emu", name + ".cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / ("lib%s.so" % name))
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_render_window.argtypes = [vp] * 6 + [i32] * 8 + [vp] + [i32] * 3 + [vp]
-    return lib
+@pytest.fixture(scope="module")
+def emu():
+    return build_emu.load("ss_emu_gain")
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    lib = _build(tmp_path_factory, "ss_emu_gain")
-    lib.emu_set_gain.argtypes = [ctypes.c_float]
-    lib.emu_set_gain.restype = None
-    lib.emu_pick_slot.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p,
-                                  ctypes.POINTER(ctypes.c_float)]
-    return lib
+def emu_plain():
+    return build_emu.load("ss_emu_window")
 
 
-@pytest.fixture(scope="module")
-def emu_plain(tmp_path_factory):
-    return _build(tmp_path_factory, "ss_emu_window")
-
-
-def _p(a):
+def _addr(a):
     return a.ctypes.data if a is not None else None
 
 
@@ -87,8 +67,8 @@ def _render(lib, case):
     T = wl if wl else N
     out = np.full((C, T), np.nan, np.float32)
     dout = np.full((C, T), np.nan, np.float32) if taps else None
-    lib.emu_render_window(_p(x), _p(rir), _p(out), _p(bounds), _p(idx), _p(w), N, P, C, L, mode, aligned, ws, wl,
-                          _p(dout), taps, 0, 1, None)
+    lib.emu_render_window(_addr(x), _addr(rir), _addr(out), _addr(bounds), _addr(idx), _addr(w), N, P, C, L, mode,
+                          aligned, ws, wl, _addr(dout), taps, 0, 1, None)
     return out, dout
 
 

@@ -9,46 +9,18 @@
     16 KB of taps against sets * rows * 32 KB of spectra); the block behind the areas (tap_block: StageTaps, transform
     Sources, CTA prefix, zero word) holds each part without overlap."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+from emu import build_emu
 from oracle import sonicsim_oracle as so
-from test_pool import _random_bounds
-from window_cases import B
-
-KSPEC = 4096
+from window_cases import B, KSPEC, _k, _p, _random_bounds
 
 
 @pytest.fixture(scope="module")
-def emu(tmp_path_factory):
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_taps.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_taps.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
-    vp, i32 = ctypes.c_void_p, ctypes.c_int
-    lib.emu_tap_bank.argtypes = [vp] + [i32] * 5 + [vp, vp]
-    lib.emu_tap_transform.argtypes = [vp, vp] + [i32] * 7 + [vp, vp]
-    lib.emu_bank_create.argtypes = [vp] + [i32] * 5 + [vp, vp]
-    lib.emu_stage_set.argtypes = [i32] * 4 + [vp] + [i32] * 2 + [vp]
-    lib.emu_stage_cap.argtypes = [vp] * 5 + [i32] * 3 + [vp]
-    lib.emu_stage_area.argtypes = [i32] * 4 + [vp]
-    lib.emu_tap_block.argtypes = [ctypes.c_int64, i32, i32, vp, vp]
-    return lib
-
-
-def _p(a):
-    return None if a is None else ctypes.c_void_p(a.ctypes.data)
-
-
-def _k(L):
-    return (L + B - 1) // B
+def emu():
+    return build_emu.load("ss_emu_taps")
 
 
 def _tap_bank(emu, h, normalize, taps):

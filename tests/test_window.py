@@ -3,27 +3,19 @@ and epilogue code as the CUDA kernels) render a window equal, bit for bit, to th
 render; the window reads nothing outside its documented read set; ss_debug_plan's windowed table is the stated subset of
 the full plan; and the argument checks of the pure-host hooks and of the Python layer."""
 import ctypes
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
-from window_cases import CASES, full_blocks, make_case, poison, read_set, windows
+from emu import build_emu
+from window_cases import CASES, _bad_bounds, full_blocks, make_case, poison, read_set, windows
 from sonicsim_b200 import _lib
 
 
 @pytest.fixture(scope="module")
-def render_window(tmp_path_factory):
+def render_window():
     """emu_render_window of tests/emu/ss_emu_window.cu, built with g++ like the other emulation libraries."""
-    src = os.path.join(ROOT, "tests", "emu", "ss_emu_window.cu")
-    so_path = str(tmp_path_factory.mktemp("emu") / "libss_emu_window.so")
-    cmd = ["g++", "-O2", "-shared", "-fPIC", "-x", "c++", "-I" + os.environ.get("CUDA_INC", "/usr/local/cuda/include"),
-           "-o", so_path, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, "g++ failed: %s\n%s" % (" ".join(cmd), res.stderr)
-    lib = ctypes.CDLL(so_path)
+    lib = build_emu.load("ss_emu_window")
     fp, ip = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int32)
 
     def ptr(a, t=fp):
@@ -185,17 +177,6 @@ def test_window_argument_checks():
             render._window(src._replace(window=win), 0, 100)
     assert render._window(src._replace(window=(99, 1)), 0, 100) == (99, 1, 1)
     assert render._window(src, 0, 100) == (0, 0, 100)
-
-
-def _bad_bounds(N=40960):
-    """Bounds tables outside the contract (ascending from 0 to N): a huge interior waypoint that would make the aligned
-    planner emit ~10^5 blocks, a descending step, a last entry != N, a first entry != 0."""
-    good = np.array([0] + [2048 + 4096 * k for k in range(9)] + [38000, N], np.int64)
-    huge = good.copy(); huge[-2] = 400000000
-    desc = good.copy(); desc[3], desc[4] = desc[4], desc[3]
-    short = good.copy(); short[-1] = N - 5
-    late = good.copy(); late[0] = 100
-    return good, [huge, desc, short, late]
 
 
 def test_debug_plan_refuses_bounds_outside_the_contract():
