@@ -1,21 +1,25 @@
 """Candidates, pools, slots and training plans that the GPU pool and dry-pool tests build their worlds from.  Test
 infrastructure."""
 import ctypes
+import threading
 
 import numpy as np
 import pytest
 import torch
 
 import draw_reference as dr
-from direct_path import direct_path_rirs
+from direct_path import direct_path_rirs, normalized
 from draw_reference import LEN, NEAR_DB, RATE, gappy_dry
-from gpu_plumbing import _R, _rms, to
+from gpu_plumbing import _R, _device_errors, _rms, pmap, to
+from mix_reference import Out, check_mixture, fold
 from oracle import sonicsim_oracle as so
 from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, delay_rirs, graded_dry, render_check_inputs
-from window_cases import _choice
+from window_cases import _choice, stage_set_np
 
 B = 4096
 NAN = float("nan")
+TRIES = 101                    # tries of the training plans' CropDraws
+PINNED_MAX = 2 << 30           # pinned host bytes a scale test may hold in banks and pools
 
 
 def fold_dev(t):
@@ -401,7 +405,8 @@ class ScaleCand:
         if quiet:
             gl = _rms(np.asarray(y, np.float64) - y64) / _rms(scale)
             assert gl <= TAU_GLOBAL, "%s: quiet crop, global RMS %.3g of the scale's > %.3g" % (label, gl, TAU_GLOBAL)
-            QUIET.setdefault(key, []).append(label)
+            with _STATS_LOCK:
+                QUIET.setdefault(key, []).append(label)
         _note(key, worst, gl if wl >= B else 0.0)
 
 
@@ -520,9 +525,13 @@ STATS = {}                       # section / variant -> [worst local ratio, wors
 QUIET = {}                       # section / variant -> labels of crops whose global error is taken against the scale
 
 
+_STATS_LOCK = threading.Lock()
+
+
 def _note(key, worst, g):
-    s = STATS.setdefault(key, [0.0, 0.0])
-    s[0], s[1] = max(s[0], worst), max(s[1], g)
+    with _STATS_LOCK:                                    # (checks run on a thread pool)
+        s = STATS.setdefault(key, [0.0, 0.0])
+        s[0], s[1] = max(s[0], worst), max(s[1], g)
 
 
 class NCand:
@@ -538,3 +547,552 @@ def normalised(R, render, c, target, taps=0):
     d = [np.empty((c.C, c.N), np.float32)] if taps else None
     out = R.render_host([host_src(render, c, taps)], lufs_targets=[target], loudness_out=lo, sr=RATE, direct_outs=d)[0]
     return torch.from_numpy(out).cuda(), (torch.from_numpy(d[0]).cuda() if taps else None), lo[0]
+
+
+# ------------------------------------------------------------------- host and tap-form pools at training scale
+def report(title):
+    """The worst float64 ratios of every section / variant key that starts with the title's section."""
+    print("\n%s:" % title)
+    for k in sorted(STATS):
+        if k.startswith(title.split(":")[0]):
+            print("  %-40s worst per-sample ratio %.3g, worst global relative RMS %.3g; %d quiet crops%s" % (
+                k, *STATS[k], len(QUIET.get(k, [])), (" (first: %s)" % QUIET[k][0]) if k in QUIET else ""))
+
+
+def pool_variant(cands):
+    """The render kernel every slot of a pool of these candidates runs: static pools k_render_fast, pools of K > 1
+    k_render<1,0>, moving pools whose every candidate picks aligned blocking on its own k_render_fast, and every other
+    moving pool (mixed blocking renders on the grid) k_render<0,0>."""
+    if cands[0].P == 1:
+        return "k_render_fast static"
+    if max(c.K for c in cands) > 1:
+        return "k_render<1,0>"
+    return "k_render_fast" if all(_choice(c.b, c.N, c.P, c.L) for c in cands) else "k_render<0,0>"
+
+
+def normalised_cand(c):
+    """The candidate with its RIR set divided by its abs-max in float32 (SS_RIR_NORMALIZE): the float64 reference of a
+    slot of a normalised bank."""
+    return ScaleCand(c.x, normalized(c.h), c.b)
+
+
+class Pools:
+    """One set of candidates as a device pool (key False) and as host pools of the bank forms in `form`: spectral banks
+    (key True) and tap-form banks (key "taps"); banks shared between candidates when `share` names the RIR set of each,
+    with direct sets of TAPS taps when `taps`, normalised when `normalize`, level tables and loudness targets.  `arms`
+    lists the keys, the device pool's first; `refs` the candidates the float64 reference renders (normalised RIRs when
+    `normalize`).  Counts the pinned bytes it holds."""
+
+    def __init__(self, cands, taps=False, levels=None, lufs=None, share=None, host_only=False, form=("spectra",),
+                 normalize=False):
+        render, R = _R()
+        self.cands, self.taps = cands, taps
+        self.refs = [normalised_cand(c) for c in cands] if normalize else cands
+        self.pools, self.banks = {}, []
+        sets = share if share is not None else list(range(len(cands)))
+        forms = (form,) if isinstance(form, str) else tuple(form)
+        arms = ([] if host_only else [(False, False, "spectra")]) + [(f == "spectra" or f, True, f) for f in forms]
+        for key, host, f in arms:
+            banks = {}
+            for c, r in zip(cands, sets):
+                if r not in banks:
+                    banks[r] = R.rir_bank(c.h if c.P > 1 else c.h[0], normalize, TAPS if taps else 0, host=host,
+                                          form=f)
+            self.banks += list(banks.values())
+            srcs = []
+            for c, r in zip(cands, sets):
+                if c.P == 1:
+                    srcs.append(render.StaticSource(c.x if host else to(c.x), banks[r]))
+                elif host:
+                    srcs.append(render.MovingSource(c.x, banks[r], c.b))
+                else:
+                    srcs.append(render.MovingSource(to(c.x), banks[r], to(c.b), bounds_host=c.b))
+            self.pools[key] = R.source_pool(srcs, levels=levels, lufs_targets=lufs, sr=RATE)
+        self.variant = pool_variant(cands)
+        self.arms = list(self.pools)
+        hosts = [k for k in self.arms if k is not False]
+        self.pinned = sum(k.host_nbytes for k in self.banks) + sum(self.pools[k].host_nbytes for k in hosts)
+        self.host = self.pools[hosts[-1]]                        # the arm the float64 checks read
+        self.gains = self.host.loudness[:, 1]
+
+    def gain(self, i):
+        g = self.gains[i]
+        return 1.0 if np.isnan(g) else float(g)
+
+    def close(self):
+        for p in self.pools.values():
+            p.close()
+        for k in self.banks:
+            k.close()
+
+
+def _hold(*pools):
+    """The pinned host bytes the test's banks and pools hold, as the library counts them (host_nbytes; the renderer's own
+    host staging buffers not included), printed and kept under 2 GB."""
+    total = sum(p.pinned for p in pools)
+    print("\npinned host memory of the banks and pools held (host_nbytes): %.1f MB" % (total / 1e6))
+    assert total <= PINNED_MAX, total
+    return total
+
+
+def a_grid(rng):
+    """Moving candidates with 59 segments of 0.3 to 3.8 k samples (grid blocking), pure-delay RIRs, graded dry
+    signals."""
+    out = []
+    for j, N in enumerate((70001, 83002)):
+        P = 60
+        np.random.seed(500 + j)
+        b = _bounds_of(so.setup_dynamic_interp(so.synth_path(rng, P), N)[0], P)
+        assert _choice(b, N, P, 4096) == 0
+        out.append(ScaleCand(graded_dry(rng, N), delay_rirs(rng, P, 3, 4096)[0], b))
+    return out
+
+
+def probe_starts(c, wl, rng):
+    """0 and N - len; the maximisers of stage_cap, (K + 2) 4096 and b[s + 1] - 1 + (K + 2) 4096; starts where xa clamps
+    to 0 and where xb clamps to N; starts with ws % 4 in {1, 2, 3}; all inside [0, N - len]."""
+    last = c.N - wl
+    d0 = (c.K + 2) * B
+    s = {0, last, d0, d0 - 1, 1, last - 1, max(0, c.N - wl - 2 * B + 1)}
+    for q in ([] if c.b is None else c.b[1:-1]):
+        s.add(int(q) - 1 + d0)
+    for m in (1, 2, 3):
+        v = int(rng.integers(0, last + 1))
+        s.add(v - v % 4 + m)
+    return sorted(v for v in s if 0 <= v <= last)
+
+
+def read_set(c, ws, wl, sets):
+    """(bytes k_stage copies - whole float4s of dry samples and the rows of every set -, rows, dry samples)."""
+    xa, xb, _, rows = (int(v[0]) for v in stage_set_np(c.N, c.P, c.C, c.K, c.b, [ws], wl))
+    return 4 * (((xb + 3) & ~3) - (xa & ~3)) + sets * rows * B * 8, rows, xb - xa
+
+
+class Probes:
+    """A plan over every pool (arm) of `pl`: for every window length, `k` slots with device starts and one with a fixed
+    start, all over the same pick and start tensors, NaN-filled guarded outputs."""
+
+    def __init__(self, pl, lens, k, fixed):
+        render, R = _R()
+        self.pl, self.lens, self.k = pl, lens, k
+        n = len(lens) * (k + 1)
+        self.picks = torch.zeros(n, dtype=torch.int32, device="cuda")
+        self.starts = torch.zeros(n, dtype=torch.int32, device="cuda")
+        self.slots = []                               # (wl, fixed start or None)
+        for wl, f in zip(lens, fixed):
+            self.slots += [(wl, None)] * k + [(wl, f)]
+        C = pl.cands[0].C
+        self.plans, self.outs, self.douts = {}, {}, {}
+        for arm, pool in pl.pools.items():
+            srcs = [render.Pooled(pool, self.picks[j], (self.starts[j] if f is None else f, wl), TAPS if pl.taps else 0)
+                    for j, (wl, f) in enumerate(self.slots)]
+            self.outs[arm] = [Out(C, wl) for wl, _ in self.slots]
+            self.douts[arm] = [Out(C, wl) for wl, _ in self.slots] if pl.taps else []
+            self.plans[arm] = R.plan_device(srcs, [o.view() for o in self.outs[arm]],
+                                            direct_outs=[o.view() for o in self.douts[arm]] if pl.taps else None)
+
+    def run(self, pk, st):
+        self.pk, self.st = list(pk), [s if f is None else f for s, (_, f) in zip(st, self.slots)]
+        self.picks.copy_(torch.tensor(self.pk, dtype=torch.int32))
+        self.starts.copy_(torch.tensor(st, dtype=torch.int32))
+        R = _R()[1]
+        self.launches, self.errors = {}, {}
+        for arm in self.plans:
+            for o in self.outs[arm] + self.douts[arm]:
+                o.reset()
+            R.reset_stats()
+            self.plans[arm].run()
+            self.launches[arm] = R.launch_count()
+            self.errors[arm] = _device_errors(R)
+        torch.cuda.synchronize()
+        first = self.pl.arms[0]
+        for arm in self.pl.arms[1:]:                      # (i) bit for bit the first arm's plan
+            assert self.errors[arm] == self.errors[first], (arm, self.errors)
+            for j in range(len(self.slots)):
+                a, b = self.outs[first][j].get(), self.outs[arm][j].get()
+                assert np.array_equal(a, b), ("twin", arm, j, self.pk[j], self.st[j])
+                if self.pl.taps:
+                    assert np.array_equal(self.douts[first][j].get(), self.douts[arm][j].get()), ("direct twin", arm, j)
+
+    def check(self, key, label):
+        last, jobs = self.pl.arms[-1], []
+        for j, (wl, _) in enumerate(self.slots):          # (ii) float64, on a thread pool
+            c = self.pl.refs[self.pk[j]]
+            g = self.pl.gain(self.pk[j])
+            what = "%s slot %d cand %d start %d len %d" % (label, j, self.pk[j], self.st[j], wl)
+            jobs.append((c, self.outs[last][j].get(), self.st[j], wl, False, g, what))
+            if self.pl.taps:
+                jobs.append((c, self.douts[last][j].get(), self.st[j], wl, True, g, what + " direct"))
+        pmap(lambda t: t[0].check(t[1], t[2], t[3], direct=t[4], gain=t[5], key=key, label=t[6]), jobs)
+
+    def close(self):
+        for p in self.plans.values():
+            p.close()
+
+
+def b_configs1(rng):
+    """bench.make_inputs(16, 0): 32 configs[1] speakers (P = 40, C = 6, 30 s; every other dry signal gappy) and 16
+    static 6-channel noises."""
+    import bench
+    items = bench.make_inputs(16, 0)
+    spk = [ScaleCand(gappy_dry(rng, len(x)) if j % 2 else x, h, b) for j, (x, h, b) in enumerate(items)]
+    N, C = bench.CFG["N"], bench.CFG["C"]
+    noi = [ScaleCand((rng.standard_normal(N) * 0.05).astype(np.float32),
+                (rng.standard_normal((1, C, 4096)) * np.exp(-np.arange(4096) / 800.0)).astype(np.float32), None)
+           for _ in range(16)]
+    return spk, noi
+
+
+class Training:
+    """16 scenes: `layout` a list of (pools key, taps) per scene, the first two the mixture's speakers and the draw's,
+    the rest its noises; one start per scene drawn by a 101-try CropDraw over mono level tables; one mono Mixture.  One
+    plan per arm of the pools (Pools.arms, the same in every pool)."""
+
+    def __init__(self, pools, layout, U=16):
+        render, R = _R()
+        self.pools, self.layout, self.U = pools, layout, U
+        S = len(layout)
+        self.picks = torch.zeros((U, S), dtype=torch.int32, device="cuda")
+        self.starts = torch.zeros(U, dtype=torch.int32, device="cuda")
+        self.u = torch.zeros((U, TRIES), dtype=torch.float64, device="cuda")
+        self.used = torch.zeros(U, dtype=torch.int32, device="cuda")
+        self.sirs = torch.zeros((U, 1), device="cuda")
+        self.snr = torch.zeros(U, device="cuda")
+        self.T = 4 * RATE
+        self.plans, self.o = {}, {}
+        self.arms = next(iter(pools.values())).arms
+        for arm in self.arms:
+            srcs, outs, douts, mixes, draws = [], [], [], [], []
+            o = dict(outs=[], douts=[], mix=[], spk=[], rms=[])
+            for u in range(U):
+                base = len(srcs)
+                for k, (key, taps) in enumerate(layout):
+                    pl = pools[key]
+                    srcs.append(render.Pooled(pl.pools[arm], self.picks[u, k], (self.starts[u], self.T),
+                                              TAPS if taps else 0))
+                    o["outs"].append(Out(pl.cands[0].C, self.T))
+                    o["douts"].append(Out(pl.cands[0].C, self.T) if taps else None)
+                o["mix"].append(Out(1, self.T))
+                o["spk"].append(Out(2, self.T))
+                o["rms"].append(Out(1, 2))
+                mixes.append(render.Mixture([base, base + 1], list(range(base + 2, base + S)), self.sirs[u],
+                                            self.snr[u], o["mix"][-1].view(self.T), o["spk"][-1].view(2, self.T),
+                                            o["rms"][-1].view(2), mono=True))
+                draws.append(render.CropDraw(self.starts[u], [base, base + 1], self.u[u], self.used[u]))
+            self.o[arm] = o
+            self.plans[arm] = R.plan_device(srcs, [x.view() for x in o["outs"]],
+                                             direct_outs=[None if x is None else x.view() for x in o["douts"]],
+                                             mixtures=mixes, draws=draws)
+
+    def bufs(self, arm):
+        o = self.o[arm]
+        return o["outs"] + [x for x in o["douts"] if x is not None] + o["mix"] + o["spk"] + o["rms"]
+
+    def draw(self, gen):
+        for k, (key, _) in enumerate(self.layout):
+            n = self.pools[key].host.n
+            self.picks[:, k].copy_(torch.randint(0, n, (self.U,), generator=gen, device="cuda", dtype=torch.int32))
+        self.u.uniform_(generator=gen)
+        self.sirs.uniform_(-6, 6, generator=gen)
+        self.snr.uniform_(10, 20, generator=gen)
+
+    def run(self, gen, tables, run, full_check, what):
+        """One run of every arm's plan; returns the number of draws checked against draw_reference."""
+        self.draw(gen)
+        R = _R()[1]
+        drawn, self.launches = {}, {}
+        for arm in self.arms:
+            for x in self.bufs(arm):
+                x.reset()
+            self.starts.fill_(-1)
+            self.used.fill_(-7)
+            R.reset_stats()
+            self.plans[arm].run()
+            self.launches[arm] = R.launch_count()
+            drawn[arm] = (self.starts.clone(), self.used.clone(), _device_errors(R))
+        torch.cuda.synchronize()
+        first = self.arms[0]
+        for arm in self.arms[1:]:                                        # (i)
+            for a, b in zip(self.bufs(first), self.bufs(arm)):
+                assert np.array_equal(a.get(), b.get()), (what, arm)
+            assert torch.equal(drawn[arm][0], drawn[first][0]) and torch.equal(drawn[arm][1], drawn[first][1]), arm
+            assert drawn[arm][2] == drawn[first][2] == 0, (arm, drawn[arm][2], drawn[first][2])
+        pk, st = self.picks.cpu().numpy(), self.starts.cpu().numpy()
+        used, u = self.used.cpu().numpy(), self.u.cpu().numpy()
+        sirs, snr = self.sirs.cpu().numpy(), self.snr.cpu().numpy()
+        o, S, checked = self.o[self.arms[-1]], len(self.layout), 0
+        for e in range(self.U):
+            a = int(st[e])
+            stems = []
+            for k, (key, taps) in enumerate(self.layout):
+                pl = self.pools[key]
+                i = int(pk[e, k])
+                y = o["outs"][S * e + k].get()
+                stems.append(y)
+                if full_check or e in (0, 7, 15):                       # (ii)
+                    c = pl.refs[i]
+                    label = "%s run %d scene %d stem %d cand %d start %d" % (what, run, e, k, i, a)
+                    c.check(y, a, self.T, gain=pl.gain(i), key="B %s %s" % (what, pl.variant), label=label)
+                    if taps:
+                        c.check(o["douts"][S * e + k].get(), a, self.T, direct=True, gain=pl.gain(i),
+                                key="B %s %s" % (what, pl.variant), label=label + " direct")
+            check_mixture(np.stack([fold(s) for s in stems[:2]]), np.stack([fold(s) for s in stems[2:]]), sirs[e],
+                          snr[e], o["mix"][e].get().reshape(-1), o["spk"][e].get().reshape(2, -1),
+                          o["rms"][e].get().reshape(-1), "%s run %d scene %d" % (what, run, e))
+            tabs = [tables[self.layout[k][0]][int(pk[e, k])] for k in range(2)]
+            Nr = [self.pools[key].cands[int(pk[e, k])].N for k, (key, _) in enumerate(self.layout)]
+            if dr.margins(tabs, [self.T, self.T], Nr, self.T, u[e]) < NEAR_DB:
+                continue
+            assert (a, int(used[e])) == dr.draw(tabs, [self.T, self.T], Nr, self.T, u[e]), (what, run, e)
+            checked += 1
+        return checked
+
+    def close(self):
+        for p in self.plans.values():
+            p.close()
+
+
+def _tables(pl):
+    return [pl.host.level_table(i).cpu().numpy() for i in range(pl.host.n)]
+
+
+def _training(pools, layout, what, runs=3, min_draws=30):
+    R = _R()[1]
+    tr = Training(pools, layout)
+    gen = torch.Generator(device="cuda")
+    gen.manual_seed(77)
+    tables = {k: _tables(p) for k, p in pools.items() if p.host.levels is not None}
+    for k, p in pools.items():
+        if p.host.levels is not None:
+            for i in range(p.host.n):
+                for arm in p.arms:
+                    assert torch.equal(p.host.level_table(i), p.pools[arm].level_table(i)), (what, k, arm, i)
+    try:
+        R.check_device_errors()
+        checked = sum(tr.run(gen, tables, r, r == 0, what) for r in range(runs))
+        assert checked >= min_draws, checked
+        for p in tr.plans.values():
+            assert p.is_graph()
+        R.check_device_errors()
+        print("\n%s: %d draws checked against draw_reference; launches per run %s" % (what, checked, tr.launches))
+        return tr.launches
+    finally:
+        tr.close()
+
+
+def copy_batches(C, cands, first, form="spectra"):
+    """render_host_stems' batching restated: candidate i's copy is its reverberant spectra (its taps, half the bytes,
+    for a tap-form pool) and dry signal, each 256-aligned (stem_copy_bytes); the buffer holds max(largest copy, min(all copies, 256 MiB)) (stem_copy_cap); inside
+    every stem group a batch takes candidates while they fit, and always at least one.  Returns every batch's first
+    candidate."""
+    row = 4 * B if form == "taps" else 8 * B
+    cb = [align_up(row * c.P * C * c.K, 256) + align_up(4 * c.N, 256) for c in cands]
+    cap = max(max(cb), min(sum(cb), STEM_BYTES))
+    starts = []
+    for g in range(len(first) - 1):
+        lo = first[g]
+        while lo < first[g + 1]:
+            starts.append(lo)
+            used, hi = 0, lo
+            while hi < first[g + 1] and (hi == lo or used + cb[hi] <= cap):
+                used += cb[hi]
+                hi += 1
+            lo = hi
+    return starts, cap
+
+
+def d_speakers(rng, L=4096):
+    import bench
+    items = bench.make_inputs(24, 0)
+    N, P, C = 30 * RATE, 60, 6
+    cut = {5: 1, 18: 7, 30: 13, 47: 29}
+    out = []
+    for j, (x, _, _) in enumerate(items):
+        n = N - cut.get(j, 0)
+        b = _random_cuts(rng, P, n)
+        out.append(ScaleCand(gappy_dry(rng, n) * np.float32(4.0) if j % 2 else x[:n].copy(), so.synth_rirs(rng, P, C, L), b))
+    return out
+
+
+def d_giant(rng, P_giant=400):
+    """A moving 8-channel pool: one candidate with P = P_giant and L = 12288 (315 MB of spectra at P = 400) between
+    ordinary ones."""
+    out = []
+    for j in range(5):
+        if j == 2:
+            P, L, N = P_giant, 12288, 400003
+        else:
+            P, L, N = 5, 4096, 300001 + 7 * j
+        out.append(ScaleCand(so.synth_dry(rng, N) * np.float32(0.5 + 0.25 * (j % 3)), so.synth_rirs(rng, P, 8, L),
+                        np.round(np.linspace(0, N, P)).astype(np.int32)))
+    return out
+
+
+def host_alone(R, render, c, target):
+    """render_host of the candidate alone over a device bank: the (C, N) stem and, with a target, (LUFS, gain)."""
+    bank = R.rir_bank(c.h)
+    try:
+        lo = []
+        y = R.render_host([render.MovingSource(c.x, bank, c.b)], lufs_targets=None if target is None else [target],
+                          loudness_out=lo, sr=RATE)[0]
+    finally:
+        bank.close()
+    return y, (tuple(lo[0]) if target is not None else None)
+
+
+# ------------------------------------------------------------------- device pools and the dry beacon draws
+class DevPool:
+    """A device source pool over candidates (test_gpu_host_pool_scale.Cand), with direct sets of `taps` taps."""
+
+    def __init__(self, cands, taps=0, levels=None):
+        render, R = _R()
+        self.cands, self.taps = cands, taps
+        self.banks = [R.rir_bank(c.h if c.P > 1 else c.h[0], direct_taps=taps) for c in cands]
+        self.srcs = [render.StaticSource(to(c.x), bk) if c.P == 1 else
+                     render.MovingSource(to(c.x), bk, to(c.b), bounds_host=c.b) for c, bk in zip(cands, self.banks)]
+        self.pool = R.source_pool(self.srcs, levels=levels)
+        self.n_max = max(c.N for c in cands)
+        # a K = 1 candidate of a pool whose candidates differ in K renders on the pool's blocking, not bit for bit as
+        # alone (test_gpu_pool_lengths): its stems are held to float64 only
+        self.bits = [c.K > 1 or all(o.K == 1 for o in cands) for c in cands]
+
+    def ref(self, i, x, s, wl):
+        """render_device of candidate i with dry x[:N] at the fixed window (s, wl): host (stem, direct stem or None)."""
+        _, R = _R()
+        c = self.cands[i]
+        out = torch.empty((c.C, wl), device="cuda")
+        dout = torch.empty((c.C, wl), device="cuda") if self.taps else None
+        src = self.srcs[i] if x is None else self.srcs[i]._replace(dry=x[:c.N].contiguous())
+        R.render_device([src._replace(window=(s, wl), direct_taps=self.taps)], [out],
+                        direct_outs=[dout] if self.taps else None)
+        return out.cpu().numpy(), (dout.cpu().numpy() if self.taps else None)
+
+    def close(self):
+        self.pool.close()
+        for b in self.banks:
+            b.close()
+
+
+
+D_TRIES = [1, 2, 31, 32, 33, 101, 4096]
+
+
+
+def dry_beacon(rng, N, zone_end):
+    """A dry signal loud (about -4.4 dB) everywhere, and with `zone_end` silent on [0, EDGE), [Z0, Z1) and
+    [zone_end - EDGE, zone_end): every crop inside a zone is exactly silent in the signal's own table."""
+    x = so.synth_dry(rng, N) * np.float32(6.0)
+    if zone_end:
+        x[:EDGE] = 0.0
+        x[Z0:Z1] = 0.0
+        x[zone_end - EDGE:zone_end] = 0.0
+    return x
+
+
+def traj_beacon(rng, N):
+    """A loud static 2-channel candidate with a 64-tap RIR (its pool's level table is loud everywhere)."""
+    h = np.zeros((1, 2, 64), np.float32)
+    h[0, :, 0] = 1.0
+    h[0, :, 1:] = rng.standard_normal((2, 63)) * 0.05 * np.exp(-np.arange(1, 64) / 16.0)
+    return ScaleCand(so.synth_dry(rng, N) * np.float32(6.0), h, None)
+
+
+
+def d_combos():
+    for tries in D_TRIES:
+        for t in sorted({t for t in TSTARS if t < tries} | {tries - 1}) + [None]:
+            yield tries, t
+
+
+def d_cases(layouts, seeds=(0,)):
+    out = []
+    for seed in seeds:
+        for n, (tries, t) in enumerate(d_combos()):
+            for j, lay in enumerate(layouts):
+                out.append(Case(lay, tries, t, False, 2000 + 1000 * seed + 17 * n + j))
+                if tries > 37 and (t is None or t > 36) and seed == 0:
+                    out.append(Case(lay, tries, t, True, 2000 + 1000 * seed + 17 * n + j + 7))
+    return out
+
+
+class DryDrawPlan:
+    """A plan of the cases' draws: every speaker lane a dry-picked slot of the trajectory pool, except the loud speakers
+    of every other draw with two or more, which are plain pooled slots (mixed); noise lanes slots of the noise pool.
+    With `dp16` (a 16-bit pool of bw.dp's values) every other dry-picked lane, alternating by draw and lane, picks from
+    it instead: a draw mixes 16-bit and float speakers, at every lane.  `lanes16` counts (draw, lane) of 16-bit picks."""
+
+    def __init__(self, bw, cases, dp16=None):
+        render, R = _R()
+        self.cases = cases
+        nd = len(cases)
+        self.starts = torch.zeros(nd, dtype=torch.int32, device="cuda")
+        self.used = torch.full((nd,), -7, dtype=torch.int32, device="cuda")
+        self.u = torch.from_numpy(np.concatenate([c.u for c in cases])).cuda()
+        pk, dk, self.what, self.slot0 = [], [], [], []
+        for k, c in enumerate(cases):
+            lanes = []
+            victim = c.layout[2]
+            for lane, (p, i) in enumerate(c.lanes):
+                if p == "noi":
+                    lanes.append(("noi", i))
+                elif i in (1, 3) and k % 2 and c.speakers.index(lane) != victim:
+                    lanes.append(("plain", 0 if i < 2 else 1))
+                else:
+                    lanes.append(("dry", i))
+                pk.append(i if p == "noi" else (0 if i < 2 else 1))
+                dk.append(i if p == "spk" else 0)
+            self.what.append(lanes)
+        self.picks = torch.tensor(pk, dtype=torch.int32, device="cuda")
+        self.dpicks = torch.tensor(dk, dtype=torch.int32, device="cuda")
+        self.out = torch.empty((len(pk), 2, WB), device="cuda")
+        srcs, draws, off = [], [], 0
+        self.lanes16 = []
+        for k, c in enumerate(cases):
+            base = len(srcs)
+            self.slot0.append(base)
+            for j, (p, _) in enumerate(self.what[k]):
+                q = base + j
+                pool = bw.np.pool if p == "noi" else bw.tp.pool
+                dry = None
+                if p == "dry":
+                    i16 = dp16 is not None and (k + j) % 2 == 0
+                    dry = render.DryPick(dp16 if i16 else bw.dp, self.dpicks[q])
+                    if i16:
+                        self.lanes16.append((k, j))
+                srcs.append(render.Pooled(pool, self.picks[q], (self.starts[k], WB), 0, dry))
+            draws.append(render.CropDraw(self.starts[k], [base + lane for lane in c.speakers],
+                                         self.u[off:off + c.tries], self.used[k]))
+            off += c.tries
+        self.plan = R.plan_device(srcs, [self.out[i] for i in range(len(srcs))], draws=draws)
+
+    def run(self):
+        self.out.fill_(NAN)
+        self.starts.fill_(-1)
+        self.plan.run()
+        torch.cuda.synchronize()
+
+    def check(self, bw, what):
+        starts, used = self.starts.cpu().numpy(), self.used.cpu().numpy()
+        worst = np.inf
+        for k, c in enumerate(self.cases):
+            label = (what, k, c.layout, c.tries, c.tstar)
+            got = (int(starts[k]), int(used[k]))
+            assert got == (c.start, c.used), (label, got, (c.start, c.used))
+            lanes = self.what[k]
+            tabs = [bw.Td[lanes[lane][1]] if lanes[lane][0] == "dry" else bw.Tp[lanes[lane][1]] for lane in c.speakers]
+            Nr = [(bw.np if p == "noi" else bw.tp).cands[i if p == "noi" else (i if p == "plain" else int(i >= 2))].N
+                  for p, i in lanes]
+            D = [WB] * len(tabs)
+            assert dr.draw(tabs, D, Nr, WB, c.u) == got, label
+            m = dr.margins(tabs, D, Nr, WB, c.u)
+            assert m >= 29.0, (label, m)                       # no draw near the threshold
+            worst = min(worst, m)
+            s = got[0]
+            for j, x in enumerate(lanes):
+                assert torch.equal(self.out[self.slot0[k] + j], bw.full[x][:, s:s + WB]), (label, j, x)
+        return worst
+
+    def close(self):
+        self.plan.close()
+
+

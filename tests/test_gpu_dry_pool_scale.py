@@ -32,8 +32,8 @@ from render_reference import TAU_GLOBAL, TAU_LOCAL, check_render, dry_signal, re
 from draw_reference import NEAR_DB, TABLE_TOL, gappy_dry
 from gpu_plumbing import _R, _device_errors, _rms, pmap, to
 from mix_reference import Out, check_mixture, fold
-from pool_worlds import (Case, EDGE, LARGE, NL, NN, NS, SMALL, ScaleCand, TSTARS, WB, Z0, Z1, _bounds_of, _random_cuts,
-                         a_aligned, a_mixed_k, a_static)
+from pool_worlds import (LARGE, NL, NN, NS, SMALL, DevPool, DryDrawPlan, ScaleCand, _bounds_of, _random_cuts,
+                         a_aligned, a_mixed_k, a_static, d_cases, d_combos, dry_beacon, traj_beacon)
 from window_cases import _choice
 
 pytestmark = pytest.mark.gpu
@@ -79,38 +79,6 @@ def check_f64(jobs):
         s = STATS.setdefault(key, [0.0, 0.0])
         s[0], s[1] = max(s[0], worst), max(s[1], g)
         QUIET[key] = QUIET.get(key, 0) + int(quiet)
-
-
-class DevPool:
-    """A device source pool over candidates (test_gpu_host_pool_scale.Cand), with direct sets of `taps` taps."""
-
-    def __init__(self, cands, taps=0, levels=None):
-        render, R = _R()
-        self.cands, self.taps = cands, taps
-        self.banks = [R.rir_bank(c.h if c.P > 1 else c.h[0], direct_taps=taps) for c in cands]
-        self.srcs = [render.StaticSource(to(c.x), bk) if c.P == 1 else
-                     render.MovingSource(to(c.x), bk, to(c.b), bounds_host=c.b) for c, bk in zip(cands, self.banks)]
-        self.pool = R.source_pool(self.srcs, levels=levels)
-        self.n_max = max(c.N for c in cands)
-        # a K = 1 candidate of a pool whose candidates differ in K renders on the pool's blocking, not bit for bit as
-        # alone (test_gpu_pool_lengths): its stems are held to float64 only
-        self.bits = [c.K > 1 or all(o.K == 1 for o in cands) for c in cands]
-
-    def ref(self, i, x, s, wl):
-        """render_device of candidate i with dry x[:N] at the fixed window (s, wl): host (stem, direct stem or None)."""
-        _, R = _R()
-        c = self.cands[i]
-        out = torch.empty((c.C, wl), device="cuda")
-        dout = torch.empty((c.C, wl), device="cuda") if self.taps else None
-        src = self.srcs[i] if x is None else self.srcs[i]._replace(dry=x[:c.N].contiguous())
-        R.render_device([src._replace(window=(s, wl), direct_taps=self.taps)], [out],
-                        direct_outs=[dout] if self.taps else None)
-        return out.cpu().numpy(), (dout.cpu().numpy() if self.taps else None)
-
-    def close(self):
-        self.pool.close()
-        for b in self.banks:
-            b.close()
 
 
 def check_stem(pl, i, xd, xh, s, wl, y, yd, key, label, jobs):
@@ -509,28 +477,6 @@ def test_multi_chunk_plan_over_two_dry_pools(chunk_budget):
 
 
 # ----------------------------------------------------------------------------------------- D. draws
-D_TRIES = [1, 2, 31, 32, 33, 101, 4096]
-
-
-def dry_beacon(rng, N, zone_end):
-    """A dry signal loud (about -4.4 dB) everywhere, and with `zone_end` silent on [0, EDGE), [Z0, Z1) and
-    [zone_end - EDGE, zone_end): every crop inside a zone is exactly silent in the signal's own table."""
-    x = so.synth_dry(rng, N) * np.float32(6.0)
-    if zone_end:
-        x[:EDGE] = 0.0
-        x[Z0:Z1] = 0.0
-        x[zone_end - EDGE:zone_end] = 0.0
-    return x
-
-
-def traj_beacon(rng, N):
-    """A loud static 2-channel candidate with a 64-tap RIR (its pool's level table is loud everywhere)."""
-    h = np.zeros((1, 2, 64), np.float32)
-    h[0, :, 0] = 1.0
-    h[0, :, 1:] = rng.standard_normal((2, 63)) * 0.05 * np.exp(-np.arange(1, 64) / 16.0)
-    return ScaleCand(so.synth_dry(rng, N) * np.float32(6.0), h, None)
-
-
 @pytest.fixture(scope="module")
 def dry_beacons():
     """Speaker lane ("spk", i) of test_gpu_pool_builds.Case is a slot of the trajectory pool (candidate 0 of NS samples
@@ -560,96 +506,6 @@ def dry_beacons():
     for p in (tp, npl):
         p.close()
     dp.close()
-
-
-def d_combos():
-    for tries in D_TRIES:
-        for t in sorted({t for t in TSTARS if t < tries} | {tries - 1}) + [None]:
-            yield tries, t
-
-
-def d_cases(layouts, seeds=(0,)):
-    out = []
-    for seed in seeds:
-        for n, (tries, t) in enumerate(d_combos()):
-            for j, lay in enumerate(layouts):
-                out.append(Case(lay, tries, t, False, 2000 + 1000 * seed + 17 * n + j))
-                if tries > 37 and (t is None or t > 36) and seed == 0:
-                    out.append(Case(lay, tries, t, True, 2000 + 1000 * seed + 17 * n + j + 7))
-    return out
-
-
-class DryDrawPlan:
-    """A plan of the cases' draws: every speaker lane a dry-picked slot of the trajectory pool, except the loud speakers
-    of every other draw with two or more, which are plain pooled slots (mixed); noise lanes slots of the noise pool."""
-
-    def __init__(self, bw, cases):
-        render, R = _R()
-        self.cases = cases
-        nd = len(cases)
-        self.starts = torch.zeros(nd, dtype=torch.int32, device="cuda")
-        self.used = torch.full((nd,), -7, dtype=torch.int32, device="cuda")
-        self.u = torch.from_numpy(np.concatenate([c.u for c in cases])).cuda()
-        pk, dk, self.what, self.slot0 = [], [], [], []
-        for k, c in enumerate(cases):
-            lanes = []
-            victim = c.layout[2]
-            for lane, (p, i) in enumerate(c.lanes):
-                if p == "noi":
-                    lanes.append(("noi", i))
-                elif i in (1, 3) and k % 2 and c.speakers.index(lane) != victim:
-                    lanes.append(("plain", 0 if i < 2 else 1))
-                else:
-                    lanes.append(("dry", i))
-                pk.append(i if p == "noi" else (0 if i < 2 else 1))
-                dk.append(i if p == "spk" else 0)
-            self.what.append(lanes)
-        self.picks = torch.tensor(pk, dtype=torch.int32, device="cuda")
-        self.dpicks = torch.tensor(dk, dtype=torch.int32, device="cuda")
-        self.out = torch.empty((len(pk), 2, WB), device="cuda")
-        srcs, draws, off = [], [], 0
-        for k, c in enumerate(cases):
-            base = len(srcs)
-            self.slot0.append(base)
-            for j, (p, _) in enumerate(self.what[k]):
-                q = base + j
-                pool = bw.np.pool if p == "noi" else bw.tp.pool
-                dry = render.DryPick(bw.dp, self.dpicks[q]) if p == "dry" else None
-                srcs.append(render.Pooled(pool, self.picks[q], (self.starts[k], WB), 0, dry))
-            draws.append(render.CropDraw(self.starts[k], [base + lane for lane in c.speakers],
-                                         self.u[off:off + c.tries], self.used[k]))
-            off += c.tries
-        self.plan = R.plan_device(srcs, [self.out[i] for i in range(len(srcs))], draws=draws)
-
-    def run(self):
-        self.out.fill_(NAN)
-        self.starts.fill_(-1)
-        self.plan.run()
-        torch.cuda.synchronize()
-
-    def check(self, bw, what):
-        starts, used = self.starts.cpu().numpy(), self.used.cpu().numpy()
-        worst = np.inf
-        for k, c in enumerate(self.cases):
-            label = (what, k, c.layout, c.tries, c.tstar)
-            got = (int(starts[k]), int(used[k]))
-            assert got == (c.start, c.used), (label, got, (c.start, c.used))
-            lanes = self.what[k]
-            tabs = [bw.Td[lanes[lane][1]] if lanes[lane][0] == "dry" else bw.Tp[lanes[lane][1]] for lane in c.speakers]
-            Nr = [(bw.np if p == "noi" else bw.tp).cands[i if p == "noi" else (i if p == "plain" else int(i >= 2))].N
-                  for p, i in lanes]
-            D = [WB] * len(tabs)
-            assert dr.draw(tabs, D, Nr, WB, c.u) == got, label
-            m = dr.margins(tabs, D, Nr, WB, c.u)
-            assert m >= 29.0, (label, m)                       # no draw near the threshold
-            worst = min(worst, m)
-            s = got[0]
-            for j, x in enumerate(lanes):
-                assert torch.equal(self.out[self.slot0[k] + j], bw.full[x][:, s:s + WB]), (label, j, x)
-        return worst
-
-    def close(self):
-        self.plan.close()
 
 
 def test_draw_warp_edges_with_dry_speakers(dry_beacons):

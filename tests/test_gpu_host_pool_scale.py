@@ -21,16 +21,15 @@ import numpy as np
 import pytest
 import torch
 
-import draw_reference as dr
 from chunk_budget import DEFAULT_CHUNK_BYTES, chunk_budget  # noqa: F401  (fixture)
 from oracle import sonicsim_oracle as so
-from render_reference import delay_rirs, graded_dry
 from window_cases import stage_set_np
-from draw_reference import NEAR_DB, TABLE_TOL, gappy_dry
+from draw_reference import TABLE_TOL, gappy_dry
 from gpu_plumbing import _R, to
-from mix_reference import Out, check_mixture, fold
-from pool_worlds import (A_LENS, QUIET, STATS, STEM_BYTES, ScaleCand, _bounds_of, _random_cuts, a_aligned, a_mixed_k,
-                         a_static, align_up, stem_groups, table_error)
+from mix_reference import Out
+from pool_worlds import (A_LENS, STEM_BYTES, Pools, Probes, ScaleCand, _hold, _random_cuts, _training, a_aligned,
+                         a_grid, a_mixed_k, a_static, align_up, b_configs1, copy_batches, d_giant, d_speakers,
+                         host_alone, probe_starts, read_set, report as _report, stem_groups, table_error)
 from window_cases import _choice
 
 pytestmark = pytest.mark.gpu
@@ -38,174 +37,12 @@ pytestmark = pytest.mark.gpu
 RATE = 16000
 B = 4096
 TAPS = 40
-TRIES = 101
 ONE_CHUNK = 1 << 30
-PINNED_MAX = 2 << 30
-
-
-def _report(title):
-    print("\n%s:" % title)
-    for k in sorted(STATS):
-        if k.startswith(title.split(":")[0]):
-            print("  %-40s worst per-sample ratio %.3g, worst global relative RMS %.3g; %d quiet crops%s" % (
-                k, *STATS[k], len(QUIET.get(k, [])), (" (first: %s)" % QUIET[k][0]) if k in QUIET else ""))
-
-
-def pool_variant(cands):
-    """The render kernel every slot of a pool of these candidates runs: static pools k_render_fast, pools of K > 1
-    k_render<1,0>, moving pools whose every candidate picks aligned blocking on its own k_render_fast, and every other
-    moving pool (mixed blocking renders on the grid) k_render<0,0>."""
-    if cands[0].P == 1:
-        return "k_render_fast static"
-    if max(c.K for c in cands) > 1:
-        return "k_render<1,0>"
-    return "k_render_fast" if all(_choice(c.b, c.N, c.P, c.L) for c in cands) else "k_render<0,0>"
-
-
-class Pools:
-    """One set of candidates as a device pool and as a host pool (banks shared between candidates when `share` names
-    the RIR set of each), with direct sets of TAPS taps when `taps`, level tables and loudness targets.  Counts the
-    pinned bytes it holds."""
-
-    def __init__(self, cands, taps=False, levels=None, lufs=None, share=None, host_only=False):
-        render, R = _R()
-        self.cands, self.taps = cands, taps
-        self.pools, self.banks = {}, []
-        sets = share if share is not None else list(range(len(cands)))
-        for host in ((True,) if host_only else (False, True)):
-            banks = {}
-            for c, r in zip(cands, sets):
-                if r not in banks:
-                    banks[r] = R.rir_bank(c.h if c.P > 1 else c.h[0], direct_taps=TAPS if taps else 0, host=host)
-            self.banks += list(banks.values())
-            srcs = []
-            for c, r in zip(cands, sets):
-                if c.P == 1:
-                    srcs.append(render.StaticSource(c.x if host else to(c.x), banks[r]))
-                elif host:
-                    srcs.append(render.MovingSource(c.x, banks[r], c.b))
-                else:
-                    srcs.append(render.MovingSource(to(c.x), banks[r], to(c.b), bounds_host=c.b))
-            self.pools[host] = R.source_pool(srcs, levels=levels, lufs_targets=lufs, sr=RATE)
-        self.variant = pool_variant(cands)
-        pinned = sum(k.host_nbytes for k in self.banks) + self.pools[True].host_nbytes
-        self.pinned = pinned
-        self.gains = self.pools[True].loudness[:, 1]
-
-    def gain(self, i):
-        g = self.gains[i]
-        return 1.0 if np.isnan(g) else float(g)
-
-    def close(self):
-        for p in self.pools.values():
-            p.close()
-        for k in self.banks:
-            k.close()
-
-
-def _hold(*pools):
-    """The pinned host bytes the test's banks and pools hold, as the library counts them (host_nbytes; the renderer's own
-    host staging buffers not included), printed and kept under 2 GB."""
-    total = sum(p.pinned for p in pools)
-    print("\npinned host memory of the banks and pools held (host_nbytes): %.1f MB" % (total / 1e6))
-    assert total <= PINNED_MAX, total
-    return total
 
 
 # ----------------------------------------------------------------------------------------- A. staged crops
-
-
-def a_grid(rng):
-    """Moving candidates with 59 segments of 0.3 to 3.8 k samples (grid blocking), pure-delay RIRs, graded dry
-    signals."""
-    out = []
-    for j, N in enumerate((70001, 83002)):
-        P = 60
-        np.random.seed(500 + j)
-        b = _bounds_of(so.setup_dynamic_interp(so.synth_path(rng, P), N)[0], P)
-        assert _choice(b, N, P, 4096) == 0
-        out.append(ScaleCand(graded_dry(rng, N), delay_rirs(rng, P, 3, 4096)[0], b))
-    return out
-
-
 A_POOLS = {"grid": (a_grid, False, "k_render<0,0>"), "aligned": (a_aligned, True, "k_render_fast"),
            "mixed-K": (a_mixed_k, False, "k_render<1,0>"), "static": (a_static, False, "k_render_fast static")}
-
-
-def probe_starts(c, wl, rng):
-    """0 and N - len; the maximisers of stage_cap, (K + 2) 4096 and b[s + 1] - 1 + (K + 2) 4096; starts where xa clamps
-    to 0 and where xb clamps to N; starts with ws % 4 in {1, 2, 3}; all inside [0, N - len]."""
-    last = c.N - wl
-    d0 = (c.K + 2) * B
-    s = {0, last, d0, d0 - 1, 1, last - 1, max(0, c.N - wl - 2 * B + 1)}
-    for q in ([] if c.b is None else c.b[1:-1]):
-        s.add(int(q) - 1 + d0)
-    for m in (1, 2, 3):
-        v = int(rng.integers(0, last + 1))
-        s.add(v - v % 4 + m)
-    return sorted(v for v in s if 0 <= v <= last)
-
-
-def read_set(c, ws, wl, sets):
-    """(bytes k_stage copies - whole float4s of dry samples and the rows of every set -, rows, dry samples)."""
-    xa, xb, _, rows = (int(v[0]) for v in stage_set_np(c.N, c.P, c.C, c.K, c.b, [ws], wl))
-    return 4 * (((xb + 3) & ~3) - (xa & ~3)) + sets * rows * B * 8, rows, xb - xa
-
-
-class Probes:
-    """A plan over both pools of `pl`: for every window length, `k` slots with device starts and one with a fixed
-    start, all over the same pick and start tensors, NaN-filled guarded outputs."""
-
-    def __init__(self, pl, lens, k, fixed):
-        render, R = _R()
-        self.pl, self.lens, self.k = pl, lens, k
-        n = len(lens) * (k + 1)
-        self.picks = torch.zeros(n, dtype=torch.int32, device="cuda")
-        self.starts = torch.zeros(n, dtype=torch.int32, device="cuda")
-        self.slots = []                               # (wl, fixed start or None)
-        for wl, f in zip(lens, fixed):
-            self.slots += [(wl, None)] * k + [(wl, f)]
-        C = pl.cands[0].C
-        self.plans, self.outs, self.douts = {}, {}, {}
-        for host, pool in pl.pools.items():
-            srcs = [render.Pooled(pool, self.picks[j], (self.starts[j] if f is None else f, wl), TAPS if pl.taps else 0)
-                    for j, (wl, f) in enumerate(self.slots)]
-            self.outs[host] = [Out(C, wl) for wl, _ in self.slots]
-            self.douts[host] = [Out(C, wl) for wl, _ in self.slots] if pl.taps else []
-            self.plans[host] = R.plan_device(srcs, [o.view() for o in self.outs[host]],
-                                             direct_outs=[o.view() for o in self.douts[host]] if pl.taps else None)
-
-    def run(self, pk, st):
-        self.pk, self.st = list(pk), [s if f is None else f for s, (_, f) in zip(st, self.slots)]
-        self.picks.copy_(torch.tensor(self.pk, dtype=torch.int32))
-        self.starts.copy_(torch.tensor(st, dtype=torch.int32))
-        R = _R()[1]
-        self.launches = {}
-        for host in self.plans:
-            for o in self.outs[host] + self.douts[host]:
-                o.reset()
-            R.reset_stats()
-            self.plans[host].run()
-            self.launches[host] = R.launch_count()
-        torch.cuda.synchronize()
-        for j in range(len(self.slots)):                  # (i) bit for bit the device-pool plan
-            a, b = self.outs[False][j].get(), self.outs[True][j].get()
-            assert np.array_equal(a, b), ("device twin", j, self.pk[j], self.st[j])
-            if self.pl.taps:
-                assert np.array_equal(self.douts[False][j].get(), self.douts[True][j].get()), ("direct twin", j)
-
-    def check(self, key, label):
-        for j, (wl, _) in enumerate(self.slots):          # (ii) float64
-            c = self.pl.cands[self.pk[j]]
-            g = self.pl.gain(self.pk[j])
-            what = "%s slot %d cand %d start %d len %d" % (label, j, self.pk[j], self.st[j], wl)
-            c.check(self.outs[True][j].get(), self.st[j], wl, gain=g, key=key, label=what)
-            if self.pl.taps:
-                c.check(self.douts[True][j].get(), self.st[j], wl, direct=True, gain=g, key=key, label=what + " direct")
-
-    def close(self):
-        for p in self.plans.values():
-            p.close()
 
 
 @pytest.mark.parametrize("kind", list(A_POOLS))
@@ -257,139 +94,6 @@ def test_staged_crops_at_every_read_set_edge(kind):
 
 
 # ----------------------------------------------------------------------------------------- B. training scale
-def b_configs1(rng):
-    """bench.make_inputs(16, 0): 32 configs[1] speakers (P = 40, C = 6, 30 s; every other dry signal gappy) and 16
-    static 6-channel noises."""
-    import bench
-    items = bench.make_inputs(16, 0)
-    spk = [ScaleCand(gappy_dry(rng, len(x)) if j % 2 else x, h, b) for j, (x, h, b) in enumerate(items)]
-    N, C = bench.CFG["N"], bench.CFG["C"]
-    noi = [ScaleCand((rng.standard_normal(N) * 0.05).astype(np.float32),
-                (rng.standard_normal((1, C, 4096)) * np.exp(-np.arange(4096) / 800.0)).astype(np.float32), None)
-           for _ in range(16)]
-    return spk, noi
-
-
-class Training:
-    """16 scenes: `layout` a list of (pools key, taps) per scene, the first two the mixture's speakers and the draw's,
-    the rest its noises; one start per scene drawn by a 101-try CropDraw over mono level tables; one mono Mixture."""
-
-    def __init__(self, pools, layout, U=16):
-        render, R = _R()
-        self.pools, self.layout, self.U = pools, layout, U
-        S = len(layout)
-        self.picks = torch.zeros((U, S), dtype=torch.int32, device="cuda")
-        self.starts = torch.zeros(U, dtype=torch.int32, device="cuda")
-        self.u = torch.zeros((U, TRIES), dtype=torch.float64, device="cuda")
-        self.used = torch.zeros(U, dtype=torch.int32, device="cuda")
-        self.sirs = torch.zeros((U, 1), device="cuda")
-        self.snr = torch.zeros(U, device="cuda")
-        self.T = 4 * RATE
-        self.plans, self.o = {}, {}
-        for host in (False, True):
-            srcs, outs, douts, mixes, draws = [], [], [], [], []
-            o = dict(outs=[], douts=[], mix=[], spk=[], rms=[])
-            for u in range(U):
-                base = len(srcs)
-                for k, (key, taps) in enumerate(layout):
-                    pl = pools[key]
-                    srcs.append(render.Pooled(pl.pools[host], self.picks[u, k], (self.starts[u], self.T),
-                                              TAPS if taps else 0))
-                    o["outs"].append(Out(pl.cands[0].C, self.T))
-                    o["douts"].append(Out(pl.cands[0].C, self.T) if taps else None)
-                o["mix"].append(Out(1, self.T))
-                o["spk"].append(Out(2, self.T))
-                o["rms"].append(Out(1, 2))
-                mixes.append(render.Mixture([base, base + 1], list(range(base + 2, base + S)), self.sirs[u],
-                                            self.snr[u], o["mix"][-1].view(self.T), o["spk"][-1].view(2, self.T),
-                                            o["rms"][-1].view(2), mono=True))
-                draws.append(render.CropDraw(self.starts[u], [base, base + 1], self.u[u], self.used[u]))
-            self.o[host] = o
-            self.plans[host] = R.plan_device(srcs, [x.view() for x in o["outs"]],
-                                             direct_outs=[None if x is None else x.view() for x in o["douts"]],
-                                             mixtures=mixes, draws=draws)
-
-    def bufs(self, host):
-        o = self.o[host]
-        return o["outs"] + [x for x in o["douts"] if x is not None] + o["mix"] + o["spk"] + o["rms"]
-
-    def draw(self, gen):
-        for k, (key, _) in enumerate(self.layout):
-            n = self.pools[key].pools[True].n
-            self.picks[:, k].copy_(torch.randint(0, n, (self.U,), generator=gen, device="cuda", dtype=torch.int32))
-        self.u.uniform_(generator=gen)
-        self.sirs.uniform_(-6, 6, generator=gen)
-        self.snr.uniform_(10, 20, generator=gen)
-
-    def run(self, gen, tables, run, full_check, what):
-        """One run of both plans; returns the number of draws checked against draw_reference."""
-        self.draw(gen)
-        for host in (False, True):
-            for x in self.bufs(host):
-                x.reset()
-            self.plans[host].run()
-        torch.cuda.synchronize()
-        for a, b in zip(self.bufs(False), self.bufs(True)):            # (i)
-            assert np.array_equal(a.get(), b.get()), what
-        pk, st = self.picks.cpu().numpy(), self.starts.cpu().numpy()
-        used, u = self.used.cpu().numpy(), self.u.cpu().numpy()
-        sirs, snr = self.sirs.cpu().numpy(), self.snr.cpu().numpy()
-        o, S, checked = self.o[True], len(self.layout), 0
-        for e in range(self.U):
-            a = int(st[e])
-            stems = []
-            for k, (key, taps) in enumerate(self.layout):
-                pl = self.pools[key]
-                i = int(pk[e, k])
-                y = o["outs"][S * e + k].get()
-                stems.append(y)
-                if full_check or e in (0, 7, 15):                       # (ii)
-                    c = pl.cands[i]
-                    label = "%s run %d scene %d stem %d cand %d start %d" % (what, run, e, k, i, a)
-                    c.check(y, a, self.T, gain=pl.gain(i), key="B %s %s" % (what, pl.variant), label=label)
-                    if taps:
-                        c.check(o["douts"][S * e + k].get(), a, self.T, direct=True, gain=pl.gain(i),
-                                key="B %s %s" % (what, pl.variant), label=label + " direct")
-            check_mixture(np.stack([fold(s) for s in stems[:2]]), np.stack([fold(s) for s in stems[2:]]), sirs[e],
-                          snr[e], o["mix"][e].get().reshape(-1), o["spk"][e].get().reshape(2, -1),
-                          o["rms"][e].get().reshape(-1), "%s run %d scene %d" % (what, run, e))
-            tabs = [tables[self.layout[k][0]][int(pk[e, k])] for k in range(2)]
-            Nr = [self.pools[key].cands[int(pk[e, k])].N for k, (key, _) in enumerate(self.layout)]
-            if dr.margins(tabs, [self.T, self.T], Nr, self.T, u[e]) < NEAR_DB:
-                continue
-            assert (a, int(used[e])) == dr.draw(tabs, [self.T, self.T], Nr, self.T, u[e]), (what, run, e)
-            checked += 1
-        return checked
-
-    def close(self):
-        for p in self.plans.values():
-            p.close()
-
-
-def _tables(pl):
-    return [pl.pools[True].level_table(i).cpu().numpy() for i in range(pl.pools[True].n)]
-
-
-def _training(pools, layout, what, runs=3, min_draws=30):
-    R = _R()[1]
-    tr = Training(pools, layout)
-    gen = torch.Generator(device="cuda")
-    gen.manual_seed(77)
-    tables = {k: _tables(p) for k, p in pools.items() if p.pools[True].levels is not None}
-    for k, p in pools.items():
-        if p.pools[True].levels is not None:
-            for i in range(p.pools[True].n):
-                assert torch.equal(p.pools[True].level_table(i), p.pools[False].level_table(i)), (what, k, i)
-    try:
-        R.check_device_errors()
-        checked = sum(tr.run(gen, tables, r, r == 0, what) for r in range(runs))
-        assert checked >= min_draws, checked
-        for p in tr.plans.values():
-            assert p.is_graph()
-        R.check_device_errors()
-        print("\n%s: %d draws checked against draw_reference" % (what, checked))
-    finally:
-        tr.close()
 
 
 @pytest.mark.parametrize("budget", ["default", "one-chunk"])
@@ -626,62 +330,6 @@ def test_many_staged_slots():
 
 
 # ----------------------------------------------------------------------------------------- D. builds across batches
-def copy_batches(C, cands, first):
-    """render_host_stems' batching restated: candidate i's copy is its reverberant spectra and dry signal, each
-    256-aligned (stem_copy_bytes); the buffer holds max(largest copy, min(all copies, 256 MiB)) (stem_copy_cap); inside
-    every stem group a batch takes candidates while they fit, and always at least one.  Returns every batch's first
-    candidate."""
-    cb = [align_up(8 * B * c.P * C * c.K, 256) + align_up(4 * c.N, 256) for c in cands]
-    cap = max(max(cb), min(sum(cb), STEM_BYTES))
-    starts = []
-    for g in range(len(first) - 1):
-        lo = first[g]
-        while lo < first[g + 1]:
-            starts.append(lo)
-            used, hi = 0, lo
-            while hi < first[g + 1] and (hi == lo or used + cb[hi] <= cap):
-                used += cb[hi]
-                hi += 1
-            lo = hi
-    return starts, cap
-
-
-def d_speakers(rng):
-    import bench
-    items = bench.make_inputs(24, 0)
-    N, P, C = 30 * RATE, 60, 6
-    cut = {5: 1, 18: 7, 30: 13, 47: 29}
-    out = []
-    for j, (x, _, _) in enumerate(items):
-        n = N - cut.get(j, 0)
-        b = _random_cuts(rng, P, n)
-        out.append(ScaleCand(gappy_dry(rng, n) * np.float32(4.0) if j % 2 else x[:n].copy(), so.synth_rirs(rng, P, C, 4096), b))
-    return out
-
-
-def d_giant(rng):
-    """A moving 8-channel pool: one candidate with P = 400 and L = 12288 (315 MB of spectra) between ordinary ones."""
-    out = []
-    for j in range(5):
-        if j == 2:
-            P, L, N = 400, 12288, 400003
-        else:
-            P, L, N = 5, 4096, 300001 + 7 * j
-        out.append(ScaleCand(so.synth_dry(rng, N) * np.float32(0.5 + 0.25 * (j % 3)), so.synth_rirs(rng, P, 8, L),
-                        np.round(np.linspace(0, N, P)).astype(np.int32)))
-    return out
-
-
-def host_alone(R, render, c, target):
-    """render_host of the candidate alone over a device bank: the (C, N) stem and, with a target, (LUFS, gain)."""
-    bank = R.rir_bank(c.h)
-    try:
-        lo = []
-        y = R.render_host([render.MovingSource(c.x, bank, c.b)], lufs_targets=None if target is None else [target],
-                          loudness_out=lo, sr=RATE)[0]
-    finally:
-        bank.close()
-    return y, (tuple(lo[0]) if target is not None else None)
 
 
 @pytest.mark.parametrize("kind", ["speakers", "giant"])
