@@ -334,7 +334,8 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * the device: bit 0 = an interp_index outside [0, P - 2], bit 1 = a device-side bounds table that is not ascending from
  * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
  * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped), bit 4 (dry
- * pools, below) = a dry pick outside [0, n) of its dry pool (clamped).  The Python device API raises IndexError /
+ * pools, below) = a dry pick outside [0, n) of its dry pool (clamped), bit 5 (dry streams, below) = an invalid
+ * entry of a stream slot's layout (skipped).  The Python device API raises IndexError /
  * ValueError from it on request
  * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
  * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
@@ -712,6 +713,46 @@ int ss_plan_create_target(ss_ctx* ctx, const ss_source* items, int n_items, cons
                           const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                           const ss_pair_gains* const* pair_gains /* NULL or n_picks entries, NULL = none */,
                           int n_picks, const ss_plan_target* targets, int n_targets, ss_plan** out);
+
+/* ---- dry streams: SonicSet's speech streams laid out at every run (SonicSim_audio.py:231-277, create_long_audio),
+ * from utterances held once in a 16-bit dry pool (ss_dry_pool_create_i16) instead of prebuilt 60 s streams.
+ * A stream slot is a pooled slot whose dry signal is a layout of m entries over a 16-bit dry pool of n utterances: two
+ * device int32 arrays ids[m] and offsets[m], 1 <= m <= 128, read at every run as picks and starts are.  At every run
+ * the layout is walked in order with a running `end`, 0 at first:
+ *   - ids[j] < 0: an empty entry, skipped (a fixed m holds a variable number of utterances);
+ *   - ids[j] >= n, offsets[j] < 0 or offsets[j] < end: an invalid entry, skipped, and ss_device_errors reports bit 5;
+ *   - otherwise the entry is kept: utterance ids[j] of len samples occupies [offsets[j], offsets[j] + len) of the
+ *     stream and end becomes offsets[j] + len.  Touching placements are fine, overlapping ones are not.
+ * The slot's dry signal is the stream's first N samples (N: the picked candidate's), zeros wherever no kept entry lies;
+ * a kept entry that reaches past N is cut there.  A stream slot's stem, direct stem, mixture contributions, rms_db,
+ * drawn start and `used` are, bit for bit, those of the same plan in which the slot takes an ss_dry_pick from a 16-bit
+ * dry pool holding the stream assembled by the rule above to the slot pool's longest N.  In a draw, a stream speaker's
+ * crop energy is summed per utterance from the dry pool's sparse tables: exact in float64, so the draw keeps those
+ * bits.
+ * A stream slot is always staged (k_stage), whatever the residency of its pool and of its dry pool; its staging area is
+ * a dry-picked slot's.  The plan uploads the n utterance lengths of each dry pool its streams use once, into its
+ * descriptor block.
+ * ss_plan_create_stream is ss_plan_create_target with n_streams entries (n_streams == 0: exactly
+ * ss_plan_create_target).  Refused at creation, before anything is allocated and with no plan created:
+ *   - SS_ERR_INVALID: n_streams < 0 or NULL streams with n_streams > 0; a slot outside [0, n_items), not pooled, named
+ *     by two streams or by a stream and a dry pick; a dry pool that is NULL, of another context or not 16-bit; m
+ *     outside [1, 128]; a NULL or unaligned ids_dev / offsets_dev; a slot whose pool has loudness gains (a stream has
+ *     no fixed (dry, trajectory) pair to measure); a draw speaker whose stream's dry pool has no level tables; a range
+ *     the plan writes that meets ids_dev or offsets_dev.
+ *   - SS_ERR_UNSUPPORTED: a slot pool whose longest candidate N exceeds 2^23 (beyond it the draws' sums need not be
+ *     exact).
+ * ss_version stays 108: the export marks the capability. */
+typedef struct {
+    int32_t slot;                     /* index into `items`: a pooled slot                                            */
+    const ss_dry_pool* pool;          /* a 16-bit dry pool of the plan's context                                      */
+    const int32_t* ids_dev;           /* device, m utterance ids (< 0: empty), read at every run                      */
+    const int32_t* offsets_dev;       /* device, m stream offsets in samples, read at every run                       */
+    int32_t m;                        /* 1..128                                                                       */
+} ss_dry_stream;
+int ss_plan_create_stream(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                          const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                          int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

@@ -2459,6 +2459,7 @@ struct ss_plan {
     const StageSlot* d_stage = nullptr;   // the staged slots' k_stage descriptors, in d_desc behind the draws
     int n_stage = 0;
     bool draw16 = false, stage16 = false; // a draw speaker / a staged slot has a 16-bit dry pick: k_draw<true> / k_stage<true>
+    bool draw_stream = false, stage_stream = false;   // a draw speaker / a staged slot is a stream slot (STREAM)
     // slots of tap-form pools: k_stage<I16, true> reads d_taps (n_stage entries) and writes n_tap transform Sources
     // (d_tap_src, CTA ranges d_tap_prefix), which one k_prepare<false> of tap_ctas CTAs transforms behind it
     const StageTap* d_taps = nullptr;
@@ -2482,6 +2483,7 @@ struct DrawReader {
     const int* dry_pick;              // ... its dry pick ...
     int n_dry;                        // ... and the dry pool's signal count
     int dry16;                        // 1: the dry pool is 16-bit (sparse tables, speaker_signal_i16; k_draw<true> only)
+                                      // 2: a stream slot (k_draw<true, true> only): dry_pick holds its DryStream
 };
 static_assert(sizeof(DrawReader) == 64, "DrawReader layout");
 struct DrawDesc {
@@ -2498,7 +2500,9 @@ struct DrawDesc {
 // ballot takes the first try at which no speaker is silent; after the last try without one, the last try's start.
 // k_draw<true> (a plan with a 16-bit dry-picked speaker) tests such a speaker from its sparse table and its signal's
 // samples (draw_silent_i16): at most 2 * 63 samples and two table entries per try, over PCIe for a host pool.
-template <bool I16>
+// k_draw<true, true> (a plan with a stream speaker) tests such a speaker by walking its layout at every try
+// (draw_silent_stream): the layout's entries are the same for every lane, the utterances' samples per lane.
+template <bool I16, bool STREAM = false>
 __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws, int n) {
     const int lane = threadIdx.x & 31, di = blockIdx.x * 4 + (threadIdx.x >> 5);
     if (di >= n) return;
@@ -2514,11 +2518,13 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
     const double* Q[kDrawSpeakers];
     double D[kDrawSpeakers];
     const int16_t* X[kDrawSpeakers];                    // (k_draw<true>) a 16-bit speaker's signal, else null
+    const DryStream* W[kDrawSpeakers];                  // (k_draw<true, true>) a stream speaker's layout, else null
 #pragma unroll
     for (int k = 0; k < kDrawSpeakers; ++k) {
-        Q[k] = nullptr; D[k] = 1.0; X[k] = nullptr;
+        Q[k] = nullptr; D[k] = 1.0; X[k] = nullptr; W[k] = nullptr;
         if (k < d.S) {
             const DrawReader& r = d.r[d.spk[k]];
+            if (STREAM && r.dry16 == 2) { W[k] = reinterpret_cast<const DryStream*>(r.dry_pick); continue; }
             Q[k] = speaker_table(r.levels, r.pick, r.n, r.dry_levels, r.dry_pick, r.n_dry);
             D[k] = r.D;
             if (I16 && r.dry16) X[k] = speaker_signal_i16(r.dry_levels, r.dry_pick, r.n_dry);
@@ -2534,8 +2540,9 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
             pass = true;
 #pragma unroll
             for (int k = 0; k < kDrawSpeakers; ++k)
-                if (k < d.S && pass && (I16 && X[k] ? draw_silent_i16(Q[k], X[k], s, d.len, d.threshold_db)
-                                                    : draw_silent(Q[k], s, d.len, D[k], d.threshold_db)))
+                if (k < d.S && pass && (STREAM && W[k] ? draw_silent_stream(*W[k], s, d.len, d.threshold_db)
+                                        : I16 && X[k] ? draw_silent_i16(Q[k], X[k], s, d.len, d.threshold_db)
+                                                      : draw_silent(Q[k], s, d.len, D[k], d.threshold_db)))
                     pass = false;
         }
         const unsigned ok = __ballot_sync(0xffffffffu, pass);
@@ -2578,30 +2585,71 @@ struct StageSlot {
     int sets;                         // spectra sets staged: 1, 2 with a direct target, 0 for a slot of a device pool
     int n_dry;                        // ... and the dry pool's signal count
     int i16;                          // 1: the dry pool is 16-bit, `dry` holds int16 addresses (k_stage<true> only)
+                                      // 2: a stream slot (k_stage<true, TAPS, true> only): `dry` holds its DryStream's
+                                      //    address, dry_pick is null
 };
 static_assert(sizeof(StageSlot) == 120, "StageSlot layout");
+// k_stage<true, TAPS, true> (a plan with a stream slot) fills such a slot's whole groups [xa & ~3, (xb + 3) & ~3) from
+// its layout: the CTA loads the m entries into shared memory, one thread walks them (stream_resolve, bit 5), then
+// every thread stores samples of the read set (stream_sample), consecutive threads consecutive samples, so that a
+// warp's int16 loads are contiguous within an utterance (coalesced over PCIe from a host arena).
+__device__ __forceinline__ void stage_stream_x(const DryStream& d, int x0, int x1, float* __restrict__ xd) {
+    __shared__ int s_id[kStreamEntries], s_off[kStreamEntries], s_len[kStreamEntries], s_a[kStreamEntries],
+        s_b[kStreamEntries];
+    __shared__ const int16_t* s_sig[kStreamEntries];
+    __shared__ const int16_t* s_p[kStreamEntries];
+    __shared__ int s_k;
+    for (int j = threadIdx.x; j < d.m; j += blockDim.x) {
+        const int id = d.ids[j];
+        const bool ok = id >= 0 && id < d.n;
+        s_id[j] = id; s_off[j] = d.offsets[j];
+        s_len[j] = ok ? d.lengths[id] : 0;
+        s_sig[j] = ok ? d.sig[id] : nullptr;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int k;
+        const unsigned err = stream_resolve(s_id, s_off, s_len, s_sig, d.m, d.n, d.cut, s_a, s_b, s_p, &k);
+        s_k = k;
+        if (err && blockIdx.x == 0) atomicOr(&g_dev_err, err);
+    }
+    __syncthreads();
+    const int nx = x1 - x0, k = s_k, stride = gridDim.x * blockDim.x;
+    for (int t0 = blockIdx.x * blockDim.x + threadIdx.x; t0 < nx; t0 += stride * kStageUnroll) {
+        float v[kStageUnroll];
+#pragma unroll
+        for (int u = 0; u < kStageUnroll; ++u) {        // every load issued before the first store
+            const int t = t0 + u * stride;
+            v[u] = t < nx ? stream_sample(s_a, s_b, s_p, k, x0 + t) : 0.0f;
+        }
+#pragma unroll
+        for (int u = 0; u < kStageUnroll; ++u) if (t0 + u * stride < nx) xd[t0 + u * stride] = v[u];
+    }
+}
 // k_stage<true> (a plan with a 16-bit dry pick) reads such a slot's dry samples as 4 int16 at a time from the whole
 // groups [xa & ~3, (xb + 3) & ~3) of the picked signal (inside its padded arena) and stores their exact float32 values,
 // so that the staging area holds what a float pool's slot stages.
 // k_stage<I16, true> (a plan with a slot of a tap-form pool) copies such a slot's tap rows [row0, row0 + rows), one
 // contiguous span of the candidate's rows, instead of sets * rows spectra rows, and writes the Source over them that the
 // plan's transform launch (k_prepare<false>) turns into the spectra the slot's view names: those k_stage<I16> copies.
-template <bool I16, bool TAPS = false>
+template <bool I16, bool TAPS = false, bool STREAM = false>
 __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots, const StageTap* __restrict__ taps) {
     const StageSlot& g = slots[blockIdx.y];
     const StageTap* const tp = TAPS && taps[blockIdx.y].taps ? &taps[blockIdx.y] : nullptr;
+    const DryStream* const ds = STREAM && g.i16 == 2 ? reinterpret_cast<const DryStream*>(g.dry) : nullptr;
     __shared__ StageView s_v;
     __shared__ const float* s_src;                      // the signal the dry samples come from
     __shared__ int s_x[2];                              // dry samples copied: whole float4s [s_x[0], s_x[1])
     if (threadIdx.x == 0) {
         const unsigned err = stage_head(g.pool, g.n, *g.pick, g.parts, g.K, g.gains, g.ws_dev, g.ws, g.len, g.C,
-                                        g.sets != 0, g.dry, g.dry ? *g.dry_pick : 0, g.n_dry, s_v, s_src, s_x[0], s_x[1],
-                                        g.pair);
+                                        g.sets != 0, ds ? nullptr : g.dry, !ds && g.dry ? *g.dry_pick : 0, g.n_dry, s_v,
+                                        s_src, s_x[0], s_x[1], g.pair);
         if (err && blockIdx.x == 0) atomicOr(&g_dev_err, err);
     }
     __syncthreads();
+    if (STREAM && ds) stage_stream_x(*ds, s_x[0], s_x[1], g.x);   // (the loop below then copies no dry samples)
     const PoolEntry& e = s_v.e;
-    const size_t nx4 = (size_t)((s_x[1] - s_x[0]) >> 2);
+    const size_t nx4 = STREAM && ds ? 0 : (size_t)((s_x[1] - s_x[0]) >> 2);
     const size_t per_set = (size_t)s_v.rows * (kSpec / 2);          // float4s per set
     const size_t rows_h = (size_t)e.P * g.C * s_v.K;                 // rows per set of the bank
     const size_t total = nx4 + (TAPS && tp ? (size_t)s_v.rows * (kB / 4) : (size_t)g.sets * per_set);
@@ -2676,8 +2724,10 @@ static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double
 }
 
 // The descriptor of draw d of a plan: its readers in the callers' order of `items`
-// (dry[i]: item i's dry pick, or null; a dry-picked speaker tests its dry pool's one-channel tables, D = len)
-static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan_draw& d, const ss_dry_pick* const* dry) {
+// (dry[i]: item i's dry pick, or null; a dry-picked speaker tests its dry pool's one-channel tables, D = len; ws[i]:
+// the device address of item i's DryStream, or null: a stream speaker walks its layout, D = len)
+static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan_draw& d, const ss_dry_pick* const* dry,
+                              const DryStream* const* ws) {
     DrawDesc g; memset(&g, 0, sizeof(g));
     g.start = d.start; g.u = d.u; g.used = d.used; g.tries = d.tries; g.S = d.S; g.threshold_db = d.threshold_db;
     for (int i = 0; i < n_items; ++i) {
@@ -2692,6 +2742,7 @@ static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan
             r.dry_levels = dry[i]->pool->level_ptr; r.dry_pick = dry[i]->pick_dev; r.n_dry = dry[i]->pool->n; r.D = it.win_len;
             r.dry16 = dry[i]->pool->i16 ? 1 : 0;
         }
+        if (ws[i]) { r.dry_pick = reinterpret_cast<const int*>(ws[i]); r.dry16 = 2; r.D = it.win_len; }
         g.r[g.n_readers++] = r;
     }
     return g;
@@ -2721,10 +2772,11 @@ static StageArea stage_area_of(const ss_source& it) {
 }
 
 // (dry[i]: caller item i's dry pick, or null; pair[i]: its pair gains' device table, or null; dir_out[k]: mixture k's
-// dereverberation targets, or null)
+// dereverberation targets, or null; strm[i]: caller item i's dry stream, or null)
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
                       const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws,
-                      const ss_dry_pick* const* dry, const float* const* pair, float* const* dir_out) {
+                      const ss_dry_pick* const* dry, const float* const* pair, float* const* dir_out,
+                      const ss_dry_stream* const* strm) {
     ss_ctx* c = p->c;
     std::vector<int> cuts, order;
     std::vector<ss_source> arranged;
@@ -2732,7 +2784,10 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
     std::vector<const ss_dry_pick*> dry_arranged(arranged.size());
     std::vector<const float*> pair_arranged(arranged.size());
-    for (size_t i = 0; i < arranged.size(); ++i) { dry_arranged[i] = dry[order[i]]; pair_arranged[i] = pair[order[i]]; }
+    std::vector<const ss_dry_stream*> strm_arranged(arranged.size());
+    for (size_t i = 0; i < arranged.size(); ++i) {
+        dry_arranged[i] = dry[order[i]]; pair_arranged[i] = pair[order[i]]; strm_arranged[i] = strm[order[i]];
+    }
     std::vector<const ss_dry_pick*> dry_describe(dry_arranged);   // the dry picks k_blocks makes (pick_pooled)
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     const size_t n_chunks = cuts.size() - 1;
@@ -2753,9 +2808,10 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     const size_t draw_off = align_up(scr_off + scr_bytes * n_mixes, 256);
     const size_t desc_bytes = draw_off + sizeof(DrawDesc) * n_draws;
     // behind the draws: the staged slots' k_stage descriptors, then their staging areas
-    std::vector<int> staged;                            // arranged items that are slots of host pools, host or 16-bit dry picks
+    std::vector<int> staged;    // arranged items that are slots of host pools, host or 16-bit dry picks, stream slots
     for (int i = 0; i < (int)arranged.size(); ++i)
-        if (items[i].pool && (items[i].pool->host_res || (dry_arranged[i] && dry_arranged[i]->pool->padded()))) {
+        if (items[i].pool && (items[i].pool->host_res || (dry_arranged[i] && dry_arranged[i]->pool->padded()) ||
+                              strm_arranged[i])) {
             staged.push_back(i);
             dry_describe[i] = nullptr;                  // k_stage stages the dry pick: the counts hold none (take_view)
         }
@@ -2767,8 +2823,44 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     const TapBlock tb = tap_block(total, (int)staged.size(), n_tap);   // (slots of tap-form pools)
     const size_t tap_off = tb.taps, tsrc_off = tb.src, tpre_off = tb.prefix, zero_off = tb.zero;
     if (n_tap) total = tb.end;
+    const size_t tap_end = total;
+    // behind those: the streams' DryStream descriptors (caller order), then the utterance lengths of each dry pool
+    // they use, uploaded once
+    std::vector<const DryStream*> ws(n_items, nullptr);
+    std::vector<DryStream> wdesc;
+    std::vector<const ss_dry_pool*> wpools;
+    std::vector<size_t> wlen_off;
+    for (int i = 0; i < n_items; ++i) if (strm[i]) wdesc.emplace_back();
+    const size_t wdesc_off = align_up(total, 256);
+    if (!wdesc.empty()) {
+        total = wdesc_off + sizeof(DryStream) * wdesc.size();
+        for (int i = 0; i < n_items; ++i)
+            if (strm[i] && std::find(wpools.begin(), wpools.end(), strm[i]->pool) == wpools.end()) {
+                wpools.push_back(strm[i]->pool);
+                wlen_off.push_back(align_up(total, 256));
+                total = wlen_off.back() + sizeof(int32_t) * (size_t)strm[i]->pool->n;
+            }
+    }
     CK(cudaMalloc((void**)&p->d_desc, total + 256));
-    std::vector<char> tap_host(n_tap ? total - tap_off : 0, 0);
+    std::vector<char> tap_host(n_tap ? tap_end - tap_off : 0, 0);
+    for (int i = 0, k = 0; i < n_items; ++i) {
+        if (!strm[i]) continue;
+        const ss_dry_stream& w = *strm[i];
+        const ss_dry_pool* dp = w.pool;
+        const size_t lo = wlen_off[std::find(wpools.begin(), wpools.end(), dp) - wpools.begin()];
+        int cut = 0;
+        for (const PoolEntry& e : caller_items[i].pool->host) cut = std::max(cut, e.N);
+        wdesc[k] = {w.ids_dev, w.offsets_dev, (const int*)(p->d_desc + lo), (const int16_t* const*)dp->ptrs,
+                    dp->levels ? dp->level_ptr : nullptr, w.m, dp->n, cut, 0};
+        ws[i] = (const DryStream*)(p->d_desc + wdesc_off) + k;
+        ++k;
+    }
+    if (!wdesc.empty()) {
+        CK(cudaMemcpy(p->d_desc + wdesc_off, wdesc.data(), sizeof(DryStream) * wdesc.size(), cudaMemcpyHostToDevice));
+        for (size_t j = 0; j < wpools.size(); ++j)
+            CK(cudaMemcpy(p->d_desc + wlen_off[j], wpools[j]->N.data(), sizeof(int32_t) * (size_t)wpools[j]->n,
+                          cudaMemcpyHostToDevice));
+    }
     for (int i = 0; i < ss_ctx::kAux; ++i)
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
     std::vector<char> host(desc_bytes + 256);
@@ -2785,6 +2877,10 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
             g.dry = d->pool->ptrs; g.dry_pick = d->pick_dev; g.n_dry = d->pool->n; g.pair = pair_arranged[staged[k]];
             g.i16 = d->pool->i16 ? 1 : 0;
             p->stage16 = p->stage16 || d->pool->i16;
+        }
+        if (const DryStream* w = ws[order[staged[k]]]) {   // (k_stage reads the layout through its DryStream)
+            g.dry = reinterpret_cast<const float* const*>(w); g.n_dry = strm_arranged[staged[k]]->pool->n; g.i16 = 2;
+            p->stage_stream = true;
         }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
         const StageArea sa = stage_area_of(it);
@@ -2829,8 +2925,11 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     if (n_draws > 0) {
         std::vector<DrawDesc> g(n_draws);
         for (int k = 0; k < n_draws; ++k) {
-            g[k] = draw_describe(caller_items, n_items, draws[k], dry);
-            for (int j = 0; j < g[k].S; ++j) p->draw16 = p->draw16 || g[k].r[g[k].spk[j]].dry16;
+            g[k] = draw_describe(caller_items, n_items, draws[k], dry, ws.data());
+            for (int j = 0; j < g[k].S; ++j) {
+                p->draw16 = p->draw16 || g[k].r[g[k].spk[j]].dry16;
+                p->draw_stream = p->draw_stream || g[k].r[g[k].spk[j]].dry16 == 2;
+            }
         }
         CK(cudaMemcpy(p->d_desc + draw_off, g.data(), sizeof(DrawDesc) * n_draws, cudaMemcpyHostToDevice));
         p->d_draw = (const DrawDesc*)(p->d_desc + draw_off);
@@ -2863,7 +2962,7 @@ static bool written_ranges_disjoint(std::vector<ByteRange>& r) {
 
 // A plan's start draws (include/sonicsim_b200.h, ss_plan_draw), all but the byte ranges (validate_mixes)
 static int validate_draws(const ss_source* items, int n_items, const ss_plan_draw* draws, int n_draws,
-                          const ss_dry_pick* const* dry) {
+                          const ss_dry_pick* const* dry, const ss_dry_stream* const* strm) {
     if (n_draws > kMaxDraws) return SS_ERR_UNSUPPORTED;
     for (int k = 0; k < n_draws; ++k) {
         const ss_plan_draw& d = draws[k];
@@ -2878,7 +2977,8 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
             const ss_source& it = items[i];
             // level tables to test: the dry pool's for a dry-picked speaker, else the pool's
             if (!it.pool || it.win_start_dev != d.start) return SS_ERR_INVALID;
-            if (dry[i] ? !dry[i]->pool->levels : !it.pool->levels) return SS_ERR_INVALID;
+            if (strm[i] ? !strm[i]->pool->levels : dry[i] ? !dry[i]->pool->levels : !it.pool->levels)
+                return SS_ERR_INVALID;
         }
         int readers = 0, len = -1;
         for (int i = 0; i < n_items; ++i) {
@@ -2897,7 +2997,7 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
 // needs a direct-path stem)
 static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                           const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks,
-                          float* const* dir_out) {
+                          float* const* dir_out, const ss_dry_stream* streams, int n_streams) {
     if (n_mixes > 65535) return SS_ERR_UNSUPPORTED;         // one gridDim.y row per mixture
     std::vector<ByteRange> r;
     // a draw writes its start (which only its readers read) and `used`, and reads its u
@@ -2969,6 +3069,10 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
         if (!dp->padded())
             for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
+    for (int k = 0; k < n_streams; ++k) {                   // a stream slot reads its layout
+        add_range(r, streams[k].ids_dev, 4 * (uint64_t)streams[k].m, false);
+        add_range(r, streams[k].offsets_dev, 4 * (uint64_t)streams[k].m, false);
+    }
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
 
@@ -2997,6 +3101,28 @@ static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_ite
     return SS_OK;
 }
 
+// A plan's dry streams (include/sonicsim_b200.h, ss_dry_stream), all but the draws' tables (validate_draws) and the
+// byte ranges (validate_mixes): strm[i] receives item i's stream, or null
+static int validate_streams(const ss_ctx* c, const ss_source* items, int n_items, const ss_dry_stream* streams,
+                            int n_streams, const ss_dry_pick* const* dry, std::vector<const ss_dry_stream*>& strm) {
+    strm.assign(n_items, nullptr);
+    for (int k = 0; k < n_streams; ++k) {
+        const ss_dry_stream& w = streams[k];
+        if (w.slot < 0 || w.slot >= n_items || strm[w.slot] || dry[w.slot]) return SS_ERR_INVALID;
+        const ss_pool* pl = items[w.slot].pool;
+        // a pooled slot of a pool without loudness gains (a stream has no fixed pair to measure), over a 16-bit dry
+        // pool of this context, with a layout of 1..kStreamEntries aligned device entries
+        if (!pl || pl->gains || !w.pool || w.pool->c != c || !w.pool->i16) return SS_ERR_INVALID;
+        if (w.m < 1 || w.m > kStreamEntries || !w.ids_dev || !w.offsets_dev || ((uintptr_t)w.ids_dev & 3) ||
+            ((uintptr_t)w.offsets_dev & 3))
+            return SS_ERR_INVALID;
+        strm[w.slot] = &w;
+    }
+    for (int k = 0; k < n_streams; ++k)                     // (beyond 2^23 samples a crop's sum need not be exact)
+        for (const PoolEntry& e : items[streams[k].slot].pool->host) if (e.N > (1 << 23)) return SS_ERR_UNSUPPORTED;
+    return SS_OK;
+}
+
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
 // and the byte ranges (validate_mixes): dir_out[k] receives mixture k's direct_out, or null
 static int validate_targets(int n_mixes, const ss_plan_target* targets, int n_targets, std::vector<float*>& dir_out) {
@@ -3012,7 +3138,7 @@ static int validate_targets(int n_mixes, const ss_plan_target* targets, int n_ta
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
-                       int n_targets, ss_plan** out) {
+                       int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
@@ -3020,11 +3146,14 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     std::vector<const ss_dry_pick*> dry;
     std::vector<const float*> pair;
     std::vector<float*> dir_out;
+    std::vector<const ss_dry_stream*> strm;
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
     { int st = validate_dry_picks(c, items, n_items, picks, pair_gains, n_picks, dry, pair); if (st) return st; }
-    { int st = validate_draws(items, n_items, draws, n_draws, dry.data()); if (st) return st; }
+    { int st = validate_streams(c, items, n_items, streams, n_streams, dry.data(), strm); if (st) return st; }
+    { int st = validate_draws(items, n_items, draws, n_draws, dry.data(), strm.data()); if (st) return st; }
     { int st = validate_targets(n_mixes, targets, n_targets, dir_out); if (st) return st; }
-    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks, dir_out.data());
+    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks, dir_out.data(), streams,
+                              n_streams);
       if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
@@ -3036,7 +3165,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
     const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data(), pair.data(),
-                              dir_out.data());
+                              dir_out.data(), strm.data());
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -3044,19 +3173,20 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 }
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
-    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws)) return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
+                       out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3065,7 +3195,8 @@ extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_item
     if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
         (n_picks > 0 && !picks))
         return SS_ERR_INVALID;
-    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
+                       0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3076,7 +3207,19 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
         (n_picks > 0 && !picks) || n_targets < 0 || (n_targets > 0 && !targets))
         return SS_ERR_INVALID;
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       out);
+                       nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                     int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                     const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                     int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
+    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
+        (n_picks > 0 && !picks) || n_targets < 0 || (n_targets > 0 && !targets) || n_streams < 0 ||
+        (n_streams > 0 && !streams))
+        return SS_ERR_INVALID;
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3086,8 +3229,9 @@ extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
-static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, cudaStream_t stream) {
-    if (i16) k_draw<true><<<(n + 3) / 4, 128, 0, stream>>>(d, n);
+static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, bool streams, cudaStream_t stream) {
+    if (streams) k_draw<true, true><<<(n + 3) / 4, 128, 0, stream>>>(d, n);
+    else if (i16) k_draw<true><<<(n + 3) / 4, 128, 0, stream>>>(d, n);
     else k_draw<false><<<(n + 3) / 4, 128, 0, stream>>>(d, n);
     CK(cudaGetLastError());
     c->launches += 1;
@@ -3098,10 +3242,15 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, cudaStrea
 // chunk's outputs) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
-    if (p->n_draw) { const int st = draw_enqueue(c, p->d_draw, p->n_draw, p->draw16, stream); if (st) return st; }
+    if (p->n_draw) {
+        const int st = draw_enqueue(c, p->d_draw, p->n_draw, p->draw16, p->draw_stream, stream);
+        if (st) return st;
+    }
     if (p->n_stage) {                                   // staged slots: after the draws, before any chunk reads a slot
         const dim3 grid(kStageCtas, p->n_stage);
-        if (p->n_tap && p->stage16) k_stage<true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
+        if (p->n_tap && p->stage_stream) k_stage<true, true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
+        else if (p->stage_stream) k_stage<true, false, true><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);
+        else if (p->n_tap && p->stage16) k_stage<true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
         else if (p->n_tap) k_stage<false, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
         else if (p->stage16) k_stage<true><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);
         else k_stage<false><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);

@@ -503,6 +503,94 @@ SS_HD const int16_t* speaker_signal_i16(const double* const* dry_levels, const i
     bool bad;
     return reinterpret_cast<const int16_t* const*>(dry_levels - n_dry)[clamp_pick(*dry_pick, n_dry, bad)];
 }
+// ---- dry streams (ss_dry_stream, include/sonicsim_b200.h): a stream slot's dry signal is laid out at every run from
+// m (ids, offsets) entries over a 16-bit dry pool of n utterances.  The walk: an entry with id < 0 is empty and
+// skipped; one with id >= n, offset < 0 or offset < end (the end of the last kept entry, 0 at first) is invalid,
+// skipped and reported (bit 5); any other is kept: utterance id of len samples occupies [offset, offset + len) of the
+// stream and end becomes offset + len.  Zeros lie wherever no kept entry does.  k_stage, k_draw and the CPU emulation
+// decide validity through this one walk.
+constexpr int kStreamEntries = 128;                    // the most entries of a layout
+constexpr unsigned kStreamBit = 32u;                   // bit 5 of ss_device_errors: an invalid entry was skipped
+// Walks entries [0, m): len_of(j, id) gives the length of entry j's utterance (id valid), kept(j, id, offset, len)
+// sees each kept entry in order and returns false to end the walk there.  Returns kStreamBit if an invalid entry was
+// met.
+template <class Len, class Kept>
+SS_HD unsigned stream_entries(const int* ids, const int* offsets, int m, int n, Len len_of, Kept kept) {
+    unsigned err = 0;
+    long long end = 0;
+    for (int j = 0; j < m; ++j) {
+        const int id = ids[j];
+        if (id < 0) continue;
+        const int o = offsets[j];
+        if (id >= n || o < 0 || o < end) { err = kStreamBit; continue; }
+        const int len = len_of(j, id);
+        end = (long long)o + len;
+        if (!kept(j, id, o, len)) break;
+    }
+    return err;
+}
+// A stream slot's descriptor in its plan's block (the plan's copy of its dry pool's utterance lengths, the pool's
+// signal and sparse-table pointers - ss_dry_pool::ptrs); cut is the slot pool's longest N, the length of the stream a
+// DryPick of the same layout would pick from a 16-bit pool.
+struct DryStream {
+    const int* ids;
+    const int* offsets;
+    const int* lengths;
+    const int16_t* const* sig;
+    const double* const* levels;                       // null without level tables
+    int m, n, cut, pad;
+};
+static_assert(sizeof(DryStream) == 56, "DryStream layout");
+// The kept entries of a layout cut at `cut`, for per-sample lookups (stream_sample): a[k] <= n < b[k] is covered by
+// utterance p[k] at sample n - a[k], k ascending in a.  len[j] is entry j's utterance length (read where its id is
+// valid) and sig[j] its signal.  *count receives the number of entries; returns stream_entries' error bits.
+SS_HD unsigned stream_resolve(const int* ids, const int* offsets, const int* len, const int16_t* const* sig, int m,
+                              int n, int cut, int* a, int* b, const int16_t** p, int* count) {
+    int k = 0;
+    const unsigned err = stream_entries(ids, offsets, m, n, [&](int j, int) { return len[j]; },
+                                        [&](int j, int, int o, int l) {
+                                            if (o < cut) {       // (an entry at or past the cut adds no sample)
+                                                const long long e = (long long)o + l;
+                                                a[k] = o; b[k] = e < cut ? (int)e : cut; p[k] = sig[j];
+                                                ++k;
+                                            }
+                                            return true;
+                                        });
+    *count = k;
+    return err;
+}
+// Sample n of a resolved stream (stream_resolve: k entries), as k_stage stores it: the covering utterance's sample
+// (i16_sample), or 0
+SS_HD float stream_sample(const int* a, const int* b, const int16_t* const* p, int k, int n) {
+    int lo = 0, hi = k;                                 // the first entry starting after n
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a[mid] <= n) lo = mid + 1; else hi = mid;
+    }
+    return lo > 0 && n < b[lo - 1] ? i16_sample(p[lo - 1][n - a[lo - 1]]) : 0.0f;
+}
+// The energy of the crop [s, s + len) of a stream (s + len at most the stream's cut): over the kept entries that meet
+// it, the utterance-local differences of sparse_level.  Every term is a multiple of 2^-30 and the sum stays below 2^23
+// (the crop's squares are at most 1 each), so the sum is exact in float64 in any order: Q[s + len] - Q[s] of the
+// assembled stream's full table, bit for bit.
+SS_HD double stream_level(const DryStream& d, int s, int len) {
+    double q = 0.0;
+    const long long lo = s, hi = (long long)s + len;
+    stream_entries(d.ids, d.offsets, d.m, d.n, [&](int, int id) { return d.lengths[id]; },
+                   [&](int, int id, int o, int l) {
+                       if (o >= hi) return false;       // (later entries start later still)
+                       const long long b0 = lo > o ? lo - o : 0, b1 = hi - o < l ? hi - o : l;
+                       if (b1 > b0)
+                           q += sparse_level(d.levels[id], d.sig[id], (int)b1) -
+                                sparse_level(d.levels[id], d.sig[id], (int)b0);
+                       return true;
+                   });
+    return q;
+}
+// draw_silent of a stream speaker (D = len)
+SS_HD bool draw_silent_stream(const DryStream& d, int s, int len, float threshold_db) {
+    return draw_silent_sums(0.0, stream_level(d, s, len), (double)len, threshold_db);
+}
 
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }

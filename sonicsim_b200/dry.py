@@ -116,6 +116,85 @@ def _place_background_audio(lens: T.List[int], total: int, length: float, sample
     return places, spans, used
 
 
+def long_audio_max_selected(lengths, total: int) -> int:
+    """The most utterances of `lengths` that get_random_wav_path's selection can take for a stream of `total` samples:
+    the largest k whose k shortest utterances fit in `total` (at least 1).  A host computation, once per corpus, for
+    long_audio_layouts(..., max_selected=)."""
+    import numpy as np
+    v = np.sort(np.asarray(lengths.cpu() if hasattr(lengths, "cpu") else lengths, dtype=np.int64).reshape(-1))
+    return max(1, int(np.searchsorted(np.cumsum(v), int(total), side="right")))
+
+
+def _long_audio_selection(lengths, total: int, count: int, width: int, kw):
+    """get_random_wav_path's selection, `count` times: (sel, chosen), both (count, width).  sel[r] is the first width
+    utterances of a uniform random order, chosen[r] marks its selected prefix (taken while the running total is below
+    0.9 * total, up to the first that would overflow `total`)."""
+    import torch
+    keys = torch.rand((count, lengths.numel()), **kw)
+    if width < lengths.numel():                       # the first `width` of the random order
+        sel = torch.topk(keys, width, dim=1, largest=False, sorted=True).indices
+    else:
+        sel = torch.argsort(keys, dim=1)
+    del keys
+    ls = lengths[sel]
+    cs = torch.cumsum(ls, dim=1)
+    take = ((cs - ls).double() < 0.9 * total) & (cs <= total)
+    return sel, torch.cumprod(take.to(torch.int8), dim=1).bool()
+
+
+def long_audio_layouts(lengths, total: int, m: int, count: int, generator=None, sample_rate: int = 16000,
+                       max_selected: T.Optional[int] = None):
+    """`count` layouts of create_long_audio streams (:231-277) over utterances of `lengths` (a 1-D integer tensor of n
+    lengths in samples, already at `sample_rate`), for render.DryStream: (ids, offsets), two int32 tensors of shape
+    (count, m) on `lengths`' device.  Torch ops only, so a training step refreshes them on the GPU without a host
+    synchronisation; `generator` (of that device) makes them reproducible.
+
+    Each row draws the arrangement create_long_audio would build for a stream of `total` samples:
+      - selection, get_random_wav_path's rule: utterances in a uniform random order without replacement, taken while
+        the running total is below 0.9 * total, stopping at the first one that would overflow `total`;
+      - placement, _place_long_audio's rule: the selected utterances in an independent uniform random order, each
+        preceded by a gap uniform in {0, ..., 10 * sample_rate}, placed while the stream's cursor stays within `total`.
+    The placement order is drawn afresh rather than reusing the selection order: given the selected set, the selection
+    order is not uniform (the stop rule reads its prefix sums), and the reference's placement order is.  The layouts
+    match the reference in distribution, not in its `random`-stream draws.  Unused entries are -1 (empty).  A row that
+    would place more than m utterances keeps its first m (in stream order), so choose m above total / (shortest
+    utterance + 10 * sample_rate / 2) with some margin when that matters.
+
+    Cost: the selection draws one float32 key per (row, utterance).  Without `max_selected` it sorts all n keys of
+    every row, and its temporaries peak at about 42 bytes per (row, utterance): 1.5 GB and 7.6 ms on an H100 for
+    count = 128 rows over a LibriSpeech-sized n = 2.8e5 (DESIGN section 6).  `max_selected`
+    (long_audio_max_selected(lengths, total), computed once per corpus) bounds how many utterances a row can select;
+    the call then keeps only the max_selected smallest keys of each row (torch.topk) and works on (count,
+    max_selected) and (count, m) tensors behind the (count, n) keys, with the same distribution: 145 MB (the keys)
+    and 1.1 ms there.  A bound below long_audio_max_selected's cuts rows short and changes the distribution."""
+    import torch
+    lengths = lengths.reshape(-1).to(torch.int64)
+    n, dev = lengths.numel(), lengths.device
+    if n < 1 or not 1 <= m <= 128 or count < 1 or (max_selected is not None and max_selected < 1):
+        raise ValueError("long_audio_layouts: need n >= 1 utterances, 1 <= m <= 128, count >= 1 and max_selected "
+                         ">= 1, got n = %d, m = %d, count = %d, max_selected = %r" % (n, m, count, max_selected))
+    kw = {"generator": generator, "device": dev}
+    width = n if max_selected is None else min(n, int(max_selected))
+    sel, chosen = _long_audio_selection(lengths, total, count, width, kw)
+    # placement: the first m of the chosen ones in a fresh random order, each behind a gap, while the cursor stays
+    # within `total` (a row keeps at most m, and what it keeps is a prefix of that order)
+    w = min(width, m)
+    key = torch.rand((count, width), **kw).masked_fill(~chosen, 2.0)
+    order = torch.topk(key, w, dim=1, largest=False, sorted=True).indices
+    ids = sel.gather(1, order)
+    valid = chosen.gather(1, order)
+    lp = lengths[ids]
+    gaps = torch.randint(0, int(10 * sample_rate) + 1, (count, w), **kw)
+    cur = torch.cumsum((gaps + lp) * valid, dim=1)
+    placed = torch.cumprod((valid & (cur <= total)).to(torch.int8), dim=1).bool()
+    offsets = cur - lp
+    out_ids = torch.full((count, m), -1, dtype=torch.int32, device=dev)
+    out_off = torch.full((count, m), -1, dtype=torch.int32, device=dev)
+    out_ids[:, :w] = torch.where(placed, ids, -1).to(torch.int32)
+    out_off[:, :w] = torch.where(placed, offsets, -1).to(torch.int32)
+    return out_ids, out_off
+
+
 _kernel_cache: T.Dict[T.Tuple[int, int, str], T.Tuple] = {}
 
 

@@ -85,7 +85,7 @@ class Pooled(T.NamedTuple):
     needs every candidate's bank to hold a direct set with these taps.  A pick outside [0, n) is clamped into range and a
     start beyond the picked candidate's N - length is clamped too (check_device_errors).  Only plan_device takes it.
     `dry`, a DryPick, makes it a dry-picked slot: the picked candidate renders with the dry signal the DryPick names in
-    place of its own."""
+    place of its own; a DryStream makes it a stream slot, whose dry signal is laid out from utterances at every run."""
     pool: T.Any
     pick: T.Any
     window: T.Tuple[T.Any, int]
@@ -107,6 +107,22 @@ class DryPick(T.NamedTuple):
     pool: T.Any
     pick: T.Any
     gains: T.Any = None
+
+
+class DryStream(T.NamedTuple):
+    """The dry signal of a pooled slot (Pooled.dry) laid out at every run from utterances, as create_long_audio lays
+    out a speech stream (SonicSim_audio.py:231-277): `pool` a 16-bit DryPool of n utterances (dry_pool(...,
+    dtype="int16")), `ids` and `offsets` contiguous 1-D CUDA int32 tensors of equal length m, 1 <= m <= 128 (e.g. rows
+    of (B, S, m) tensors from dry.long_audio_layouts), read on the device at every run.  The layout is walked in order:
+    an entry with id < 0 is empty and skipped; one with id >= n, offset < 0 or offset before the end of the last kept
+    entry is invalid and skipped (check_device_errors raises ValueError); any other places utterance `id` at samples
+    [offset, offset + its length) of the stream.  The slot renders its picked candidate with the stream's first N
+    samples, zeros where no utterance lies (an utterance reaching past N is cut there): bit for bit a DryPick from a
+    16-bit pool holding the assembled stream.  A stream speaker of a CropDraw is tested on its crop's energy, summed per
+    utterance from the pool's level tables (dry_pool(..., levels=True)).  Pools with loudness gains take no streams."""
+    pool: T.Any
+    ids: T.Any
+    offsets: T.Any
 
 
 class CropDraw(T.NamedTuple):
@@ -562,8 +578,10 @@ def _hold_banks(plan, sources):
     releases them at once, once)."""
     banks = []
     for s in sources:
-        dry = s.dry if isinstance(s, Pooled) and isinstance(s.dry, DryPick) else None
-        held = [s.pool] + ([dry.pool, dry.gains] if dry else []) if isinstance(s, Pooled) else [_rirs(s)[0]]
+        # a dry-picked slot's dry pool and pair gains, a stream slot's utterance pool
+        dry = s.dry if isinstance(s, Pooled) and isinstance(s.dry, (DryPick, DryStream)) else None
+        held = ([s.pool] + ([dry.pool, getattr(dry, "gains", None)] if dry else []) if isinstance(s, Pooled)
+                else [_rirs(s)[0]])
         for b in held:
             if isinstance(b, (RirBank, SourcePool, DryPool, PairGains)) and all(b is not o for o in banks):
                 banks.append(b)
@@ -994,14 +1012,17 @@ class Renderer:
 
         A Pooled slot with `dry` = DryPick(dry_pool, pick) also takes its dry signal from a DryPool at every run, so
         that every (dry signal, trajectory) pair is reachable in the same single graph launch
-        (dry_picks.random_(0, n) before the run)."""
+        (dry_picks.random_(0, n) before the run).  With `dry` = DryStream(utterance_pool, ids, offsets) the slot's dry
+        stream is laid out from a 16-bit utterance pool at every run (ss_plan_create_stream): a fresh arrangement of
+        utterances and gaps per step (dry.long_audio_layouts into the ids and offsets before the run)."""
         dry = self._device_dry(sources)
+        streams = self._device_streams(sources)
         items, n, keep = self._device_items(sources, outs, direct_outs)
         targets = []
         mixes = self._device_mixes(mixtures, outs, keep, items, targets) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
-                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None)
+                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1013,10 +1034,10 @@ class Renderer:
                 if isinstance(d, DryPick):
                     raise ValueError("plan_device: source %d has a DryPick but is not a pooled slot (render.Pooled)" % i)
                 continue
-            if d is None:
+            if d is None or isinstance(d, DryStream):
                 continue
             if not isinstance(d, DryPick):
-                raise ValueError("plan_device: the dry of pooled source %d must be a DryPick or None" % i)
+                raise ValueError("plan_device: the dry of pooled source %d must be a DryPick or None, or a DryStream" % i)
             if not isinstance(d.pool, DryPool):
                 raise ValueError("plan_device: the dry pool of source %d must be a DryPool" % i)
             _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
@@ -1043,6 +1064,37 @@ class Renderer:
             pick = _tensor(d.pick, "plan_device", "source %d" % i, "dry pick", torch.int32, self.device, count=(1, 1))
             picks.append(_lib.SsDryPick(slot=i, pool=d.pool._h.value, pick_dev=pick))
         return (_lib.SsDryPick * len(picks))(*picks) if picks else None
+
+    def _device_streams(self, sources):
+        """Validated ss_dry_stream array of a plan's stream slots, or None without any."""
+        import torch
+        streams = []
+        for i, s in enumerate(sources):
+            d = getattr(s, "dry", None)
+            if not isinstance(d, DryStream):
+                continue
+            if not isinstance(s, Pooled):
+                raise ValueError("plan_device: source %d has a DryStream but is not a pooled slot (render.Pooled)" % i)
+            if not isinstance(d.pool, DryPool):
+                raise ValueError("plan_device: the utterance pool of source %d must be a DryPool" % i)
+            _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
+            if d.pool.dtype != "int16":
+                raise ValueError("plan_device: the DryStream of source %d needs a 16-bit DryPool (dry_pool(..., "
+                                 "dtype=\"int16\")): a float32 pool's crop energies are not exact" % i)
+            pl = s.pool
+            if isinstance(pl, SourcePool):
+                if pl.gains:
+                    raise ValueError("plan_device: pooled source %d has a DryStream over a pool with loudness gains: a "
+                                     "stream has no fixed (dry signal, trajectory) pair to measure" % i)
+                if max(pl._sizes) > 1 << 23:
+                    raise ValueError("plan_device: pooled source %d has a DryStream over a pool whose longest "
+                                     "candidate (N = %d) exceeds 2^23 samples" % (i, max(pl._sizes)))
+            own = "source %d" % i
+            m = d.ids.numel() if isinstance(d.ids, torch.Tensor) else 0
+            ids = _tensor(d.ids, "plan_device", own, "stream ids", torch.int32, self.device, ("m",), (1, 128))
+            off = _tensor(d.offsets, "plan_device", own, "stream offsets", torch.int32, self.device, (m,))
+            streams.append(_lib.SsDryStream(slot=i, pool=d.pool._h.value, ids_dev=ids, offsets_dev=off, m=m))
+        return (_lib.SsDryStream * len(streams))(*streams) if streams else None
 
     @staticmethod
     def _device_pair_gains(sources):
@@ -1095,7 +1147,7 @@ class Renderer:
                     raise ValueError("plan_device: speaker %d of draw %d does not take its window start from the "
                                      "draw's start tensor" % (v, k))
                 dry = sources[v].dry
-                if isinstance(dry, DryPick):
+                if isinstance(dry, (DryPick, DryStream)):
                     if not dry.pool.levels:
                         raise ValueError("plan_device: speaker %d of draw %d: its DryPool has no level tables "
                                          "(dry_pool(levels=True))" % (v, k))
@@ -1242,6 +1294,9 @@ class Renderer:
         if bits.value & 4:
             raise ValueError("a window start on the device was outside [0, N - length]; the window was clamped into "
                              "that range")
+        if bits.value & 32:
+            raise ValueError("a DryStream layout on the device held an invalid entry (an id >= n, a negative offset or "
+                             "an offset before the end of the previous utterance); it was skipped")
 
     def launch_count(self) -> int:
         return int(self.lib.ss_launch_count(self.ctx))
@@ -1267,16 +1322,21 @@ class DevicePlan:
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
     dry-picked slots take their dry signals from dry pools (ss_plan_create_dry), with pair gains their gains from
-    pair-gain tables (ss_plan_create_pair), and with dereverberation targets its mixtures also write those
-    (ss_plan_create_target)."""
+    pair-gain tables (ss_plan_create_pair), with dereverberation targets its mixtures also write those
+    (ss_plan_create_target), and with stream slots it lays out their dry streams (ss_plan_create_stream)."""
 
-    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None):
+    def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
+                 streams=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
-        self.draws, self.dry, self.pair_gains, self.targets = draws, dry, pair_gains, targets
+        self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
         self._plan = ctypes.c_void_p()
         if n > 0:
             args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry)
-            if targets is not None:
+            if streams is not None:
+                st = renderer.lib.ss_plan_create_stream(*args, pair_gains, len(dry) if dry else 0, targets,
+                                                        len(targets) if targets else 0, streams, len(streams),
+                                                        ctypes.byref(self._plan))
+            elif targets is not None:
                 st = renderer.lib.ss_plan_create_target(*args, pair_gains, len(dry) if dry else 0, targets,
                                                         len(targets), ctypes.byref(self._plan))
             elif pair_gains is None:
