@@ -1184,11 +1184,21 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
     }
     return bytes;
 }
+// What a plan knows of one of its items besides the ss_source: its dry pick, pair gains and dry stream
+// (validate_dry_picks, validate_streams) and, once plan_build has laid out the plan's descriptors, the device addresses
+// of its staging area's view (a staged slot) and of its DryStream (a stream slot)
+struct PlanSlot {
+    const ss_dry_pick* dry = nullptr;
+    const float* pair = nullptr;       // the device table of its pair gains, or null
+    const ss_dry_stream* strm = nullptr;
+    StageView* view = nullptr;
+    const DryStream* ws = nullptr;
+};
 // Fill the descriptor block of items[first, last) at `hbase` (host memory) for its device address `dbase`, carve the
-// chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.
+// chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.  A plan's
+// chunk passes `slots`: slots[first + i] is the record of items[first + i].
 static void chunk_describe(const ss_source* items, const Shape* shapes, int first, int last, char* hbase, char* dbase,
-                           char* scratch, int sm_count, ChunkLaunch* L, StageView* const* views = nullptr,
-                           const ss_dry_pick* const* dry = nullptr, const float* const* pair = nullptr) {
+                           char* scratch, int sm_count, ChunkLaunch* L, const PlanSlot* const* slots = nullptr) {
     const int n = last - first;
     const bool host_tables = chunk_host_tables(items, first, last);
     const size_t off_ps = align_up(sizeof(Source) * n, 16);
@@ -1203,6 +1213,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
     for (int i = 0; i < n; ++i) {
         const ss_source& it = items[first + i];
         const Shape& sh = shapes[first + i];
+        const PlanSlot* const rec = slots ? slots[first + i] : nullptr;
         Source s;
         memset(&s, 0, sizeof(s));
         s.x = it.x; s.rir = it.rir; s.out = it.out;
@@ -1218,7 +1229,7 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
             s.K = it.pool->parts_host[0];
             pick_candidate(s, it.pool->host[0]);
             any_pooled = true;
-            L->any_gain = L->any_gain || it.pool->gains || (pair && pair[first + i]);
+            L->any_gain = L->any_gain || it.pool->gains || (rec && rec->pair);
         } else if (it.rir_bank) {
             // spectra (and cuts) from the bank: no RIR rows, no cut table, no k_rir_absmax / k_rir_direct work
             set_banked(s, it.rir_bank->spec, (it.flags & SS_DIRECT_TARGET) ? it.rir_bank->cut : nullptr, sh.win != 0);
@@ -1265,13 +1276,15 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                     memcpy(hb_counts + 12, &it.pick_dev, sizeof(it.pick_dev));
                     memcpy(hb_counts + 14, &it.pool->gains, sizeof(it.pool->gains));
                     memcpy(hb_counts + 16, &it.pool->parts, sizeof(it.pool->parts));
-                    if (views) memcpy(hb_counts + 18, &views[first + i], sizeof(StageView*));   // stage_view
-                    if (dry && dry[first + i]) {            // dry_table, dry_pick_ptr, dry_size, pair_table
-                        const ss_dry_pick& d = *dry[first + i];
+                    if (rec) memcpy(hb_counts + 18, &rec->view, sizeof(rec->view));            // stage_view
+                    // dry_table, dry_pick_ptr, dry_size, pair_table of the dry picks k_blocks makes (pick_pooled): a
+                    // staged slot's is k_stage's, and its counts hold none (take_view)
+                    if (rec && rec->dry && !rec->view) {
+                        const ss_dry_pick& d = *rec->dry;
                         memcpy(hb_counts + 20, &d.pool->ptrs, sizeof(d.pool->ptrs));
                         memcpy(hb_counts + 22, &d.pick_dev, sizeof(d.pick_dev));
                         hb_counts[24] = d.pool->n;
-                        if (pair) memcpy(hb_counts + 26, &pair[first + i], sizeof(pair[first + i]));
+                        memcpy(hb_counts + 26, &rec->pair, sizeof(rec->pair));
                     }
                 }
             } else {
@@ -2704,9 +2717,12 @@ extern "C" void ss_plan_destroy(ss_plan* p) {
     delete p;
 }
 
+// A plan's mixture with its dereverberation targets (ss_plan_target's direct_out), or null
+struct PlanMix : ss_plan_mix { float* dir_out; };
+
 // The descriptor of mixture m of a plan: rows of the callers' `items` outputs (before arrange_chunks regroups them);
 // with dir_out, its speakers' direct-path stems and the (S, E) targets
-static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double* scratch, float* dir_out) {
+static MixItem mix_describe(const ss_source* items, const PlanMix& m, double* scratch) {
     MixItem d; memset(&d, 0, sizeof(d));
     const ss_source& a = items[m.speakers[0]];
     const int64_t T = a.win_len > 0 ? a.win_len : a.N;
@@ -2716,21 +2732,19 @@ static MixItem mix_describe(const ss_source* items, const ss_plan_mix& m, double
     d.sirs = m.sirs; d.snr = m.snr; d.mix = m.mix; d.spk_out = m.speakers_out; d.rms_out = m.rms_db; d.scratch = scratch;
     d.E = mono ? T : (int64_t)a.C * T; d.T = T; d.Cf = mono ? a.C : 1;
     d.S = m.S; d.M = m.M; d.delay = m.noise_delay;
-    if (dir_out) {
+    if (m.dir_out) {
         for (int s = 0; s < m.S; ++s) d.dir[s] = items[m.speakers[s]].out_direct;
-        d.dir_out = dir_out;
+        d.dir_out = m.dir_out;
     }
     return d;
 }
 
-// The descriptor of draw d of a plan: its readers in the callers' order of `items`
-// (dry[i]: item i's dry pick, or null; a dry-picked speaker tests its dry pool's one-channel tables, D = len; ws[i]:
-// the device address of item i's DryStream, or null: a stream speaker walks its layout, D = len)
-static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan_draw& d, const ss_dry_pick* const* dry,
-                              const DryStream* const* ws) {
+// The descriptor of draw d of a plan: its readers in the callers' order of `items` (a dry-picked speaker tests its dry
+// pool's one-channel tables, D = len; a stream speaker walks its layout through its DryStream, D = len)
+static DrawDesc draw_describe(const ss_source* items, const std::vector<PlanSlot>& slots, const ss_plan_draw& d) {
     DrawDesc g; memset(&g, 0, sizeof(g));
     g.start = d.start; g.u = d.u; g.used = d.used; g.tries = d.tries; g.S = d.S; g.threshold_db = d.threshold_db;
-    for (int i = 0; i < n_items; ++i) {
+    for (int i = 0; i < (int)slots.size(); ++i) {
         const ss_source& it = items[i];
         if (it.win_start_dev != d.start) continue;
         for (int k = 0; k < d.S; ++k) if (d.speakers[k] == i) g.spk[k] = g.n_readers;
@@ -2738,11 +2752,11 @@ static DrawDesc draw_describe(const ss_source* items, int n_items, const ss_plan
         g.len = it.win_len;
         DrawReader r = {pl->table, it.pick_dev, pl->level_ptr, pl->n,
                         (double)it.win_len * ((pl->level_flags & SS_MIX_MONO) ? 1 : pl->C), nullptr, nullptr, 0};
-        if (dry[i]) {
-            r.dry_levels = dry[i]->pool->level_ptr; r.dry_pick = dry[i]->pick_dev; r.n_dry = dry[i]->pool->n; r.D = it.win_len;
-            r.dry16 = dry[i]->pool->i16 ? 1 : 0;
+        if (const ss_dry_pick* p = slots[i].dry) {
+            r.dry_levels = p->pool->level_ptr; r.dry_pick = p->pick_dev; r.n_dry = p->pool->n; r.D = it.win_len;
+            r.dry16 = p->pool->i16 ? 1 : 0;
         }
-        if (ws[i]) { r.dry_pick = reinterpret_cast<const int*>(ws[i]); r.dry16 = 2; r.D = it.win_len; }
+        if (slots[i].ws) { r.dry_pick = reinterpret_cast<const int*>(slots[i].ws); r.dry16 = 2; r.D = it.win_len; }
         g.r[g.n_readers++] = r;
     }
     return g;
@@ -2771,174 +2785,145 @@ static StageArea stage_area_of(const ss_source& it) {
     return stage_area(stage_sets(it), cap.first, cap.second, it.pool->taps);
 }
 
-// (dry[i]: caller item i's dry pick, or null; pair[i]: its pair gains' device table, or null; dir_out[k]: mixture k's
-// dereverberation targets, or null; strm[i]: caller item i's dry stream, or null)
-static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes, int n_items,
-                      const ss_plan_mix* mixes, int n_mixes, const ss_plan_draw* draws, int n_draws,
-                      const ss_dry_pick* const* dry, const float* const* pair, float* const* dir_out,
-                      const ss_dry_stream* const* strm) {
+// Lay out, fill and upload a plan's descriptors.  The host fills one image, each section at a 256-byte boundary: the
+// chunk descriptors, the mixtures' MixItems, the draws' DrawDescs, the staged slots' StageSlots, the tap block
+// (tap_block, with slots of tap-form pools), the streams' DryStreams (caller order) and the utterance lengths of each
+// dry pool the streams use; one copy uploads it.  Behind the image, written by the device only and never uploaded: one
+// scratch block per mixture, then the staged slots' staging areas.  slots[i] is caller item i's record; plan_build
+// notes where its view and its DryStream landed.
+static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes,
+                      std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix, const ss_plan_draw* draws,
+                      int n_draws) {
     ss_ctx* c = p->c;
+    const int n_items = (int)slots.size();
     std::vector<int> cuts, order;
     std::vector<ss_source> arranged;
     std::vector<Shape> arranged_shapes;
     arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
-    std::vector<const ss_dry_pick*> dry_arranged(arranged.size());
-    std::vector<const float*> pair_arranged(arranged.size());
-    std::vector<const ss_dry_stream*> strm_arranged(arranged.size());
-    for (size_t i = 0; i < arranged.size(); ++i) {
-        dry_arranged[i] = dry[order[i]]; pair_arranged[i] = pair[order[i]]; strm_arranged[i] = strm[order[i]];
-    }
-    std::vector<const ss_dry_pick*> dry_describe(dry_arranged);   // the dry picks k_blocks makes (pick_pooled)
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
+    std::vector<PlanSlot*> rec(arranged.size());         // rec[i]: the record of arranged item i
+    std::vector<int> staged;    // arranged items that are slots of host pools, host or 16-bit dry picks, stream slots
+    int n_tap = 0, n_strm = 0;
+    for (int i = 0; i < (int)arranged.size(); ++i) {
+        rec[i] = &slots[order[i]];
+        const PlanSlot& r = *rec[i];
+        n_strm += r.strm ? 1 : 0;
+        if (items[i].pool && (items[i].pool->host_res || (r.dry && r.dry->pool->padded()) || r.strm)) {
+            staged.push_back(i);
+            n_tap += items[i].pool->taps ? 1 : 0;
+        }
+    }
+    if (staged.size() > 65535) return SS_ERR_UNSUPPORTED;   // one gridDim.y row of k_stage per slot
+    size_t at = 0;
+    auto take = [&at](size_t bytes) { const size_t o = at; at = align_up(at + bytes, 256); return o; };
     const size_t n_chunks = cuts.size() - 1;
-    std::vector<size_t> off(n_chunks + 1, 0);
+    std::vector<size_t> off(n_chunks);
     size_t scratch_need[ss_ctx::kAux] = {};
     for (size_t k = 0; k < n_chunks; ++k) {
-        off[k + 1] = off[k] + align_up(chunk_desc_bytes(items, shapes, cuts[k], cuts[k + 1]), 256);
+        off[k] = take(chunk_desc_bytes(items, shapes, cuts[k], cuts[k + 1]));
         const size_t sb = chunk_scratch_bytes(items, shapes, cuts[k], cuts[k + 1]);
         size_t& m = scratch_need[n_chunks < 2 ? 0 : k % ss_ctx::kAux];
         m = sb > m ? sb : m;
     }
+    const size_t mix_off = take(sizeof(MixItem) * mix.size());
+    const size_t draw_off = take(sizeof(DrawDesc) * n_draws);
+    const size_t stage_off = take(sizeof(StageSlot) * staged.size());
+    const TapBlock tb = tap_block(at, (int)staged.size(), n_tap);
+    if (n_tap) at = tb.end;
+    const size_t wdesc_off = take(sizeof(DryStream) * n_strm);
+    std::vector<const ss_dry_pool*> wpools;              // each with its lengths at wlen_off
+    std::vector<size_t> wlen_off;
+    for (const PlanSlot& s : slots)
+        if (s.strm && std::find(wpools.begin(), wpools.end(), s.strm->pool) == wpools.end()) {
+            wpools.push_back(s.strm->pool);
+            wlen_off.push_back(take(sizeof(int32_t) * (size_t)s.strm->pool->n));
+        }
+    const size_t image = at;
+    const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
+    const size_t scr_off = take(scr_bytes * mix.size());
+    std::vector<size_t> area_off(staged.size());
+    for (size_t k = 0; k < staged.size(); ++k) area_off[k] = take(stage_area_of(items[staged[k]]).end);
     CK(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
     for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaEventCreateWithFlags(&p->ev_join[i], cudaEventDisableTiming));
     CK(cudaStreamCreateWithFlags(&p->s_cap, cudaStreamNonBlocking));
-    // behind the chunk descriptors: the mixtures' descriptors, then one mixture scratch block each
-    const size_t mix_off = off[n_chunks], scr_off = mix_off + align_up(sizeof(MixItem) * n_mixes, 256);
-    const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
-    const size_t draw_off = align_up(scr_off + scr_bytes * n_mixes, 256);
-    const size_t desc_bytes = draw_off + sizeof(DrawDesc) * n_draws;
-    // behind the draws: the staged slots' k_stage descriptors, then their staging areas
-    std::vector<int> staged;    // arranged items that are slots of host pools, host or 16-bit dry picks, stream slots
-    for (int i = 0; i < (int)arranged.size(); ++i)
-        if (items[i].pool && (items[i].pool->host_res || (dry_arranged[i] && dry_arranged[i]->pool->padded()) ||
-                              strm_arranged[i])) {
-            staged.push_back(i);
-            dry_describe[i] = nullptr;                  // k_stage stages the dry pick: the counts hold none (take_view)
-        }
-    if (staged.size() > 65535) return SS_ERR_UNSUPPORTED;   // one gridDim.y row of k_stage per slot
-    const size_t stage_off = align_up(desc_bytes, 256), area_off = align_up(stage_off + sizeof(StageSlot) * staged.size(), 256);
-    size_t total = area_off;
-    int n_tap = 0;
-    for (int i : staged) { total += stage_area_of(items[i]).end; n_tap += items[i].pool->taps ? 1 : 0; }
-    const TapBlock tb = tap_block(total, (int)staged.size(), n_tap);   // (slots of tap-form pools)
-    const size_t tap_off = tb.taps, tsrc_off = tb.src, tpre_off = tb.prefix, zero_off = tb.zero;
-    if (n_tap) total = tb.end;
-    const size_t tap_end = total;
-    // behind those: the streams' DryStream descriptors (caller order), then the utterance lengths of each dry pool
-    // they use, uploaded once
-    std::vector<const DryStream*> ws(n_items, nullptr);
-    std::vector<DryStream> wdesc;
-    std::vector<const ss_dry_pool*> wpools;
-    std::vector<size_t> wlen_off;
-    for (int i = 0; i < n_items; ++i) if (strm[i]) wdesc.emplace_back();
-    const size_t wdesc_off = align_up(total, 256);
-    if (!wdesc.empty()) {
-        total = wdesc_off + sizeof(DryStream) * wdesc.size();
-        for (int i = 0; i < n_items; ++i)
-            if (strm[i] && std::find(wpools.begin(), wpools.end(), strm[i]->pool) == wpools.end()) {
-                wpools.push_back(strm[i]->pool);
-                wlen_off.push_back(align_up(total, 256));
-                total = wlen_off.back() + sizeof(int32_t) * (size_t)strm[i]->pool->n;
-            }
-    }
-    CK(cudaMalloc((void**)&p->d_desc, total + 256));
-    std::vector<char> tap_host(n_tap ? tap_end - tap_off : 0, 0);
-    for (int i = 0, k = 0; i < n_items; ++i) {
-        if (!strm[i]) continue;
-        const ss_dry_stream& w = *strm[i];
+    CK(cudaMalloc((void**)&p->d_desc, at + 256));
+    for (int i = 0; i < ss_ctx::kAux; ++i)
+        if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
+    char* const d = p->d_desc;
+    std::vector<char> host(image, 0);
+    for (int i = 0, k = 0; i < n_items; ++i) {           // the streams first: staged slots and draws name them
+        if (!slots[i].strm) continue;
+        const ss_dry_stream& w = *slots[i].strm;
         const ss_dry_pool* dp = w.pool;
         const size_t lo = wlen_off[std::find(wpools.begin(), wpools.end(), dp) - wpools.begin()];
         int cut = 0;
         for (const PoolEntry& e : caller_items[i].pool->host) cut = std::max(cut, e.N);
-        wdesc[k] = {w.ids_dev, w.offsets_dev, (const int*)(p->d_desc + lo), (const int16_t* const*)dp->ptrs,
-                    dp->levels ? dp->level_ptr : nullptr, w.m, dp->n, cut, 0};
-        ws[i] = (const DryStream*)(p->d_desc + wdesc_off) + k;
-        ++k;
+        ((DryStream*)(host.data() + wdesc_off))[k] = {w.ids_dev, w.offsets_dev, (const int*)(d + lo),
+                                                      (const int16_t* const*)dp->ptrs,
+                                                      dp->levels ? dp->level_ptr : nullptr, w.m, dp->n, cut, 0};
+        slots[i].ws = (const DryStream*)(d + wdesc_off) + k++;
     }
-    if (!wdesc.empty()) {
-        CK(cudaMemcpy(p->d_desc + wdesc_off, wdesc.data(), sizeof(DryStream) * wdesc.size(), cudaMemcpyHostToDevice));
-        for (size_t j = 0; j < wpools.size(); ++j)
-            CK(cudaMemcpy(p->d_desc + wlen_off[j], wpools[j]->N.data(), sizeof(int32_t) * (size_t)wpools[j]->n,
-                          cudaMemcpyHostToDevice));
-    }
-    for (int i = 0; i < ss_ctx::kAux; ++i)
-        if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
-    std::vector<char> host(desc_bytes + 256);
-    std::vector<StageView*> views(arranged.size(), nullptr);
-    std::vector<StageSlot> stage(staged.size());
-    for (size_t k = 0, at = area_off; k < staged.size(); ++k) {
+    for (size_t j = 0; j < wpools.size(); ++j)
+        memcpy(host.data() + wlen_off[j], wpools[j]->N.data(), sizeof(int32_t) * (size_t)wpools[j]->n);
+    for (size_t k = 0; k < staged.size(); ++k) {
         const ss_source& it = items[staged[k]];
+        PlanSlot& r = *rec[staged[k]];
         const ss_pool* pl = it.pool;
-        StageSlot& g = stage[k];
-        memset(&g, 0, sizeof(g));
+        StageSlot& g = ((StageSlot*)(host.data() + stage_off))[k];
         g.pool = pl->table; g.pick = it.pick_dev; g.ws_dev = it.win_start_dev; g.parts = pl->parts; g.gains = pl->gains;
         g.n = pl->n; g.C = pl->C; g.K = pl->K; g.ws = it.win_start; g.len = it.win_len; g.sets = stage_sets(it);
-        if (const ss_dry_pick* d = dry_arranged[staged[k]]) {
-            g.dry = d->pool->ptrs; g.dry_pick = d->pick_dev; g.n_dry = d->pool->n; g.pair = pair_arranged[staged[k]];
-            g.i16 = d->pool->i16 ? 1 : 0;
-            p->stage16 = p->stage16 || d->pool->i16;
+        if (const ss_dry_pick* dp = r.dry) {
+            g.dry = dp->pool->ptrs; g.dry_pick = dp->pick_dev; g.n_dry = dp->pool->n; g.pair = r.pair;
+            g.i16 = dp->pool->i16 ? 1 : 0;
+            p->stage16 = p->stage16 || dp->pool->i16;
         }
-        if (const DryStream* w = ws[order[staged[k]]]) {   // (k_stage reads the layout through its DryStream)
-            g.dry = reinterpret_cast<const float* const*>(w); g.n_dry = strm_arranged[staged[k]]->pool->n; g.i16 = 2;
+        if (r.ws) {                                     // (k_stage reads the layout through its DryStream)
+            g.dry = reinterpret_cast<const float* const*>(r.ws); g.n_dry = r.strm->pool->n; g.i16 = 2;
             p->stage_stream = true;
         }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
         const StageArea sa = stage_area_of(it);
-        char* const a = p->d_desc + at;
+        char* const a = d + area_off[k];
         g.view = (StageView*)(a + sa.view);
         g.spec = g.sets ? (float2*)(a + sa.spec) : nullptr;
         g.x = (float*)(a + sa.x);
-        at += sa.end;
-        views[staged[k]] = g.view;
+        r.view = g.view;
         if (pl->taps) {                                 // its tap rows, transform Source and CTA range
             const int t = p->n_tap++;
-            StageTap& q = ((StageTap*)tap_host.data())[k];
+            StageTap& q = ((StageTap*)(host.data() + tb.taps))[k];
             q.taps = (float*)(a + sa.taps);
-            q.src = (Source*)(p->d_desc + tsrc_off) + t;
-            q.zero = (int*)(p->d_desc + zero_off);
-            int* const prefix = (int*)(tap_host.data() + (tpre_off - tap_off));
+            q.src = (Source*)(d + tb.src) + t;
+            q.zero = (int*)(d + tb.zero);
+            int* const prefix = (int*)(host.data() + tb.prefix);
             prefix[t + 1] = prefix[t] + g.sets * ((cap.first + 1) >> 1);   // pairs of the most rows any run stages
         }
     }
-    if (n_tap) {
-        p->tap_ctas = ((const int*)(tap_host.data() + (tpre_off - tap_off)))[n_tap];
-        CK(cudaMemcpy(p->d_desc + tap_off, tap_host.data(), tap_host.size(), cudaMemcpyHostToDevice));
-        p->d_taps = (const StageTap*)(p->d_desc + tap_off);
-        p->d_tap_src = (const Source*)(p->d_desc + tsrc_off);
-        p->d_tap_prefix = (const int*)(p->d_desc + tpre_off);
-    }
     p->chunks.resize(n_chunks);
     for (size_t k = 0; k < n_chunks; ++k)
-        chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], p->d_desc + off[k],
-                       p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], views.data(),
-                       dry_describe.data(), pair_arranged.data());
-    for (int k = 0; k < n_mixes; ++k) {
+        chunk_describe(items, shapes, cuts[k], cuts[k + 1], host.data() + off[k], d + off[k],
+                       p->d_scratch[n_chunks < 2 ? 0 : k % ss_ctx::kAux], c->sm_count, &p->chunks[k], rec.data());
+    for (size_t k = 0; k < mix.size(); ++k) {
         ((MixItem*)(host.data() + mix_off))[k] =
-            mix_describe(caller_items, mixes[k], (double*)(p->d_desc + scr_off + scr_bytes * k), dir_out[k]);
-        p->mix_direct = p->mix_direct || dir_out[k];
+            mix_describe(caller_items, mix[k], (double*)(d + scr_off + scr_bytes * k));
+        p->mix_direct = p->mix_direct || mix[k].dir_out;
     }
-    if (n_mixes > 0) {
-        p->d_mix = (const MixItem*)(p->d_desc + mix_off);
-        p->n_mix = n_mixes;
-    }
-    CK(cudaMemcpy(p->d_desc, host.data(), scr_off, cudaMemcpyHostToDevice));
-    if (n_draws > 0) {
-        std::vector<DrawDesc> g(n_draws);
-        for (int k = 0; k < n_draws; ++k) {
-            g[k] = draw_describe(caller_items, n_items, draws[k], dry, ws.data());
-            for (int j = 0; j < g[k].S; ++j) {
-                p->draw16 = p->draw16 || g[k].r[g[k].spk[j]].dry16;
-                p->draw_stream = p->draw_stream || g[k].r[g[k].spk[j]].dry16 == 2;
-            }
+    for (int k = 0; k < n_draws; ++k) {
+        DrawDesc& g = ((DrawDesc*)(host.data() + draw_off))[k];
+        g = draw_describe(caller_items, slots, draws[k]);
+        for (int j = 0; j < g.S; ++j) {
+            p->draw16 = p->draw16 || g.r[g.spk[j]].dry16;
+            p->draw_stream = p->draw_stream || g.r[g.spk[j]].dry16 == 2;
         }
-        CK(cudaMemcpy(p->d_desc + draw_off, g.data(), sizeof(DrawDesc) * n_draws, cudaMemcpyHostToDevice));
-        p->d_draw = (const DrawDesc*)(p->d_desc + draw_off);
-        p->n_draw = n_draws;
     }
-    if (!stage.empty()) {
-        CK(cudaMemcpy(p->d_desc + stage_off, stage.data(), sizeof(StageSlot) * stage.size(), cudaMemcpyHostToDevice));
-        p->d_stage = (const StageSlot*)(p->d_desc + stage_off);
-        p->n_stage = (int)stage.size();
+    CK(cudaMemcpy(d, host.data(), image, cudaMemcpyHostToDevice));
+    if (!mix.empty()) { p->d_mix = (const MixItem*)(d + mix_off); p->n_mix = (int)mix.size(); }
+    if (n_draws > 0) { p->d_draw = (const DrawDesc*)(d + draw_off); p->n_draw = n_draws; }
+    if (!staged.empty()) { p->d_stage = (const StageSlot*)(d + stage_off); p->n_stage = (int)staged.size(); }
+    if (n_tap) {
+        p->tap_ctas = ((const int*)(host.data() + tb.prefix))[n_tap];
+        p->d_taps = (const StageTap*)(d + tb.taps);
+        p->d_tap_src = (const Source*)(d + tb.src);
+        p->d_tap_prefix = (const int*)(d + tb.prefix);
     }
     return SS_OK;
 }
@@ -2961,8 +2946,9 @@ static bool written_ranges_disjoint(std::vector<ByteRange>& r) {
 }
 
 // A plan's start draws (include/sonicsim_b200.h, ss_plan_draw), all but the byte ranges (validate_mixes)
-static int validate_draws(const ss_source* items, int n_items, const ss_plan_draw* draws, int n_draws,
-                          const ss_dry_pick* const* dry, const ss_dry_stream* const* strm) {
+static int validate_draws(const ss_source* items, const std::vector<PlanSlot>& slots, const ss_plan_draw* draws,
+                          int n_draws) {
+    const int n_items = (int)slots.size();
     if (n_draws > kMaxDraws) return SS_ERR_UNSUPPORTED;
     for (int k = 0; k < n_draws; ++k) {
         const ss_plan_draw& d = draws[k];
@@ -2977,8 +2963,8 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
             const ss_source& it = items[i];
             // level tables to test: the dry pool's for a dry-picked speaker, else the pool's
             if (!it.pool || it.win_start_dev != d.start) return SS_ERR_INVALID;
-            if (strm[i] ? !strm[i]->pool->levels : dry[i] ? !dry[i]->pool->levels : !it.pool->levels)
-                return SS_ERR_INVALID;
+            const PlanSlot& r = slots[i];
+            if (r.strm ? !r.strm->pool->levels : r.dry ? !r.dry->pool->levels : !it.pool->levels) return SS_ERR_INVALID;
         }
         int readers = 0, len = -1;
         for (int i = 0; i < n_items; ++i) {
@@ -2993,12 +2979,11 @@ static int validate_draws(const ss_source* items, int n_items, const ss_plan_dra
     return SS_OK;
 }
 
-// (dir_out[k]: mixture k's dereverberation targets, or null: S * E floats written, and every speaker of the mixture
-// needs a direct-path stem)
-static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
-                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks, int n_picks,
-                          float* const* dir_out, const ss_dry_stream* streams, int n_streams) {
-    if (n_mixes > 65535) return SS_ERR_UNSUPPORTED;         // one gridDim.y row per mixture
+// (a mixture's dir_out, when not null: S * E floats written, and every speaker of the mixture needs a direct-path stem)
+static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix,
+                          const ss_plan_draw* draws, int n_draws) {
+    const int n_items = (int)slots.size();
+    if (mix.size() > 65535) return SS_ERR_UNSUPPORTED;      // one gridDim.y row per mixture
     std::vector<ByteRange> r;
     // a draw writes its start (which only its readers read) and `used`, and reads its u
     for (int k = 0; k < n_draws; ++k) {
@@ -3006,8 +2991,7 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
         add_range(r, draws[k].used, 4, true);
         add_range(r, draws[k].u, 8 * (uint64_t)draws[k].tries, false);
     }
-    for (int k = 0; k < n_mixes; ++k) {
-        const ss_plan_mix& m = mixes[k];
+    for (const PlanMix& m : mix) {
         if (m.S < 1 || m.M < 1 || m.S > kMixStems || m.M > kMixStems) return SS_ERR_UNSUPPORTED;
         if (!m.snr || (m.S > 1 && !m.sirs) || !m.mix || (m.flags & ~SS_MIX_MONO) || m.noise_delay < 0)
             return SS_ERR_INVALID;
@@ -3024,11 +3008,11 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
             const ss_source& b = items[stems[j]];
             if (b.C != a.C || (b.win_len > 0 ? b.win_len : b.N) != T) return SS_ERR_INVALID;
         }
-        if (dir_out[k])
+        if (m.dir_out)
             for (int s = 0; s < m.S; ++s) if (!(items[m.speakers[s]].flags & SS_DIRECT_TARGET)) return SS_ERR_INVALID;
         const uint64_t E = (m.flags & SS_MIX_MONO) ? (uint64_t)T : (uint64_t)a.C * T;
         add_range(r, m.mix, 4 * E, true);
-        add_range(r, dir_out[k], 4 * E * m.S, true);
+        add_range(r, m.dir_out, 4 * E * m.S, true);
         add_range(r, m.speakers_out, 4 * E * m.S, true);
         add_range(r, m.rms_db, 4 * (uint64_t)m.S, true);
         add_range(r, m.sirs, 4 * (uint64_t)(m.S - 1), false);
@@ -3060,32 +3044,31 @@ static int validate_mixes(const ss_source* items, int n_items, const ss_plan_mix
             add_range(r, e.x, 4 * (uint64_t)e.N, false);
             add_range(r, e.bounds, 4 * (uint64_t)e.P, false);
         }
-    // a dry-picked slot may read any signal of its dry pool, and reads its dry pick
+    // a dry-picked slot may read any signal of its dry pool, and reads its dry pick; a stream slot reads its layout
     std::vector<const ss_dry_pool*> dpools;
-    for (int k = 0; k < n_picks; ++k) {
-        add_range(r, picks[k].pick_dev, 4, false);
-        if (std::find(dpools.begin(), dpools.end(), picks[k].pool) == dpools.end()) dpools.push_back(picks[k].pool);
+    for (const PlanSlot& s : slots) {
+        if (s.dry) {
+            add_range(r, s.dry->pick_dev, 4, false);
+            if (std::find(dpools.begin(), dpools.end(), s.dry->pool) == dpools.end()) dpools.push_back(s.dry->pool);
+        }
+        if (s.strm) {
+            add_range(r, s.strm->ids_dev, 4 * (uint64_t)s.strm->m, false);
+            add_range(r, s.strm->offsets_dev, 4 * (uint64_t)s.strm->m, false);
+        }
     }
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
         if (!dp->padded())
             for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
-    for (int k = 0; k < n_streams; ++k) {                   // a stream slot reads its layout
-        add_range(r, streams[k].ids_dev, 4 * (uint64_t)streams[k].m, false);
-        add_range(r, streams[k].offsets_dev, 4 * (uint64_t)streams[k].m, false);
-    }
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
 
-// A plan's dry picks (include/sonicsim_b200.h, ss_dry_pick), all but the byte ranges (validate_mixes): dry[i] receives
-// item i's pick, or null, and pair[i] the device table of its pair gains (pair_gains[k] of pick k), or null
-static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_items, const ss_dry_pick* picks,
-                              const ss_pair_gains* const* pair_gains, int n_picks, std::vector<const ss_dry_pick*>& dry,
-                              std::vector<const float*>& pair) {
-    dry.assign(n_items, nullptr);
-    pair.assign(n_items, nullptr);
+// A plan's dry picks (include/sonicsim_b200.h, ss_dry_pick), all but the byte ranges (validate_mixes): the record of
+// each pick's slot receives the pick and the device table of its pair gains (pair_gains[k] of pick k), or null
+static int validate_dry_picks(const ss_ctx* c, const ss_source* items, const ss_dry_pick* picks,
+                              const ss_pair_gains* const* pair_gains, int n_picks, std::vector<PlanSlot>& slots) {
     for (int k = 0; k < n_picks; ++k) {
         const ss_dry_pick& d = picks[k];
-        if (d.slot < 0 || d.slot >= n_items || dry[d.slot]) return SS_ERR_INVALID;      // one dry pick per slot
+        if (d.slot < 0 || d.slot >= (int)slots.size() || slots[d.slot].dry) return SS_ERR_INVALID;   // one per slot
         if (!d.pool || d.pool->c != c || !d.pick_dev || ((uintptr_t)d.pick_dev & 3)) return SS_ERR_INVALID;
         const ss_pool* pl = items[d.slot].pool;
         const ss_pair_gains* const t = pair_gains ? pair_gains[k] : nullptr;
@@ -3095,20 +3078,19 @@ static int validate_dry_picks(const ss_ctx* c, const ss_source* items, int n_ite
         if (!pl || (pl->host_res && !d.pool->padded()) || (pl->gains && !t)) return SS_ERR_INVALID;
         if (t && (t->pool != pl || t->dry != d.pool)) return SS_ERR_INVALID;
         for (const PoolEntry& e : pl->host) if (e.N > d.pool->n_min) return SS_ERR_INVALID;
-        dry[d.slot] = &d;
-        pair[d.slot] = t ? t->gains : nullptr;
+        slots[d.slot].dry = &d;
+        slots[d.slot].pair = t ? t->gains : nullptr;
     }
     return SS_OK;
 }
 
 // A plan's dry streams (include/sonicsim_b200.h, ss_dry_stream), all but the draws' tables (validate_draws) and the
-// byte ranges (validate_mixes): strm[i] receives item i's stream, or null
-static int validate_streams(const ss_ctx* c, const ss_source* items, int n_items, const ss_dry_stream* streams,
-                            int n_streams, const ss_dry_pick* const* dry, std::vector<const ss_dry_stream*>& strm) {
-    strm.assign(n_items, nullptr);
+// byte ranges (validate_mixes): the record of each stream's slot receives the stream
+static int validate_streams(const ss_ctx* c, const ss_source* items, const ss_dry_stream* streams, int n_streams,
+                            std::vector<PlanSlot>& slots) {
     for (int k = 0; k < n_streams; ++k) {
         const ss_dry_stream& w = streams[k];
-        if (w.slot < 0 || w.slot >= n_items || strm[w.slot] || dry[w.slot]) return SS_ERR_INVALID;
+        if (w.slot < 0 || w.slot >= (int)slots.size() || slots[w.slot].strm || slots[w.slot].dry) return SS_ERR_INVALID;
         const ss_pool* pl = items[w.slot].pool;
         // a pooled slot of a pool without loudness gains (a stream has no fixed pair to measure), over a 16-bit dry
         // pool of this context, with a layout of 1..kStreamEntries aligned device entries
@@ -3116,7 +3098,7 @@ static int validate_streams(const ss_ctx* c, const ss_source* items, int n_items
         if (w.m < 1 || w.m > kStreamEntries || !w.ids_dev || !w.offsets_dev || ((uintptr_t)w.ids_dev & 3) ||
             ((uintptr_t)w.offsets_dev & 3))
             return SS_ERR_INVALID;
-        strm[w.slot] = &w;
+        slots[w.slot].strm = &w;
     }
     for (int k = 0; k < n_streams; ++k)                     // (beyond 2^23 samples a crop's sum need not be exact)
         for (const PoolEntry& e : items[streams[k].slot].pool->host) if (e.N > (1 << 23)) return SS_ERR_UNSUPPORTED;
@@ -3124,37 +3106,38 @@ static int validate_streams(const ss_ctx* c, const ss_source* items, int n_items
 }
 
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
-// and the byte ranges (validate_mixes): dir_out[k] receives mixture k's direct_out, or null
-static int validate_targets(int n_mixes, const ss_plan_target* targets, int n_targets, std::vector<float*>& dir_out) {
-    dir_out.assign(n_mixes, nullptr);
+// and the byte ranges (validate_mixes): mix receives the mixtures, each with its target's direct_out, or null
+static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan_target* targets, int n_targets,
+                            std::vector<PlanMix>& mix) {
+    for (int k = 0; k < n_mixes; ++k) mix.push_back({mixes[k], nullptr});
     for (int j = 0; j < n_targets; ++j) {
         const ss_plan_target& t = targets[j];
-        if (t.mix < 0 || t.mix >= n_mixes || dir_out[t.mix] || !t.direct_out) return SS_ERR_INVALID;
-        dir_out[t.mix] = t.direct_out;
+        if (t.mix < 0 || t.mix >= n_mixes || mix[t.mix].dir_out || !t.direct_out) return SS_ERR_INVALID;
+        mix[t.mix].dir_out = t.direct_out;
     }
     return SS_OK;
 }
 
+// Every ss_plan_create* export.  A call refused for its arguments leaves *out untouched; a later refusal leaves it null.
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                        int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
-    if (!c || !out || !items || n_items <= 0) return SS_ERR_INVALID;
+    auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
+    if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
+        bad(targets, n_targets) || bad(streams, n_streams))
+        return SS_ERR_INVALID;
     *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
-    std::vector<const ss_dry_pick*> dry;
-    std::vector<const float*> pair;
-    std::vector<float*> dir_out;
-    std::vector<const ss_dry_stream*> strm;
+    std::vector<PlanSlot> slots(n_items);
+    std::vector<PlanMix> mix;
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
-    { int st = validate_dry_picks(c, items, n_items, picks, pair_gains, n_picks, dry, pair); if (st) return st; }
-    { int st = validate_streams(c, items, n_items, streams, n_streams, dry.data(), strm); if (st) return st; }
-    { int st = validate_draws(items, n_items, draws, n_draws, dry.data(), strm.data()); if (st) return st; }
-    { int st = validate_targets(n_mixes, targets, n_targets, dir_out); if (st) return st; }
-    { int st = validate_mixes(items, n_items, mixes, n_mixes, draws, n_draws, picks, n_picks, dir_out.data(), streams,
-                              n_streams);
-      if (st) return st; }
+    { int st = validate_dry_picks(c, items, picks, pair_gains, n_picks, slots); if (st) return st; }
+    { int st = validate_streams(c, items, streams, n_streams, slots); if (st) return st; }
+    { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
+    { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
+    { int st = validate_mixes(items, slots, mix, draws, n_draws); if (st) return st; }
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
@@ -3164,8 +3147,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), n_items, mixes, n_mixes, draws, n_draws, dry.data(), pair.data(),
-                              dir_out.data(), strm.data());
+    const int st = plan_build(p, items, shapes.data(), slots, mix, draws, n_draws);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -3178,13 +3160,11 @@ extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
-    if (n_mixes < 0 || (n_mixes > 0 && !mixes)) return SS_ERR_INVALID;
     return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
-    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws)) return SS_ERR_INVALID;
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
                        out);
 }
@@ -3192,9 +3172,6 @@ extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items,
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
-    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
-        (n_picks > 0 && !picks))
-        return SS_ERR_INVALID;
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
                        0, out);
 }
@@ -3203,9 +3180,6 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
-    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
-        (n_picks > 0 && !picks) || n_targets < 0 || (n_targets > 0 && !targets))
-        return SS_ERR_INVALID;
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
                        nullptr, 0, out);
 }
@@ -3214,10 +3188,6 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
-    if (n_mixes < 0 || (n_mixes > 0 && !mixes) || n_draws < 0 || (n_draws > 0 && !draws) || n_picks < 0 ||
-        (n_picks > 0 && !picks) || n_targets < 0 || (n_targets > 0 && !targets) || n_streams < 0 ||
-        (n_streams > 0 && !streams))
-        return SS_ERR_INVALID;
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
                        streams, n_streams, out);
 }
@@ -3225,7 +3195,8 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
-    return ss_plan_create_pair(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
+                       out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start

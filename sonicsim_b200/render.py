@@ -1321,9 +1321,9 @@ class DevicePlan:
     """A batch of device-resident sources bound to its output tensors (Renderer.plan_device): an ss_plan of the C ABI -
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
-    dry-picked slots take their dry signals from dry pools (ss_plan_create_dry), with pair gains their gains from
-    pair-gain tables (ss_plan_create_pair), with dereverberation targets its mixtures also write those
-    (ss_plan_create_target), and with stream slots it lays out their dry streams (ss_plan_create_stream)."""
+    dry-picked slots take their dry signals from dry pools, with pair gains their gains from pair-gain tables; with
+    dereverberation targets its mixtures also write those, and with stream slots it lays out their dry streams.  Every
+    plan is created by ss_plan_create_stream, with NULL and a count of 0 for each part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
                  streams=None):
@@ -1331,19 +1331,10 @@ class DevicePlan:
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
         self._plan = ctypes.c_void_p()
         if n > 0:
-            args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry)
-            if streams is not None:
-                st = renderer.lib.ss_plan_create_stream(*args, pair_gains, len(dry) if dry else 0, targets,
-                                                        len(targets) if targets else 0, streams, len(streams),
-                                                        ctypes.byref(self._plan))
-            elif targets is not None:
-                st = renderer.lib.ss_plan_create_target(*args, pair_gains, len(dry) if dry else 0, targets,
-                                                        len(targets), ctypes.byref(self._plan))
-            elif pair_gains is None:
-                st = renderer.lib.ss_plan_create_dry(*args, len(dry) if dry else 0, ctypes.byref(self._plan))
-            else:
-                st = renderer.lib.ss_plan_create_pair(*args, pair_gains, len(dry), ctypes.byref(self._plan))
-            _lib.check(st)
+            _lib.check(renderer.lib.ss_plan_create_stream(
+                renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
+                pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
+                len(streams) if streams else 0, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
