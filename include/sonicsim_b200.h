@@ -334,8 +334,8 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * the device: bit 0 = an interp_index outside [0, P - 2], bit 1 = a device-side bounds table that is not ascending from
  * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
  * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped), bit 4 (dry
- * pools, below) = a dry pick outside [0, n) of its dry pool (clamped), bit 5 (dry streams, below) = an invalid
- * entry of a stream slot's layout (skipped).  The Python device API raises IndexError /
+ * pools, below) = a dry pick outside [0, n) of its dry pool (clamped), bit 5 (dry streams and background streams,
+ * below) = an invalid entry of a stream or bed slot's layout (skipped).  The Python device API raises IndexError /
  * ValueError from it on request
  * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
  * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
@@ -753,6 +753,50 @@ int ss_plan_create_stream(ss_ctx* ctx, const ss_source* items, int n_items, cons
                           const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                           const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                           int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out);
+
+/* ---- background streams: SonicSet's noise and music beds laid out at every run (SonicSim_audio.py:279-340,
+ * create_background_audio), from clips held once in a dry pool (float32 or 16-bit) instead of beds built once.
+ * A bed slot is a pooled slot whose dry signal is a layout of m entries over a dry pool of n clips: four device int32
+ * arrays ids[m], offsets[m], heads[m] and counts[m], 1 <= m <= 128, read at every run.  The layout is walked in order
+ * with a running `end`, 0 at first:
+ *   - ids[j] < 0: an empty entry, skipped;
+ *   - ids[j] >= n, offsets[j] < 0, heads[j] < 0, counts[j] < 1, heads[j] + counts[j] beyond the clip's length or
+ *     offsets[j] < end: an invalid entry, skipped, and ss_device_errors reports bit 5;
+ *   - otherwise the entry is kept: clip samples [heads[j], heads[j] + counts[j]) occupy [offsets[j], offsets[j] +
+ *     counts[j]) of the stream and end becomes offsets[j] + counts[j].
+ * A dry stream (above) is the case heads[j] = 0, counts[j] = the utterance's length; both decide validity by one walk.
+ * The slot's dry signal is the stream's first N samples (N: the picked candidate's), zeros wherever no kept entry lies.
+ * A bed slot's stem, direct stem and mixture contributions are, bit for bit, those of the same plan in which the slot
+ * takes an ss_dry_pick from a dry pool of the same sample format holding the bed assembled by the rule above to the
+ * slot pool's longest N (of the same residency, or a float32 host pool over a host source pool, where a float32 device
+ * dry pool is refused).  A bed slot is always staged (k_stage), over any dry pool and any source pool; its staging area
+ * is a dry-picked slot's.  The plan uploads the n clip lengths of each dry pool its streams and beds use once, into its
+ * descriptor block.  A bed slot may read a draw's start but is no draw speaker: the draws test speakers only.
+ * ss_plan_create_bg is ss_plan_create_stream with n_bgs bed entries (n_bgs == 0: exactly ss_plan_create_stream).
+ * Refused at creation with SS_ERR_INVALID, before anything is allocated and with *out untouched:
+ *   - n_bgs < 0, or NULL bgs with n_bgs > 0;
+ *   - a slot outside [0, n_items), not pooled, named by two beds, or by a bed and a dry pick or a dry stream;
+ *   - a dry pool that is NULL or of another context;
+ *   - m outside [1, 128];
+ *   - a NULL or unaligned ids_dev / offsets_dev / heads_dev / counts_dev;
+ *   - a slot whose pool has loudness gains (a bed has no fixed (dry, trajectory) pair to measure);
+ *   - a slot that is a speaker of a draw;
+ *   - a range the plan writes that meets any of the four arrays.
+ * ss_version stays 108: the export marks the capability. */
+typedef struct {
+    int32_t slot;                     /* index into `items`: a pooled slot                                            */
+    const ss_dry_pool* pool;          /* a dry pool of the plan's context, float32 or 16-bit                          */
+    const int32_t* ids_dev;           /* device, m clip ids (< 0: empty), read at every run                           */
+    const int32_t* offsets_dev;       /* device, m stream offsets in samples, read at every run                       */
+    const int32_t* heads_dev;         /* device, m first clip samples placed, read at every run                       */
+    const int32_t* counts_dev;        /* device, m clip samples placed, read at every run                             */
+    int32_t m;                        /* 1..128                                                                       */
+} ss_bg_stream;
+int ss_plan_create_bg(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                      const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                      int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                      ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

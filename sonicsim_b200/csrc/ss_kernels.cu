@@ -1184,15 +1184,19 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
     }
     return bytes;
 }
-// What a plan knows of one of its items besides the ss_source: its dry pick, pair gains and dry stream
-// (validate_dry_picks, validate_streams) and, once plan_build has laid out the plan's descriptors, the device addresses
-// of its staging area's view (a staged slot) and of its DryStream (a stream slot)
+// What a plan knows of one of its items besides the ss_source: its dry pick, pair gains, dry stream and background
+// stream (validate_dry_picks, validate_streams, validate_bgs) and, once plan_build has laid out the plan's descriptors,
+// the device addresses of its staging area's view (a staged slot), of its DryStream (a stream slot) and of its BgStream
+// (a bed slot)
 struct PlanSlot {
     const ss_dry_pick* dry = nullptr;
     const float* pair = nullptr;       // the device table of its pair gains, or null
     const ss_dry_stream* strm = nullptr;
+    const ss_bg_stream* bg = nullptr;
     StageView* view = nullptr;
     const DryStream* ws = nullptr;
+    const BgStream* wb = nullptr;
+    const ss_dry_pool* clips() const { return strm ? strm->pool : bg ? bg->pool : nullptr; }   // a layout's dry pool
 };
 // Fill the descriptor block of items[first, last) at `hbase` (host memory) for its device address `dbase`, carve the
 // chunk's spectra / tables / work items out of `scratch` (device), and note the launch parameters in `L`.  A plan's
@@ -2473,6 +2477,7 @@ struct ss_plan {
     int n_stage = 0;
     bool draw16 = false, stage16 = false; // a draw speaker / a staged slot has a 16-bit dry pick: k_draw<true> / k_stage<true>
     bool draw_stream = false, stage_stream = false;   // a draw speaker / a staged slot is a stream slot (STREAM)
+    bool stage_bg = false;                            // a staged slot is a bed slot (k_stage<true, TAPS, true, true>)
     // slots of tap-form pools: k_stage<I16, true> reads d_taps (n_stage entries) and writes n_tap transform Sources
     // (d_tap_src, CTA ranges d_tap_prefix), which one k_prepare<false> of tap_ctas CTAs transforms behind it
     const StageTap* d_taps = nullptr;
@@ -2600,6 +2605,8 @@ struct StageSlot {
     int i16;                          // 1: the dry pool is 16-bit, `dry` holds int16 addresses (k_stage<true> only)
                                       // 2: a stream slot (k_stage<true, TAPS, true> only): `dry` holds its DryStream's
                                       //    address, dry_pick is null
+                                      // 3: a bed slot (k_stage<true, TAPS, true, true> only): `dry` holds its
+                                      //    BgStream's address, dry_pick is null
 };
 static_assert(sizeof(StageSlot) == 120, "StageSlot layout");
 // k_stage<true, TAPS, true> (a plan with a stream slot) fills such a slot's whole groups [xa & ~3, (xb + 3) & ~3) from
@@ -2639,30 +2646,71 @@ __device__ __forceinline__ void stage_stream_x(const DryStream& d, int x0, int x
         for (int u = 0; u < kStageUnroll; ++u) if (t0 + u * stride < nx) xd[t0 + u * stride] = v[u];
     }
 }
+// k_stage<true, TAPS, true, true> (a plan with a bed slot) fills such a slot's groups as stage_stream_x fills a stream
+// slot's, from its resolved bed layout (bg_resolve, bit 5; bg_sample): int16 clips through i16_sample, float32 clips as
+// they are, whichever the slot's dry pool holds.
+__device__ __forceinline__ void stage_bg_x(const BgStream& d, int x0, int x1, float* __restrict__ xd) {
+    __shared__ int s_id[kStreamEntries], s_off[kStreamEntries], s_hd[kStreamEntries], s_cnt[kStreamEntries],
+        s_len[kStreamEntries], s_a[kStreamEntries], s_b[kStreamEntries];
+    __shared__ const char* s_sig[kStreamEntries];
+    __shared__ const char* s_p[kStreamEntries];
+    __shared__ int s_k;
+    for (int j = threadIdx.x; j < d.m; j += blockDim.x) {
+        const int id = d.ids[j];
+        const bool ok = id >= 0 && id < d.n;
+        s_id[j] = id; s_off[j] = d.offsets[j]; s_hd[j] = d.heads[j]; s_cnt[j] = d.counts[j];
+        s_len[j] = ok ? d.lengths[id] : 0;
+        s_sig[j] = ok ? d.sig[id] : nullptr;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int k;
+        const unsigned err = bg_resolve(s_id, s_off, s_hd, s_cnt, s_len, s_sig, d.i16 ? 2 : 4, d.m, d.n, d.cut, s_a, s_b,
+                                        s_p, &k);
+        s_k = k;
+        if (err && blockIdx.x == 0) atomicOr(&g_dev_err, err);
+    }
+    __syncthreads();
+    const int nx = x1 - x0, k = s_k, stride = gridDim.x * blockDim.x;
+    const bool i16 = d.i16 != 0;
+    for (int t0 = blockIdx.x * blockDim.x + threadIdx.x; t0 < nx; t0 += stride * kStageUnroll) {
+        float v[kStageUnroll];
+#pragma unroll
+        for (int u = 0; u < kStageUnroll; ++u) {        // every load issued before the first store
+            const int t = t0 + u * stride;
+            v[u] = t < nx ? bg_sample(s_a, s_b, s_p, k, x0 + t, i16) : 0.0f;
+        }
+#pragma unroll
+        for (int u = 0; u < kStageUnroll; ++u) if (t0 + u * stride < nx) xd[t0 + u * stride] = v[u];
+    }
+}
 // k_stage<true> (a plan with a 16-bit dry pick) reads such a slot's dry samples as 4 int16 at a time from the whole
 // groups [xa & ~3, (xb + 3) & ~3) of the picked signal (inside its padded arena) and stores their exact float32 values,
 // so that the staging area holds what a float pool's slot stages.
 // k_stage<I16, true> (a plan with a slot of a tap-form pool) copies such a slot's tap rows [row0, row0 + rows), one
 // contiguous span of the candidate's rows, instead of sets * rows spectra rows, and writes the Source over them that the
 // plan's transform launch (k_prepare<false>) turns into the spectra the slot's view names: those k_stage<I16> copies.
-template <bool I16, bool TAPS = false, bool STREAM = false>
+template <bool I16, bool TAPS = false, bool STREAM = false, bool BG = false>
 __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slots, const StageTap* __restrict__ taps) {
     const StageSlot& g = slots[blockIdx.y];
     const StageTap* const tp = TAPS && taps[blockIdx.y].taps ? &taps[blockIdx.y] : nullptr;
     const DryStream* const ds = STREAM && g.i16 == 2 ? reinterpret_cast<const DryStream*>(g.dry) : nullptr;
+    const BgStream* const bs = BG && g.i16 == 3 ? reinterpret_cast<const BgStream*>(g.dry) : nullptr;
+    const void* const laid = BG && bs ? (const void*)bs : (const void*)ds;   // a stream or bed slot: no dry pick
     __shared__ StageView s_v;
     __shared__ const float* s_src;                      // the signal the dry samples come from
     __shared__ int s_x[2];                              // dry samples copied: whole float4s [s_x[0], s_x[1])
     if (threadIdx.x == 0) {
         const unsigned err = stage_head(g.pool, g.n, *g.pick, g.parts, g.K, g.gains, g.ws_dev, g.ws, g.len, g.C,
-                                        g.sets != 0, ds ? nullptr : g.dry, !ds && g.dry ? *g.dry_pick : 0, g.n_dry, s_v,
+                                        g.sets != 0, laid ? nullptr : g.dry, !laid && g.dry ? *g.dry_pick : 0, g.n_dry, s_v,
                                         s_src, s_x[0], s_x[1], g.pair);
         if (err && blockIdx.x == 0) atomicOr(&g_dev_err, err);
     }
     __syncthreads();
     if (STREAM && ds) stage_stream_x(*ds, s_x[0], s_x[1], g.x);   // (the loop below then copies no dry samples)
+    if (BG && bs) stage_bg_x(*bs, s_x[0], s_x[1], g.x);
     const PoolEntry& e = s_v.e;
-    const size_t nx4 = STREAM && ds ? 0 : (size_t)((s_x[1] - s_x[0]) >> 2);
+    const size_t nx4 = (STREAM || BG) && laid ? 0 : (size_t)((s_x[1] - s_x[0]) >> 2);
     const size_t per_set = (size_t)s_v.rows * (kSpec / 2);          // float4s per set
     const size_t rows_h = (size_t)e.P * g.C * s_v.K;                 // rows per set of the bank
     const size_t total = nx4 + (TAPS && tp ? (size_t)s_v.rows * (kB / 4) : (size_t)g.sets * per_set);
@@ -2787,10 +2835,10 @@ static StageArea stage_area_of(const ss_source& it) {
 
 // Lay out, fill and upload a plan's descriptors.  The host fills one image, each section at a 256-byte boundary: the
 // chunk descriptors, the mixtures' MixItems, the draws' DrawDescs, the staged slots' StageSlots, the tap block
-// (tap_block, with slots of tap-form pools), the streams' DryStreams (caller order) and the utterance lengths of each
-// dry pool the streams use; one copy uploads it.  Behind the image, written by the device only and never uploaded: one
-// scratch block per mixture, then the staged slots' staging areas.  slots[i] is caller item i's record; plan_build
-// notes where its view and its DryStream landed.
+// (tap_block, with slots of tap-form pools), the streams' DryStreams and the beds' BgStreams (caller order) and the
+// clip lengths of each dry pool the streams and beds use; one copy uploads it.  Behind the image, written by the device
+// only and never uploaded: one scratch block per mixture, then the staged slots' staging areas.  slots[i] is caller
+// item i's record; plan_build notes where its view, its DryStream and its BgStream landed.
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes,
                       std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix, const ss_plan_draw* draws,
                       int n_draws) {
@@ -2802,13 +2850,14 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     std::vector<PlanSlot*> rec(arranged.size());         // rec[i]: the record of arranged item i
-    std::vector<int> staged;    // arranged items that are slots of host pools, host or 16-bit dry picks, stream slots
-    int n_tap = 0, n_strm = 0;
+    std::vector<int> staged;    // arranged items that are slots of host pools, host or 16-bit dry picks, stream and bed
+    int n_tap = 0, n_strm = 0, n_bg = 0;                 // slots
     for (int i = 0; i < (int)arranged.size(); ++i) {
         rec[i] = &slots[order[i]];
         const PlanSlot& r = *rec[i];
         n_strm += r.strm ? 1 : 0;
-        if (items[i].pool && (items[i].pool->host_res || (r.dry && r.dry->pool->padded()) || r.strm)) {
+        n_bg += r.bg ? 1 : 0;
+        if (items[i].pool && (items[i].pool->host_res || (r.dry && r.dry->pool->padded()) || r.strm || r.bg)) {
             staged.push_back(i);
             n_tap += items[i].pool->taps ? 1 : 0;
         }
@@ -2831,12 +2880,13 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     const TapBlock tb = tap_block(at, (int)staged.size(), n_tap);
     if (n_tap) at = tb.end;
     const size_t wdesc_off = take(sizeof(DryStream) * n_strm);
+    const size_t bdesc_off = take(sizeof(BgStream) * n_bg);
     std::vector<const ss_dry_pool*> wpools;              // each with its lengths at wlen_off
     std::vector<size_t> wlen_off;
     for (const PlanSlot& s : slots)
-        if (s.strm && std::find(wpools.begin(), wpools.end(), s.strm->pool) == wpools.end()) {
-            wpools.push_back(s.strm->pool);
-            wlen_off.push_back(take(sizeof(int32_t) * (size_t)s.strm->pool->n));
+        if (s.clips() && std::find(wpools.begin(), wpools.end(), s.clips()) == wpools.end()) {
+            wpools.push_back(s.clips());
+            wlen_off.push_back(take(sizeof(int32_t) * (size_t)s.clips()->n));
         }
     const size_t image = at;
     const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
@@ -2851,17 +2901,23 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
     char* const d = p->d_desc;
     std::vector<char> host(image, 0);
-    for (int i = 0, k = 0; i < n_items; ++i) {           // the streams first: staged slots and draws name them
-        if (!slots[i].strm) continue;
-        const ss_dry_stream& w = *slots[i].strm;
-        const ss_dry_pool* dp = w.pool;
-        const size_t lo = wlen_off[std::find(wpools.begin(), wpools.end(), dp) - wpools.begin()];
+    for (int i = 0, k = 0, kb = 0; i < n_items; ++i) {   // the streams and beds first: staged slots and draws name them
+        const ss_dry_pool* dp = slots[i].clips();
+        if (!dp) continue;
+        const int* const lengths = (const int*)(d + wlen_off[std::find(wpools.begin(), wpools.end(), dp) - wpools.begin()]);
         int cut = 0;
         for (const PoolEntry& e : caller_items[i].pool->host) cut = std::max(cut, e.N);
-        ((DryStream*)(host.data() + wdesc_off))[k] = {w.ids_dev, w.offsets_dev, (const int*)(d + lo),
-                                                      (const int16_t* const*)dp->ptrs,
-                                                      dp->levels ? dp->level_ptr : nullptr, w.m, dp->n, cut, 0};
-        slots[i].ws = (const DryStream*)(d + wdesc_off) + k++;
+        if (const ss_dry_stream* w = slots[i].strm) {
+            ((DryStream*)(host.data() + wdesc_off))[k] = {w->ids_dev, w->offsets_dev, lengths,
+                                                          (const int16_t* const*)dp->ptrs,
+                                                          dp->levels ? dp->level_ptr : nullptr, w->m, dp->n, cut, 0};
+            slots[i].ws = (const DryStream*)(d + wdesc_off) + k++;
+        } else {
+            const ss_bg_stream& b = *slots[i].bg;
+            ((BgStream*)(host.data() + bdesc_off))[kb] = {b.ids_dev, b.offsets_dev, b.heads_dev, b.counts_dev, lengths,
+                                                          (const char* const*)dp->ptrs, b.m, dp->n, cut, dp->i16 ? 1 : 0};
+            slots[i].wb = (const BgStream*)(d + bdesc_off) + kb++;
+        }
     }
     for (size_t j = 0; j < wpools.size(); ++j)
         memcpy(host.data() + wlen_off[j], wpools[j]->N.data(), sizeof(int32_t) * (size_t)wpools[j]->n);
@@ -2880,6 +2936,10 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         if (r.ws) {                                     // (k_stage reads the layout through its DryStream)
             g.dry = reinterpret_cast<const float* const*>(r.ws); g.n_dry = r.strm->pool->n; g.i16 = 2;
             p->stage_stream = true;
+        }
+        if (r.wb) {                                     // (k_stage reads the layout through its BgStream)
+            g.dry = reinterpret_cast<const float* const*>(r.wb); g.n_dry = r.bg->pool->n; g.i16 = 3;
+            p->stage_bg = true;
         }
         const std::pair<int, int> cap = stage_cap(const_cast<ss_pool*>(pl), it.win_len);
         const StageArea sa = stage_area_of(it);
@@ -3044,7 +3104,8 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
             add_range(r, e.x, 4 * (uint64_t)e.N, false);
             add_range(r, e.bounds, 4 * (uint64_t)e.P, false);
         }
-    // a dry-picked slot may read any signal of its dry pool, and reads its dry pick; a stream slot reads its layout
+    // a dry-picked slot may read any signal of its dry pool, and reads its dry pick; a stream slot reads its layout; a
+    // bed slot reads its layout and may read any clip of its dry pool
     std::vector<const ss_dry_pool*> dpools;
     for (const PlanSlot& s : slots) {
         if (s.dry) {
@@ -3054,6 +3115,11 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
         if (s.strm) {
             add_range(r, s.strm->ids_dev, 4 * (uint64_t)s.strm->m, false);
             add_range(r, s.strm->offsets_dev, 4 * (uint64_t)s.strm->m, false);
+        }
+        if (s.bg) {                                         // a bed slot reads its layout and any clip of its pool
+            for (const int32_t* a : {s.bg->ids_dev, s.bg->offsets_dev, s.bg->heads_dev, s.bg->counts_dev})
+                add_range(r, a, 4 * (uint64_t)s.bg->m, false);
+            if (std::find(dpools.begin(), dpools.end(), s.bg->pool) == dpools.end()) dpools.push_back(s.bg->pool);
         }
     }
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
@@ -3105,6 +3171,30 @@ static int validate_streams(const ss_ctx* c, const ss_source* items, const ss_dr
     return SS_OK;
 }
 
+// A plan's background streams (include/sonicsim_b200.h, ss_bg_stream), all but the byte ranges (validate_mixes): the
+// record of each bed's slot receives the bed
+static int validate_bgs(const ss_ctx* c, const ss_source* items, const ss_bg_stream* bgs, int n_bgs,
+                        const ss_plan_draw* draws, int n_draws, std::vector<PlanSlot>& slots) {
+    for (int k = 0; k < n_bgs; ++k) {
+        const ss_bg_stream& b = bgs[k];
+        if (b.slot < 0 || b.slot >= (int)slots.size()) return SS_ERR_INVALID;
+        const PlanSlot& r = slots[b.slot];
+        if (r.bg || r.strm || r.dry) return SS_ERR_INVALID;
+        const ss_pool* pl = items[b.slot].pool;
+        // a pooled slot of a pool without loudness gains (a bed has no fixed pair to measure), over a dry pool of this
+        // context, with a layout of 1..kStreamEntries aligned device entries
+        if (!pl || pl->gains || !b.pool || b.pool->c != c) return SS_ERR_INVALID;
+        if (b.m < 1 || b.m > kStreamEntries) return SS_ERR_INVALID;
+        for (const int32_t* a : {b.ids_dev, b.offsets_dev, b.heads_dev, b.counts_dev})
+            if (!a || ((uintptr_t)a & 3)) return SS_ERR_INVALID;
+        for (int j = 0; j < n_draws; ++j)                   // (the draws test speakers only: a bed may be a reader)
+            for (int s = 0; s < draws[j].S && s < kDrawSpeakers; ++s)
+                if (draws[j].speakers[s] == b.slot) return SS_ERR_INVALID;
+        slots[b.slot].bg = &b;
+    }
+    return SS_OK;
+}
+
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
 // and the byte ranges (validate_mixes): mix receives the mixtures, each with its target's direct_out, or null
 static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan_target* targets, int n_targets,
@@ -3118,16 +3208,16 @@ static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan
     return SS_OK;
 }
 
-// Every ss_plan_create* export.  A call refused for its arguments leaves *out untouched; a later refusal leaves it null.
+// Every ss_plan_create* export.  A call refused for its arguments leaves *out untouched; a later failure leaves it null.
 static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
-                       int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
+                       int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                       ss_plan** out) {
     auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
     if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
-        bad(targets, n_targets) || bad(streams, n_streams))
+        bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs))
         return SS_ERR_INVALID;
-    *out = nullptr;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
     std::vector<PlanSlot> slots(n_items);
@@ -3135,9 +3225,11 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     { int st = shape_dev_items(c, items, n_items, shapes, true); if (st) return st; }
     { int st = validate_dry_picks(c, items, picks, pair_gains, n_picks, slots); if (st) return st; }
     { int st = validate_streams(c, items, streams, n_streams, slots); if (st) return st; }
+    { int st = validate_bgs(c, items, bgs, n_bgs, draws, n_draws, slots); if (st) return st; }
     { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
     { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
     { int st = validate_mixes(items, slots, mix, draws, n_draws); if (st) return st; }
+    *out = nullptr;
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
     p->c = c;
@@ -3155,25 +3247,27 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 }
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
-    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
+                       out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
-    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, out);
+    return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
+                       0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-                       out);
+                       nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
-                       0, out);
+                       0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3181,7 +3275,7 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3189,14 +3283,23 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, out);
+                       streams, n_streams, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                                 const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                 const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                 int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
+                                 int n_bgs, ss_plan** out) {
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, bgs, n_bgs, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
-                       out);
+                       nullptr, 0, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
@@ -3219,7 +3322,9 @@ static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     }
     if (p->n_stage) {                                   // staged slots: after the draws, before any chunk reads a slot
         const dim3 grid(kStageCtas, p->n_stage);
-        if (p->n_tap && p->stage_stream) k_stage<true, true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
+        if (p->n_tap && p->stage_bg) k_stage<true, true, true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
+        else if (p->stage_bg) k_stage<true, false, true, true><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);
+        else if (p->n_tap && p->stage_stream) k_stage<true, true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
         else if (p->stage_stream) k_stage<true, false, true><<<grid, 256, 0, stream>>>(p->d_stage, nullptr);
         else if (p->n_tap && p->stage16) k_stage<true, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);
         else if (p->n_tap) k_stage<false, true><<<grid, 256, 0, stream>>>(p->d_stage, p->d_taps);

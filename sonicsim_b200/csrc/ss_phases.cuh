@@ -508,14 +508,16 @@ SS_HD const int16_t* speaker_signal_i16(const double* const* dry_levels, const i
 // skipped; one with id >= n, offset < 0 or offset < end (the end of the last kept entry, 0 at first) is invalid,
 // skipped and reported (bit 5); any other is kept: utterance id of len samples occupies [offset, offset + len) of the
 // stream and end becomes offset + len.  Zeros lie wherever no kept entry does.  k_stage, k_draw and the CPU emulation
-// decide validity through this one walk.
+// decide validity through this one walk (layout_entries), which background streams (ss_bg_stream, bg_entries) share:
+// a speech stream is the bed form with head 0 and count len.
 constexpr int kStreamEntries = 128;                    // the most entries of a layout
 constexpr unsigned kStreamBit = 32u;                   // bit 5 of ss_device_errors: an invalid entry was skipped
-// Walks entries [0, m): len_of(j, id) gives the length of entry j's utterance (id valid), kept(j, id, offset, len)
-// sees each kept entry in order and returns false to end the walk there.  Returns kStreamBit if an invalid entry was
-// met.
-template <class Len, class Kept>
-SS_HD unsigned stream_entries(const int* ids, const int* offsets, int m, int n, Len len_of, Kept kept) {
+// Walks entries [0, m) of a layout over n clips: span(j, id, head, count) sets the clip samples [head, head + count)
+// entry j places (id valid) and returns false when they are not a non-empty range of the clip (an invalid entry);
+// kept(j, id, offset, head, count) sees each kept entry in order and returns false to end the walk there.  Returns
+// kStreamBit if an invalid entry was met.
+template <class Span, class Kept>
+SS_HD unsigned layout_entries(const int* ids, const int* offsets, int m, int n, Span span, Kept kept) {
     unsigned err = 0;
     long long end = 0;
     for (int j = 0; j < m; ++j) {
@@ -523,11 +525,43 @@ SS_HD unsigned stream_entries(const int* ids, const int* offsets, int m, int n, 
         if (id < 0) continue;
         const int o = offsets[j];
         if (id >= n || o < 0 || o < end) { err = kStreamBit; continue; }
-        const int len = len_of(j, id);
-        end = (long long)o + len;
-        if (!kept(j, id, o, len)) break;
+        int head, count;
+        if (!span(j, id, head, count)) { err = kStreamBit; continue; }
+        end = (long long)o + count;
+        if (!kept(j, id, o, head, count)) break;
     }
     return err;
+}
+// A speech stream's walk: len_of(j, id) gives the length of entry j's utterance (id valid), kept(j, id, offset, len)
+// sees each kept entry in order and returns false to end the walk there.  Returns kStreamBit if an invalid entry was
+// met.
+template <class Len, class Kept>
+SS_HD unsigned stream_entries(const int* ids, const int* offsets, int m, int n, Len len_of, Kept kept) {
+    return layout_entries(ids, offsets, m, n,
+                          [&](int j, int id, int& head, int& count) { head = 0; count = len_of(j, id); return true; },
+                          [&](int j, int id, int o, int, int count) { return kept(j, id, o, count); });
+}
+// A background stream's walk: entry j places clip samples [heads[j], heads[j] + counts[j]), which must lie in the clip
+// of len_of(j, id) samples with counts[j] >= 1; kept as for layout_entries.
+template <class Len, class Kept>
+SS_HD unsigned bg_entries(const int* ids, const int* offsets, const int* heads, const int* counts, int m, int n,
+                          Len len_of, Kept kept) {
+    return layout_entries(ids, offsets, m, n,
+                          [&](int j, int id, int& head, int& count) {
+                              head = heads[j]; count = counts[j];
+                              return head >= 0 && count >= 1 && (long long)head + count <= len_of(j, id);
+                          },
+                          kept);
+}
+// The kept entry covering stream sample n of a resolved layout whose k entries start at a[] ascending, plus one: 0 when
+// none starts at or before n (the caller tests n < b[lo - 1])
+SS_HD int layout_find(const int* a, int k, int n) {
+    int lo = 0, hi = k;                                 // the first entry starting after n
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (a[mid] <= n) lo = mid + 1; else hi = mid;
+    }
+    return lo;
 }
 // A stream slot's descriptor in its plan's block (the plan's copy of its dry pool's utterance lengths, the pool's
 // signal and sparse-table pointers - ss_dry_pool::ptrs); cut is the slot pool's longest N, the length of the stream a
@@ -562,11 +596,7 @@ SS_HD unsigned stream_resolve(const int* ids, const int* offsets, const int* len
 // Sample n of a resolved stream (stream_resolve: k entries), as k_stage stores it: the covering utterance's sample
 // (i16_sample), or 0
 SS_HD float stream_sample(const int* a, const int* b, const int16_t* const* p, int k, int n) {
-    int lo = 0, hi = k;                                 // the first entry starting after n
-    while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (a[mid] <= n) lo = mid + 1; else hi = mid;
-    }
+    const int lo = layout_find(a, k, n);
     return lo > 0 && n < b[lo - 1] ? i16_sample(p[lo - 1][n - a[lo - 1]]) : 0.0f;
 }
 // The energy of the crop [s, s + len) of a stream (s + len at most the stream's cut): over the kept entries that meet
@@ -590,6 +620,47 @@ SS_HD double stream_level(const DryStream& d, int s, int len) {
 // draw_silent of a stream speaker (D = len)
 SS_HD bool draw_silent_stream(const DryStream& d, int s, int len, float threshold_db) {
     return draw_silent_sums(0.0, stream_level(d, s, len), (double)len, threshold_db);
+}
+// ---- background streams (ss_bg_stream, include/sonicsim_b200.h): a bed slot's dry signal is laid out at every run
+// from m (ids, offsets, heads, counts) entries over a dry pool of n clips, float32 or 16-bit (bg_entries' walk).
+// A bed slot's descriptor in its plan's block: the layout, the plan's copy of the clip lengths and the pool's signal
+// pointers (float or int16 addresses, i16 telling which); cut as for DryStream.
+struct BgStream {
+    const int* ids;
+    const int* offsets;
+    const int* heads;
+    const int* counts;
+    const int* lengths;
+    const char* const* sig;
+    int m, n, cut, i16;
+};
+static_assert(sizeof(BgStream) == 64, "BgStream layout");
+// The kept entries of a bed layout cut at `cut`, as stream_resolve resolves a speech stream's: a[k] <= n < b[k] is
+// covered by element n - a[k] of p[k], the clip's address sig[j] advanced by its head (elements of `size` bytes).
+// len[j] is entry j's clip length (read where its id is valid).
+SS_HD unsigned bg_resolve(const int* ids, const int* offsets, const int* heads, const int* counts, const int* len,
+                          const char* const* sig, int size, int m, int n, int cut, int* a, int* b, const char** p,
+                          int* count) {
+    int k = 0;
+    const unsigned err = bg_entries(ids, offsets, heads, counts, m, n, [&](int j, int) { return len[j]; },
+                                    [&](int j, int, int o, int h, int c) {
+                                        if (o < cut) {
+                                            const long long e = (long long)o + c;
+                                            a[k] = o; b[k] = e < cut ? (int)e : cut; p[k] = sig[j] + (size_t)h * size;
+                                            ++k;
+                                        }
+                                        return true;
+                                    });
+    *count = k;
+    return err;
+}
+// Sample n of a resolved bed (bg_resolve: k entries), as k_stage stores it: the covering clip's sample (an int16 clip's
+// through i16_sample), or 0
+SS_HD float bg_sample(const int* a, const int* b, const char* const* p, int k, int n, bool i16) {
+    const int lo = layout_find(a, k, n);
+    if (lo == 0 || n >= b[lo - 1]) return 0.0f;
+    const int t = n - a[lo - 1];
+    return i16 ? i16_sample(reinterpret_cast<const int16_t*>(p[lo - 1])[t]) : reinterpret_cast<const float*>(p[lo - 1])[t];
 }
 
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed

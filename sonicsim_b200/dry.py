@@ -195,6 +195,87 @@ def long_audio_layouts(lengths, total: int, m: int, count: int, generator=None, 
     return out_ids, out_off
 
 
+def background_audio_layouts(lengths, total: int, m: int, count: int, generator=None, sample_rate: int = 16000,
+                             select_lengths=None):
+    """`count` layouts of create_background_audio beds (:281-340) over clips of `lengths` (a 1-D integer tensor of n
+    lengths in samples, already at `sample_rate`), for render.BackgroundStream: (ids, offsets, heads, counts), four
+    int32 tensors of shape (count, m) on `lengths`' device, -1 in unused entries.  Torch ops only, so a training step
+    refreshes them on the GPU without a host synchronisation; `generator` (of that device) makes them reproducible.
+
+    Each row draws the bed create_background_audio would build for `total` samples:
+      - selection, get_random_wav_path_from_json's rule with threshold 0.4: clips in a uniform random order without
+        replacement, taken while the running total of `select_lengths` (default `lengths`) is below 0.4 * total; the
+        clip whose addition reaches `total` is still taken, and selection stops there.  SonicSet's JSONs list clips at
+        their native rate (44.1 kHz) and the reference compares those against the 16 kHz total: pass them as
+        `select_lengths` to keep that;
+      - placement, _place_background_audio's rule: the selected clips in an independent uniform random order, each
+        followed by a tail uniform in {0, ..., 10 * sample_rate}.  The first clip whose length plus tail reaches the
+        remaining samples is the end clip: with slack = floor((total - cursor) * 0.1), lead and trail uniform in
+        {0, ..., slack}, its samples [lead, lead + count) go to cursor + lead, count = min(len, total - trail - cursor)
+        - lead, if count > 0, and the row ends there.
+    The layouts match the reference in distribution, not in its `random`-stream draws.  A row that would need more than
+    m entries keeps its first m (in stream order); beds hold a few clips of tens of seconds, so a small m suffices.
+
+    Cost: one float32 key per (row, clip) for the selection and one for the placement order; background corpora hold
+    thousands of clips, so every key of every row is sorted."""
+    import torch
+    lengths = lengths.reshape(-1).to(torch.int64)
+    sl = lengths if select_lengths is None else select_lengths.reshape(-1).to(device=lengths.device, dtype=torch.int64)
+    n, dev = lengths.numel(), lengths.device
+    if n < 1 or sl.numel() != n or not 1 <= m <= 128 or count < 1:
+        raise ValueError("background_audio_layouts: need n >= 1 clips with as many select_lengths, 1 <= m <= 128 and "
+                         "count >= 1, got n = %d, %d select_lengths, m = %d, count = %d" % (n, sl.numel(), m, count))
+    kw = {"generator": generator, "device": dev}
+    sel = torch.argsort(torch.rand((count, n), **kw), dim=1)
+    ls = sl[sel]
+    # clip i of the order is taken while the total before it is below 0.4 * total (a prefix: the totals only grow, and
+    # the one that reaches `total` ends the selection with every later total above 0.4 * total)
+    chosen = (torch.cumsum(ls, dim=1) - ls).double() < 0.4 * total
+    w = min(n, m)
+    key = torch.rand((count, n), **kw).masked_fill(~chosen, 2.0)
+    order = torch.topk(key, w, dim=1, largest=False, sorted=True).indices
+    ids = sel.gather(1, order)
+    valid = chosen.gather(1, order)
+    lp = lengths[ids]
+    tails = torch.randint(0, int(10 * sample_rate) + 1, (count, w), **kw)
+    span = (lp + tails) * valid
+    cum = torch.cumsum(span, dim=1)
+    cursor = cum - span
+    reach = valid & (cum >= total)                       # the end clip is the first valid one that reaches `total`
+    end = reach & (torch.cumsum(reach.to(torch.int32), dim=1) == 1)
+    whole = valid & ~reach                               # (every valid clip before the end clip)
+    slack = torch.floor((total - cursor).double() * 0.1)
+    lead = torch.minimum(torch.floor(torch.rand((count, w), dtype=torch.float64, **kw) * (slack + 1)), slack).long()
+    trail = torch.minimum(torch.floor(torch.rand((count, w), dtype=torch.float64, **kw) * (slack + 1)), slack).long()
+    cnt_end = torch.minimum(lp, total - trail - cursor) - lead
+    keep_end = end & (cnt_end > 0)
+    keep = (whole & (lp > 0)) | keep_end
+    out = [torch.full((count, m), -1, dtype=torch.int32, device=dev) for _ in range(4)]
+    out[0][:, :w] = torch.where(keep, ids, -1).to(torch.int32)
+    out[1][:, :w] = torch.where(keep, torch.where(keep_end, cursor + lead, cursor), -1).to(torch.int32)
+    out[2][:, :w] = torch.where(keep, torch.where(keep_end, lead, 0), -1).to(torch.int32)
+    out[3][:, :w] = torch.where(keep, torch.where(keep_end, cnt_end, lp), -1).to(torch.int32)
+    return tuple(out)
+
+
+def background_clips(paths, sample_rate: int = 16000, loader=None):
+    """The clips of a background corpus as 1-D float32 CPU tensors, each exactly the signal create_background_audio
+    adds for its path: resampled to `sample_rate` (_load_resampled) and, when stereo, averaged to mono.  A clip of any
+    other channel count than 1 or 2 raises ValueError.  A float32 or 16-bit dry pool of render.BackgroundStream beds is
+    built from these."""
+    import torch
+    loader = loader or _default_loader
+    out = []
+    for p in paths:
+        clip = _load_resampled(p, sample_rate, loader)
+        if clip.dim() != 2 or clip.shape[0] not in (1, 2):
+            raise ValueError("background_clips: %s has shape %s, need (1, n) or (2, n)" % (p, tuple(clip.shape)))
+        if clip.shape[0] == 2:
+            clip = clip.mean(dim=0, keepdim=True)
+        out.append(clip[0].to(torch.float32).contiguous())
+    return out
+
+
 _kernel_cache: T.Dict[T.Tuple[int, int, str], T.Tuple] = {}
 
 

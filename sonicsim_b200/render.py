@@ -85,7 +85,8 @@ class Pooled(T.NamedTuple):
     needs every candidate's bank to hold a direct set with these taps.  A pick outside [0, n) is clamped into range and a
     start beyond the picked candidate's N - length is clamped too (check_device_errors).  Only plan_device takes it.
     `dry`, a DryPick, makes it a dry-picked slot: the picked candidate renders with the dry signal the DryPick names in
-    place of its own; a DryStream makes it a stream slot, whose dry signal is laid out from utterances at every run."""
+    place of its own; a DryStream makes it a stream slot, whose dry signal is laid out from utterances at every run, and
+    a BackgroundStream a bed slot, whose noise or music bed is laid out from clips at every run."""
     pool: T.Any
     pick: T.Any
     window: T.Tuple[T.Any, int]
@@ -123,6 +124,24 @@ class DryStream(T.NamedTuple):
     pool: T.Any
     ids: T.Any
     offsets: T.Any
+
+
+class BackgroundStream(T.NamedTuple):
+    """The dry signal of a pooled slot (Pooled.dry) laid out at every run from clips, as create_background_audio lays
+    out a noise or music bed (SonicSim_audio.py:279-340): `pool` a DryPool of n clips, float32 or 16-bit (e.g. from
+    dry.background_clips), and `ids`, `offsets`, `heads`, `counts` contiguous 1-D CUDA int32 tensors of one length m,
+    1 <= m <= 128 (e.g. rows of (B, m) tensors from dry.background_audio_layouts), read on the device at every run.
+    The layout is walked in order: an entry with id < 0 is empty and skipped; one with id >= n, offset < 0, head < 0,
+    count < 1, head + count beyond the clip, or an offset before the end of the last kept entry is invalid and skipped
+    (check_device_errors raises ValueError); any other places clip samples [head, head + count) at stream samples
+    [offset, offset + count).  The slot renders its picked candidate with the stream's first N samples, zeros where no
+    clip lies: bit for bit a DryPick from a pool of the same dtype holding the assembled bed.  A bed slot may read a
+    CropDraw's start but is none of its speakers; pools with loudness gains take no beds."""
+    pool: T.Any
+    ids: T.Any
+    offsets: T.Any
+    heads: T.Any
+    counts: T.Any
 
 
 class CropDraw(T.NamedTuple):
@@ -578,8 +597,8 @@ def _hold_banks(plan, sources):
     releases them at once, once)."""
     banks = []
     for s in sources:
-        # a dry-picked slot's dry pool and pair gains, a stream slot's utterance pool
-        dry = s.dry if isinstance(s, Pooled) and isinstance(s.dry, (DryPick, DryStream)) else None
+        # a dry-picked slot's dry pool and pair gains, a stream slot's utterance pool, a bed slot's clip pool
+        dry = s.dry if isinstance(s, Pooled) and isinstance(s.dry, (DryPick, DryStream, BackgroundStream)) else None
         held = ([s.pool] + ([dry.pool, getattr(dry, "gains", None)] if dry else []) if isinstance(s, Pooled)
                 else [_rirs(s)[0]])
         for b in held:
@@ -1014,15 +1033,18 @@ class Renderer:
         that every (dry signal, trajectory) pair is reachable in the same single graph launch
         (dry_picks.random_(0, n) before the run).  With `dry` = DryStream(utterance_pool, ids, offsets) the slot's dry
         stream is laid out from a 16-bit utterance pool at every run (ss_plan_create_stream): a fresh arrangement of
-        utterances and gaps per step (dry.long_audio_layouts into the ids and offsets before the run)."""
+        utterances and gaps per step (dry.long_audio_layouts into the ids and offsets before the run).  With `dry` =
+        BackgroundStream(clip_pool, ids, offsets, heads, counts) the slot's noise or music bed is laid out from a clip
+        pool at every run (ss_plan_create_bg; dry.background_audio_layouts into the four arrays before the run)."""
         dry = self._device_dry(sources)
         streams = self._device_streams(sources)
+        bgs = self._device_bgs(sources)
         items, n, keep = self._device_items(sources, outs, direct_outs)
         targets = []
         mixes = self._device_mixes(mixtures, outs, keep, items, targets) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
-                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams)
+                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1034,10 +1056,11 @@ class Renderer:
                 if isinstance(d, DryPick):
                     raise ValueError("plan_device: source %d has a DryPick but is not a pooled slot (render.Pooled)" % i)
                 continue
-            if d is None or isinstance(d, DryStream):
+            if d is None or isinstance(d, (DryStream, BackgroundStream)):
                 continue
             if not isinstance(d, DryPick):
-                raise ValueError("plan_device: the dry of pooled source %d must be a DryPick or None, or a DryStream" % i)
+                raise ValueError("plan_device: the dry of pooled source %d must be a DryPick or None, or a DryStream or a "
+                                 "BackgroundStream" % i)
             if not isinstance(d.pool, DryPool):
                 raise ValueError("plan_device: the dry pool of source %d must be a DryPool" % i)
             _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
@@ -1096,6 +1119,32 @@ class Renderer:
             streams.append(_lib.SsDryStream(slot=i, pool=d.pool._h.value, ids_dev=ids, offsets_dev=off, m=m))
         return (_lib.SsDryStream * len(streams))(*streams) if streams else None
 
+    def _device_bgs(self, sources):
+        """Validated ss_bg_stream array of a plan's bed slots, or None without any."""
+        import torch
+        bgs = []
+        for i, s in enumerate(sources):
+            d = getattr(s, "dry", None)
+            if not isinstance(d, BackgroundStream):
+                continue
+            if not isinstance(s, Pooled):
+                raise ValueError("plan_device: source %d has a BackgroundStream but is not a pooled slot "
+                                 "(render.Pooled)" % i)
+            if not isinstance(d.pool, DryPool):
+                raise ValueError("plan_device: the clip pool of source %d must be a DryPool" % i)
+            _check_usable(d.pool, self, "plan_device: the DryPool of source %d" % i)
+            if isinstance(s.pool, SourcePool) and s.pool.gains:
+                raise ValueError("plan_device: pooled source %d has a BackgroundStream over a pool with loudness gains: "
+                                 "a bed has no fixed (dry signal, trajectory) pair to measure" % i)
+            own = "source %d" % i
+            m = d.ids.numel() if isinstance(d.ids, torch.Tensor) else 0
+            ids = _tensor(d.ids, "plan_device", own, "bed ids", torch.int32, self.device, ("m",), (1, 128))
+            ptr = [_tensor(a, "plan_device", own, "bed " + f, torch.int32, self.device, (m,))
+                   for a, f in ((d.offsets, "offsets"), (d.heads, "heads"), (d.counts, "counts"))]
+            bgs.append(_lib.SsBgStream(slot=i, pool=d.pool._h.value, ids_dev=ids, offsets_dev=ptr[0], heads_dev=ptr[1],
+                                       counts_dev=ptr[2], m=m))
+        return (_lib.SsBgStream * len(bgs))(*bgs) if bgs else None
+
     @staticmethod
     def _device_pair_gains(sources):
         """The ss_pair_gains handles of a plan's dry picks (the order of _device_dry), or None when no pick has gains."""
@@ -1147,6 +1196,9 @@ class Renderer:
                     raise ValueError("plan_device: speaker %d of draw %d does not take its window start from the "
                                      "draw's start tensor" % (v, k))
                 dry = sources[v].dry
+                if isinstance(dry, BackgroundStream):
+                    raise ValueError("plan_device: speaker %d of draw %d is a bed slot (BackgroundStream): the draws "
+                                     "test speakers only" % (v, k))
                 if isinstance(dry, (DryPick, DryStream)):
                     if not dry.pool.levels:
                         raise ValueError("plan_device: speaker %d of draw %d: its DryPool has no level tables "
@@ -1295,8 +1347,9 @@ class Renderer:
             raise ValueError("a window start on the device was outside [0, N - length]; the window was clamped into "
                              "that range")
         if bits.value & 32:
-            raise ValueError("a DryStream layout on the device held an invalid entry (an id >= n, a negative offset or "
-                             "an offset before the end of the previous utterance); it was skipped")
+            raise ValueError("a DryStream or BackgroundStream layout on the device held an invalid entry (an id >= n, a "
+                             "negative offset, a head and count outside the clip or an offset before the end of the "
+                             "previous entry); it was skipped")
 
     def launch_count(self) -> int:
         return int(self.lib.ss_launch_count(self.ctx))
@@ -1322,19 +1375,21 @@ class DevicePlan:
     descriptors, block tables and scratch resident on the device, the launches captured into a CUDA graph.  With
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
     dry-picked slots take their dry signals from dry pools, with pair gains their gains from pair-gain tables; with
-    dereverberation targets its mixtures also write those, and with stream slots it lays out their dry streams.  Every
-    plan is created by ss_plan_create_stream, with NULL and a count of 0 for each part it does not have."""
+    dereverberation targets its mixtures also write those, with stream slots it lays out their dry streams and with bed
+    slots their noise and music beds.  Every plan is created by ss_plan_create_bg, with NULL and a count of 0 for each
+    part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
-                 streams=None):
+                 streams=None, bgs=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
+        self.bgs = bgs
         self._plan = ctypes.c_void_p()
         if n > 0:
-            _lib.check(renderer.lib.ss_plan_create_stream(
+            _lib.check(renderer.lib.ss_plan_create_bg(
                 renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
                 pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
-                len(streams) if streams else 0, ctypes.byref(self._plan)))
+                len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
