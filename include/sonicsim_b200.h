@@ -335,7 +335,8 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * 0 to N (checked for grid-blocked sources), bit 2 (version 104) = a moving window's start outside [0, N - win_len]
  * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped), bit 4 (dry
  * pools, below) = a dry pick outside [0, n) of its dry pool (clamped), bit 5 (dry streams and background streams,
- * below) = an invalid entry of a stream or bed slot's layout (skipped).  The Python device API raises IndexError /
+ * below) = an invalid entry of a stream or bed slot's layout (skipped), bit 6 (loudness slots, ss_stream_lufs below) =
+ * a loudness target read at a run that was not finite (that slot stored unscaled).  The Python device API raises IndexError /
  * ValueError from it on request
  * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
  * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
@@ -797,6 +798,53 @@ int ss_plan_create_bg(ss_ctx* ctx, const ss_source* items, int n_items, const ss
                       const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                       int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
                       ss_plan** out);
+
+/* ---- loudness slots: a stream or bed slot stored at SonicSet's loudness (SonicSet.py:97-101, get_lufs_norm_audio over
+ * the whole 60 s stem), measured at every run.  A stream or bed has no fixed (dry signal, trajectory) pair to measure
+ * once, so the plan renders the slot's whole stem at every run and measures it there.  At every run, inside the plan's
+ * single graph launch, a loudness slot:
+ *   1. renders its whole stem [0, N) - the picked candidate with the layout of that run - into plan-owned scratch,
+ *      through the staging (k_stage) and render kernels every pooled slot uses (the slot's window is not rendered);
+ *   2. measures it with the launches of ss_loudness_dev (k_kweight, k_kw_scan) over gating tables uploaded once;
+ *   3. k_loud_gate<true> reads *target_dev and computes (LUFS, gain) with the float64 arithmetic of ss_render_host_ex
+ *      (-inf LUFS is gained as -40) into result_dev, or plan scratch without one;
+ *   4. k_loud_crop writes the slot's crop as whole[:, start : start + win_len] * (float)gain, one float32 multiply
+ *      rounded once (k_loud_scale's arithmetic), and the direct-path crop of a slot with SS_DIRECT_TARGET with the same
+ *      gain.  The start is the slot's (win_start, or *win_start_dev clamped into [0, N - win_len]: bit 2).
+ * So the stem and direct stem of every run equal, bit for bit, the crop at that start of ss_render_host_ex of the
+ * picked candidate with the stream or bed assembled by that run's layout and target_lufs = *target_dev, and result_dev
+ * receives what that call's result receives.  A non-finite target stores the slot unscaled (gain 1), its result is
+ * (LUFS, NaN) and ss_device_errors reports bit 6.  Draws, mixtures, rms_db and dereverberation targets read the
+ * normalised crops; the draws still test a stream speaker's dry crop, so starts and `used` keep their bits.
+ * Order within a run: draws, staging and renders, the six measuring launches, k_loud_crop, then the mixtures: a plan
+ * with loudness slots launches 7 kernels per run more than the same plan without them, plus one launch group (k_blocks,
+ * k_prepare, k_render) for every further chunk its whole stems take under the chunk budget (ss_set_chunk_bytes).  A
+ * plan without loudness slots launches exactly as ss_plan_create_bg's.  Scratch, allocated at creation: per slot C * N
+ * floats (twice that with SS_DIRECT_TARGET), SS_LOUD_SCRATCH_DOUBLES * C * n_e doubles and, without result_dev, two
+ * doubles; and the gating tables, once per distinct plan.
+ *   - gating: the slot's gating plan over N samples (brk / blk_lo / blk_hi, n_e, n_blocks, rate, block_size) as for
+ *     ss_render_host_ex; target_lufs and result are ignored.  Every entry has one rate.
+ *   - target_dev: device, one double, read at every run.  result_dev: NULL, or device, two doubles written at every run.
+ * ss_plan_create_lufs is ss_plan_create_bg with n_lufs entries (n_lufs == 0: exactly ss_plan_create_bg).  Refused at
+ * creation, before anything is allocated and with *out untouched:
+ *   - SS_ERR_INVALID: n_lufs < 0 or NULL lufs with n_lufs > 0; a slot outside [0, n_items), that is not a stream or bed
+ *     slot (ss_dry_stream, ss_bg_stream) or is named twice; a NULL brk, entries that the checks of ss_post_lufs refuse,
+ *     a brk that is not ascending from 0 with brk[n_e] <= N, or a gating block outside [0, n_e]; a NULL or unaligned
+ *     target_dev, an unaligned result_dev; a result_dev range that meets anything else the plan reads or writes;
+ *   - SS_ERR_UNSUPPORTED: a slot of a host pool (SS_BANK_HOST, spectra or taps: a whole stem would stage every bank
+ *     row over PCIe at every run), a slot pool whose candidates differ in N, C > 8.
+ * ss_version stays 108: the export marks the capability. */
+typedef struct {
+    int32_t slot;                     /* index into `items`: a stream or bed slot                                     */
+    ss_post_lufs gating;              /* host gating plan of the slot's N; target_lufs and result ignored             */
+    const double* target_dev;         /* device, the target LUFS, read at every run                                  */
+    double* result_dev;               /* device, (LUFS, gain) written at every run, or NULL                          */
+} ss_stream_lufs;
+int ss_plan_create_lufs(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                        const ss_stream_lufs* lufs, int n_lufs, ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

@@ -101,6 +101,13 @@ GatingTables gating_tables(const ss_post_lufs* post, int n);
 // out = data normalises the stem in place, NULL measures only.  `scratch`: loud_scratch_bytes(q, C).
 ss_loud_item loud_item(const ss_post_lufs& q, const char* tab, const float* data, float* out, int32_t N, int32_t C,
                        double* scratch, double* result);
+// Loudness slots of plans (ss_stream_lufs): the device descriptor of item `a` (target_dev left null), and the measuring
+// launches of ss_loudness_dev - k_kweight, k_kw_scan, k_loud_gate<true>, six launches - over n_items descriptors already
+// in device memory, `prefix` their n_items + 1 work-item offsets (C * n_e each), all at one `rate`.
+namespace ss { struct LoudItem; }
+ss::LoudItem to_item(const ss_loud_item& a);
+int loud_measure_enqueue(ss_ctx* c, const ss::LoudItem* items, const int* prefix, int n_items, int total, double rate,
+                         cudaStream_t stream);
 inline size_t loud_scratch_bytes(const ss_post_lufs& q, int32_t C) {
     return align_up(8 * (size_t)SS_LOUD_SCRATCH_DOUBLES * C * q.n_e, 256);
 }

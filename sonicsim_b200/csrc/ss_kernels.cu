@@ -36,6 +36,7 @@
 
 #include "ss_internal.h"
 #include "ss_phases.cuh"
+#include "ss_loud.cuh"
 
 using namespace ss;
 
@@ -1193,6 +1194,7 @@ struct PlanSlot {
     const float* pair = nullptr;       // the device table of its pair gains, or null
     const ss_dry_stream* strm = nullptr;
     const ss_bg_stream* bg = nullptr;
+    const ss_stream_lufs* lufs = nullptr;   // a loudness slot's target (validate_lufs), or null
     StageView* view = nullptr;
     const DryStream* ws = nullptr;
     const BgStream* wb = nullptr;
@@ -2484,6 +2486,13 @@ struct ss_plan {
     const Source* d_tap_src = nullptr;
     const int* d_tap_prefix = nullptr;
     int n_tap = 0, tap_ctas = 0;
+    // loudness slots (ss_stream_lufs): their measuring descriptors (k_kweight, k_kw_scan, k_loud_gate<true>) and work-item
+    // offsets, and their crops (k_loud_crop), in d_desc
+    const LoudItem* d_loud = nullptr;
+    const int* d_loud_prefix = nullptr;
+    const LoudCrop* d_crop = nullptr;
+    int n_loud = 0, loud_total = 0, crop_ctas = 0;
+    double loud_rate = 0;
 };
 
 // ----------------------------------------------------------------------------- k_draw
@@ -2752,6 +2761,36 @@ __global__ void __launch_bounds__(256) k_stage(const StageSlot* __restrict__ slo
     }
 }
 
+// ----------------------------------------------------------------------------- k_loud_crop
+// The crops of a plan's loudness slots, after their whole stems were measured: one gridDim.y row per slot, the crop
+// and the direct-path crop cut out of the whole stems at the slot's start and scaled by the gain of the run
+// (loud_crop_head), float4 at a time when the whole stem, the start, the length and the outputs allow it.
+__global__ void __launch_bounds__(256) k_loud_crop(const LoudCrop* __restrict__ crops) {
+    const LoudCrop& q = crops[blockIdx.y];
+    int start;
+    float g;
+    const unsigned err = loud_crop_head(q, start, g);
+    if (err && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(&g_dev_err, err);
+    const long long total = (long long)q.C * q.len, stride = (long long)gridDim.x * blockDim.x;
+    const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (int dir = 0; dir < 2; ++dir) {
+        const float* const src = dir ? q.whole_dir : q.whole;
+        float* const dst = dir ? q.out_dir : q.out;
+        if (!dst) continue;
+        if (((q.N | start | q.len) & 3) == 0 && (((uintptr_t)src | (uintptr_t)dst) & 15) == 0) {
+            const long long row4 = q.len >> 2;
+            for (long long i = i0; i < total >> 2; i += stride) {
+                const long long c = i / row4, t = i - c * row4;
+                float4 v = reinterpret_cast<const float4*>(src + c * q.N + start)[t];
+                v.x *= g; v.y *= g; v.z *= g; v.w *= g;
+                reinterpret_cast<float4*>(dst)[i] = v;
+            }
+        } else {
+            for (long long i = i0; i < total; i += stride) dst[i] = loud_crop_sample(q, start, g, dir, i);
+        }
+    }
+}
+
 extern "C" void ss_plan_destroy(ss_plan* p) {
     if (!p) return;
     cudaSetDevice(p->c->device);
@@ -2836,9 +2875,12 @@ static StageArea stage_area_of(const ss_source& it) {
 // Lay out, fill and upload a plan's descriptors.  The host fills one image, each section at a 256-byte boundary: the
 // chunk descriptors, the mixtures' MixItems, the draws' DrawDescs, the staged slots' StageSlots, the tap block
 // (tap_block, with slots of tap-form pools), the streams' DryStreams and the beds' BgStreams (caller order) and the
-// clip lengths of each dry pool the streams and beds use; one copy uploads it.  Behind the image, written by the device
-// only and never uploaded: one scratch block per mixture, then the staged slots' staging areas.  slots[i] is caller
-// item i's record; plan_build notes where its view, its DryStream and its BgStream landed.
+// clip lengths of each dry pool the streams and beds use, and for loudness slots their LoudItems, work-item offsets,
+// LoudCrops and gating tables; one copy uploads it.  Behind the image, written by the device only and never uploaded:
+// one scratch block per mixture, the staged slots' staging areas, then per loudness slot its whole stems, its loudness
+// scratch and (without a result_dev) its result.  slots[i] is caller item i's record; plan_build notes where its view,
+// its DryStream and its BgStream landed.  A loudness slot is chunked, staged and rendered as the window [0, N) into its
+// whole stems; draws and mixtures keep reading the caller's item, whose crop k_loud_crop writes.
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes,
                       std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix, const ss_plan_draw* draws,
                       int n_draws) {
@@ -2847,7 +2889,17 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     std::vector<int> cuts, order;
     std::vector<ss_source> arranged;
     std::vector<Shape> arranged_shapes;
-    arrange_chunks(c, caller_items, caller_shapes, n_items, arranged, arranged_shapes, cuts, &order);
+    std::vector<ss_source> rendered(caller_items, caller_items + n_items);   // loudness slots: the window [0, N)
+    std::vector<Shape> rendered_shapes(caller_shapes, caller_shapes + n_items);
+    std::vector<int> loud;                               // the loudness slots, in caller order
+    for (int i = 0; i < n_items; ++i) {
+        if (!slots[i].lufs) continue;
+        ss_source& w = rendered[i];
+        w.win_start = 0; w.win_start_dev = nullptr; w.win_len = w.pool->host[0].N;
+        rendered_shapes[i] = shape_pooled(w);
+        loud.push_back(i);
+    }
+    arrange_chunks(c, rendered.data(), rendered_shapes.data(), n_items, arranged, arranged_shapes, cuts, &order);
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
     std::vector<PlanSlot*> rec(arranged.size());         // rec[i]: the record of arranged item i
     std::vector<int> staged;    // arranged items that are slots of host pools, host or 16-bit dry picks, stream and bed
@@ -2888,11 +2940,29 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
             wpools.push_back(s.clips());
             wlen_off.push_back(take(sizeof(int32_t) * (size_t)s.clips()->n));
         }
+    const int n_loud = (int)loud.size();
+    std::vector<ss_post_lufs> gating(n_loud);
+    for (int k = 0; k < n_loud; ++k) gating[k] = slots[loud[k]].lufs->gating;
+    const GatingTables gtabs = gating_tables(gating.data(), n_loud);
+    const size_t loud_off = take(sizeof(LoudItem) * n_loud);
+    const size_t lpre_off = take(sizeof(int) * (n_loud + 1));
+    const size_t crop_off = take(sizeof(LoudCrop) * n_loud);
+    const size_t gtab_off = take(gtabs.bytes.size());
     const size_t image = at;
     const size_t scr_bytes = sizeof(double) * (size_t)ss_mix_scratch_doubles();
     const size_t scr_off = take(scr_bytes * mix.size());
     std::vector<size_t> area_off(staged.size());
     for (size_t k = 0; k < staged.size(); ++k) area_off[k] = take(stage_area_of(items[staged[k]]).end);
+    // a loudness slot's whole stem (C * N floats), its whole direct-path stem, loudness scratch and result
+    std::vector<size_t> whole_off(n_items), wdir_off(n_items), lscr_off(n_loud), lres_off(n_loud);
+    for (int k = 0; k < n_loud; ++k) {
+        const ss_source& w = rendered[loud[k]];
+        const size_t stem = sizeof(float) * (size_t)w.C * w.win_len;
+        whole_off[loud[k]] = take(stem);
+        if (w.flags & SS_DIRECT_TARGET) wdir_off[loud[k]] = take(stem);
+        lscr_off[k] = take(loud_scratch_bytes(gating[k], w.C));
+        if (!slots[loud[k]].lufs->result_dev) lres_off[k] = take(2 * sizeof(double));
+    }
     CK(cudaEventCreateWithFlags(&p->ev_fork, cudaEventDisableTiming));
     for (int i = 0; i < ss_ctx::kAux; ++i) CK(cudaEventCreateWithFlags(&p->ev_join[i], cudaEventDisableTiming));
     CK(cudaStreamCreateWithFlags(&p->s_cap, cudaStreamNonBlocking));
@@ -2901,6 +2971,40 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         if (scratch_need[i]) CK(cudaMalloc((void**)&p->d_scratch[i], align_up(scratch_need[i], 1 << 20)));
     char* const d = p->d_desc;
     std::vector<char> host(image, 0);
+    for (size_t i = 0; i < arranged.size(); ++i) {       // loudness slots render into their whole stems
+        if (!rec[i]->lufs) continue;
+        arranged[i].out = (float*)(d + whole_off[order[i]]);
+        if (arranged[i].flags & SS_DIRECT_TARGET) arranged[i].out_direct = (float*)(d + wdir_off[order[i]]);
+    }
+    if (n_loud) {
+        if (!gtabs.bytes.empty()) memcpy(host.data() + gtab_off, gtabs.bytes.data(), gtabs.bytes.size());
+        int* const prefix = (int*)(host.data() + lpre_off);
+        int total = 0;
+        for (int k = 0; k < n_loud; ++k) {
+            const int i = loud[k];
+            const ss_stream_lufs& q = *slots[i].lufs;
+            const ss_source& w = rendered[i];
+            const ss_source& a = caller_items[i];
+            double* const result = q.result_dev ? q.result_dev : (double*)(d + lres_off[k]);
+            const float* const whole = (const float*)(d + whole_off[i]);
+            const float* const wdir = (w.flags & SS_DIRECT_TARGET) ? (const float*)(d + wdir_off[i]) : nullptr;
+            LoudItem it = to_item(loud_item(q.gating, d + gtab_off + gtabs.at[k], whole, nullptr, w.win_len, w.C,
+                                            (double*)(d + lscr_off[k]), result));
+            it.target_dev = q.target_dev;
+            memcpy(host.data() + loud_off + sizeof(LoudItem) * k, &it, sizeof(it));
+            const LoudCrop crop = {whole, wdir, a.out, wdir ? a.out_direct : nullptr, a.win_start_dev, q.target_dev,
+                                   result, a.win_start, a.win_len, w.win_len, w.C};
+            memcpy(host.data() + crop_off + sizeof(LoudCrop) * k, &crop, sizeof(crop));
+            prefix[k] = total;
+            total += w.C * q.gating.n_e;
+            p->crop_ctas = std::max(p->crop_ctas, (int)std::min<long long>(64, ((long long)w.C * a.win_len + 1023) / 1024));
+        }
+        prefix[n_loud] = total;
+        p->d_loud = (const LoudItem*)(d + loud_off);
+        p->d_loud_prefix = (const int*)(d + lpre_off);
+        p->d_crop = (const LoudCrop*)(d + crop_off);
+        p->n_loud = n_loud; p->loud_total = total; p->loud_rate = gating[0].rate;
+    }
     for (int i = 0, k = 0, kb = 0; i < n_items; ++i) {   // the streams and beds first: staged slots and draws name them
         const ss_dry_pool* dp = slots[i].clips();
         if (!dp) continue;
@@ -3121,6 +3225,10 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
                 add_range(r, a, 4 * (uint64_t)s.bg->m, false);
             if (std::find(dpools.begin(), dpools.end(), s.bg->pool) == dpools.end()) dpools.push_back(s.bg->pool);
         }
+        if (s.lufs) {                                       // a loudness slot reads its target, writes its result
+            add_range(r, s.lufs->target_dev, 8, false);
+            add_range(r, s.lufs->result_dev, 16, true);
+        }
     }
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
         if (!dp->padded())
@@ -3195,6 +3303,40 @@ static int validate_bgs(const ss_ctx* c, const ss_source* items, const ss_bg_str
     return SS_OK;
 }
 
+// A plan's loudness slots (include/sonicsim_b200.h, ss_stream_lufs), all but the byte ranges (validate_mixes): the
+// record of each slot receives its entry.  After validate_streams and validate_bgs, which name the stream and bed slots.
+static int validate_lufs(const ss_source* items, const ss_stream_lufs* lufs, int n_lufs, std::vector<PlanSlot>& slots) {
+    std::vector<ss_post_lufs> post(n_lufs);
+    for (int k = 0; k < n_lufs; ++k) {
+        const ss_stream_lufs& q = lufs[k];
+        if (q.slot < 0 || q.slot >= (int)slots.size()) return SS_ERR_INVALID;
+        const PlanSlot& r = slots[q.slot];
+        if (r.lufs || !(r.strm || r.bg) || !q.gating.brk || !q.target_dev || ((uintptr_t)q.target_dev & 7) ||
+            ((uintptr_t)q.result_dev & 7))
+            return SS_ERR_INVALID;
+        for (int j = 0; j < k; ++j) if (lufs[j].slot == q.slot) return SS_ERR_INVALID;
+        post[k] = q.gating;
+    }
+    if (check_post_lufs(post.data(), n_lufs)) return SS_ERR_INVALID;
+    for (int k = 0; k < n_lufs; ++k) {
+        // a device pool (a whole stem of a host pool would stage every bank row at every run) of one N, C <= 8
+        const ss_pool* pl = items[lufs[k].slot].pool;
+        if (pl->host_res || pl->C > 8) return SS_ERR_UNSUPPORTED;
+        for (const PoolEntry& e : pl->host) if (e.N != pl->host[0].N) return SS_ERR_UNSUPPORTED;
+    }
+    for (int k = 0; k < n_lufs; ++k) {
+        // gating tables inside the whole stem: k_kweight reads samples [brk[0], brk[n_e]), k_loud_gate intervals
+        const ss_post_lufs& g = lufs[k].gating;
+        const int N = items[lufs[k].slot].pool->host[0].N;
+        if (g.brk[0] != 0 || g.brk[g.n_e] > N) return SS_ERR_INVALID;
+        for (int e = 0; e < g.n_e; ++e) if (g.brk[e + 1] < g.brk[e]) return SS_ERR_INVALID;
+        for (int j = 0; j < g.n_blocks; ++j)
+            if (g.blk_lo[j] < 0 || g.blk_hi[j] < g.blk_lo[j] || g.blk_hi[j] > g.n_e) return SS_ERR_INVALID;
+    }
+    for (int k = 0; k < n_lufs; ++k) slots[lufs[k].slot].lufs = &lufs[k];
+    return SS_OK;
+}
+
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
 // and the byte ranges (validate_mixes): mix receives the mixtures, each with its target's direct_out, or null
 static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan_target* targets, int n_targets,
@@ -3213,10 +3355,10 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
-                       ss_plan** out) {
+                       const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
     auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
     if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
-        bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs))
+        bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs) || bad(lufs, n_lufs))
         return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
@@ -3226,6 +3368,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     { int st = validate_dry_picks(c, items, picks, pair_gains, n_picks, slots); if (st) return st; }
     { int st = validate_streams(c, items, streams, n_streams, slots); if (st) return st; }
     { int st = validate_bgs(c, items, bgs, n_bgs, draws, n_draws, slots); if (st) return st; }
+    { int st = validate_lufs(items, lufs, n_lufs, slots); if (st) return st; }
     { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
     { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
     { int st = validate_mixes(items, slots, mix, draws, n_draws); if (st) return st; }
@@ -3248,26 +3391,26 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
     return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                       out);
+                       nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                       0, out);
+                       0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
-                       0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3275,7 +3418,7 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3283,7 +3426,7 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, nullptr, 0, out);
+                       streams, n_streams, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
@@ -3292,14 +3435,23 @@ extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items,
                                  int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                  int n_bgs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, out);
+                       streams, n_streams, bgs, n_bgs, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                   const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                   int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
+                                   int n_bgs, const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
-                       nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
@@ -3312,8 +3464,8 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, bool stre
     return SS_OK;
 }
 
-// the start draws, the host-pool staging, the launches of every chunk (run_chunks), then the mixtures (which read every
-// chunk's outputs) on `stream`
+// the start draws, the host-pool staging, the launches of every chunk (run_chunks), the loudness slots' measurements
+// and crops, then the mixtures (which read every chunk's outputs and the crops) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
     if (p->n_draw) {
@@ -3344,6 +3496,13 @@ static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
         return chunk_enqueue(c, p->chunks[k], s, c->profiling);
     });
     if (rc) return rc;
+    if (p->n_loud) {                                    // loudness slots: measure the whole stems, then cut the crops
+        const int st = loud_measure_enqueue(c, p->d_loud, p->d_loud_prefix, p->n_loud, p->loud_total, p->loud_rate, stream);
+        if (st) return st;
+        k_loud_crop<<<dim3(p->crop_ctas, p->n_loud), 256, 0, stream>>>(p->d_crop);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
     return p->n_mix ? mix_enqueue(c, p->d_mix, p->n_mix, stream, p->mix_direct) : SS_OK;
 }
 

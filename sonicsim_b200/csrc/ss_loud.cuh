@@ -45,10 +45,13 @@ struct LoudItem {
                              // the K-weighted signal), then the per-interval filter states of the three passes below
     double* result;          // [0] integrated loudness (LUFS, -inf allowed), [1] linear gain applied
     long long stride_n, stride_c;
-    int N, C, n_e, n_blocks, pad_[2];
+    int N, C, n_e, n_blocks;
+    const double* target_dev;   // k_loud_gate<true> (loudness slots of plans): the target LUFS, read at every run;
+                                // null elsewhere (in the bytes that were padding, so that the layout is unchanged)
     double inv_norm;         // 1 / (T_g * rate)
     double target;           // target LUFS (SonicSim_audio.py:77 `norm`)
 };
+static_assert(sizeof(LoudItem) == 112, "LoudItem layout");
 constexpr int kLoudScratch = 20;   // doubles of scratch per (channel, elementary interval)
 
 // ---- K-weighting of one channel, EXACT and parallel over the elementary intervals.
@@ -150,6 +153,13 @@ SS_HD void kweight_pass(const LoudItem& it, const KCoef& k, int c, int e) {
     kw_end<PASS>(it, k, c, e, st);
 }
 
+// The result of a stem whose target is read on the device (a plan's loudness slot, ss_stream_lufs): the gain of
+// loudness_gate for a finite target; NaN for a non-finite one, whose slot is stored unscaled (loud_crop_gain).
+SS_HD void loud_result_dev(double lufs, double target, double* result) {
+    const double used = isinf(lufs) ? -40.0 : lufs;                                    // SonicSim_audio.py:73-75
+    result[0] = lufs;
+    result[1] = isfinite(target) ? pow(10.0, (target - used) / 20.0) : NAN;           // pyln.normalize.loudness
+}
 SS_HD double channel_gain(int c) { return (c == 3 || c == 4) ? 1.41 : 1.0; }   // pyloudnorm G = [1,1,1,1.41,1.41]
 
 // Gating (pyloudnorm meter.py integrated_loudness) for one stem; single thread.
@@ -183,6 +193,7 @@ SS_HD void loudness_gate(const LoudItem& it) {
     double s = 0;
     for (int c = 0; c < C; ++c) s += channel_gain(c) * (cnt ? zsum[c] / cnt : 0.0);   // nan_to_num(mean of empty) = 0
     double lufs = -0.691 + 10.0 * log10(s);                                            // log10(0) = -inf
+    if (it.target_dev) { loud_result_dev(lufs, *it.target_dev, it.result); return; }   // (k_loud_gate<true>)
     double used = isinf(lufs) ? -40.0 : lufs;                                          // SonicSim_audio.py:73-75
     it.result[0] = lufs;
     it.result[1] = pow(10.0, (it.target - used) / 20.0);                              // pyln.normalize.loudness

@@ -135,6 +135,9 @@ __device__ __forceinline__ double gate_reduce(double v, double* sh) {
     for (int w = 0; w < kGateThreads / 32; ++w) r += sh[w];
     return r;                                            // the same value in every thread
 }
+// k_loud_gate<true> (the loudness slots of plans) reads each item's target from target_dev at every run
+// (loud_result_dev): a non-finite target gives the gain NaN.
+template <bool DEV_TARGET = false>
 __global__ void __launch_bounds__(kGateThreads) k_loud_gate(const LoudItem* __restrict__ items, int n_items) {
     __shared__ double sh[kGateThreads / 32];
     const LoudItem& it = items[blockIdx.x];
@@ -178,6 +181,7 @@ __global__ void __launch_bounds__(kGateThreads) k_loud_gate(const LoudItem* __re
         if (pass == 0) gamma_r = -0.691 + 10.0 * log10(s) - 10.0;
         else if (threadIdx.x == 0) {
             const double lufs = -0.691 + 10.0 * log10(s);                      // log10(0) = -inf
+            if (DEV_TARGET) { loud_result_dev(lufs, *it.target_dev, it.result); return; }
             const double used = isinf(lufs) ? -40.0 : lufs;                     // SonicSim_audio.py:73-75
             it.result[0] = lufs;
             it.result[1] = pow(10.0, (it.target - used) / 20.0);               // pyln.normalize.loudness
@@ -203,6 +207,23 @@ k_loud_scale(const LoudItem* __restrict__ items) {
     }
 }
 
+// Internal (ss_internal.h): the measuring launches of ss_loudness_dev over n_items descriptors already in device memory,
+// with k_loud_gate<true>: six launches, asynchronous on `stream`.
+int loud_measure_enqueue(ss_ctx* c, const LoudItem* items, const int* prefix, int n_items, int total, double rate,
+                         cudaStream_t stream) {
+    const KCoef k = make_kcoef(rate);
+    const dim3 scan_grid(8, n_items);
+    k_kweight<1><<<(total + 127) / 128, 128, 0, stream>>>(items, prefix, n_items, k);
+    k_kw_scan<<<scan_grid, 32, 0, stream>>>(items, 0);
+    k_kweight<2><<<(total + 127) / 128, 128, 0, stream>>>(items, prefix, n_items, k);
+    k_kw_scan<<<scan_grid, 32, 0, stream>>>(items, 1);
+    k_kweight<3><<<(total + 127) / 128, 128, 0, stream>>>(items, prefix, n_items, k);
+    k_loud_gate<true><<<n_items, kGateThreads, 0, stream>>>(items, n_items);
+    CK(cudaGetLastError());
+    c->launches += 6;
+    return SS_OK;
+}
+
 // (stride_n, stride_c) describe a dense (N, C) or (C, N) block of N*C floats: k_loud_scale writes `out` as the N*C
 // floats that follow it, so that is the only layout in which out[q] = gain * data[q] scales element (n, c) in place.
 static bool dense_layout(int64_t N, int64_t C, int64_t sn, int64_t sc) {
@@ -217,7 +238,7 @@ static int validate_loud(const ss_loud_item& it) {
     return SS_OK;
 }
 
-static LoudItem to_item(const ss_loud_item& a) {
+LoudItem to_item(const ss_loud_item& a) {
     LoudItem it;
     memset(&it, 0, sizeof(it));
     it.data = a.data; it.out = a.out; it.brk = a.brk; it.blk_lo = a.blk_lo; it.blk_hi = a.blk_hi;

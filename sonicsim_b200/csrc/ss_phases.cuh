@@ -237,6 +237,41 @@ SS_HD int clamp_win_start(int v, int N, int win_len, bool& bad) {
 // a windowed source's moving start (counts[6..7], 8-byte aligned), or null: the start is counts[4]
 SS_HD const int* win_start_ptr(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 6); }
 
+// ---- loudness slots of plans (ss_stream_lufs): a stream or bed slot is rendered whole, [0, N), into plan scratch,
+// measured there at every run (k_kweight, k_kw_scan, k_loud_gate<true>), and k_loud_crop cuts its crop out of the
+// whole stem with the gain of that run.  One descriptor per slot:
+struct LoudCrop {
+    const float* whole;        // (C, N) the slot's whole stem ...
+    const float* whole_dir;    // ... and its whole direct-path stem, or null
+    float* out;                // (C, len) the slot's crop ...
+    float* out_dir;            // ... and its direct-path crop, or null
+    const int* ws_dev;         // the slot's moving start, or null: ws
+    const double* target;      // the target LUFS, read at every run
+    const double* result;      // (LUFS, gain) that k_loud_gate<true> wrote at this run
+    int ws, len, N, C;
+};
+// Head of k_loud_crop: the crop's start, clamped as a pooled window's start is (bit 2), and the float32 gain of the
+// crops, (float)result[1] as k_loud_scale takes it, or 1 with bit 6 for a non-finite target (stored unscaled).
+// Returns the error bits.
+SS_HD unsigned loud_crop_head(const LoudCrop& q, int& start, float& g) {
+    unsigned err = 0;
+    start = q.ws;
+    if (q.ws_dev) {
+        bool bad;
+        start = clamp_win_start(*q.ws_dev, q.N, q.len, bad);
+        if (bad) err |= 4u;
+    }
+    const double t = *q.target;
+    if (isfinite(t)) g = (float)q.result[1];
+    else { g = 1.0f; err |= 64u; }
+    return err;
+}
+// element i of set `dir` (0: the stem, 1: the direct-path stem) of a crop: channel i / len, sample i % len
+SS_HD float loud_crop_sample(const LoudCrop& q, int start, float g, int dir, long long i) {
+    const long long c = i / q.len, t = i - c * q.len;
+    return (dir ? q.whole_dir : q.whole)[c * q.N + start + t] * g;
+}
+
 // ---- source pools (ss_pool, include/sonicsim_b200.h).  A pooled slot is a windowed source whose candidate is picked on
 // the device at every run: the head of k_blocks reads the pick, clamps it and writes the candidate's fields into the
 // slot's Source (pick_candidate) before anything reads them.  One compact entry per candidate in the pool's table:

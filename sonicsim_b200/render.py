@@ -110,7 +110,13 @@ class DryPick(T.NamedTuple):
     gains: T.Any = None
 
 
-class DryStream(T.NamedTuple):
+class _DryStreamFields(T.NamedTuple):
+    pool: T.Any
+    ids: T.Any
+    offsets: T.Any
+
+
+class DryStream(_DryStreamFields):
     """The dry signal of a pooled slot (Pooled.dry) laid out at every run from utterances, as create_long_audio lays
     out a speech stream (SonicSim_audio.py:231-277): `pool` a 16-bit DryPool of n utterances (dry_pool(...,
     dtype="int16")), `ids` and `offsets` contiguous 1-D CUDA int32 tensors of equal length m, 1 <= m <= 128 (e.g. rows
@@ -120,10 +126,25 @@ class DryStream(T.NamedTuple):
     [offset, offset + its length) of the stream.  The slot renders its picked candidate with the stream's first N
     samples, zeros where no utterance lies (an utterance reaching past N is cut there): bit for bit a DryPick from a
     16-bit pool holding the assembled stream.  A stream speaker of a CropDraw is tested on its crop's energy, summed per
-    utterance from the pool's level tables (dry_pool(..., levels=True)).  Pools with loudness gains take no streams."""
-    pool: T.Any
-    ids: T.Any
-    offsets: T.Any
+    utterance from the pool's level tables (dry_pool(..., levels=True)).  Pools with loudness gains take no streams.
+    `lufs`, a StemLoudness, stores the slot's crops at SonicSet's loudness, measured over the whole stem at every run.
+    It is a keyword attribute outside the tuple: a DryStream stays the (pool, ids, offsets) tuple that callers unpack,
+    compare and rebuild (_replace and repr carry `lufs`; tuple equality does not look at it)."""
+
+    def __new__(cls, pool, ids, offsets, lufs=None):
+        self = super().__new__(cls, pool, ids, offsets)
+        self.lufs = lufs
+        return self
+
+    def _replace(self, **kw):
+        lufs = kw.pop("lufs", self.lufs)
+        return DryStream(*super()._replace(**kw), lufs=lufs)
+
+    def __repr__(self):
+        return "%s, lufs=%r)" % (super().__repr__()[:-1], self.lufs)
+
+    def __getnewargs__(self):
+        return tuple(self) + (self.lufs,)
 
 
 class BackgroundStream(T.NamedTuple):
@@ -136,12 +157,34 @@ class BackgroundStream(T.NamedTuple):
     (check_device_errors raises ValueError); any other places clip samples [head, head + count) at stream samples
     [offset, offset + count).  The slot renders its picked candidate with the stream's first N samples, zeros where no
     clip lies: bit for bit a DryPick from a pool of the same dtype holding the assembled bed.  A bed slot may read a
-    CropDraw's start but is none of its speakers; pools with loudness gains take no beds."""
+    CropDraw's start but is none of its speakers; pools with loudness gains take no beds.  `lufs`, a StemLoudness,
+    stores the slot's crops at SonicSet's loudness, measured over the whole stem at every run."""
     pool: T.Any
     ids: T.Any
     offsets: T.Any
     heads: T.Any
     counts: T.Any
+    lufs: T.Any = None
+
+
+class StemLoudness(T.NamedTuple):
+    """The loudness target of a stream or bed slot (DryStream.lufs, BackgroundStream.lufs): SonicSet stores every stem
+    loudness-normalised over the whole stem (SonicSet.py:97-101, get_lufs_norm_audio), and a stream or bed laid out at
+    every run has no fixed stem to measure once.  At every run the plan renders the slot's whole stem [0, N), measures
+    it like render_host(..., lufs_targets=) and stores the slot's crop, and its direct-path crop, cut out of that stem and
+    scaled by the gain: bit for bit the crop at the run's start of render_host(..., lufs_targets=[target]) of the
+    picked candidate with the stream or bed that run lays out.  `target`: a one-element CUDA float64 tensor read at
+    every run (e.g. lufs[b, k] of a (B, K) tensor refreshed with uniform_(-19, -15) before run()); a non-finite target
+    stores the slot unscaled (check_device_errors raises ValueError).  `result`: None, or a contiguous two-element CUDA
+    float64 tensor that receives (measured LUFS, linear gain) at every run (gain NaN for a non-finite target).  `sr`:
+    the rate of the gating plan, built once from the pool's N.  The slot's SourcePool must be device-resident, without
+    loudness gains, with C <= 8 and every candidate of one N (SonicSet's stems are all 60 s); every loudness slot of a
+    plan has one sr.  Each slot adds C * N floats of plan scratch (twice that with direct_taps) and 20 * C doubles
+    per 0.1 s of its N; a plan with such slots launches 7 kernels more per run, plus a launch group per further chunk its
+    whole stems take."""
+    target: T.Any
+    result: T.Any = None
+    sr: float = 16000.0
 
 
 class CropDraw(T.NamedTuple):
@@ -547,6 +590,15 @@ def _as_i16(x, own, device, keep):
         raise ValueError("dry_pool: %s must be int16 or float on the int16 grid, got %s" % (own, a.dtype))
     keep.append(a)
     return a.ctypes.data, a.size
+
+
+def _cuda_tensors(obj):
+    """Every CUDA tensor in `obj`, a nesting of tuples (NamedTuples included) and lists."""
+    if _is_tensor(obj):
+        return [obj] if obj.is_cuda else []
+    if isinstance(obj, (tuple, list)):
+        return [t for v in obj for t in _cuda_tensors(v)]
+    return []
 
 
 def _check_usable(held, renderer, what):
@@ -1043,8 +1095,9 @@ class Renderer:
         targets = []
         mixes = self._device_mixes(mixtures, outs, keep, items, targets) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
+        lufs = self._device_lufs(sources, (outs, direct_outs, mixtures, draws), keep)
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
-                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs)
+                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1144,6 +1197,65 @@ class Renderer:
             bgs.append(_lib.SsBgStream(slot=i, pool=d.pool._h.value, ids_dev=ids, offsets_dev=ptr[0], heads_dev=ptr[1],
                                        counts_dev=ptr[2], m=m))
         return (_lib.SsBgStream * len(bgs))(*bgs) if bgs else None
+
+    def _device_lufs(self, sources, others, keep):
+        """Validated ss_stream_lufs array of a plan's loudness slots (StemLoudness of a DryStream or BackgroundStream),
+        or None without any; the gating plans are appended to `keep`.  `others`: the plan's other arguments, whose
+        tensors no result may meet."""
+        import torch
+        from .SonicSim_audio import gating_block_size, gating_plan
+        entries, held, rates = [], [], set()
+        for i, s in enumerate(sources):
+            d = getattr(s, "dry", None)
+            q = getattr(d, "lufs", None) if isinstance(d, (DryStream, BackgroundStream)) else None
+            if q is None:
+                continue
+            if not isinstance(q, StemLoudness):
+                raise ValueError("plan_device: the lufs of source %d must be a StemLoudness" % i)
+            pl = s.pool
+            if pl.resident != "device":
+                raise ValueError("plan_device: source %d has a loudness target over a host pool: its whole stem would "
+                                 "stage every bank row over PCIe at every run" % i)
+            if len(set(pl._sizes)) > 1:
+                raise ValueError("plan_device: source %d has a loudness target over a pool whose candidates differ in N "
+                                 "(%d to %d samples)" % (i, min(pl._sizes), max(pl._sizes)))
+            if pl.C > 8:
+                raise ValueError("plan_device: loudness normalisation supports at most 8 channels, the pool of source %d "
+                                 "has %d" % (i, pl.C))
+            own = "source %d" % i
+            target = _tensor(q.target, "plan_device", own, "loudness target", torch.float64, self.device, count=(1, 1))
+            result = (_tensor(q.result, "plan_device", own, "loudness result", torch.float64, self.device, count=(2, 2))
+                      if q.result is not None else None)
+            sr = float(q.sr)
+            if not sr > 0 or not math.isfinite(sr):
+                raise ValueError("plan_device: the sr of the loudness target of source %d must be > 0, got %r" % (i, q.sr))
+            rates.add(sr)
+            if len(rates) > 1:
+                raise ValueError("plan_device: the loudness targets of a plan must share one sr, got %s" % sorted(rates))
+            N = pl._sizes[0]
+            block = float(gating_block_size(N, sr))
+            brk, blo, bhi = gating_plan(N, sr, block)
+            keep.append((brk, blo, bhi))
+            gating = SsPostLufs(brk=brk.ctypes.data, blk_lo=blo.ctypes.data, blk_hi=bhi.ctypes.data, n_e=len(brk) - 1,
+                                n_blocks=len(blo), rate=sr, block_size=block)
+            entries.append(_lib.SsStreamLufs(slot=i, gating=gating, target_dev=target, result_dev=result))
+            held.append(q)
+        if not entries:
+            return None
+        # a result is written at every run: it meets no other tensor the plan reads or writes, nor another result
+        tensors = {id(t): t for t in _cuda_tensors((sources, others, held))}
+        spans = [(k, t.data_ptr(), t.data_ptr() + t.numel() * t.element_size()) for k, t in tensors.items()]
+        seen = []
+        for e, q in zip(entries, held):
+            if q.result is None:
+                continue
+            lo, hi = e.result_dev, e.result_dev + 16
+            if any(k != id(q.result) and a < hi and lo < b for k, a, b in spans) or any(a < hi and lo < b
+                                                                                      for a, b in seen):
+                raise ValueError("plan_device: the loudness result of source %d meets another tensor of the plan"
+                                 % e.slot)
+            seen.append((lo, hi))
+        return (_lib.SsStreamLufs * len(entries))(*entries)
 
     @staticmethod
     def _device_pair_gains(sources):
@@ -1350,6 +1462,8 @@ class Renderer:
             raise ValueError("a DryStream or BackgroundStream layout on the device held an invalid entry (an id >= n, a "
                              "negative offset, a head and count outside the clip or an offset before the end of the "
                              "previous entry); it was skipped")
+        if bits.value & 64:
+            raise ValueError("a StemLoudness target on the device was not finite; that slot was stored unscaled")
 
     def launch_count(self) -> int:
         return int(self.lib.ss_launch_count(self.ctx))
@@ -1376,20 +1490,21 @@ class DevicePlan:
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
     dry-picked slots take their dry signals from dry pools, with pair gains their gains from pair-gain tables; with
     dereverberation targets its mixtures also write those, with stream slots it lays out their dry streams and with bed
-    slots their noise and music beds.  Every plan is created by ss_plan_create_bg, with NULL and a count of 0 for each
-    part it does not have."""
+    slots their noise and music beds, with loudness slots it measures their whole stems at every run.  Every plan is
+    created by ss_plan_create_lufs, with NULL and a count of 0 for each part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
-                 streams=None, bgs=None):
+                 streams=None, bgs=None, lufs=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
-        self.bgs = bgs
+        self.bgs, self.lufs = bgs, lufs
         self._plan = ctypes.c_void_p()
         if n > 0:
-            _lib.check(renderer.lib.ss_plan_create_bg(
+            _lib.check(renderer.lib.ss_plan_create_lufs(
                 renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
                 pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
-                len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, ctypes.byref(self._plan)))
+                len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, lufs, len(lufs) if lufs else 0,
+                ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
