@@ -846,6 +846,60 @@ int ss_plan_create_lufs(ss_ctx* ctx, const ss_source* items, int n_items, const 
                         int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
                         const ss_stream_lufs* lufs, int n_lufs, ss_plan** out);
 
+/* ---- layout draws: a plan draws the layouts of its stream and bed slots itself at every run, by the rules of
+ * create_long_audio (SonicSim_audio.py:231-277) and create_background_audio (:279-340), instead of reading layouts
+ * the caller refreshed before the run.  At the head of every run, before the start draws, one kernel launch (k_layout,
+ * one warp per draw) writes each drawn slot's own layout arrays (ids_dev, offsets_dev and a bed's heads_dev, counts_dev
+ * of its ss_dry_stream or ss_bg_stream); staging, draws, loudness slots and mixtures then read them as they read any
+ * layout, and they hold that run's layout after it.  The layouts match the rules in distribution (the docstrings of
+ * dry.long_audio_layouts and dry.background_audio_layouts), not in the reference's `random` draws.
+ * Random stream (ss_phases.cuh states it once): Philox4x32-10 keyed by the 64-bit seed; block b of draw r (the entry's
+ * index in `layouts`) at counter t is philox(ctr = (b, r, t_lo, t_hi), key = (seed_lo, seed_hi)), its 4 words consumed
+ * in order; a uniform integer in [0, k) takes the next two words as x = w0 | w1 << 32 and is umulhi64(x, k).
+ * rng_dev holds (seed, t), two int64 read at every run and never written: the same pair draws the same layouts, bit for
+ * bit; a training step bumps t (rng[1] += 1) before the run.  Per row, in the order its words are drawn:
+ *   - selection, a sparse Fisher-Yates order over the pool's n lengths: a stream takes utterances while the running
+ *     total is below 0.9 * total and stops at the first that would overflow `total` (get_random_wav_path); a bed takes
+ *     clips while the running total of select_lengths (NULL: the clip lengths) is below 0.4 * total, and the clip that
+ *     reaches `total` is taken and ends it (get_random_wav_path_from_json);
+ *   - placement, the selected ids in a fresh uniform order (a partial Fisher-Yates) while the cursor is below `total`:
+ *     a stream draws a gap in {0, ..., 10 * sample_rate} before each utterance and places it while cursor + gap + len
+ *     <= total; a bed draws a tail in {0, ..., 10 * sample_rate} after each clip, and the first clip whose length plus
+ *     tail reaches the remaining samples is the end clip: slack = floor((total - cursor) * 0.1), lead and trail uniform
+ *     in {0, ..., slack}, kept at cursor + lead with head lead and count min(len, total - trail - cursor) - lead when
+ *     that count is above 0;
+ *   - the first m entries in stream order, then -1 in every array.
+ * K, the most one row can select, is worked out at creation from the pool's lengths: for a stream the largest k whose
+ * k shortest utterances fit in `total` (at least 1, dry.long_audio_max_selected); for a bed the most clips whose
+ * select_lengths stay below 0.4 * total, plus the one that crosses it (at most n).  A row's scratch is a hash map of
+ * 2K to 4K entries and K ids in shared memory.
+ * ss_plan_create_layout is ss_plan_create_lufs with n_layouts entries (n_layouts == 0: exactly ss_plan_create_lufs); a
+ * plan with layout draws launches one kernel per run more.  Refused at creation, before anything is allocated and with
+ * *out untouched:
+ *   - SS_ERR_INVALID:
+ *     - n_layouts < 0, or NULL layouts with n_layouts > 0;
+ *     - a slot that is not a stream or bed slot (ss_dry_stream, ss_bg_stream), or that two entries name;
+ *     - a NULL or unaligned (8 bytes) rng_dev;
+ *     - total < 1, sample_rate < 1 or 10 * sample_rate above INT32_MAX;
+ *     - select_lengths on a stream slot, or a negative select_lengths entry;
+ *     - an rng_dev range that meets a range the plan writes;
+ *     - a drawn slot's layout arrays meeting any other range the plan reads or writes, another slot's layout included.
+ *   - SS_ERR_UNSUPPORTED: K above 1024.
+ * ss_version stays 108: the export marks the capability. */
+typedef struct {
+    int32_t slot;                     /* index into `items`: a stream or bed slot                                     */
+    const int64_t* rng_dev;           /* device, (seed, t), read at every run                                         */
+    int32_t total;                    /* samples of the stream create_long_audio / create_background_audio would build */
+    int32_t sample_rate;              /* gaps and tails are uniform in {0, ..., 10 * sample_rate}                     */
+    const int32_t* select_lengths;    /* host, n entries; bed slots only; NULL = the clip lengths                     */
+} ss_layout_draw;
+int ss_plan_create_layout(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                          const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                          int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                          const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
+                          ss_plan** out);
+
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,
  * both clamped at +40 dB, sums).  E = elements per stem (channels * samples). */

@@ -1185,8 +1185,9 @@ static size_t chunk_desc_bytes(const ss_source* items, const Shape* shapes, int 
     }
     return bytes;
 }
-// What a plan knows of one of its items besides the ss_source: its dry pick, pair gains, dry stream and background
-// stream (validate_dry_picks, validate_streams, validate_bgs) and, once plan_build has laid out the plan's descriptors,
+// What a plan knows of one of its items besides the ss_source: its dry pick, pair gains, dry stream, background
+// stream, loudness target and layout draw (validate_dry_picks, validate_streams, validate_bgs, validate_lufs,
+// validate_layouts) and, once plan_build has laid out the plan's descriptors,
 // the device addresses of its staging area's view (a staged slot), of its DryStream (a stream slot) and of its BgStream
 // (a bed slot)
 struct PlanSlot {
@@ -1195,6 +1196,7 @@ struct PlanSlot {
     const ss_dry_stream* strm = nullptr;
     const ss_bg_stream* bg = nullptr;
     const ss_stream_lufs* lufs = nullptr;   // a loudness slot's target (validate_lufs), or null
+    const ss_layout_draw* layout = nullptr; // a drawn slot's layout draw (validate_layouts), or null
     StageView* view = nullptr;
     const DryStream* ws = nullptr;
     const BgStream* wb = nullptr;
@@ -2493,6 +2495,10 @@ struct ss_plan {
     const LoudCrop* d_crop = nullptr;
     int n_loud = 0, loud_total = 0, crop_ctas = 0;
     double loud_rate = 0;
+    // layout draws (ss_layout_draw): their descriptors (k_layout) in d_desc, and the dynamic shared memory of the most
+    // scratch any of them needs
+    const LayoutDesc* d_layout = nullptr;
+    int n_layout = 0, layout_smem = 0;
 };
 
 // ----------------------------------------------------------------------------- k_draw
@@ -2585,6 +2591,19 @@ __global__ void __launch_bounds__(128) k_draw(const DrawDesc* __restrict__ draws
         *d.start = start;
         if (d.used) *d.used = used;
     }
+}
+
+// ----------------------------------------------------------------------------- k_layout
+// Layout draws of a plan (ss_layout_draw): one warp per draw.  The warp clears the row's hash map in shared memory,
+// then lane 0 draws the row (layout_row, a sequential walk over at most K + 1 selection and 2 * min(K, m) + 2 placement
+// draws) and writes the slot's layout arrays.
+__global__ void __launch_bounds__(32) k_layout(const LayoutDesc* __restrict__ descs) {
+    extern __shared__ int scratch[];
+    const LayoutDesc d = descs[blockIdx.x];
+    const int cap = d.map_cap;
+    for (int i = threadIdx.x; i < cap; i += 32) scratch[i] = -1;
+    __syncwarp();
+    if (threadIdx.x == 0) layout_row(d, scratch, scratch + cap, scratch + 2 * cap);
 }
 
 // ----------------------------------------------------------------------------- k_stage
@@ -2872,18 +2891,33 @@ static StageArea stage_area_of(const ss_source& it) {
     return stage_area(stage_sets(it), cap.first, cap.second, it.pool->taps);
 }
 
+// K of a layout draw (ss_layout_draw): the most a row can select.  A stream: the largest k whose k shortest utterances
+// fit in `total` (at least 1).  A bed: the most clips whose selection lengths stay below 0.4 * total, plus the one that
+// crosses it (at most n).
+static int64_t layout_bound(const ss_layout_draw& L, const ss_dry_pool* dp, bool bed) {
+    std::vector<int64_t> v(dp->N.begin(), dp->N.end());
+    if (L.select_lengths) v.assign(L.select_lengths, L.select_lengths + dp->n);
+    std::sort(v.begin(), v.end());
+    int64_t acc = 0, k = 0;
+    for (int64_t l : v) {
+        if (bed ? !((double)(acc + l) < 0.4 * (double)L.total) : acc + l > L.total) break;
+        acc += l; ++k;
+    }
+    return bed ? std::min<int64_t>(dp->n, k + 1) : std::max<int64_t>(1, k);
+}
+
 // Lay out, fill and upload a plan's descriptors.  The host fills one image, each section at a 256-byte boundary: the
 // chunk descriptors, the mixtures' MixItems, the draws' DrawDescs, the staged slots' StageSlots, the tap block
 // (tap_block, with slots of tap-form pools), the streams' DryStreams and the beds' BgStreams (caller order) and the
-// clip lengths of each dry pool the streams and beds use, and for loudness slots their LoudItems, work-item offsets,
-// LoudCrops and gating tables; one copy uploads it.  Behind the image, written by the device only and never uploaded:
+// clip lengths of each dry pool the streams and beds use, the layout draws' LayoutDescs and their select lengths, and
+// for loudness slots their LoudItems, work-item offsets, LoudCrops and gating tables; one copy uploads it.  Behind the image, written by the device only and never uploaded:
 // one scratch block per mixture, the staged slots' staging areas, then per loudness slot its whole stems, its loudness
 // scratch and (without a result_dev) its result.  slots[i] is caller item i's record; plan_build notes where its view,
 // its DryStream and its BgStream landed.  A loudness slot is chunked, staged and rendered as the window [0, N) into its
 // whole stems; draws and mixtures keep reading the caller's item, whose crop k_loud_crop writes.
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes,
                       std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix, const ss_plan_draw* draws,
-                      int n_draws) {
+                      int n_draws, const ss_layout_draw* layouts, int n_layouts) {
     ss_ctx* c = p->c;
     const int n_items = (int)slots.size();
     std::vector<int> cuts, order;
@@ -2940,6 +2974,13 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
             wpools.push_back(s.clips());
             wlen_off.push_back(take(sizeof(int32_t) * (size_t)s.clips()->n));
         }
+    auto lengths_at = [&](const ss_dry_pool* dp) {
+        return wlen_off[std::find(wpools.begin(), wpools.end(), dp) - wpools.begin()];
+    };
+    const size_t ldesc_off = take(sizeof(LayoutDesc) * n_layouts);
+    std::vector<size_t> lsel_off(n_layouts);             // a bed draw's select_lengths
+    for (int k = 0; k < n_layouts; ++k)
+        if (layouts[k].select_lengths) lsel_off[k] = take(sizeof(int32_t) * (size_t)slots[layouts[k].slot].clips()->n);
     const int n_loud = (int)loud.size();
     std::vector<ss_post_lufs> gating(n_loud);
     for (int k = 0; k < n_loud; ++k) gating[k] = slots[loud[k]].lufs->gating;
@@ -3008,7 +3049,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     for (int i = 0, k = 0, kb = 0; i < n_items; ++i) {   // the streams and beds first: staged slots and draws name them
         const ss_dry_pool* dp = slots[i].clips();
         if (!dp) continue;
-        const int* const lengths = (const int*)(d + wlen_off[std::find(wpools.begin(), wpools.end(), dp) - wpools.begin()]);
+        const int* const lengths = (const int*)(d + lengths_at(dp));
         int cut = 0;
         for (const PoolEntry& e : caller_items[i].pool->host) cut = std::max(cut, e.N);
         if (const ss_dry_stream* w = slots[i].strm) {
@@ -3025,6 +3066,27 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     }
     for (size_t j = 0; j < wpools.size(); ++j)
         memcpy(host.data() + wlen_off[j], wpools[j]->N.data(), sizeof(int32_t) * (size_t)wpools[j]->n);
+    for (int k = 0; k < n_layouts; ++k) {                // the layout draws write their slots' own layout arrays
+        const ss_layout_draw& L = layouts[k];
+        const PlanSlot& r = slots[L.slot];
+        const ss_dry_pool* dp = r.clips();
+        LayoutDesc& g = ((LayoutDesc*)(host.data() + ldesc_off))[k];
+        g.rng = L.rng_dev; g.lengths = (const int*)(d + lengths_at(dp));
+        if (L.select_lengths) {
+            memcpy(host.data() + lsel_off[k], L.select_lengths, sizeof(int32_t) * (size_t)dp->n);
+            g.select = (const int*)(d + lsel_off[k]);
+        }
+        if (r.strm) {
+            g.ids = const_cast<int*>(r.strm->ids_dev); g.offsets = const_cast<int*>(r.strm->offsets_dev); g.m = r.strm->m;
+        } else {
+            g.ids = const_cast<int*>(r.bg->ids_dev); g.offsets = const_cast<int*>(r.bg->offsets_dev);
+            g.heads = const_cast<int*>(r.bg->heads_dev); g.counts = const_cast<int*>(r.bg->counts_dev); g.m = r.bg->m;
+        }
+        g.n = dp->n; g.total = L.total; g.gap_max = 10 * L.sample_rate; g.r = k;
+        g.K = (int)layout_bound(L, dp, r.bg != nullptr);
+        g.map_cap = layout_map_cap(g.K);
+        p->layout_smem = std::max(p->layout_smem, (int)sizeof(int) * layout_scratch_ints(g.K));
+    }
     for (size_t k = 0; k < staged.size(); ++k) {
         const ss_source& it = items[staged[k]];
         PlanSlot& r = *rec[staged[k]];
@@ -3082,6 +3144,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     CK(cudaMemcpy(d, host.data(), image, cudaMemcpyHostToDevice));
     if (!mix.empty()) { p->d_mix = (const MixItem*)(d + mix_off); p->n_mix = (int)mix.size(); }
     if (n_draws > 0) { p->d_draw = (const DrawDesc*)(d + draw_off); p->n_draw = n_draws; }
+    if (n_layouts > 0) { p->d_layout = (const LayoutDesc*)(d + ldesc_off); p->n_layout = n_layouts; }
     if (!staged.empty()) { p->d_stage = (const StageSlot*)(d + stage_off); p->n_stage = (int)staged.size(); }
     if (n_tap) {
         p->tap_ctas = ((const int*)(host.data() + tb.prefix))[n_tap];
@@ -3209,20 +3272,22 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
             add_range(r, e.bounds, 4 * (uint64_t)e.P, false);
         }
     // a dry-picked slot may read any signal of its dry pool, and reads its dry pick; a stream slot reads its layout; a
-    // bed slot reads its layout and may read any clip of its dry pool
+    // bed slot reads its layout and may read any clip of its dry pool; a drawn slot writes its layout and reads its rng
     std::vector<const ss_dry_pool*> dpools;
     for (const PlanSlot& s : slots) {
         if (s.dry) {
             add_range(r, s.dry->pick_dev, 4, false);
             if (std::find(dpools.begin(), dpools.end(), s.dry->pool) == dpools.end()) dpools.push_back(s.dry->pool);
         }
+        const bool drawn = s.layout != nullptr;
+        if (drawn) add_range(r, s.layout->rng_dev, 16, false);
         if (s.strm) {
-            add_range(r, s.strm->ids_dev, 4 * (uint64_t)s.strm->m, false);
-            add_range(r, s.strm->offsets_dev, 4 * (uint64_t)s.strm->m, false);
+            add_range(r, s.strm->ids_dev, 4 * (uint64_t)s.strm->m, drawn);
+            add_range(r, s.strm->offsets_dev, 4 * (uint64_t)s.strm->m, drawn);
         }
         if (s.bg) {                                         // a bed slot reads its layout and any clip of its pool
             for (const int32_t* a : {s.bg->ids_dev, s.bg->offsets_dev, s.bg->heads_dev, s.bg->counts_dev})
-                add_range(r, a, 4 * (uint64_t)s.bg->m, false);
+                add_range(r, a, 4 * (uint64_t)s.bg->m, drawn);
             if (std::find(dpools.begin(), dpools.end(), s.bg->pool) == dpools.end()) dpools.push_back(s.bg->pool);
         }
         if (s.lufs) {                                       // a loudness slot reads its target, writes its result
@@ -3233,6 +3298,17 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
         if (!dp->padded())
             for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
+    // the items' outputs count as read above (mixtures read them); a layout draw's rng meets none of them either
+    for (const PlanSlot& s : slots) {
+        if (!s.layout) continue;
+        const uintptr_t lo = (uintptr_t)s.layout->rng_dev, hi = lo + 16;
+        for (int i = 0; i < n_items; ++i) {
+            const ss_source& it = items[i];
+            const uint64_t n_out = 4 * (uint64_t)it.C * (it.win_len > 0 ? it.win_len : it.N);
+            for (const float* o : {it.out, (it.flags & SS_DIRECT_TARGET) ? it.out_direct : nullptr})
+                if (o && (uintptr_t)o < hi && lo < (uintptr_t)o + n_out) return SS_ERR_INVALID;
+        }
+    }
     return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
 }
 
@@ -3337,6 +3413,27 @@ static int validate_lufs(const ss_source* items, const ss_stream_lufs* lufs, int
     return SS_OK;
 }
 
+// A plan's layout draws (include/sonicsim_b200.h, ss_layout_draw), all but the byte ranges (validate_mixes): the record
+// of each drawn slot receives its draw.  After validate_streams and validate_bgs, which name the stream and bed slots.
+static int validate_layouts(const ss_layout_draw* layouts, int n_layouts, std::vector<PlanSlot>& slots) {
+    for (int k = 0; k < n_layouts; ++k) {
+        const ss_layout_draw& L = layouts[k];
+        if (L.slot < 0 || L.slot >= (int)slots.size()) return SS_ERR_INVALID;
+        const PlanSlot& r = slots[L.slot];
+        if (r.layout || !(r.strm || r.bg) || !L.rng_dev || ((uintptr_t)L.rng_dev & 7) || L.total < 1 ||
+            L.sample_rate < 1 || L.sample_rate > INT32_MAX / 10 || (r.strm && L.select_lengths))
+            return SS_ERR_INVALID;
+        if (L.select_lengths)
+            for (int i = 0; i < r.bg->pool->n; ++i) if (L.select_lengths[i] < 0) return SS_ERR_INVALID;
+        slots[L.slot].layout = &L;
+    }
+    for (int k = 0; k < n_layouts; ++k) {
+        const PlanSlot& r = slots[layouts[k].slot];
+        if (layout_bound(layouts[k], r.clips(), r.bg != nullptr) > kLayoutCap) return SS_ERR_UNSUPPORTED;
+    }
+    return SS_OK;
+}
+
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
 // and the byte ranges (validate_mixes): mix receives the mixtures, each with its target's direct_out, or null
 static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan_target* targets, int n_targets,
@@ -3355,10 +3452,12 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
-                       const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
+                       const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
+                       ss_plan** out) {
     auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
     if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
-        bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs) || bad(lufs, n_lufs))
+        bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs) || bad(lufs, n_lufs) ||
+        bad(layouts, n_layouts))
         return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
@@ -3369,6 +3468,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     { int st = validate_streams(c, items, streams, n_streams, slots); if (st) return st; }
     { int st = validate_bgs(c, items, bgs, n_bgs, draws, n_draws, slots); if (st) return st; }
     { int st = validate_lufs(items, lufs, n_lufs, slots); if (st) return st; }
+    { int st = validate_layouts(layouts, n_layouts, slots); if (st) return st; }
     { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
     { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
     { int st = validate_mixes(items, slots, mix, draws, n_draws); if (st) return st; }
@@ -3382,7 +3482,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), slots, mix, draws, n_draws);
+    const int st = plan_build(p, items, shapes.data(), slots, mix, draws, n_draws, layouts, n_layouts);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -3391,26 +3491,26 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
     return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                       0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3418,7 +3518,7 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3426,7 +3526,7 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
@@ -3435,7 +3535,7 @@ extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items,
                                  int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                  int n_bgs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3444,14 +3544,24 @@ extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_item
                                    int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                    int n_bgs, const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                     int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                     const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                     int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
+                                     int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
+                                     int n_layouts, ss_plan** out) {
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
@@ -3464,10 +3574,16 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, bool stre
     return SS_OK;
 }
 
-// the start draws, the host-pool staging, the launches of every chunk (run_chunks), the loudness slots' measurements
-// and crops, then the mixtures (which read every chunk's outputs and the crops) on `stream`
+// the layout draws, the start draws (which walk stream layouts), the host-pool staging, the launches of every chunk
+// (run_chunks), the loudness slots' measurements and crops, then the mixtures (which read every chunk's outputs and the
+// crops) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
+    if (p->n_layout) {
+        k_layout<<<p->n_layout, 32, p->layout_smem, stream>>>(p->d_layout);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
     if (p->n_draw) {
         const int st = draw_enqueue(c, p->d_draw, p->n_draw, p->draw16, p->draw_stream, stream);
         if (st) return st;

@@ -698,6 +698,149 @@ SS_HD float bg_sample(const int* a, const int* b, const char* const* p, int k, i
     return i16 ? i16_sample(reinterpret_cast<const int16_t*>(p[lo - 1])[t]) : reinterpret_cast<const float*>(p[lo - 1])[t];
 }
 
+// ---- layout draws (ss_layout_draw, include/sonicsim_b200.h): a plan draws a stream or bed slot's layout itself at
+// every run (k_layout), from a counter-based generator, by the rules of dry.long_audio_layouts and
+// dry.background_audio_layouts.  The random stream is a format: the kernel, the CPU emulation and the tests' Python
+// restatement follow it word for word.
+//   - Philox4x32-10 (Salmon et al., SC'11), written out here so that g++ compiles it for the emulation.
+//   - The key is the 64-bit seed (seed_lo, seed_hi).  Block b of layout draw r (its index in the plan's list of draws)
+//     at counter t is philox(ctr = (b, r, t_lo, t_hi), key), b = 0, 1, ...; its 4 words are consumed in order.
+//   - A uniform integer in [0, k) takes the next two words, x = w0 | w1 << 32, and is umulhi64(x, k).
+// (seed, t) are two int64 in device memory, read at every run: the same pair draws the same layouts, bit for bit.
+constexpr int kLayoutCap = 1024;                       // the most utterances or clips one row may select
+SS_HD uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+    for (int i = 0; i < 10; ++i) {
+        if (i) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+        const uint64_t p0 = (uint64_t)0xD2511F53u * c.x, p1 = (uint64_t)0xCD9E8D57u * c.z;
+        c = make_uint4((uint32_t)(p1 >> 32) ^ c.y ^ k0, (uint32_t)p1, (uint32_t)(p0 >> 32) ^ c.w ^ k1, (uint32_t)p0);
+    }
+    return c;
+}
+SS_HD uint64_t umulhi64(uint64_t a, uint64_t b) {
+#if defined(__CUDA_ARCH__)
+    return __umul64hi(a, b);
+#else
+    return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+// The word stream of one layout draw at one (seed, t)
+struct LayoutRng {
+    uint32_t k0, k1, r, t0, t1, b;
+    int w;                                             // words of buf consumed
+    uint4 buf;
+};
+SS_HD LayoutRng layout_rng(int64_t seed, int64_t t, int r) {
+    LayoutRng g;
+    g.k0 = (uint32_t)(uint64_t)seed; g.k1 = (uint32_t)((uint64_t)seed >> 32);
+    g.r = (uint32_t)r; g.t0 = (uint32_t)(uint64_t)t; g.t1 = (uint32_t)((uint64_t)t >> 32);
+    g.b = 0; g.w = 4; g.buf = make_uint4(0, 0, 0, 0);
+    return g;
+}
+SS_HD uint32_t rng_word(LayoutRng& g) {
+    if (g.w == 4) { g.buf = philox4x32_10(make_uint4(g.b++, g.r, g.t0, g.t1), g.k0, g.k1); g.w = 0; }
+    const int w = g.w++;
+    return w == 0 ? g.buf.x : w == 1 ? g.buf.y : w == 2 ? g.buf.z : g.buf.w;
+}
+// a uniform integer in [0, k), k >= 1
+SS_HD uint64_t rng_below(LayoutRng& g, uint64_t k) {
+    const uint64_t lo = rng_word(g);
+    return umulhi64(lo | (uint64_t)rng_word(g) << 32, k);
+}
+// One layout draw's descriptor in its plan's block.  heads == null: a speech stream (create_long_audio's rule), else a
+// bed (create_background_audio's).  lengths: the plan's copy of the dry pool's n lengths; select: a bed's n selection
+// lengths, or null for the lengths themselves.  K (<= kLayoutCap) bounds what a row can select: the scratch of a row is
+// a hash map of map_cap (a power of two >= 2K + 2) keys and values and K selected ids.
+struct LayoutDesc {
+    const int64_t* rng;
+    const int* lengths;
+    const int* select;
+    int* ids;
+    int* offsets;
+    int* heads;
+    int* counts;
+    int n, m, total, gap_max, K, r, map_cap, pad;
+};
+static_assert(sizeof(LayoutDesc) == 88, "LayoutDesc layout");
+SS_HD int layout_map_cap(int K) { int c = 2; while (c < 2 * K + 2) c <<= 1; return c; }
+SS_HD int layout_scratch_ints(int K) { return 2 * layout_map_cap(K) + K; }
+// The sparse Fisher-Yates array: position i holds the map's value for key i, or i itself (keys -1: empty slots)
+SS_HD unsigned fy_slot(int i, int mask) { return ((uint32_t)i * 2654435769u >> 7) & (unsigned)mask; }
+SS_HD int fy_get(const int* keys, const int* vals, int mask, int i) {
+    for (unsigned h = fy_slot(i, mask);; h = (h + 1) & (unsigned)mask) {
+        if (keys[h] == i) return vals[h];
+        if (keys[h] < 0) return i;
+    }
+}
+SS_HD void fy_put(int* keys, int* vals, int mask, int i, int v) {
+    for (unsigned h = fy_slot(i, mask);; h = (h + 1) & (unsigned)mask)
+        if (keys[h] == i || keys[h] < 0) { keys[h] = i; vals[h] = v; return; }
+}
+// One row, in the order its words are drawn (keys: map_cap entries of -1; vals: map_cap; sel: K):
+//   1. selection, a uniform order over the n ids without replacement (step s swaps position s with s + u, u uniform
+//      in [0, n - s)): a stream takes the drawn utterance while the running total is below 0.9 * total and stops at the
+//      first that would overflow `total` (get_random_wav_path); a bed takes clips while the running total of `select`
+//      is below 0.4 * total, and the clip that reaches `total` is taken and ends it (get_random_wav_path_from_json);
+//   2. placement, the selected ids in a fresh uniform order (step j swaps j with j + v, v uniform in [0, s - j)) while
+//      the cursor is below `total`, each followed by one more draw: a stream's gap in {0, ..., gap_max} before the
+//      utterance, placed while cursor + gap + len <= total (_place_long_audio); a bed's tail in {0, ..., gap_max} after
+//      the clip, and the first clip with len + tail >= total - cursor is the end clip: slack = floor((total - cursor) *
+//      0.1), lead and trail uniform in {0, ..., slack}, kept with head lead and count min(len, total - trail - cursor) -
+//      lead when that is above 0 (_place_background_audio);
+//   3. the first m entries in stream order, then -1 in every array.
+SS_HD void layout_row(const LayoutDesc& d, int* keys, int* vals, int* sel) {
+    LayoutRng g = layout_rng(d.rng[0], d.rng[1], d.r);
+    const int mask = d.map_cap - 1;
+    const bool bed = d.heads != nullptr;
+    const int* const sl = d.select ? d.select : d.lengths;
+    const double thr = (bed ? 0.4 : 0.9) * (double)d.total;
+    long long acc = 0;
+    int s = 0;
+    while (s < d.n && (double)acc < thr) {
+        const int p = s + (int)rng_below(g, (uint64_t)(d.n - s));
+        const int x = fy_get(keys, vals, mask, p);
+        const long long l = sl[x];
+        if (!bed && acc + l > d.total) break;
+        if (s == d.K) break;                           // (never: K bounds every selection)
+        fy_put(keys, vals, mask, p, fy_get(keys, vals, mask, s));
+        sel[s++] = x;
+        if (bed && !(acc + l < d.total)) break;
+        acc += l;
+    }
+    long long cur = 0;
+    int k = 0;
+    auto put = [&](int id, long long o, long long h, long long c) {
+        d.ids[k] = id; d.offsets[k] = (int)o;
+        if (bed) { d.heads[k] = (int)h; d.counts[k] = (int)c; }
+        ++k;
+    };
+    for (int j = 0; j < s && cur < d.total && k < d.m; ++j) {
+        const int v = j + (int)rng_below(g, (uint64_t)(s - j));
+        const int id = sel[v];
+        sel[v] = sel[j]; sel[j] = id;
+        const long long l = d.lengths[id];
+        const long long gap = (long long)rng_below(g, (uint64_t)d.gap_max + 1);
+        if (!bed) {
+            if (cur + gap + l > d.total) break;
+            put(id, cur + gap, 0, l);
+            cur += gap + l;
+        } else if (l + gap >= d.total - cur) {
+            const long long slack = (long long)floor((double)(d.total - cur) * 0.1);
+            const long long lead = (long long)rng_below(g, (uint64_t)slack + 1);
+            const long long trail = (long long)rng_below(g, (uint64_t)slack + 1);
+            const long long c = (l < d.total - trail - cur ? l : d.total - trail - cur) - lead;
+            if (c > 0) put(id, cur + lead, lead, c);
+            break;
+        } else {
+            put(id, cur, 0, l);
+            cur += l + gap;
+        }
+    }
+    for (; k < d.m; ++k) {
+        d.ids[k] = -1; d.offsets[k] = -1;
+        if (bed) { d.heads[k] = -1; d.counts[k] = -1; }
+    }
+}
+
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
 SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }

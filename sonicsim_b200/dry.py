@@ -125,6 +125,17 @@ def long_audio_max_selected(lengths, total: int) -> int:
     return max(1, int(np.searchsorted(np.cumsum(v), int(total), side="right")))
 
 
+def background_audio_max_selected(select_lengths, total: int) -> int:
+    """The most clips that get_random_wav_path_from_json's selection (threshold 0.4) can take for a bed of `total`
+    samples over clips of `select_lengths`: the most whose running total stays below 0.4 * total, plus the one that
+    crosses it (at most n).  A host computation, once per corpus; render.LayoutDraw refuses beds above 1024."""
+    import numpy as np
+    v = np.sort(np.asarray(select_lengths.cpu() if hasattr(select_lengths, "cpu") else select_lengths,
+                           dtype=np.int64).reshape(-1))
+    below = int(np.count_nonzero(np.cumsum(v).astype(np.float64) < 0.4 * int(total)))
+    return min(v.size, below + 1)
+
+
 def _long_audio_selection(lengths, total: int, count: int, width: int, kw):
     """get_random_wav_path's selection, `count` times: (sel, chosen), both (count, width).  sel[r] is the first width
     utterances of a uniform random order, chosen[r] marks its selected prefix (taken while the running total is below

@@ -187,6 +187,27 @@ class StemLoudness(T.NamedTuple):
     sr: float = 16000.0
 
 
+class LayoutDraw(T.NamedTuple):
+    """A stream or bed slot whose layout the plan draws itself at every run (Renderer.plan_device(layouts=...)), by the
+    rule of dry.long_audio_layouts (a DryStream slot) or dry.background_audio_layouts (a BackgroundStream slot), in one
+    kernel launch at the head of the run.  `slot`: index into the plan's sources.  `rng`: a two-element CUDA int64 tensor
+    (seed, t) read at every run and never written (one tensor may serve every draw of a plan): the same (seed, t) draws
+    the same layouts bit for bit, and a training step bumps t (rng[1] += 1) before plan.run(), as u.uniform_() refreshes
+    a CropDraw.  Draw r of `layouts` takes Philox4x32-10 blocks (b, r, t) under the key seed (include/sonicsim_b200.h,
+    ss_layout_draw, states the stream).  `total`: the samples of the stream create_long_audio or create_background_audio
+    would build; gaps and tails are uniform in {0, ..., 10 * sample_rate}.  `select_lengths` (bed slots only): n
+    non-negative selection lengths, e.g. the clips' native-rate lengths from SonicSet's JSON (see
+    dry.background_audio_layouts); None selects by the clip lengths.  The draw writes the slot's own ids, offsets (and
+    heads, counts) tensors, which then hold that run's layout.  The layouts match the rules in distribution, not torch's
+    bits.  A row may select at most 1024 utterances or clips (dry.long_audio_max_selected,
+    dry.background_audio_max_selected)."""
+    slot: int
+    rng: T.Any
+    total: int
+    sample_rate: int = 16000
+    select_lengths: T.Any = None
+
+
 class CropDraw(T.NamedTuple):
     """A crop start drawn on the device at every run of a device plan (Renderer.plan_device(draws=...)): the dataloader's
     start loop (movingdatamodule.py:81-99).  `start`: the one-element CUDA int32 tensor that the windows of this
@@ -1052,7 +1073,7 @@ class Renderer:
             stream = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.lib.ss_render_dev(self.ctx, items, n, ctypes.c_void_p(stream)))
 
-    def plan_device(self, sources, outs, direct_outs=None, mixtures=None, draws=None) -> "DevicePlan":
+    def plan_device(self, sources, outs, direct_outs=None, mixtures=None, draws=None, layouts=None) -> "DevicePlan":
         """Bind a batch of device-resident sources to its output tensors once; `plan.run()` then renders it with a
         single C-ABI call - one CUDA graph launch (ss_plan_run; a generation loop overwrites the same tensors and
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
@@ -1087,7 +1108,13 @@ class Renderer:
         stream is laid out from a 16-bit utterance pool at every run (ss_plan_create_stream): a fresh arrangement of
         utterances and gaps per step (dry.long_audio_layouts into the ids and offsets before the run).  With `dry` =
         BackgroundStream(clip_pool, ids, offsets, heads, counts) the slot's noise or music bed is laid out from a clip
-        pool at every run (ss_plan_create_bg; dry.background_audio_layouts into the four arrays before the run)."""
+        pool at every run (ss_plan_create_bg; dry.background_audio_layouts into the four arrays before the run).
+
+        `layouts`: LayoutDraw entries, stream and bed slots whose layouts the plan draws itself at the head of every run
+        (ss_plan_create_layout, one kernel launch more per run) instead of the caller's refresh: a step is then
+
+            rng[1] += 1; u.uniform_(); picks.copy_(...); sirs.uniform_(-6, 6); snr.uniform_(10, 20)
+            plan.run()"""
         dry = self._device_dry(sources)
         streams = self._device_streams(sources)
         bgs = self._device_bgs(sources)
@@ -1096,8 +1123,9 @@ class Renderer:
         mixes = self._device_mixes(mixtures, outs, keep, items, targets) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
         lufs = self._device_lufs(sources, (outs, direct_outs, mixtures, draws), keep)
+        lay = self._device_layouts(layouts, sources, (outs, direct_outs, mixtures, draws), keep) if layouts else None
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
-                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs)
+                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs, lay)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1256,6 +1284,76 @@ class Renderer:
                                  % e.slot)
             seen.append((lo, hi))
         return (_lib.SsStreamLufs * len(entries))(*entries)
+
+    def _device_layouts(self, layouts, sources, others, keep):
+        """Validated ss_layout_draw array of a plan's layout draws; their select_lengths arrays are appended to `keep`.
+        `others`: the plan's other arguments, whose tensors the drawn layouts may not meet."""
+        import torch
+        from . import dry as _dry
+        arr = (_lib.SsLayoutDraw * len(layouts))()
+        drawn, rngs = [], []
+        for k, d in enumerate(layouts):
+            if not isinstance(d, LayoutDraw):
+                raise ValueError("plan_device: layout %d must be a LayoutDraw" % k)
+            i = int(d.slot)
+            s = sources[i] if 0 <= i < len(sources) else None
+            w = getattr(s, "dry", None)
+            if not isinstance(s, Pooled) or not isinstance(w, (DryStream, BackgroundStream)):
+                raise ValueError("plan_device: layout %d names source %d, which is not a stream or bed slot (a Pooled "
+                                 "slot with a DryStream or BackgroundStream)" % (k, i))
+            if any(int(e.slot) == i for e in layouts[:k]):
+                raise ValueError("plan_device: layout %d names source %d, which another layout draw names" % (k, i))
+            own = "layout %d" % k
+            rng = _tensor(d.rng, "plan_device", own, "rng", torch.int64, self.device, count=(2, 2))
+            if rng % 8:
+                raise ValueError("plan_device: the rng of layout %d must be 8-byte aligned" % k)
+            total, sr = int(d.total), int(d.sample_rate)
+            if not 1 <= total < 1 << 31 or not 1 <= sr <= 214748364:
+                raise ValueError("plan_device: layout %d needs 1 <= total < 2^31 and 1 <= sample_rate <= 214748364 "
+                                 "(10 s of samples in int32), got %d and %d" % (k, total, sr))
+            bed = isinstance(w, BackgroundStream)
+            sel = None
+            if d.select_lengths is not None:
+                if not bed:
+                    raise ValueError("plan_device: layout %d has select_lengths, but source %d is a stream slot: only "
+                                     "beds select by other lengths" % (k, i))
+                sel = np.asarray(d.select_lengths.cpu() if _is_tensor(d.select_lengths) else d.select_lengths)
+                if sel.shape != (w.pool.n,) or not np.issubdtype(sel.dtype, np.integer) or \
+                        (sel.size and (sel.min() < 0 or sel.max() >= 1 << 31)):
+                    raise ValueError("plan_device: the select_lengths of layout %d must be %d non-negative int32 "
+                                     "lengths, one per clip" % (k, w.pool.n))
+                sel = np.ascontiguousarray(sel, dtype=np.int32)
+                keep.append(sel)
+            K = (_dry.background_audio_max_selected(sel if sel is not None else w.pool.sizes, total) if bed
+                 else _dry.long_audio_max_selected(w.pool.sizes, total))
+            if K > 1024:
+                raise ValueError("plan_device: layout %d could select %d %s, at most 1024" %
+                                 (k, K, "clips" if bed else "utterances"))
+            arrays = (w.ids, w.offsets) + ((w.heads, w.counts) if bed else ())
+            drawn += [a for a in arrays if _is_tensor(a)]
+            rngs.append(d.rng)
+            arr[k] = _lib.SsLayoutDraw(slot=i, rng_dev=rng, total=total, sample_rate=sr,
+                                       select_lengths=sel.ctypes.data if sel is not None else None)
+        # a drawn layout is written at every run: it meets no other tensor the plan reads or writes, another drawn
+        # layout included; an rng meets nothing the plan writes
+        outs, direct_outs, mixtures, draws = others
+        stems = [getattr(s.dry, "lufs", None) for s in sources if isinstance(s, Pooled)]
+        span = lambda t: (t.data_ptr(), t.data_ptr() + t.numel() * t.element_size())   # noqa: E731
+        every = _cuda_tensors((sources, others, stems))
+        for a in drawn:
+            lo, hi = span(a)
+            if sum(1 for t in every if t is a) + sum(1 for t in drawn if t is a) > 2 or \
+                    any(t is not a and span(t)[0] < hi and lo < span(t)[1] for t in every):
+                raise ValueError("plan_device: a layout tensor drawn by the plan meets another tensor of the plan")
+        written = drawn + _cuda_tensors((outs, direct_outs, [q.result for q in stems if q is not None],
+                                         [(m.mix, m.speakers_out, m.rms_db, m.direct_out) for m in mixtures or ()],
+                                         [(d.start, d.used) for d in draws or ()]))
+        for t in rngs:
+            lo, hi = span(t)
+            if any(a < hi and lo < b for a, b in map(span, written)):
+                raise ValueError("plan_device: a layout draw's rng meets a tensor the plan writes")
+        keep.append(list(layouts))
+        return arr
 
     @staticmethod
     def _device_pair_gains(sources):
@@ -1490,21 +1588,22 @@ class DevicePlan:
     mixtures, the plan also assembles them at every run; with draws, it first draws their starts; with dry picks, its
     dry-picked slots take their dry signals from dry pools, with pair gains their gains from pair-gain tables; with
     dereverberation targets its mixtures also write those, with stream slots it lays out their dry streams and with bed
-    slots their noise and music beds, with loudness slots it measures their whole stems at every run.  Every plan is
-    created by ss_plan_create_lufs, with NULL and a count of 0 for each part it does not have."""
+    slots their noise and music beds, with loudness slots it measures their whole stems at every run, with layout draws
+    it draws its stream and bed layouts at every run.  Every plan is created by ss_plan_create_layout, with NULL and a
+    count of 0 for each part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
-                 streams=None, bgs=None, lufs=None):
+                 streams=None, bgs=None, lufs=None, layouts=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
-        self.bgs, self.lufs = bgs, lufs
+        self.bgs, self.lufs, self.layouts = bgs, lufs, layouts
         self._plan = ctypes.c_void_p()
         if n > 0:
-            _lib.check(renderer.lib.ss_plan_create_lufs(
+            _lib.check(renderer.lib.ss_plan_create_layout(
                 renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
                 pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
                 len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, lufs, len(lufs) if lufs else 0,
-                ctypes.byref(self._plan)))
+                layouts, len(layouts) if layouts else 0, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
