@@ -900,6 +900,63 @@ int ss_plan_create_layout(ss_ctx* ctx, const ss_source* items, int n_items, cons
                           const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
                           ss_plan** out);
 
+/* ---- value draws: a plan writes the per-run values its slots, start draws, mixtures and loudness slots read (picks,
+ * dry picks, win_start_dev, sirs, snr, a draw's u, loudness targets) itself, at the head of every run, instead of
+ * reading values the caller refreshed before the run: the dataloader's random.choice of a scene, random.sample of its
+ * speakers, randint crop starts, SIR ~ U(-6, 6), SNR ~ U(10, 20) and loudness targets, from one counter.  One kernel
+ * launch (k_values, one warp per row) runs first in the run, before the layout draws and the start draws; everything
+ * after it reads the tensors it wrote as it reads them today.  The values match the rules in distribution, not torch's
+ * or `random`'s bits.
+ * Random stream (ss_phases.cuh states it once), the generator and key of ss_layout_draw: element j of row b of value
+ * draw r (its index in `values`) at counter t takes block philox(ctr = (b, 0x80000000 | r << 11 | j >> 1, t_lo, t_hi),
+ * key = (seed_lo, seed_hi)) and its words 2 (j & 1) and 2 (j & 1) + 1 as x = w0 | w1 << 32.  Layout draws use c1 = r
+ * < 2^31, so the two streams never share a block, and a plan's layout bits do not change when value draws are added.
+ *   - SS_VALUE_F64: u = (x >> 11) * 2^-53; SS_VALUE_F32: u = (x >> 40) * 2^-24; v = low + (high - low) * u in double
+ *     (product and sum rounded separately), rounded once to the output type; a result that is not below high becomes
+ *     the largest value of the type below high;
+ *   - SS_VALUE_INT: ilow + umulhi64(x, ihigh - ilow);
+ *   - SS_VALUE_DISTINCT: each row an ordered sample without replacement (random.sample) from [ilow, ihigh): a partial
+ *     Fisher-Yates over [0, n), n = ihigh - ilow, element j taking y = umulhi64(x_j, n - j), pos = j + y, writing
+ *     ilow + a[pos] and setting a[pos] = a[j], a the identity;
+ *   - base >= 0: the value is out_base[b] * stride + value, in int64 (out_base: the out of entry `base`, one int32 per
+ *     row), e.g. speakers of scene-major pools: picks[b, j] = scene[b] * 3 + sample.
+ * rng_dev holds (seed, t), read at every run and never written: the same pair draws the same values, bit for bit.
+ * ss_plan_create_values is ss_plan_create_layout with n_values entries (n_values == 0: exactly ss_plan_create_layout);
+ * a plan with value draws launches one kernel per run more.  Refused at creation, before anything is allocated and with
+ * *out untouched:
+ *   - SS_ERR_INVALID:
+ *     - n_values < 0, or NULL values with n_values > 0; an unknown kind;
+ *     - a NULL or misaligned out (4 bytes; 8 for SS_VALUE_F64) or rng_dev (8 bytes);
+ *     - rows outside [1, 65535] or different from the first entry's; k outside [1, 4096];
+ *     - real kinds: non-finite low or high, low >= high, a base; SS_VALUE_F32 bounds not representable in float32;
+ *     - int kinds: ilow >= ihigh; SS_VALUE_DISTINCT with k > 64 or k > ihigh - ilow;
+ *     - a base that is not an earlier int kind entry with k = 1; stride < 1 with a base; an int32 overflow of
+ *       out_base * stride + value possible over the base entry's values;
+ *     - an out that meets another entry's out, any rng_dev, or any range the plan reads or writes other than the small
+ *       per-run inputs: items' pick_dev and win_start_dev (not one a start draw writes), dry picks' pick_dev, mixtures'
+ *       sirs and snr, start draws' u, loudness slots' target_dev;
+ *     - an rng_dev that meets a range the plan writes.
+ *   - SS_ERR_UNSUPPORTED: more than 2^20 entries.
+ * ss_version stays 108: the export marks the capability. */
+enum { SS_VALUE_F32 = 0, SS_VALUE_F64 = 1, SS_VALUE_INT = 2, SS_VALUE_DISTINCT = 3 };
+typedef struct {
+    void* out;                        /* device, rows x k (row-major) float / double / int32, written at every run    */
+    const int64_t* rng_dev;           /* device, (seed, t), read at every run                                         */
+    int32_t kind;                     /* SS_VALUE_*                                                                   */
+    int32_t rows;                     /* B, the same in every entry                                                   */
+    int32_t k;                        /* elements per row                                                             */
+    int32_t base;                     /* int kinds: index of an earlier int entry with k = 1, or -1                   */
+    double low, high;                 /* real kinds: [low, high)                                                      */
+    int32_t ilow, ihigh;              /* int kinds: [ilow, ihigh)                                                     */
+    int32_t stride;                   /* with a base: >= 1                                                            */
+} ss_value_draw;
+int ss_plan_create_values(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                          const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                          int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                          const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
+                          const ss_value_draw* values, int n_values, ss_plan** out);
+
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,
  * both clamped at +40 dB, sums).  E = elements per stem (channels * samples). */

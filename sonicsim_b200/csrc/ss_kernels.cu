@@ -2499,6 +2499,9 @@ struct ss_plan {
     // scratch any of them needs
     const LayoutDesc* d_layout = nullptr;
     int n_layout = 0, layout_smem = 0;
+    // value draws (ss_value_draw): their descriptors (k_values) in d_desc, and the rows every one of them has
+    const ValueDesc* d_value = nullptr;
+    int n_value = 0, value_rows = 0;
 };
 
 // ----------------------------------------------------------------------------- k_draw
@@ -2604,6 +2607,23 @@ __global__ void __launch_bounds__(32) k_layout(const LayoutDesc* __restrict__ de
     for (int i = threadIdx.x; i < cap; i += 32) scratch[i] = -1;
     __syncwarp();
     if (threadIdx.x == 0) layout_row(d, scratch, scratch + cap, scratch + 2 * cap);
+}
+
+// ----------------------------------------------------------------------------- k_values
+// Value draws of a plan (ss_value_draw): one warp per row b, four rows per CTA.  The warp runs the draws in list order,
+// its lanes striding over the row's elements (value_row; a distinct row on lane 0, its map in shared memory), with a
+// __syncwarp between draws so that a base draw's value is written before a later draw of the row reads it.
+constexpr int kValueWarps = 4;
+__global__ void __launch_bounds__(32 * kValueWarps) k_values(const ValueDesc* __restrict__ descs, int n, int rows) {
+    __shared__ uint32_t map[kValueWarps][2 * kValueMapCap];
+    const int w = threadIdx.x >> 5;
+    const int b = blockIdx.x * kValueWarps + w;
+    if (b >= rows) return;
+    for (int r = 0; r < n; ++r) {
+        const ValueDesc d = descs[r];
+        value_row(d, b, threadIdx.x & 31, 32, map[w], map[w] + kValueMapCap);
+        __syncwarp();
+    }
 }
 
 // ----------------------------------------------------------------------------- k_stage
@@ -2909,15 +2929,17 @@ static int64_t layout_bound(const ss_layout_draw& L, const ss_dry_pool* dp, bool
 // Lay out, fill and upload a plan's descriptors.  The host fills one image, each section at a 256-byte boundary: the
 // chunk descriptors, the mixtures' MixItems, the draws' DrawDescs, the staged slots' StageSlots, the tap block
 // (tap_block, with slots of tap-form pools), the streams' DryStreams and the beds' BgStreams (caller order) and the
-// clip lengths of each dry pool the streams and beds use, the layout draws' LayoutDescs and their select lengths, and
-// for loudness slots their LoudItems, work-item offsets, LoudCrops and gating tables; one copy uploads it.  Behind the image, written by the device only and never uploaded:
+// clip lengths of each dry pool the streams and beds use, the layout draws' LayoutDescs and their select lengths, the
+// value draws' ValueDescs, and for loudness slots their LoudItems, work-item offsets, LoudCrops and gating tables; one
+// copy uploads it.  Behind the image, written by the device only and never uploaded:
 // one scratch block per mixture, the staged slots' staging areas, then per loudness slot its whole stems, its loudness
 // scratch and (without a result_dev) its result.  slots[i] is caller item i's record; plan_build notes where its view,
 // its DryStream and its BgStream landed.  A loudness slot is chunked, staged and rendered as the window [0, N) into its
 // whole stems; draws and mixtures keep reading the caller's item, whose crop k_loud_crop writes.
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes,
                       std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix, const ss_plan_draw* draws,
-                      int n_draws, const ss_layout_draw* layouts, int n_layouts) {
+                      int n_draws, const ss_layout_draw* layouts, int n_layouts, const ss_value_draw* values,
+                      int n_values) {
     ss_ctx* c = p->c;
     const int n_items = (int)slots.size();
     std::vector<int> cuts, order;
@@ -2981,6 +3003,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     std::vector<size_t> lsel_off(n_layouts);             // a bed draw's select_lengths
     for (int k = 0; k < n_layouts; ++k)
         if (layouts[k].select_lengths) lsel_off[k] = take(sizeof(int32_t) * (size_t)slots[layouts[k].slot].clips()->n);
+    const size_t vdesc_off = take(sizeof(ValueDesc) * n_values);
     const int n_loud = (int)loud.size();
     std::vector<ss_post_lufs> gating(n_loud);
     for (int k = 0; k < n_loud; ++k) gating[k] = slots[loud[k]].lufs->gating;
@@ -3087,6 +3110,14 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
         g.map_cap = layout_map_cap(g.K);
         p->layout_smem = std::max(p->layout_smem, (int)sizeof(int) * layout_scratch_ints(g.K));
     }
+    for (int k = 0; k < n_values; ++k) {                 // the value draws write the caller's per-run inputs
+        const ss_value_draw& v = values[k];
+        ValueDesc& g = ((ValueDesc*)(host.data() + vdesc_off))[k];
+        g.out = v.out; g.rng = v.rng_dev;
+        g.base = v.base >= 0 ? (const int*)values[v.base].out : nullptr;
+        g.low = v.low; g.high = v.high; g.ilow = v.ilow; g.n = (uint32_t)((int64_t)v.ihigh - v.ilow);
+        g.kind = v.kind; g.k = v.k; g.r = k; g.stride = v.base >= 0 ? v.stride : 0;
+    }
     for (size_t k = 0; k < staged.size(); ++k) {
         const ss_source& it = items[staged[k]];
         PlanSlot& r = *rec[staged[k]];
@@ -3145,6 +3176,9 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     if (!mix.empty()) { p->d_mix = (const MixItem*)(d + mix_off); p->n_mix = (int)mix.size(); }
     if (n_draws > 0) { p->d_draw = (const DrawDesc*)(d + draw_off); p->n_draw = n_draws; }
     if (n_layouts > 0) { p->d_layout = (const LayoutDesc*)(d + ldesc_off); p->n_layout = n_layouts; }
+    if (n_values > 0) {
+        p->d_value = (const ValueDesc*)(d + vdesc_off); p->n_value = n_values; p->value_rows = values[0].rows;
+    }
     if (!staged.empty()) { p->d_stage = (const StageSlot*)(d + stage_off); p->n_stage = (int)staged.size(); }
     if (n_tap) {
         p->tap_ctas = ((const int*)(host.data() + tb.prefix))[n_tap];
@@ -3157,9 +3191,10 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
 
 // Byte ranges of a plan's mixtures: every range a mixture writes (mix, speakers_out, rms_db) meets no other range of
 // the plan - no other written range, no mixture's sirs / snr, nothing an item reads or writes.  One sort and one sweep.
-struct ByteRange { uintptr_t lo, hi; bool written; };
-static void add_range(std::vector<ByteRange>& r, const void* p, uint64_t bytes, bool written) {
-    if (p && bytes > 0) r.push_back({(uintptr_t)p, (uintptr_t)p + (uintptr_t)bytes, written});
+// `input`: a small per-run input that a value draw may write (validate_value_ranges).
+struct ByteRange { uintptr_t lo, hi; bool written, input; };
+static void add_range(std::vector<ByteRange>& r, const void* p, uint64_t bytes, bool written, bool input = false) {
+    if (p && bytes > 0) r.push_back({(uintptr_t)p, (uintptr_t)p + (uintptr_t)bytes, written, input});
 }
 static bool written_ranges_disjoint(std::vector<ByteRange>& r) {
     std::sort(r.begin(), r.end(), [](const ByteRange& a, const ByteRange& b) { return a.lo < b.lo; });
@@ -3207,8 +3242,9 @@ static int validate_draws(const ss_source* items, const std::vector<PlanSlot>& s
 }
 
 // (a mixture's dir_out, when not null: S * E floats written, and every speaker of the mixture needs a direct-path stem)
+// `ranges` receives every range the plan reads or writes (validate_value_ranges).
 static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix,
-                          const ss_plan_draw* draws, int n_draws) {
+                          const ss_plan_draw* draws, int n_draws, std::vector<ByteRange>& ranges) {
     const int n_items = (int)slots.size();
     if (mix.size() > 65535) return SS_ERR_UNSUPPORTED;      // one gridDim.y row per mixture
     std::vector<ByteRange> r;
@@ -3216,7 +3252,7 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
     for (int k = 0; k < n_draws; ++k) {
         add_range(r, draws[k].start, 4, true);
         add_range(r, draws[k].used, 4, true);
-        add_range(r, draws[k].u, 8 * (uint64_t)draws[k].tries, false);
+        add_range(r, draws[k].u, 8 * (uint64_t)draws[k].tries, false, true);
     }
     for (const PlanMix& m : mix) {
         if (m.S < 1 || m.M < 1 || m.S > kMixStems || m.M > kMixStems) return SS_ERR_UNSUPPORTED;
@@ -3242,8 +3278,8 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
         add_range(r, m.dir_out, 4 * E * m.S, true);
         add_range(r, m.speakers_out, 4 * E * m.S, true);
         add_range(r, m.rms_db, 4 * (uint64_t)m.S, true);
-        add_range(r, m.sirs, 4 * (uint64_t)(m.S - 1), false);
-        add_range(r, m.snr, 4, false);
+        add_range(r, m.sirs, 4 * (uint64_t)(m.S - 1), false, true);
+        add_range(r, m.snr, 4, false, true);
     }
     for (int i = 0; i < n_items; ++i) {
         const ss_source& it = items[i];
@@ -3259,8 +3295,8 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
         }
         bool drawn = false;
         for (int k = 0; k < n_draws; ++k) drawn = drawn || draws[k].start == it.win_start_dev;
-        if (!drawn) add_range(r, it.win_start_dev, 4, false);
-        add_range(r, it.pick_dev, 4, false);
+        if (!drawn) add_range(r, it.win_start_dev, 4, false, true);
+        add_range(r, it.pick_dev, 4, false, true);
     }
     // a pooled slot may read any candidate: every candidate's x and bounds, once per pool
     std::vector<const ss_pool*> pools;
@@ -3276,7 +3312,7 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
     std::vector<const ss_dry_pool*> dpools;
     for (const PlanSlot& s : slots) {
         if (s.dry) {
-            add_range(r, s.dry->pick_dev, 4, false);
+            add_range(r, s.dry->pick_dev, 4, false, true);
             if (std::find(dpools.begin(), dpools.end(), s.dry->pool) == dpools.end()) dpools.push_back(s.dry->pool);
         }
         const bool drawn = s.layout != nullptr;
@@ -3291,7 +3327,7 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
             if (std::find(dpools.begin(), dpools.end(), s.bg->pool) == dpools.end()) dpools.push_back(s.bg->pool);
         }
         if (s.lufs) {                                       // a loudness slot reads its target, writes its result
-            add_range(r, s.lufs->target_dev, 8, false);
+            add_range(r, s.lufs->target_dev, 8, false, true);
             add_range(r, s.lufs->result_dev, 16, true);
         }
     }
@@ -3309,7 +3345,9 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
                 if (o && (uintptr_t)o < hi && lo < (uintptr_t)o + n_out) return SS_ERR_INVALID;
         }
     }
-    return written_ranges_disjoint(r) ? SS_OK : SS_ERR_INVALID;
+    if (!written_ranges_disjoint(r)) return SS_ERR_INVALID;
+    ranges = std::move(r);
+    return SS_OK;
 }
 
 // A plan's dry picks (include/sonicsim_b200.h, ss_dry_pick), all but the byte ranges (validate_mixes): the record of
@@ -3434,6 +3472,63 @@ static int validate_layouts(const ss_layout_draw* layouts, int n_layouts, std::v
     return SS_OK;
 }
 
+// A plan's value draws (include/sonicsim_b200.h, ss_value_draw), all but the byte ranges (validate_value_ranges)
+static int validate_values(const ss_value_draw* values, int n_values) {
+    if (n_values > kValueDrawsMax) return SS_ERR_UNSUPPORTED;
+    std::vector<int64_t> lo(n_values), hi(n_values);    // the least and the most value of each int32 entry
+    for (int k = 0; k < n_values; ++k) {
+        const ss_value_draw& v = values[k];
+        const bool real = v.kind == SS_VALUE_F32 || v.kind == SS_VALUE_F64;
+        if (!real && v.kind != SS_VALUE_INT && v.kind != SS_VALUE_DISTINCT) return SS_ERR_INVALID;
+        const uintptr_t align = v.kind == SS_VALUE_F64 ? 8 : 4;
+        if (!v.out || ((uintptr_t)v.out & (align - 1)) || !v.rng_dev || ((uintptr_t)v.rng_dev & 7))
+            return SS_ERR_INVALID;
+        if (v.rows < 1 || v.rows > 65535 || v.rows != values[0].rows || v.k < 1 || v.k > 4096) return SS_ERR_INVALID;
+        if (real) {
+            if (!isfinite(v.low) || !isfinite(v.high) || !(v.low < v.high) || v.base != -1) return SS_ERR_INVALID;
+            if (v.kind == SS_VALUE_F32 && ((double)(float)v.low != v.low || (double)(float)v.high != v.high))
+                return SS_ERR_INVALID;
+            continue;
+        }
+        const int64_t n = (int64_t)v.ihigh - v.ilow;
+        if (n < 1 || (v.kind == SS_VALUE_DISTINCT && (v.k > 64 || v.k > n))) return SS_ERR_INVALID;
+        lo[k] = v.ilow;
+        hi[k] = (int64_t)v.ihigh - 1;
+        if (v.base == -1) continue;
+        if (v.base < 0 || v.base >= k || v.stride < 1) return SS_ERR_INVALID;
+        const ss_value_draw& b = values[v.base];
+        if ((b.kind != SS_VALUE_INT && b.kind != SS_VALUE_DISTINCT) || b.k != 1) return SS_ERR_INVALID;
+        lo[k] += lo[v.base] * v.stride;                  // |base| < 2^31 and stride < 2^31: no int64 overflow
+        hi[k] += hi[v.base] * v.stride;
+        if (lo[k] < INT32_MIN || hi[k] > INT32_MAX) return SS_ERR_INVALID;
+    }
+    return SS_OK;
+}
+
+// The byte ranges of a plan's value draws.  `ranges`: every range the rest of the plan reads or writes
+// (validate_mixes).  A value draw's out meets nothing but the small per-run inputs (picks, dry picks, undrawn starts,
+// sirs, snr, a draw's u, loudness targets): no other out, no rng, nothing else the plan reads or writes; an rng meets
+// nothing the plan writes.
+static int validate_value_ranges(const ss_source* items, int n_items, const ss_value_draw* values, int n_values,
+                                 std::vector<ByteRange> ranges) {
+    if (n_values == 0) return SS_OK;
+    ranges.erase(std::remove_if(ranges.begin(), ranges.end(), [](const ByteRange& x) { return x.input; }),
+                 ranges.end());
+    for (int k = 0; k < n_values; ++k) {
+        const ss_value_draw& v = values[k];
+        add_range(ranges, v.out, (uint64_t)v.rows * v.k * (v.kind == SS_VALUE_F64 ? 8 : 4), true);
+        add_range(ranges, v.rng_dev, 16, false);
+        const uintptr_t lo = (uintptr_t)v.rng_dev, hi = lo + 16;  // (the items' outputs count as read ranges)
+        for (int i = 0; i < n_items; ++i) {
+            const ss_source& it = items[i];
+            const uint64_t n_out = 4 * (uint64_t)it.C * (it.win_len > 0 ? it.win_len : it.N);
+            for (const float* o : {it.out, (it.flags & SS_DIRECT_TARGET) ? it.out_direct : nullptr})
+                if (o && (uintptr_t)o < hi && lo < (uintptr_t)o + n_out) return SS_ERR_INVALID;
+        }
+    }
+    return written_ranges_disjoint(ranges) ? SS_OK : SS_ERR_INVALID;
+}
+
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
 // and the byte ranges (validate_mixes): mix receives the mixtures, each with its target's direct_out, or null
 static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan_target* targets, int n_targets,
@@ -3453,11 +3548,11 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
                        const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
-                       ss_plan** out) {
+                       const ss_value_draw* values, int n_values, ss_plan** out) {
     auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
     if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
         bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs) || bad(lufs, n_lufs) ||
-        bad(layouts, n_layouts))
+        bad(layouts, n_layouts) || bad(values, n_values))
         return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
@@ -3469,9 +3564,12 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     { int st = validate_bgs(c, items, bgs, n_bgs, draws, n_draws, slots); if (st) return st; }
     { int st = validate_lufs(items, lufs, n_lufs, slots); if (st) return st; }
     { int st = validate_layouts(layouts, n_layouts, slots); if (st) return st; }
+    { int st = validate_values(values, n_values); if (st) return st; }
     { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
     { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
-    { int st = validate_mixes(items, slots, mix, draws, n_draws); if (st) return st; }
+    std::vector<ByteRange> ranges;
+    { int st = validate_mixes(items, slots, mix, draws, n_draws, ranges); if (st) return st; }
+    { int st = validate_value_ranges(items, n_items, values, n_values, std::move(ranges)); if (st) return st; }
     *out = nullptr;
     ss_plan* p = new (std::nothrow) ss_plan();
     if (!p) return SS_ERR_NOMEM;
@@ -3482,7 +3580,8 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         ss_pool* pl = const_cast<ss_pool*>(items[i].pool);
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
-    const int st = plan_build(p, items, shapes.data(), slots, mix, draws, n_draws, layouts, n_layouts);
+    const int st = plan_build(p, items, shapes.data(), slots, mix, draws, n_draws, layouts, n_layouts, values,
+                              n_values);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -3491,26 +3590,26 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
     return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3518,7 +3617,7 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3526,7 +3625,7 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
@@ -3535,7 +3634,7 @@ extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items,
                                  int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                  int n_bgs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3544,7 +3643,7 @@ extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_item
                                    int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                    int n_bgs, const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3554,14 +3653,24 @@ extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_it
                                      int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
                                      int n_layouts, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_values(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                     int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                     const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                     int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
+                                     int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
+                                     int n_layouts, const ss_value_draw* values, int n_values, ss_plan** out) {
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
@@ -3574,11 +3683,18 @@ static int draw_enqueue(ss_ctx* c, const DrawDesc* d, int n, bool i16, bool stre
     return SS_OK;
 }
 
-// the layout draws, the start draws (which walk stream layouts), the host-pool staging, the launches of every chunk
+// the value draws (whose values everything after them may read), the layout draws, the start draws (which walk stream
+// layouts), the host-pool staging, the launches of every chunk
 // (run_chunks), the loudness slots' measurements and crops, then the mixtures (which read every chunk's outputs and the
 // crops) on `stream`
 static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
     ss_ctx* c = p->c;
+    if (p->n_value) {
+        k_values<<<(p->value_rows + kValueWarps - 1) / kValueWarps, 32 * kValueWarps, 0, stream>>>(p->d_value, p->n_value,
+                                                                                                p->value_rows);
+        CK(cudaGetLastError());
+        c->launches += 1;
+    }
     if (p->n_layout) {
         k_layout<<<p->n_layout, 32, p->layout_smem, stream>>>(p->d_layout);
         CK(cudaGetLastError());

@@ -841,6 +841,99 @@ SS_HD void layout_row(const LayoutDesc& d, int* keys, int* vals, int* sel) {
     }
 }
 
+// ---- value draws (ss_value_draw, include/sonicsim_b200.h): a plan writes the per-run values its slots, draws,
+// mixtures and loudness slots read (picks, starts, SIRs, SNRs, crop variates, loudness targets) itself at the head of
+// every run (k_values), from the generator of the layout draws.  The random stream is a format, followed word for word
+// by the kernel, the CPU emulation and the tests' Python restatement:
+//   - the key is the 64-bit seed (seed_lo, seed_hi), as for layout draws;
+//   - element j of row b of value draw r (its index in the plan's list of value draws) at counter t takes block
+//     philox(ctr = (b, 0x80000000 | r << 11 | j >> 1, t_lo, t_hi), key) and its words 2 (j & 1) and 2 (j & 1) + 1 as
+//     x = w0 | w1 << 32.  Layout draws use c1 = r < 2^31, so the two streams never share a block (r < 2^20, k <= 4096);
+//   - float64: u = (x >> 11) * 2^-53; float32: u = (x >> 40) * 2^-24; v = low + (high - low) * u in float64 (product
+//     and sum rounded separately), rounded once to the output type; a result not below high becomes the largest value
+//     of the type below high;
+//   - int32: low + umulhi64(x, high - low);
+//   - distinct: a partial Fisher-Yates over [0, n), n = high - low: element j takes y = umulhi64(x_j, n - j) and
+//     pos = j + y, writes low + a[pos] and sets a[pos] = a[j] (a: the identity, held as a sparse map);
+//   - with a base draw, the value is base[b] * stride + value (int64; creation rules out int32 overflow).
+// Every element is independent of the others except within a distinct row.
+enum { VALUE_F32 = 0, VALUE_F64 = 1, VALUE_INT = 2, VALUE_DISTINCT = 3 };
+constexpr int kValueDrawsMax = 1 << 20;                // r < 2^20: r << 11 stays below bit 31
+constexpr int kValueMapCap = 128;                      // sparse Fisher-Yates map of a distinct row: >= 2k keys, k <= 64
+struct ValueDesc {
+    void* out;                                         // rows x k elements of the kind's type
+    const int64_t* rng;                                // (seed, t)
+    const int* base;                                   // int kinds: the (rows,) out of an earlier draw, or null
+    double low, high;                                  // real kinds
+    int ilow;                                          // int kinds: low
+    uint32_t n;                                        // int kinds: high - low
+    int kind, k, r, stride;
+};
+static_assert(sizeof(ValueDesc) == 64, "ValueDesc layout");
+SS_HD uint64_t value_word(uint32_t k0, uint32_t k1, uint32_t t0, uint32_t t1, int r, int b, int j) {
+    const uint4 w = philox4x32_10(make_uint4((uint32_t)b, 0x80000000u | (uint32_t)r << 11 | (uint32_t)j >> 1, t0, t1),
+                                  k0, k1);
+    return (j & 1) ? (w.z | (uint64_t)w.w << 32) : (w.x | (uint64_t)w.y << 32);
+}
+// low + (high - low) * u, the product and the sum each rounded once
+SS_HD double value_lerp(double low, double high, double u) {
+#if defined(__CUDA_ARCH__)
+    return __dadd_rn(low, __dmul_rn(high - low, u));
+#else
+    return low + (high - low) * u;
+#endif
+}
+// The float64 and the float32 value of word x in [low, high)
+SS_HD double value_f64(double low, double high, uint64_t x) {
+    const double v = value_lerp(low, high, (double)(x >> 11) * 0x1p-53);
+    return v < high ? v : nextafter(high, -(double)INFINITY);
+}
+SS_HD float value_f32(double low, double high, uint64_t x) {
+    const float v = (float)value_lerp(low, high, (double)(x >> 40) * 0x1p-24);
+    return v < (float)high ? v : nextafterf((float)high, -INFINITY);
+}
+SS_HD unsigned vmap_slot(uint32_t i) { return (i * 2654435769u) >> 25; }   // 7 bits: kValueMapCap slots
+SS_HD uint32_t vmap_get(const uint32_t* keys, const uint32_t* vals, uint32_t i) {
+    for (unsigned h = vmap_slot(i);; h = (h + 1) & (kValueMapCap - 1)) {
+        if (keys[h] == i) return vals[h];
+        if (keys[h] == 0xFFFFFFFFu) return i;
+    }
+}
+SS_HD void vmap_put(uint32_t* keys, uint32_t* vals, uint32_t i, uint32_t v) {
+    for (unsigned h = vmap_slot(i);; h = (h + 1) & (kValueMapCap - 1))
+        if (keys[h] == i || keys[h] == 0xFFFFFFFFu) { keys[h] = i; vals[h] = v; return; }
+}
+// Row b of value draw d: lane `lane` of `lanes` writes elements lane, lane + lanes, ...; a distinct row is drawn by
+// lane 0 alone over the kValueMapCap keys and values of its map (the others return).  A base draw's row b must be
+// written and visible before this call.
+SS_HD void value_row(const ValueDesc& d, int b, int lane, int lanes, uint32_t* keys, uint32_t* vals) {
+    const uint64_t seed = (uint64_t)d.rng[0], t = (uint64_t)d.rng[1];
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32), t0 = (uint32_t)t, t1 = (uint32_t)(t >> 32);
+    const size_t row = (size_t)b * d.k;
+    if (d.kind == VALUE_F32 || d.kind == VALUE_F64) {
+        for (int j = lane; j < d.k; j += lanes) {
+            const uint64_t x = value_word(k0, k1, t0, t1, d.r, b, j);
+            if (d.kind == VALUE_F64) static_cast<double*>(d.out)[row + j] = value_f64(d.low, d.high, x);
+            else static_cast<float*>(d.out)[row + j] = value_f32(d.low, d.high, x);
+        }
+        return;
+    }
+    const int64_t add = (int64_t)d.ilow + (d.base ? (int64_t)d.base[b] * d.stride : 0);
+    int* const out = static_cast<int*>(d.out) + row;
+    if (d.kind == VALUE_INT) {
+        for (int j = lane; j < d.k; j += lanes)
+            out[j] = (int)(add + (int64_t)umulhi64(value_word(k0, k1, t0, t1, d.r, b, j), d.n));
+        return;
+    }
+    if (lane) return;
+    for (int i = 0; i < kValueMapCap; ++i) keys[i] = 0xFFFFFFFFu;
+    for (int j = 0; j < d.k; ++j) {
+        const uint32_t pos = (uint32_t)j + (uint32_t)umulhi64(value_word(k0, k1, t0, t1, d.r, b, j), d.n - (uint32_t)j);
+        out[j] = (int)(add + vmap_get(keys, vals, pos));
+        vmap_put(keys, vals, pos, vmap_get(keys, vals, (uint32_t)j));
+    }
+}
+
 // blocks of the table that meet the window: [win_first(s), win_first(s) + win_blocks(s)); all of them when unwindowed
 SS_HD int win_first(const Source& s) { return s.h_rows ? s.counts[2] : 0; }
 SS_HD int win_blocks(const Source& s) { return s.h_rows ? s.counts[3] : s.counts[0]; }

@@ -5,6 +5,7 @@ has no such symbols.  They render many (utterance, source) units with one C-ABI 
 (ss_render_host / ss_render_dev) instead of the reference's serial per-source loop
 (SonicSet.py:77-94).  Host arrays in / out by default; `Renderer.render_device` takes CUDA tensors.
 """
+import collections
 import ctypes
 import math
 import typing as T
@@ -206,6 +207,34 @@ class LayoutDraw(T.NamedTuple):
     total: int
     sample_rate: int = 16000
     select_lengths: T.Any = None
+
+
+class ValueDraw(T.NamedTuple):
+    """Per-run values that a device plan draws itself at the head of every run (Renderer.plan_device(values=...)), in
+    one kernel launch before everything that reads them: the picks, dry picks, crop starts, SIRs, SNRs, CropDraw
+    variates and StemLoudness targets that a training loop would otherwise refresh with torch before plan.run().
+    `out`: a contiguous CUDA tensor of shape (B,) or (B, k), 1 <= k <= 4096, written at every run; the plan's other
+    parts read it as they read any such tensor.  float32 / float64: uniform reals in [low, high) (float32 bounds must be
+    exact in float32); int32: uniform integers in [low, high).  `rng`: a two-element CUDA int64 tensor (seed, t) read at
+    every run and never written, as LayoutDraw.rng (one tensor may serve every draw): a training step is then
+
+        rng[1] += 1
+        plan.run()
+
+    and the batch is a pure function of (seed, t).  `distinct` (int32 only, k <= min(64, high - low)): each row is an
+    ordered sample without replacement, as random.sample(range(low, high), k).  `base` (int32 only): the `out`, of shape
+    (B,), of an earlier int32 ValueDraw of the same plan; the values become base[b] * stride + value (stride >= 1), e.g.
+    speaker picks within the scene a first draw chose, over scene-major pools.  Draw r of `values` takes Philox4x32-10
+    blocks under the key seed in a stream of its own (include/sonicsim_b200.h, ss_value_draw, states it), apart from
+    the layout draws' blocks.  Every ValueDraw of a plan has the same B, at most 65535.  The values match the rules in
+    distribution, not torch's or `random`'s bits."""
+    out: T.Any
+    rng: T.Any
+    low: float = 0.0
+    high: float = 1.0
+    distinct: bool = False
+    base: T.Any = None
+    stride: int = 0
 
 
 class CropDraw(T.NamedTuple):
@@ -1073,7 +1102,8 @@ class Renderer:
             stream = torch.cuda.current_stream(self.device).cuda_stream
         _lib.check(self.lib.ss_render_dev(self.ctx, items, n, ctypes.c_void_p(stream)))
 
-    def plan_device(self, sources, outs, direct_outs=None, mixtures=None, draws=None, layouts=None) -> "DevicePlan":
+    def plan_device(self, sources, outs, direct_outs=None, mixtures=None, draws=None, layouts=None,
+                    values=None) -> "DevicePlan":
         """Bind a batch of device-resident sources to its output tensors once; `plan.run()` then renders it with a
         single C-ABI call - one CUDA graph launch (ss_plan_run; a generation loop overwrites the same tensors and
         calls run() again).  Every tensor must be a contiguous CUDA tensor of this renderer's device: float32 dry
@@ -1111,10 +1141,25 @@ class Renderer:
         pool at every run (ss_plan_create_bg; dry.background_audio_layouts into the four arrays before the run).
 
         `layouts`: LayoutDraw entries, stream and bed slots whose layouts the plan draws itself at the head of every run
-        (ss_plan_create_layout, one kernel launch more per run) instead of the caller's refresh: a step is then
+        (ss_plan_create_layout, one kernel launch more per run) instead of the caller's refresh.
 
-            rng[1] += 1; u.uniform_(); picks.copy_(...); sirs.uniform_(-6, 6); snr.uniform_(10, 20)
-            plan.run()"""
+        `values`: ValueDraw entries, the per-run values (picks, dry picks, starts, sirs, snr, a CropDraw's u, StemLoudness
+        targets) that the plan draws itself at the head of every run (ss_plan_create_values, one kernel launch more per
+        run).  With scene-major speaker pools (3 candidates per scene) and per-scene noise pools, the separation step
+        (movingdatamodule.py:56-126) is
+
+            values = [ValueDraw(scene, rng, 0, SCENES),                 # random.choice; noise slots pick scene[b]
+                      ValueDraw(picks, rng, 0, 3, distinct=True, base=scene, stride=3),   # random.sample(range(1, 4), S)
+                      ValueDraw(sirs, rng, -6, 6), ValueDraw(snr, rng, 10, 20),
+                      ValueDraw(u, rng)]                                # CropDraw variates, (B, 101) float64
+            plan = R.plan_device(srcs, outs, mixtures=mixes, draws=draws, layouts=layouts, values=values)
+            ...
+            rng[1] += 1                                                 # the whole step's randomness
+            plan.run()
+
+        Plain starts (`ValueDraw(starts, rng, 0, N - length + 1)`), dry picks and loudness targets (float64, e.g.
+        U(-19, -15) for speech, U(-26, -22) for noise and U(-31, -27) for music, one tensor per range) are drawn the same
+        way."""
         dry = self._device_dry(sources)
         streams = self._device_streams(sources)
         bgs = self._device_bgs(sources)
@@ -1124,8 +1169,11 @@ class Renderer:
         drw = self._device_draws(draws, sources, keep) if draws else None
         lufs = self._device_lufs(sources, (outs, direct_outs, mixtures, draws), keep)
         lay = self._device_layouts(layouts, sources, (outs, direct_outs, mixtures, draws), keep) if layouts else None
+        val = self._device_values(values, sources, (outs, direct_outs, mixtures, draws, layouts), keep) \
+            if values else None
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
-                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs, lay)
+                          (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs, lay,
+                          val)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1353,6 +1401,119 @@ class Renderer:
             if any(a < hi and lo < b for a, b in map(span, written)):
                 raise ValueError("plan_device: a layout draw's rng meets a tensor the plan writes")
         keep.append(list(layouts))
+        return arr
+
+    def _device_values(self, values, sources, others, keep):
+        """Validated ss_value_draw array of a plan's value draws.  `others`: the plan's other arguments; a drawn `out`
+        meets none of their tensors but the small per-run inputs it may write."""
+        import torch
+        kinds = {torch.float32: _lib.SS_VALUE_F32, torch.float64: _lib.SS_VALUE_F64, torch.int32: _lib.SS_VALUE_INT}
+        if len(values) > 1 << 20:
+            raise ValueError("plan_device: at most 2^20 value draws, got %d" % len(values))
+        arr = (_lib.SsValueDraw * len(values))()
+        span_of = []                                   # int32 draws: (least, most) value
+        rows = None
+        for r, v in enumerate(values):
+            own = "value draw %d" % r
+            if not isinstance(v, ValueDraw):
+                raise ValueError("plan_device: %s must be a ValueDraw" % own)
+            o = v.out
+            if not _is_tensor(o) or o.dtype not in kinds:
+                raise ValueError("plan_device: the out of %s must be a float32, float64 or int32 CUDA tensor" % own)
+            _tensor(o, "plan_device", own, "out", o.dtype, self.device)
+            if o.dim() not in (1, 2) or not 1 <= o.shape[0] <= 65535 or (o.dim() == 2 and not 1 <= o.shape[1] <= 4096):
+                raise ValueError("plan_device: the out of %s must have shape (B,) or (B, k) with 1 <= B <= 65535 and "
+                                 "1 <= k <= 4096, got %s" % (own, tuple(o.shape)))
+            B, k = int(o.shape[0]), int(o.shape[1]) if o.dim() == 2 else 1
+            if rows is not None and B != rows:
+                raise ValueError("plan_device: %s has %d rows, value draw 0 has %d: every value draw of a plan has the "
+                                 "same B" % (own, B, rows))
+            rows = B
+            rng = _tensor(v.rng, "plan_device", own, "rng", torch.int64, self.device, count=(2, 2))
+            if rng % 8:
+                raise ValueError("plan_device: the rng of %s must be 8-byte aligned" % own)
+            kind = kinds[o.dtype]
+            e = _lib.SsValueDraw(out=o.data_ptr(), rng_dev=rng, kind=kind, rows=B, k=k, base=-1)
+            if kind != _lib.SS_VALUE_INT:
+                low, high = float(v.low), float(v.high)
+                if not (np.isfinite(low) and np.isfinite(high) and low < high):
+                    raise ValueError("plan_device: %s needs finite low < high, got [%r, %r)" % (own, v.low, v.high))
+                if kind == _lib.SS_VALUE_F32 and (float(np.float32(low)) != low or float(np.float32(high)) != high):
+                    raise ValueError("plan_device: the bounds of float32 %s must be exact in float32, got [%r, %r)"
+                                     % (own, low, high))
+                if v.distinct or v.base is not None or v.stride:
+                    raise ValueError("plan_device: distinct, base and stride are for int32 draws only (%s)" % own)
+                e.low, e.high = low, high
+                span_of.append(None)
+            else:
+                low, high = v.low, v.high
+                if int(low) != low or int(high) != high or not -(1 << 31) <= int(low) < int(high) < 1 << 31:
+                    raise ValueError("plan_device: int32 %s needs integer bounds -2^31 <= low < high < 2^31, got "
+                                     "[%r, %r)" % (own, v.low, v.high))
+                low, high = int(low), int(high)
+                if v.distinct:
+                    if k > 64 or k > high - low:
+                        raise ValueError("plan_device: distinct %s samples k = %d of %d values, at most min(64, "
+                                         "high - low)" % (own, k, high - low))
+                    e.kind = _lib.SS_VALUE_DISTINCT
+                e.ilow, e.ihigh = low, high
+                lo, hi = low, high - 1
+                if v.base is not None:
+                    j = next((j for j in range(r) if values[j].out is v.base), None)
+                    if j is None or span_of[j] is None or values[j].out.numel() != B:
+                        raise ValueError("plan_device: the base of %s must be the (B,) out of an earlier int32 value "
+                                         "draw" % own)
+                    if int(v.stride) < 1:
+                        raise ValueError("plan_device: %s needs stride >= 1 with a base, got %r" % (own, v.stride))
+                    lo, hi = lo + span_of[j][0] * int(v.stride), hi + span_of[j][1] * int(v.stride)
+                    if lo < -(1 << 31) or hi >= 1 << 31:
+                        raise ValueError("plan_device: base * stride + value of %s may overflow int32" % own)
+                    e.base, e.stride = j, int(v.stride)
+                elif v.stride:
+                    raise ValueError("plan_device: %s has a stride but no base" % own)
+                span_of.append((lo, hi))
+            arr[r] = e
+        # an out meets nothing the plan reads or writes but the small per-run inputs; an rng meets nothing written
+        outs, direct_outs, mixtures, draws, layouts = others
+        starts = [d.start.data_ptr() for d in draws or () if _is_tensor(d.start)]
+        lufs = [q for s in sources for q in [getattr(getattr(s, "dry", None), "lufs", None)] if q is not None]
+        inputs = [q.target for q in lufs]
+        stems = []                                     # (a DryStream's lufs lies outside its tuple)
+        for s in sources:
+            if not isinstance(s, Pooled):
+                continue
+            inputs.append(s.pick)
+            if _is_tensor(s.window[0]) and s.window[0].data_ptr() not in starts:
+                inputs.append(s.window[0])
+            if isinstance(s.dry, DryPick):
+                inputs.append(s.dry.pick)
+            if isinstance(s.dry, DryStream) and s.dry.lufs is not None:
+                stems.append(s.dry.lufs)
+        inputs += [t for m in mixtures or () for t in (m.sirs, m.snr)] + [d.u for d in draws or ()]
+        every = _cuda_tensors((sources, others, stems))
+        uses = collections.Counter(id(t) for t in every)
+        uses.subtract(id(t) for t in inputs if _is_tensor(t))
+        span = lambda t: (t.data_ptr(), t.data_ptr() + t.numel() * t.element_size())   # noqa: E731
+        meets = lambda a, b: a[0] < b[1] and b[0] < a[1]                                  # noqa: E731
+        other = [span(t) for t in every if uses[id(t)] > 0]
+        drawn = [span(v.out) for v in values]
+        rngs = [span(v.rng) for v in values]
+        for r, a in enumerate(drawn):
+            if any(meets(a, b) for b in other + rngs) or any(meets(a, b) for b in drawn[:r]):
+                raise ValueError("plan_device: the out of value draw %d meets another tensor of the plan (only picks, "
+                                 "dry picks, starts, sirs, snr, a CropDraw's u and StemLoudness targets may be drawn)" % r)
+        written = [span(t) for t in _cuda_tensors((outs, direct_outs, [q.result for q in lufs],
+                                                   [(m.mix, m.speakers_out, m.rms_db, m.direct_out)
+                                                    for m in mixtures or ()],
+                                                   [(d.start, d.used) for d in draws or ()]))]
+        for d in layouts or ():
+            w = sources[int(d.slot)].dry
+            written += [span(t) for t in (w.ids, w.offsets) + ((w.heads, w.counts) if isinstance(w, BackgroundStream)
+                                                               else ()) if _is_tensor(t)]
+        for r, a in enumerate(rngs):
+            if any(meets(a, b) for b in written):
+                raise ValueError("plan_device: the rng of value draw %d meets a tensor the plan writes" % r)
+        keep.append(list(values))
         return arr
 
     @staticmethod
@@ -1589,21 +1750,25 @@ class DevicePlan:
     dry-picked slots take their dry signals from dry pools, with pair gains their gains from pair-gain tables; with
     dereverberation targets its mixtures also write those, with stream slots it lays out their dry streams and with bed
     slots their noise and music beds, with loudness slots it measures their whole stems at every run, with layout draws
-    it draws its stream and bed layouts at every run.  Every plan is created by ss_plan_create_layout, with NULL and a
+    it draws its stream and bed layouts at every run, with value draws it draws its per-run inputs at every run.  A plan
+    with value draws is created by ss_plan_create_values, every other plan by ss_plan_create_layout, with NULL and a
     count of 0 for each part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
-                 streams=None, bgs=None, lufs=None, layouts=None):
+                 streams=None, bgs=None, lufs=None, layouts=None, values=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
-        self.bgs, self.lufs, self.layouts = bgs, lufs, layouts
+        self.bgs, self.lufs, self.layouts, self.values = bgs, lufs, layouts, values
         self._plan = ctypes.c_void_p()
         if n > 0:
-            _lib.check(renderer.lib.ss_plan_create_layout(
-                renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
-                pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
-                len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, lufs, len(lufs) if lufs else 0,
-                layouts, len(layouts) if layouts else 0, ctypes.byref(self._plan)))
+            args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
+                    pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
+                    len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, lufs, len(lufs) if lufs else 0,
+                    layouts, len(layouts) if layouts else 0)
+            if values:
+                _lib.check(renderer.lib.ss_plan_create_values(*args, values, len(values), ctypes.byref(self._plan)))
+            else:
+                _lib.check(renderer.lib.ss_plan_create_layout(*args, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
