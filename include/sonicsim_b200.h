@@ -336,8 +336,9 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * (rendered clamped into that range), bit 3 (version 106) = a pooled slot's pick outside [0, n) (clamped), bit 4 (dry
  * pools, below) = a dry pick outside [0, n) of its dry pool (clamped), bit 5 (dry streams and background streams,
  * below) = an invalid entry of a stream or bed slot's layout (skipped), bit 6 (loudness slots, ss_stream_lufs below) =
- * a loudness target read at a run that was not finite (that slot stored unscaled).  The Python device API raises IndexError /
- * ValueError from it on request
+ * a loudness target read at a run that was not finite (that slot stored unscaled), bit 7 (speaker groups,
+ * ss_layout_group below) = a grouped layout draw's group outside [0, G) (clamped).  The Python device API raises
+ * IndexError / ValueError from it on request
  * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
  * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
 int ss_device_errors(ss_ctx* ctx, uint32_t* bits);
@@ -956,6 +957,47 @@ int ss_plan_create_values(ss_ctx* ctx, const ss_source* items, int n_items, cons
                           int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
                           const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
                           const ss_value_draw* values, int n_values, ss_plan** out);
+
+/* ---- speaker groups of layout draws: SonicSet builds every speech stream from one LibriSpeech speaker's utterances
+ * (create_long_audio(audio_path, 60) over a speaker directory, SonicSim_audio.py:243; SonicSet.py:198 picks three
+ * different speakers per scene).  A grouped layout draw lays its stream slot out from one contiguous group of its
+ * pool's utterances, named at every run by a device int32, instead of from the whole pool.
+ * Rule and random stream (ss_phases.cuh states it once): the pool's n utterances are split into G >= 1 groups by host
+ * bounds 0 = bounds[0] < bounds[1] < ... < bounds[G] = n.  At every run the draw reads g from group_dev:
+ *   - g outside [0, G) is clamped into range and ss_device_errors reports bit 7;
+ *   - the row is exactly the ungrouped draw r (ss_layout_draw above) over a pool holding only utterances
+ *     [bounds[g], bounds[g + 1]) in order: the same Philox blocks (b, r, t_lo, t_hi), the same words in the same order;
+ *     every id it writes is offset by bounds[g];
+ *   - reading g consumes no words.
+ * So G = 1 is the ungrouped draw, and group g over the whole pool is the ungrouped draw over that group's sub-pool with
+ * its ids shifted.  A value draw (SS_VALUE_DISTINCT over [0, G)) may write group_dev: the scene's S distinct speakers of
+ * np.random.choice(speech_list, S, replace=False).  K (the most a row can select) is the largest K of the groups.
+ * Stream slots only: SonicSet's beds draw from the split's whole clip JSON.
+ * ss_plan_create_groups is ss_plan_create_values with n_grouped entries (n_grouped == 0: exactly
+ * ss_plan_create_values).  A plan with grouped draws launches as many kernels per run as the same plan without groups
+ * (k_layout_grouped instead of k_layout).  Refused at creation, before anything is allocated and with *out untouched:
+ *   - SS_ERR_INVALID:
+ *     - n_grouped < 0, or NULL groups with n_grouped > 0;
+ *     - a layout index outside [0, n_layouts), or one that two entries name;
+ *     - the draw of a bed slot;
+ *     - n_groups < 1, NULL bounds, or bounds that do not ascend strictly from 0 to the pool's n;
+ *     - a NULL or misaligned (4 bytes) group_dev;
+ *     - a group_dev that meets a range the plan writes other than a value draw's out.
+ *   - SS_ERR_UNSUPPORTED: K above 1024 in any group.
+ * ss_version stays 108: the export marks the capability. */
+typedef struct {
+    int32_t layout;                   /* index into `layouts`: the draw of a stream slot                              */
+    int32_t n_groups;                 /* G >= 1                                                                       */
+    const int32_t* bounds;            /* host, G + 1 entries, 0 = bounds[0] < ... < bounds[G] = the pool's n          */
+    const int32_t* group_dev;         /* device, one int32 read at every run                                          */
+} ss_layout_group;
+int ss_plan_create_groups(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                          const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                          const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                          int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                          const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
+                          const ss_value_draw* values, int n_values, const ss_layout_group* groups, int n_grouped,
+                          ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

@@ -1197,6 +1197,7 @@ struct PlanSlot {
     const ss_bg_stream* bg = nullptr;
     const ss_stream_lufs* lufs = nullptr;   // a loudness slot's target (validate_lufs), or null
     const ss_layout_draw* layout = nullptr; // a drawn slot's layout draw (validate_layouts), or null
+    const ss_layout_group* group = nullptr; // a drawn stream slot's speaker groups (validate_layouts), or null
     StageView* view = nullptr;
     const DryStream* ws = nullptr;
     const BgStream* wb = nullptr;
@@ -2499,6 +2500,8 @@ struct ss_plan {
     // scratch any of them needs
     const LayoutDesc* d_layout = nullptr;
     int n_layout = 0, layout_smem = 0;
+    // with grouped layout draws (ss_layout_group): one LayoutGroup per layout draw (k_layout_grouped), or null
+    const LayoutGroup* d_layout_group = nullptr;
     // value draws (ss_value_draw): their descriptors (k_values) in d_desc, and the rows every one of them has
     const ValueDesc* d_value = nullptr;
     int n_value = 0, value_rows = 0;
@@ -2607,6 +2610,22 @@ __global__ void __launch_bounds__(32) k_layout(const LayoutDesc* __restrict__ de
     for (int i = threadIdx.x; i < cap; i += 32) scratch[i] = -1;
     __syncwarp();
     if (threadIdx.x == 0) layout_row(d, scratch, scratch + cap, scratch + 2 * cap);
+}
+
+// Layout draws of a plan with grouped draws (ss_layout_group), launched instead of k_layout: one warp per draw, as
+// k_layout, each grouped draw narrowed to its group's utterances (layout_row_grouped; groups[i].group null: k_layout's
+// row).  A clamped group sets bit 7.
+__global__ void __launch_bounds__(32) k_layout_grouped(const LayoutDesc* __restrict__ descs,
+                                                       const LayoutGroup* __restrict__ groups) {
+    extern __shared__ int scratch[];
+    const LayoutDesc d = descs[blockIdx.x];
+    const int cap = d.map_cap;
+    for (int i = threadIdx.x; i < cap; i += 32) scratch[i] = -1;
+    __syncwarp();
+    if (threadIdx.x == 0) {
+        const unsigned err = layout_row_grouped(d, groups[blockIdx.x], scratch, scratch + cap, scratch + 2 * cap);
+        if (err) atomicOr(&g_dev_err, err);
+    }
 }
 
 // ----------------------------------------------------------------------------- k_values
@@ -2914,7 +2933,22 @@ static StageArea stage_area_of(const ss_source& it) {
 // K of a layout draw (ss_layout_draw): the most a row can select.  A stream: the largest k whose k shortest utterances
 // fit in `total` (at least 1).  A bed: the most clips whose selection lengths stay below 0.4 * total, plus the one that
 // crosses it (at most n).
-static int64_t layout_bound(const ss_layout_draw& L, const ss_dry_pool* dp, bool bed) {
+static int64_t layout_bound(const ss_layout_draw& L, const ss_dry_pool* dp, bool bed,
+                            const ss_layout_group* grp = nullptr) {
+    if (grp) {                                          // a grouped stream: the largest K of its groups
+        int64_t K = 1;
+        for (int g = 0; g < grp->n_groups; ++g) {
+            std::vector<int64_t> v(dp->N.begin() + grp->bounds[g], dp->N.begin() + grp->bounds[g + 1]);
+            std::sort(v.begin(), v.end());
+            int64_t acc = 0, k = 0;
+            for (int64_t l : v) {
+                if (acc + l > L.total) break;
+                acc += l; ++k;
+            }
+            K = std::max(K, k);
+        }
+        return K;
+    }
     std::vector<int64_t> v(dp->N.begin(), dp->N.end());
     if (L.select_lengths) v.assign(L.select_lengths, L.select_lengths + dp->n);
     std::sort(v.begin(), v.end());
@@ -2939,7 +2973,7 @@ static int64_t layout_bound(const ss_layout_draw& L, const ss_dry_pool* dp, bool
 static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* caller_shapes,
                       std::vector<PlanSlot>& slots, const std::vector<PlanMix>& mix, const ss_plan_draw* draws,
                       int n_draws, const ss_layout_draw* layouts, int n_layouts, const ss_value_draw* values,
-                      int n_values) {
+                      int n_values, const ss_layout_group* groups, int n_grouped) {
     ss_ctx* c = p->c;
     const int n_items = (int)slots.size();
     std::vector<int> cuts, order;
@@ -3003,6 +3037,9 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     std::vector<size_t> lsel_off(n_layouts);             // a bed draw's select_lengths
     for (int k = 0; k < n_layouts; ++k)
         if (layouts[k].select_lengths) lsel_off[k] = take(sizeof(int32_t) * (size_t)slots[layouts[k].slot].clips()->n);
+    const size_t lgrp_off = n_grouped ? take(sizeof(LayoutGroup) * n_layouts) : 0;   // with grouped draws: one each
+    std::vector<size_t> gb_off(n_grouped);                // a grouped draw's bounds
+    for (int j = 0; j < n_grouped; ++j) gb_off[j] = take(sizeof(int32_t) * ((size_t)groups[j].n_groups + 1));
     const size_t vdesc_off = take(sizeof(ValueDesc) * n_values);
     const int n_loud = (int)loud.size();
     std::vector<ss_post_lufs> gating(n_loud);
@@ -3106,9 +3143,15 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
             g.heads = const_cast<int*>(r.bg->heads_dev); g.counts = const_cast<int*>(r.bg->counts_dev); g.m = r.bg->m;
         }
         g.n = dp->n; g.total = L.total; g.gap_max = 10 * L.sample_rate; g.r = k;
-        g.K = (int)layout_bound(L, dp, r.bg != nullptr);
+        g.K = (int)layout_bound(L, dp, r.bg != nullptr, r.group);
         g.map_cap = layout_map_cap(g.K);
         p->layout_smem = std::max(p->layout_smem, (int)sizeof(int) * layout_scratch_ints(g.K));
+    }
+    for (int j = 0; j < n_grouped; ++j) {                // grouped draws: their group and bounds (others: null)
+        const ss_layout_group& q = groups[j];
+        memcpy(host.data() + gb_off[j], q.bounds, sizeof(int32_t) * ((size_t)q.n_groups + 1));
+        LayoutGroup& e = ((LayoutGroup*)(host.data() + lgrp_off))[q.layout];
+        e.group = q.group_dev; e.bounds = (const int*)(d + gb_off[j]); e.G = q.n_groups;
     }
     for (int k = 0; k < n_values; ++k) {                 // the value draws write the caller's per-run inputs
         const ss_value_draw& v = values[k];
@@ -3176,6 +3219,7 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     if (!mix.empty()) { p->d_mix = (const MixItem*)(d + mix_off); p->n_mix = (int)mix.size(); }
     if (n_draws > 0) { p->d_draw = (const DrawDesc*)(d + draw_off); p->n_draw = n_draws; }
     if (n_layouts > 0) { p->d_layout = (const LayoutDesc*)(d + ldesc_off); p->n_layout = n_layouts; }
+    if (n_grouped > 0) p->d_layout_group = (const LayoutGroup*)(d + lgrp_off);
     if (n_values > 0) {
         p->d_value = (const ValueDesc*)(d + vdesc_off); p->n_value = n_values; p->value_rows = values[0].rows;
     }
@@ -3317,6 +3361,7 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
         }
         const bool drawn = s.layout != nullptr;
         if (drawn) add_range(r, s.layout->rng_dev, 16, false);
+        if (s.group) add_range(r, s.group->group_dev, 4, false, true);   // (a value draw may write it)
         if (s.strm) {
             add_range(r, s.strm->ids_dev, 4 * (uint64_t)s.strm->m, drawn);
             add_range(r, s.strm->offsets_dev, 4 * (uint64_t)s.strm->m, drawn);
@@ -3334,15 +3379,18 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
         if (!dp->padded())
             for (int i = 0; i < dp->n; ++i) add_range(r, dp->x[i], 4 * (uint64_t)dp->N[i], false);
-    // the items' outputs count as read above (mixtures read them); a layout draw's rng meets none of them either
+    // the items' outputs count as read above (mixtures read them); a layout draw's rng and group meet none of them
+    // either
     for (const PlanSlot& s : slots) {
         if (!s.layout) continue;
-        const uintptr_t lo = (uintptr_t)s.layout->rng_dev, hi = lo + 16;
-        for (int i = 0; i < n_items; ++i) {
-            const ss_source& it = items[i];
-            const uint64_t n_out = 4 * (uint64_t)it.C * (it.win_len > 0 ? it.win_len : it.N);
-            for (const float* o : {it.out, (it.flags & SS_DIRECT_TARGET) ? it.out_direct : nullptr})
-                if (o && (uintptr_t)o < hi && lo < (uintptr_t)o + n_out) return SS_ERR_INVALID;
+        for (int q = 0; q < (s.group ? 2 : 1); ++q) {
+            const uintptr_t lo = q ? (uintptr_t)s.group->group_dev : (uintptr_t)s.layout->rng_dev, hi = lo + (q ? 4 : 16);
+            for (int i = 0; i < n_items; ++i) {
+                const ss_source& it = items[i];
+                const uint64_t n_out = 4 * (uint64_t)it.C * (it.win_len > 0 ? it.win_len : it.N);
+                for (const float* o : {it.out, (it.flags & SS_DIRECT_TARGET) ? it.out_direct : nullptr})
+                    if (o && (uintptr_t)o < hi && lo < (uintptr_t)o + n_out) return SS_ERR_INVALID;
+            }
         }
     }
     if (!written_ranges_disjoint(r)) return SS_ERR_INVALID;
@@ -3451,9 +3499,11 @@ static int validate_lufs(const ss_source* items, const ss_stream_lufs* lufs, int
     return SS_OK;
 }
 
-// A plan's layout draws (include/sonicsim_b200.h, ss_layout_draw), all but the byte ranges (validate_mixes): the record
-// of each drawn slot receives its draw.  After validate_streams and validate_bgs, which name the stream and bed slots.
-static int validate_layouts(const ss_layout_draw* layouts, int n_layouts, std::vector<PlanSlot>& slots) {
+// A plan's layout draws (include/sonicsim_b200.h, ss_layout_draw) and their speaker groups (ss_layout_group), all but
+// the byte ranges (validate_mixes): the record of each drawn slot receives its draw and its groups.  After
+// validate_streams and validate_bgs, which name the stream and bed slots.
+static int validate_layouts(const ss_layout_draw* layouts, int n_layouts, const ss_layout_group* groups, int n_grouped,
+                            std::vector<PlanSlot>& slots) {
     for (int k = 0; k < n_layouts; ++k) {
         const ss_layout_draw& L = layouts[k];
         if (L.slot < 0 || L.slot >= (int)slots.size()) return SS_ERR_INVALID;
@@ -3465,9 +3515,21 @@ static int validate_layouts(const ss_layout_draw* layouts, int n_layouts, std::v
             for (int i = 0; i < r.bg->pool->n; ++i) if (L.select_lengths[i] < 0) return SS_ERR_INVALID;
         slots[L.slot].layout = &L;
     }
+    // a grouped draw: a stream slot's draw, named once, over bounds that ascend strictly from 0 to its pool's n, with
+    // an aligned group_dev
+    for (int j = 0; j < n_grouped; ++j) {
+        const ss_layout_group& q = groups[j];
+        if (q.layout < 0 || q.layout >= n_layouts) return SS_ERR_INVALID;
+        const PlanSlot& r = slots[layouts[q.layout].slot];
+        if (r.group || !r.strm || q.n_groups < 1 || !q.bounds || !q.group_dev || ((uintptr_t)q.group_dev & 3))
+            return SS_ERR_INVALID;
+        if (q.bounds[0] != 0 || q.bounds[q.n_groups] != r.strm->pool->n) return SS_ERR_INVALID;
+        for (int g = 0; g < q.n_groups; ++g) if (q.bounds[g + 1] <= q.bounds[g]) return SS_ERR_INVALID;
+        slots[layouts[q.layout].slot].group = &q;
+    }
     for (int k = 0; k < n_layouts; ++k) {
         const PlanSlot& r = slots[layouts[k].slot];
-        if (layout_bound(layouts[k], r.clips(), r.bg != nullptr) > kLayoutCap) return SS_ERR_UNSUPPORTED;
+        if (layout_bound(layouts[k], r.clips(), r.bg != nullptr, r.group) > kLayoutCap) return SS_ERR_UNSUPPORTED;
     }
     return SS_OK;
 }
@@ -3548,11 +3610,12 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
                        const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
-                       const ss_value_draw* values, int n_values, ss_plan** out) {
+                       const ss_value_draw* values, int n_values, const ss_layout_group* groups, int n_grouped,
+                       ss_plan** out) {
     auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
     if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
         bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs) || bad(lufs, n_lufs) ||
-        bad(layouts, n_layouts) || bad(values, n_values))
+        bad(layouts, n_layouts) || bad(values, n_values) || bad(groups, n_grouped))
         return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
@@ -3563,7 +3626,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     { int st = validate_streams(c, items, streams, n_streams, slots); if (st) return st; }
     { int st = validate_bgs(c, items, bgs, n_bgs, draws, n_draws, slots); if (st) return st; }
     { int st = validate_lufs(items, lufs, n_lufs, slots); if (st) return st; }
-    { int st = validate_layouts(layouts, n_layouts, slots); if (st) return st; }
+    { int st = validate_layouts(layouts, n_layouts, groups, n_grouped, slots); if (st) return st; }
     { int st = validate_values(values, n_values); if (st) return st; }
     { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
     { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
@@ -3581,7 +3644,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
         if (pl && std::find(p->pools.begin(), p->pools.end(), pl) == p->pools.end()) p->pools.push_back(pl);
     }
     const int st = plan_build(p, items, shapes.data(), slots, mix, draws, n_draws, layouts, n_layouts, values,
-                              n_values);
+                              n_values, groups, n_grouped);
     if (st != SS_OK) { ss_plan_destroy(p); return st; }
     for (ss_pool* pl : p->pools) pl->planned = true;   // its descriptors hold the pool's gain pointer (ss_pool_loudness)
     *out = p;
@@ -3590,26 +3653,26 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
     return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3617,7 +3680,7 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3625,7 +3688,7 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
@@ -3634,7 +3697,7 @@ extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items,
                                  int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                  int n_bgs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3643,7 +3706,7 @@ extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_item
                                    int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                    int n_bgs, const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3653,7 +3716,7 @@ extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_it
                                      int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
                                      int n_layouts, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_values(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3663,14 +3726,27 @@ extern "C" int ss_plan_create_values(ss_ctx* c, const ss_source* items, int n_it
                                      int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
                                      int n_layouts, const ss_value_draw* values, int n_values, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, nullptr, 0,
+                       out);
+}
+
+extern "C" int ss_plan_create_groups(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                     int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                     const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                     int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
+                                     int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
+                                     int n_layouts, const ss_value_draw* values, int n_values,
+                                     const ss_layout_group* groups, int n_grouped, ss_plan** out) {
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, groups,
+                       n_grouped, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start
@@ -3696,7 +3772,10 @@ static int plan_enqueue(ss_plan* p, cudaStream_t stream) {
         c->launches += 1;
     }
     if (p->n_layout) {
-        k_layout<<<p->n_layout, 32, p->layout_smem, stream>>>(p->d_layout);
+        if (p->d_layout_group)
+            k_layout_grouped<<<p->n_layout, 32, p->layout_smem, stream>>>(p->d_layout, p->d_layout_group);
+        else
+            k_layout<<<p->n_layout, 32, p->layout_smem, stream>>>(p->d_layout);
         CK(cudaGetLastError());
         c->launches += 1;
     }

@@ -841,6 +841,43 @@ SS_HD void layout_row(const LayoutDesc& d, int* keys, int* vals, int* sel) {
     }
 }
 
+// ---- grouped layout draws (ss_layout_group, include/sonicsim_b200.h): a stream slot's draw over one of G >= 1
+// contiguous groups of its pool's utterances, 0 = b[0] < b[1] < ... < b[G] = n (e.g. one LibriSpeech speaker's
+// utterances each, as SonicSet builds every stream from one speaker), the group g read from device memory at every run.
+//   - g outside [0, G) is clamped into range and the run reports bit 7 (ss_device_errors);
+//   - the row is then exactly the ungrouped draw r over a pool holding only utterances [b[g], b[g + 1]), in order: the
+//     same Philox blocks (b, r, t_lo, t_hi), the same words in the same order; every id it writes is offset by b[g];
+//   - reading g consumes no words.
+// So G = 1 is the ungrouped draw, and group g over the whole pool is the ungrouped draw over that group's sub-pool with
+// its ids shifted.  K of a grouped draw is the largest K of its groups (a larger K than a group's own changes none of
+// its words: the bound is never reached).
+struct LayoutGroup {
+    const int* group;                                  // device, one int32 read at every run; null: an ungrouped draw
+    const int* bounds;                                 // the plan's copy of the G + 1 bounds
+    int G, pad;
+};
+static_assert(sizeof(LayoutGroup) == 24, "LayoutGroup layout");
+// The row of layout draw d under its group entry q (q.group null: layout_row's row itself); returns the error bits
+SS_HD unsigned layout_row_grouped(LayoutDesc d, const LayoutGroup& q, int* keys, int* vals, int* sel) {
+    unsigned err = 0;
+    int lo = 0;
+    if (q.group) {                                     // narrow the pool to the group's utterances
+        int g = *q.group;
+        if (g < 0 || g >= q.G) {
+            g = g < 0 ? 0 : q.G - 1;
+            err = 128u;
+        }
+        lo = q.bounds[g];
+        d.lengths += lo;
+        d.n = q.bounds[g + 1] - lo;
+    }
+    layout_row(d, keys, vals, sel);
+    if (lo)
+        for (int k = 0; k < d.m; ++k)
+            if (d.ids[k] != -1) d.ids[k] += lo;
+    return err;
+}
+
 // ---- value draws (ss_value_draw, include/sonicsim_b200.h): a plan writes the per-run values its slots, draws,
 // mixtures and loudness slots read (picks, starts, SIRs, SNRs, crop variates, loudness targets) itself at the head of
 // every run (k_values), from the generator of the layout draws.  The random stream is a format, followed word for word

@@ -27,11 +27,16 @@ def _load_resampled(path, sample_rate, loader):
     return waveform
 
 
+def _wav_candidates(audio_dir: str) -> T.List[str]:
+    """The files get_random_wav_path draws from: every file of the tree but the .txt ones, in os.walk order."""
+    return [os.path.join(root, name) for root, _, names in os.walk(str(audio_dir)) for name in names
+            if not name.endswith(".txt")]
+
+
 def get_random_wav_path(audio_dir: str, length: int, threshold: float = 0.9, loader=None) -> T.List[str]:
     """:152-190 - random files of a directory tree whose total length lands in [threshold*length, length]."""
     loader = loader or _default_loader
-    candidates = [os.path.join(root, name) for root, _, names in os.walk(str(audio_dir)) for name in names
-                  if not name.endswith(".txt")]
+    candidates = _wav_candidates(audio_dir)
     print(f"audio_path_list: {len(candidates)}")
     n_samples = {p: loader(p)[0].shape[-1] for p in candidates}
     chosen, total = [], 0
@@ -116,13 +121,48 @@ def _place_background_audio(lens: T.List[int], total: int, length: float, sample
     return places, spans, used
 
 
-def long_audio_max_selected(lengths, total: int) -> int:
-    """The most utterances of `lengths` that get_random_wav_path's selection can take for a stream of `total` samples:
-    the largest k whose k shortest utterances fit in `total` (at least 1).  A host computation, once per corpus, for
-    long_audio_layouts(..., max_selected=)."""
+def speaker_groups(speaker_dirs) -> T.Tuple[T.List[str], T.List[int]]:
+    """An utterance corpus in speaker order, for grouped stream layouts (long_audio_layouts(groups=), render.LayoutDraw
+    (groups=)): (paths, bounds).  For each directory of `speaker_dirs` (e.g. the lines of SonicSet's
+    {mode}_speech.txt, one LibriSpeech speaker each), the files get_random_wav_path would draw from, in its order
+    (os.walk, .txt files left out); paths concatenates them and bounds (G + 1 ints, 0 = bounds[0] < ... < bounds[G] =
+    len(paths)) delimits speaker g's files as paths[bounds[g]:bounds[g + 1]].  A pool built from paths in this order
+    (one signal per path) has these bounds as its groups.  A directory without such files raises ValueError."""
+    paths, bounds = [], [0]
+    for d in speaker_dirs:
+        files = _wav_candidates(d)
+        if not files:
+            raise ValueError("speaker_groups: %s holds no file get_random_wav_path would draw" % (d,))
+        paths += files
+        bounds.append(len(paths))
+    if len(bounds) < 2:
+        raise ValueError("speaker_groups: need at least one speaker directory")
+    return paths, bounds
+
+
+def _group_bounds(groups, n: int, api: str):
+    """`groups` (G + 1 bounds: a host sequence, array or tensor) as an int64 NumPy array, checked to ascend strictly
+    from 0 to n."""
     import numpy as np
-    v = np.sort(np.asarray(lengths.cpu() if hasattr(lengths, "cpu") else lengths, dtype=np.int64).reshape(-1))
-    return max(1, int(np.searchsorted(np.cumsum(v), int(total), side="right")))
+    b = np.asarray(groups.cpu() if hasattr(groups, "cpu") else groups)
+    if b.ndim != 1 or b.size < 2 or not (np.issubdtype(b.dtype, np.integer) or b.dtype == object):
+        raise ValueError("%s: groups must be G + 1 >= 2 integer bounds, got %r" % (api, groups))
+    b = b.astype(np.int64)
+    if b[0] != 0 or b[-1] != n or (np.diff(b) < 1).any():
+        raise ValueError("%s: groups must ascend strictly from 0 to the %d utterances of the pool" % (api, n))
+    return b
+
+
+def long_audio_max_selected(lengths, total: int, groups=None) -> int:
+    """The most utterances of `lengths` that get_random_wav_path's selection can take for a stream of `total` samples:
+    the largest k whose k shortest utterances fit in `total` (at least 1).  With `groups` (G + 1 bounds, see
+    speaker_groups), the largest such k over the groups, each of which a row selects from alone.  A host computation,
+    once per corpus, for long_audio_layouts(..., max_selected=)."""
+    import numpy as np
+    v = np.asarray(lengths.cpu() if hasattr(lengths, "cpu") else lengths, dtype=np.int64).reshape(-1)
+    b = [0, v.size] if groups is None else _group_bounds(groups, v.size, "long_audio_max_selected")
+    return max(max(1, int(np.searchsorted(np.cumsum(np.sort(v[lo:hi])), int(total), side="right")))
+               for lo, hi in zip(b[:-1], b[1:]))
 
 
 def background_audio_max_selected(select_lengths, total: int) -> int:
@@ -136,12 +176,16 @@ def background_audio_max_selected(select_lengths, total: int) -> int:
     return min(v.size, below + 1)
 
 
-def _long_audio_selection(lengths, total: int, count: int, width: int, kw):
+def _long_audio_selection(lengths, total: int, count: int, width: int, kw, lo=None, hi=None):
     """get_random_wav_path's selection, `count` times: (sel, chosen), both (count, width).  sel[r] is the first width
     utterances of a uniform random order, chosen[r] marks its selected prefix (taken while the running total is below
-    0.9 * total, up to the first that would overflow `total`)."""
+    0.9 * total, up to the first that would overflow `total`).  With lo and hi ((count,) tensors), row r selects from
+    utterances [lo[r], hi[r]) only: the others sort behind them and are never chosen."""
     import torch
     keys = torch.rand((count, lengths.numel()), **kw)
+    if lo is not None:
+        idx = torch.arange(lengths.numel(), device=keys.device)
+        keys.masked_fill_((idx < lo[:, None]) | (idx >= hi[:, None]), 2.0)
     if width < lengths.numel():                       # the first `width` of the random order
         sel = torch.topk(keys, width, dim=1, largest=False, sorted=True).indices
     else:
@@ -150,11 +194,13 @@ def _long_audio_selection(lengths, total: int, count: int, width: int, kw):
     ls = lengths[sel]
     cs = torch.cumsum(ls, dim=1)
     take = ((cs - ls).double() < 0.9 * total) & (cs <= total)
+    if lo is not None:
+        take &= (sel >= lo[:, None]) & (sel < hi[:, None])
     return sel, torch.cumprod(take.to(torch.int8), dim=1).bool()
 
 
 def long_audio_layouts(lengths, total: int, m: int, count: int, generator=None, sample_rate: int = 16000,
-                       max_selected: T.Optional[int] = None):
+                       max_selected: T.Optional[int] = None, groups=None, group=None):
     """`count` layouts of create_long_audio streams (:231-277) over utterances of `lengths` (a 1-D integer tensor of n
     lengths in samples, already at `sample_rate`), for render.DryStream: (ids, offsets), two int32 tensors of shape
     (count, m) on `lengths`' device.  Torch ops only, so a training step refreshes them on the GPU without a host
@@ -177,16 +223,36 @@ def long_audio_layouts(lengths, total: int, m: int, count: int, generator=None, 
     (long_audio_max_selected(lengths, total), computed once per corpus) bounds how many utterances a row can select;
     the call then keeps only the max_selected smallest keys of each row (torch.topk) and works on (count,
     max_selected) and (count, m) tensors behind the (count, n) keys, with the same distribution: 145 MB (the keys)
-    and 1.1 ms there.  A bound below long_audio_max_selected's cuts rows short and changes the distribution."""
+    and 1.1 ms there.  A bound below long_audio_max_selected's cuts rows short and changes the distribution.
+
+    Speaker groups, as SonicSet builds every stream from one speaker's utterances: `groups` (G + 1 host bounds, 0 =
+    groups[0] < ... < groups[G] = n, see speaker_groups) splits the utterances into G contiguous groups, and `group`
+    (a (count,) integer tensor on `lengths`' device, e.g. a ValueDraw of distinct speakers) names row i's group.  Row
+    i then follows the rule above over the utterances [groups[g], groups[g + 1]) of g = group[i] alone, its ids
+    numbered in the whole pool; a group outside [0, G) is clamped into range, as a plan's grouped LayoutDraw clamps
+    it.  This matches the plan's grouped draws in distribution.  `max_selected` stays a bound over every group
+    (long_audio_max_selected(lengths, total, groups)).  Without groups every row selects from all n utterances, which
+    over a multi-speaker corpus strings together utterances of about as many speakers as the stream holds."""
     import torch
     lengths = lengths.reshape(-1).to(torch.int64)
     n, dev = lengths.numel(), lengths.device
     if n < 1 or not 1 <= m <= 128 or count < 1 or (max_selected is not None and max_selected < 1):
         raise ValueError("long_audio_layouts: need n >= 1 utterances, 1 <= m <= 128, count >= 1 and max_selected "
                          ">= 1, got n = %d, m = %d, count = %d, max_selected = %r" % (n, m, count, max_selected))
+    lo = hi = None
+    if (groups is None) != (group is None):
+        raise ValueError("long_audio_layouts: give both groups and group, or neither")
+    if groups is not None:
+        b = _group_bounds(groups, n, "long_audio_layouts")
+        if not isinstance(group, torch.Tensor) or group.numel() != count or group.device != dev or \
+                group.dtype.is_floating_point or group.dtype.is_complex or group.dtype == torch.bool:
+            raise ValueError("long_audio_layouts: group must be a (count,) integer tensor on the device of lengths")
+        bt = torch.from_numpy(b).to(dev)
+        g = group.reshape(-1).to(torch.int64).clamp(0, b.size - 2)
+        lo, hi = bt[g], bt[g + 1]
     kw = {"generator": generator, "device": dev}
     width = n if max_selected is None else min(n, int(max_selected))
-    sel, chosen = _long_audio_selection(lengths, total, count, width, kw)
+    sel, chosen = _long_audio_selection(lengths, total, count, width, kw, lo, hi)
     # placement: the first m of the chosen ones in a fresh random order, each behind a gap, while the cursor stays
     # within `total` (a row keeps at most m, and what it keeps is a prefix of that order)
     w = min(width, m)

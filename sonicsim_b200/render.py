@@ -188,7 +188,15 @@ class StemLoudness(T.NamedTuple):
     sr: float = 16000.0
 
 
-class LayoutDraw(T.NamedTuple):
+class _LayoutDrawFields(T.NamedTuple):
+    slot: int
+    rng: T.Any
+    total: int
+    sample_rate: int = 16000
+    select_lengths: T.Any = None
+
+
+class LayoutDraw(_LayoutDrawFields):
     """A stream or bed slot whose layout the plan draws itself at every run (Renderer.plan_device(layouts=...)), by the
     rule of dry.long_audio_layouts (a DryStream slot) or dry.background_audio_layouts (a BackgroundStream slot), in one
     kernel launch at the head of the run.  `slot`: index into the plan's sources.  `rng`: a two-element CUDA int64 tensor
@@ -201,12 +209,33 @@ class LayoutDraw(T.NamedTuple):
     dry.background_audio_layouts); None selects by the clip lengths.  The draw writes the slot's own ids, offsets (and
     heads, counts) tensors, which then hold that run's layout.  The layouts match the rules in distribution, not torch's
     bits.  A row may select at most 1024 utterances or clips (dry.long_audio_max_selected,
-    dry.background_audio_max_selected)."""
-    slot: int
-    rng: T.Any
-    total: int
-    sample_rate: int = 16000
-    select_lengths: T.Any = None
+    dry.background_audio_max_selected).
+
+    Speaker groups (stream slots only), as SonicSet builds every stream from one LibriSpeech speaker: `groups`, G + 1
+    host bounds 0 = groups[0] < ... < groups[G] = the pool's n (a sequence, array or tensor; dry.speaker_groups builds
+    them), splits the utterance pool into G contiguous groups, and `group`, a one-element CUDA int32 tensor read at
+    every run (e.g. spk[b, k] of a (B, S) tensor a ValueDraw(spk, rng, 0, G, distinct=True) writes), names the group
+    this run lays the stream out from.  The row is then exactly the ungrouped draw over a pool of that group's
+    utterances alone, with the same words, its ids shifted by groups[g] into the whole pool; a group outside [0, G) is
+    clamped into range (check_device_errors raises IndexError).  Give both or neither; 1024 bounds every group's
+    selection (dry.long_audio_max_selected(lengths, total, groups)).  `groups` and `group` are attributes outside the
+    tuple: a LayoutDraw stays the (slot, rng, total, sample_rate, select_lengths) tuple callers unpack and rebuild
+    (_replace and repr carry them; tuple equality does not look at them)."""
+
+    def __new__(cls, slot, rng, total, sample_rate=16000, select_lengths=None, groups=None, group=None):
+        self = super().__new__(cls, slot, rng, total, sample_rate, select_lengths)
+        self.groups, self.group = groups, group
+        return self
+
+    def _replace(self, **kw):
+        groups, group = kw.pop("groups", self.groups), kw.pop("group", self.group)
+        return LayoutDraw(*super()._replace(**kw), groups=groups, group=group)
+
+    def __repr__(self):
+        return "%s, groups=%r, group=%r)" % (super().__repr__()[:-1], self.groups, self.group)
+
+    def __getnewargs__(self):
+        return tuple(self) + (self.groups, self.group)
 
 
 class ValueDraw(T.NamedTuple):
@@ -1159,7 +1188,16 @@ class Renderer:
 
         Plain starts (`ValueDraw(starts, rng, 0, N - length + 1)`), dry picks and loudness targets (float64, e.g.
         U(-19, -15) for speech, U(-26, -22) for noise and U(-31, -27) for music, one tensor per range) are drawn the same
-        way."""
+        way.
+
+        With stream slots over a 16-bit pool in speaker order (paths, bounds = dry.speaker_groups(speaker_dirs), G =
+        len(bounds) - 1), the step also draws each example's S distinct speakers (SonicSet.py:198) and lays every stream
+        out from its speaker's utterances alone (create_long_audio over one speaker directory), in the same launches
+        (ss_plan_create_groups):
+
+            values = [ValueDraw(spk, rng, 0, G, distinct=True), ...]    # np.random.choice(speech_list, S, False)
+            layouts = [LayoutDraw(slot_of[b][k], rng, 60 * 16000, groups=bounds, group=spk[b, k:k + 1])
+                       for b in range(B) for k in range(S)]"""
         dry = self._device_dry(sources)
         streams = self._device_streams(sources)
         bgs = self._device_bgs(sources)
@@ -1168,12 +1206,15 @@ class Renderer:
         mixes = self._device_mixes(mixtures, outs, keep, items, targets) if mixtures else None
         drw = self._device_draws(draws, sources, keep) if draws else None
         lufs = self._device_lufs(sources, (outs, direct_outs, mixtures, draws), keep)
-        lay = self._device_layouts(layouts, sources, (outs, direct_outs, mixtures, draws), keep) if layouts else None
+        grouped = []
+        lay = self._device_layouts(layouts, sources, (outs, direct_outs, mixtures, draws), keep, grouped) \
+            if layouts else None
+        grp = (_lib.SsLayoutGroup * len(grouped))(*grouped) if grouped else None
         val = self._device_values(values, sources, (outs, direct_outs, mixtures, draws, layouts), keep) \
             if values else None
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
                           (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs, lay,
-                          val)
+                          val, grp)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1333,13 +1374,14 @@ class Renderer:
             seen.append((lo, hi))
         return (_lib.SsStreamLufs * len(entries))(*entries)
 
-    def _device_layouts(self, layouts, sources, others, keep):
-        """Validated ss_layout_draw array of a plan's layout draws; their select_lengths arrays are appended to `keep`.
-        `others`: the plan's other arguments, whose tensors the drawn layouts may not meet."""
+    def _device_layouts(self, layouts, sources, others, keep, grouped=None):
+        """Validated ss_layout_draw array of a plan's layout draws; their select_lengths and group bounds arrays are
+        appended to `keep`, and the ss_layout_group entry of each grouped draw to `grouped` (a list; None: the plan may
+        have no grouped draw).  `others`: the plan's other arguments, whose tensors the drawn layouts may not meet."""
         import torch
         from . import dry as _dry
         arr = (_lib.SsLayoutDraw * len(layouts))()
-        drawn, rngs = [], []
+        drawn, rngs, gtens = [], [], []                 # gtens: the group tensors of grouped draws
         for k, d in enumerate(layouts):
             if not isinstance(d, LayoutDraw):
                 raise ValueError("plan_device: layout %d must be a LayoutDraw" % k)
@@ -1352,6 +1394,23 @@ class Renderer:
             if any(int(e.slot) == i for e in layouts[:k]):
                 raise ValueError("plan_device: layout %d names source %d, which another layout draw names" % (k, i))
             own = "layout %d" % k
+            bed = isinstance(w, BackgroundStream)
+            bounds = None
+            if d.groups is not None or d.group is not None:     # speaker groups: a stream slot's, both given
+                if bed:
+                    raise ValueError("plan_device: layout %d has speaker groups, but source %d is a bed slot: beds draw "
+                                     "from the whole clip pool" % (k, i))
+                if d.groups is None or d.group is None:
+                    raise ValueError("plan_device: layout %d needs both groups and group, or neither" % k)
+                bounds = np.ascontiguousarray(_dry._group_bounds(d.groups, w.pool.n, "plan_device: " + own),
+                                              dtype=np.int32)
+                gp = _tensor(d.group, "plan_device", own, "group", torch.int32, self.device, count=(1, 1))
+                if grouped is None:
+                    raise ValueError("plan_device: layout %d has speaker groups, which this call does not take" % k)
+                keep.append(bounds)
+                grouped.append(_lib.SsLayoutGroup(layout=k, n_groups=bounds.size - 1, bounds=bounds.ctypes.data,
+                                                  group_dev=gp))
+                gtens.append(d.group)
             rng = _tensor(d.rng, "plan_device", own, "rng", torch.int64, self.device, count=(2, 2))
             if rng % 8:
                 raise ValueError("plan_device: the rng of layout %d must be 8-byte aligned" % k)
@@ -1359,7 +1418,6 @@ class Renderer:
             if not 1 <= total < 1 << 31 or not 1 <= sr <= 214748364:
                 raise ValueError("plan_device: layout %d needs 1 <= total < 2^31 and 1 <= sample_rate <= 214748364 "
                                  "(10 s of samples in int32), got %d and %d" % (k, total, sr))
-            bed = isinstance(w, BackgroundStream)
             sel = None
             if d.select_lengths is not None:
                 if not bed:
@@ -1373,10 +1431,10 @@ class Renderer:
                 sel = np.ascontiguousarray(sel, dtype=np.int32)
                 keep.append(sel)
             K = (_dry.background_audio_max_selected(sel if sel is not None else w.pool.sizes, total) if bed
-                 else _dry.long_audio_max_selected(w.pool.sizes, total))
+                 else _dry.long_audio_max_selected(w.pool.sizes, total, bounds))
             if K > 1024:
-                raise ValueError("plan_device: layout %d could select %d %s, at most 1024" %
-                                 (k, K, "clips" if bed else "utterances"))
+                raise ValueError("plan_device: layout %d could select %d %s, at most 1024%s" %
+                                 (k, K, "clips" if bed else "utterances", " in one group" if bounds is not None else ""))
             arrays = (w.ids, w.offsets) + ((w.heads, w.counts) if bed else ())
             drawn += [a for a in arrays if _is_tensor(a)]
             rngs.append(d.rng)
@@ -1400,6 +1458,10 @@ class Renderer:
             lo, hi = span(t)
             if any(a < hi and lo < b for a, b in map(span, written)):
                 raise ValueError("plan_device: a layout draw's rng meets a tensor the plan writes")
+        for t in gtens:                                # (a ValueDraw may write a group: _device_values checks that)
+            lo, hi = span(t)
+            if any(a < hi and lo < b for a, b in map(span, written)):
+                raise ValueError("plan_device: a layout draw's group meets a tensor the plan writes")
         keep.append(list(layouts))
         return arr
 
@@ -1490,7 +1552,9 @@ class Renderer:
             if isinstance(s.dry, DryStream) and s.dry.lufs is not None:
                 stems.append(s.dry.lufs)
         inputs += [t for m in mixtures or () for t in (m.sirs, m.snr)] + [d.u for d in draws or ()]
-        every = _cuda_tensors((sources, others, stems))
+        groups = [d.group for d in layouts or () if d.group is not None]      # (outside their LayoutDraw's tuple)
+        inputs += groups                               # a grouped layout draw's group
+        every = _cuda_tensors((sources, others, stems, groups))
         uses = collections.Counter(id(t) for t in every)
         uses.subtract(id(t) for t in inputs if _is_tensor(t))
         span = lambda t: (t.data_ptr(), t.data_ptr() + t.numel() * t.element_size())   # noqa: E731
@@ -1701,7 +1765,8 @@ class Renderer:
         """Waits for the device and raises what the reference would have raised for a trajectory the device path met
         but could not refuse up front: IndexError for an interp_index outside [0, P - 2] (NumPy's fancy index at
         SonicSim_moving.py:89-90), ValueError for a device-side bounds table that is not ascending from 0 to N or for a
-        window start tensor that held a value outside [0, N - length] (the window was rendered clamped into range)."""
+        window start tensor that held a value outside [0, N - length] (the window was rendered clamped into range);
+        IndexError too for a pick, dry pick or grouped LayoutDraw's group outside its range (clamped into it)."""
         bits = ctypes.c_uint32()
         _lib.check(self.lib.ss_device_errors(self.ctx, ctypes.byref(bits)))
         if bits.value & 1:
@@ -1712,6 +1777,9 @@ class Renderer:
         if bits.value & 16:
             raise IndexError("a dry pick on the device was out of range for the signals of its DryPool; it was clamped "
                              "into [0, n)")
+        if bits.value & 128:
+            raise IndexError("a grouped LayoutDraw's group on the device was out of range for its G groups; it was "
+                             "clamped into [0, G)")
         if bits.value & 2:
             raise ValueError("a device-side trajectory bounds table is not ascending from 0 to N")
         if bits.value & 4:
@@ -1750,25 +1818,23 @@ class DevicePlan:
     dry-picked slots take their dry signals from dry pools, with pair gains their gains from pair-gain tables; with
     dereverberation targets its mixtures also write those, with stream slots it lays out their dry streams and with bed
     slots their noise and music beds, with loudness slots it measures their whole stems at every run, with layout draws
-    it draws its stream and bed layouts at every run, with value draws it draws its per-run inputs at every run.  A plan
-    with value draws is created by ss_plan_create_values, every other plan by ss_plan_create_layout, with NULL and a
-    count of 0 for each part it does not have."""
+    it draws its stream and bed layouts at every run, with value draws it draws its per-run inputs at every run, with
+    grouped layout draws it lays each such stream out from the group of utterances its group tensor names.  Every plan
+    is created by ss_plan_create_groups, with NULL and a count of 0 for each part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
-                 streams=None, bgs=None, lufs=None, layouts=None, values=None):
+                 streams=None, bgs=None, lufs=None, layouts=None, values=None, groups=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
-        self.bgs, self.lufs, self.layouts, self.values = bgs, lufs, layouts, values
+        self.bgs, self.lufs, self.layouts, self.values, self.groups = bgs, lufs, layouts, values, groups
         self._plan = ctypes.c_void_p()
         if n > 0:
             args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
                     pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
                     len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, lufs, len(lufs) if lufs else 0,
-                    layouts, len(layouts) if layouts else 0)
-            if values:
-                _lib.check(renderer.lib.ss_plan_create_values(*args, values, len(values), ctypes.byref(self._plan)))
-            else:
-                _lib.check(renderer.lib.ss_plan_create_layout(*args, ctypes.byref(self._plan)))
+                    layouts, len(layouts) if layouts else 0, values, len(values) if values else 0, groups,
+                    len(groups) if groups else 0)
+            _lib.check(renderer.lib.ss_plan_create_groups(*args, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
