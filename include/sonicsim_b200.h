@@ -337,7 +337,8 @@ int ss_render_dev(ss_ctx* ctx, const ss_source* items, int n_items, void* stream
  * pools, below) = a dry pick outside [0, n) of its dry pool (clamped), bit 5 (dry streams and background streams,
  * below) = an invalid entry of a stream or bed slot's layout (skipped), bit 6 (loudness slots, ss_stream_lufs below) =
  * a loudness target read at a run that was not finite (that slot stored unscaled), bit 7 (speaker groups,
- * ss_layout_group below) = a grouped layout draw's group outside [0, G) (clamped).  The Python device API raises
+ * ss_layout_group below) = a grouped layout draw's group outside [0, G) (clamped), bit 8 (trajectories, ss_trajectory
+ * below) = an invalid path or bounds table of a pooled slot (its candidate's own path rendered).  The Python device API raises
  * IndexError / ValueError from it on request
  * (Renderer.check_device_errors).  The bits live in one device word per GPU, shared by every context of the
  * process on that GPU: with several such contexts, a call on one returns and clears the bits another one's kernels set. */
@@ -998,6 +999,48 @@ int ss_plan_create_groups(ss_ctx* ctx, const ss_source* items, int n_items, cons
                           const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
                           const ss_value_draw* values, int n_values, const ss_layout_group* groups, int n_grouped,
                           ss_plan** out);
+
+/* ---- trajectories of pooled slots: SonicSet times every stem's path anew (setup_dynamic_interp, SonicSim_moving.py
+ * :15-45), and the same RIRs serve the path walked backwards or a contiguous stretch of it.  A trajectory entry makes a
+ * pooled slot of a moving device pool render, at every run, the path its two device arrays hold over its picked
+ * candidate of P positions and N samples:
+ *   - path_dev: 3 int32 (a, b, dir), 0 <= a < b <= P - 1; dir 0 visits positions a, a + 1, ..., b (forward), dir 1
+ *     visits b, b - 1, ..., a (reverse);
+ *   - bounds_dev: p_max int32 (p_max: the pool's largest P), of which the first b - a + 1 are the visited path's
+ *     cumulative segment bounds in SS_MOVING_BOUNDS form (0 first, N last, non-decreasing).
+ * The slot renders visited position j with bank position a + j (forward) or b - j (reverse) and these bounds; its dry
+ * signal, window, direct stem, dry pick, stream or bed stay as they are.  (0, P - 1, 0) with the candidate's own bounds
+ * renders bit for bit what the slot renders without the entry, and a forward (a, b) with bounds B what the candidate
+ * renders with bounds that are B over [a, b] and empty elsewhere.  An invalid path or bounds table renders the
+ * candidate's own forward path and bounds, and ss_device_errors reports bit 8.  A loudness slot (ss_stream_lufs)
+ * measures its whole stem with the run's trajectory.  The slot's block table, work items and dry spectra are sized for
+ * any bounds table of at most P - 1 segments of any candidate (ss_phases.cuh, traj_table_cap).
+ * ss_plan_create_traj is ss_plan_create_groups with n_trajs entries (n_trajs == 0: exactly ss_plan_create_groups; a
+ * plan with trajectories launches as many kernels per run as without).  Refused at creation, before anything is
+ * allocated and with *out untouched:
+ *   - SS_ERR_INVALID:
+ *     - n_trajs < 0, or NULL trajs with n_trajs > 0;
+ *     - a slot outside [0, n_items), one that two entries name, or one that is not a pooled slot of a moving pool;
+ *     - a pool with loudness gains (ss_pool_loudness) or a dry pick with pair gains: both were measured with the
+ *       candidates' own timing;
+ *     - a start draw's speaker that renders its candidate's own dry signal (its level table is that stem's);
+ *     - a NULL or misaligned (4 bytes) path_dev or bounds_dev, or one that meets any other range the plan reads or
+ *       writes.
+ *   - SS_ERR_UNSUPPORTED: a slot of a host pool (SS_BANK_HOST), whose staging is sized from the host bounds.
+ * Capability marker: the export ss_plan_create_traj.  A library that exports it takes trajectories; ss_version stays
+ * 108, which callers of the earlier exports compare against, so it does not mark this capability. */
+typedef struct {
+    int32_t slot;                     /* index into `items`: a pooled slot of a moving device pool                   */
+    const int32_t* path_dev;          /* device, (a, b, dir), read at every run                                       */
+    const int32_t* bounds_dev;        /* device, p_max int32, the first b - a + 1 read at every run                   */
+} ss_trajectory;
+int ss_plan_create_traj(ss_ctx* ctx, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
+                        const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                        const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
+                        const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
+                        const ss_value_draw* values, int n_values, const ss_layout_group* groups, int n_grouped,
+                        const ss_trajectory* trajs, int n_trajs, ss_plan** out);
 
 /* ---- mixture assembly of the training dataloader: separation/look2hear/datas/movingdatamodule.py
  * :29-32 (compute_mch_rms_dB) and :105-124 (SIR gains of the interferers, SNR gain of the summed noise,

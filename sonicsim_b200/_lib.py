@@ -116,6 +116,11 @@ class SsLayoutGroup(ctypes.Structure):
                 ("group_dev", ctypes.c_void_p)]
 
 
+class SsTrajectory(ctypes.Structure):
+    """`ss_trajectory` of include/sonicsim_b200.h."""
+    _fields_ = [("slot", ctypes.c_int32), ("path_dev", ctypes.c_void_p), ("bounds_dev", ctypes.c_void_p)]
+
+
 class SsValueDraw(ctypes.Structure):
     """`ss_value_draw` of include/sonicsim_b200.h."""
     _fields_ = [("out", ctypes.c_void_p), ("rng_dev", ctypes.c_void_p), ("kind", ctypes.c_int32),
@@ -266,6 +271,8 @@ def load():
                                                                                         ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_plan_create_groups.argtypes = lib.ss_plan_create_values.argtypes[:-1] + [ctypes.POINTER(SsLayoutGroup),
                                                                                         ctypes.c_int, ctypes.POINTER(vp)]
+        lib.ss_plan_create_traj.argtypes = lib.ss_plan_create_groups.argtypes[:-1] + [ctypes.POINTER(SsTrajectory),
+                                                                                      ctypes.c_int, ctypes.POINTER(vp)]
         lib.ss_render_host.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int]
         lib.ss_render_host_ex.argtypes = [vp, ctypes.POINTER(SsSource), ctypes.c_int, ctypes.POINTER(SsPostLufs)]
         lib.ss_convolve_fixed_receiver.argtypes = [vp, vp, vp, vp, i32, i32, i32]
@@ -298,7 +305,7 @@ def load():
 
 
 EXPORTS = ["ss_version", "ss_strerror", "ss_last_cuda_error", "ss_create", "ss_destroy",
-           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_flags", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_host_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_dry_pool_create_i16", "ss_dry_pool_level_stride", "ss_dry_pool_signal_i16", "ss_plan_create_dry", "ss_pair_gains_create", "ss_pair_gains_bytes", "ss_pair_gains_destroy", "ss_plan_create_pair", "ss_plan_create_target", "ss_plan_create_stream", "ss_plan_create_bg", "ss_plan_create_lufs", "ss_plan_create_layout", "ss_plan_create_values", "ss_plan_create_groups", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
+           "ss_set_chunk_bytes", "ss_render_dev", "ss_device_errors", "ss_plan_create", "ss_plan_create_mix", "ss_plan_create_ex", "ss_plan_run", "ss_plan_is_graph", "ss_plan_destroy", "ss_bank_create_dev", "ss_bank_create_host", "ss_bank_bytes", "ss_bank_host_bytes", "ss_bank_flags", "ss_bank_destroy", "ss_pool_create", "ss_pool_bytes", "ss_pool_host_bytes", "ss_pool_destroy", "ss_pool_levels", "ss_pool_level_table", "ss_pool_loudness", "ss_dry_pool_create", "ss_dry_pool_bytes", "ss_dry_pool_host_bytes", "ss_dry_pool_level_table", "ss_dry_pool_destroy", "ss_dry_pool_create_i16", "ss_dry_pool_level_stride", "ss_dry_pool_signal_i16", "ss_plan_create_dry", "ss_pair_gains_create", "ss_pair_gains_bytes", "ss_pair_gains_destroy", "ss_plan_create_pair", "ss_plan_create_target", "ss_plan_create_stream", "ss_plan_create_bg", "ss_plan_create_lufs", "ss_plan_create_layout", "ss_plan_create_values", "ss_plan_create_groups", "ss_plan_create_traj", "ss_render_host", "ss_render_host_ex", "ss_convolve_fixed_receiver",
            "ss_convolve_moving_receiver", "ss_loudness_dev", "ss_lufs_norm_host", "ss_mix_scratch_doubles", "ss_mix_dev", "ss_mix_host",
            "ss_mix_host_ex", "ss_overlap_dev", "ss_overlap_host", "ss_dry_assemble_dev", "ss_debug_plan", "ss_debug_chunks", "ss_launch_count", "ss_reset_stats", "ss_set_profiling", "ss_get_profile", "ss_host_alloc",
            "ss_host_free"]

@@ -44,7 +44,7 @@ using namespace ss;
 // of ss_render_dev (idx outside [0, P - 2]; bounds not ascending from 0 to N) sets a bit here; ss_device_errors reads
 // and clears it.  bit 0: index out of range, bit 1: bounds not monotone / not ending at N, bit 2: a moving window's
 // start outside [0, N - win_len] (clamped), bit 3: a pooled slot's pick outside [0, n) (clamped), bit 4: a dry pick
-// outside [0, n) of its dry pool (clamped).
+// outside [0, n) of its dry pool (clamped), bit 8: an invalid trajectory of a pooled slot (its candidate's own path used).
 __device__ unsigned g_dev_err;
 
 // twiddle tables, filled from the host in double precision (ss_create)
@@ -118,9 +118,11 @@ __device__ void write_blocks(const Source& S, int lane, int g0, int g1) {
 // when the pool's candidates differ in K (pick_parts), and its loudness gain, counts[11] - into its Source in the
 // descriptor block (pick_slot), which is why k_prepare then reads the Source table from global memory (k_prepare<false>).
 // A dry-picked slot then reads its dry pick, clamps it (bit 4) and puts the picked dry signal in place of x (pick_dry);
-// with pair gains (ss_pair_gains) it takes the pair's gain in place of the candidate's.
+// with pair gains (ss_pair_gains) it takes the pair's gain in place of the candidate's.  A slot with a trajectory
+// (ss_trajectory) then takes the run's path and bounds over the picked candidate (take_trajectory, bit 8), and after the
+// scan its work items are filled here (fill_traj_items) instead of by k_prepare's range warps.
 __global__ void __launch_bounds__(256)
-k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
+k_blocks(Source* srcs, int n_src, int* __restrict__ total_items, RItem* __restrict__ items) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     for (int si = warp; si < n_src; si += nwarps) {
         Source& S = srcs[si];
@@ -132,6 +134,10 @@ k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
                     take_view(S, *sv);                  // a host pool: k_stage picked (bit 3) and staged the candidate
                 } else {
                     const unsigned err = pick_pooled(S);   // the pick (bit 3), and a dry pick (bit 4)
+                    if (err) atomicOr(&g_dev_err, err);
+                }
+                if (has_traj(S)) {                      // the run's trajectory over the picked candidate (bit 8)
+                    const unsigned err = take_trajectory(S);
                     if (err) atomicOr(&g_dev_err, err);
                 }
             }
@@ -166,6 +172,14 @@ k_blocks(Source* srcs, int n_src, int* __restrict__ total_items) {
             carry += __shfl_sync(0xffffffffu, incl, 31);
         }
         if (lane == 0) *total_items = carry;
+    }
+    __syncthreads();
+    for (int si = warp; si < n_src; si += nwarps) {            // slots with a trajectory: their items, here
+        Source& S = srcs[si];
+        if (!has_traj(S)) continue;
+        fill_traj_items(S, items, lane, 32);
+        __syncwarp();
+        if (lane == 0) S.counts[0] = 0;
     }
 }
 
@@ -828,6 +842,7 @@ struct ss_pool {
     std::vector<int32_t> bounds_host;     // every moving candidate's bounds, back to back
     std::vector<int64_t> bounds_off;      // candidate i's bounds at bounds_host[bounds_off[i]]
     std::vector<std::pair<int, int>> caps;  // (win_len, table size) already worked out (pool_table_cap)
+    std::vector<std::pair<int, int>> traj_caps;   // the same for slots with a trajectory (traj_table_cap)
     std::vector<const ss_bank*> banks;    // candidate i's bank (ss_pool_levels renders the candidates)
     cudaEvent_t ready = nullptr;          // behind the construction of every candidate's bank
     // level tables (ss_pool_levels): every candidate's N + 1 doubles back to back, and a device array of n pointers
@@ -973,6 +988,7 @@ struct Shape {
     // time window (win_len > 0); zero otherwise
     int win;
     int pooled;               // a pooled slot (shape_pooled)
+    int traj;                 // a pooled slot with a trajectory (ss_trajectory): tables sized by traj_table_cap
     int tab_host;             // the window's blocks are known here (all but aligned blocking over device-side bounds)
     int g0, g1, k0, k1;       // tab_host: full-table blocks in the table / meeting the window (window_span)
     int row0, rows;           // RIR rows transformed per set (window_rows)
@@ -1066,14 +1082,28 @@ static Shape shape_of(const ss_source& it) {
 // A pooled slot: a moving window (tables built by k_blocks, the whole candidate read) under the pool's blocking, sized
 // once for the largest table (each candidate with its own K), position count and item count any candidate needs.  The
 // table sizes are worked out once per pool and window length.  K is the pool's largest: it picks the kernel variant.
-static Shape shape_pooled(const ss_source& it) {
+// A slot with a trajectory (traj) is sized for any bounds its runs may take (traj_table_cap).
+static Shape shape_pooled(const ss_source& it, bool traj = false) {
     ss_pool* pl = const_cast<ss_pool*>(it.pool);
     Shape s;
     memset(&s, 0, sizeof(s));
-    s.K = pl->K; s.aligned = pl->aligned; s.win = 1; s.pooled = 1; s.p_max = pl->p_max;
+    s.K = pl->K; s.aligned = pl->aligned; s.win = 1; s.pooled = 1; s.p_max = pl->p_max; s.traj = traj ? 1 : 0;
     s.per = (it.mode == SS_STATIC ? (it.C + 1) / 2 : it.C) * direct_sets(it);
     s.nblk_max = -1;
-    for (const auto& q : pl->caps) if (q.first == it.win_len) s.nblk_max = q.second;
+    std::vector<std::pair<int, int>>& caps = traj ? pl->traj_caps : pl->caps;
+    for (const auto& q : caps) if (q.first == it.win_len) s.nblk_max = q.second;
+    if (s.nblk_max < 0 && traj) {
+        std::vector<int> N(pl->n), P(pl->n);
+        int cap_max = 0;
+        for (int i = 0; i < pl->n; ++i) {
+            N[i] = pl->host[i].N; P[i] = pl->host[i].P;
+            cap_max = std::max(cap_max, table_cap(pl->aligned, (N[i] + kB - 1) / kB, P[i]));
+        }
+        std::vector<Block> full((size_t)cap_max);
+        s.nblk_max = traj_table_cap(pl->aligned, N.data(), P.data(), pl->parts_host.data(), pl->n, it.win_len, pl->K,
+                                    full.data());
+        caps.push_back({it.win_len, s.nblk_max});
+    }
     if (s.nblk_max < 0) {
         std::vector<const int*> bounds;
         std::vector<int> N(pl->n), P(pl->n);
@@ -1166,8 +1196,9 @@ static bool chunk_host_tables(const ss_source* items, int first, int last) {
 }
 // counts of a source (Source::counts): [0, 1] and, windowed, [2, 15] - which the host fills even when k_blocks builds the
 // block table, so that they always travel in the descriptor block - and for a pooled slot [16..17] (pool_parts),
-// [18..19] (stage_view), [20..24] (dry_table, dry_pick_ptr, dry_size) and [26..27] (pair_table), 112 bytes
-static size_t counts_bytes(const Shape& sh) { return sh.pooled ? 112 : sh.win ? 64 : 16; }
+// [18..19] (stage_view), [20..24] (dry_table, dry_pick_ptr, dry_size) and [26..27] (pair_table), 112 bytes; with a
+// trajectory also [25] and [28..31] (has_traj, traj_path, traj_bounds), 128 bytes
+static size_t counts_bytes(const Shape& sh) { return sh.traj ? 128 : sh.pooled ? 112 : sh.win ? 64 : 16; }
 static const float kUnitGain = 1.0f;      // counts[11] of every windowed source until a pooled slot picks (stem_gain)
 // descriptor block: Source[n] | prefix_prepare[n+1] | total | per source: blocks, rstep, counts (host-built tables) or
 // counts (windowed source, device-built tables)
@@ -1198,6 +1229,7 @@ struct PlanSlot {
     const ss_stream_lufs* lufs = nullptr;   // a loudness slot's target (validate_lufs), or null
     const ss_layout_draw* layout = nullptr; // a drawn slot's layout draw (validate_layouts), or null
     const ss_layout_group* group = nullptr; // a drawn stream slot's speaker groups (validate_layouts), or null
+    const ss_trajectory* traj = nullptr;    // its trajectory (validate_trajectories), or null
     StageView* view = nullptr;
     const DryStream* ws = nullptr;
     const BgStream* wb = nullptr;
@@ -1295,6 +1327,11 @@ static void chunk_describe(const ss_source* items, const Shape* shapes, int firs
                         hb_counts[24] = d.pool->n;
                         memcpy(hb_counts + 26, &rec->pair, sizeof(rec->pair));
                     }
+                    if (rec && rec->traj) {                     // has_traj, traj_path, traj_bounds
+                        hb_counts[25] = 1;
+                        memcpy(hb_counts + 28, &rec->traj->path_dev, sizeof(rec->traj->path_dev));
+                        memcpy(hb_counts + 30, &rec->traj->bounds_dev, sizeof(rec->traj->bounds_dev));
+                    }
                 }
             } else {
                 s.counts = (int*)scratch;
@@ -1338,7 +1375,7 @@ static int chunk_enqueue(ss_ctx* c, const ChunkLaunch& L, cudaStream_t stream, b
         CK(cudaEventRecord(pf.e0, stream));
     }
     if (!L.host_tables) {
-        k_blocks<<<1, 256, 0, stream>>>(const_cast<Source*>(L.ds), L.n, L.d_total);
+        k_blocks<<<1, 256, 0, stream>>>(const_cast<Source*>(L.ds), L.n, L.d_total, L.d_items);
         CK(cudaGetLastError());
         c->launches += 1;
     }
@@ -2983,11 +3020,13 @@ static int plan_build(ss_plan* p, const ss_source* caller_items, const Shape* ca
     std::vector<Shape> rendered_shapes(caller_shapes, caller_shapes + n_items);
     std::vector<int> loud;                               // the loudness slots, in caller order
     for (int i = 0; i < n_items; ++i) {
-        if (!slots[i].lufs) continue;
+        if (!slots[i].lufs && !slots[i].traj) continue;
         ss_source& w = rendered[i];
-        w.win_start = 0; w.win_start_dev = nullptr; w.win_len = w.pool->host[0].N;
-        rendered_shapes[i] = shape_pooled(w);
-        loud.push_back(i);
+        if (slots[i].lufs) {
+            w.win_start = 0; w.win_start_dev = nullptr; w.win_len = w.pool->host[0].N;
+            loud.push_back(i);
+        }
+        rendered_shapes[i] = shape_pooled(w, slots[i].traj != nullptr);
     }
     arrange_chunks(c, rendered.data(), rendered_shapes.data(), n_items, arranged, arranged_shapes, cuts, &order);
     const ss_source* items = arranged.data(); const Shape* shapes = arranged_shapes.data();
@@ -3375,6 +3414,10 @@ static int validate_mixes(const ss_source* items, const std::vector<PlanSlot>& s
             add_range(r, s.lufs->target_dev, 8, false, true);
             add_range(r, s.lufs->result_dev, 16, true);
         }
+        if (s.traj) {                                       // a trajectory meets nothing else the plan reads or writes
+            add_range(r, s.traj->path_dev, 12, true);
+            add_range(r, s.traj->bounds_dev, 4 * (uint64_t)items[s.traj->slot].pool->p_max, true);
+        }
     }
     for (const ss_dry_pool* dp : dpools)                    // (a host or 16-bit dry pool owns its arena: nothing a plan writes)
         if (!dp->padded())
@@ -3591,6 +3634,30 @@ static int validate_value_ranges(const ss_source* items, int n_items, const ss_v
     return written_ranges_disjoint(ranges) ? SS_OK : SS_ERR_INVALID;
 }
 
+// A plan's trajectories (include/sonicsim_b200.h, ss_trajectory), all but the byte ranges (validate_mixes): the record
+// of each trajectory's slot receives it.  After validate_dry_picks, validate_streams and validate_draws: a slot of a
+// moving device pool without loudness gains, whose dry pick has no pair gains, and which is no start draw's speaker
+// unless it is dry-picked or a stream slot (a speaker's level table is then its dry signal's, not its candidate's stem).
+static int validate_trajectories(const ss_source* items, const ss_trajectory* trajs, int n_trajs,
+                                 const ss_plan_draw* draws, int n_draws, std::vector<PlanSlot>& slots) {
+    for (int k = 0; k < n_trajs; ++k) {
+        const ss_trajectory& t = trajs[k];
+        if (t.slot < 0 || t.slot >= (int)slots.size() || slots[t.slot].traj) return SS_ERR_INVALID;
+        const ss_pool* pl = items[t.slot].pool;
+        const PlanSlot& r = slots[t.slot];
+        if (!pl || pl->mode != SS_MOVING_BOUNDS || pl->gains || r.pair) return SS_ERR_INVALID;
+        if (!t.path_dev || !t.bounds_dev || ((uintptr_t)t.path_dev & 3) || ((uintptr_t)t.bounds_dev & 3))
+            return SS_ERR_INVALID;
+        if (!r.dry && !r.strm)
+            for (int j = 0; j < n_draws; ++j)
+                for (int s = 0; s < draws[j].S; ++s) if (draws[j].speakers[s] == t.slot) return SS_ERR_INVALID;
+        slots[t.slot].traj = &t;
+    }
+    for (int k = 0; k < n_trajs; ++k)                       // (a host pool's staging is sized from its host bounds)
+        if (items[trajs[k].slot].pool->host_res) return SS_ERR_UNSUPPORTED;
+    return SS_OK;
+}
+
 // A plan's dereverberation targets (include/sonicsim_b200.h, ss_plan_target), all but the speakers' direct-path stems
 // and the byte ranges (validate_mixes): mix receives the mixtures, each with its target's direct_out, or null
 static int validate_targets(const ss_plan_mix* mixes, int n_mixes, const ss_plan_target* targets, int n_targets,
@@ -3611,11 +3678,11 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
                        int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs, int n_bgs,
                        const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts, int n_layouts,
                        const ss_value_draw* values, int n_values, const ss_layout_group* groups, int n_grouped,
-                       ss_plan** out) {
+                       const ss_trajectory* trajs, int n_trajs, ss_plan** out) {
     auto bad = [](const void* a, int n) { return n < 0 || (n > 0 && !a); };   // an array and its count
     if (!c || !out || !items || n_items <= 0 || bad(mixes, n_mixes) || bad(draws, n_draws) || bad(picks, n_picks) ||
         bad(targets, n_targets) || bad(streams, n_streams) || bad(bgs, n_bgs) || bad(lufs, n_lufs) ||
-        bad(layouts, n_layouts) || bad(values, n_values) || bad(groups, n_grouped))
+        bad(layouts, n_layouts) || bad(values, n_values) || bad(groups, n_grouped) || bad(trajs, n_trajs))
         return SS_ERR_INVALID;
     CK(cudaSetDevice(c->device));
     std::vector<Shape> shapes;
@@ -3629,6 +3696,7 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
     { int st = validate_layouts(layouts, n_layouts, groups, n_grouped, slots); if (st) return st; }
     { int st = validate_values(values, n_values); if (st) return st; }
     { int st = validate_draws(items, slots, draws, n_draws); if (st) return st; }
+    { int st = validate_trajectories(items, trajs, n_trajs, draws, n_draws, slots); if (st) return st; }
     { int st = validate_targets(mixes, n_mixes, targets, n_targets, mix); if (st) return st; }
     std::vector<ByteRange> ranges;
     { int st = validate_mixes(items, slots, mix, draws, n_draws, ranges); if (st) return st; }
@@ -3653,26 +3721,26 @@ static int plan_create(ss_ctx* c, const ss_source* items, int n_items, const ss_
 
 extern "C" int ss_plan_create(ss_ctx* c, const ss_source* items, int n_items, ss_plan** out) {
     return plan_create(c, items, n_items, nullptr, 0, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_mix(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, nullptr, 0, nullptr, nullptr, 0, nullptr, 0, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_ex(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                  int n_mixes, const ss_plan_draw* draws, int n_draws, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, nullptr, nullptr, 0, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_pair(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                    int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                    const ss_pair_gains* const* pair_gains, int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, nullptr, 0, nullptr,
-                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3680,7 +3748,7 @@ extern "C" int ss_plan_create_target(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3688,7 +3756,7 @@ extern "C" int ss_plan_create_stream(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
                                      int n_targets, const ss_dry_stream* streams, int n_streams, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes, int n_mixes,
@@ -3697,7 +3765,7 @@ extern "C" int ss_plan_create_bg(ss_ctx* c, const ss_source* items, int n_items,
                                  int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                  int n_bgs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3706,7 +3774,7 @@ extern "C" int ss_plan_create_lufs(ss_ctx* c, const ss_source* items, int n_item
                                    int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
                                    int n_bgs, const ss_stream_lufs* lufs, int n_lufs, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3716,7 +3784,7 @@ extern "C" int ss_plan_create_layout(ss_ctx* c, const ss_source* items, int n_it
                                      int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
                                      int n_layouts, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
-                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, nullptr, 0, nullptr, 0, out);
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, nullptr, 0, nullptr, 0, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_values(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3727,7 +3795,7 @@ extern "C" int ss_plan_create_values(ss_ctx* c, const ss_source* items, int n_it
                                      int n_layouts, const ss_value_draw* values, int n_values, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
                        streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, nullptr, 0,
-                       out);
+                       nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_groups(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
@@ -3739,14 +3807,27 @@ extern "C" int ss_plan_create_groups(ss_ctx* c, const ss_source* items, int n_it
                                      const ss_layout_group* groups, int n_grouped, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
                        streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, groups,
-                       n_grouped, out);
+                       n_grouped, nullptr, 0, out);
 }
 
 extern "C" int ss_plan_create_dry(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
                                   int n_picks, ss_plan** out) {
     return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, nullptr, n_picks, nullptr, 0, nullptr, 0,
-                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+                       nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, out);
+}
+
+extern "C" int ss_plan_create_traj(ss_ctx* c, const ss_source* items, int n_items, const ss_plan_mix* mixes,
+                                   int n_mixes, const ss_plan_draw* draws, int n_draws, const ss_dry_pick* picks,
+                                   const ss_pair_gains* const* pair_gains, int n_picks, const ss_plan_target* targets,
+                                   int n_targets, const ss_dry_stream* streams, int n_streams, const ss_bg_stream* bgs,
+                                   int n_bgs, const ss_stream_lufs* lufs, int n_lufs, const ss_layout_draw* layouts,
+                                   int n_layouts, const ss_value_draw* values, int n_values,
+                                   const ss_layout_group* groups, int n_grouped, const ss_trajectory* trajs,
+                                   int n_trajs, ss_plan** out) {
+    return plan_create(c, items, n_items, mixes, n_mixes, draws, n_draws, picks, pair_gains, n_picks, targets, n_targets,
+                       streams, n_streams, bgs, n_bgs, lufs, n_lufs, layouts, n_layouts, values, n_values, groups,
+                       n_grouped, trajs, n_trajs, out);
 }
 
 // The start draws (k_draw) on `stream`, ahead of everything that reads a start

@@ -84,7 +84,8 @@ struct RItem {
     const double* rstep;   //   "
     const int* idx;        // (mode 2)
     const float* w;        // (mode 2)
-    int pstride;           // float2 words between positions (moving: C*K*kSpec) / to channel c+1 (static: K*kSpec)
+    int pstride;           // float2 words between positions (moving: C*K*kSpec, negated for a reverse trajectory:
+                           // fill_traj_items) / to channel c+1 (static: K*kSpec); applied as a signed product
     int n0, n_end;         // output samples [n0, n_end)
     int p_lo, p_hi;        // transforms p = p_lo, p_lo + 2, ... <= p_hi   (static: 0, 0)
     int mode;
@@ -342,6 +343,63 @@ SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, co
 SS_HD int pool_table_cap(int aligned, const int* const* bounds, const int* N, const int* P, int n, int win_len, int K,
                          Block* full) {
     return pool_table_cap(aligned, bounds, N, P, nullptr, n, win_len, K, full);
+}
+// ---- trajectories of pooled slots (ss_trajectory, include/sonicsim_b200.h).  A slot with a trajectory reads, at every
+// run, a path (a, b, dir) over its picked candidate's P positions and a bounds table of b - a + 1 entries, and renders the
+// visited path: its local position j is bank position a + j (dir 0, forward) or b - j (dir 1, reverse), timed by the
+// drawn bounds instead of the candidate's own.  Its counts block is 128 bytes: counts[25] bit 0 (written by the host)
+// marks the trajectory, [28..29] and [30..31] hold the device pointers of its path and bounds.  The head of k_blocks
+// (take_trajectory) runs after the pick: it shifts the slot's spectra (and cut table) to position a, takes the drawn
+// bounds and P = b - a + 1, and sets counts[25] bit 1 for a reverse path.  h_rows keeps the bank's P*C*K: it is the
+// offset of the direct set, which follows the same map.  A banked slot reads its cut table only as the mark of a direct
+// set, so the cut table is shifted to position a whatever the direction.  The slot's work items are then filled by
+// k_blocks itself, after its item scan (fill_traj_items): fill_items as k_prepare's range warps call it, and for a
+// reverse path each item's RIR pointer moved to the last visited position with the position stride negated.  counts[0]
+// is then set to 0, so that k_prepare's range warps leave the slot's items alone; its dry-window CTAs read the block
+// table, not counts[0].  k_prepare is thus the parent's code for every source.  An invalid path (a >= b, a < 0,
+// b > P - 1, dir not 0 or 1) or bounds table (not non-decreasing from 0 to N) leaves the candidate's own forward path and
+// bounds, and the run reports kTrajBit.
+constexpr unsigned kTrajBit = 256u;                    // bit 8 of ss_device_errors
+SS_HD bool has_traj(const Source& s) { return s.h_rows && pool_table(s) && (s.counts[25] & 1); }
+SS_HD const int* traj_path(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 28); }
+SS_HD const int* traj_bounds(const Source& s) { return *reinterpret_cast<const int* const*>(s.counts + 30); }
+// a path (a, b, dir) over P positions and its bounds table b[0 .. b - a] of an N-sample candidate, as the slot takes them
+SS_HD bool traj_valid(const int* path, const int* bounds, int P, int N) {
+    const int a = path[0], b = path[1], dir = path[2];
+    if (a < 0 || a >= b || b > P - 1 || (dir != 0 && dir != 1)) return false;
+    if (bounds[0] != 0 || bounds[b - a] != N) return false;
+    for (int q = 0; q < b - a; ++q) if (bounds[q + 1] < bounds[q]) return false;
+    return true;
+}
+// The head of k_blocks for a slot with a trajectory, after the pick wrote the candidate into the slot's Source.  Returns
+// the error bits to report.
+SS_HD unsigned take_trajectory(Source& s) {
+    const int* const path = traj_path(s);
+    const int* const bounds = traj_bounds(s);
+    s.counts[25] = 1;
+    if (!traj_valid(path, bounds, s.P, s.N)) return kTrajBit;
+    const int a = path[0];
+    s.hspec += (size_t)a * s.C * s.K * kSpec;
+    if (s.cut) s.cut += (size_t)a * s.C;
+    s.bounds = bounds;
+    s.P = path[1] - a + 1;
+    s.counts[25] = 1 | (path[2] << 1);
+    return 0;
+}
+// Table size of a slot with a trajectory: drawn bounds may cut blocks at other samples than any candidate's own, so
+// under aligned blocking the table holds the blocks of any bounds table of at most P[i] - 1 segments over N[i] samples,
+// at any start: the device-side bound of window_table_cap (at most ceil(o / 4096) + 1 blocks of each segment a window
+// overlaps by o samples, one block in front and the last one's partner), never more than the whole candidate's
+// table_cap (at most one partial block per segment).  Grid blocking does not read the bounds: pool_table_cap's.
+SS_HD int traj_table_cap(int aligned, const int* N, const int* P, const int* Ks, int n, int win_len, int K, Block* full) {
+    if (!aligned) return pool_table_cap(0, nullptr, N, P, Ks, n, win_len, K, full);
+    int best = 0;
+    for (int i = 0; i < n; ++i) {
+        const int cap = table_cap(1, (N[i] + kB - 1) / kB, P[i]);
+        const int c = window_table_cap(nullptr, 0, N[i], win_len, Ks ? Ks[i] : K, P[i], cap);
+        best = c > best ? c : best;
+    }
+    return best;
 }
 // ---- host pools (SS_BANK_HOST, include/sonicsim_b200.h): banks and dry signals in pinned host memory.  At every run
 // k_stage copies the read set of each pooled slot's picked candidate into the slot's staging area in device memory and
@@ -1040,10 +1098,29 @@ SS_HD void fill_items(const Source& s, RItem* items, int blk, const Block& bk, i
     }
 }
 
+// The work items of a slot with a trajectory (take_trajectory), filled by k_blocks after its item scan (lane `lane` of
+// `nlanes`): every block of the window as k_prepare's range warps fill it, then, for a reverse path, item position p
+// moved to position P - 1 - p of the shifted set (H0 at the last visited position, the stride negated; the render
+// kernels take H0 + (ptrdiff_t)p * pstride).  counts[0] = 0 afterwards (by the caller,
+// once every lane is done) keeps k_prepare's range warps off the slot.
+SS_HD void fill_traj_items(const Source& s, RItem* items, int lane, int nlanes) {
+    const bool rev = (s.counts[25] & 2) != 0;
+    const int first = win_first(s), per = items_per_block(s);
+    for (int blk = first; blk < first + win_blocks(s); ++blk) {
+        fill_items(s, items, blk, block_positions(s, s.blocks[blk], 0, 0), lane, nlanes, stem_gain(s));
+        if (!rev) continue;
+        RItem* const dst = items + s.counts[1] + (size_t)(blk - first) * per;
+        for (int i = lane; i < per; i += nlanes) {         // the items this lane wrote
+            dst[i].H0 += (ptrdiff_t)(s.P - 1) * dst[i].pstride;
+            dst[i].pstride = -dst[i].pstride;
+        }
+    }
+}
+
 // k_render_fast: the two filter spectra of an item's single transform.  Aligned moving source: positions p_lo, p_lo + 1;
 // static source: channels c, c + 1 - a static item without a partner channel reuses the first filter (its imaginary
 // output is not stored).
-SS_HD const float2* item_hp(const RItem& it) { return it.H0 + (size_t)it.p_lo * it.pstride; }
+SS_HD const float2* item_hp(const RItem& it) { return it.H0 + (ptrdiff_t)it.p_lo * it.pstride; }
 SS_HD const float2* item_hq(const RItem& it) {
     const bool has = it.mode == MODE_STATIC ? it.row1 != nullptr : true;
     return item_hp(it) + (has ? it.pstride : 0);
@@ -1053,7 +1130,7 @@ SS_HD const float2* item_hq(const RItem& it) {
 SS_HD XDesc make_xdesc(const RItem& it, int p) {
     XDesc d;
     d.X = it.X;
-    d.Hp = it.H0 + (size_t)p * it.pstride;
+    d.Hp = it.H0 + (ptrdiff_t)p * it.pstride;
     const bool has_q = (it.mode == MODE_STATIC) ? (it.row1 != nullptr) : (p + 1 <= it.p_hi);
     d.Hq = has_q ? d.Hp + it.pstride : nullptr;
     d.row = it.row; d.row1 = it.row1;

@@ -77,7 +77,15 @@ class Mixture(T.NamedTuple):
     direct_out: T.Any = None
 
 
-class Pooled(T.NamedTuple):
+class _PooledFields(T.NamedTuple):
+    pool: T.Any
+    pick: T.Any
+    window: T.Tuple[T.Any, int]
+    direct_taps: int = 0
+    dry: T.Any = None
+
+
+class Pooled(_PooledFields):
     """A pooled slot of a device plan (Renderer.plan_device): at every run it renders the candidate of `pool`
     (Renderer.source_pool) named by `pick`, a one-element CUDA int32 tensor read on the device at that run (e.g.
     picks[b, k] of a (B, S) tensor) - the dataloader's random choice of scene, speakers and noise without host work.
@@ -87,12 +95,41 @@ class Pooled(T.NamedTuple):
     start beyond the picked candidate's N - length is clamped too (check_device_errors).  Only plan_device takes it.
     `dry`, a DryPick, makes it a dry-picked slot: the picked candidate renders with the dry signal the DryPick names in
     place of its own; a DryStream makes it a stream slot, whose dry signal is laid out from utterances at every run, and
-    a BackgroundStream a bed slot, whose noise or music bed is laid out from clips at every run."""
-    pool: T.Any
-    pick: T.Any
-    window: T.Tuple[T.Any, int]
-    direct_taps: int = 0
-    dry: T.Any = None
+    a BackgroundStream a bed slot, whose noise or music bed is laid out from clips at every run.  `trajectory`, a
+    Trajectory, renders the picked candidate along the path and timing it holds at that run instead of the candidate's
+    own.  It is a keyword attribute outside the tuple, as DryStream.lufs is: a Pooled stays the five-field tuple."""
+
+    def __new__(cls, pool, pick, window, direct_taps=0, dry=None, trajectory=None):
+        self = super().__new__(cls, pool, pick, window, direct_taps, dry)
+        self.trajectory = trajectory
+        return self
+
+    def _replace(self, **kw):
+        trajectory = kw.pop("trajectory", self.trajectory)
+        return Pooled(*super()._replace(**kw), trajectory=trajectory)
+
+    def __repr__(self):
+        return "%s, trajectory=%r)" % (super().__repr__()[:-1], self.trajectory)
+
+    def __getnewargs__(self):
+        return tuple(self) + (self.trajectory,)
+
+
+class Trajectory(T.NamedTuple):
+    """The trajectory of a pooled slot (Pooled.trajectory) of a moving pool, read on the device at every run: `path` a
+    contiguous 3-element CUDA int32 tensor (a, b, dir) with 0 <= a < b <= P - 1 of the picked candidate, dir 0 for the
+    forward path over positions a, a + 1, ..., b or 1 for the reverse path b, b - 1, ..., a; `bounds` a contiguous CUDA
+    int32 tensor of the pool's p_max entries (SourcePool.p_max, its largest P), whose first b - a + 1 are the visited
+    path's cumulative segment bounds (0 first, the candidate's N last, non-decreasing; SonicSim_moving.bounds_from_counts
+    of its per-segment sample counts).  The slot renders visited position j with the candidate's RIRs at position a + j
+    (forward) or b - j (reverse) and these bounds; its dry signal, window, direct stem, dry pick, stream or bed stay as
+    they are.  (0, P - 1, 0) with the candidate's own bounds renders bit for bit the slot without a trajectory.  An
+    invalid path or bounds table renders the candidate's own forward path and bounds (check_device_errors raises
+    ValueError).  Device pools only, without loudness gains or pair gains (both measured with the stored timing); a
+    CropDraw speaker with a trajectory needs a DryPick or a DryStream, whose level tables do not depend on it.  A
+    StemLoudness slot measures its whole stem with the run's trajectory."""
+    path: T.Any
+    bounds: T.Any
 
 
 class DryPick(T.NamedTuple):
@@ -450,6 +487,7 @@ class SourcePool(_Held):
         self._sizes = list(sizes) if sizes is not None else [int(s.dry.numel()) for s in self.candidates]
         self.host_nbytes = int(renderer.lib.ss_pool_host_bytes(handle))
         self.n, self.mode, self.C, self.L = len(self.candidates), mode, C, L
+        self.p_max = max(_rirs(c)[2] for c in self.candidates)     # the most positions: a Trajectory's bounds length
         self.n_min, self.direct_taps, self.levels = n_min, direct_taps, levels
         self._loudness = loudness if loudness is not None else np.full((self.n, 2), np.nan)
         self.nbytes = int(renderer.lib.ss_pool_bytes(handle))
@@ -1212,9 +1250,62 @@ class Renderer:
         grp = (_lib.SsLayoutGroup * len(grouped))(*grouped) if grouped else None
         val = self._device_values(values, sources, (outs, direct_outs, mixtures, draws, layouts), keep) \
             if values else None
+        trj = self._device_trajectories(sources, draws, (outs, direct_outs, mixtures, draws, layouts, values))
         return DevicePlan(self, items, n, keep, mixes, drw, dry, self._device_pair_gains(sources) if dry else None,
                           (_lib.SsPlanTarget * len(targets))(*targets) if targets else None, streams, bgs, lufs, lay,
-                          val, grp)
+                          val, grp, trj)
+
+    def _device_trajectories(self, sources, draws, others):
+        """Validated ss_trajectory array of a plan's slots with a Trajectory, or None without any.  `others`: the plan's
+        other arguments, whose tensors no path or bounds may meet."""
+        import torch
+        entries, held = [], []
+        speakers = {int(k) for d in (draws or ()) if isinstance(d, CropDraw) for k in d.speakers}
+        for i, s in enumerate(sources):
+            t = getattr(s, "trajectory", None)
+            if t is None:
+                continue
+            if not isinstance(t, Trajectory):
+                raise ValueError("plan_device: the trajectory of source %d must be a Trajectory" % i)
+            pl = s.pool
+            if pl.mode != _lib.SS_MOVING_BOUNDS:
+                raise ValueError("plan_device: source %d has a Trajectory over a static pool" % i)
+            if pl.resident != "device":
+                raise ValueError("plan_device: source %d has a Trajectory over a host pool, whose staging is sized from "
+                                 "its candidates' own bounds" % i)
+            if pl.gains:
+                raise ValueError("plan_device: source %d has a Trajectory over a pool with loudness gains, which were "
+                                 "measured with the candidates' own timing" % i)
+            d = s.dry
+            if isinstance(d, DryPick) and d.gains is not None:
+                raise ValueError("plan_device: source %d has a Trajectory and a DryPick with pair gains, which were "
+                                 "measured with the candidates' own timing" % i)
+            if i in speakers and not isinstance(d, (DryPick, DryStream)):
+                raise ValueError("plan_device: source %d has a Trajectory and is a CropDraw speaker that renders its "
+                                 "candidate's own dry signal, whose level table describes the stored timing" % i)
+            own = "source %d" % i
+            path = _tensor(t.path, "plan_device", own, "trajectory path", torch.int32, self.device, count=(3, 3))
+            bounds = _tensor(t.bounds, "plan_device", own, "trajectory bounds", torch.int32, self.device,
+                             (pl.p_max,))
+            entries.append(_lib.SsTrajectory(slot=i, path_dev=path, bounds_dev=bounds))
+            held.append(t)
+        if not entries:
+            return None
+        # a path or bounds meets no other tensor the plan reads or writes, nor another path or bounds.  Trajectories
+        # are attributes outside the Pooled tuples, so no span below is a path or bounds as such: a tensor met here is
+        # one the plan also uses for something else, whatever object holds it.
+        pools = [s.pool for s in sources if isinstance(s, Pooled)]
+        tensors = _cuda_tensors((sources, others, [tuple(p.candidates) for p in pools]))
+        spans = [(x.data_ptr(), x.data_ptr() + x.numel() * x.element_size()) for x in tensors]
+        seen = []
+        for e, t in zip(entries, held):
+            for x in (t.path, t.bounds):
+                lo, hi = x.data_ptr(), x.data_ptr() + x.numel() * x.element_size()
+                if any(a < hi and lo < b for a, b in spans) or any(a < hi and lo < b for a, b in seen):
+                    raise ValueError("plan_device: the trajectory of source %d meets another tensor of the plan"
+                                     % e.slot)
+                seen.append((lo, hi))
+        return (_lib.SsTrajectory * len(entries))(*entries)
 
     def _device_dry(self, sources):
         """Validated ss_dry_pick array of a plan's dry-picked slots, or None without any."""
@@ -1766,7 +1857,8 @@ class Renderer:
         but could not refuse up front: IndexError for an interp_index outside [0, P - 2] (NumPy's fancy index at
         SonicSim_moving.py:89-90), ValueError for a device-side bounds table that is not ascending from 0 to N or for a
         window start tensor that held a value outside [0, N - length] (the window was rendered clamped into range);
-        IndexError too for a pick, dry pick or grouped LayoutDraw's group outside its range (clamped into it)."""
+        IndexError too for a pick, dry pick or grouped LayoutDraw's group outside its range (clamped into it), and
+        ValueError for a Trajectory whose path or bounds were invalid at a run (the candidate's own path rendered)."""
         bits = ctypes.c_uint32()
         _lib.check(self.lib.ss_device_errors(self.ctx, ctypes.byref(bits)))
         if bits.value & 1:
@@ -1791,6 +1883,9 @@ class Renderer:
                              "previous entry); it was skipped")
         if bits.value & 64:
             raise ValueError("a StemLoudness target on the device was not finite; that slot was stored unscaled")
+        if bits.value & 256:
+            raise ValueError("a Trajectory on the device held an invalid path or bounds table; that slot rendered its "
+                             "candidate's own path")
 
     def launch_count(self) -> int:
         return int(self.lib.ss_launch_count(self.ctx))
@@ -1819,22 +1914,24 @@ class DevicePlan:
     dereverberation targets its mixtures also write those, with stream slots it lays out their dry streams and with bed
     slots their noise and music beds, with loudness slots it measures their whole stems at every run, with layout draws
     it draws its stream and bed layouts at every run, with value draws it draws its per-run inputs at every run, with
-    grouped layout draws it lays each such stream out from the group of utterances its group tensor names.  Every plan
-    is created by ss_plan_create_groups, with NULL and a count of 0 for each part it does not have."""
+    grouped layout draws it lays each such stream out from the group of utterances its group tensor names, with
+    trajectories its slots follow the path and timing their Trajectory holds at every run.  Every plan is created by
+    ss_plan_create_traj, with NULL and a count of 0 for each part it does not have."""
 
     def __init__(self, renderer, items, n, keep, mixes=None, draws=None, dry=None, pair_gains=None, targets=None,
-                 streams=None, bgs=None, lufs=None, layouts=None, values=None, groups=None):
+                 streams=None, bgs=None, lufs=None, layouts=None, values=None, groups=None, trajectories=None):
         self.renderer, self.items, self.n, self._keep, self.mixes = renderer, items, n, keep, mixes
         self.draws, self.dry, self.pair_gains, self.targets, self.streams = draws, dry, pair_gains, targets, streams
         self.bgs, self.lufs, self.layouts, self.values, self.groups = bgs, lufs, layouts, values, groups
+        self.trajectories = trajectories
         self._plan = ctypes.c_void_p()
         if n > 0:
             args = (renderer.ctx, items, n, mixes, len(mixes) if mixes else 0, draws, len(draws) if draws else 0, dry,
                     pair_gains, len(dry) if dry else 0, targets, len(targets) if targets else 0, streams,
                     len(streams) if streams else 0, bgs, len(bgs) if bgs else 0, lufs, len(lufs) if lufs else 0,
                     layouts, len(layouts) if layouts else 0, values, len(values) if values else 0, groups,
-                    len(groups) if groups else 0)
-            _lib.check(renderer.lib.ss_plan_create_groups(*args, ctypes.byref(self._plan)))
+                    len(groups) if groups else 0, trajectories, len(trajectories) if trajectories else 0)
+            _lib.check(renderer.lib.ss_plan_create_traj(*args, ctypes.byref(self._plan)))
         self._banks = _hold_banks(self, keep[0])
 
     def run(self, stream: T.Optional[int] = None):
